@@ -9,9 +9,8 @@ batches, one `sync()` after each phase, read-back verified against the source.
 
 One STEP = `--rounds` rounds of (write size-mb -> sync -> read it back -> sync), every round
 with fresh keys (first-writer-wins would turn a re-write into a no-op).  Defaults: 4 GiB per
-phase x 24 rounds = 192 GiB moved per GPU per step, so that K = 20 steps are a timed region
-of ~1.4 s at N = 1 and ~6 s at N >= 2 (round 1 timed 0.02 s; 16 rounds gave 0.93 s at
-N = 1).  The pool cannot hold a whole
+phase x 24 rounds = 192 GiB moved per GPU per step, so that K = 10 steps are a timed region
+of ~1.6 s at N = 1 on an H100.  The pool cannot hold a whole
 run: it is purged and re-reserved between epochs, OUTSIDE the timed regions, whose
 device-measured durations (CUDA events, barrier + synchronize on both sides) are summed.
 
@@ -70,7 +69,38 @@ def parse_args():
                    help="reference arm: MB written+read per step (one round)")
     p.add_argument("--quick", action="store_true",
                    help="small shapes for a functional check (256 MB x 2 rounds, no extras)")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="after the timed steps, write what the last timed read returned to "
+                        "DIR/*.npy (per-block sums of every page + a fixed sample of pages)")
     return p.parse_args()
+
+
+# the dump stays under 64 MB at any size: <= 2M float64 sums + a float32 sample of whole pages
+DUMP_MAX_SUMS = 2 << 20
+DUMP_SAMPLE_BYTES = 44 << 20
+
+
+def dump_outputs(out_dir, dst, nblocks, elems, rank, world):
+    """The timed path's result as a caller receives it: `dst`, the bf16 pages read back in the
+    last timed round.  Every page enters through its float64 sum (the sum of a group of
+    consecutive pages when there are more than DUMP_MAX_SUMS); a seeded sample of whole pages
+    is written as float32 (the same pages in every run with the same arguments)."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    suffix = f"_rank{rank}" if world > 1 else ""
+    pages = dst.view(nblocks, elems)
+    sums = torch.cat([p.double().sum(dim=1) for p in pages.split(1024)])  # bounded scratch
+    group = -(-nblocks // DUMP_MAX_SUMS)
+    if group > 1:
+        sums = torch.nn.functional.pad(sums, (0, -nblocks % group)).view(-1, group).sum(dim=1)
+    nsample = min(nblocks, max(1, DUMP_SAMPLE_BYTES // (elems * 4)))
+    pick = np.sort(np.random.default_rng(0).choice(nblocks, nsample, replace=False))
+    sample = pages[torch.from_numpy(pick).to(dst.device)].float()
+    np.save(os.path.join(out_dir, f"read_page_sums{suffix}.npy"), sums.cpu().numpy())
+    np.save(os.path.join(out_dir, f"read_pages_sample{suffix}.npy"), sample.cpu().numpy())
+    np.save(os.path.join(out_dir, f"read_pages_sample_index{suffix}.npy"), pick.astype(np.float64))
 
 
 def reference_arm(args):
@@ -313,7 +343,7 @@ def main():
     if world != args.gpus and world > 1:
         raise SystemExit(f"--gpus {args.gpus} but WORLD_SIZE={world}")
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a CUDA device (run it through gpurun)")
+        raise SystemExit("bench.py needs a CUDA device")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     dist = None
@@ -383,7 +413,7 @@ def main():
     conn = ist.InfinityConnection(ccfg)
     conn.connect()
 
-    # ---- synthetic KV pages (bf16), far larger than L2 (126 MB): nothing is served from cache
+    # ---- synthetic KV pages (bf16), far larger than L2 (50 MB): nothing is served from cache
     gen = torch.Generator(device=dev).manual_seed(1234 + rank)
     src = torch.empty(nblocks * elems, device=dev, dtype=torch.bfloat16)
     chunk = 64 << 20
@@ -467,6 +497,8 @@ def main():
         ms = run_rounds(args.steps * rounds, record=True)
         clocks = sampler.stop()
         launches = conn.stats()["kernel_launches"] - launches0
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, dst, nblocks, elems, rank, world)
         nr = args.steps * rounds
         w_ms = (host_t["issue_write"] + host_t["sync_write"]) / nr * 1e3
         r_ms = (host_t["issue_read"] + host_t["sync_read"]) / nr * 1e3
@@ -486,7 +518,7 @@ def main():
 
     # ---- independent rooflines, measured now on this box by the COPY ENGINE (no kernel of
     #      this repo): every rank copies 1 GiB to its ring peer at the same time
-    roof = {"nominal_nvlink_GBps_per_dir_per_gpu": 900}
+    roof = {"nominal_nvlink_GBps_per_dir_per_gpu": 450}  # H100 SXM: 18 NVLink 4 links
     try:
         ce_bytes = 1 << 30
         a = torch.empty(ce_bytes, dtype=torch.uint8, device=dev)
@@ -518,7 +550,7 @@ def main():
     except Exception as e:  # noqa: BLE001
         roof["ce_error"] = repr(e)[:200]
     if world > 1:
-        roof["fraction_of_nominal_900"] = round(value / (world * 900.0), 3)
+        roof["fraction_of_nominal_450"] = round(value / (world * 450.0), 3)
     else:
         peaks = {}
         try:
@@ -526,9 +558,10 @@ def main():
                 peaks = json.load(f)
         except Exception:  # noqa: BLE001
             pass
-        hbm = peaks.get("hbm_gbs", 6650.0)
-        roof["measured_hbm_copy_GBps"] = hbm
-        roof["fraction_of_measured_hbm_copy"] = round(value / (hbm / 2), 3)
+        if "hbm_gbs" in peaks:  # only a measured figure, never a default
+            hbm = peaks["hbm_gbs"]
+            roof["measured_hbm_copy_GBps"] = hbm
+            roof["fraction_of_measured_hbm_copy"] = round(value / (hbm / 2), 3)
 
     # ---- end to end: pinned host pages -> H2D (layer-wise, overlapped) -> write -> sync ->
     #      read -> sync, every round; D2H of the result at the end of the step
@@ -669,7 +702,7 @@ def main():
                        "phase_bytes": size_bytes, "global_batch": nblocks * world,
                        "seq_len": None, "layers_per_phase": layers,
                        "parallelism": f"{world} pool shards, ring placement (rank r -> GPU (r+1)%N)",
-                       "l2": f"working set {2 * size_bytes >> 20} MiB per GPU per round >> 126 MB L2 "
+                       "l2": f"working set {2 * size_bytes >> 20} MiB per GPU per round >> 50 MB L2 "
                              "(no flush needed)",
                        "variant": args.variant, "streams": args.streams,
                        "pipe_stage_kb": args.stage_kb or "default", "pipe_ring_kb": args.ring_kb or "default",

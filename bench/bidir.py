@@ -53,7 +53,8 @@ def timed(active, table, variant, ctas):
 
 
 res = []
-for variant, ctas in (("ldst256", 0), ("ldst256", 296), ("tma", 0)):
+sms = torch.cuda.get_device_properties(0).multi_processor_count
+for variant, ctas in (("ldst256", 0), ("ldst256", 2 * sms), ("tma", 0)):
     for name, table in (("push", push), ("pull", pull)):
         uni = timed([0], table, variant, ctas)[0]
         bi = timed([0, 1], table, variant, ctas)

@@ -273,8 +273,8 @@ def fanin(ctx: Ctx, pages: int = 64, iters: int = 2):
             "page_kib": layout.page_bytes >> 10, "bytes_per_client_per_iter": per_client,
             "write_GBps_aggregate": round(total / w / 1e6, 1),
             "read_GBps_aggregate": round(total / r / 1e6, 1),
-            "roofline": "pool GPU ingress / egress: 900 GB/s nominal, ~770 copy engine",
-            "fraction_of_900": [round(total / w / 1e6 / 900, 3), round(total / r / 1e6 / 900, 3)],
+            "roofline": "pool GPU ingress / egress: 450 GB/s nominal (H100 SXM, NVLink 4)",
+            "fraction_of_450": [round(total / w / 1e6 / 450, 3), round(total / r / 1e6 / 450, 3)],
             "verified": okall, "timing": "CUDA events around issue+sync, max over ranks"}
 
 
@@ -332,8 +332,8 @@ def fp8_ring(ctx: Ctx, size_mb: int = 2048, iters: int = 2, layers: int = 32, **
             "read_GBps_fp8_bytes": round(fp8_bytes / r / 1e6, 1),
             "write_GBps_bf16_equiv": round(bf16_bytes / w / 1e6, 1),
             "read_GBps_bf16_equiv": round(bf16_bytes / r / 1e6, 1),
-            "fraction_of_900_on_fp8_bytes": [round(fp8_bytes / w / 1e6 / ctx.world / 900, 3),
-                                             round(fp8_bytes / r / 1e6 / ctx.world / 900, 3)],
+            "fraction_of_450_on_fp8_bytes": [round(fp8_bytes / w / 1e6 / ctx.world / 450, 3),
+                                             round(fp8_bytes / r / 1e6 / ctx.world / 450, 3)],
             "max_rel_err_vs_bf16": round(err, 4),
             "timing": "CUDA events around issue+sync, max over ranks"}
 
@@ -410,7 +410,7 @@ def nvls_bcast(ctx: Ctx, blocks_n: int = 512, iters: int = 3, match_keys: int = 
     out.update({
         "writer_egress_GBps": round(total / w / 1e6, 1),
         "delivered_GBps": round((ctx.world - 1) * total / w / 1e6, 1),
-        "fraction_of_900_egress": round(total / w / 1e6 / 900, 3),
+        "fraction_of_450_egress": round(total / w / 1e6 / 450, 3),
         "readers_local_replica_GBps_aggregate": round(ctx.world * total / r / 1e6, 1),
         "verified": ctx.allsum(0.0 if ok else 1.0) == 0.0})
     # get_match_last_index: device kernel vs server op, same keys (half present)

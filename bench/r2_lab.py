@@ -4,7 +4,7 @@
   ce      : copy-engine rooflines - cudaMemcpyPeerAsync GPU0->GPU1 alone and both directions
             at once (the independent NVLink roofline bench.py quotes), local cudaMemcpy
   geom    : TMA pipeline (kv_pipe) ring geometry x grid at 128 KB blocks, local / push / pull
-  sizes   : block-size sweep, TMA pipeline vs 256-bit ld/st, local / push / pull
+  sizes   : block-size sweep, TMA pipeline vs ld/st, local / push / pull
   bidir   : both GPUs pushing / pulling at once with the kernels (ring topology of bench.py)
   mcast   : cluster multicast read (1 fetch, K destinations) vs K separate copies
 
@@ -104,11 +104,12 @@ def paths(two):
 def lab_geom(out, two):
     rows = []
     bs = 128 << 10
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
     for name, (src, dst) in paths(two).items():
         descs = descs_for(src, dst, bs, "cuda:0")
         for stage_kb, ring_kb in ((8, 64), (16, 64), (16, 128), (32, 128), (16, 192), (32, 192)):
-            for ctas in ((16, 32, 74, 148) if name != "local" else (148, 296)):
-                if ring_kb > 110 and ctas > 148:
+            for ctas in ((16, 32, sms // 2, sms) if name != "local" else (sms, 2 * sms)):
+                if ring_kb > 110 and ctas > sms:
                     continue
                 ms = ev_time(lambda: ops.kv_copy(descs, bs, variant="tma", max_ctas=ctas,
                                                  stage_bytes=stage_kb << 10,
@@ -184,7 +185,7 @@ def lab_mcast(out, two):
         per = [ops.make_descs([src.data_ptr() + i * bs for i in range(n)],
                               [d.data_ptr() + i * bs for i in range(n)], "cuda:0") for d in dsts]
         deltas = [d.data_ptr() - dsts[0].data_ptr() for d in dsts]
-        if two:  # multicast bulk loads from a peer-mapped source wedged a B200: never again
+        if two:  # multicast bulk loads from a peer-mapped source once wedged a GPU: never again
             ms_c = float("nan")
             ops.kv_copy(descs, bs, variant="tma", fan_deltas=deltas)
         else:

@@ -80,9 +80,10 @@ def main():
     total = a.total_mb << 20
     sizes = [4096, 16384, 65536, 131072, 262144, 1 << 20, 16 << 20]
     variants = ["ldst", "ldst256", "tma"]
-    grids = [0, 148, 296, 592]
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    grids = [0, sms, 2 * sms, 4 * sms]
     if a.quick:
-        sizes, grids = [4096, 131072, 1 << 20], [0, 148]
+        sizes, grids = [4096, 131072, 1 << 20], [0, sms]
     rows = sweep("cuda:0", "cuda:0", "cuda:0", total, sizes, variants, grids, "local hbm->hbm")
     if a.peer and torch.cuda.device_count() >= 2:
         assert native.enable_peer_access(0, 1) and native.enable_peer_access(1, 0)

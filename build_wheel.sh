@@ -1,5 +1,5 @@
 #!/bin/bash
-# Wheels with the prebuilt sm_100a native module, one per CPython ABI found on this host
+# Wheels with the prebuilt sm_90a native module, one per CPython ABI found on this host
 # (reference counterpart: build_manylinux_wheels.sh, which loops over cp310/cp311/cp312 inside
 # a manylinux container and repairs with auditwheel).  The module links the CUDA runtime
 # statically and needs no NIC libraries, so no repair step is needed; the version comes from

@@ -1,6 +1,6 @@
 // Configuration structs shared by C++, the pybind layer and the Python kwargs/argparse
 // surface.  Field names of the first block of each struct are the reference's
-// (src/config.h:13-32); the second block is the B200 fabric extension.
+// (src/config.h:13-32); the second block is the NVLink fabric extension.
 #pragma once
 
 #include <cstddef>

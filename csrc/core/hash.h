@@ -1,4 +1,4 @@
-// 64-bit keyed hash shared by host C++ and sm_100a device code.
+// 64-bit keyed hash shared by host C++ and sm_90a device code.
 //
 // The store identifies a key by a 128-bit fingerprint (hash with two seeds).  The host
 // kv map uses it as its hasher, the HBM-resident index stores it instead of key bytes,

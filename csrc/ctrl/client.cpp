@@ -462,8 +462,7 @@ int Connection::sync_local() {
     // The commit list is taken BEFORE waiting for the GPU, so it names only blocks whose
     // kernels the drain below covers, and it is shipped right away as a STAGED commit: the
     // server decodes it and pulls the block headers into its cache while this thread waits
-    // for the kernels; the SYNC that follows the drain applies it.  (Measured at N=1: the
-    // commit of 8192 blocks was ~0.1 ms of a 0.5 ms write phase when it followed the drain.)
+    // for the kernels; the SYNC that follows the drain applies it.
     std::vector<uint64_t> addrs;
     {
         std::lock_guard<std::mutex> lk(mu_);

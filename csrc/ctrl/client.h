@@ -7,7 +7,7 @@
 //
 // The data plane is redesigned for an NVSwitch box: instead of posting RDMA work requests
 // to a NIC (reference: src/libinfinistore.cpp:860-1099) the client maps the server's HBM
-// pool segments into its own address space and launches sm_100a kernels on ITS GPU that
+// pool segments into its own address space and launches sm_90a kernels on ITS GPU that
 // move a whole batch of pages with peer loads/stores over NVLink and publish the commit
 // in-band (kernels/kv_copy.cu).  The server CPU only allocates and indexes.
 #pragma once

@@ -413,8 +413,7 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
             F.max_ctas = L.max_ctas;
             F.all_local = all_local;
             F.aligned16 = (align_or & 15) == 0;
-            // TMA-pipelined flavour over NVLink (write 622 vs 537, read 705 vs 507 GB/s of fp8
-            // bytes), per-thread flavour on local HBM (1705 vs 1223): profiles/r2_lab_fp8_2gpu.json
+            // TMA-pipelined flavour over NVLink, per-thread flavour on local HBM
             F.variant = all_local ? 1 : 0;
             e = write ? kernels::launch_kv_write_fp8(F, stream) : kernels::launch_kv_read_fp8(F, stream);
         } else {
@@ -606,9 +605,8 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
             seg_base[s] = reinterpret_cast<uint64_t>(seg_dev_ptr(ctx, s));
             all_remote = all_remote && ctx->seg_remote[s];
         }
-        // fp8 pages pulled over NVLink: one CTA per SM.  With both link directions busy, 296
-        // CTAs of 8 compute warps pull 954 GB/s (2 GPUs, fp8 bytes), 148 pull 1085
-        // (bench/configs.py fp8 --max-ctas 148, round 2); writes prefer two per SM.
+        // fp8 pages over NVLink: reads one CTA per SM, writes two per SM.  A grid choice not
+        // re-measured on H100: bench/configs.py fp8 --max-ctas N compares grid caps.
         const int grid_cap = max_ctas_ ? max_ctas_
                              : all_remote ? (fp8_elems ? 1 : 2) * kernels::sm_count()
                                           : 0;
@@ -620,13 +618,12 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
         // The fused kernels resolve a key in every CTA that moves a piece of its block, reading
         // the key bytes from the pinned ring each time: right for a batch of blocks (items are
         // whole blocks, or chunks when that balances the grid better - kernels/balance.h),
-        // wasteful when a few LARGE blocks are split over many CTAs (measured: 4 MB
-        // single-block read 83 us vs 42 us) - then resolve each key once with the lookup kernel
-        // and feed the descriptors to kv_copy.
+        // wasteful when a few LARGE blocks are split over many CTAs - then resolve each key
+        // once with the lookup kernel and feed the descriptors to kv_copy.
         // A handful of blocks (<= 4 MB in all): latency matters, not bandwidth.  One launch of
         // the ld/st flavour, which splits a block into 32 KB chunks over CTAs (each resolves its
         // block's key itself - a few redundant probes) and re-checks the entries in the same
-        // kernel: lookup + copy + validate would be three launches (+7..15 us per read).
+        // kernel: lookup + copy + validate would be three launches.
         const bool small_batch = n * size_t(block_size) <= (4u << 20);
         const bool whole_blocks = !small_batch && uint32_t(block_size) <= (1u << 20) && n >= 32;
         kernels::ReadFusedLaunch R;

@@ -99,8 +99,8 @@ struct Connection::DevCtx {
 
     // Launch streams.  Back-to-back page-mover kernels of one connection are independent of
     // each other, but in a single stream the fixed head (launch, descriptor fetch) and tail
-    // (store acks, fence, commit) of every kernel are exposed: +5..30 us on a 45 us NVLink
-    // launch (profiles/r1_launch_overhead_*.json).  Round-robin over a few internal streams
+    // (store acks, fence, commit) of every kernel are exposed (bench/launch_overhead.py
+    // measures them).  Round-robin over a few internal streams
     // lets the tail of one kernel overlap the body of the next.  Ordering: every launch
     // waits for the caller's stream (the pages are ready); reads / lookups additionally wait
     // for earlier writes of this connection; completion is established by sync().
@@ -181,8 +181,8 @@ struct Connection::DevCtx {
     }
 
     // Completion of everything launched so far.  A blocking cudaStreamSynchronize sleeps on an
-    // interrupt (+5..10 us for a transfer that itself takes 10 us); short transfers are
-    // therefore polled with cudaStreamQuery for a bounded time first.
+    // interrupt, whose wake-up is long next to a short transfer; short transfers are therefore
+    // polled with cudaStreamQuery for a bounded time first.
     void wait_all() {
         DeviceGuard g(device);
         for (cudaStream_t s : busy) {

@@ -829,10 +829,10 @@ bool Server::dispatch(Conn* c) {
             case kOpTouch: code = handle_touch(c); break;
             case kOpSync: {
                 // Reply first, apply the staged commit right after: the reply leaves this
-                // thread's hands before the (0.3 ms for 32k blocks) map update, which the
+                // thread's hands before the map update, which the
                 // client therefore does not wait for - and nobody can observe the gap, because
                 // every later request of every connection is served by this same thread, after
-                // the update.  (Measured: the apply was 17 % of a 4 GiB write phase at N = 1.)
+                // the update.
                 std::vector<uint64_t> apply;
                 apply.swap(c->staged);
                 c->leases.clear();  // the client's reads have completed

@@ -4,7 +4,7 @@
 // Role parity with the reference's libuv front-end + server bootstrap
 // (src/infinistore.cpp:1113-1298): accept, 2-state header/body stream parser tolerant of
 // arbitrary TCP segmentation, per-op dispatch, replies of `int code + payload`.  It is
-// NOT a libuv port: libuv headers do not exist on the target image, and the B200 design
+// NOT a libuv port: libuv headers do not exist on the target image, and this design
 // moves all data movement to client-side kernels, so the server never touches CUDA on a
 // request path (no per-request stream/event/IPC-open as in the reference's local path).
 //

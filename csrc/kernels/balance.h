@@ -1,8 +1,8 @@
 // How to cut a batch of equal-sized blocks into work items for a persistent grid.
 //
 // A CTA takes items first, first + grid, first + 2 * grid, ...  With whole blocks as items the
-// batch finishes when the CTAs with ceil(n / grid) blocks finish: 512 blocks on 296 CTAs keep
-// 216 CTAs busy for two blocks and 80 for one - 86 % of the grid's throughput, and the ring
+// batch finishes when the CTAs with ceil(n / grid) blocks finish: 512 blocks on 264 CTAs keep
+// 248 CTAs busy for two blocks and 16 for one - 97 % of the grid's throughput, and the ring
 // benchmarks issue exactly such batches (one layer's pages per call).  Splitting a block into
 // `cpb` chunks makes the items finer; a chunk costs a descriptor (fused reads: a probe of the
 // index) and, on writes, one more arrival at the block's commit counter, so the coarsest

@@ -1,4 +1,4 @@
-// Device-side building blocks shared by the sm_100a kernels: vector / cache-hinted memory
+// Device-side building blocks shared by the sm_90a kernels: vector / cache-hinted memory
 // ops, system-scope acquire/release, mbarrier + 1-D bulk-async (TMA) copies, multimem.
 // Inline PTX only; SASS mnemonics to look for are noted beside each wrapper.
 #pragma once
@@ -35,24 +35,6 @@ __device__ __forceinline__ void st_stream_v4(void* p, const uint4& v) {  // STG.
                  "r"(v.y), "r"(v.z), "r"(v.w)
                  : "memory");
 }
-struct alignas(32) u32x8 {
-    uint32_t v[8];
-};
-__device__ __forceinline__ u32x8 ld_v8(const void* p) {  // LDG.E.ENL2.256
-    u32x8 r;
-    asm volatile("ld.global.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]), "=r"(r.v[4]),
-                   "=r"(r.v[5]), "=r"(r.v[6]), "=r"(r.v[7])
-                 : "l"(p));
-    return r;
-}
-__device__ __forceinline__ void st_v8(void* p, const u32x8& r) {  // STG.E.ENL2.256
-    asm volatile("st.global.v8.u32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(r.v[0]),
-                 "r"(r.v[1]), "r"(r.v[2]), "r"(r.v[3]), "r"(r.v[4]), "r"(r.v[5]), "r"(r.v[6]),
-                 "r"(r.v[7])
-                 : "memory");
-}
-
 // ---------------------------------------------------------------- system-scope sync
 __device__ __forceinline__ void fence_sys() { asm volatile("fence.acq_rel.sys;" ::: "memory"); }
 __device__ __forceinline__ void fence_gpu() { asm volatile("fence.acq_rel.gpu;" ::: "memory"); }

@@ -1,5 +1,5 @@
 // The key index algorithm: claim / find / erase / validate on the bucketed table
-// (kernels.h: IndexBucket).  Written once for both sides: the sm_100a kernels run it with
+// (kernels.h: IndexBucket).  Written once for both sides: the sm_90a kernels run it with
 // system-scope PTX memory operations on (usually peer-mapped) HBM, the native unit tests
 // run the same code on the CPU with __atomic builtins, threads standing in for GPUs.
 //

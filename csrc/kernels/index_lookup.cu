@@ -31,8 +31,7 @@ using namespace dev;
 // fabric loads behind one SM's load unit.
 //
 // Key bytes usually sit in the client's pinned ring (PCIe): a thread that walked its own key
-// with serial 8-byte loads paid one PCIe round trip per 8 bytes (1.4 ms for 4096 keys in
-// round 1).  The warp's 32 keys are packed back to back, so the warp first stages their whole
+// with serial 8-byte loads paid one PCIe round trip per 8 bytes.  The warp's 32 keys are packed back to back, so the warp first stages their whole
 // byte range into shared memory with coalesced 8-byte loads - a handful of PCIe reads in
 // flight at once - and every thread then hashes its key from shared memory.
 constexpr int kLookupThreads = 32;

@@ -1,4 +1,4 @@
-// Host-callable launchers of the sm_100a data-plane kernels.
+// Host-callable launchers of the sm_90a data-plane kernels.
 //
 // These kernels replace every byte-moving / lookup call site of the reference, which has
 // no device code at all (SURVEY §2.2): per-block cudaMemcpyAsync (src/infinistore.cpp:
@@ -90,7 +90,7 @@ enum CopyVariant : int {
     kCopyAuto = 0,
     kCopyLdSt = 1,  // 128-bit ld/st, all threads: LDG.128 / STG.128 on (peer) global memory
     kCopyTma = 2,   // warp-specialised TMA pipeline (kv_pipe.cu): UBLKCP.S.G / UBLKCP.G.S + mbarriers
-    kCopyLdSt256 = 3,  // 256-bit ld/st (LDG.E.ENL2.256 / STG.E.ENL2.256)
+    kCopyLdSt256 = 3,  // 32-byte aligned ld/st: 128-bit vectors, eight in flight per thread
 };
 
 struct CopyLaunch {
@@ -122,9 +122,9 @@ struct CopyLaunch {
     int64_t fan_delta[4] = {0, 0, 0, 0};
 };
 // Picks the data path (CopyVariant) and launches it.  kCopyAuto: the TMA pipeline for every
-// 16-byte aligned transfer of blocks >= kPipeMinBytes, 256-bit ld/st below that (one issuing
-// thread per CTA cannot keep up with the per-block work of small blocks: 534 vs 2307 GB/s at
-// 4 KB, 2090 vs 3035 at 16 KB, equal from 64 KB on - profiles/r2_lab_1gpu.json).
+// 16-byte aligned transfer of blocks >= kPipeMinBytes, ld/st below that (one issuing thread
+// per CTA cannot keep up with the per-block work of small blocks; bench/sweep_copy.py
+// compares the variants per block size).
 cudaError_t launch_kv_copy(const CopyLaunch& a, cudaStream_t stream);
 constexpr uint32_t kPipeMinBytes = 64u << 10;
 // The TMA pipeline itself (kv_pipe.cu); needs 16-byte aligned addresses and sizes.

@@ -3,7 +3,7 @@
 //
 // One launch moves a whole batch of pages (a layer's worth) described by a descriptor
 // array; either side of every descriptor may be a peer-mapped address, so the bytes cross
-// NVLink 5 / NVSwitch from inside the kernel.  This replaces, for one batch,
+// NVLink / NVSwitch from inside the kernel.  This replaces, for one batch,
 //   * N cudaMemcpyAsync calls on a fresh stream + event (reference local path,
 //     src/infinistore.cpp:623-624,747-748),
 //   * N RDMA_WRITE work requests chained 32 at a time (src/libinfinistore.cpp:905-970,
@@ -12,12 +12,12 @@
 //     255-271): the kernel publishes each block in the HBM-resident index itself, with
 //     release semantics at system scope, once the block's bytes have landed.
 //
-// Data paths, selected per launch (measured, not guessed — see profiles/):
+// Data paths, selected per launch (bench/sweep_copy.py compares them):
 //   kCopyTma  : the default - the warp-specialised TMA pipeline of kv_pipe.cu (loader /
 //               storer / control warps around an mbarrier-guarded SMEM ring);
-//   kCopyLdSt / kCopyLdSt256 : this file - every thread streams 128-bit (or 256-bit)
-//               vectors, 4 in flight per thread; used for small or unaligned blocks and for
-//               NVLS multicast stores (multimem.st has no bulk form).
+//   kCopyLdSt / kCopyLdSt256 : this file - every thread streams 128-bit vectors, 4 (or,
+//               for 32-byte aligned blocks, 8) in flight per thread; used for small or
+//               unaligned blocks and for NVLS multicast stores (multimem.st has no bulk form).
 #include <algorithm>
 #include <cstring>
 #include <mutex>
@@ -37,8 +37,7 @@ constexpr uint32_t kLdStChunk = 32u << 10;  // work item of the ld/st path
 
 // ---------------------------------------------------------------- ld/st path (copy_span.cuh)
 // Descriptors of small batches travel in the kernel parameters (constant bank): reading
-// them from the pinned host ring costs a PCIe round trip at the start of every launch
-// (+3-4 us of 18 on a 32 MB launch, profiles/r1_launch_overhead_v1.json).
+// them from the pinned host ring costs a PCIe round trip at the start of every launch.
 constexpr int kParamDescs = 256;
 template <int N>
 struct DescParam {
@@ -95,11 +94,11 @@ __global__ void __launch_bounds__(kLdStThreads + 32)
 int sm_count() {
     static int cached[64] = {0};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
     if (!cached[dev]) {
         int n = 0;
         if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-            n = 148;
+            n = 132;
         cached[dev] = n;
     }
     return cached[dev];
@@ -121,9 +120,8 @@ cudaError_t launch_kv_copy(const CopyLaunch& a, cudaStream_t stream) {
         if (!aligned16) return cudaErrorInvalidValue;  // multimem.st moves 16-byte vectors
         variant = kCopyLdSt;
     }
-    // auto: the TMA pipeline wherever it applies (profiles/r2_sweep_*: it matches or beats the
-    // ld/st kernels from 8 KB blocks up, on local HBM and over NVLink, with 3 warps per CTA);
-    // small blocks are bound by per-block issue cost, where 256 threads win
+    // auto: the TMA pipeline from kPipeMinBytes up (3 warps per CTA); small blocks are bound
+    // by per-block issue cost, where 256 threads win
     if (variant == kCopyAuto)
         variant = (aligned16 && a.bytes >= kPipeMinBytes) ? kCopyTma
                                                           : (aligned32 ? kCopyLdSt256 : kCopyLdSt);

@@ -1,9 +1,8 @@
 // kv_doorbell: a persistent worker CTA for single-block operations (the latency path).
 //
-// A write or read of ONE block through the ordinary path costs a kernel launch (4-5 us until
-// the first instruction), an event record + wait when it runs on an internal stream, and a
-// completion that the host detects by polling the stream (2-3 us): ~25 us per operation over
-// NVLink for a 4 KB block, of which the data movement is a few.  With
+// A write or read of ONE block through the ordinary path costs a kernel launch, an event
+// record + wait when it runs on an internal stream, and a completion that the host detects by
+// polling the stream; for a 4 KB block the data movement is the smallest part.  With
 // ClientConfig(doorbell=True) the client keeps ONE CTA resident that polls a request ring in
 // pinned host memory:
 //

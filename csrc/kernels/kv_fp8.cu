@@ -15,7 +15,7 @@
 // load), reduces |x| max with shuffles inside the half, and emits 8 bytes per lane (one
 // coalesced 128-byte store per row).  Eight rows are in flight per warp to cover the
 // NVLink / HBM latency.
-// There is no direct bf16<->e4m3 cvt on sm_100a: quantise via f32, dequantise via f16x2.
+// There is no direct bf16<->e4m3 cvt on sm_90a: quantise via f32, dequantise via f16x2.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 

@@ -1,7 +1,7 @@
-// kv_pipe: the Blackwell-native page movers — warp-specialised TMA pipelines.
+// kv_pipe: the Hopper-native page movers — warp-specialised TMA pipelines.
 //
 // This is the default data path of write_cache / read_cache: every byte moves
-//     global (local HBM or a peer GPU over NVLink 5) --cp.async.bulk--> SMEM ring
+//     global (local HBM or a peer GPU over NVLink 4) --cp.async.bulk--> SMEM ring
 //     SMEM ring --cp.async.bulk--> global (peer pool or local KV cache)
 // with no register staging and two or three warps per CTA, so a transfer that overlaps
 // prefill leaves the SM's issue slots and register file to the model's kernels.  It
@@ -538,12 +538,11 @@ EncodeTiledFn encode_tiled_fn() {
 PipeGeometry pipe_geometry(uint32_t bytes, uint32_t stage_pref, uint32_t ring_pref) {
     PipeGeometry g;
     // 16 KB slots, 4 of them (64 KB per CTA), ONE CTA per SM per launch: a single launch then
-    // runs a little below the best single-kernel geometry (32 KB x 4 at 128 KB per CTA: 3225
-    // vs 2561 GB/s on local HBM, equal over NVLink), but three such kernels fit an SM side by
+    // may run below the best single-kernel geometry (larger slots per CTA), but three such
+    // kernels fit an SM side by
     // side, and that is what the API needs - the calls of a phase go round-robin over the
     // connection's streams, and the next kernel must be able to start (descriptor fetch, index
-    // claims) while the previous one drains (store acknowledgements, system fence, commit):
-    // ~20 us of every 180 us call over NVLink otherwise (profiles/r2_bench_n2_ring*.json).
+    // claims) while the previous one drains (store acknowledgements, system fence, commit).
     const uint32_t stage_cap = stage_pref ? stage_pref : (16u << 10);
     const uint32_t ring = ring_pref ? ring_pref : (64u << 10);
     g.stage_bytes = std::min(stage_cap, (bytes + 15u) & ~15u);
@@ -683,7 +682,7 @@ cudaError_t launch_kv_pipe_mcast(const McastLaunch& a, cudaStream_t stream) {
     if ((a.ndst != 2 && a.ndst != 4) || (a.bytes % 16) != 0 || (a.align_or & 15) != 0)
         return cudaErrorInvalidValue;
     // The multicast bulk load is used on LOCAL sources only: with a peer-mapped source
-    // (NVLink aperture) the launch wedged a B200 in round 2 (gpurun strike) - the fabric path
+    // (NVLink aperture) the launch once wedged a GPU - the fabric path
     // of multicast TMA reads is not something this store relies on.  Peer sources take the
     // fan-out flavour of kv_pipe_copy instead (one load, K stores per CTA).
     if (!a.src_local) return cudaErrorNotSupported;

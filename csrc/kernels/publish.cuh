@@ -6,8 +6,8 @@
 // GPU that observes the entry's tag (ld.acquire.sys) is guaranteed to observe the block.
 //
 // Two phases, run by a dedicated CONTROL WARP of every CTA so that the copy warps never
-// wait on a fabric round trip (measured: doing the whole insertion after the data cost
-// +30 us per 32 MB launch over NVLink, profiles/r1_launch_overhead_v1.json):
+// wait on a fabric round trip (doing the whole insertion after the data would add the
+// claim's NVLink round trips to every launch's tail):
 //   claim  (kernel start, overlaps the copy): CAS a way's h1 from 0 (one NVLink round
 //          trip), fill h2/addr/size with posted stores; tag stays 0 = invisible.
 //   commit (after the block's last chunk has landed): one posted st.release.sys of the tag.
@@ -33,7 +33,7 @@ struct Publish {
     unsigned long long* trace = nullptr;  // optional: 8 %globaltimer stamps per CTA (bench only)
     // true: some destination (pool block or index table) is NOT in this GPU's own HBM, so
     // "performed" must mean acknowledged across NVLink: fence.acq_rel.sys (MEMBAR.SYS +
-    // ERRBAR, ~10 us).  false: everything is local; the local L2 is the point of coherence
+    // ERRBAR).  false: everything is local; the local L2 is the point of coherence
     // for local memory, also for peers reading it over NVLink, so gpu scope suffices.
     bool sys = true;
     uint32_t debug = 0;  // bench only: 1 = skip claim, 2 = skip fence, 4 = skip commit store
@@ -58,7 +58,7 @@ __device__ inline uint32_t claim_entry(const Publish& pub, const IndexEntry& rec
 
 // The caller has just executed fence.acq_rel.sys; fence + relaxed store is a release
 // pattern, so the tag needs no second MEMBAR.SYS/ERRBAR (the most expensive instruction of
-// the epilogue, profiles/r1_ncu_kv_copy_*.txt).
+// the epilogue).
 __device__ inline void commit_entry(const Publish& pub, uint32_t slot_plus1, uint32_t tag) {
     if (!slot_plus1 || (pub.debug & 4)) return;
     idx::commit(idx::table_of_slot(pub.table, pub.shards, slot_plus1), idx::slot_local(slot_plus1),
@@ -127,7 +127,7 @@ __device__ inline void control_warp(const Publish& pub, uint32_t lane, uint32_t 
         // acq_rel counter in local memory: every arriver fenced its stores BEFORE its
         // increment, so when the last arriver observes the full count all chunks of the block
         // are already performed; its tag store is issued after that in program order
-        // (no second MEMBAR.SYS: profiles/r1_trace_write_epilogue_v1.json, +10 us each).
+        // (no second MEMBAR.SYS).
         const uint32_t arrived = cpb == 1 ? 1 : atom_add_acq_rel_gpu(done + block, 1u) + 1;
         if (arrived != cpb) continue;
         const uint32_t s = __ldcg(slot_of + block);

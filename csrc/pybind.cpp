@@ -6,7 +6,7 @@
 // and remote_addr:u8 @8 (itemsize 16).  Every blocking call releases the GIL; callbacks
 // of the async API re-acquire it on the connection's completion thread.
 // Extras: a Server class (several servers per process, SPMD ranks hosting pool shards),
-// introspection (stats, segments), and raw launchers of the sm_100a kernels plus the wire
+// introspection (stats, segments), and raw launchers of the sm_90a kernels plus the wire
 // codec / allocator for unit tests.
 #include <pybind11/functional.h>
 #include <pybind11/numpy.h>
@@ -336,7 +336,7 @@ T* as_ptr(uint64_t p) {
 }  // namespace
 
 PYBIND11_MODULE(_infinistore, m) {
-    m.doc() = "B200-native KV-cache store: control plane, fabric and sm_100a kernels";
+    m.doc() = "H100-native KV-cache store: control plane, fabric and sm_90a kernels";
 
     PYBIND11_NUMPY_DTYPE(RemoteBlock, rkey, gen, remote_addr);
 
@@ -761,7 +761,7 @@ PYBIND11_MODULE(_infinistore, m) {
         .def("size", &fabric::NvlsGroup::size);
 
     // ------------------------------------------------------------ raw kernel launchers
-    py::module_ k = m.def_submodule("kernels", "raw launchers of the sm_100a kernels");
+    py::module_ k = m.def_submodule("kernels", "raw launchers of the sm_90a kernels");
     k.attr("COPY_AUTO") = int(kernels::kCopyAuto);
     k.attr("COPY_LDST") = int(kernels::kCopyLdSt);
     k.attr("COPY_TMA") = int(kernels::kCopyTma);

@@ -6,7 +6,7 @@
 // op-specific payload.  Opcodes and return codes keep the reference's values so that the
 // control plane is recognisable on the wire.
 //
-// Differences by design (B200-native data plane, no ibverbs message channel):
+// Differences by design (GPU-native data plane, no ibverbs message channel):
 //   * the allocate / read-lookup / commit messages ('D','A','T'), which the reference
 //     carries inside RDMA SEND messages, ride the same TCP connection here;
 //   * 'P' (pool map) is new: it hands the client the list of pool segments (HBM IPC

@@ -1,4 +1,4 @@
-"""Drop-in alias: ``import infinistore`` resolves to the B200-native package, so code
+"""Drop-in alias: ``import infinistore`` resolves to the H100-native package, so code
 written against the reference (``infinistore.ClientConfig``, ``python -m
 infinistore.server`` ...) runs unchanged."""
 import sys as _sys

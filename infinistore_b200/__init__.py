@@ -1,4 +1,4 @@
-"""infinistore_b200 — a Blackwell-native KV-cache block store with infiniStore's API.
+"""infinistore_b200 — an H100-native KV-cache block store with infiniStore's API.
 
 The package exports the reference's public names (its ``infinistore/__init__.py``) plus the
 additions of this implementation; everything lives in ``lib.py``.

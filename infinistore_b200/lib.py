@@ -1,4 +1,4 @@
-"""Python API of the B200-native KV-cache store.
+"""Python API of the H100-native KV-cache store.
 
 Public names and call signatures follow the reference package so that callers can switch
 packages without code changes (reference: infinistore/lib.py:21-707): ``ClientConfig``,
@@ -10,7 +10,7 @@ packages without code changes (reference: infinistore/lib.py:21-707): ``ClientCo
 
 What differs is the substrate.  ``TYPE_RDMA`` here means "one-sided remote access over the
 NVLink fabric": the server's block pool is HBM on a pool GPU, mapped into the client
-process, and ``rdma_write_cache`` / ``read_cache`` launch sm_100a kernels on the client's
+process, and ``rdma_write_cache`` / ``read_cache`` launch sm_90a kernels on the client's
 GPU that move the whole batch of pages with peer loads/stores and publish the commit
 in-band.  ``dev_name`` / ``ib_port`` / ``link_type`` are accepted for compatibility and
 ignored.  Units are the reference's: offsets and page sizes in ELEMENTS for the
@@ -329,7 +329,7 @@ def _device_of(cache: torch.Tensor) -> int:
     return cache.device.index if cache.device.type == "cuda" else -1
 
 
-try:  # raw handle of torch's current stream without building a Stream object (~0.2 us)
+try:  # raw handle of torch's current stream without building a Stream object
     _raw_current_stream = torch._C._cuda_getCurrentRawStream
 except AttributeError:  # pragma: no cover
     _raw_current_stream = None

@@ -5,7 +5,7 @@ The reference is model-agnostic (it moves opaque byte blocks; its only "model" i
 nn.Sequential of example/demo_prefill.py:21-48).  What callers need from a KV store is the
 page geometry (bytes per page per layer), a key scheme that encodes layer / TP rank /
 prefix hash (docs/source/design.rst:50) and layer-wise streaming; this package provides
-those for real model configurations - plus the two consumer-side shapes the B200 read
+those for real model configurations - plus the two consumer-side shapes the device read
 kernels serve directly: a head-major decode cache filled by the layout-swizzling read
 (``HeadMajorKVCache``) and several caches of one GPU filled by one fetch (``read_layer_multi``).
 """

@@ -1,4 +1,4 @@
-"""Tensor-level wrappers over the raw sm_100a kernel launchers.
+"""Tensor-level wrappers over the raw sm_90a kernel launchers.
 
 The store's hot path (``InfinityConnection``) drives the kernels from C++; these wrappers
 exist for unit tests, the micro-benchmarks under ``bench/`` and for users who want the
@@ -68,7 +68,7 @@ def kv_copy_multicast(descs: torch.Tensor, nbytes: int, dst_deltas: Sequence[int
     thread-block cluster: the source is fetched ONCE (``cp.async.bulk ...
     .multicast::cluster`` into every CTA's shared memory) and each CTA of the cluster stores
     it to its own destination (csrc/kernels/kv_pipe.cu: kv_pipe_mcast).  LOCAL sources only:
-    a multicast bulk load from a peer-mapped (NVLink) address wedged a B200 in round 2; for
+    a multicast bulk load from a peer-mapped (NVLink) address once wedged a GPU; for
     peer sources use ``kv_copy(..., variant="tma", fan_deltas=...)``."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
     assert len(dst_deltas) in (2, 4), "clusters of 2 or 4 CTAs"

@@ -244,7 +244,7 @@ def check_p2p_access():
 
 
 def parse_args(argv=None):
-    p = argparse.ArgumentParser(description="B200-native infinistore server")
+    p = argparse.ArgumentParser(description="H100-native infinistore server")
     p.add_argument("--auto-increase", action="store_true",
                    help="add a pool segment automatically when the pool fills up")
     p.add_argument("--host", default="0.0.0.0", type=str, help="listen address, default 0.0.0.0")

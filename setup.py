@@ -58,7 +58,7 @@ setup(
     distclass=BinaryDistribution,
     name="infinistore-b200",
     version=get_version(),
-    description="Blackwell-native KV-cache block store with infiniStore's API",
+    description="H100-native KV-cache block store with infiniStore's API",
     packages=find_packages(include=["infinistore_b200", "infinistore_b200.*", "infinistore"]),
     package_data={"infinistore_b200": ["_infinistore*.so"]},
     python_requires=">=3.10",

@@ -1,4 +1,4 @@
-"""GPU tests of the B200-only features: fp8 KV path through the store, the fused read
+"""GPU tests of the fabric-level features: fp8 KV path through the store, the fused read
 kernel's corner cases, sharded HBM pools, the paged KV cache and NVLS broadcast."""
 import random
 import string
@@ -53,8 +53,8 @@ def test_fp8_kv_path_through_the_store(hbm_server, device_lookup):
 @pytest.mark.parametrize("n,elems,max_ctas", [
     (300, 2048, 3),      # 100 items per CTA: four resolver rounds, queue halves recycled
     (5, 1 << 20, 0),     # few big pages: chunked over the grid, every CTA resolves its block
-    (148 * 3, 8192, 0),  # whole pages per CTA
-    (200, 65536, 0),     # 200 pages of 8 tiles on 296 CTAs: quarter pages balance the grid
+    (132 * 3, 8192, 0),  # whole pages per CTA (three per H100 SM)
+    (300, 65536, 0),     # 8 tiles a page on 264 CTAs (2 per SM): quarter pages balance the grid
 ])
 def test_fp8_fused_read_resolves_dequantises_and_reports_misses(hbm_server, n, elems, max_ctas):
     """read_cache_fp8 through the device index is ONE launch (resolver warp inside the
@@ -92,10 +92,10 @@ def test_fp8_fused_read_resolves_dequantises_and_reports_misses(hbm_server, n, e
 
 
 def test_unbalanced_batches_are_moved_in_chunks(hbm_server):
-    """200 pages of 128 KB on 148 CTAs: whole pages would leave 96 CTAs idle for the second
-    round, so writes and fused reads move half pages (kernels/balance.h).  The chunks of a
-    page are committed through the cross-CTA counter; the read resolves a page in every CTA
-    that moves a piece of it."""
+    """200 pages of 128 KB on 132 CTAs (one per H100 SM): whole pages would leave 64 CTAs
+    idle for the second round, so writes and fused reads move chunks (kernels/balance.h).  The
+    chunks of a page are committed through the cross-CTA counter; the read resolves a page in
+    every CTA that moves a piece of it."""
     _, port = hbm_server
     conn = make_conn(port, device_lookup=True)
     n, elems = 200, 65536

@@ -1,4 +1,4 @@
-"""Numerics of the sm_100a kernels against plain PyTorch references (run on the B200 box)."""
+"""Numerics of the sm_90a kernels against plain PyTorch references (run on the H100)."""
 import numpy as np
 import pytest
 import torch

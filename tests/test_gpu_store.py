@@ -1,4 +1,4 @@
-"""End-to-end store on an HBM pool (run on the B200 box): ports of the reference's
+"""End-to-end store on an HBM pool (run on the H100): ports of the reference's
 integration tests (infinistore/test_infinistore.py) onto the NVLink fabric."""
 import asyncio
 import multiprocessing as mp

@@ -103,19 +103,21 @@ def test_chunk_plan_balances_a_persistent_grid():
         cpb = -(-units // chunk)
         return -(-n * cpb // ctas) * chunk
 
-    # the flagship batch (1024 pages of 8 ring slots on 148 CTAs) stays whole
-    assert plan(1024, 8, 4, 64, 148) == (8, 1)
-    # one layer of the fp8 ring bench: 512 pages of 8 tiles on 296 CTAs -> quarters (14 vs 16)
-    assert plan(512, 8, 2, 64, 296) == (2, 4)
+    # the flagship batch (1024 pages of 8 ring slots, one CTA per H100 SM) stays whole
+    assert plan(1024, 8, 4, 64, 132) == (8, 1)
+    # 300 fp8 pages of 8 tiles on 264 CTAs (two per SM) -> quarters (10 vs 16 whole)
+    assert plan(300, 8, 2, 64, 264) == (2, 4)
+    # 512 such pages: whole pages already keep the grid as busy as quarters (16 vs 16)
+    assert plan(512, 8, 2, 64, 264) == (8, 1)
     # a lone 1 MB block: the smallest chunks allowed
-    assert plan(1, 64, 4, 64, 148) == (4, 16)
+    assert plan(1, 64, 4, 64, 132) == (4, 16)
     # never below min, never above max, short blocks are one item
-    assert plan(7, 3, 4, 64, 148) == (3, 1)
-    assert plan(100000, 4096, 4, 64, 148)[0] <= 64
+    assert plan(7, 3, 4, 64, 132) == (3, 1)
+    assert plan(100000, 4096, 4, 64, 132)[0] <= 64
     import random
     rnd = random.Random(7)
     for _ in range(300):
-        n, units, ctas = rnd.randint(1, 5000), rnd.randint(1, 300), rnd.choice([1, 3, 148, 296])
+        n, units, ctas = rnd.randint(1, 5000), rnd.randint(1, 300), rnd.choice([1, 3, 132, 264])
         lo = rnd.randint(1, 8)
         chunk, cpb = plan(n, units, lo, 64, ctas)
         assert cpb == -(-units // chunk) and min(lo, units) <= chunk <= max(min(units, 64), min(lo, units))

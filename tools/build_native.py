@@ -1,9 +1,10 @@
 """Build the native module in-tree: infinistore_b200/_infinistore*.so.
 
-g++ (C++20) for the host runtime, nvcc 12.9 for the sm_100a kernels
-(`-gencode arch=compute_100a,code=sm_100a -lineinfo`), one shared object, static cudart so
+g++ (C++20) for the host runtime, nvcc 12.9 for the sm_90a kernels
+(`-gencode arch=compute_90a,code=sm_90a -lineinfo`), one shared object, static cudart so
 that the module imports on hosts without a GPU or driver (reference counterpart:
-src/Makefile, which has no nvcc step at all).  Objects are cached by mtime under build/.
+src/Makefile, which has no nvcc step at all).  Objects are cached under build/ by mtime and
+compile flags.
 
     python tools/build_native.py [--force] [--tests] [--jobs N]
 """
@@ -25,7 +26,7 @@ PKG = ROOT / "infinistore_b200"
 
 CUDA_HOME = Path(os.environ.get("CUDA_HOME", "/usr/local/cuda"))
 NVCC = str(CUDA_HOME / "bin" / "nvcc")
-GENCODE = ["-gencode", "arch=compute_100a,code=sm_100a"]
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 HOST_SOURCES = [
     "wire/messages.cpp",
@@ -98,6 +99,11 @@ def build(force: bool = False, jobs: int | None = None, verbose: bool = False) -
                   "-fvisibility=hidden", "-pthread"]
     nvcc_flags = [*GENCODE, "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
                   "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
+    # objects built with other flags (e.g. for another architecture) are stale
+    stamp = BUILD / "flags.txt"
+    flags_id = " ".join([*host_flags, *nvcc_flags])
+    if not stamp.exists() or stamp.read_text() != flags_id:
+        force = True
     if verbose:
         nvcc_flags += ["-Xptxas", "-v"]
 
@@ -133,6 +139,7 @@ def build(force: bool = False, jobs: int | None = None, verbose: bool = False) -
               f"-L{CUDA_HOME / 'lib64'}", "-lcudart_static", "-lrt", "-ldl", "-lpthread",
               "-Wl,--exclude-libs,ALL"])
         os.replace(tmp, out)
+    stamp.write_text(flags_id)
     return out
 
 
@@ -177,7 +184,7 @@ def build_loopback_test(force: bool = False, sanitize="address") -> Path:
 
 
 def sass_listing(dst_dir: Path) -> list[Path]:
-    """cuobjdump -sass of every kernel object (committed under docs/sass/)."""
+    """cuobjdump -sass of every kernel object (written to docs/sass/, not committed)."""
     dst_dir.mkdir(parents=True, exist_ok=True)
     written = []
     for rel in CUDA_SOURCES:

@@ -9,7 +9,7 @@
 #   quick   bench.py without extras / e2e  lab    bench/r2_lab.py sweeps (1 or 2 GPUs)
 #   lat     bench/configs.py latency       ncu    bench/ncu_driver.py under ncu --set full (1 process)
 #   fp8     bench/configs.py fp8 (ring)    fanin  bench/configs.py fanin
-#   fp8ab   fp8 ring with grid caps 296 / 148, twice, interleaved
+#   fp8ab   fp8 ring with grid caps 264 / 132 (2 / 1 per H100 SM), twice, interleaved
 #
 # A step that runs into its limit may have wedged the GPU (it has happened: a multicast bulk
 # load from peer memory); going on would burn the whole gpurun limit, so the script aborts.
@@ -43,7 +43,7 @@ for s in $STEPS; do
     ref)    step ref 600 $LAUNCH bench.py --impl reference --gpus $N --steps 3 --warmup 1 ;;
     lat)    step lat 200 $LAUNCH bench/configs.py latency ;;
     fp8)    step fp8 300 $LAUNCH bench/configs.py fp8 ;;
-    fp8ab)  for i in 1 2; do for c in 296 148; do   # interleaved A/B of the client's grid cap
+    fp8ab)  for i in 1 2; do for c in 264 132; do   # interleaved A/B of the client's grid cap
                 launch; step fp8_ctas${c}_$i 300 $LAUNCH bench/configs.py fp8 --max-ctas $c
             done; done ;;
     fanin)  step fanin 300 $LAUNCH bench/configs.py fanin ;;

@@ -3,7 +3,7 @@
 # the TMA pipelines), synccheck.  Each tool under its own limit; output -> gpurun_out/sanitizer.txt
 mkdir -p gpurun_out
 OUT=gpurun_out/sanitizer.txt
-echo "# compute-sanitizer on tests/test_gpu_kernels.py + the doorbell / fused-fp8 store tests (B200, 1 GPU)" > $OUT
+echo "# compute-sanitizer on tests/test_gpu_kernels.py + the doorbell / fused-fp8 store tests (1 GPU)" > $OUT
 run() {
     local tool=$1 secs=$2; shift 2
     echo "== $tool" >> $OUT

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Summarise an .ncu-rep into a small text file for profiles/: key raw metrics per kernel
+"""Summarise an .ncu-rep into a small text file: key raw metrics per kernel
 instance plus the top stall instructions of the first instance (needs -lineinfo builds).
 
-    python tools/ncu_summary.py gpurun_out/prof.ncu-rep profiles/r1_ncu_kv_copy.txt
+    python tools/ncu_summary.py prof.ncu-rep ncu_kv_copy.txt
 """
 import csv
 import io
