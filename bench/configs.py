@@ -12,6 +12,8 @@ run (so they land in the driver-visible JSON line under `extra` / `baselines`) a
                       replica; plus get_match_last_index on the device vs the server op.
   fp8     (config 5)  fp8 KV path: write fused with the bf16->e4m3 cast, read fused with the
                       dequantising gather, 64 KB (fp8) blocks, ring over N GPUs.
+  gather              Llama-3-8B in vLLM's layout, 2048 pages: per-layer keys against one
+                      gathered key per page (all layers' K and V), 32 KB and 64 KB parts.
 
 Timing: CUDA events recorded on the rank's current stream around (issue + sync()); the
 stream is otherwise idle, so the pair brackets the transfer on the device clock; every number
@@ -338,6 +340,109 @@ def fp8_ring(ctx: Ctx, size_mb: int = 2048, iters: int = 2, layers: int = 32, **
             "timing": "CUDA events around issue+sync, max over ranks"}
 
 
+# --------------------------------------------------------------------------- gathered blocks
+def gather(ctx: Ctx, pages: int = 2048, layers: int = 32, iters: int = 2):
+    """Llama-3-8B KV in vLLM's flash layout, one [2, pages, block_size, 8, 128] bf16 tensor per
+    layer.  (a) per-layer keys: one rdma_write_cache / read_cache per layer and K|V, i.e.
+    2 * layers calls and keys per page; (b) one key per page holding every layer's K and V:
+    one rdma_write_cache_gather and one read_cache_scatter.  block_size 16 makes 32 KB parts
+    (the ld/st kernels), 32 makes 64 KB parts (the TMA pipeline): one workload on each side of
+    kPipeMinBytes.  Pages are written from one permutation of the page ids and read into
+    another.  The pool sits on the ring peer (local HBM with one process), as in fp8_ring."""
+    port = ctx.base_port + 80
+    heads, dim = 8, 128
+    out = {"model": "llama-3-8b", "layers": layers, "pages": pages,
+           "pool": "NVLink (ring peer)" if ctx.world > 1 else "local HBM",
+           "timing": "CUDA events around issue+sync, max over ranks; host_us = stats() "
+                     "ns_build + ns_launch per phase"}
+    for block_size in (16, 32):
+        page = block_size * heads * dim                  # elements of one K (or V) page
+        part_bytes = page * 2
+        block_bytes = 2 * layers * part_bytes
+        server = start_shard_server(ctx.local, port + ctx.rank, pages * block_bytes + (512 << 20),
+                                    granule_kb=16)
+        ctx.barrier()
+        conn = _client(ctx, port + (ctx.rank + 1) % ctx.world)
+        src = [torch.randn(2, pages, block_size, heads, dim, device=ctx.dev).to(torch.bfloat16)
+               for _ in range(layers)]
+        dst = [torch.empty_like(t) for t in src]
+        for t in src + dst:
+            conn.register_mr(t)
+        g = torch.Generator().manual_seed(block_size)
+        wp = torch.randperm(pages, generator=g).numpy().astype(np.int64)
+        rp = torch.randperm(pages, generator=g).numpy().astype(np.int64)
+        wpt, rpt = torch.from_numpy(wp).to(ctx.dev), torch.from_numpy(rp).to(ctx.dev)
+        res = {"part_kb": part_bytes >> 10,
+               "path": "TMA pipeline" if part_bytes >= 64 << 10 else "ld/st"}
+        for arm in ("per_layer", "gathered"):
+            tw, tr = DevTimer(), DevTimer()
+            host_ns = [0, 0]
+            launches = [0, 0]
+            ok = True
+            for it in range(iters + 1):
+                tag = uuid.uuid4().hex[:12]
+                for t in dst:
+                    t.zero_()
+                if arm == "per_layer":
+                    keys = [[f"{tag}/L{l}/{'KV'[kv]}/{p}" for p in range(pages)]
+                            for l in range(layers) for kv in (0, 1)]
+                    remote = [conn.allocate_rdma(k, part_bytes) for k in keys]
+                else:
+                    keys = [f"{tag}/all/{p}" for p in range(pages)]
+                    remote = conn.allocate_rdma(keys, block_bytes)
+                    sparts = [(t, b) for t in src for b in (0, pages * page)]
+                    dparts = [(t, b) for t in dst for b in (0, pages * page)]
+                torch.cuda.synchronize()
+                ctx.barrier()
+                for phase, timer in ((0, tw), (1, tr)):
+                    s0 = conn.stats()
+                    timer.start()
+                    if arm == "per_layer":
+                        for i in range(2 * layers):
+                            l, kv = divmod(i, 2)
+                            if phase == 0:
+                                conn.rdma_write_cache(src[l], kv * pages * page + wp * page, page,
+                                                      remote[i])
+                            else:
+                                conn.read_cache(dst[l], (keys[i], kv * pages * page + rp * page),
+                                                page)
+                    elif phase == 0:
+                        conn.rdma_write_cache_gather(sparts, wp * page, page, remote)
+                    else:
+                        conn.read_cache_scatter(dparts, (keys, rp * page), page)
+                    conn.sync()
+                    if it:
+                        timer.stop()
+                        s1 = conn.stats()
+                        host_ns[phase] += (s1["ns_build"] - s0["ns_build"]
+                                           + s1["ns_launch"] - s0["ns_launch"])
+                        launches[phase] += s1["kernel_launches"] - s0["kernel_launches"]
+                    else:
+                        timer.ms = 0.0
+                ctx.barrier()
+                ok = ok and all(torch.equal(d[:, rpt], s[:, wpt]) for s, d in zip(src, dst))
+                server.purge()  # the next iteration's keys take the space
+                ctx.barrier()
+            w, r = ctx.allmax(tw.ms), ctx.allmax(tr.ms)
+            nbytes = ctx.world * pages * block_bytes * iters
+            res[arm] = {"keys_per_phase": pages * (2 * layers if arm == "per_layer" else 1),
+                        "calls_per_phase": 2 * layers if arm == "per_layer" else 1,
+                        "kernel_launches_write": launches[0] // iters,
+                        "kernel_launches_read": launches[1] // iters,
+                        "write_read_GBps": round(2 * nbytes / (w + r) / 1e6, 1),
+                        "write_GBps": round(nbytes / w / 1e6, 1),
+                        "read_GBps": round(nbytes / r / 1e6, 1),
+                        "host_us_write": round(host_ns[0] / iters / 1e3, 1),
+                        "host_us_read": round(host_ns[1] / iters / 1e3, 1),
+                        "pages_match": bool(ctx.allmin(float(ok)))}
+        out[f"block_size_{block_size}"] = res
+        conn.close()
+        del src, dst
+        ctx.barrier()
+        server.stop()
+    return out
+
+
 # --------------------------------------------------------------------------- config 4
 def nvls_bcast(ctx: Ctx, blocks_n: int = 512, iters: int = 3, match_keys: int = 4096):
     """1 writer -> N replicas through the STORE API: rank 0 hosts a server with an
@@ -457,7 +562,7 @@ def _standalone_ctx():
         if dist is None:
             return x
         t = torch.tensor([x], dtype=torch.float64, device=dev)
-        dist.all_reduce(t, op=op)
+        dist.all_reduce(t, op=getattr(dist.ReduceOp, op))
         return float(t.item())
 
     def barrier():
@@ -467,13 +572,12 @@ def _standalone_ctx():
 
     return Ctx(dist, rank, world, local, dev,
                25000 + int(os.environ.get("MASTER_PORT", "0")) % 2000, barrier,
-               lambda x: red(x, dist.ReduceOp.MAX), lambda x: red(x, dist.ReduceOp.SUM),
-               lambda x: red(x, dist.ReduceOp.MIN))
+               lambda x: red(x, "MAX"), lambda x: red(x, "SUM"), lambda x: red(x, "MIN"))
 
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("config", choices=["fanin", "bcast", "fp8", "latency", "baselines"])
+    ap.add_argument("config", choices=["fanin", "bcast", "fp8", "gather", "latency", "baselines"])
     ap.add_argument("--max-ctas", type=int, default=0, help="fp8: grid cap of the client's kernels")
     ap.add_argument("--layers", type=int, default=32,
                     help="fp8: calls per phase (pages per call = 16384 / layers)")
@@ -485,6 +589,8 @@ def main():
         res = fp8_ring(ctx, layers=a.layers, **({"max_ctas": a.max_ctas} if a.max_ctas else {}))
     elif a.config == "bcast":
         res = nvls_bcast(ctx)
+    elif a.config == "gather":
+        res = gather(ctx)
     elif a.config == "baselines":
         res = baselines(ctx, 128 << 10)
     else:

@@ -171,6 +171,20 @@ class Connection {
                    uint64_t stream);
     int r_rdma_fp8(const std::vector<KeyOffset>& blocks, int elems, uint64_t base_ptr, int device,
                    uint64_t stream);
+    // Gathered blocks (kernels::GatherLaunch): a block is `nparts` parts of part_bytes, part s
+    // at part_base[s] + the block's local byte offset (one page of every layer under one key).
+    struct GatherSpec {
+        const uint64_t* part_base = nullptr;  // absolute addresses, all on `device` (or host)
+        uint32_t nparts = 0;
+        uint32_t part_bytes = 0;
+        uint32_t first_part = 0;  // reads: stored part first_part + s lands in part s
+    };
+    // offsets in bytes; blocks allocated with nparts * part_bytes bytes (trusted)
+    int w_rdma_gather(const GatherSpec& g, const uint64_t* offsets, size_t noffsets,
+                      const RemoteBlock* blocks, size_t nblocks, int device, uint64_t stream);
+    // a stored block must hold (first_part + nparts) * part_bytes bytes, else it is a miss
+    int r_rdma_scatter(const GatherSpec& g, const std::vector<KeyOffset>& blocks, int device,
+                       uint64_t stream);
 
     // --- async flavours: the callback runs on the connection's completion thread
     int allocate_async(const std::vector<std::string>& keys, int block_size,
@@ -229,7 +243,8 @@ class Connection {
     std::shared_ptr<fabric::Mapping> mapping(uint32_t seg, int device);
     int move_blocks(bool write, const uint64_t* local_off, uint64_t scale,
                     const RemoteBlock* blocks, size_t n, int block_size, uint64_t base_ptr,
-                    int device, uint64_t stream, int fp8_elems = 0, MoveResult* res = nullptr);
+                    int device, uint64_t stream, int fp8_elems = 0, MoveResult* res = nullptr,
+                    const GatherSpec* gather = nullptr);
     // tell the server that the blocks at `addrs` were not (completely) written: it releases
     // them, device-index entries included
     int discard_blocks(const uint64_t* addrs, size_t count);
@@ -240,7 +255,8 @@ class Connection {
                                           const std::vector<RemoteBlock>* rb, void* stream);
     int read_via_device_index(const std::vector<KeyOffset>& blocks, int block_size,
                               uint64_t base_ptr, int device, uint64_t stream, int fp8_elems = 0,
-                              MoveResult* res = nullptr, const PackedKeys* packed = nullptr);
+                              MoveResult* res = nullptr, const PackedKeys* packed = nullptr,
+                              const GatherSpec* gather = nullptr);
     int match_via_device_index(const std::vector<std::string_view>& keys, bool exist_only);
     int ensure_host_registered(uint64_t ptr, size_t bytes, int device, bool temporary);
     void release_temporary_host_regs();

@@ -191,11 +191,13 @@ kernels::IndexShards Connection::index_shards(DevCtx* ctx, bool* all_local) {
 }
 
 // Move n blocks between the caller's tensor and the pool.  local_off[i] * scale is the
-// byte offset of block i from base_ptr.
+// byte offset of block i from base_ptr.  With `gather` (base_ptr 0), block i is
+// gather->nparts parts, part s at gather->part_base[s] + local_off[i] * scale, and
+// block_size = nparts * part_bytes.
 int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scale,
                             const RemoteBlock* blocks, size_t n, int block_size,
                             uint64_t base_ptr, int device, uint64_t stream_in, int fp8_elems,
-                            MoveResult* res) {
+                            MoveResult* res, const GatherSpec* gather) {
     NvtxRange nvtx(write ? "istore.write_blocks" : "istore.read_blocks");
     std::lock_guard<std::mutex> lk(mu_);
     if (n == 0) return 0;
@@ -236,16 +238,32 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
                 auto m = mapping(addr_seg(blocks[i].remote_addr), -1);
                 if (!m || !m->host_ptr) return -1;
                 uint8_t* pool = m->host_ptr + addr_off(blocks[i].remote_addr);
-                uint8_t* local = reinterpret_cast<uint8_t*>(base_ptr + local_off[i] * scale);
-                if (write)
-                    std::memcpy(pool, local, size_t(block_size));
-                else
-                    std::memcpy(local, pool, size_t(block_size));
+                if (gather) {  // one memcpy per part
+                    const size_t pb = gather->part_bytes;
+                    for (uint32_t s = 0; s < gather->nparts; ++s) {
+                        uint8_t* local =
+                            reinterpret_cast<uint8_t*>(gather->part_base[s] + local_off[i] * scale);
+                        if (write)
+                            std::memcpy(pool + s * pb, local, pb);
+                        else
+                            std::memcpy(local, pool + (gather->first_part + s) * pb, pb);
+                    }
+                } else {
+                    uint8_t* local = reinterpret_cast<uint8_t*>(base_ptr + local_off[i] * scale);
+                    if (write)
+                        std::memcpy(pool, local, size_t(block_size));
+                    else
+                        std::memcpy(local, pool, size_t(block_size));
+                }
                 if (write) sink.push_back(blocks[i].remote_addr);
                 stats_.host_copies++;
             }
             (write ? stats_.bytes_written : stats_.bytes_read) += live * uint64_t(block_size);
             return 0;
+        }
+        if (gather) {
+            fail("gathered blocks of CPU tensors need a host-memory pool (--pool-backend host)");
+            return -1;
         }
         if (!fabric::cuda_available()) {
             fail("a CUDA device is required to reach an HBM pool");
@@ -264,7 +282,7 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
     DevCtx* ctx = dev_ctx(kd);
     if (!ctx) return -1;
     DeviceGuard g(kd);
-    if (cfg_.doorbell && write && n == 1 && device >= 0 && !fp8_elems && !res &&
+    if (cfg_.doorbell && write && n == 1 && device >= 0 && !fp8_elems && !res && !gather &&
         !is_fake_block(blocks[0])) {
         // latency mode: one block, handed to the persistent worker (no launch, no event)
         const RemoteBlock& rb = blocks[0];
@@ -306,10 +324,18 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
         }
     }
 
+    // gathered blocks: at most 2^30 work items per launch (a chunk is >= 16 KB or a whole part)
+    size_t max_batch = kMaxBatch;
+    uint64_t gather_align = 0;
+    if (gather) {
+        const uint64_t items = uint64_t(gather->nparts) * ((gather->part_bytes + 16383u) / 16384u);
+        max_batch = std::max<size_t>(1, std::min<uint64_t>(kMaxBatch, (1ull << 30) / items));
+        for (uint32_t s = 0; s < gather->nparts; ++s) gather_align |= gather->part_base[s];
+    }
     size_t i = 0;
     while (i < n) {
         const uint64_t t_build0 = now_ns();
-        const size_t batch_cap = std::min(kMaxBatch, n - i);
+        const size_t batch_cap = std::min(max_batch, n - i);
         const size_t at_desc = ctx->ring_alloc(batch_cap * sizeof(kernels::CopyDesc));
         auto* descs = reinterpret_cast<kernels::CopyDesc*>(ctx->ring_h + at_desc);
         size_t at_rec = 0;
@@ -336,6 +362,10 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
                 segbase = seg_dev_ptr(ctx, seg);
                 if (!segbase && !(seg < ctx->seg_mc.size() && ctx->seg_mc[seg])) return -1;
                 seg_ptr = ctx->seg_ptr.data();
+            }
+            if (gather && seg < ctx->seg_mc.size() && ctx->seg_mc[seg]) {
+                fail("gathered blocks cannot live in the replicated (NVLS) region");
+                return -1;
             }
             if (write && seg < ctx->seg_mc.size() && ctx->seg_mc[seg]) {
                 segbase = ctx->seg_mc[seg];  // replicated block: write through the multicast VA
@@ -399,7 +429,28 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
         const uint64_t t_launch0 = now_ns();
         stats_.ns_build += t_launch0 - t_build0;
         cudaError_t e;
-        if (fp8_elems) {
+        if (gather) {
+            kernels::GatherLaunch G;
+            G.descs = L.descs;
+            G.n = m;
+            G.write = write;
+            G.part_base = gather->part_base;
+            G.nparts = gather->nparts;
+            G.part_bytes = gather->part_bytes;
+            G.first_part = gather->first_part;
+            G.align_or = align_or | gather_align;
+            G.recs = L.recs;
+            G.table = L.table;
+            G.table_mask = L.table_mask;
+            G.done = L.done;
+            G.status = L.status;
+            G.max_ctas = L.max_ctas;
+            G.all_local = L.all_local;
+            G.shards = L.shards;
+            G.stage_bytes = pipe_stage_;
+            G.ring_bytes = pipe_ring_;
+            e = kernels::launch_kv_gather(G, stream);
+        } else if (fp8_elems) {
             kernels::Fp8Launch F;
             F.descs = L.descs;
             F.n = m;
@@ -489,6 +540,46 @@ int Connection::r_rdma(const std::vector<KeyOffset>& blocks, int block_size, uin
                        stream, 0, res);
 }
 
+static bool gather_spec_ok(const Connection::GatherSpec& g) {
+    return g.part_base && g.nparts >= 1 && g.nparts <= kernels::kGatherMaxParts && g.part_bytes &&
+           uint64_t(g.nparts) * g.part_bytes <= uint64_t(INT32_MAX);
+}
+
+int Connection::w_rdma_gather(const GatherSpec& g, const uint64_t* offsets, size_t noffsets,
+                              const RemoteBlock* blocks, size_t nblocks, int device,
+                              uint64_t stream) {
+    if (noffsets != nblocks || !gather_spec_ok(g)) {
+        fail("w_rdma_gather: bad parts list, or offsets and remote blocks differ in length");
+        return -1;
+    }
+    GatherSpec w = g;
+    w.first_part = 0;
+    return move_blocks(true, offsets, 1, blocks, nblocks, int(g.nparts * g.part_bytes), 0, device,
+                       stream, 0, nullptr, &w);
+}
+
+int Connection::r_rdma_scatter(const GatherSpec& g, const std::vector<KeyOffset>& blocks,
+                               int device, uint64_t stream) {
+    if (blocks.empty()) return 0;
+    if (!gather_spec_ok(g) ||
+        uint64_t(g.first_part) + g.nparts > uint64_t(INT32_MAX) / g.part_bytes) {
+        fail("r_rdma_scatter: bad parts list");
+        return -1;
+    }
+    const int block_size = int(g.nparts * g.part_bytes);
+    if (device_lookup_ && server_hbm_ && device >= 0 && device_index_usable())
+        return read_via_device_index(blocks, block_size, 0, device, stream, 0, nullptr, nullptr, &g);
+    std::vector<RemoteBlock> rb;
+    // the stored block must hold every part asked for
+    const int r = lookup_blocks(kOpReadLookup, blocks, int((g.first_part + g.nparts) * g.part_bytes),
+                                rb);
+    if (r != 0) return r;
+    std::vector<uint64_t> offs(blocks.size());
+    for (size_t i = 0; i < blocks.size(); ++i) offs[i] = blocks[i].offset;
+    return move_blocks(false, offs.data(), 1, rb.data(), rb.size(), block_size, 0, device, stream,
+                       0, nullptr, &g);
+}
+
 int Connection::rw_local(char op, const std::vector<KeyOffset>& blocks, int block_size,
                          uint64_t base_ptr, int device, uint64_t stream) {
     if (blocks.empty()) return 0;
@@ -532,7 +623,8 @@ static size_t pack_keys(const std::string_view* keys, size_t n, uint8_t* bytes, 
 
 int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int block_size,
                                       uint64_t base_ptr, int device, uint64_t stream_in,
-                                      int fp8_elems, MoveResult* res, const PackedKeys* packed) {
+                                      int fp8_elems, MoveResult* res, const PackedKeys* packed,
+                                      const GatherSpec* gather) {
     NvtxRange nvtx("istore.read_via_device_index");
     std::lock_guard<std::mutex> lk(mu_);
     DevCtx* ctx = dev_ctx(device);
@@ -542,8 +634,17 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
         fail("the server exposes no device index");
         return -1;
     }
+    // gathered blocks (scattered into parts): kv_pipe_scatter_read, or lookup + gather +
+    // validate for batches with fewer blocks than CTAs or unaligned parts (see below)
+    size_t step = kMaxBatch;
+    uint64_t gather_align = 0;
+    if (gather) {
+        const uint64_t items = uint64_t(gather->nparts) * ((gather->part_bytes + 16383u) / 16384u);
+        step = std::max<size_t>(1, std::min<uint64_t>(kMaxBatch, (1ull << 30) / items));
+        for (uint32_t s = 0; s < gather->nparts; ++s) gather_align |= gather->part_base[s];
+    }
     DeviceGuard g(device);
-    if (cfg_.doorbell && blocks.size() == 1 && !fp8_elems && !res &&
+    if (cfg_.doorbell && blocks.size() == 1 && !fp8_elems && !res && !gather &&
         doorbell_ready(ctx, stream_in, size_t(block_size))) {
         // latency mode: the key is hashed here, the worker probes, copies and re-checks
         const KeyHash kh = hash_key(reinterpret_cast<const uint8_t*>(blocks[0].key.data()),
@@ -564,9 +665,9 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
         res->stream = stream;
         res->device = device;
     }
-    for (size_t base = 0; base < blocks.size(); base += kMaxBatch) {
+    for (size_t base = 0; base < blocks.size(); base += step) {
         const uint64_t t_build0 = now_ns();
-        const size_t n = std::min(kMaxBatch, blocks.size() - base);
+        const size_t n = std::min(step, blocks.size() - base);
         // keys into the pinned ring, in the layout the kernels hash them from; three memcpys
         // when the caller holds them like that already (one batch), a pass over the keys else
         const bool prepacked = packed && base == 0 && packed->n == blocks.size() && n == blocks.size();
@@ -629,7 +730,26 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
         kernels::ReadFusedLaunch R;
         R.align_or = align_or;
         const bool fp8_fused = fp8_elems && kernels::fp8_read_fused_supported(R, uint32_t(fp8_elems));
-        if (fp8_fused || (!fp8_elems && (whole_blocks || small_batch))) {
+        // gathered blocks: one launch (resolver warp + gather pipeline, a CTA per block) once
+        // every CTA has a block of its own; fewer blocks: lookup + gather + validate below
+        kernels::GatherLaunch G;
+        bool gather_fused = false;
+        if (gather) {
+            G.n = uint32_t(n);
+            G.part_base = gather->part_base;
+            G.nparts = gather->nparts;
+            G.part_bytes = gather->part_bytes;
+            G.first_part = gather->first_part;
+            G.align_or = align_or | gather_align;
+            G.status = ctx->status_d;
+            G.max_ctas = grid_cap;
+            G.stage_bytes = pipe_stage_;
+            G.ring_bytes = pipe_ring_;
+            R.n = uint32_t(n);
+            R.max_ctas = grid_cap;
+            gather_fused = kernels::scatter_read_fused_supported(R, G);
+        }
+        if (gather_fused || (!gather && (fp8_fused || (!fp8_elems && (whole_blocks || small_batch))))) {
             // one kernel: hash + probe + move
             R.key_bytes = ctx->ring_d + at_bytes;
             R.key_off = reinterpret_cast<const uint32_t*>(ctx->ring_d + at_off);
@@ -654,8 +774,9 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
             R.ring_bytes = pipe_ring_;
             // fp8 pages: the resolver rides in the dequantising TMA pipeline (one launch
             // instead of lookup + read + validate: 32 calls of 512 pages were launch-bound)
-            e = fp8_fused ? kernels::launch_kv_fp8_read_fused(R, uint32_t(fp8_elems), stream)
-                          : kernels::launch_kv_read_fused(R, stream);
+            e = gather_fused ? kernels::launch_kv_pipe_scatter_read(R, G, stream)
+                : fp8_fused  ? kernels::launch_kv_fp8_read_fused(R, uint32_t(fp8_elems), stream)
+                             : kernels::launch_kv_read_fused(R, stream);
             stats_.kernel_launches += 1;
         } else {
             kernels::LookupLaunch Q;
@@ -673,13 +794,17 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
             Q.out_descs = out;
             Q.dst_off = reinterpret_cast<const uint64_t*>(ctx->ring_d + at_dst);
             Q.dst_base = base_ptr;
-            Q.need_bytes = uint32_t(block_size);
+            Q.need_bytes = gather ? (gather->first_part + gather->nparts) * gather->part_bytes
+                                  : uint32_t(block_size);
             Q.status = ctx->status_d;
             // optimistic read: the entries are re-checked after the copy (purge / eviction)
             Q.found_at = reinterpret_cast<kernels::LookupLaunch::FoundAt*>(
                     ctx->scratch + ctx->scratch_alloc(n * sizeof(kernels::LookupLaunch::FoundAt)));
             e = kernels::launch_index_lookup(Q, stream);
-            if (e == cudaSuccess && fp8_elems) {
+            if (e == cudaSuccess && gather) {
+                G.descs = out;  // {pool address or 0, local byte offset} (dst_base 0)
+                e = kernels::launch_kv_gather(G, stream);
+            } else if (e == cudaSuccess && fp8_elems) {
                 kernels::Fp8Launch F;
                 F.descs = out;
                 F.n = uint32_t(n);

@@ -129,6 +129,54 @@ cudaError_t launch_kv_copy(const CopyLaunch& a, cudaStream_t stream);
 constexpr uint32_t kPipeMinBytes = 64u << 10;
 // The TMA pipeline itself (kv_pipe.cu); needs 16-byte aligned addresses and sizes.
 cudaError_t launch_kv_pipe_copy(const CopyLaunch& a, cudaStream_t stream);
+
+// Gathered blocks: pool block i is the concatenation of `nparts` parts of part_bytes each,
+// part s taken from (write) or scattered to (read) part_base[s] + the block's local offset -
+// one page of every layer of a paged KV cache under one key, with no pack/unpack kernel.
+// Work item = (block, part, chunk), numbered block * nparts * cpp + part * cpp + chunk, so a
+// chunk never crosses a part and the in-band commit (publish.cuh) counts nparts * cpp
+// arrivals per block.  The part bases travel in the kernel parameters.
+constexpr uint32_t kGatherMaxParts = 256;
+struct GatherLaunch {
+    // per block, device-addressable: write {local byte offset, pool address},
+    // read {pool address or 0 = miss, local byte offset}
+    const CopyDesc* descs = nullptr;
+    uint32_t n = 0;
+    bool write = false;
+    const uint64_t* part_base = nullptr;  // host array of nparts absolute addresses
+    uint32_t nparts = 0;
+    uint32_t part_bytes = 0;
+    uint32_t first_part = 0;  // reads: pool part first_part + s lands in part s
+    uint64_t align_or = 0;    // OR of every part base and local offset
+    // optional in-band commit (writes), as in CopyLaunch; recs[i].size covers all parts
+    const IndexEntry* recs = nullptr;
+    IndexBucket* table = nullptr;
+    uint64_t table_mask = 0;
+    uint32_t* done = nullptr;  // 3*n zeroed u32 of client-local device scratch
+    uint32_t* status = nullptr;  // reads: a missing block counts once in kStatMiss
+    int max_ctas = 0;
+    bool all_local = false;
+    IndexShards shards;
+    uint32_t stage_bytes = 0;  // TMA pipeline geometry, 0 = default
+    uint32_t ring_bytes = 0;
+};
+// The TMA pipeline for 16-byte aligned parts of at least kPipeMinBytes, the ld/st kernel
+// (kv_copy.cu) otherwise: the same rule launch_kv_copy applies to whole blocks.
+cudaError_t launch_kv_gather(const GatherLaunch& a, cudaStream_t stream);
+cudaError_t launch_kv_pipe_gather(const GatherLaunch& a, cudaStream_t stream);
+struct GatherParts {
+    uint64_t base[kGatherMaxParts];
+};
+struct ReadFusedLaunch;
+// A scattered read through the device index in ONE launch (kv_pipe.cu): the resolver warp of
+// kv_pipe_read feeding the gather pipeline.  CTA c owns blocks c, c + grid, ...: each key is
+// probed once, by the CTA that moves all of its parts, and re-checked after the copy.  `r`
+// carries keys, dst_off (local byte offsets; dst_base 0), index, segments, status, grid cap
+// and ring geometry; `g` the parts (descs, recs and write are ignored).  Needs 16-byte aligned
+// parts and at least as many blocks as CTAs (fewer: lookup + launch_kv_gather + validate).
+bool scatter_read_fused_supported(const ReadFusedLaunch& r, const GatherLaunch& g);
+cudaError_t launch_kv_pipe_scatter_read(const ReadFusedLaunch& r, const GatherLaunch& g,
+                                        cudaStream_t stream);
 struct PipeGeometry {
     uint32_t stage_bytes = 0;
     uint32_t stages = 0;

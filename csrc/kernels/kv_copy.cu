@@ -89,6 +89,55 @@ __global__ void __launch_bounds__(kLdStThreads + 32)
     if (pub.recs) ctrl_barrier_arrive(kLdStThreads + 32);
 }
 
+// ---------------------------------------------------------------- gathered blocks (ld/st)
+// Item = chunk c of part s of block b, numbered (b * nparts + s) * cpp + c (GatherLaunch).
+// write: local parts.base[s] + desc.src -> pool desc.dst + s * part_bytes;
+// read:  pool desc.src + (first_part + s) * part_bytes -> local parts.base[s] + desc.dst.
+// The minimum of 3 CTAs per SM lets the 32-byte flavour keep 64 registers; without it ptxas
+// held it to 56 and spilled.
+template <int VEC>
+__global__ void __launch_bounds__(kLdStThreads + 32, 3)
+    kv_gather_ldst_kernel(const CopyDesc* __restrict__ descs,
+                          const __grid_constant__ GatherParts parts, uint32_t n, uint32_t nparts,
+                          uint32_t part_bytes, uint32_t first_part, uint32_t chunk, uint32_t cpp,
+                          bool write, Publish pub) {
+    const uint32_t cpb = nparts * cpp;  // items per block: what the commit counter counts
+    const uint32_t total = n * cpb;
+    if (threadIdx.x >= kLdStThreads) {
+        if (!pub.recs) return;
+        const uint32_t count = blockIdx.x < total ? (total - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+        control_warp(pub, threadIdx.x - kLdStThreads, blockIdx.x, count, gridDim.x, cpb,
+                     kLdStThreads + 32);
+        return;
+    }
+    uint32_t item = blockIdx.x;
+    CopyDesc next = item < total ? descs[item / cpb] : CopyDesc{0, 0};
+    for (; item < total; item += gridDim.x) {
+        const CopyDesc d = next;
+        const uint32_t nxt = item + gridDim.x;
+        if (nxt < total) next = descs[nxt / cpb];  // prefetch: descriptors may sit in host memory
+        const uint32_t in_block = item % cpb;
+        if (!write && d.src == 0) {  // key not found: one miss per block, parts left untouched
+            if (threadIdx.x == 0 && in_block == 0 && pub.status) atomicAdd(pub.status + kStatMiss, 1u);
+            continue;
+        }
+        const uint32_t s = in_block / cpp;
+        const uint32_t off = (in_block % cpp) * chunk;
+        const uint32_t len = min(chunk, part_bytes - off);
+        const uint64_t local = parts.base[s] + (write ? d.src : d.dst) + off;
+        const uint64_t pool = (write ? d.dst + uint64_t(s) * part_bytes
+                                     : d.src + uint64_t(first_part + s) * part_bytes) + off;
+        uint8_t* dst = reinterpret_cast<uint8_t*>(write ? pool : local);
+        const uint8_t* src = reinterpret_cast<const uint8_t*>(write ? local : pool);
+        if constexpr (VEC == 1) {
+            for (uint32_t b = threadIdx.x; b < len; b += kLdStThreads) dst[b] = src[b];
+        } else {
+            copy_span<VEC>(dst, src, len);
+        }
+    }
+    if (pub.recs) ctrl_barrier_arrive(kLdStThreads + 32);
+}
+
 }  // namespace
 
 int sm_count() {
@@ -171,6 +220,50 @@ cudaError_t launch_kv_copy(const CopyLaunch& a, cudaStream_t stream) {
         kv_copy_ldst_kernel<16, true><<<ctas, T, 0, stream>>>(a.descs, pd, a.n, a.bytes, chunk, cpb, pub);
     else
         kv_copy_ldst_kernel<16, false><<<ctas, T, 0, stream>>>(a.descs, none, a.n, a.bytes, chunk, cpb, pub);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_kv_gather(const GatherLaunch& a, cudaStream_t stream) {
+    if (a.n == 0 || a.part_bytes == 0) return cudaSuccess;
+    if (a.nparts == 0 || a.nparts > kGatherMaxParts || !a.part_base) return cudaErrorInvalidValue;
+    if (uint64_t(a.nparts) * a.part_bytes > 0xffffffffull) return cudaErrorInvalidValue;
+    const bool aligned16 = (a.part_bytes % 16) == 0 && (a.align_or & 15) == 0;
+    const bool aligned32 = (a.part_bytes % 32) == 0 && (a.align_or & 31) == 0;
+    // the per-part rule of launch_kv_copy: a part is what one item stream moves contiguously
+    if (aligned16 && a.part_bytes >= kPipeMinBytes) return launch_kv_pipe_gather(a, stream);
+    Publish pub{a.recs, a.table, a.table_mask, a.done, a.status, a.n, nullptr, !a.all_local, 0,
+                a.shards};
+    if (!a.write || !a.table || !a.done) pub.recs = nullptr;
+    const int sms = sm_count();
+    const uint64_t parts_total = uint64_t(a.n) * a.nparts;
+    // whole parts as items once there are as many parts as SMs (see launch_kv_copy)
+    uint32_t chunk = std::min(a.part_bytes, kLdStChunk);
+    if (parts_total >= uint64_t(sms) && a.part_bytes <= (1u << 20)) chunk = a.part_bytes;
+    const uint32_t cpp = (a.part_bytes + chunk - 1) / chunk;
+    const uint64_t total = parts_total * cpp;
+    if (total > 0x7fffffffull) return cudaErrorInvalidValue;  // the caller splits the batch
+    constexpr int T = kLdStThreads + 32;
+    static int resident16 = 0, resident32 = 0;
+    if (!resident16) {
+        int b16 = 0, b32 = 0;
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b16, kv_gather_ldst_kernel<16>, T, 0);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b32, kv_gather_ldst_kernel<32>, T, 0);
+        resident16 = std::max(b16, 1);
+        resident32 = std::max(b32, 1);
+    }
+    int ctas = a.max_ctas > 0 ? a.max_ctas : (aligned32 ? resident32 : resident16) * sms;
+    ctas = int(std::min<uint64_t>(uint64_t(ctas), total));
+    GatherParts parts;
+    std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
+    if (!aligned16)
+        kv_gather_ldst_kernel<1><<<ctas, T, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.part_bytes,
+                                                         a.first_part, chunk, cpp, a.write, pub);
+    else if (aligned32)
+        kv_gather_ldst_kernel<32><<<ctas, T, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.part_bytes,
+                                                          a.first_part, chunk, cpp, a.write, pub);
+    else
+        kv_gather_ldst_kernel<16><<<ctas, T, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.part_bytes,
+                                                          a.first_part, chunk, cpp, a.write, pub);
     return cudaGetLastError();
 }
 

@@ -220,6 +220,67 @@ __global__ void __launch_bounds__(kPipeThreads)
     }
 }
 
+// ---------------------------------------------------------------- kv_pipe_gather
+// Gathered blocks (GatherLaunch) through the same loader / storer bodies: part s of block b is
+// the virtual block b * nparts + s of part_bytes (sh.n virtual blocks, sh.cpb chunks each), so
+// global item numbers are those of GatherLaunch and the control warp counts nparts * sh.cpb
+// arrivals per real block.  The descriptor window walks the real blocks' descriptors.
+__global__ void __launch_bounds__(kPipeThreads)
+    kv_pipe_gather_kernel(const CopyDesc* __restrict__ descs,
+                          const __grid_constant__ GatherParts parts, const Shape sh,
+                          uint32_t nparts, uint32_t first_part, bool write, Publish pub) {
+    extern __shared__ __align__(128) uint8_t ring[];
+    __shared__ __align__(8) uint64_t full[kPipeMaxStages];
+    __shared__ __align__(8) uint64_t empty[kPipeMaxStages];
+    const uint32_t cpb = nparts * sh.cpb;  // items per real block
+    const uint32_t total = sh.n * sh.cpb;
+    const uint32_t grid = gridDim.x;
+    const uint32_t nitems = blockIdx.x < total ? (total - blockIdx.x + grid - 1) / grid : 0;
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) {
+        for (uint32_t s = 0; s < sh.stages; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], 1);
+        }
+        mbar_fence_init();
+    }
+    __syncthreads();
+    if (warp == 2) {  // control warp: in-band commit
+        if (pub.recs) control_warp(pub, lane, blockIdx.x, nitems, grid, cpb, 64);
+        return;
+    }
+    DescWindow<false> win{descs, nullptr, blockIdx.x, grid, cpb, nitems, lane};
+    win.init();
+    auto desc_at = [&](uint32_t k) {
+        const CopyDesc b = win.at(k);
+        const uint32_t item = blockIdx.x + k * grid;
+        const uint32_t s = (item % cpb) / sh.cpb;
+        CopyDesc d;
+        if (write) {
+            d.src = parts.base[s] + b.src;
+            d.dst = b.dst + uint64_t(s) * sh.bytes;
+        } else {
+            d.src = b.src ? b.src + uint64_t(first_part + s) * sh.bytes : 0;
+            d.dst = parts.base[s] + b.dst;
+        }
+        return d;
+    };
+    if (warp == 0) {
+        loader_body(sh, blockIdx.x, grid, nitems, lane, ring, full, empty, desc_at);
+    } else {
+        // misses are counted here, once per block, not by storer_body once per part
+        storer_body(sh, blockIdx.x, grid, nitems, lane, ring, full, empty, nullptr,
+                    [&](uint32_t k) {
+                        const CopyDesc d = desc_at(k);
+                        if (lane == 0 && d.src == 0 && (blockIdx.x + k * grid) % cpb == 0 &&
+                            pub.status)
+                            atomicAdd(pub.status + kStatMiss, 1u);
+                        return d;
+                    });
+        if (pub.recs) ctrl_barrier_arrive(64);
+    }
+}
+
 // ---------------------------------------------------------------- kv_pipe_read (fused)
 // resolver warp + queue: resolve.cuh
 __global__ void __launch_bounds__(kPipeThreads)
@@ -255,6 +316,60 @@ __global__ void __launch_bounds__(kPipeThreads)
         storer_body(sh, blockIdx.x, grid, nitems, lane, ring, full, empty, a.status,
                     [&](uint32_t k) { return resolved_desc<true, true>(rq, k, lane); });
         resolved_done(rq, nitems, lane);
+    }
+}
+
+// ---------------------------------------------------------------- kv_pipe_scatter_read (fused)
+// CTA c owns blocks c, c + grid, ...; the resolver warp resolves them in that order, one probe
+// per key.  Loader and storer walk the CTA's local items k = 0, 1, ...: part (k / cpb) % nparts
+// (sh.cpb chunks per part) of the CTA's block k / (nparts * sh.cpb), so every part of a block
+// is moved by the CTA that resolved it.  The resolver re-checks each entry once the storer has
+// handed its queue half back (every load of those blocks has completed by then).
+__global__ void __launch_bounds__(kPipeThreads)
+    kv_pipe_scatter_read_kernel(const __grid_constant__ ResolveArgs a,
+                                const __grid_constant__ GatherParts parts, const Shape sh,
+                                uint32_t nparts, uint32_t first_part) {
+    extern __shared__ __align__(128) uint8_t ring[];
+    __shared__ __align__(8) uint64_t full[kPipeMaxStages];
+    __shared__ __align__(8) uint64_t empty[kPipeMaxStages];
+    __shared__ __align__(16) ResolveQueue rq;
+    const uint32_t grid = gridDim.x;
+    const uint32_t nblocks = blockIdx.x < sh.n ? (sh.n - blockIdx.x + grid - 1) / grid : 0;
+    const uint32_t per_block = nparts * sh.cpb;
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) {
+        for (uint32_t s = 0; s < sh.stages; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], 1);
+        }
+        resolve_queue_init(rq);
+        mbar_fence_init();
+    }
+    __syncthreads();
+    if (warp == 2) {  // ---- resolver: a hit must hold every part asked for
+        resolver_warp(a, rq, (first_part + nparts) * sh.bytes, blockIdx.x, grid, 1, nblocks, lane);
+        return;
+    }
+    const bool storer = warp == 1;
+    uint32_t cur_j = ~0u;  // the CTA's block whose descriptor `cur` holds
+    CopyDesc cur{0, 0};
+    auto desc_at = [&](uint32_t k) {  // warp-wide; k non-decreasing, so j advances one by one
+        const uint32_t j = k / per_block;
+        if (j != cur_j) {
+            cur = storer ? resolved_desc<true, true>(rq, j, lane) : resolved_desc<false, true>(rq, j, lane);
+            cur_j = j;
+            // a missing key is one miss, whatever the number of parts
+            if (storer && lane == 0 && cur.src == 0 && a.status) atomicAdd(a.status + kStatMiss, 1u);
+        }
+        const uint32_t s = (k / sh.cpb) % nparts;
+        return CopyDesc{cur.src ? cur.src + uint64_t(first_part + s) * sh.bytes : 0,
+                        parts.base[s] + cur.dst};
+    };
+    if (warp == 0) {
+        loader_body(sh, 0, 1, nblocks * per_block, lane, ring, full, empty, desc_at);
+    } else {
+        storer_body(sh, 0, 1, nblocks * per_block, lane, ring, full, empty, nullptr, desc_at);
+        resolved_done(rq, nblocks, lane);
     }
 }
 
@@ -499,6 +614,12 @@ cudaError_t ensure_pipe_attrs() {
         e = cudaFuncSetAttribute(kv_pipe_read_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  kMax);
     if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(kv_pipe_gather_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 kMax);
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(kv_pipe_scatter_read_kernel,
+                                 cudaFuncAttributeMaxDynamicSharedMemorySize, kMax);
+    if (e == cudaSuccess)
         e = cudaFuncSetAttribute(kv_pipe_mcast_kernel<2>,
                                  cudaFuncAttributeMaxDynamicSharedMemorySize, kMax);
     if (e == cudaSuccess)
@@ -589,6 +710,81 @@ cudaError_t launch_kv_pipe_copy(const CopyLaunch& a, cudaStream_t stream) {
         const PipeDescParam<1> none{};
         kv_pipe_copy_kernel<false><<<ctas, kPipeThreads, g.smem, stream>>>(a.descs, none, sh, pub, fan);
     }
+    return cudaGetLastError();
+}
+
+cudaError_t launch_kv_pipe_gather(const GatherLaunch& a, cudaStream_t stream) {
+    if (a.n == 0 || a.part_bytes == 0) return cudaSuccess;
+    if (a.nparts == 0 || a.nparts > kGatherMaxParts || !a.part_base || (a.part_bytes % 16) != 0 ||
+        (a.align_or & 15) != 0)
+        return cudaErrorInvalidValue;
+    cudaError_t e = ensure_pipe_attrs();
+    if (e != cudaSuccess) return e;
+    Publish pub{a.recs, a.table, a.table_mask, a.done, a.status, a.n, nullptr, !a.all_local, 0,
+                a.shards};
+    if (!a.write || !a.table || !a.done) pub.recs = nullptr;
+    const int sms = sm_count();
+    const PipeGeometry g = pipe_geometry(a.part_bytes, a.stage_bytes, a.ring_bytes);
+    int ctas = a.max_ctas > 0 ? std::min(a.max_ctas, sms) : sms;
+    // chunks of one part, balanced over the grid as for whole blocks (balance.h)
+    const uint64_t parts_total = uint64_t(a.n) * a.nparts;
+    if (parts_total > 0x7fffffffull) return cudaErrorInvalidValue;
+    const ChunkPlan plan = plan_chunks(uint32_t(parts_total),
+                                       (a.part_bytes + g.stage_bytes - 1) / g.stage_bytes, 4,
+                                       std::max(4u, (1u << 20) / g.stage_bytes), uint32_t(ctas));
+    const uint32_t chunk = std::min(a.part_bytes, plan.chunk * g.stage_bytes);
+    const uint32_t cpp = (a.part_bytes + chunk - 1) / chunk;
+    const uint64_t total = parts_total * cpp;
+    if (total > 0x7fffffffull) return cudaErrorInvalidValue;  // the caller splits the batch
+    ctas = int(std::min<uint64_t>(uint64_t(ctas), total));
+    const Shape sh{uint32_t(parts_total), a.part_bytes, chunk, cpp, g.stage_bytes, g.stages};
+    GatherParts parts;
+    std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
+    kv_pipe_gather_kernel<<<ctas, kPipeThreads, g.smem, stream>>>(a.descs, parts, sh, a.nparts,
+                                                                  a.first_part, a.write, pub);
+    return cudaGetLastError();
+}
+
+static int scatter_read_ctas(const ReadFusedLaunch& r) {
+    return r.max_ctas > 0 ? std::min(r.max_ctas, sm_count()) : sm_count();
+}
+
+bool scatter_read_fused_supported(const ReadFusedLaunch& r, const GatherLaunch& g) {
+    return g.nparts >= 1 && g.nparts <= kGatherMaxParts && g.part_base && g.part_bytes &&
+           (g.part_bytes % 16) == 0 && (g.align_or & 15) == 0 &&
+           r.n >= uint32_t(scatter_read_ctas(r));
+}
+
+cudaError_t launch_kv_pipe_scatter_read(const ReadFusedLaunch& r, const GatherLaunch& g,
+                                        cudaStream_t stream) {
+    if (r.n == 0) return cudaSuccess;
+    if (!scatter_read_fused_supported(r, g) ||
+        uint64_t(g.first_part + g.nparts) * g.part_bytes > 0xffffffffull ||
+        uint64_t(r.n) * g.nparts > 0x7fffffffull)
+        return cudaErrorInvalidValue;
+    cudaError_t e = ensure_pipe_attrs();
+    if (e != cudaSuccess) return e;
+    const PipeGeometry geo = pipe_geometry(g.part_bytes, r.stage_bytes, r.ring_bytes);
+    const int ctas = scatter_read_ctas(r);
+    ResolveArgs ra{};
+    ra.key_bytes = r.key_bytes;
+    ra.key_off = r.key_off;
+    ra.key_len = r.key_len;
+    ra.dst_off = r.dst_off;
+    ra.dst_base = r.dst_base;
+    ra.table = r.table;
+    ra.table_mask = r.table_mask;
+    ra.shards = r.shards;
+    ra.nsegs = r.nsegs;
+    for (uint32_t s = 0; s < r.nsegs && s < uint32_t(ReadFusedLaunch::kMaxSegs); ++s)
+        ra.seg_base[s] = r.seg_base[s];
+    ra.status = r.status;
+    GatherParts parts;
+    std::memcpy(parts.base, g.part_base, size_t(g.nparts) * sizeof(uint64_t));
+    // whole parts as items: a CTA moves whole blocks, the ring cuts them into pieces
+    const Shape sh{r.n, g.part_bytes, g.part_bytes, 1, geo.stage_bytes, geo.stages};
+    kv_pipe_scatter_read_kernel<<<ctas, kPipeThreads, geo.smem, stream>>>(ra, parts, sh, g.nparts,
+                                                                          g.first_part);
     return cudaGetLastError();
 }
 

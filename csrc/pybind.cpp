@@ -549,6 +549,46 @@ PYBIND11_MODULE(_infinistore, m) {
             py::arg("blocks"), py::arg("elems"), py::arg("base_ptr"), py::arg("device") = -1,
             py::arg("stream") = 0, py::arg("scale") = 1)
         .def(
+            "w_rdma_gather",
+            [](Connection& c, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
+               const py::object& offsets, const py::object& remote_blocks, int device,
+               uint64_t stream, uint64_t scale) {
+                BlockSpan rb;
+                OffsetSpan off;
+                blocks_from_py(remote_blocks, rb);
+                offsets_from_py(offsets, off);
+                std::vector<uint64_t> bytes(off.n);
+                for (size_t i = 0; i < off.n; ++i) bytes[i] = off.data[i] * scale;
+                Connection::GatherSpec g;
+                g.part_base = part_base.data();
+                g.nparts = uint32_t(part_base.size());
+                g.part_bytes = part_bytes;
+                py::gil_scoped_release rel;
+                return c.w_rdma_gather(g, bytes.data(), bytes.size(), rb.data, rb.n, device, stream);
+            },
+            py::arg("part_base"), py::arg("part_bytes"), py::arg("offsets"),
+            py::arg("remote_blocks"), py::arg("device") = -1, py::arg("stream") = 0,
+            py::arg("scale") = 1,
+            "gathered write: block i = part s at part_base[s] + offsets[i] * scale, s = 0..S-1")
+        .def(
+            "r_rdma_scatter",
+            [](Connection& c, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
+               uint32_t first_part, const py::object& blocks, int device, uint64_t stream,
+               uint64_t scale) {
+                std::vector<KeyOffset> kb;
+                blocks_list_from_py(blocks, scale, kb);
+                Connection::GatherSpec g;
+                g.part_base = part_base.data();
+                g.nparts = uint32_t(part_base.size());
+                g.part_bytes = part_bytes;
+                g.first_part = first_part;
+                py::gil_scoped_release rel;
+                return c.r_rdma_scatter(g, kb, device, stream);
+            },
+            py::arg("part_base"), py::arg("part_bytes"), py::arg("first_part"), py::arg("blocks"),
+            py::arg("device") = -1, py::arg("stream") = 0, py::arg("scale") = 1,
+            "scattered read: stored part first_part + s of each block -> part_base[s] + offset")
+        .def(
             "rw_local",
             [](Connection& c, const std::string& op, const py::object& blocks, int block_size,
                uint64_t base_ptr, int device, uint64_t stream, uint64_t scale) {
@@ -809,6 +849,42 @@ PYBIND11_MODULE(_infinistore, m) {
         py::arg("status") = 0, py::arg("align_or") = 0, py::arg("trace") = 0,
         py::arg("all_local") = false, py::arg("debug") = 0, py::arg("stage_bytes") = 0,
         py::arg("ring_bytes") = 0, py::arg("fan_delta") = std::vector<int64_t>());
+    k.attr("GATHER_MAX_PARTS") = int(kernels::kGatherMaxParts);
+    k.def(
+        "kv_gather",
+        [](uint64_t descs, uint32_t n, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
+           uint32_t first_part, bool write, int max_ctas, uint64_t stream, uint64_t recs,
+           uint64_t table, uint64_t table_mask, uint64_t done, uint64_t status, uint64_t align_or,
+           uint32_t stage_bytes, uint32_t ring_bytes) {
+            if (part_base.empty() || part_base.size() > kernels::kGatherMaxParts)
+                throw std::runtime_error("kv_gather: 1 to GATHER_MAX_PARTS parts");
+            kernels::GatherLaunch G;
+            G.descs = as_ptr<const kernels::CopyDesc>(descs);
+            G.n = n;
+            G.write = write;
+            G.part_base = part_base.data();
+            G.nparts = uint32_t(part_base.size());
+            G.part_bytes = part_bytes;
+            G.first_part = first_part;
+            G.align_or = align_or;
+            G.recs = as_ptr<const kernels::IndexEntry>(recs);
+            G.table = as_ptr<kernels::IndexBucket>(table);
+            G.table_mask = table_mask;
+            G.done = as_ptr<uint32_t>(done);
+            G.status = as_ptr<uint32_t>(status);
+            G.max_ctas = max_ctas;
+            G.stage_bytes = stage_bytes;
+            G.ring_bytes = ring_bytes;
+            const cudaError_t e = kernels::launch_kv_gather(G, as_ptr<CUstream_st>(stream));
+            if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
+        },
+        py::arg("descs"), py::arg("n"), py::arg("part_base"), py::arg("part_bytes"),
+        py::arg("first_part") = 0, py::arg("write") = true, py::arg("max_ctas") = 0,
+        py::arg("stream") = 0, py::arg("recs") = 0, py::arg("table") = 0,
+        py::arg("table_mask") = 0, py::arg("done") = 0, py::arg("status") = 0,
+        py::arg("align_or") = 0, py::arg("stage_bytes") = 0, py::arg("ring_bytes") = 0,
+        "gathered blocks: descs[i] = write {local byte offset, block address} / read {block "
+        "address or 0, local byte offset}; part s of block i at part_base[s] + local offset");
     k.def(
         "kv_pipe_mcast",
         [](uint64_t descs, uint32_t n, uint32_t bytes, const std::vector<int64_t>& delta,

@@ -23,6 +23,7 @@ import os
 import time
 from typing import List, Tuple
 
+import numpy as np
 import torch
 
 from . import _infinistore
@@ -34,6 +35,10 @@ LINK_ETHERNET = "Ethernet"
 LINK_IB = "IB"
 
 _LOG_LEVELS = ("error", "debug", "info", "warning")
+# gathered blocks: parts per block (2 x 126 layers of Llama-3.1-405B fit), and the block size
+# the kernels and the wire carry (a signed 32-bit byte count)
+GATHER_MAX_PARTS = _infinistore.kernels.GATHER_MAX_PARTS
+_GATHER_MAX_BLOCK_BYTES = (1 << 31) - 1
 _CUDA_STREAM_LEGACY = 1  # cudaStreamLegacy handle: torch's default stream has handle 0
 
 
@@ -584,6 +589,107 @@ class InfinityConnection:
         pages, heads, tokens, dim = cache.shape
         ret = self.conn.r_rdma_hnd(blocks, tokens, heads, dim, info.es, info.ptr, pages, info.dev,
                                    self._stream(info, cache, stream))
+        if ret < 0:
+            raise Exception(f"Failed to read to infinistore, ret = {ret}: {self.conn.last_error()}")
+
+    # ------------------------------------------------------------------ gathered blocks
+    def _gather_parts(self, parts, max_offset: int, part_size: int):
+        """Checks a parts list ``[(tensor, base), ...]`` before anything is enqueued.  Returns
+        (absolute byte address of every part, device ordinal or -1, element size)."""
+        if self._mode != "rdma":
+            raise Exception("gathered blocks need a connected rdma connection")
+        parts = list(parts)
+        if not 1 <= len(parts) <= GATHER_MAX_PARTS:
+            raise ValueError(f"a parts list holds 1 to {GATHER_MAX_PARTS} parts, not {len(parts)}")
+        for i, part in enumerate(parts):
+            if not (isinstance(part, (tuple, list)) and len(part) == 2
+                    and isinstance(part[0], torch.Tensor)):
+                raise ValueError(f"part {i} is not a (tensor, base) pair")
+        if int(part_size) <= 0:
+            raise ValueError("part_size must be positive")
+        first = parts[0][0]
+        es = first.element_size()
+        if len(parts) * int(part_size) * es > _GATHER_MAX_BLOCK_BYTES:
+            raise ValueError(f"{len(parts)} parts of {int(part_size) * es} bytes exceed the "
+                             f"{_GATHER_MAX_BLOCK_BYTES}-byte block limit")
+        bases = []
+        for i, (t, base) in enumerate(parts):
+            base = int(base)
+            if not t.is_contiguous():
+                raise ValueError(f"part {i}: tensor must be contiguous")
+            if t.device != first.device:
+                raise ValueError(f"part {i}: tensor on {t.device}, part 0 on {first.device}")
+            if t.dtype != first.dtype:
+                raise ValueError(f"part {i}: dtype {t.dtype}, part 0 has {first.dtype}")
+            if base < 0 or base + max_offset + int(part_size) > t.numel():
+                raise ValueError(f"part {i}: base {base} + offset {max_offset} + part_size "
+                                 f"{int(part_size)} runs past the tensor's {t.numel()} elements")
+            bases.append(t.data_ptr() + base * es)
+        dev = _device_of(first)
+        if dev < 0 and self.conn.server_has_hbm():
+            raise ValueError("gathered blocks of CPU tensors need a host-memory pool "
+                             "(--pool-backend host)")
+        return bases, dev, es
+
+    def rdma_write_cache_gather(self, parts, offsets, part_size: int, remote_blocks,
+                                stream="current"):
+        """Write block ``i`` as the concatenation over ``s`` of
+        ``parts[s][0].view(-1)[parts[s][1] + offsets[i] : ... + part_size]``.
+
+        ``parts`` is a list of up to ``GATHER_MAX_PARTS`` pairs ``(tensor, base)`` - contiguous
+        tensors of one device and dtype, ``base`` in elements; ``offsets`` (a list or an int64
+        ndarray) and ``part_size`` are in elements.  One key then covers, e.g., one page of
+        every layer's K and V of a vLLM-style cache, and the gather runs inside the write
+        kernel: no pack kernel, no staging buffer.  The blocks must have been allocated with
+        ``len(parts) * part_size * element_size`` bytes; that is trusted, as
+        ``rdma_write_cache`` trusts ``page_size``.  Blocks the server marked as already
+        existing are skipped (first writer wins); the in-band commit publishes a block once,
+        after all of its parts have landed.  CPU tensors need a host-memory pool."""
+        offs = np.ascontiguousarray(offsets, dtype=np.int64).reshape(-1)
+        if len(offs) != len(remote_blocks):
+            raise ValueError(f"{len(offs)} offsets for {len(remote_blocks)} remote blocks")
+        if len(offs) and int(offs.min()) < 0:
+            raise ValueError("offsets must not be negative")
+        bases, dev, es = self._gather_parts(parts, int(offs.max()) if len(offs) else 0, part_size)
+        if not len(offs):
+            return 0
+        ret = self.conn.w_rdma_gather(bases, int(part_size) * es, offs, remote_blocks, dev,
+                                      _stream_of(parts[0][0], stream), es)
+        if ret < 0:
+            raise Exception(f"Failed to write to infinistore, ret = {ret}: {self.conn.last_error()}")
+        return 0
+
+    def read_cache_scatter(self, parts, blocks, part_size: int, first_part: int = 0,
+                           stream="current"):
+        """Scatter parts ``first_part .. first_part + len(parts) - 1`` of every stored block
+        into the parts list (see ``rdma_write_cache_gather``): stored part ``first_part + s``
+        of block ``(key, offset)`` lands at ``parts[s][1] + offset`` of ``parts[s][0]``.
+
+        ``blocks`` is ``[(key, offset)]`` or ``(keys, offsets)``, offsets in elements.
+        ``first_part`` lets a decoder fetch one layer of all-layer blocks while the previous
+        layer computes.  A missing key raises (with ``device_lookup``, ``sync()`` reports it)
+        and counts once, not once per part; its destination parts are left untouched.  With
+        ``device_lookup`` a stored block shorter than ``(first_part + len(parts)) * part_size``
+        elements is a miss, and a block purged or evicted during the read is reported as one."""
+        if isinstance(blocks, tuple) and len(blocks) == 2 and isinstance(blocks[1], np.ndarray):
+            keys = list(blocks[0])
+            offs = np.ascontiguousarray(blocks[1], dtype=np.int64).reshape(-1)
+            if len(keys) != len(offs):
+                raise ValueError(f"{len(keys)} keys for {len(offs)} offsets")
+        else:
+            keys = [b[0] for b in blocks]
+            offs = np.asarray([int(b[1]) for b in blocks], dtype=np.int64)
+        if len(offs) and int(offs.min()) < 0:
+            raise ValueError("offsets must not be negative")
+        if int(first_part) < 0:
+            raise ValueError("first_part must not be negative")
+        bases, dev, es = self._gather_parts(parts, int(offs.max()) if len(offs) else 0, part_size)
+        if (int(first_part) + len(bases)) * int(part_size) * es > _GATHER_MAX_BLOCK_BYTES:
+            raise ValueError("first_part + parts run past the block size limit")
+        if not len(offs):
+            return
+        ret = self.conn.r_rdma_scatter(bases, int(part_size) * es, int(first_part), (keys, offs),
+                                       dev, _stream_of(parts[0][0], stream), es)
         if ret < 0:
             raise Exception(f"Failed to read to infinistore, ret = {ret}: {self.conn.last_error()}")
 

@@ -75,6 +75,10 @@ def chain_hashes(token_ids: Sequence[int], page_tokens: int, salt: str = "") -> 
     return out
 
 
-def page_key(model: str, layer: int, kind: str, tp_rank: int, page_hash: str) -> str:
-    """Key of one page: model / layer / K|V / TP rank / chained prefix hash."""
+ALL_LAYERS = "all"  # layer field of a key whose block holds one page of every layer
+
+
+def page_key(model: str, layer, kind: str, tp_rank: int, page_hash: str) -> str:
+    """Key of one page: model / layer (or ``ALL_LAYERS``) / K|V|KV / TP rank / chained
+    prefix hash."""
     return f"{model}/L{layer}/{kind}/tp{tp_rank}/{page_hash}"

@@ -6,7 +6,7 @@ from typing import List, Optional, Sequence
 import numpy as np
 import torch
 
-from .kv_layout import KVLayout, page_key
+from .kv_layout import ALL_LAYERS, KVLayout, page_key
 
 
 def layer_keys(layout: KVLayout, tp_rank: int, layer: int, kv: int,
@@ -86,23 +86,69 @@ class PagedKVCache:
             n += len(keys)
         return n
 
+    # ------------------------------------------------------------------ all-layer pages
+    # One key per page: the block is the page's K and V of every layer, parts 2l (K) and
+    # 2l + 1 (V), gathered by the write kernel and scattered by the read kernel.
+    def page_keys(self, page_hashes: Sequence[str]) -> List[str]:
+        """Store keys of all-layer pages (``write_pages``)."""
+        return [page_key(self.layout.name, ALL_LAYERS, "KV", self.tp_rank, h) for h in page_hashes]
+
+    def _parts(self, layers: range):
+        return [(self.data, self.page_offset(layer, kv, 0)) for layer in layers for kv in (0, 1)]
+
+    def write_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
+                    stream="current") -> int:
+        """Upload every layer's K and V of each page under one key per page.  Returns the
+        number of blocks written."""
+        self._ensure_registered(conn)
+        layers = range(self.layout.layers)
+        keys = self.page_keys(page_hashes)
+        blocks = conn.allocate_rdma(keys, 2 * len(layers) * self.layout.page_bytes)
+        offs = np.asarray(pages, dtype=np.int64) * self.layout.page_elems
+        conn.rdma_write_cache_gather(self._parts(layers), offs, self.layout.page_elems, blocks,
+                                     stream=stream)
+        return len(keys)
+
+    def read_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
+                   layers: Optional[range] = None, stream="current") -> int:
+        """Fetch pages written by ``write_pages`` into pages ``pages``.  ``layers`` (a range
+        with step 1, default all) reads only those layers' parts of the blocks, so layer l
+        can be fetched while layer l - 1 computes.  Returns the number of blocks read."""
+        self._ensure_registered(conn)
+        layers = range(self.layout.layers) if layers is None else layers
+        if layers.step != 1 or not len(layers) or layers.start < 0 or layers.stop > self.layout.layers:
+            raise ValueError(f"layers must be a non-empty step-1 range within "
+                             f"0..{self.layout.layers}")
+        keys = self.page_keys(page_hashes)
+        offs = np.asarray(pages, dtype=np.int64) * self.layout.page_elems
+        conn.read_cache_scatter(self._parts(layers), (keys, offs), self.layout.page_elems,
+                                first_part=2 * layers.start, stream=stream)
+        return len(keys)
+
     def cached_prefix_pages(self, conn, page_hashes: Sequence[str],
-                            layer: Optional[int] = None) -> int:
+                            layer: Optional[int] = None, all_layer_pages: bool = False) -> int:
         """How many leading pages of this prefix the store already holds (last layer's V
-        pages are written last, so probing them answers for the whole stack)."""
+        pages are written last, so probing them answers for the whole stack).
+        ``all_layer_pages``: the pages were written with ``write_pages`` (one key each)."""
         if not page_hashes:
             return 0
-        keys = self.keys(self.layout.layers - 1 if layer is None else layer, 1, page_hashes)
+        if all_layer_pages:
+            keys = self.page_keys(page_hashes)
+        else:
+            keys = self.keys(self.layout.layers - 1 if layer is None else layer, 1, page_hashes)
         try:
             return conn.get_match_last_index(keys) + 1
         except Exception:
             return 0
 
-    def touch_prefix(self, conn, page_hashes: Sequence[str]) -> int:
+    def touch_prefix(self, conn, page_hashes: Sequence[str], all_layer_pages: bool = False) -> int:
         """Tell an evicting store (``--evict``) that these pages were just used: every layer's
         K and V block of every page becomes most-recently-used.  Needed by clients that read
         through the device index, whose reads the server never sees.  Returns the number of
-        blocks refreshed."""
+        blocks refreshed.  ``all_layer_pages``: the pages were written with ``write_pages``."""
+        if all_layer_pages:
+            keys = self.page_keys(page_hashes)
+            return conn.touch(keys) if keys else 0
         keys: List[str] = []
         for layer in range(self.layout.layers):
             for kv in (0, 1):

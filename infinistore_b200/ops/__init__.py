@@ -61,6 +61,25 @@ def kv_copy(descs: torch.Tensor, nbytes: int, variant: str = "auto", max_ctas: i
                   stage_bytes, ring_bytes, [int(d) for d in fan_deltas] if fan_deltas else [])
 
 
+def kv_gather(descs: torch.Tensor, part_base: Sequence[int], part_bytes: int, write: bool,
+              first_part: int = 0, max_ctas: int = 0, status: Optional[torch.Tensor] = None,
+              align_or: int = 0, stage_bytes: int = 0, ring_bytes: int = 0) -> None:
+    """Gathered blocks (csrc/kernels/kernels.h ``GatherLaunch``): block i is len(part_base)
+    parts of ``part_bytes``, part s at ``part_base[s] + local offset``.  ``descs`` is (n, 2)
+    int64: write {local byte offset, block address}, read {block address or 0 = miss, local
+    byte offset}; a read moves stored parts first_part... .  ``align_or`` must include the
+    local offsets (the part bases are added here): it picks the vector width."""
+    assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
+    bases = [int(b) for b in part_base]
+    for b in bases:
+        align_or |= b
+    with torch.cuda.device(descs.device):
+        K.kv_gather(descs.data_ptr(), descs.shape[0], bases, part_bytes, first_part, write,
+                    max_ctas, _stream(descs.device), 0, 0, 0, 0,
+                    status.data_ptr() if status is not None else 0, align_or, stage_bytes,
+                    ring_bytes)
+
+
 def kv_copy_multicast(descs: torch.Tensor, nbytes: int, dst_deltas: Sequence[int],
                       max_clusters: int = 0, status: Optional[torch.Tensor] = None,
                       stage_bytes: int = 0, ring_bytes: int = 0) -> None:
