@@ -96,6 +96,9 @@ struct ClientStats {
     uint64_t calls = 0;
     uint64_t doorbell_ops = 0;      // single-block operations served by the persistent worker
     uint64_t doorbell_launches = 0;  // (re)launches of the worker
+    // staging allocations (descriptors, records, keys, counters) that had to block the host
+    // until an earlier launch of this connection completed before reusing its bytes
+    uint64_t drains = 0;
 };
 
 class Connection {

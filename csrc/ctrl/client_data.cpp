@@ -27,6 +27,7 @@ Connection::DevCtx* Connection::dev_ctx(int device) {
     DeviceGuard g(device);
     auto ctx = std::make_unique<DevCtx>();
     ctx->device = device;
+    ctx->drains = &stats_.drains;
     void* dp = nullptr;
     if (cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess ||
         cudaHostAlloc(reinterpret_cast<void**>(&ctx->ring_h), kRingBytes,
@@ -188,6 +189,14 @@ kernels::IndexShards Connection::index_shards(DevCtx* ctx, bool* all_local) {
     }
     sh.n = n;
     return sh;
+}
+
+// `auto` for pages in this GPU's own HBM: the ld/st kernels (256 copy threads per CTA, every
+// SM filled, 128 bytes in flight per thread) against the TMA pipeline's one issuing thread per
+// role.  On H100 they move the flagship's 128 KB pages HBM to HBM faster, most of it in the
+// read phase (docs/kernels.md); pools behind NVLink keep the TMA pipeline.
+static int local_auto_variant(int variant, bool local) {
+    return variant == kernels::kCopyAuto && local ? int(kernels::kCopyLdSt256) : variant;
 }
 
 // Move n blocks between the caller's tensor and the pool.  local_off[i] * scale is the
@@ -407,7 +416,7 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
         L.bytes = uint32_t(block_size);
         L.align_or = align_or;
         L.status = ctx->status_d;
-        L.variant = copy_variant_;
+        L.variant = local_auto_variant(copy_variant_, all_local && !L.multicast);
         L.stage_bytes = pipe_stage_;
         L.ring_bytes = pipe_ring_;
         L.max_ctas = max_ctas_ ? max_ctas_ : (all_remote ? 2 * kernels::sm_count() : 0);
@@ -701,10 +710,11 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
         const uint32_t nsegs =
             uint32_t(std::min<size_t>(segs_.size(), kernels::LookupLaunch::kMaxSegs));
         uint64_t seg_base[kernels::LookupLaunch::kMaxSegs] = {0};
-        bool all_remote = true;
+        bool all_remote = true, all_local = true;
         for (uint32_t s = 0; s < nsegs; ++s) {
             seg_base[s] = reinterpret_cast<uint64_t>(seg_dev_ptr(ctx, s));
             all_remote = all_remote && ctx->seg_remote[s];
+            all_local = all_local && !ctx->seg_remote[s];
         }
         // fp8 pages over NVLink: reads one CTA per SM, writes two per SM.  A grid choice not
         // re-measured on H100: bench/configs.py fp8 --max-ctas N compares grid caps.
@@ -769,7 +779,8 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
             // always: a purge (or an eviction) may free a block while a device-path read is
             // copying it; the post-copy tag check turns that into a reported miss
             R.validate = true;
-            R.variant = small_batch ? int(kernels::kCopyLdSt256) : copy_variant_;
+            R.variant = small_batch ? int(kernels::kCopyLdSt256)
+                                    : local_auto_variant(copy_variant_, all_local);
             R.stage_bytes = pipe_stage_;
             R.ring_bytes = pipe_ring_;
             // fp8 pages: the resolver rides in the dequantising TMA pipeline (one launch
@@ -821,7 +832,7 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
                 L.bytes = uint32_t(block_size);
                 L.align_or = align_or;
                 L.status = ctx->status_d;
-                L.variant = copy_variant_;
+                L.variant = local_auto_variant(copy_variant_, all_local);
                 L.stage_bytes = pipe_stage_;
                 L.ring_bytes = pipe_ring_;
                 L.max_ctas = grid_cap;

@@ -14,6 +14,7 @@
 #include "../fabric/segment.h"
 #include "../kernels/kernels.h"
 #include "client.h"
+#include "staging.h"
 
 namespace istore {
 
@@ -69,11 +70,8 @@ struct Connection::DevCtx {
     std::vector<uint8_t*> seg_mc;     // NVLS replica segments: multicast base (writes)
     uint8_t* ring_h = nullptr;  // pinned + mapped: descriptors, publish records, key bytes
     uint8_t* ring_d = nullptr;
-    size_t ring_head = 0;
     uint8_t* scratch = nullptr;  // device memory: descriptors built by the lookup kernel
-    size_t scratch_head = 0;
     uint8_t* zeros = nullptr;    // device memory kept zero between launches (counters/tickets)
-    size_t zeros_head = 0;
     uint32_t* status_h = nullptr;
     uint32_t* status_d = nullptr;
     std::vector<cudaStream_t> busy;  // streams with launches since the last wait_all()
@@ -169,6 +167,7 @@ struct Connection::DevCtx {
             cudaEventDestroy(pool_ev[i]);
         }
         if (user_ev) cudaEventDestroy(user_ev);
+        for (cudaEvent_t ev; staging.take_free(&ev);) cudaEventDestroy(ev);
         if (stream) {
             cudaStreamSynchronize(stream);
             cudaStreamDestroy(stream);
@@ -200,46 +199,46 @@ struct Connection::DevCtx {
         }
         busy.clear();
         dirty = false;
+        staging.retire_all();
     }
     cudaStream_t last = nullptr;  // stream of the most recent launch
+    // Staging reuse (staging.h): one event per launch, recorded behind it on its stream.  A
+    // launch leaves the FIFO at wait_all() or when its bytes come round, so the FIFO holds at
+    // most one lap of launches; their events are recycled.
+    enum { kRing, kScratch, kZeros, kRegions };
+    StagingFifo<cudaEvent_t, kRegions> staging;
+    uint64_t* drains = nullptr;  // ClientStats::drains of the connection
     void mark(cudaStream_t s) {
         dirty = true;
         last = s;
+        cudaEvent_t ev;
+        if (!staging.take_free(&ev)) {
+            DeviceGuard g(device);
+            cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+        }
+        cudaEventRecord(ev, s);
+        staging.push(ev);
         for (cudaStream_t b : busy)
             if (b == s) return;
         busy.push_back(s);
     }
-    // Bump allocators.  When a region wraps, everything launched from it must be done.
-    size_t ring_alloc(size_t bytes) {
-        bytes = align_up(bytes, 64);
-        if (ring_head + bytes > kRingBytes) {
-            wait_all();
-            ring_head = 0;
-        }
-        const size_t at = ring_head;
-        ring_head += bytes;
-        return at;
+    // Bump allocators.  Bytes come round again only after the launches that used them one lap
+    // earlier have completed; launches that are still running on other bytes are not waited for.
+    // zeros: every kernel returns the counters it was given to zero before it completes, so
+    // waiting for those launches is also what makes the reused bytes zero again.
+    size_t alloc(int region, size_t bytes, size_t size) {
+        const uint64_t at = staging.place(region, bytes, size, [this](cudaEvent_t ev) {
+            if (cudaEventQuery(ev) != cudaErrorNotReady) return;  // done, or failed: sync() reports it
+            cudaEventSynchronize(ev);
+            if (drains) ++*drains;
+        });
+        return size_t(at % size);
     }
+    size_t ring_alloc(size_t bytes) { return alloc(kRing, align_up(bytes, 64), kRingBytes); }
     size_t scratch_alloc(size_t bytes) {
-        bytes = align_up(bytes, 256);
-        if (scratch_head + bytes > kScratchBytes) {
-            wait_all();
-            scratch_head = 0;
-        }
-        const size_t at = scratch_head;
-        scratch_head += bytes;
-        return at;
+        return alloc(kScratch, align_up(bytes, 256), kScratchBytes);
     }
-    size_t zeros_alloc(size_t bytes) {
-        bytes = align_up(bytes, 256);
-        if (zeros_head + bytes > kZeroBytes) {
-            wait_all();
-            zeros_head = 0;
-        }
-        const size_t at = zeros_head;
-        zeros_head += bytes;
-        return at;
-    }
+    size_t zeros_alloc(size_t bytes) { return alloc(kZeros, align_up(bytes, 256), kZeroBytes); }
 };
 
 }  // namespace istore

@@ -30,6 +30,7 @@
 #include "core/trace.h"
 #include "ctrl/client.h"
 #include "ctrl/server.h"
+#include "ctrl/staging.h"
 #include "fabric/nvls.h"
 #include "fabric/segment.h"
 #include "kernels/balance.h"
@@ -631,6 +632,7 @@ PYBIND11_MODULE(_infinistore, m) {
             d["ns_streams"] = s.ns_streams;
             d["ns_launch"] = s.ns_launch;
             d["calls"] = s.calls;
+            d["drains"] = s.drains;
             return d;
         });
 
@@ -1246,6 +1248,27 @@ PYBIND11_MODULE(_infinistore, m) {
         .def("used_blocks", &MemoryPool::used_blocks)
         .def("total_blocks", &MemoryPool::total_blocks)
         .def("usage", &MemoryPool::usage);
+    // staging-space reuse of a client device context (ctrl/staging.h), events as integers
+    using Staging = StagingFifo<int64_t, 3>;
+    py::class_<Staging>(t, "StagingFifo")
+        .def(py::init<>())
+        .def("place",
+             [](Staging& f, int region, size_t bytes, size_t size) {
+                 if (region < 0 || region >= 3 || size == 0 || bytes > size)
+                     throw py::value_error("needs region in [0, 3) and bytes <= size");
+                 py::list waited;
+                 const uint64_t at = f.place(region, bytes, size, [&](int64_t ev) { waited.append(ev); });
+                 return py::make_tuple(at, waited);
+             })
+        .def("push", &Staging::push)
+        .def("retire_all", &Staging::retire_all)
+        .def("take_free",
+             [](Staging& f) -> py::object {
+                 int64_t ev;
+                 if (!f.take_free(&ev)) return py::none();
+                 return py::int_(ev);
+             })
+        .def("in_flight", &Staging::in_flight);
     py::class_<MM>(t, "MM")
         .def(py::init<>())
         .def("add_pool", &MM::add_pool)
