@@ -148,6 +148,21 @@ struct Connection::Task {
     bool commit = false;
     std::vector<uint64_t> commits;  // addresses written by exactly this task's launches
     std::function<void(int)> done_cb;
+
+    // Complete with the launches of `res`: an event recorded behind them on their stream,
+    // or, when there is no event, a wait for the whole stream now.
+    void wait_for(const MoveResult& res) {
+        DeviceGuard g(res.device);
+        if (cudaEventCreateWithFlags(&event, cudaEventDisableTiming) == cudaSuccess &&
+            cudaEventRecord(event, static_cast<cudaStream_t>(res.stream)) == cudaSuccess) {
+            device = res.device;
+            return;
+        }
+        if (event) cudaEventDestroy(event);
+        event = nullptr;
+        (void)cudaGetLastError();
+        if (cudaStreamSynchronize(static_cast<cudaStream_t>(res.stream)) != cudaSuccess) status = -1;
+    }
 };
 
 Connection::Connection() {}
@@ -816,19 +831,7 @@ int Connection::w_rdma_async(const std::vector<uint64_t>& offsets, int block_siz
                          device, stream, &res);
     t.status = r;
     t.done_cb = std::move(cb);
-    if (res.launched && res.device >= 0) {
-        DeviceGuard g(res.device);
-        if (cudaEventCreateWithFlags(&t.event, cudaEventDisableTiming) == cudaSuccess &&
-            cudaEventRecord(t.event, static_cast<cudaStream_t>(res.stream)) == cudaSuccess) {
-            t.device = res.device;
-        } else {
-            // no event: fall back to waiting for the whole stream before the commit
-            if (t.event) cudaEventDestroy(t.event);
-            t.event = nullptr;
-            (void)cudaGetLastError();
-            if (cudaStreamSynchronize(static_cast<cudaStream_t>(res.stream)) != cudaSuccess) t.status = -1;
-        }
-    }
+    if (res.launched && res.device >= 0) t.wait_for(res);  // the commit waits for it
     post(std::move(t));
     return r;
 }
@@ -842,18 +845,7 @@ int Connection::r_rdma_async(const std::vector<KeyOffset>& blocks, int block_siz
     t.kind = Task::kWaitEvent;
     t.status = r;
     t.done_cb = std::move(cb);
-    if (r == 0 && res.launched && res.device >= 0) {
-        DeviceGuard g(res.device);
-        if (cudaEventCreateWithFlags(&t.event, cudaEventDisableTiming) == cudaSuccess &&
-            cudaEventRecord(t.event, static_cast<cudaStream_t>(res.stream)) == cudaSuccess) {
-            t.device = res.device;
-        } else {
-            if (t.event) cudaEventDestroy(t.event);
-            t.event = nullptr;
-            (void)cudaGetLastError();
-            if (cudaStreamSynchronize(static_cast<cudaStream_t>(res.stream)) != cudaSuccess) t.status = -1;
-        }
-    }
+    if (r == 0 && res.launched && res.device >= 0) t.wait_for(res);
     post(std::move(t));
     return r;
 }

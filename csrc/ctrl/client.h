@@ -35,9 +35,12 @@ namespace istore {
 namespace kernels {
 struct CopyDesc;
 struct IndexShards;
+struct LookupLaunch;
+struct GatherLaunch;
 }
 using kernels_CopyDesc = kernels::CopyDesc;
 using kernels_IndexShards = kernels::IndexShards;
+struct KeyBatch;
 
 // Non-owning: the key bytes must stay valid for the duration of the call.
 struct KeyOffset {
@@ -218,6 +221,7 @@ class Connection {
    private:
     struct DevCtx;
     struct Task;
+    struct LaunchScope;
 
     // control plane
     int transact(char op, const void* body, size_t len, int32_t* code,
@@ -253,9 +257,22 @@ class Connection {
     int discard_blocks(const uint64_t* addrs, size_t count);
     uint8_t* seg_dev_ptr(DevCtx* ctx, uint32_t seg);
     kernels_IndexShards index_shards(DevCtx* ctx, bool* all_local);
+    kernels::GatherLaunch gather_launch(const GatherSpec& g, uint32_t n, uint64_t align_or,
+                                        uint32_t* status, int max_ctas);
+    template <typename Launch>
+    bool set_index(DevCtx* ctx, Launch& L, bool segs = true);
     const kernels_CopyDesc* resolve_descs(DevCtx* ctx, const std::vector<KeyOffset>& blocks,
-                                          size_t base, size_t n, int block_size, uint64_t dst_base,
-                                          const std::vector<RemoteBlock>* rb, void* stream);
+                                          size_t base, const KeyBatch& b, const PackedKeys* packed,
+                                          uint32_t need_bytes, uint64_t dst_base,
+                                          const std::vector<RemoteBlock>* rb, void* stream,
+                                          kernels::LookupLaunch* checked = nullptr);
+    template <typename Launch>
+    int read_resolved(const std::vector<KeyOffset>& blocks, int block_size, int device,
+                      uint64_t stream, uint64_t dst_base, const char* what, Launch&& launch);
+    int read_blocks(char op, const std::vector<KeyOffset>& blocks, int block_size,
+                    uint64_t base_ptr, int device, uint64_t stream, int fp8_elems = 0,
+                    MoveResult* res = nullptr, const PackedKeys* packed = nullptr,
+                    const GatherSpec* gather = nullptr);
     int read_via_device_index(const std::vector<KeyOffset>& blocks, int block_size,
                               uint64_t base_ptr, int device, uint64_t stream, int fp8_elems = 0,
                               MoveResult* res = nullptr, const PackedKeys* packed = nullptr,

@@ -14,6 +14,7 @@
 #include "../kernels/kernels.h"
 #include "../wire/messages.h"
 #include "client_dev.h"
+#include "read_plan.h"
 
 namespace istore {
 
@@ -191,12 +192,99 @@ kernels::IndexShards Connection::index_shards(DevCtx* ctx, bool* all_local) {
     return sh;
 }
 
-// `auto` for pages in this GPU's own HBM: the ld/st kernels (256 copy threads per CTA, every
-// SM filled, 128 bytes in flight per thread) against the TMA pipeline's one issuing thread per
-// role.  On H100 they move the flagship's 128 KB pages HBM to HBM faster, most of it in the
-// read phase (docs/kernels.md); pools behind NVLink keep the TMA pipeline.
-static int local_auto_variant(int variant, bool local) {
-    return variant == kernels::kCopyAuto && local ? int(kernels::kCopyLdSt256) : variant;
+// Shard 0 of the device index (segment 0's table) and the further shards as seen from ctx's
+// device, and with `segs` the segment bases the lookup kernels turn hits into addresses with.
+// false when segment 0 carries no index this device can reach.
+template <typename Launch>
+bool Connection::set_index(DevCtx* ctx, Launch& L, bool segs) {
+    auto m0 = mapping(0, ctx->device);
+    if (!m0 || !m0->dev_ptr || !segs_[0].index_slots) return false;
+    if (segs) {
+        L.nsegs = uint32_t(std::min<size_t>(segs_.size(), Launch::kMaxSegs));
+        for (uint32_t s = 0; s < L.nsegs; ++s)
+            L.seg_base[s] = reinterpret_cast<uint64_t>(seg_dev_ptr(ctx, s));
+    }
+    L.table = reinterpret_cast<kernels::IndexBucket*>(m0->dev_ptr + segs_[0].index_off);
+    L.table_mask = kernels::index_bucket_mask(segs_[0].index_slots);
+    L.shards = index_shards(ctx, nullptr);
+    return true;
+}
+
+// The steps around the launches of one data-plane call.  The constructor makes the device
+// context current for the scope; the doorbell fast paths go between it and begin(), which
+// quiesces the doorbell worker and picks the launch stream.  launched() follows each batch.
+struct Connection::LaunchScope {
+    Connection& c;
+    DevCtx* ctx;
+    DeviceGuard guard;
+    MoveResult* res;
+    cudaStream_t stream = nullptr;
+
+    LaunchScope(Connection& conn, int device, MoveResult* r)
+        : c(conn), ctx(conn.dev_ctx(device)), guard(ctx ? device : -1), res(r) {}
+    int begin(uint64_t stream_in, bool write) {
+        if (c.doorbell_quiesce(ctx) != 0) return -1;
+        const uint64_t t_pick0 = now_ns();
+        stream = ctx->pick(reinterpret_cast<cudaStream_t>(stream_in), write, c.streams_);
+        c.stats_.ns_streams += now_ns() - t_pick0;
+        c.stats_.calls++;
+        if (res) {
+            res->stream = stream;
+            res->device = ctx->device;
+        }
+        return 0;
+    }
+    // -1 when the batch's launches failed (reported as `what` and the CUDA error); otherwise
+    // sync() waits for them, and they are counted.
+    int launched(cudaError_t e, const char* what, uint32_t launches, bool write, uint64_t bytes) {
+        if (e != cudaSuccess) {
+            c.fail(std::string(what) + cudaGetErrorString(e));
+            return -1;
+        }
+        ctx->mark(stream);
+        if (res) res->launched = true;
+        c.stats_.kernel_launches += launches;
+        (write ? c.stats_.bytes_written : c.stats_.bytes_read) += bytes;
+        return 0;
+    }
+};
+
+// The parts of a gathered launch of n blocks whose local offsets OR to `align_or` (the part
+// bases' alignment counts with theirs); descriptors and commit fields are the caller's.
+kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n, uint64_t align_or,
+                                                uint32_t* status, int max_ctas) {
+    kernels::GatherLaunch G;
+    G.n = n;
+    G.part_base = g.part_base;
+    G.nparts = g.nparts;
+    G.part_bytes = g.part_bytes;
+    G.first_part = g.first_part;
+    G.align_or = align_or;
+    for (uint32_t s = 0; s < g.nparts; ++s) G.align_or |= g.part_base[s];
+    G.status = status;
+    G.max_ctas = max_ctas;
+    G.stage_bytes = pipe_stage_;
+    G.ring_bytes = pipe_ring_;
+    return G;
+}
+
+// The blocks of blocks[base, ...) that the next launch stages (staging.h: key_batch) within
+// half the ring, so that a launch's placements never come round to each other.  *packed is
+// kept only when it covers the call and the call fits in one launch.  n == 0: one key is
+// longer than the ring.
+static KeyBatch next_key_batch(const std::vector<KeyOffset>& blocks, size_t base,
+                               size_t max_blocks, const PackedKeys** packed = nullptr) {
+    const size_t left = blocks.size() - base;
+    const PackedKeys* p = packed ? *packed : nullptr;
+    if (p && base == 0 && p->n == left && left <= max_blocks &&
+        p->nbytes + 16 * left <= kRingBytes / 2)
+        return KeyBatch{left, p->nbytes};
+    if (packed) *packed = nullptr;
+    const KeyBatch b = key_batch(left, max_blocks, kRingBytes / 2,
+                                 [&](size_t i) { return blocks[base + i].key.size(); });
+    // a lone key must not reach its own offsets after a wrap: ring_alloc rounds each of the
+    // four placements up to 64 bytes: at most 56 + 60 + 60 + 56 < 256 bytes beyond key_bytes + 16n
+    return b.key_bytes + 16 * b.n + 256 > kRingBytes ? KeyBatch{} : b;
 }
 
 // Move n blocks between the caller's tensor and the pool.  local_off[i] * scale is the
@@ -288,9 +376,9 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
     }
 
     // --- kernel path on `kd`
-    DevCtx* ctx = dev_ctx(kd);
+    LaunchScope scope(*this, kd, res);
+    DevCtx* ctx = scope.ctx;
     if (!ctx) return -1;
-    DeviceGuard g(kd);
     if (cfg_.doorbell && write && n == 1 && device >= 0 && !fp8_elems && !res && !gather &&
         !is_fake_block(blocks[0])) {
         // latency mode: one block, handed to the persistent worker (no launch, no event)
@@ -313,15 +401,7 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
             return 0;
         }
     }
-    if (doorbell_quiesce(ctx) != 0) return -1;
-    const uint64_t t_pick0 = now_ns();
-    cudaStream_t stream = ctx->pick(reinterpret_cast<cudaStream_t>(stream_in), write, streams_);
-    stats_.ns_streams += now_ns() - t_pick0;
-    stats_.calls++;
-    if (res) {
-        res->stream = stream;
-        res->device = kd;
-    }
+    if (scope.begin(stream_in, write) != 0) return -1;
 
     // the device index lives in segment 0
     kernels::IndexBucket* table = nullptr;
@@ -333,14 +413,8 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
         }
     }
 
-    // gathered blocks: at most 2^30 work items per launch (a chunk is >= 16 KB or a whole part)
-    size_t max_batch = kMaxBatch;
-    uint64_t gather_align = 0;
-    if (gather) {
-        const uint64_t items = uint64_t(gather->nparts) * ((gather->part_bytes + 16383u) / 16384u);
-        max_batch = std::max<size_t>(1, std::min<uint64_t>(kMaxBatch, (1ull << 30) / items));
-        for (uint32_t s = 0; s < gather->nparts; ++s) gather_align |= gather->part_base[s];
-    }
+    const size_t max_batch =
+        gather ? gather_max_blocks(kMaxBatch, gather->nparts, gather->part_bytes) : kMaxBatch;
     size_t i = 0;
     while (i < n) {
         const uint64_t t_build0 = now_ns();
@@ -439,26 +513,16 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
         stats_.ns_build += t_launch0 - t_build0;
         cudaError_t e;
         if (gather) {
-            kernels::GatherLaunch G;
+            kernels::GatherLaunch G = gather_launch(*gather, m, align_or, L.status, L.max_ctas);
             G.descs = L.descs;
-            G.n = m;
             G.write = write;
-            G.part_base = gather->part_base;
-            G.nparts = gather->nparts;
-            G.part_bytes = gather->part_bytes;
-            G.first_part = gather->first_part;
-            G.align_or = align_or | gather_align;
             G.recs = L.recs;
             G.table = L.table;
             G.table_mask = L.table_mask;
             G.done = L.done;
-            G.status = L.status;
-            G.max_ctas = L.max_ctas;
             G.all_local = L.all_local;
             G.shards = L.shards;
-            G.stage_bytes = pipe_stage_;
-            G.ring_bytes = pipe_ring_;
-            e = kernels::launch_kv_gather(G, stream);
+            e = kernels::launch_kv_gather(G, scope.stream);
         } else if (fp8_elems) {
             kernels::Fp8Launch F;
             F.descs = L.descs;
@@ -473,22 +537,20 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
             F.max_ctas = L.max_ctas;
             F.all_local = all_local;
             F.aligned16 = (align_or & 15) == 0;
-            // TMA-pipelined flavour over NVLink, per-thread flavour on local HBM
+            // TMA-pipelined flavour over NVLink, per-thread flavour on local HBM.  Intentional:
+            // the lookup-then-fp8 read (read_plan.h) uses all_remote ? 0 : 1 instead, and the
+            // two differ for a pool that mixes local and remote segments.
             F.variant = all_local ? 1 : 0;
-            e = write ? kernels::launch_kv_write_fp8(F, stream) : kernels::launch_kv_read_fp8(F, stream);
+            e = write ? kernels::launch_kv_write_fp8(F, scope.stream)
+                      : kernels::launch_kv_read_fp8(F, scope.stream);
         } else {
-            e = kernels::launch_kv_copy(L, stream);
+            e = kernels::launch_kv_copy(L, scope.stream);
         }
         stats_.ns_launch += now_ns() - t_launch0;
-        if (e != cudaSuccess) {
-            fail(std::string("page mover launch failed: ") + cudaGetErrorString(e));
+        if (scope.launched(e, "page mover launch failed: ", 1, write,
+                           uint64_t(m) * uint64_t(block_size)) != 0)
             return -1;
-        }
-        ctx->mark(stream);
-        if (res) res->launched = true;
         sink.insert(sink.end(), batch_commits.begin(), batch_commits.end());
-        stats_.kernel_launches++;
-        (write ? stats_.bytes_written : stats_.bytes_read) += uint64_t(m) * uint64_t(block_size);
     }
     return 0;
 }
@@ -523,30 +585,36 @@ int Connection::r_rdma_fp8(const std::vector<KeyOffset>& blocks, int elems, uint
         fail("r_rdma_fp8: needs a CUDA tensor and pages of a multiple of 128 elements");
         return -1;
     }
-    const int bytes = int(kernels::fp8_block_bytes(uint32_t(elems), 128));
-    if (device_lookup_ && server_hbm_ && device_index_usable())
-        return read_via_device_index(blocks, bytes, base_ptr, device, stream, elems);
-    std::vector<RemoteBlock> rb;
-    const int r = lookup_blocks(kOpReadLookup, blocks, bytes, rb);
-    if (r != 0) return r;
-    std::vector<uint64_t> offs(blocks.size());
-    for (size_t i = 0; i < blocks.size(); ++i) offs[i] = blocks[i].offset;
-    return move_blocks(false, offs.data(), 1, rb.data(), rb.size(), bytes, base_ptr, device,
-                       stream, elems);
+    return read_blocks(kOpReadLookup, blocks, int(kernels::fp8_block_bytes(uint32_t(elems), 128)),
+                       base_ptr, device, stream, elems);
 }
 
 int Connection::r_rdma(const std::vector<KeyOffset>& blocks, int block_size, uint64_t base_ptr,
                        int device, uint64_t stream, MoveResult* res, const PackedKeys* packed) {
     if (blocks.empty()) return 0;
+    return read_blocks(kOpReadLookup, blocks, block_size, base_ptr, device, stream, 0, res, packed);
+}
+
+// Bytes a stored block must hold to serve the read: every part asked for.
+static uint32_t need_bytes_of(int block_size, const Connection::GatherSpec* g) {
+    return g ? (g->first_part + g->nparts) * g->part_bytes : uint32_t(block_size);
+}
+
+// A read through the device index when this connection can use it from `device`; otherwise
+// the server resolves the keys (`op`) and move_blocks copies.
+int Connection::read_blocks(char op, const std::vector<KeyOffset>& blocks, int block_size,
+                            uint64_t base_ptr, int device, uint64_t stream, int fp8_elems,
+                            MoveResult* res, const PackedKeys* packed, const GatherSpec* gather) {
     if (device_lookup_ && server_hbm_ && device >= 0 && device_index_usable())
-        return read_via_device_index(blocks, block_size, base_ptr, device, stream, 0, res, packed);
+        return read_via_device_index(blocks, block_size, base_ptr, device, stream, fp8_elems, res,
+                                     packed, gather);
     std::vector<RemoteBlock> rb;
-    const int r = lookup_blocks(kOpReadLookup, blocks, block_size, rb);
+    const int r = lookup_blocks(op, blocks, int(need_bytes_of(block_size, gather)), rb);
     if (r != 0) return r;
     std::vector<uint64_t> offs(blocks.size());
     for (size_t i = 0; i < blocks.size(); ++i) offs[i] = blocks[i].offset;
     return move_blocks(false, offs.data(), 1, rb.data(), rb.size(), block_size, base_ptr, device,
-                       stream, 0, res);
+                       stream, fp8_elems, res, gather);
 }
 
 static bool gather_spec_ok(const Connection::GatherSpec& g) {
@@ -575,30 +643,19 @@ int Connection::r_rdma_scatter(const GatherSpec& g, const std::vector<KeyOffset>
         fail("r_rdma_scatter: bad parts list");
         return -1;
     }
-    const int block_size = int(g.nparts * g.part_bytes);
-    if (device_lookup_ && server_hbm_ && device >= 0 && device_index_usable())
-        return read_via_device_index(blocks, block_size, 0, device, stream, 0, nullptr, nullptr, &g);
-    std::vector<RemoteBlock> rb;
-    // the stored block must hold every part asked for
-    const int r = lookup_blocks(kOpReadLookup, blocks, int((g.first_part + g.nparts) * g.part_bytes),
-                                rb);
-    if (r != 0) return r;
-    std::vector<uint64_t> offs(blocks.size());
-    for (size_t i = 0; i < blocks.size(); ++i) offs[i] = blocks[i].offset;
-    return move_blocks(false, offs.data(), 1, rb.data(), rb.size(), block_size, 0, device, stream,
-                       0, nullptr, &g);
+    return read_blocks(kOpReadLookup, blocks, int(g.nparts * g.part_bytes), 0, device, stream, 0,
+                       nullptr, nullptr, &g);
 }
 
 int Connection::rw_local(char op, const std::vector<KeyOffset>& blocks, int block_size,
                          uint64_t base_ptr, int device, uint64_t stream) {
     if (blocks.empty()) return 0;
     if (op != kOpLocalRead && op != kOpLocalWrite) return -1;
-    if (op == kOpLocalRead && device_lookup_ && server_hbm_ && device >= 0 && device_index_usable())
-        return read_via_device_index(blocks, block_size, base_ptr, device, stream);
+    if (op == kOpLocalRead) return read_blocks(op, blocks, block_size, base_ptr, device, stream);
     std::vector<RemoteBlock> rb;
     const int r = lookup_blocks(op, blocks, block_size, rb);
     if (r != 0) return r;
-    if (op == kOpLocalWrite && server_hbm_) {
+    if (server_hbm_) {
         std::lock_guard<std::mutex> lk(mu_);
         for (size_t i = 0; i < blocks.size(); ++i) {
             if (is_fake_block(rb[i])) continue;
@@ -609,25 +666,8 @@ int Connection::rw_local(char op, const std::vector<KeyOffset>& blocks, int bloc
     }
     std::vector<uint64_t> offs(blocks.size());
     for (size_t i = 0; i < blocks.size(); ++i) offs[i] = blocks[i].offset;
-    return move_blocks(op == kOpLocalWrite, offs.data(), 1, rb.data(), rb.size(), block_size,
-                       base_ptr, device, stream);
-}
-
-// Pack keys into the pinned ring so that the lookup kernel can hash them: each key starts
-// on an 8-byte boundary and is zero padded to a multiple of 8.
-static size_t pack_keys(const std::string_view* keys, size_t n, uint8_t* bytes, uint32_t* off,
-                        uint32_t* len) {
-    size_t at = 0;
-    for (size_t i = 0; i < n; ++i) {
-        const std::string_view k = keys[i];
-        off[i] = uint32_t(at);
-        len[i] = uint32_t(k.size());
-        const size_t padded = align_up(k.size() ? k.size() : 1, 8);
-        std::memcpy(bytes + at, k.data(), k.size());
-        std::memset(bytes + at + k.size(), 0, padded - k.size());
-        at += padded;
-    }
-    return at;
+    return move_blocks(true, offs.data(), 1, rb.data(), rb.size(), block_size, base_ptr, device,
+                       stream);
 }
 
 int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int block_size,
@@ -636,23 +676,14 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
                                       const GatherSpec* gather) {
     NvtxRange nvtx("istore.read_via_device_index");
     std::lock_guard<std::mutex> lk(mu_);
-    DevCtx* ctx = dev_ctx(device);
+    LaunchScope scope(*this, device, res);
+    DevCtx* ctx = scope.ctx;
     if (!ctx) return -1;
     auto m0 = mapping(0, device);
     if (!m0 || !m0->dev_ptr || !segs_[0].index_slots) {
         fail("the server exposes no device index");
         return -1;
     }
-    // gathered blocks (scattered into parts): kv_pipe_scatter_read, or lookup + gather +
-    // validate for batches with fewer blocks than CTAs or unaligned parts (see below)
-    size_t step = kMaxBatch;
-    uint64_t gather_align = 0;
-    if (gather) {
-        const uint64_t items = uint64_t(gather->nparts) * ((gather->part_bytes + 16383u) / 16384u);
-        step = std::max<size_t>(1, std::min<uint64_t>(kMaxBatch, (1ull << 30) / items));
-        for (uint32_t s = 0; s < gather->nparts; ++s) gather_align |= gather->part_base[s];
-    }
-    DeviceGuard g(device);
     if (cfg_.doorbell && blocks.size() == 1 && !fp8_elems && !res && !gather &&
         doorbell_ready(ctx, stream_in, size_t(block_size))) {
         // latency mode: the key is hashed here, the worker probes, copies and re-checks
@@ -665,181 +696,102 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
         stats_.bytes_read += uint64_t(block_size);
         return 0;
     }
-    if (doorbell_quiesce(ctx) != 0) return -1;
-    const uint64_t t_pick0 = now_ns();
-    cudaStream_t stream = ctx->pick(reinterpret_cast<cudaStream_t>(stream_in), false, streams_);
-    stats_.ns_streams += now_ns() - t_pick0;
-    stats_.calls++;
-    if (res) {
-        res->stream = stream;
-        res->device = device;
-    }
-    for (size_t base = 0; base < blocks.size(); base += step) {
+    if (scope.begin(stream_in, false) != 0) return -1;
+    const size_t max_batch =
+        gather ? gather_max_blocks(kMaxBatch, gather->nparts, gather->part_bytes) : kMaxBatch;
+    KeyBatch b;
+    for (size_t base = 0; base < blocks.size(); base += b.n) {
         const uint64_t t_build0 = now_ns();
-        const size_t n = std::min(step, blocks.size() - base);
-        // keys into the pinned ring, in the layout the kernels hash them from; three memcpys
-        // when the caller holds them like that already (one batch), a pass over the keys else
-        const bool prepacked = packed && base == 0 && packed->n == blocks.size() && n == blocks.size();
-        size_t key_bytes = 0;
-        std::vector<std::string_view> kp;
-        if (prepacked) {
-            key_bytes = packed->nbytes;
-        } else {
-            kp.resize(n);
-            for (size_t i = 0; i < n; ++i) {
-                kp[i] = blocks[base + i].key;
-                key_bytes += align_up(std::max<size_t>(kp[i].size(), 1), 8);
-            }
+        b = next_key_batch(blocks, base, max_batch, &packed);
+        if (!b.n) {
+            fail("read: a key does not fit the staging ring");
+            return -1;
         }
-        const size_t at_bytes = ctx->ring_alloc(key_bytes);
-        const size_t at_off = ctx->ring_alloc(n * 4);
-        const size_t at_len = ctx->ring_alloc(n * 4);
-        const size_t at_dst = ctx->ring_alloc(n * 8);
-        if (prepacked) {
-            std::memcpy(ctx->ring_h + at_bytes, packed->bytes, key_bytes);
-            std::memcpy(ctx->ring_h + at_off, packed->off, n * 4);
-            std::memcpy(ctx->ring_h + at_len, packed->len, n * 4);
-        } else {
-            pack_keys(kp.data(), n, ctx->ring_h + at_bytes,
-                      reinterpret_cast<uint32_t*>(ctx->ring_h + at_off),
-                      reinterpret_cast<uint32_t*>(ctx->ring_h + at_len));
+        const size_t n = b.n;
+        kernels::ReadFusedLaunch R;
+        set_index(ctx, R);
+        DeviceReadIn in{.n = n, .block_bytes = uint32_t(block_size),
+                        .fp8_elems = uint32_t(fp8_elems), .gather = gather != nullptr,
+                        .copy_variant = copy_variant_, .all_local = true, .all_remote = true,
+                        .max_ctas = max_ctas_, .sm_count = kernels::sm_count()};
+        // over every known segment, not only the ones this batch touches: intentional
+        for (uint32_t s = 0; s < R.nsegs; ++s) {
+            in.all_remote = in.all_remote && ctx->seg_remote[s];
+            in.all_local = in.all_local && !ctx->seg_remote[s];
         }
-        auto* dst = reinterpret_cast<uint64_t*>(ctx->ring_h + at_dst);
-        for (size_t i = 0; i < n; ++i) dst[i] = blocks[base + i].offset;
-
-        const uint32_t nsegs =
-            uint32_t(std::min<size_t>(segs_.size(), kernels::LookupLaunch::kMaxSegs));
-        uint64_t seg_base[kernels::LookupLaunch::kMaxSegs] = {0};
-        bool all_remote = true, all_local = true;
-        for (uint32_t s = 0; s < nsegs; ++s) {
-            seg_base[s] = reinterpret_cast<uint64_t>(seg_dev_ptr(ctx, s));
-            all_remote = all_remote && ctx->seg_remote[s];
-            all_local = all_local && !ctx->seg_remote[s];
-        }
-        // fp8 pages over NVLink: reads one CTA per SM, writes two per SM.  A grid choice not
-        // re-measured on H100: bench/configs.py fp8 --max-ctas N compares grid caps.
-        const int grid_cap = max_ctas_ ? max_ctas_
-                             : all_remote ? (fp8_elems ? 1 : 2) * kernels::sm_count()
-                                          : 0;
         uint64_t align_or = base_ptr;
         for (size_t i = 0; i < n; ++i) align_or |= blocks[base + i].offset;
-        const uint64_t t_launch0 = now_ns();
-        stats_.ns_build += t_launch0 - t_build0;
-        cudaError_t e;
-        // The fused kernels resolve a key in every CTA that moves a piece of its block, reading
-        // the key bytes from the pinned ring each time: right for a batch of blocks (items are
-        // whole blocks, or chunks when that balances the grid better - kernels/balance.h),
-        // wasteful when a few LARGE blocks are split over many CTAs - then resolve each key
-        // once with the lookup kernel and feed the descriptors to kv_copy.
-        // A handful of blocks (<= 4 MB in all): latency matters, not bandwidth.  One launch of
-        // the ld/st flavour, which splits a block into 32 KB chunks over CTAs (each resolves its
-        // block's key itself - a few redundant probes) and re-checks the entries in the same
-        // kernel: lookup + copy + validate would be three launches.
-        const bool small_batch = n * size_t(block_size) <= (4u << 20);
-        const bool whole_blocks = !small_batch && uint32_t(block_size) <= (1u << 20) && n >= 32;
-        kernels::ReadFusedLaunch R;
+        // the fused kernels' support checks see the batch as it would be launched
+        R.n = uint32_t(n);
         R.align_or = align_or;
-        const bool fp8_fused = fp8_elems && kernels::fp8_read_fused_supported(R, uint32_t(fp8_elems));
-        // gathered blocks: one launch (resolver warp + gather pipeline, a CTA per block) once
-        // every CTA has a block of its own; fewer blocks: lookup + gather + validate below
+        R.max_ctas = device_read_grid_cap(max_ctas_, in.all_remote, fp8_elems != 0, in.sm_count);
         kernels::GatherLaunch G;
-        bool gather_fused = false;
-        if (gather) {
-            G.n = uint32_t(n);
-            G.part_base = gather->part_base;
-            G.nparts = gather->nparts;
-            G.part_bytes = gather->part_bytes;
-            G.first_part = gather->first_part;
-            G.align_or = align_or | gather_align;
-            G.status = ctx->status_d;
-            G.max_ctas = grid_cap;
-            G.stage_bytes = pipe_stage_;
-            G.ring_bytes = pipe_ring_;
-            R.n = uint32_t(n);
-            R.max_ctas = grid_cap;
-            gather_fused = kernels::scatter_read_fused_supported(R, G);
-        }
-        if (gather_fused || (!gather && (fp8_fused || (!fp8_elems && (whole_blocks || small_batch))))) {
+        if (gather) G = gather_launch(*gather, uint32_t(n), align_or, ctx->status_d, R.max_ctas);
+        in.fp8_fused_ok = fp8_elems && kernels::fp8_read_fused_supported(R, uint32_t(fp8_elems));
+        in.scatter_fused_ok = gather && kernels::scatter_read_fused_supported(R, G);
+        const DeviceReadPlan plan = plan_device_read(in);
+        uint64_t t_launch0 = now_ns();
+        cudaError_t e = cudaSuccess;
+        if (plan.fused()) {
             // one kernel: hash + probe + move
-            R.key_bytes = ctx->ring_d + at_bytes;
-            R.key_off = reinterpret_cast<const uint32_t*>(ctx->ring_d + at_off);
-            R.key_len = reinterpret_cast<const uint32_t*>(ctx->ring_d + at_len);
-            R.dst_off = reinterpret_cast<const uint64_t*>(ctx->ring_d + at_dst);
+            const StagedKeys keys = ctx->stage_keys(blocks, base, b, packed);
+            R.key_bytes = keys.bytes;
+            R.key_off = keys.off;
+            R.key_len = keys.len;
+            R.dst_off = keys.dst;
             R.dst_base = base_ptr;
-            R.n = uint32_t(n);
             R.bytes = uint32_t(block_size);
-            R.align_or = copy_variant_ == kernels::kCopyLdSt ? (align_or | 16) : align_or;
-            R.table = reinterpret_cast<const kernels::IndexBucket*>(m0->dev_ptr + segs_[0].index_off);
-            R.table_mask = kernels::index_bucket_mask(segs_[0].index_slots);
-            R.shards = index_shards(ctx, nullptr);
-            R.nsegs = nsegs;
-            for (uint32_t s = 0; s < nsegs; ++s) R.seg_base[s] = seg_base[s];
+            if (plan.ldst_align) R.align_or |= 16;
             R.status = ctx->status_d;
-            R.max_ctas = grid_cap;
             // always: a purge (or an eviction) may free a block while a device-path read is
             // copying it; the post-copy tag check turns that into a reported miss
             R.validate = true;
-            R.variant = small_batch ? int(kernels::kCopyLdSt256)
-                                    : local_auto_variant(copy_variant_, all_local);
+            R.variant = plan.variant;
             R.stage_bytes = pipe_stage_;
             R.ring_bytes = pipe_ring_;
-            // fp8 pages: the resolver rides in the dequantising TMA pipeline (one launch
-            // instead of lookup + read + validate: 32 calls of 512 pages were launch-bound)
-            e = gather_fused ? kernels::launch_kv_pipe_scatter_read(R, G, stream)
-                : fp8_fused  ? kernels::launch_kv_fp8_read_fused(R, uint32_t(fp8_elems), stream)
-                             : kernels::launch_kv_read_fused(R, stream);
-            stats_.kernel_launches += 1;
+            t_launch0 = now_ns();
+            e = plan.path == ReadPath::kFusedScatter
+                    ? kernels::launch_kv_pipe_scatter_read(R, G, scope.stream)
+                : plan.path == ReadPath::kFusedFp8
+                    ? kernels::launch_kv_fp8_read_fused(R, uint32_t(fp8_elems), scope.stream)
+                    : kernels::launch_kv_read_fused(R, scope.stream);
         } else {
-            kernels::LookupLaunch Q;
-            Q.key_bytes = ctx->ring_d + at_bytes;
-            Q.key_off = reinterpret_cast<const uint32_t*>(ctx->ring_d + at_off);
-            Q.key_len = reinterpret_cast<const uint32_t*>(ctx->ring_d + at_len);
-            Q.n = uint32_t(n);
-            Q.table = reinterpret_cast<const kernels::IndexBucket*>(m0->dev_ptr + segs_[0].index_off);
-            Q.table_mask = kernels::index_bucket_mask(segs_[0].index_slots);
-            Q.shards = index_shards(ctx, nullptr);
-            Q.nsegs = nsegs;
-            for (uint32_t s = 0; s < nsegs; ++s) Q.seg_base[s] = seg_base[s];
-            auto* out = reinterpret_cast<kernels::CopyDesc*>(
-                ctx->scratch + ctx->scratch_alloc(n * sizeof(kernels::CopyDesc)));
-            Q.out_descs = out;
-            Q.dst_off = reinterpret_cast<const uint64_t*>(ctx->ring_d + at_dst);
-            Q.dst_base = base_ptr;
-            Q.need_bytes = gather ? (gather->first_part + gather->nparts) * gather->part_bytes
-                                  : uint32_t(block_size);
-            Q.status = ctx->status_d;
             // optimistic read: the entries are re-checked after the copy (purge / eviction)
-            Q.found_at = reinterpret_cast<kernels::LookupLaunch::FoundAt*>(
-                    ctx->scratch + ctx->scratch_alloc(n * sizeof(kernels::LookupLaunch::FoundAt)));
-            e = kernels::launch_index_lookup(Q, stream);
-            if (e == cudaSuccess && gather) {
-                G.descs = out;  // {pool address or 0, local byte offset} (dst_base 0)
-                e = kernels::launch_kv_gather(G, stream);
-            } else if (e == cudaSuccess && fp8_elems) {
+            kernels::LookupLaunch Q;
+            const kernels::CopyDesc* descs =
+                resolve_descs(ctx, blocks, base, b, packed, need_bytes_of(block_size, gather),
+                              base_ptr, nullptr, scope.stream, &Q);
+            if (!descs) {
+                fail("device-index read: cannot resolve the blocks");
+                return -1;
+            }
+            if (plan.path == ReadPath::kLookupGather) {
+                G.descs = descs;  // {pool address or 0, local byte offset} (dst_base 0)
+                e = kernels::launch_kv_gather(G, scope.stream);
+            } else if (plan.path == ReadPath::kLookupFp8) {
                 kernels::Fp8Launch F;
-                F.descs = out;
+                F.descs = descs;
                 F.n = uint32_t(n);
                 F.elems = uint32_t(fp8_elems);
                 F.status = ctx->status_d;
-                F.max_ctas = grid_cap;
+                F.max_ctas = plan.grid_cap;
                 F.aligned16 = (align_or & 15) == 0;
-                F.variant = all_remote ? 0 : 1;
-                e = kernels::launch_kv_read_fp8(F, stream);
-            } else if (e == cudaSuccess) {
+                F.variant = plan.variant;
+                e = kernels::launch_kv_read_fp8(F, scope.stream);
+            } else {
                 kernels::CopyLaunch L;
-                L.descs = out;
+                L.descs = descs;
                 L.n = uint32_t(n);
                 L.bytes = uint32_t(block_size);
                 L.align_or = align_or;
                 L.status = ctx->status_d;
-                L.variant = local_auto_variant(copy_variant_, all_local);
+                L.variant = plan.variant;
                 L.stage_bytes = pipe_stage_;
                 L.ring_bytes = pipe_ring_;
-                L.max_ctas = grid_cap;
-                e = kernels::launch_kv_copy(L, stream);
+                L.max_ctas = plan.grid_cap;
+                e = kernels::launch_kv_copy(L, scope.stream);
             }
-            stats_.kernel_launches += 2;
-            if (e == cudaSuccess && Q.found_at) {
+            if (e == cudaSuccess) {
                 // the server evicts: the entries must still be the ones the lookup resolved
                 kernels::ValidateLaunch V;
                 V.found_at = Q.found_at;
@@ -847,80 +799,95 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
                 V.table = Q.table;
                 V.shards = Q.shards;
                 V.status = ctx->status_d;
-                e = kernels::launch_index_validate(V, stream);
-                stats_.kernel_launches += 1;
+                e = kernels::launch_index_validate(V, scope.stream);
             }
         }
+        stats_.ns_build += t_launch0 - t_build0;
         stats_.ns_launch += now_ns() - t_launch0;
-        if (e != cudaSuccess) {
-            fail(std::string("device-index read failed to launch: ") + cudaGetErrorString(e));
+        // lookup + copy + validate: resolve_descs counted the lookup
+        if (scope.launched(e, "device-index read failed to launch: ", plan.fused() ? 1 : 2, false,
+                           uint64_t(n) * uint64_t(block_size)) != 0)
             return -1;
-        }
-        ctx->mark(stream);
-        if (res) res->launched = true;
-        stats_.bytes_read += uint64_t(n) * uint64_t(block_size);
     }
     return 0;
 }
 
 // Device-addressable copy descriptors {mapped pool address (0 = miss), dst_base + offset} for
-// blocks[base, base + n): resolved on the GPU by the lookup kernel (rb == nullptr, the
-// descriptors land in device scratch) or taken from a server lookup (rb, pinned ring).
+// blocks[base, base + b.n): resolved on the GPU by the lookup kernel (rb == nullptr, the
+// descriptors land in device scratch) or taken from a server lookup (rb, pinned ring).  With
+// `checked`, the lookup also records where it found every hit (found_at), and *checked is
+// left holding the launch, for a validate launch after the copy.
 const kernels::CopyDesc* Connection::resolve_descs(DevCtx* ctx, const std::vector<KeyOffset>& blocks,
-                                                   size_t base, size_t n, int block_size,
+                                                   size_t base, const KeyBatch& b,
+                                                   const PackedKeys* packed, uint32_t need_bytes,
                                                    uint64_t dst_base,
                                                    const std::vector<RemoteBlock>* rb,
-                                                   void* stream_v) {
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+                                                   void* stream, kernels::LookupLaunch* checked) {
+    const size_t n = b.n;
+    if (n == 0) return nullptr;
     if (rb) {
         const size_t at_desc = ctx->ring_alloc(n * sizeof(kernels::CopyDesc));
         auto* descs = reinterpret_cast<kernels::CopyDesc*>(ctx->ring_h + at_desc);
         for (size_t i = 0; i < n; ++i) {
-            const RemoteBlock& b = (*rb)[base + i];
-            uint8_t* segbase = seg_dev_ptr(ctx, addr_seg(b.remote_addr));
+            const RemoteBlock& rbi = (*rb)[base + i];
+            uint8_t* segbase = seg_dev_ptr(ctx, addr_seg(rbi.remote_addr));
             if (!segbase) return nullptr;
-            descs[i].src = reinterpret_cast<uint64_t>(segbase) + addr_off(b.remote_addr);
+            descs[i].src = reinterpret_cast<uint64_t>(segbase) + addr_off(rbi.remote_addr);
             descs[i].dst = dst_base + blocks[base + i].offset;
         }
         return reinterpret_cast<const kernels::CopyDesc*>(ctx->ring_d + at_desc);
     }
-    auto m0 = mapping(0, ctx->device);
-    if (!m0 || !m0->dev_ptr) return nullptr;
-    size_t key_bytes = 0;
-    std::vector<std::string_view> kp(n);
-    for (size_t i = 0; i < n; ++i) {
-        kp[i] = blocks[base + i].key;
-        key_bytes += align_up(std::max<size_t>(kp[i].size(), 1), 8);
-    }
-    const size_t at_bytes = ctx->ring_alloc(key_bytes);
-    const size_t at_off = ctx->ring_alloc(n * 4);
-    const size_t at_len = ctx->ring_alloc(n * 4);
-    const size_t at_dst = ctx->ring_alloc(n * 8);
-    pack_keys(kp.data(), n, ctx->ring_h + at_bytes, reinterpret_cast<uint32_t*>(ctx->ring_h + at_off),
-              reinterpret_cast<uint32_t*>(ctx->ring_h + at_len));
-    auto* dst = reinterpret_cast<uint64_t*>(ctx->ring_h + at_dst);
-    for (size_t i = 0; i < n; ++i) dst[i] = blocks[base + i].offset;
-    kernels::LookupLaunch Q;
-    Q.key_bytes = ctx->ring_d + at_bytes;
-    Q.key_off = reinterpret_cast<const uint32_t*>(ctx->ring_d + at_off);
-    Q.key_len = reinterpret_cast<const uint32_t*>(ctx->ring_d + at_len);
+    kernels::LookupLaunch own;
+    kernels::LookupLaunch& Q = checked ? *checked : own;
+    if (!set_index(ctx, Q)) return nullptr;
+    const StagedKeys keys = ctx->stage_keys(blocks, base, b, packed);
+    Q.key_bytes = keys.bytes;
+    Q.key_off = keys.off;
+    Q.key_len = keys.len;
     Q.n = uint32_t(n);
-    Q.table = reinterpret_cast<const kernels::IndexBucket*>(m0->dev_ptr + segs_[0].index_off);
-    Q.table_mask = kernels::index_bucket_mask(segs_[0].index_slots);
-    Q.shards = index_shards(ctx, nullptr);
-    Q.nsegs = uint32_t(std::min<size_t>(segs_.size(), kernels::LookupLaunch::kMaxSegs));
-    for (uint32_t sgi = 0; sgi < Q.nsegs; ++sgi)
-        Q.seg_base[sgi] = reinterpret_cast<uint64_t>(seg_dev_ptr(ctx, sgi));
-    auto* out = reinterpret_cast<kernels::CopyDesc*>(
+    Q.out_descs = reinterpret_cast<kernels::CopyDesc*>(
         ctx->scratch + ctx->scratch_alloc(n * sizeof(kernels::CopyDesc)));
-    Q.out_descs = out;
-    Q.dst_off = reinterpret_cast<const uint64_t*>(ctx->ring_d + at_dst);
+    Q.dst_off = keys.dst;
     Q.dst_base = dst_base;
-    Q.need_bytes = uint32_t(block_size);
+    Q.need_bytes = need_bytes;
     Q.status = ctx->status_d;
-    if (kernels::launch_index_lookup(Q, stream) != cudaSuccess) return nullptr;
+    if (checked)
+        Q.found_at = reinterpret_cast<kernels::LookupLaunch::FoundAt*>(
+            ctx->scratch + ctx->scratch_alloc(n * sizeof(kernels::LookupLaunch::FoundAt)));
+    if (kernels::launch_index_lookup(Q, static_cast<cudaStream_t>(stream)) != cudaSuccess)
+        return nullptr;
     stats_.kernel_launches++;
-    return out;
+    return Q.out_descs;
+}
+
+// The reads that resolve their blocks to descriptors first and launch their own kernels on
+// them: launch(scope, descs, base, n) runs once per batch and returns 0 or -1.
+template <typename Launch>
+int Connection::read_resolved(const std::vector<KeyOffset>& blocks, int block_size, int device,
+                              uint64_t stream_in, uint64_t dst_base, const char* what,
+                              Launch&& launch) {
+    const bool via_index = device_lookup_ && device_index_usable();
+    std::vector<RemoteBlock> rb;
+    if (!via_index) {
+        const int r = lookup_blocks(kOpReadLookup, blocks, block_size, rb);
+        if (r != 0) return r;
+    }
+    std::lock_guard<std::mutex> lk(mu_);
+    LaunchScope scope(*this, device, nullptr);
+    if (!scope.ctx || scope.begin(stream_in, false) != 0) return -1;
+    KeyBatch b;
+    for (size_t base = 0; base < blocks.size(); base += b.n) {
+        b = next_key_batch(blocks, base, kMaxBatch);
+        const kernels::CopyDesc* descs = resolve_descs(scope.ctx, blocks, base, b, nullptr,
+                                                       uint32_t(block_size), dst_base,
+                                                       via_index ? nullptr : &rb, scope.stream);
+        if (!descs) {
+            fail(std::string(what) + ": cannot resolve the blocks");
+            return -1;
+        }
+        if (launch(scope, descs, base, b.n) != 0) return -1;
+    }
+    return 0;
 }
 
 // The same pages into several destination tensors (TP ranks / beams sharing a prefix): every
@@ -935,40 +902,22 @@ int Connection::r_rdma_multi(const std::vector<KeyOffset>& blocks, int block_siz
         return -1;
     }
     if (bases.size() == 1) return r_rdma(blocks, block_size, bases[0], device, stream_in);
-    const bool via_index = device_lookup_ && device_index_usable();
-    std::vector<RemoteBlock> rb;
-    if (!via_index) {
-        const int r = lookup_blocks(kOpReadLookup, blocks, block_size, rb);
-        if (r != 0) return r;
-    }
     NvtxRange nvtx("istore.read_multi");
-    std::lock_guard<std::mutex> lk(mu_);
-    DevCtx* ctx = dev_ctx(device);
-    if (!ctx) return -1;
-    DeviceGuard g(device);
-    if (doorbell_quiesce(ctx) != 0) return -1;
-    cudaStream_t stream = ctx->pick(reinterpret_cast<cudaStream_t>(stream_in), false, streams_);
-    stats_.calls++;
     uint64_t align_or = 0;
     for (uint64_t b : bases) align_or |= b;
-    for (size_t base = 0; base < blocks.size(); base += kMaxBatch) {
-        const size_t n = std::min(kMaxBatch, blocks.size() - base);
+    auto launch = [&](LaunchScope& scope, const kernels::CopyDesc* descs_d, size_t base,
+                      size_t n) {
         for (size_t i = 0; i < n; ++i) align_or |= blocks[base + i].offset;
-        const kernels::CopyDesc* descs_d =
-            resolve_descs(ctx, blocks, base, n, block_size, bases[0], via_index ? nullptr : &rb, stream);
-        if (!descs_d) {
-            fail("multi-destination read: cannot resolve the blocks");
-            return -1;
-        }
         // Local pool: thread-block clusters (multicast bulk load into 2 or 4 CTAs, one
         // destination each; an odd last destination shares a 2-cluster with its predecessor,
         // which is rewritten with the same bytes).  Pool behind NVLink: one load, K stores
         // per CTA (the fan-out flavour of the TMA pipeline) - the fabric still carries every
         // page once.
         bool src_local = true;
-        for (size_t sgi = 0; sgi < ctx->seg_remote.size(); ++sgi)
-            if (ctx->seg_ptr[sgi] && ctx->seg_remote[sgi]) src_local = false;
+        for (size_t sgi = 0; sgi < scope.ctx->seg_remote.size(); ++sgi)
+            if (scope.ctx->seg_ptr[sgi] && scope.ctx->seg_remote[sgi]) src_local = false;
         cudaError_t e = cudaSuccess;
+        uint32_t launches = 0;
         size_t r = 0;
         while (e == cudaSuccess && r < bases.size()) {
             const size_t left = bases.size() - r;
@@ -979,12 +928,12 @@ int Connection::r_rdma_multi(const std::vector<KeyOffset>& blocks, int block_siz
                 M.bytes = uint32_t(block_size);
                 M.align_or = align_or;
                 M.src_local = true;
-                M.status = r == 0 ? ctx->status_d : nullptr;  // count a miss once
+                M.status = r == 0 ? scope.ctx->status_d : nullptr;  // count a miss once
                 const size_t first = left >= 2 ? r : r - 1;
                 M.ndst = left >= 4 ? 4 : 2;
                 for (int j = 0; j < M.ndst; ++j)
                     M.delta[j] = int64_t(bases[first + size_t(j)]) - int64_t(bases[0]);
-                e = kernels::launch_kv_pipe_mcast(M, stream);
+                e = kernels::launch_kv_pipe_mcast(M, scope.stream);
                 r = first + size_t(M.ndst);
             } else {
                 kernels::CopyLaunch L;
@@ -992,25 +941,22 @@ int Connection::r_rdma_multi(const std::vector<KeyOffset>& blocks, int block_siz
                 L.n = uint32_t(n);
                 L.bytes = uint32_t(block_size);
                 L.align_or = align_or;
-                L.status = r == 0 ? ctx->status_d : nullptr;
+                L.status = r == 0 ? scope.ctx->status_d : nullptr;
                 L.variant = kernels::kCopyTma;
                 L.max_ctas = max_ctas_;
                 L.fan_n = int(std::min<size_t>(left, 4));
                 for (int j = 0; j < L.fan_n; ++j)
                     L.fan_delta[j] = int64_t(bases[r + size_t(j)]) - int64_t(bases[0]);
-                e = kernels::launch_kv_pipe_copy(L, stream);
+                e = kernels::launch_kv_pipe_copy(L, scope.stream);
                 r += size_t(L.fan_n);
             }
-            stats_.kernel_launches++;
+            ++launches;
         }
-        if (e != cudaSuccess) {
-            fail(std::string("multi-destination read failed to launch: ") + cudaGetErrorString(e));
-            return -1;
-        }
-        ctx->mark(stream);
-        stats_.bytes_read += uint64_t(n) * uint64_t(block_size) * bases.size();
-    }
-    return 0;
+        return scope.launched(e, "multi-destination read failed to launch: ", launches, false,
+                              uint64_t(n) * uint64_t(block_size) * bases.size());
+    };
+    return read_resolved(blocks, block_size, device, stream_in, bases[0],
+                         "multi-destination read", launch);
 }
 
 // read_cache fused with the layout swizzle of the attention consumer: pages are stored
@@ -1031,31 +977,12 @@ int Connection::r_rdma_hnd(const std::vector<KeyOffset>& blocks, int tokens, int
             fail("read_cache_hnd: page index beyond the destination tensor");
             return -1;
         }
-    const bool via_index = device_lookup_ && device_index_usable();
-    std::vector<RemoteBlock> rb;
-    if (!via_index) {
-        const int r = lookup_blocks(kOpReadLookup, blocks, block_size, rb);
-        if (r != 0) return r;
-    }
     NvtxRange nvtx("istore.read_hnd");
-    std::lock_guard<std::mutex> lk(mu_);
-    DevCtx* ctx = dev_ctx(device);
-    if (!ctx) return -1;
-    DeviceGuard g(device);
-    if (doorbell_quiesce(ctx) != 0) return -1;
-    cudaStream_t stream = ctx->pick(reinterpret_cast<cudaStream_t>(stream_in), false, streams_);
-    stats_.calls++;
-    for (size_t base = 0; base < blocks.size(); base += kMaxBatch) {
-        const size_t n = std::min(kMaxBatch, blocks.size() - base);
-        // dst_base 0: the descriptor's dst field carries the page index
-        const kernels::CopyDesc* descs_d =
-            resolve_descs(ctx, blocks, base, n, block_size, 0, via_index ? nullptr : &rb, stream);
-        if (!descs_d) {
-            fail("read_cache_hnd: cannot resolve the blocks");
-            return -1;
-        }
+    // dst_base 0: the descriptor's dst field carries the page index
+    return read_resolved(blocks, block_size, device, stream_in, 0, "read_cache_hnd",
+                         [&](LaunchScope& scope, const kernels::CopyDesc* descs, size_t, size_t n) {
         kernels::HndLaunch H;
-        H.descs = descs_d;
+        H.descs = descs;
         H.n = uint32_t(n);
         H.tokens = uint32_t(tokens);
         H.heads = uint32_t(heads);
@@ -1063,18 +990,12 @@ int Connection::r_rdma_hnd(const std::vector<KeyOffset>& blocks, int tokens, int
         H.elem_size = uint32_t(elem_size);
         H.dst_base = base_ptr;
         H.num_pages = uint32_t(num_pages);
-        H.status = ctx->status_d;
+        H.status = scope.ctx->status_d;
         H.max_ctas = max_ctas_;
-        const cudaError_t e = kernels::launch_kv_pipe_hnd(H, stream);
-        if (e != cudaSuccess) {
-            fail(std::string("layout-swizzling read failed to launch: ") + cudaGetErrorString(e));
-            return -1;
-        }
-        stats_.kernel_launches++;
-        ctx->mark(stream);
-        stats_.bytes_read += uint64_t(n) * uint64_t(block_size);
-    }
-    return 0;
+        return scope.launched(kernels::launch_kv_pipe_hnd(H, scope.stream),
+                              "layout-swizzling read failed to launch: ", 1, false,
+                              uint64_t(n) * uint64_t(block_size));
+    });
 }
 
 int Connection::match_via_device_index(const std::vector<std::string_view>& keys, bool exist_only) {
@@ -1082,33 +1003,20 @@ int Connection::match_via_device_index(const std::vector<std::string_view>& keys
     const int device = cfg_.device >= 0 ? cfg_.device : std::max(default_device_, 0);
     DevCtx* ctx = dev_ctx(device);
     if (!ctx) return -3;
-    auto m0 = mapping(0, device);
-    if (!m0 || !m0->dev_ptr || !segs_[0].index_slots) return -3;
-    const size_t n = keys.size();
-    size_t key_bytes = 0;
-    std::vector<std::string_view> kp(n);
-    for (size_t i = 0; i < n; ++i) {
-        kp[i] = keys[i];
-        key_bytes += align_up(std::max<size_t>(keys[i].size(), 1), 8);
-    }
-    if (key_bytes + n * 8 + 4096 > kRingBytes / 2) return -3;  // too large: use the control plane
     DeviceGuard g(device);
-    if (doorbell_quiesce(ctx) != 0) return -3;
-    const size_t at_bytes = ctx->ring_alloc(key_bytes);
-    const size_t at_off = ctx->ring_alloc(n * 4);
-    const size_t at_len = ctx->ring_alloc(n * 4);
-    pack_keys(kp.data(), n, ctx->ring_h + at_bytes,
-              reinterpret_cast<uint32_t*>(ctx->ring_h + at_off),
-              reinterpret_cast<uint32_t*>(ctx->ring_h + at_len));
     kernels::LookupLaunch Q;
-    Q.key_bytes = ctx->ring_d + at_bytes;
-    Q.key_off = reinterpret_cast<const uint32_t*>(ctx->ring_d + at_off);
-    Q.key_len = reinterpret_cast<const uint32_t*>(ctx->ring_d + at_len);
-    Q.n = uint32_t(n);
-    Q.table = reinterpret_cast<const kernels::IndexBucket*>(m0->dev_ptr + segs_[0].index_off);
-    Q.table_mask = kernels::index_bucket_mask(segs_[0].index_slots);
-    Q.shards = index_shards(ctx, nullptr);
-    const size_t words = (n + 31) / 32;
+    if (!set_index(ctx, Q, false)) return -3;
+    std::vector<KeyOffset> blocks(keys.size());
+    for (size_t i = 0; i < keys.size(); ++i) blocks[i] = KeyOffset{keys[i], 0};
+    const KeyBatch b = next_key_batch(blocks, 0, blocks.size());
+    if (b.n < blocks.size()) return -3;  // more than one launch stages: use the control plane
+    if (doorbell_quiesce(ctx) != 0) return -3;
+    const StagedKeys staged = ctx->stage_keys(blocks, 0, b, nullptr);
+    Q.key_bytes = staged.bytes;
+    Q.key_off = staged.off;
+    Q.key_len = staged.len;
+    Q.n = uint32_t(b.n);
+    const size_t words = (b.n + 31) / 32;
     Q.present = reinterpret_cast<uint32_t*>(ctx->scratch + ctx->scratch_alloc(words * 4));
     Q.ticket = reinterpret_cast<uint32_t*>(ctx->zeros + ctx->zeros_alloc(4));
     Q.status = ctx->status_d;

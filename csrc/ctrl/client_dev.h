@@ -60,6 +60,15 @@ inline void doorbell_write_line(kernels::DoorbellReq* slot, uint64_t seq, uint32
     std::atomic_thread_fence(std::memory_order_seq_cst);  // out of the store buffer now
 }
 
+// One launch's keys in the pinned ring, as the device reads them: packed the way the lookup
+// kernels hash them (client.h: PackedKeys), with every block's destination offset.
+struct StagedKeys {
+    const uint8_t* bytes = nullptr;
+    const uint32_t* off = nullptr;
+    const uint32_t* len = nullptr;
+    const uint64_t* dst = nullptr;
+};
+
 // Per-device data-plane state.
 struct Connection::DevCtx {
     int device = -1;
@@ -239,6 +248,42 @@ struct Connection::DevCtx {
         return alloc(kScratch, align_up(bytes, 256), kScratchBytes);
     }
     size_t zeros_alloc(size_t bytes) { return alloc(kZeros, align_up(bytes, 256), kZeroBytes); }
+
+    // Stage the keys and destination offsets of blocks[base, base + b.n) for one launch.
+    // `packed` holds the call's keys in the staged layout already (b is then the whole call):
+    // three memcpys instead of a pass over the keys.
+    StagedKeys stage_keys(const std::vector<KeyOffset>& blocks, size_t base, const KeyBatch& b,
+                          const PackedKeys* packed) {
+        const size_t n = b.n;
+        const size_t at_bytes = ring_alloc(b.key_bytes);
+        const size_t at_off = ring_alloc(n * 4);
+        const size_t at_len = ring_alloc(n * 4);
+        const size_t at_dst = ring_alloc(n * 8);
+        auto* off = reinterpret_cast<uint32_t*>(ring_h + at_off);
+        auto* len = reinterpret_cast<uint32_t*>(ring_h + at_len);
+        auto* dst = reinterpret_cast<uint64_t*>(ring_h + at_dst);
+        if (packed) {
+            std::memcpy(ring_h + at_bytes, packed->bytes, b.key_bytes);
+            std::memcpy(off, packed->off, n * 4);
+            std::memcpy(len, packed->len, n * 4);
+        } else {
+            // each key on an 8-byte boundary, zero padded to a multiple of 8
+            size_t at = 0;
+            for (size_t i = 0; i < n; ++i) {
+                const std::string_view k = blocks[base + i].key;
+                const size_t padded = align_up(k.size() ? k.size() : 1, 8);
+                off[i] = uint32_t(at);
+                len[i] = uint32_t(k.size());
+                std::memcpy(ring_h + at_bytes + at, k.data(), k.size());
+                std::memset(ring_h + at_bytes + at + k.size(), 0, padded - k.size());
+                at += padded;
+            }
+        }
+        for (size_t i = 0; i < n; ++i) dst[i] = blocks[base + i].offset;
+        return StagedKeys{ring_d + at_bytes, reinterpret_cast<const uint32_t*>(ring_d + at_off),
+                          reinterpret_cast<const uint32_t*>(ring_d + at_len),
+                          reinterpret_cast<const uint64_t*>(ring_d + at_dst)};
+    }
 };
 
 }  // namespace istore

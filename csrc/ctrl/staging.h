@@ -1,8 +1,9 @@
 // Reuse of a device context's staging regions (client_dev.h): the pinned ring, the device
-// scratch and the zeroed counters.  Each region is a bump allocator over a fixed buffer, and a
-// launch uses the bytes handed out since the previous launch.  When the allocator comes round
-// to bytes again, the launches that used them one lap earlier must have completed; only those
-// are waited for, so the launches of the current lap keep running.
+// scratch and the zeroed counters; and how many blocks one launch stages.  Each region is a
+// bump allocator over a fixed buffer, and a launch uses the bytes handed out since the
+// previous launch.  When the allocator comes round to bytes again, the launches that used them
+// one lap earlier must have completed; only those are waited for, so the launches of the
+// current lap keep running.
 //
 // Positions are byte counts since the context was created: they never wrap, and the offset
 // into a region of `size` bytes is pos % size.  No CUDA in here (Event is a plain handle and the
@@ -84,5 +85,36 @@ class StagingFifo {
     uint64_t pos_[R] = {};
     uint64_t first_[R];  // first byte placed since the last push, kNone when there is none
 };
+
+// One launch's share of a call's keys, taken from the front of the `left` keys still to go:
+// at most max_blocks keys, whose staged bytes stay within max_bytes.  A key stages its bytes
+// zero padded to a multiple of 8 (an empty key takes 8) plus 16 bytes of offset, length and
+// destination.  The batch holds at least one key, so a call always makes progress: a key
+// above the bound is staged on its own.  key_len(i) is the length of the i-th key from the front.
+struct KeyBatch {
+    size_t n = 0;          // keys
+    size_t key_bytes = 0;  // their padded bytes
+};
+template <typename KeyLen>
+KeyBatch key_batch(size_t left, size_t max_blocks, size_t max_bytes, KeyLen&& key_len) {
+    KeyBatch b;
+    size_t staged = 0;
+    for (; b.n < left && b.n < max_blocks; ++b.n) {
+        const size_t len = key_len(b.n);
+        const size_t padded = ((len ? len : 1) + 7) & ~size_t(7);
+        staged += padded + 16;
+        if (staged > max_bytes && b.n > 0) break;
+        b.key_bytes += padded;
+    }
+    return b;
+}
+
+// Gathered blocks of nparts parts: at most 2^30 work items per launch (a chunk is >= 16 KB or
+// a whole part), and never fewer than one block.
+inline size_t gather_max_blocks(size_t max_blocks, uint32_t nparts, uint32_t part_bytes) {
+    const uint64_t items = uint64_t(nparts) * ((uint64_t(part_bytes) + 16383u) / 16384u);
+    const uint64_t cap = (1ull << 30) / items;
+    return cap == 0 ? 1 : cap < max_blocks ? size_t(cap) : max_blocks;
+}
 
 }  // namespace istore

@@ -29,6 +29,8 @@
 #include "core/mempool.h"
 #include "core/trace.h"
 #include "ctrl/client.h"
+#include "ctrl/client_dev.h"
+#include "ctrl/read_plan.h"
 #include "ctrl/server.h"
 #include "ctrl/staging.h"
 #include "fabric/nvls.h"
@@ -1269,6 +1271,47 @@ PYBIND11_MODULE(_infinistore, m) {
                  return py::int_(ev);
              })
         .def("in_flight", &Staging::in_flight);
+    // how a read call is split into launches (ctrl/staging.h), with the client's limits
+    t.attr("RING_BYTES") = kRingBytes;
+    t.attr("MAX_BATCH") = kMaxBatch;
+    t.def("gather_max_blocks", [](uint32_t nparts, uint32_t part_bytes) {
+        if (nparts == 0 || part_bytes == 0) throw py::value_error("needs nparts, part_bytes > 0");
+        return gather_max_blocks(kMaxBatch, nparts, part_bytes);
+    });
+    t.def("key_batches",
+          [](const std::vector<size_t>& key_lens, size_t max_blocks) {
+              if (max_blocks == 0) throw py::value_error("needs max_blocks > 0");
+              py::list out;  // (keys, padded key bytes) of every launch
+              for (size_t base = 0; base < key_lens.size();) {
+                  const KeyBatch b = key_batch(key_lens.size() - base, max_blocks, kRingBytes / 2,
+                                               [&](size_t i) { return key_lens[base + i]; });
+                  out.append(py::make_tuple(b.n, b.key_bytes));
+                  base += b.n;
+              }
+              return out;
+          },
+          py::arg("key_lens"), py::arg("max_blocks") = kMaxBatch);
+    // which kernels a read through the device index runs (ctrl/read_plan.h)
+    t.def("plan_device_read",
+          [](size_t n, uint32_t block_bytes, uint32_t fp8_elems, bool gather, bool fp8_fused_ok,
+             bool scatter_fused_ok, int copy_variant, bool all_local, bool all_remote, int max_ctas,
+             int sm_count) {
+              const DeviceReadPlan p = plan_device_read(DeviceReadIn{
+                  n, block_bytes, fp8_elems, gather, fp8_fused_ok, scatter_fused_ok, copy_variant,
+                  all_local, all_remote, max_ctas, sm_count});
+              static const char* const kPaths[] = {"fused_copy",  "fused_fp8",  "fused_scatter",
+                                                   "lookup_copy", "lookup_fp8", "lookup_gather"};
+              py::dict d;
+              d["path"] = kPaths[int(p.path)];
+              d["variant"] = p.variant;
+              d["grid_cap"] = p.grid_cap;
+              d["ldst_align"] = p.ldst_align;
+              return d;
+          },
+          py::arg("n"), py::arg("block_bytes"), py::arg("fp8_elems") = 0, py::arg("gather") = false,
+          py::arg("fp8_fused_ok") = false, py::arg("scatter_fused_ok") = false,
+          py::arg("copy_variant") = 0, py::arg("all_local") = false, py::arg("all_remote") = false,
+          py::arg("max_ctas") = 0, py::arg("sm_count") = 132);
     py::class_<MM>(t, "MM")
         .def(py::init<>())
         .def("add_pool", &MM::add_pool)

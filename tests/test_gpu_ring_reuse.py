@@ -179,3 +179,48 @@ def test_rounds_through_every_staging_region_without_a_full_drain():
         conn.close()
     finally:
         srv.stop()
+
+
+@pytest.mark.gpu
+def test_a_read_whose_keys_outgrow_the_ring_takes_several_launches():
+    """65536 keys of 300 bytes stage about 21 MB (keys, offsets, lengths, destinations): more
+    than the 16 MB ring.  One read_cache call through the device index splits them into
+    launches of at most half the ring each, and every page arrives."""
+    import torch
+
+    import infinistore_b200 as ist
+    from infinistore_b200 import _infinistore as m
+
+    nb, elems = 65536, 2048  # 4 KB pages of bf16
+    cfg = m.ServerConfig()
+    cfg.service_port = 0
+    cfg.host = "127.0.0.1"
+    cfg.pool_backend = "hbm"
+    cfg.pool_devices = [0]
+    cfg.prealloc_bytes = nb * elems * 2 + (256 << 20)
+    cfg.minimal_allocate_size = 4
+    srv = m.Server(cfg)
+    port = srv.start()
+    try:
+        conn = ist.InfinityConnection(ist.ClientConfig(
+            host_addr="127.0.0.1", service_port=port, connection_type=ist.TYPE_RDMA,
+            log_level="warning", device=0, device_lookup=True))
+        conn.connect()
+        tag = uuid.uuid4().hex
+        keys = [f"{tag}-{i:06d}-".ljust(300, "k") for i in range(nb)]
+        assert {len(k) for k in keys} == {300}
+        src = torch.randn(nb * elems, device="cuda:0").to(torch.bfloat16)
+        dst = torch.zeros_like(src)
+        conn.register_mr(src)
+        conn.register_mr(dst)
+        offs = [i * elems for i in range(nb)]
+        conn.rdma_write_cache(src, offs, elems, conn.allocate_rdma(keys, elems * 2))
+        conn.sync()
+        before = conn.stats()["kernel_launches"]
+        conn.read_cache(dst, list(zip(keys, offs)), elems)
+        conn.sync()
+        assert conn.stats()["kernel_launches"] - before > 1
+        assert torch.equal(src, dst)
+        conn.close()
+    finally:
+        srv.stop()
