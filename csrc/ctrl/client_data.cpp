@@ -741,7 +741,6 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
             R.dst_off = keys.dst;
             R.dst_base = base_ptr;
             R.bytes = uint32_t(block_size);
-            if (plan.ldst_align) R.align_or |= 16;
             R.status = ctx->status_d;
             // always: a purge (or an eviction) may free a block while a device-path read is
             // copying it; the post-copy tag check turns that into a reported miss

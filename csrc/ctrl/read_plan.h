@@ -35,7 +35,6 @@ struct DeviceReadPlan {
     ReadPath path = ReadPath::kLookupCopy;
     int variant = kernels::kCopyAuto;  // of the launch that moves the pages (unused by gathers)
     int grid_cap = 0;                  // max_ctas of every launch
-    bool ldst_align = false;           // fused launches: align_or | 16 forces the ld/st kernel
     bool fused() const { return path <= ReadPath::kFusedScatter; }
 };
 
@@ -77,13 +76,16 @@ inline DeviceReadPlan plan_device_read(const DeviceReadIn& in) {
         p.path = in.fp8_fused_ok ? ReadPath::kFusedFp8 : ReadPath::kLookupFp8;
     else
         p.path = whole_blocks || small_batch ? ReadPath::kFusedCopy : ReadPath::kLookupCopy;
-    // lookup then fp8: the TMA pipeline (0) when every segment is remote, the ld/st kernels
-    // (1) otherwise.  Intentional: move_blocks' rule is all_local ? 1 : 0, and the two differ
+    // lookup then fp8: the TMA pipeline when every segment is remote, the ld/st kernels
+    // otherwise.  Intentional: move_blocks' rule is all_local ? ld/st : TMA, and the two differ
     // for a pool that mixes local and remote segments.
-    p.variant = p.path == ReadPath::kLookupFp8 ? (in.all_remote ? 0 : 1)
-                : p.fused() && small_batch     ? int(kernels::kCopyLdSt256)
-                                               : local_auto_variant(in.copy_variant, in.all_local);
-    p.ldst_align = p.fused() && in.copy_variant == kernels::kCopyLdSt;
+    if (p.path == ReadPath::kLookupFp8)
+        p.variant = in.all_remote ? kernels::kFp8Auto : kernels::kFp8LdSt;
+    else if (p.path == ReadPath::kFusedCopy && in.copy_variant == kernels::kCopyLdSt)
+        p.variant = kernels::kCopyLdSt;  // the 16-byte ld/st read kernel (launch_plan.h)
+    else
+        p.variant = p.fused() && small_batch ? int(kernels::kCopyLdSt256)
+                                             : local_auto_variant(in.copy_variant, in.all_local);
     return p;
 }
 

@@ -5,13 +5,28 @@
 // 32-byte vectors held are kept in flight as eight 16-byte vectors, warp-contiguous.
 #pragma once
 
+#include <algorithm>
+
 #include "common.cuh"
+#include "launch_plan.h"
 
 namespace istore::kernels {
 
 using namespace dev;
 
 constexpr int kLdStThreads = 256;
+
+// CTAs per SM the 16- and 32-byte flavours of an ld/st kernel keep resident, for launches of
+// `threads` threads.  The callers keep the answer for the life of the process.
+template <typename K16, typename K32>
+LdStResident ldst_resident(K16* k16, K32* k32, int threads) {
+    LdStResident r;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&r.r16, k16, threads, 0);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&r.r32, k32, threads, 0);
+    r.r16 = std::max(r.r16, 1);
+    r.r32 = std::max(r.r32, 1);
+    return r;
+}
 
 // NVLS: one 16-byte store to a multicast address lands in every replica  (multimem.st)
 __device__ __forceinline__ void st_multicast_v4(void* mc, const uint4& v) {

@@ -10,6 +10,7 @@
 #include <cuda_runtime_api.h>
 
 #include <cstdint>
+#include <initializer_list>
 
 namespace istore::kernels {
 
@@ -177,13 +178,6 @@ struct ReadFusedLaunch;
 bool scatter_read_fused_supported(const ReadFusedLaunch& r, const GatherLaunch& g);
 cudaError_t launch_kv_pipe_scatter_read(const ReadFusedLaunch& r, const GatherLaunch& g,
                                         cudaStream_t stream);
-struct PipeGeometry {
-    uint32_t stage_bytes = 0;
-    uint32_t stages = 0;
-    size_t smem = 0;
-};
-PipeGeometry pipe_geometry(uint32_t bytes, uint32_t stage_pref, uint32_t ring_pref);
-
 // fp8 (e4m3) fused variants: the write converts bf16 pages to e4m3 with one fp32 scale
 // per `group` elements (the head_dim row) and stores payload + scales into the pool block;
 // the read dequantises back to bf16 while scattering into the paged KV cache.
@@ -201,11 +195,14 @@ struct Fp8Launch {
     bool all_local = false;
     IndexShards shards;     // further index shards (shard 0 = table / table_mask)
     bool aligned16 = true;  // every page address is 16-byte aligned (bulk copies need it)
-    int variant = 0;        // 0 = auto (TMA pipeline, 8 compute warps), 1 = ld/st kernels,
-                            // 2 = TMA pipeline with 4 compute warps (A/B)
+    int variant = 0;        // Fp8Variant
+};
+enum Fp8Variant : int {
+    kFp8Auto = 0,  // the TMA pipeline with 8 compute warps, ld/st kernels where it does not fit
+    kFp8LdSt = 1,  // the ld/st kernels
+    kFp8Tma4 = 2,  // the TMA pipeline with 4 compute warps (A/B)
 };
 // The TMA-pipelined flavour (kv_fp8_pipe.cu): needs elems % 512 == 0 and aligned pages.
-bool fp8_pipe_supported(const Fp8Launch& a);
 cudaError_t launch_kv_fp8_pipe(const Fp8Launch& a, bool write, cudaStream_t stream);
 // bytes a quantised page occupies in the pool: elems (e4m3) + 4 * elems/group (scales)
 inline uint32_t fp8_block_bytes(uint32_t elems, uint32_t group) {
@@ -306,7 +303,6 @@ struct ReadFusedLaunch {
 // aligned and the blocks are >= kPipeMinBytes; the ld/st kernel otherwise.  Both re-check
 // every entry after its copy.
 cudaError_t launch_kv_read_fused(const ReadFusedLaunch& a, cudaStream_t stream);
-bool pipe_read_supported(const ReadFusedLaunch& a);
 cudaError_t launch_kv_pipe_read(const ReadFusedLaunch& a, cudaStream_t stream);
 // The same for fp8 pages ([elems x e4m3][elems/128 x fp32 scale] in the pool, bf16 at the
 // destination): resolver + dequantising TMA pipeline in one launch (kv_fp8_pipe.cu).
@@ -424,5 +420,12 @@ cudaError_t launch_kv_doorbell(const DoorbellLaunch& a, cudaStream_t stream);
 
 // Number of SMs of the current device (cached per device).
 int sm_count();
+// Raises the dynamic shared-memory limit of each kernel to its `bytes`, once per device:
+// `done` holds the caller's flag of every device.
+struct SmemLimit {
+    const void* kernel;
+    int bytes;
+};
+cudaError_t set_smem_limits_once(bool (&done)[64], std::initializer_list<SmemLimit> limits);
 
 }  // namespace istore::kernels

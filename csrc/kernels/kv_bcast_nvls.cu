@@ -11,6 +11,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "launch_plan.h"
 
 namespace istore::kernels {
 
@@ -111,8 +112,7 @@ cudaError_t launch_kv_bcast_nvls(const BcastLaunch& a, cudaStream_t stream) {
     const uint32_t chunk = std::min(a.bytes, kChunk);
     const uint32_t cpb = (a.bytes + chunk - 1) / chunk;
     const uint64_t total = uint64_t(a.n) * cpb;
-    int ctas = a.max_ctas > 0 ? a.max_ctas : 4 * sm_count();
-    ctas = int(std::min<uint64_t>(uint64_t(ctas), total));
+    const int ctas = clamp_grid(a.max_ctas > 0 ? a.max_ctas : 4 * sm_count(), total);
     kv_bcast_nvls_kernel<<<ctas, kThreads, 0, stream>>>(a.descs, a.n, a.bytes, chunk, cpb, a.flags_mc);
     return cudaGetLastError();
 }
@@ -125,8 +125,7 @@ uint32_t bcast_chunks_per_block(uint32_t bytes) {
 cudaError_t launch_kv_read_when_ready(const ReadyLaunch& a, cudaStream_t stream) {
     if (a.n == 0 || a.bytes == 0) return cudaSuccess;
     if (a.bytes % 16 || !a.flags_local) return cudaErrorInvalidValue;
-    int ctas = a.max_ctas > 0 ? a.max_ctas : 2 * sm_count();
-    ctas = int(std::min<uint32_t>(uint32_t(ctas), a.n));
+    const int ctas = clamp_grid(a.max_ctas > 0 ? a.max_ctas : 2 * sm_count(), a.n);
     kv_read_when_ready_kernel<<<ctas, kThreads, 0, stream>>>(a.descs, a.n, a.bytes, a.flags_local,
                                                             a.ready_value, a.status);
     return cudaGetLastError();

@@ -18,7 +18,6 @@
 //   kCopyLdSt / kCopyLdSt256 : this file - every thread streams 128-bit vectors, 4 (or,
 //               for 32-byte aligned blocks, 8) in flight per thread; used for small or
 //               unaligned blocks and for NVLS multicast stores (multimem.st has no bulk form).
-#include <algorithm>
 #include <cstring>
 #include <mutex>
 
@@ -33,12 +32,8 @@ namespace {
 
 using namespace dev;
 
-constexpr uint32_t kLdStChunk = 32u << 10;  // work item of the ld/st path
-
 // ---------------------------------------------------------------- ld/st path (copy_span.cuh)
-// Descriptors of small batches travel in the kernel parameters (constant bank): reading
-// them from the pinned host ring costs a PCIe round trip at the start of every launch.
-constexpr int kParamDescs = 256;
+// Small batches: descriptors in the kernel parameters (launch_plan.h).
 template <int N>
 struct DescParam {
     CopyDesc d[N];
@@ -153,118 +148,77 @@ int sm_count() {
     return cached[dev];
 }
 
+cudaError_t set_smem_limits_once(bool (&done)[64], std::initializer_list<SmemLimit> limits) {
+    static std::mutex mu;
+    int dev = 0;
+    cudaGetDevice(&dev);
+    std::lock_guard<std::mutex> lk(mu);
+    if (dev < 0 || dev >= 64 || done[dev]) return cudaSuccess;
+    for (const SmemLimit& l : limits) {
+        const cudaError_t e =
+            cudaFuncSetAttribute(l.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, l.bytes);
+        if (e != cudaSuccess) return e;
+    }
+    done[dev] = true;
+    return cudaSuccess;
+}
+
 cudaError_t launch_kv_copy(const CopyLaunch& a, cudaStream_t stream) {
     if (a.n == 0 || a.bytes == 0) return cudaSuccess;
-    Publish pub{a.recs, a.table, a.table_mask, a.done, a.status, a.n, a.trace, !a.all_local, a.debug,
-                a.shards};
-    if (!a.table || !a.done) pub.recs = nullptr;
-    const int sms = sm_count();
-
-    int variant = a.variant;
-    // Alignment: bulk copies need 16-byte aligned addresses and sizes (the caller ORs every
-    // local address into align_or; pool blocks are granule aligned).
-    const bool aligned16 = (a.bytes % 16) == 0 && (a.align_or & 15) == 0;
-    const bool aligned32 = (a.bytes % 32) == 0 && (a.align_or & 31) == 0;
-    if (a.multicast) {
-        if (!aligned16) return cudaErrorInvalidValue;  // multimem.st moves 16-byte vectors
-        variant = kCopyLdSt;
-    }
-    // auto: the TMA pipeline from kPipeMinBytes up (3 warps per CTA); small blocks are bound
-    // by per-block issue cost, where 256 threads win
-    if (variant == kCopyAuto)
-        variant = (aligned16 && a.bytes >= kPipeMinBytes) ? kCopyTma
-                                                          : (aligned32 ? kCopyLdSt256 : kCopyLdSt);
-    if (!aligned16 && (variant == kCopyTma || variant == kCopyLdSt256)) variant = kCopyLdSt;
-    if (variant == kCopyLdSt256 && !aligned32) variant = kCopyLdSt;
-
-    // small batches: descriptors ride in the kernel parameters
-    const bool param = a.descs_host != nullptr && a.n <= uint32_t(kParamDescs) && aligned16;
-    DescParam<kParamDescs> pd;
-    if (param) std::memcpy(pd.d, a.descs_host, size_t(a.n) * sizeof(CopyDesc));
-    const DescParam<1> none{};
-
-    if (variant == kCopyTma) return launch_kv_pipe_copy(a, stream);
-
-    // Work item = one 32 KB chunk, or - when there are at least as many blocks as SMs - one
-    // whole block: then a block is moved by a single CTA, its commit needs no cross-CTA
-    // counter (claim, one fence, one store) and a reader resolves every key exactly once.
-    uint32_t chunk = std::min(a.bytes, kLdStChunk);
-    if (a.n >= uint32_t(sms) && a.bytes <= (1u << 20)) chunk = a.bytes;
-    const uint32_t cpb = (a.bytes + chunk - 1) / chunk;
-    const uint64_t total = uint64_t(a.n) * cpb;
     constexpr int T = kLdStThreads + 32;
-    // One wave: every CTA is resident and loops over its items, so the commit epilogue
-    // (fence + release) runs once per CTA instead of once per item and per wave.
-    static int resident16 = 0, resident32 = 0;
-    if (!resident16) {
-        int b16 = 0, b32 = 0;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b16, kv_copy_ldst_kernel<16, false>, T, 0);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b32, kv_copy_ldst_kernel<32, false>, T, 0);
-        resident16 = std::max(b16, 1);
-        resident32 = std::max(b32, 1);
+    static const LdStResident res =
+        ldst_resident(kv_copy_ldst_kernel<16, false>, kv_copy_ldst_kernel<32, false>, T);
+    const LaunchPlan p = plan_copy(a, sm_count(), res);
+    if (!p.valid) return cudaErrorInvalidValue;
+    if (p.kernel == Kernel::kTma) return launch_kv_pipe_copy(a, stream);
+    const Publish pub = publish_of(a, true, a.trace, a.debug);
+    DescParam<kParamDescs> pd;
+    if (p.param) std::memcpy(pd.d, a.descs_host, size_t(a.n) * sizeof(CopyDesc));
+    const DescParam<1> none{};
+    const auto go = [&](auto* kernel, const auto& descs_param) {
+        kernel<<<p.ctas, T, 0, stream>>>(a.descs, descs_param, a.n, a.bytes, p.chunk, p.cpb, pub);
+        return cudaGetLastError();
+    };
+    switch (p.kernel) {
+        case Kernel::kLdSt16Mc:
+            return p.param ? go(kv_copy_ldst_kernel<16, true, true>, pd)
+                           : go(kv_copy_ldst_kernel<16, false, true>, none);
+        case Kernel::kLdSt1:
+            return go(kv_copy_ldst_kernel<1, false>, none);
+        case Kernel::kLdSt32:
+            return p.param ? go(kv_copy_ldst_kernel<32, true>, pd)
+                           : go(kv_copy_ldst_kernel<32, false>, none);
+        default:
+            return p.param ? go(kv_copy_ldst_kernel<16, true>, pd)
+                           : go(kv_copy_ldst_kernel<16, false>, none);
     }
-    const int per_sm = (variant == kCopyLdSt256) ? resident32 : resident16;
-    int ctas = a.max_ctas > 0 ? a.max_ctas : per_sm * sms;
-    ctas = int(std::min<uint64_t>(uint64_t(ctas), total));
-    if (a.multicast && param)
-        kv_copy_ldst_kernel<16, true, true><<<ctas, T, 0, stream>>>(a.descs, pd, a.n, a.bytes, chunk, cpb, pub);
-    else if (a.multicast)
-        kv_copy_ldst_kernel<16, false, true><<<ctas, T, 0, stream>>>(a.descs, none, a.n, a.bytes, chunk, cpb, pub);
-    else if (!aligned16)
-        kv_copy_ldst_kernel<1, false><<<ctas, T, 0, stream>>>(a.descs, none, a.n, a.bytes, chunk, cpb, pub);
-    else if (variant == kCopyLdSt256 && param)
-        kv_copy_ldst_kernel<32, true><<<ctas, T, 0, stream>>>(a.descs, pd, a.n, a.bytes, chunk, cpb, pub);
-    else if (variant == kCopyLdSt256)
-        kv_copy_ldst_kernel<32, false><<<ctas, T, 0, stream>>>(a.descs, none, a.n, a.bytes, chunk, cpb, pub);
-    else if (param)
-        kv_copy_ldst_kernel<16, true><<<ctas, T, 0, stream>>>(a.descs, pd, a.n, a.bytes, chunk, cpb, pub);
-    else
-        kv_copy_ldst_kernel<16, false><<<ctas, T, 0, stream>>>(a.descs, none, a.n, a.bytes, chunk, cpb, pub);
-    return cudaGetLastError();
 }
 
 cudaError_t launch_kv_gather(const GatherLaunch& a, cudaStream_t stream) {
     if (a.n == 0 || a.part_bytes == 0) return cudaSuccess;
     if (a.nparts == 0 || a.nparts > kGatherMaxParts || !a.part_base) return cudaErrorInvalidValue;
     if (uint64_t(a.nparts) * a.part_bytes > 0xffffffffull) return cudaErrorInvalidValue;
-    const bool aligned16 = (a.part_bytes % 16) == 0 && (a.align_or & 15) == 0;
-    const bool aligned32 = (a.part_bytes % 32) == 0 && (a.align_or & 31) == 0;
-    // the per-part rule of launch_kv_copy: a part is what one item stream moves contiguously
-    if (aligned16 && a.part_bytes >= kPipeMinBytes) return launch_kv_pipe_gather(a, stream);
-    Publish pub{a.recs, a.table, a.table_mask, a.done, a.status, a.n, nullptr, !a.all_local, 0,
-                a.shards};
-    if (!a.write || !a.table || !a.done) pub.recs = nullptr;
-    const int sms = sm_count();
-    const uint64_t parts_total = uint64_t(a.n) * a.nparts;
-    // whole parts as items once there are as many parts as SMs (see launch_kv_copy)
-    uint32_t chunk = std::min(a.part_bytes, kLdStChunk);
-    if (parts_total >= uint64_t(sms) && a.part_bytes <= (1u << 20)) chunk = a.part_bytes;
-    const uint32_t cpp = (a.part_bytes + chunk - 1) / chunk;
-    const uint64_t total = parts_total * cpp;
-    if (total > 0x7fffffffull) return cudaErrorInvalidValue;  // the caller splits the batch
     constexpr int T = kLdStThreads + 32;
-    static int resident16 = 0, resident32 = 0;
-    if (!resident16) {
-        int b16 = 0, b32 = 0;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b16, kv_gather_ldst_kernel<16>, T, 0);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b32, kv_gather_ldst_kernel<32>, T, 0);
-        resident16 = std::max(b16, 1);
-        resident32 = std::max(b32, 1);
-    }
-    int ctas = a.max_ctas > 0 ? a.max_ctas : (aligned32 ? resident32 : resident16) * sms;
-    ctas = int(std::min<uint64_t>(uint64_t(ctas), total));
+    static const LdStResident res =
+        ldst_resident(kv_gather_ldst_kernel<16>, kv_gather_ldst_kernel<32>, T);
+    const LaunchPlan p = plan_gather(a, sm_count(), res);
+    if (!p.valid) return cudaErrorInvalidValue;  // the caller splits the batch
+    if (p.kernel == Kernel::kTma) return launch_kv_pipe_gather(a, stream);
     GatherParts parts;
     std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
-    if (!aligned16)
-        kv_gather_ldst_kernel<1><<<ctas, T, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.part_bytes,
-                                                         a.first_part, chunk, cpp, a.write, pub);
-    else if (aligned32)
-        kv_gather_ldst_kernel<32><<<ctas, T, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.part_bytes,
-                                                          a.first_part, chunk, cpp, a.write, pub);
-    else
-        kv_gather_ldst_kernel<16><<<ctas, T, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.part_bytes,
-                                                          a.first_part, chunk, cpp, a.write, pub);
-    return cudaGetLastError();
+    const auto go = [&](auto* kernel) {
+        kernel<<<p.ctas, T, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.part_bytes, a.first_part,
+                                         p.chunk, p.cpb, a.write, publish_of(a, a.write));
+        return cudaGetLastError();
+    };
+    switch (p.kernel) {
+        case Kernel::kLdSt1:
+            return go(kv_gather_ldst_kernel<1>);
+        case Kernel::kLdSt32:
+            return go(kv_gather_ldst_kernel<32>);
+        default:
+            return go(kv_gather_ldst_kernel<16>);
+    }
 }
 
 }  // namespace istore::kernels

@@ -19,10 +19,9 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
-#include <algorithm>
-
 #include "common.cuh"
 #include "kernels.h"
+#include "launch_plan.h"
 #include "publish.cuh"
 
 namespace istore::kernels {
@@ -32,7 +31,6 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 constexpr uint32_t kRow = 128;                 // elements sharing a scale
-constexpr uint32_t kChunkElems = 8192;         // CTA work item: 64 rows
 constexpr float kE4m3Max = 448.f;
 
 __device__ __forceinline__ uint2 ld_u2(const void* p) {
@@ -194,32 +192,20 @@ __global__ void __launch_bounds__(kThreads)
 cudaError_t launch_kv_write_fp8(const Fp8Launch& a, cudaStream_t stream) {
     if (a.n == 0 || a.elems == 0) return cudaSuccess;
     if (a.group != kRow || a.elems % kRow != 0) return cudaErrorInvalidValue;
-    if (a.variant != 1 && fp8_pipe_supported(a)) return launch_kv_fp8_pipe(a, true, stream);
-    Publish pub{a.recs, a.table, a.table_mask, a.done, a.status, a.n, nullptr, !a.all_local, 0,
-                a.shards};
-    if (!a.table || !a.done) pub.recs = nullptr;
-    // whole pages per CTA when there are enough of them (single-CTA commit, see kv_copy.cu)
-    uint32_t chunk = kChunkElems;
-    if (a.n >= uint32_t(sm_count()) && a.elems <= (1u << 19)) chunk = a.elems;
-    const uint32_t cpb = (a.elems + chunk - 1) / chunk;
-    const uint64_t total = uint64_t(a.n) * cpb;
-    int ctas = a.max_ctas > 0 ? a.max_ctas : 6 * sm_count();
-    ctas = int(std::min<uint64_t>(uint64_t(ctas), total));
-    kv_write_fp8_kernel<<<ctas, kThreads + 32, 0, stream>>>(a.descs, a.n, a.elems, chunk, cpb, pub);
+    const LaunchPlan p = plan_fp8(a, sm_count());
+    if (p.kernel != Kernel::kLdStFp8) return launch_kv_fp8_pipe(a, true, stream);
+    kv_write_fp8_kernel<<<p.ctas, kThreads + 32, 0, stream>>>(a.descs, a.n, a.elems, p.chunk, p.cpb,
+                                                             publish_of(a, true));
     return cudaGetLastError();
 }
 
 cudaError_t launch_kv_read_fp8(const Fp8Launch& a, cudaStream_t stream) {
     if (a.n == 0 || a.elems == 0) return cudaSuccess;
     if (a.group != kRow || a.elems % kRow != 0) return cudaErrorInvalidValue;
-    if (a.variant != 1 && fp8_pipe_supported(a)) return launch_kv_fp8_pipe(a, false, stream);
-    uint32_t chunk = kChunkElems;
-    if (a.n >= uint32_t(sm_count()) && a.elems <= (1u << 19)) chunk = a.elems;
-    const uint32_t cpb = (a.elems + chunk - 1) / chunk;
-    const uint64_t total = uint64_t(a.n) * cpb;
-    int ctas = a.max_ctas > 0 ? a.max_ctas : 6 * sm_count();
-    ctas = int(std::min<uint64_t>(uint64_t(ctas), total));
-    kv_read_fp8_kernel<<<ctas, kThreads, 0, stream>>>(a.descs, a.n, a.elems, chunk, cpb, a.status);
+    const LaunchPlan p = plan_fp8(a, sm_count());
+    if (p.kernel != Kernel::kLdStFp8) return launch_kv_fp8_pipe(a, false, stream);
+    kv_read_fp8_kernel<<<p.ctas, kThreads, 0, stream>>>(a.descs, a.n, a.elems, p.chunk, p.cpb,
+                                                        a.status);
     return cudaGetLastError();
 }
 

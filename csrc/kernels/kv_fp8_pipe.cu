@@ -23,13 +23,11 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
-#include <algorithm>
-#include <mutex>
 #include <type_traits>
 
-#include "balance.h"
 #include "common.cuh"
 #include "kernels.h"
+#include "launch_plan.h"
 #include "publish.cuh"
 #include "resolve.cuh"
 
@@ -42,6 +40,7 @@ using namespace dev;
 constexpr uint32_t kRow = 128;                  // elements sharing a scale
 constexpr uint32_t kTileRows = 64;              // rows per tile
 constexpr uint32_t kTileElems = kRow * kTileRows;
+static_assert(kTileElems == kFp8Chunk, "plan_fp8 cuts pages into whole tiles");
 constexpr uint32_t kTileBf16 = kTileElems * 2;  // 16 KB
 constexpr uint32_t kTileQ = kTileElems;         // 8 KB
 constexpr uint32_t kTileScale = kTileRows * 4;  // 256 B
@@ -256,70 +255,40 @@ __global__ void __launch_bounds__((3 + NCW) * 32)
     });
 }
 
-std::mutex g_mu;
-bool g_attr[64] = {false};
-
 constexpr size_t kSmemWrite = kInStages * kTileBf16 + kOutStages * (kTileQ + kTileScale);
 constexpr size_t kSmemRead = kInStages * (kTileQ + kTileScale) + kOutStages * kTileBf16;
 
 cudaError_t ensure_attrs() {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    std::lock_guard<std::mutex> lk(g_mu);
-    if (dev < 0 || dev >= 64 || g_attr[dev]) return cudaSuccess;
-    cudaError_t e = cudaSuccess;
-    auto set = [&](auto* fn, size_t bytes) {
-        if (e == cudaSuccess)
-            e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(bytes));
-    };
-    set(kv_fp8_pipe_kernel<true, 4, false>, kSmemWrite);
-    set(kv_fp8_pipe_kernel<true, 8, false>, kSmemWrite);
-    set(kv_fp8_pipe_kernel<false, 4, false>, kSmemRead);
-    set(kv_fp8_pipe_kernel<false, 8, false>, kSmemRead);
-    set(kv_fp8_pipe_kernel<false, 8, true>, kSmemRead);
-    if (e != cudaSuccess) return e;
-    g_attr[dev] = true;
-    return cudaSuccess;
-}
-
-Fp8Shape shape_of(const Fp8Launch& a, int ctas) {
-    // whole pages per CTA when that keeps the grid evenly busy (single-CTA commit), else
-    // chunks of at least two tiles (balance.h); never more than 512 K elements per item
-    const uint32_t tiles = (a.elems + kTileElems - 1) / kTileElems;
-    const ChunkPlan plan = plan_chunks(a.n, tiles, 2, 64, uint32_t(ctas));
-    const uint32_t chunk = std::min(a.elems, plan.chunk * kTileElems);
-    return Fp8Shape{a.n, a.elems, chunk, (a.elems + chunk - 1) / chunk};
+    static bool done[64] = {false};
+    return set_smem_limits_once(
+        done,
+        {{reinterpret_cast<const void*>(kv_fp8_pipe_kernel<true, 4, false>), int(kSmemWrite)},
+         {reinterpret_cast<const void*>(kv_fp8_pipe_kernel<true, 8, false>), int(kSmemWrite)},
+         {reinterpret_cast<const void*>(kv_fp8_pipe_kernel<false, 4, false>), int(kSmemRead)},
+         {reinterpret_cast<const void*>(kv_fp8_pipe_kernel<false, 8, false>), int(kSmemRead)},
+         {reinterpret_cast<const void*>(kv_fp8_pipe_kernel<false, 8, true>), int(kSmemRead)}});
 }
 
 }  // namespace
-
-bool fp8_pipe_supported(const Fp8Launch& a) {
-    return a.group == kRow && a.elems % 512 == 0 && a.elems > 0 && a.aligned16;
-}
 
 cudaError_t launch_kv_fp8_pipe(const Fp8Launch& a, bool write, cudaStream_t stream) {
     if (a.n == 0) return cudaSuccess;
     if (!fp8_pipe_supported(a)) return cudaErrorInvalidValue;
     cudaError_t e = ensure_attrs();
     if (e != cudaSuccess) return e;
-    Publish pub{a.recs, a.table, a.table_mask, a.done, a.status, a.n, nullptr, !a.all_local, 0,
-                a.shards};
-    if (!write || !a.table || !a.done) pub.recs = nullptr;
-    const int sms = sm_count();
-    int ctas = a.max_ctas > 0 ? std::min(a.max_ctas, 2 * sms) : 2 * sms;  // ~90 KB smem: 2 per SM
-    const Fp8Shape sh = shape_of(a, ctas);
-    ctas = int(std::min<uint64_t>(uint64_t(ctas), uint64_t(sh.n) * sh.cpb));
-    const bool wide = a.variant != 2;  // 8 compute warps unless variant 2 asks for 4 (A/B)
+    const Publish pub = publish_of(a, write);
+    const LaunchPlan p = plan_fp8_pipe(a, sm_count());
+    const Fp8Shape sh{a.n, a.elems, p.chunk, p.cpb};
     const ResolveArgs none{};
-    if (write && wide)
-        kv_fp8_pipe_kernel<true, 8, false><<<ctas, (3 + 8) * 32, kSmemWrite, stream>>>(a.descs, sh, pub, a.status, none);
-    else if (write)
-        kv_fp8_pipe_kernel<true, 4, false><<<ctas, (3 + 4) * 32, kSmemWrite, stream>>>(a.descs, sh, pub, a.status, none);
-    else if (wide)
-        kv_fp8_pipe_kernel<false, 8, false><<<ctas, (3 + 8) * 32, kSmemRead, stream>>>(a.descs, sh, pub, a.status, none);
-    else
-        kv_fp8_pipe_kernel<false, 4, false><<<ctas, (3 + 4) * 32, kSmemRead, stream>>>(a.descs, sh, pub, a.status, none);
-    return cudaGetLastError();
+    const auto go = [&](auto* kernel, int warps, size_t smem) {
+        kernel<<<p.ctas, warps * 32, smem, stream>>>(a.descs, sh, pub, a.status, none);
+        return cudaGetLastError();
+    };
+    if (write)
+        return p.kernel == Kernel::kTma4 ? go(kv_fp8_pipe_kernel<true, 4, false>, 3 + 4, kSmemWrite)
+                                         : go(kv_fp8_pipe_kernel<true, 8, false>, 3 + 8, kSmemWrite);
+    return p.kernel == Kernel::kTma4 ? go(kv_fp8_pipe_kernel<false, 4, false>, 3 + 4, kSmemRead)
+                                     : go(kv_fp8_pipe_kernel<false, 8, false>, 3 + 8, kSmemRead);
 }
 
 // read_cache_fp8 through the device index in one launch: keys -> (resolver warp) -> pool
@@ -334,29 +303,13 @@ cudaError_t launch_kv_fp8_read_fused(const ReadFusedLaunch& a, uint32_t elems, c
     if (!fp8_read_fused_supported(a, elems)) return cudaErrorInvalidValue;
     cudaError_t e = ensure_attrs();
     if (e != cudaSuccess) return e;
-    ResolveArgs r{};
-    r.key_bytes = a.key_bytes;
-    r.key_off = a.key_off;
-    r.key_len = a.key_len;
-    r.dst_off = a.dst_off;
-    r.dst_base = a.dst_base;
-    r.table = a.table;
-    r.table_mask = a.table_mask;
-    r.shards = a.shards;
-    r.nsegs = a.nsegs;
-    for (uint32_t s = 0; s < a.nsegs && s < uint32_t(ReadFusedLaunch::kMaxSegs); ++s)
-        r.seg_base[s] = a.seg_base[s];
-    r.status = a.status;
-    Fp8Launch shape_in;
-    shape_in.n = a.n;
-    shape_in.elems = elems;
-    const int sms = sm_count();
-    int ctas = a.max_ctas > 0 ? std::min(a.max_ctas, 2 * sms) : 2 * sms;
-    const Fp8Shape sh = shape_of(shape_in, ctas);
-    ctas = int(std::min<uint64_t>(uint64_t(ctas), uint64_t(sh.n) * sh.cpb));
-    Publish pub{};
-    pub.recs = nullptr;
-    kv_fp8_pipe_kernel<false, 8, true><<<ctas, (3 + 8) * 32, kSmemRead, stream>>>(nullptr, sh, pub, a.status, r);
+    Fp8Launch f;  // the shape of an fp8 pipeline read of these pages
+    f.n = a.n;
+    f.elems = elems;
+    f.max_ctas = a.max_ctas;
+    const LaunchPlan p = plan_fp8_pipe(f, sm_count());
+    kv_fp8_pipe_kernel<false, 8, true><<<p.ctas, (3 + 8) * 32, kSmemRead, stream>>>(
+        nullptr, Fp8Shape{f.n, f.elems, p.chunk, p.cpb}, Publish{}, a.status, resolve_args(a));
     return cudaGetLastError();
 }
 

@@ -33,13 +33,12 @@
 
 #include <algorithm>
 #include <cstring>
-#include <mutex>
 
 #include "../core/hash.h"
 #include "common.cuh"
 #include "index.cuh"
-#include "balance.h"
 #include "kernels.h"
+#include "launch_plan.h"
 #include "publish.cuh"
 #include "resolve.cuh"
 
@@ -49,10 +48,7 @@ namespace {
 
 using namespace dev;
 
-constexpr int kPipeMaxStages = 32;
-constexpr int kStoreLag = 2;  // bulk-store groups that may still be reading SMEM
 constexpr int kPipeThreads = 96;
-constexpr int kPipeParamDescs = 256;
 
 template <int N>
 struct PipeDescParam {
@@ -71,7 +67,7 @@ struct Shape {
 template <bool PARAM>
 struct DescWindow {
     const CopyDesc* descs;
-    const PipeDescParam<PARAM ? kPipeParamDescs : 1>* pd;
+    const PipeDescParam<PARAM ? kParamDescs : 1>* pd;
     uint32_t first, stride, cpb, nitems, lane;
     CopyDesc cur, nxt;
     uint32_t window = 0;
@@ -188,7 +184,7 @@ __device__ __forceinline__ void storer_body(const Shape& sh, uint32_t first, uin
 template <bool PARAM>
 __global__ void __launch_bounds__(kPipeThreads)
     kv_pipe_copy_kernel(const CopyDesc* __restrict__ descs,
-                        const __grid_constant__ PipeDescParam<PARAM ? kPipeParamDescs : 1> pd,
+                        const __grid_constant__ PipeDescParam<PARAM ? kParamDescs : 1> pd,
                         const Shape sh, Publish pub, const FanOut fan) {
     extern __shared__ __align__(128) uint8_t ring[];
     __shared__ __align__(8) uint64_t full[kPipeMaxStages];
@@ -596,41 +592,18 @@ __global__ void __launch_bounds__(64)
     }
 }
 
-std::mutex g_pipe_attr_mu;
-bool g_pipe_attr_set[64] = {false};
-
 cudaError_t ensure_pipe_attrs() {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    std::lock_guard<std::mutex> lk(g_pipe_attr_mu);
-    if (dev < 0 || dev >= 64 || g_pipe_attr_set[dev]) return cudaSuccess;
+    static bool done[64] = {false};
     const int kMax = 200 << 10;
-    cudaError_t e = cudaFuncSetAttribute(kv_pipe_copy_kernel<false>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, kMax);
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(kv_pipe_copy_kernel<true>,
-                                 cudaFuncAttributeMaxDynamicSharedMemorySize, kMax);
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(kv_pipe_read_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 kMax);
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(kv_pipe_gather_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 kMax);
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(kv_pipe_scatter_read_kernel,
-                                 cudaFuncAttributeMaxDynamicSharedMemorySize, kMax);
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(kv_pipe_mcast_kernel<2>,
-                                 cudaFuncAttributeMaxDynamicSharedMemorySize, kMax);
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(kv_pipe_mcast_kernel<4>,
-                                 cudaFuncAttributeMaxDynamicSharedMemorySize, kMax);
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(kv_pipe_hnd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 kMax);
-    if (e != cudaSuccess) return e;
-    g_pipe_attr_set[dev] = true;
-    return cudaSuccess;
+    return set_smem_limits_once(
+        done, {{reinterpret_cast<const void*>(kv_pipe_copy_kernel<false>), kMax},
+               {reinterpret_cast<const void*>(kv_pipe_copy_kernel<true>), kMax},
+               {reinterpret_cast<const void*>(kv_pipe_read_kernel), kMax},
+               {reinterpret_cast<const void*>(kv_pipe_gather_kernel), kMax},
+               {reinterpret_cast<const void*>(kv_pipe_scatter_read_kernel), kMax},
+               {reinterpret_cast<const void*>(kv_pipe_mcast_kernel<2>), kMax},
+               {reinterpret_cast<const void*>(kv_pipe_mcast_kernel<4>), kMax},
+               {reinterpret_cast<const void*>(kv_pipe_hnd_kernel), kMax}});
 }
 
 // cuTensorMapEncodeTiled through the runtime's driver-entry-point lookup: the module links
@@ -655,60 +628,27 @@ EncodeTiledFn encode_tiled_fn() {
 
 }  // namespace
 
-// Ring geometry: slots of up to `stage` bytes (16-byte multiple), as many as fit `ring` bytes.
-PipeGeometry pipe_geometry(uint32_t bytes, uint32_t stage_pref, uint32_t ring_pref) {
-    PipeGeometry g;
-    // 16 KB slots, 4 of them (64 KB per CTA), ONE CTA per SM per launch: a single launch then
-    // may run below the best single-kernel geometry (larger slots per CTA), but three such
-    // kernels fit an SM side by
-    // side, and that is what the API needs - the calls of a phase go round-robin over the
-    // connection's streams, and the next kernel must be able to start (descriptor fetch, index
-    // claims) while the previous one drains (store acknowledgements, system fence, commit).
-    const uint32_t stage_cap = stage_pref ? stage_pref : (16u << 10);
-    const uint32_t ring = ring_pref ? ring_pref : (64u << 10);
-    g.stage_bytes = std::min(stage_cap, (bytes + 15u) & ~15u);
-    g.stages = std::max<uint32_t>(kStoreLag + 1,
-                                  std::min<uint32_t>(kPipeMaxStages, ring / g.stage_bytes));
-    g.smem = size_t(g.stages) * g.stage_bytes;
-    return g;
-}
-
 cudaError_t launch_kv_pipe_copy(const CopyLaunch& a, cudaStream_t stream) {
     if (a.n == 0 || a.bytes == 0) return cudaSuccess;
     if ((a.bytes % 16) != 0 || (a.align_or & 15) != 0 || a.multicast) return cudaErrorInvalidValue;
     cudaError_t e = ensure_pipe_attrs();
     if (e != cudaSuccess) return e;
-    Publish pub{a.recs, a.table, a.table_mask, a.done, a.status, a.n, a.trace, !a.all_local, a.debug,
-                a.shards};
-    if (!a.table || !a.done) pub.recs = nullptr;
-    const int sms = sm_count();
-    const PipeGeometry g = pipe_geometry(a.bytes, a.stage_bytes, a.ring_bytes);
-    // One CTA per SM: the rest of the SM's shared memory is for the kernels of the connection's
-    // other streams (see pipe_geometry).  Work item: a whole block when that keeps the grid
-    // evenly busy (the commit of a block then needs no cross-CTA counter), otherwise chunks of
-    // at least four ring slots and at most 1 MB (balance.h).
-    int ctas = a.max_ctas > 0 ? std::min(a.max_ctas, sms) : sms;
-    const ChunkPlan plan = plan_chunks(a.n, (a.bytes + g.stage_bytes - 1) / g.stage_bytes, 4,
-                                       std::max(4u, (1u << 20) / g.stage_bytes), uint32_t(ctas));
-    const uint32_t chunk = std::min(a.bytes, plan.chunk * g.stage_bytes);
-    const uint32_t cpb = (a.bytes + chunk - 1) / chunk;
-    const uint64_t total = uint64_t(a.n) * cpb;
-    ctas = int(std::min<uint64_t>(uint64_t(ctas), total));
-    const Shape sh{a.n, a.bytes, chunk, cpb, g.stage_bytes, g.stages};
+    const Publish pub = publish_of(a, true, a.trace, a.debug);
     FanOut fan;
     if (a.fan_n > 1) {
         if (a.fan_n > 4 || pub.recs) return cudaErrorInvalidValue;  // reads only
         fan.n = uint32_t(a.fan_n);
         for (int r = 0; r < a.fan_n; ++r) fan.delta[r] = a.fan_delta[r];
     }
-    const bool param = a.descs_host != nullptr && a.n <= uint32_t(kPipeParamDescs);
-    if (param) {
-        PipeDescParam<kPipeParamDescs> pd;
+    const LaunchPlan p = plan_pipe_copy(a, sm_count());
+    const Shape sh{a.n, a.bytes, p.chunk, p.cpb, p.geo.stage_bytes, p.geo.stages};
+    if (p.param) {
+        PipeDescParam<kParamDescs> pd;
         std::memcpy(pd.d, a.descs_host, size_t(a.n) * sizeof(CopyDesc));
-        kv_pipe_copy_kernel<true><<<ctas, kPipeThreads, g.smem, stream>>>(a.descs, pd, sh, pub, fan);
+        kv_pipe_copy_kernel<true><<<p.ctas, kPipeThreads, p.geo.smem, stream>>>(a.descs, pd, sh, pub, fan);
     } else {
         const PipeDescParam<1> none{};
-        kv_pipe_copy_kernel<false><<<ctas, kPipeThreads, g.smem, stream>>>(a.descs, none, sh, pub, fan);
+        kv_pipe_copy_kernel<false><<<p.ctas, kPipeThreads, p.geo.smem, stream>>>(a.descs, none, sh, pub, fan);
     }
     return cudaGetLastError();
 }
@@ -720,39 +660,20 @@ cudaError_t launch_kv_pipe_gather(const GatherLaunch& a, cudaStream_t stream) {
         return cudaErrorInvalidValue;
     cudaError_t e = ensure_pipe_attrs();
     if (e != cudaSuccess) return e;
-    Publish pub{a.recs, a.table, a.table_mask, a.done, a.status, a.n, nullptr, !a.all_local, 0,
-                a.shards};
-    if (!a.write || !a.table || !a.done) pub.recs = nullptr;
-    const int sms = sm_count();
-    const PipeGeometry g = pipe_geometry(a.part_bytes, a.stage_bytes, a.ring_bytes);
-    int ctas = a.max_ctas > 0 ? std::min(a.max_ctas, sms) : sms;
-    // chunks of one part, balanced over the grid as for whole blocks (balance.h)
-    const uint64_t parts_total = uint64_t(a.n) * a.nparts;
-    if (parts_total > 0x7fffffffull) return cudaErrorInvalidValue;
-    const ChunkPlan plan = plan_chunks(uint32_t(parts_total),
-                                       (a.part_bytes + g.stage_bytes - 1) / g.stage_bytes, 4,
-                                       std::max(4u, (1u << 20) / g.stage_bytes), uint32_t(ctas));
-    const uint32_t chunk = std::min(a.part_bytes, plan.chunk * g.stage_bytes);
-    const uint32_t cpp = (a.part_bytes + chunk - 1) / chunk;
-    const uint64_t total = parts_total * cpp;
-    if (total > 0x7fffffffull) return cudaErrorInvalidValue;  // the caller splits the batch
-    ctas = int(std::min<uint64_t>(uint64_t(ctas), total));
-    const Shape sh{uint32_t(parts_total), a.part_bytes, chunk, cpp, g.stage_bytes, g.stages};
+    const LaunchPlan p = plan_pipe_gather(a, sm_count());
+    if (!p.valid) return cudaErrorInvalidValue;  // the caller splits the batch
+    const Shape sh{a.n * a.nparts, a.part_bytes, p.chunk, p.cpb, p.geo.stage_bytes, p.geo.stages};
     GatherParts parts;
     std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
-    kv_pipe_gather_kernel<<<ctas, kPipeThreads, g.smem, stream>>>(a.descs, parts, sh, a.nparts,
-                                                                  a.first_part, a.write, pub);
+    kv_pipe_gather_kernel<<<p.ctas, kPipeThreads, p.geo.smem, stream>>>(
+        a.descs, parts, sh, a.nparts, a.first_part, a.write, publish_of(a, a.write));
     return cudaGetLastError();
-}
-
-static int scatter_read_ctas(const ReadFusedLaunch& r) {
-    return r.max_ctas > 0 ? std::min(r.max_ctas, sm_count()) : sm_count();
 }
 
 bool scatter_read_fused_supported(const ReadFusedLaunch& r, const GatherLaunch& g) {
     return g.nparts >= 1 && g.nparts <= kGatherMaxParts && g.part_base && g.part_bytes &&
            (g.part_bytes % 16) == 0 && (g.align_or & 15) == 0 &&
-           r.n >= uint32_t(scatter_read_ctas(r));
+           r.n >= uint32_t(scatter_read_ctas(r, sm_count()));
 }
 
 cudaError_t launch_kv_pipe_scatter_read(const ReadFusedLaunch& r, const GatherLaunch& g,
@@ -765,31 +686,13 @@ cudaError_t launch_kv_pipe_scatter_read(const ReadFusedLaunch& r, const GatherLa
     cudaError_t e = ensure_pipe_attrs();
     if (e != cudaSuccess) return e;
     const PipeGeometry geo = pipe_geometry(g.part_bytes, r.stage_bytes, r.ring_bytes);
-    const int ctas = scatter_read_ctas(r);
-    ResolveArgs ra{};
-    ra.key_bytes = r.key_bytes;
-    ra.key_off = r.key_off;
-    ra.key_len = r.key_len;
-    ra.dst_off = r.dst_off;
-    ra.dst_base = r.dst_base;
-    ra.table = r.table;
-    ra.table_mask = r.table_mask;
-    ra.shards = r.shards;
-    ra.nsegs = r.nsegs;
-    for (uint32_t s = 0; s < r.nsegs && s < uint32_t(ReadFusedLaunch::kMaxSegs); ++s)
-        ra.seg_base[s] = r.seg_base[s];
-    ra.status = r.status;
     GatherParts parts;
     std::memcpy(parts.base, g.part_base, size_t(g.nparts) * sizeof(uint64_t));
     // whole parts as items: a CTA moves whole blocks, the ring cuts them into pieces
     const Shape sh{r.n, g.part_bytes, g.part_bytes, 1, geo.stage_bytes, geo.stages};
-    kv_pipe_scatter_read_kernel<<<ctas, kPipeThreads, geo.smem, stream>>>(ra, parts, sh, g.nparts,
-                                                                          g.first_part);
+    kv_pipe_scatter_read_kernel<<<scatter_read_ctas(r, sm_count()), kPipeThreads, geo.smem, stream>>>(
+        resolve_args(r), parts, sh, g.nparts, g.first_part);
     return cudaGetLastError();
-}
-
-bool pipe_read_supported(const ReadFusedLaunch& a) {
-    return (a.bytes % 16) == 0 && (a.align_or & 15) == 0;
 }
 
 cudaError_t launch_kv_pipe_read(const ReadFusedLaunch& a, cudaStream_t stream) {
@@ -797,29 +700,9 @@ cudaError_t launch_kv_pipe_read(const ReadFusedLaunch& a, cudaStream_t stream) {
     if (!pipe_read_supported(a)) return cudaErrorInvalidValue;
     cudaError_t e = ensure_pipe_attrs();
     if (e != cudaSuccess) return e;
-    const PipeGeometry g = pipe_geometry(a.bytes, a.stage_bytes, a.ring_bytes);
-    int ctas = a.max_ctas > 0 ? std::min(a.max_ctas, sm_count()) : sm_count();
-    // a block that is split over several CTAs is resolved by each of them (balance.h)
-    const ChunkPlan plan = plan_chunks(a.n, (a.bytes + g.stage_bytes - 1) / g.stage_bytes, 4,
-                                       std::max(4u, (1u << 20) / g.stage_bytes), uint32_t(ctas));
-    const uint32_t chunk = std::min(a.bytes, plan.chunk * g.stage_bytes);
-    const uint32_t cpb = (a.bytes + chunk - 1) / chunk;
-    ctas = int(std::min<uint64_t>(uint64_t(ctas), uint64_t(a.n) * cpb));
-    ResolveArgs r{};
-    r.key_bytes = a.key_bytes;
-    r.key_off = a.key_off;
-    r.key_len = a.key_len;
-    r.dst_off = a.dst_off;
-    r.dst_base = a.dst_base;
-    r.table = a.table;
-    r.table_mask = a.table_mask;
-    r.shards = a.shards;
-    r.nsegs = a.nsegs;
-    for (uint32_t s = 0; s < a.nsegs && s < uint32_t(ReadFusedLaunch::kMaxSegs); ++s)
-        r.seg_base[s] = a.seg_base[s];
-    r.status = a.status;
-    const Shape sh{a.n, a.bytes, chunk, cpb, g.stage_bytes, g.stages};
-    kv_pipe_read_kernel<<<ctas, kPipeThreads, g.smem, stream>>>(r, sh);
+    const LaunchPlan p = plan_pipe_read(a, sm_count());
+    const Shape sh{a.n, a.bytes, p.chunk, p.cpb, p.geo.stage_bytes, p.geo.stages};
+    kv_pipe_read_kernel<<<p.ctas, kPipeThreads, p.geo.smem, stream>>>(resolve_args(a), sh);
     return cudaGetLastError();
 }
 
@@ -867,8 +750,7 @@ cudaError_t launch_kv_pipe_hnd(const HndLaunch& a, cudaStream_t stream) {
     h.stages = stages;
     h.status = a.status;
     const size_t smem = size_t(stages) * tile_bytes;
-    int ctas = a.max_ctas > 0 ? std::min(a.max_ctas, sm_count()) : sm_count();
-    ctas = int(std::min<uint32_t>(uint32_t(ctas), a.n));
+    const int ctas = clamp_grid(capped_grid(a.max_ctas, sm_count()), a.n);
     kv_pipe_hnd_kernel<<<ctas, 64, smem, stream>>>(tmap, h);
     return cudaGetLastError();
 }
@@ -894,8 +776,8 @@ cudaError_t launch_kv_pipe_mcast(const McastLaunch& a, cudaStream_t stream) {
     m.stages = g.stages;
     for (int r = 0; r < 4; ++r) m.delta[r] = r < a.ndst ? a.delta[r] : 0;
     m.status = a.status;
-    int clusters = a.max_clusters > 0 ? a.max_clusters : sm_count() / a.ndst;
-    clusters = int(std::min<uint32_t>(uint32_t(clusters), a.n));
+    // a caller's cluster count is not bounded by the SM count
+    const int clusters = clamp_grid(a.max_clusters > 0 ? a.max_clusters : sm_count() / a.ndst, a.n);
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(unsigned(clusters * a.ndst));
     cfg.blockDim = dim3(64);

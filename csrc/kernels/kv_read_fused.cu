@@ -11,8 +11,6 @@
 // per CTA, overlapped with the copies of other CTAs and of kernels in other streams.
 // With a store that evicts (a.validate) the resolver re-checks every entry after its copy:
 // an optimistic read that reports a block evicted underneath it as a miss.
-#include <algorithm>
-
 #include "../core/hash.h"
 #include "copy_span.cuh"
 #include "index.cuh"
@@ -135,35 +133,24 @@ __global__ void __launch_bounds__(kThreads)
 
 cudaError_t launch_kv_read_fused(const ReadFusedLaunch& a, cudaStream_t stream) {
     if (a.n == 0 || a.bytes == 0) return cudaSuccess;
+    static const LdStResident res =
+        ldst_resident(kv_read_fused_kernel<16>, kv_read_fused_kernel<32>, kThreads);
+    const LaunchPlan p = plan_read_fused(a, sm_count(), res);
     // default: resolver warp + TMA pipeline (kv_pipe.cu); this file's ld/st kernel serves
     // small or unaligned pages.  Both re-check every entry after its copy.
-    if ((a.variant == kCopyTma || (a.variant == kCopyAuto && a.bytes >= kPipeMinBytes)) &&
-        pipe_read_supported(a))
-        return launch_kv_pipe_read(a, stream);
-    uint32_t chunk = std::min(a.bytes, 32u << 10);
-    if (a.n >= uint32_t(sm_count()) && a.bytes <= (1u << 20)) chunk = a.bytes;  // see kv_copy.cu
-    const uint32_t cpb = (a.bytes + chunk - 1) / chunk;
-    const uint64_t total = uint64_t(a.n) * cpb;
-    const bool aligned16 = (a.bytes % 16) == 0 && (a.align_or & 15) == 0;
-    const bool aligned32 = (a.bytes % 32) == 0 && (a.align_or & 31) == 0;
-    static int resident16 = 0, resident32 = 0;
-    if (!resident16) {
-        int b16 = 0, b32 = 0;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b16, kv_read_fused_kernel<16>, kThreads, 0);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b32, kv_read_fused_kernel<32>, kThreads, 0);
-        resident16 = std::max(b16, 1);
-        resident32 = std::max(b32, 1);
+    if (p.kernel == Kernel::kTma) return launch_kv_pipe_read(a, stream);
+    const auto go = [&](auto* kernel) {
+        kernel<<<p.ctas, kThreads, 0, stream>>>(a, p.chunk, p.cpb);
+        return cudaGetLastError();
+    };
+    switch (p.kernel) {
+        case Kernel::kLdSt1:
+            return go(kv_read_fused_kernel<1>);
+        case Kernel::kLdSt32:
+            return go(kv_read_fused_kernel<32>);
+        default:
+            return go(kv_read_fused_kernel<16>);
     }
-    const int per_sm = aligned32 ? resident32 : resident16;
-    int ctas = a.max_ctas > 0 ? a.max_ctas : per_sm * sm_count();
-    ctas = int(std::min<uint64_t>(uint64_t(ctas), total));
-    if (!aligned16)
-        kv_read_fused_kernel<1><<<ctas, kThreads, 0, stream>>>(a, chunk, cpb);
-    else if (aligned32)
-        kv_read_fused_kernel<32><<<ctas, kThreads, 0, stream>>>(a, chunk, cpb);
-    else
-        kv_read_fused_kernel<16><<<ctas, kThreads, 0, stream>>>(a, chunk, cpb);
-    return cudaGetLastError();
 }
 
 }  // namespace istore::kernels

@@ -40,6 +40,15 @@ struct Publish {
     IndexShards shards;  // further index shards (shard 0 = table / mask)
 };
 
+// The commit of a launch (CopyLaunch, GatherLaunch, Fp8Launch): none (recs = nullptr) unless
+// the launch writes and carries an index table and scratch.
+template <typename Launch>
+inline Publish publish_of(const Launch& a, bool write, unsigned long long* trace = nullptr,
+                          uint32_t debug = 0) {
+    return Publish{write && a.table && a.done ? a.recs : nullptr, a.table, a.table_mask, a.done,
+                   a.status, a.n, trace, !a.all_local, debug, a.shards};
+}
+
 __device__ inline unsigned long long globaltimer_ns() {
     unsigned long long t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));

@@ -36,6 +36,23 @@ struct ResolveArgs {
     uint32_t* status;
 };
 
+inline ResolveArgs resolve_args(const ReadFusedLaunch& a) {
+    ResolveArgs r{};
+    r.key_bytes = a.key_bytes;
+    r.key_off = a.key_off;
+    r.key_len = a.key_len;
+    r.dst_off = a.dst_off;
+    r.dst_base = a.dst_base;
+    r.table = a.table;
+    r.table_mask = a.table_mask;
+    r.shards = a.shards;
+    r.nsegs = a.nsegs;
+    for (uint32_t s = 0; s < a.nsegs && s < uint32_t(ReadFusedLaunch::kMaxSegs); ++s)
+        r.seg_base[s] = a.seg_base[s];
+    r.status = a.status;
+    return r;
+}
+
 constexpr int kResolveBatch = 32;  // descriptors per queue half: one per resolver lane
 
 struct ResolveQueue {

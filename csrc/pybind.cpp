@@ -37,6 +37,7 @@
 #include "fabric/segment.h"
 #include "kernels/balance.h"
 #include "kernels/kernels.h"
+#include "kernels/launch_plan.h"
 #include "wire/messages.h"
 
 namespace py = pybind11;
@@ -1305,13 +1306,100 @@ PYBIND11_MODULE(_infinistore, m) {
               d["path"] = kPaths[int(p.path)];
               d["variant"] = p.variant;
               d["grid_cap"] = p.grid_cap;
-              d["ldst_align"] = p.ldst_align;
               return d;
           },
           py::arg("n"), py::arg("block_bytes"), py::arg("fp8_elems") = 0, py::arg("gather") = false,
           py::arg("fp8_fused_ok") = false, py::arg("scatter_fused_ok") = false,
           py::arg("copy_variant") = 0, py::arg("all_local") = false, py::arg("all_remote") = false,
           py::arg("max_ctas") = 0, py::arg("sm_count") = 132);
+    // which kernel a page-mover launcher runs, its work split and grid (kernels/launch_plan.h);
+    // the resident CTAs per SM of the ld/st kernels are the occupancy API's answer on a GPU
+    const auto plan_dict = [](const kernels::LaunchPlan& p) {
+        static const char* const kKernels[] = {"ldst1", "ldst16", "ldst32",  "ldst16_mc",
+                                               "tma",   "tma4",   "ldst_fp8"};
+        py::dict d;
+        d["valid"] = p.valid;
+        d["kernel"] = kKernels[int(p.kernel)];
+        d["param"] = p.param;
+        d["chunk"] = p.chunk;
+        d["cpb"] = p.cpb;
+        d["ctas"] = p.ctas;
+        d["stage_bytes"] = p.geo.stage_bytes;
+        d["stages"] = p.geo.stages;
+        d["smem"] = p.geo.smem;
+        return d;
+    };
+    static const kernels::CopyDesc kHostDescs[1] = {};  // plan_copy only asks whether there are any
+    t.def("plan_copy",
+          [plan_dict](uint32_t n, uint32_t bytes, uint64_t align_or, int variant, bool multicast,
+                      bool descs_host, int max_ctas, uint32_t stage_bytes, uint32_t ring_bytes,
+                      int sm_count, int resident16, int resident32) {
+              kernels::CopyLaunch a;
+              a.n = n;
+              a.bytes = bytes;
+              a.align_or = align_or;
+              a.variant = variant;
+              a.multicast = multicast;
+              a.descs_host = descs_host ? kHostDescs : nullptr;
+              a.max_ctas = max_ctas;
+              a.stage_bytes = stage_bytes;
+              a.ring_bytes = ring_bytes;
+              return plan_dict(kernels::plan_copy(a, sm_count, {resident16, resident32}));
+          },
+          py::arg("n"), py::arg("bytes"), py::arg("align_or") = 0, py::arg("variant") = 0,
+          py::arg("multicast") = false, py::arg("descs_host") = false, py::arg("max_ctas") = 0,
+          py::arg("stage_bytes") = 0, py::arg("ring_bytes") = 0, py::arg("sm_count") = 132,
+          py::arg("resident16") = 1, py::arg("resident32") = 1);
+    t.def("plan_gather",
+          [plan_dict](uint32_t n, uint32_t nparts, uint32_t part_bytes, uint64_t align_or,
+                      int max_ctas, uint32_t stage_bytes, uint32_t ring_bytes, int sm_count,
+                      int resident16, int resident32) {
+              kernels::GatherLaunch a;
+              a.n = n;
+              a.nparts = nparts;
+              a.part_bytes = part_bytes;
+              a.align_or = align_or;
+              a.max_ctas = max_ctas;
+              a.stage_bytes = stage_bytes;
+              a.ring_bytes = ring_bytes;
+              return plan_dict(kernels::plan_gather(a, sm_count, {resident16, resident32}));
+          },
+          py::arg("n"), py::arg("nparts"), py::arg("part_bytes"), py::arg("align_or") = 0,
+          py::arg("max_ctas") = 0, py::arg("stage_bytes") = 0, py::arg("ring_bytes") = 0,
+          py::arg("sm_count") = 132, py::arg("resident16") = 1, py::arg("resident32") = 1);
+    t.def("plan_read_fused",
+          [plan_dict](uint32_t n, uint32_t bytes, uint64_t align_or, int variant, int max_ctas,
+                      uint32_t stage_bytes, uint32_t ring_bytes, int sm_count, int resident16,
+                      int resident32) {
+              kernels::ReadFusedLaunch a;
+              a.n = n;
+              a.bytes = bytes;
+              a.align_or = align_or;
+              a.variant = variant;
+              a.max_ctas = max_ctas;
+              a.stage_bytes = stage_bytes;
+              a.ring_bytes = ring_bytes;
+              py::dict d = plan_dict(kernels::plan_read_fused(a, sm_count, {resident16, resident32}));
+              d["scatter_ctas"] = kernels::scatter_read_ctas(a, sm_count);
+              return d;
+          },
+          py::arg("n"), py::arg("bytes"), py::arg("align_or") = 0, py::arg("variant") = 0,
+          py::arg("max_ctas") = 0, py::arg("stage_bytes") = 0, py::arg("ring_bytes") = 0,
+          py::arg("sm_count") = 132, py::arg("resident16") = 1, py::arg("resident32") = 1);
+    t.def("plan_fp8",
+          [plan_dict](uint32_t n, uint32_t elems, int variant, bool aligned16, uint32_t group,
+                      int max_ctas, int sm_count) {
+              kernels::Fp8Launch a;
+              a.n = n;
+              a.elems = elems;
+              a.variant = variant;
+              a.aligned16 = aligned16;
+              a.group = group;
+              a.max_ctas = max_ctas;
+              return plan_dict(kernels::plan_fp8(a, sm_count));
+          },
+          py::arg("n"), py::arg("elems"), py::arg("variant") = 0, py::arg("aligned16") = true,
+          py::arg("group") = 128, py::arg("max_ctas") = 0, py::arg("sm_count") = 132);
     py::class_<MM>(t, "MM")
         .def(py::init<>())
         .def("add_pool", &MM::add_pool)

@@ -13,90 +13,90 @@ SMS = 132
 KB, MB = 1 << 10, 1 << 20
 FP8_PAGE = 8192 + 4 * 8192 // 128  # bytes of an fp8 page of 8192 elements: e4m3 + scales
 
-# (case, plan_device_read arguments, expected (path, variant, grid_cap, ldst_align));
+# (case, plan_device_read arguments, expected (path, variant, grid_cap));
 # variant None: the path runs no launch that takes one
 CASES = [
     ("small batch, local", dict(n=16, block_bytes=64 * KB, all_local=True),
-     ("fused_copy", LDST256, 0, False)),
+     ("fused_copy", LDST256, 0)),
     ("small batch over NVLink", dict(n=16, block_bytes=64 * KB, all_remote=True),
-     ("fused_copy", LDST256, 2 * SMS, False)),
+     ("fused_copy", LDST256, 2 * SMS)),
+    # an ldst connection reads fused copies with the 16-byte ld/st kernel
     ("small batch, ldst", dict(n=4, block_bytes=64 * KB, copy_variant=LDST, all_local=True),
-     ("fused_copy", LDST256, 0, True)),
+     ("fused_copy", LDST, 0)),
     ("whole blocks, auto, local", dict(n=2048, block_bytes=128 * KB, all_local=True),
-     ("fused_copy", LDST256, 0, False)),
+     ("fused_copy", LDST256, 0)),
     ("whole blocks, auto, over NVLink", dict(n=2048, block_bytes=128 * KB, all_remote=True),
-     ("fused_copy", AUTO, 2 * SMS, False)),
+     ("fused_copy", AUTO, 2 * SMS)),
     ("whole blocks, auto, mixed pool", dict(n=2048, block_bytes=128 * KB),
-     ("fused_copy", AUTO, 0, False)),
+     ("fused_copy", AUTO, 0)),
     ("whole blocks, tma, local", dict(n=2048, block_bytes=128 * KB, copy_variant=TMA,
                                       all_local=True),
-     ("fused_copy", TMA, 0, False)),
+     ("fused_copy", TMA, 0)),
     ("whole blocks, tma, over NVLink", dict(n=2048, block_bytes=128 * KB, copy_variant=TMA,
                                             all_remote=True),
-     ("fused_copy", TMA, 2 * SMS, False)),
+     ("fused_copy", TMA, 2 * SMS)),
     ("whole blocks, ldst, local", dict(n=2048, block_bytes=128 * KB, copy_variant=LDST,
                                        all_local=True),
-     ("fused_copy", LDST, 0, True)),
+     ("fused_copy", LDST, 0)),
     ("whole blocks, max_ctas", dict(n=2048, block_bytes=128 * KB, all_remote=True, max_ctas=8),
-     ("fused_copy", AUTO, 8, False)),
+     ("fused_copy", AUTO, 8)),
     ("large blocks, local", dict(n=8, block_bytes=2 * MB, all_local=True),
-     ("lookup_copy", LDST256, 0, False)),
+     ("lookup_copy", LDST256, 0)),
     ("large blocks, ldst", dict(n=8, block_bytes=2 * MB, copy_variant=LDST, all_local=True),
-     ("lookup_copy", LDST, 0, False)),
+     ("lookup_copy", LDST, 0)),
     ("few blocks above 4 MB, over NVLink", dict(n=16, block_bytes=512 * KB, all_remote=True),
-     ("lookup_copy", AUTO, 2 * SMS, False)),
+     ("lookup_copy", AUTO, 2 * SMS)),
     ("large blocks, tma, max_ctas", dict(n=8, block_bytes=2 * MB, copy_variant=TMA,
                                          all_local=True, max_ctas=20),
-     ("lookup_copy", TMA, 20, False)),
+     ("lookup_copy", TMA, 20)),
     ("fp8 fused, local", dict(n=512, block_bytes=FP8_PAGE, fp8_elems=8192, fp8_fused_ok=True,
                               all_local=True),
-     ("fused_fp8", LDST256, 0, False)),
+     ("fused_fp8", LDST256, 0)),
     ("fp8 fused, small batch", dict(n=4, block_bytes=FP8_PAGE, fp8_elems=8192,
                                     fp8_fused_ok=True, all_remote=True),
-     ("fused_fp8", LDST256, SMS, False)),
+     ("fused_fp8", LDST256, SMS)),
     ("fp8 fused over NVLink", dict(n=512, block_bytes=FP8_PAGE, fp8_elems=8192,
                                    fp8_fused_ok=True, all_remote=True),
-     ("fused_fp8", AUTO, SMS, False)),
+     ("fused_fp8", AUTO, SMS)),
     ("fp8 unfused, local", dict(n=512, block_bytes=FP8_PAGE, fp8_elems=8192, all_local=True),
-     ("lookup_fp8", 1, 0, False)),
+     ("lookup_fp8", 1, 0)),
     ("fp8 unfused over NVLink", dict(n=512, block_bytes=FP8_PAGE, fp8_elems=8192,
                                      all_remote=True),
-     ("lookup_fp8", 0, SMS, False)),
+     ("lookup_fp8", 0, SMS)),
     # not move_blocks' rule (all_local ? 1 : 0): a mixed pool reads with the ld/st kernels
     ("fp8 unfused, mixed pool", dict(n=512, block_bytes=FP8_PAGE, fp8_elems=8192),
-     ("lookup_fp8", 1, 0, False)),
+     ("lookup_fp8", 1, 0)),
     ("fp8 unfused, small batch", dict(n=4, block_bytes=FP8_PAGE, fp8_elems=8192,
                                       all_local=True),
-     ("lookup_fp8", 1, 0, False)),
+     ("lookup_fp8", 1, 0)),
     ("gathered, fused, local", dict(n=2048, block_bytes=64 * 32 * KB, gather=True,
                                     scatter_fused_ok=True, all_local=True),
-     ("fused_scatter", LDST256, 0, False)),
+     ("fused_scatter", LDST256, 0)),
     ("gathered, fused, small batch, ldst", dict(n=132, block_bytes=8 * KB, gather=True,
                                                 scatter_fused_ok=True, copy_variant=LDST),
-     ("fused_scatter", LDST256, 0, True)),
+     ("fused_scatter", LDST256, 0)),
     ("gathered, fused, over NVLink", dict(n=2048, block_bytes=64 * 32 * KB, gather=True,
                                           scatter_fused_ok=True, all_remote=True),
-     ("fused_scatter", AUTO, 2 * SMS, False)),
+     ("fused_scatter", AUTO, 2 * SMS)),
     ("gathered, unfused", dict(n=16, block_bytes=64 * 32 * KB, gather=True, all_local=True),
-     ("lookup_gather", None, 0, False)),
+     ("lookup_gather", None, 0)),
     ("gathered, unfused over NVLink", dict(n=16, block_bytes=MB, gather=True, all_remote=True),
-     ("lookup_gather", None, 2 * SMS, False)),
+     ("lookup_gather", None, 2 * SMS)),
     # a gathered read never takes the fp8 or plain copy paths
     ("gathered, small batch, unfused", dict(n=4, block_bytes=8 * KB, gather=True,
                                             fp8_fused_ok=True),
-     ("lookup_gather", None, 0, False)),
+     ("lookup_gather", None, 0)),
 ]
 
 
 @pytest.mark.parametrize("case,kw,want", CASES, ids=[c[0] for c in CASES])
-def test_plan_device_read(case, kw, want):
+def test_device_read_plans(case, kw, want):
     p = T.plan_device_read(sm_count=SMS, **kw)
-    path, variant, grid_cap, ldst_align = want
+    path, variant, grid_cap = want
     assert p["path"] == path
     if variant is not None:
         assert p["variant"] == variant
     assert p["grid_cap"] == grid_cap
-    assert p["ldst_align"] == ldst_align
 
 
 def test_every_path_is_covered():
