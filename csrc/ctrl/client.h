@@ -182,7 +182,7 @@ class Connection {
     struct GatherSpec {
         const uint64_t* part_base = nullptr;  // absolute addresses, all on `device` (or host)
         uint32_t nparts = 0;
-        uint32_t part_bytes = 0;
+        uint32_t part_bytes = 0;  // pool bytes of a part (fp8: fp8_gather_bytes(1, elems))
         uint32_t first_part = 0;  // reads: stored part first_part + s lands in part s
     };
     // offsets in bytes; blocks allocated with nparts * part_bytes bytes (trusted)
@@ -191,6 +191,17 @@ class Connection {
     // a stored block must hold (first_part + nparts) * part_bytes bytes, else it is a miss
     int r_rdma_scatter(const GatherSpec& g, const std::vector<KeyOffset>& blocks, int device,
                        uint64_t stream);
+    // Gathered fp8 blocks: every part is a bf16 page of `elems` elements (a multiple of 512) in
+    // the caller's CUDA tensors and an fp8 page in the pool, part s at byte
+    // kernels::fp8_gather_bytes(s, elems) of the block (g.part_bytes is not read).  Blocks are
+    // allocated with fp8_gather_bytes(nparts, elems) bytes; a stored block must hold
+    // fp8_gather_bytes(first_part + nparts, elems) bytes, else it is a miss.  Part bases and
+    // offsets must be 16-byte aligned.
+    int w_rdma_gather_fp8(const GatherSpec& g, int elems, const uint64_t* offsets,
+                          size_t noffsets, const RemoteBlock* blocks, size_t nblocks, int device,
+                          uint64_t stream);
+    int r_rdma_scatter_fp8(const GatherSpec& g, int elems, const std::vector<KeyOffset>& blocks,
+                           int device, uint64_t stream);
 
     // --- async flavours: the callback runs on the connection's completion thread
     int allocate_async(const std::vector<std::string>& keys, int block_size,

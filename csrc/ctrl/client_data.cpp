@@ -268,6 +268,13 @@ kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n,
     return G;
 }
 
+// Blocks per launch of a gathered call (staging.h: gather_max_blocks).  fp8 parts are counted
+// in bf16 bytes: the fp8 kernels cut a part into chunks of at least kFp8Chunk elements (16 KB
+// of bf16), or take it whole.
+static size_t gather_batch_cap(const Connection::GatherSpec& g, int fp8_elems) {
+    return gather_max_blocks(kMaxBatch, g.nparts, fp8_elems ? 2 * uint32_t(fp8_elems) : g.part_bytes);
+}
+
 // The blocks of blocks[base, ...) that the next launch stages (staging.h: key_batch) within
 // half the ring, so that a launch's placements never come round to each other.  *packed is
 // kept only when it covers the call and the call fits in one launch.  n == 0: one key is
@@ -413,8 +420,7 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
         }
     }
 
-    const size_t max_batch =
-        gather ? gather_max_blocks(kMaxBatch, gather->nparts, gather->part_bytes) : kMaxBatch;
+    const size_t max_batch = gather ? gather_batch_cap(*gather, fp8_elems) : kMaxBatch;
     size_t i = 0;
     while (i < n) {
         const uint64_t t_build0 = now_ns();
@@ -522,7 +528,12 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
             G.done = L.done;
             G.all_local = L.all_local;
             G.shards = L.shards;
-            e = kernels::launch_kv_gather(G, scope.stream);
+            // fp8 parts: the variant rule of the per-page fp8 path below
+            e = fp8_elems ? kernels::launch_kv_gather_fp8(G, uint32_t(fp8_elems),
+                                                          all_local ? kernels::kFp8LdSt
+                                                                    : kernels::kFp8Auto,
+                                                          scope.stream)
+                          : kernels::launch_kv_gather(G, scope.stream);
         } else if (fp8_elems) {
             kernels::Fp8Launch F;
             F.descs = L.descs;
@@ -647,6 +658,54 @@ int Connection::r_rdma_scatter(const GatherSpec& g, const std::vector<KeyOffset>
                        nullptr, nullptr, &g);
 }
 
+// Gathered fp8 blocks: the checks a launch would fail, made before anything is enqueued.
+static bool gather_fp8_ok(const Connection::GatherSpec& g, int elems, const uint64_t* offs,
+                          size_t n, uint64_t first_part) {
+    if (elems <= 0 || elems % 512 || !g.part_base || g.nparts < 1 ||
+        g.nparts > kernels::kGatherMaxParts ||
+        kernels::fp8_gather_bytes(uint32_t(first_part + g.nparts), uint32_t(elems)) >
+            uint64_t(INT32_MAX))
+        return false;
+    uint64_t align_or = 0;
+    for (uint32_t s = 0; s < g.nparts; ++s) align_or |= g.part_base[s];
+    for (size_t i = 0; i < n; ++i) align_or |= offs[i];
+    return (align_or & 15) == 0;
+}
+
+int Connection::w_rdma_gather_fp8(const GatherSpec& g, int elems, const uint64_t* offsets,
+                                  size_t noffsets, const RemoteBlock* blocks, size_t nblocks,
+                                  int device, uint64_t stream) {
+    if (noffsets != nblocks || device < 0 || !gather_fp8_ok(g, elems, offsets, noffsets, 0)) {
+        fail("w_rdma_gather_fp8: needs CUDA tensors, parts of a multiple of 512 elements, "
+             "16-byte aligned part bases and offsets, and one offset per remote block");
+        return -1;
+    }
+    GatherSpec w = g;
+    w.part_bytes = uint32_t(kernels::fp8_gather_bytes(1, uint32_t(elems)));
+    w.first_part = 0;
+    return move_blocks(true, offsets, 1, blocks, nblocks,
+                       int(kernels::fp8_gather_bytes(g.nparts, uint32_t(elems))), 0, device,
+                       stream, elems, nullptr, &w);
+}
+
+int Connection::r_rdma_scatter_fp8(const GatherSpec& g, int elems,
+                                   const std::vector<KeyOffset>& blocks, int device,
+                                   uint64_t stream) {
+    if (blocks.empty()) return 0;
+    std::vector<uint64_t> offs(blocks.size());
+    for (size_t i = 0; i < blocks.size(); ++i) offs[i] = blocks[i].offset;
+    if (device < 0 || !gather_fp8_ok(g, elems, offs.data(), offs.size(), g.first_part)) {
+        fail("r_rdma_scatter_fp8: needs CUDA tensors, parts of a multiple of 512 elements and "
+             "16-byte aligned part bases and offsets");
+        return -1;
+    }
+    GatherSpec r = g;
+    r.part_bytes = uint32_t(kernels::fp8_gather_bytes(1, uint32_t(elems)));
+    return read_blocks(kOpReadLookup, blocks,
+                       int(kernels::fp8_gather_bytes(g.nparts, uint32_t(elems))), 0, device,
+                       stream, elems, nullptr, nullptr, &r);
+}
+
 int Connection::rw_local(char op, const std::vector<KeyOffset>& blocks, int block_size,
                          uint64_t base_ptr, int device, uint64_t stream) {
     if (blocks.empty()) return 0;
@@ -697,8 +756,7 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
         return 0;
     }
     if (scope.begin(stream_in, false) != 0) return -1;
-    const size_t max_batch =
-        gather ? gather_max_blocks(kMaxBatch, gather->nparts, gather->part_bytes) : kMaxBatch;
+    const size_t max_batch = gather ? gather_batch_cap(*gather, fp8_elems) : kMaxBatch;
     KeyBatch b;
     for (size_t base = 0; base < blocks.size(); base += b.n) {
         const uint64_t t_build0 = now_ns();
@@ -767,6 +825,10 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
             if (plan.path == ReadPath::kLookupGather) {
                 G.descs = descs;  // {pool address or 0, local byte offset} (dst_base 0)
                 e = kernels::launch_kv_gather(G, scope.stream);
+            } else if (plan.path == ReadPath::kLookupGatherFp8) {
+                G.descs = descs;
+                e = kernels::launch_kv_gather_fp8(G, uint32_t(fp8_elems), plan.variant,
+                                                  scope.stream);
             } else if (plan.path == ReadPath::kLookupFp8) {
                 kernels::Fp8Launch F;
                 F.descs = descs;

@@ -29,11 +29,12 @@ enum class ReadPath {
     kLookupCopy,    // index_lookup, kv_copy, index_validate
     kLookupFp8,     // index_lookup, kv_read_fp8, index_validate
     kLookupGather,  // index_lookup, kv_gather, index_validate
+    kLookupGatherFp8,  // index_lookup, kv_gather_fp8, index_validate
 };
 
 struct DeviceReadPlan {
     ReadPath path = ReadPath::kLookupCopy;
-    int variant = kernels::kCopyAuto;  // of the launch that moves the pages (unused by gathers)
+    int variant = kernels::kCopyAuto;  // of the launch that moves the pages (unused by bf16 gathers)
     int grid_cap = 0;                  // max_ctas of every launch
     bool fused() const { return path <= ReadPath::kFusedScatter; }
 };
@@ -70,16 +71,20 @@ inline DeviceReadPlan plan_device_read(const DeviceReadIn& in) {
     // every CTA has a block of its own; fewer blocks: lookup + gather + validate.
     // fp8 pages: the resolver rides in the dequantising TMA pipeline (one launch instead of
     // lookup + read + validate: 32 calls of 512 pages were launch-bound).
-    if (in.gather)
+    // gathered fp8 blocks: each key is probed once by the lookup kernel and re-checked after the
+    // dequantising scatter; never the bf16 scatter pipeline.
+    if (in.gather && in.fp8_elems)
+        p.path = ReadPath::kLookupGatherFp8;
+    else if (in.gather)
         p.path = in.scatter_fused_ok ? ReadPath::kFusedScatter : ReadPath::kLookupGather;
     else if (in.fp8_elems)
         p.path = in.fp8_fused_ok ? ReadPath::kFusedFp8 : ReadPath::kLookupFp8;
     else
         p.path = whole_blocks || small_batch ? ReadPath::kFusedCopy : ReadPath::kLookupCopy;
-    // lookup then fp8: the TMA pipeline when every segment is remote, the ld/st kernels
-    // otherwise.  Intentional: move_blocks' rule is all_local ? ld/st : TMA, and the two differ
-    // for a pool that mixes local and remote segments.
-    if (p.path == ReadPath::kLookupFp8)
+    // lookup then fp8 (per-page or gathered): the TMA pipeline when every segment is remote,
+    // the ld/st kernels otherwise.  Intentional: move_blocks' rule is all_local ? ld/st : TMA,
+    // and the two differ for a pool that mixes local and remote segments.
+    if (p.path == ReadPath::kLookupFp8 || p.path == ReadPath::kLookupGatherFp8)
         p.variant = in.all_remote ? kernels::kFp8Auto : kernels::kFp8LdSt;
     else if (p.path == ReadPath::kFusedCopy && in.copy_variant == kernels::kCopyLdSt)
         p.variant = kernels::kCopyLdSt;  // the 16-byte ld/st read kernel (launch_plan.h)

@@ -208,8 +208,24 @@ cudaError_t launch_kv_fp8_pipe(const Fp8Launch& a, bool write, cudaStream_t stre
 inline uint32_t fp8_block_bytes(uint32_t elems, uint32_t group) {
     return elems + 4u * (elems / group);
 }
+// Gathered fp8 blocks: nparts quantised pages end to end, part s at byte
+// fp8_gather_bytes(s, elems) of the block; fp8_gather_bytes(nparts, elems) is the block's size
+// (Llama-3-8B, 16-token pages: 64 parts of 16384 elements = 1,081,344 bytes).  elems % 512 == 0
+// keeps every part 16-byte aligned inside a granule-aligned block.
+inline uint64_t fp8_gather_bytes(uint32_t nparts, uint32_t elems) {
+    return uint64_t(nparts) * fp8_block_bytes(elems, 128);
+}
 cudaError_t launch_kv_write_fp8(const Fp8Launch& a, cudaStream_t stream);
 cudaError_t launch_kv_read_fp8(const Fp8Launch& a, cudaStream_t stream);
+// The gathered form of the two above: each part of a GatherLaunch is a bf16 page of `elems`
+// elements (a multiple of 512; part_bytes is not read) at part_base[s] + the block's local
+// offset, and each is quantised into / dequantised from its own fp8 page of the pool block.
+// Every part of a block is byte-identical to the block launch_kv_write_fp8 stores for that
+// page.  variant kFp8LdSt: the ld/st kernels (kv_fp8.cu), anything else: the TMA pipeline with
+// 8 compute warps (kv_fp8_pipe.cu).  Part bases and local offsets must be 16-byte aligned.
+cudaError_t launch_kv_gather_fp8(const GatherLaunch& a, uint32_t elems, int variant,
+                                 cudaStream_t stream);
+cudaError_t launch_kv_fp8_pipe_gather(const GatherLaunch& a, uint32_t elems, cudaStream_t stream);
 
 // Device-side key lookup: hash the packed key bytes, probe the index, and either build
 // copy descriptors for a following kv_copy (read path) or produce a presence bitmap and

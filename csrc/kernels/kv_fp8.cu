@@ -7,6 +7,8 @@
 //                  block, then the in-band commit.  Half the NVLink bytes of a bf16 write and
 //                  no separate cast kernel / staging buffer.
 //   kv_read_fp8  : pool block -> dequantised bf16 scattered into the destination pages.
+//   kv_write_fp8_gather / kv_read_fp8_scatter : the same for gathered blocks, whose parts are
+//                  fp8 pages end to end (launch_kv_gather_fp8, fp8_pages.cuh).
 // The reference moves raw bytes only (dtype-agnostic, infinistore/lib.py:377-379); this is
 // the "write fused with fp8 cast / read fused with gather" item of the north star.
 //
@@ -19,7 +21,10 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
+#include <cstring>
+
 #include "common.cuh"
+#include "fp8_pages.cuh"
 #include "kernels.h"
 #include "launch_plan.h"
 #include "publish.cuh"
@@ -73,10 +78,13 @@ __device__ __forceinline__ uint4 ld_u4(const void* p) {
     return r;
 }
 
-// Threads [0, 256) quantise + store; warp 8 is the control warp (in-band commit).
-__global__ void __launch_bounds__(kThreads + 32)
-    kv_write_fp8_kernel(const CopyDesc* __restrict__ descs, uint32_t n, uint32_t elems,
-                        uint32_t chunk, uint32_t cpb, Publish pub) {
+// Threads [0, 256) quantise + store; warp 8 is the control warp (in-band commit).  Work item
+// k is chunk k % cpp of page k / cpp (`pages`, fp8_pages.cuh); n blocks of pages.nparts pages.
+template <typename Pages>
+__device__ __forceinline__ void write_fp8(const CopyDesc* __restrict__ descs, uint32_t n,
+                                          uint32_t elems, uint32_t chunk, uint32_t cpp,
+                                          const Publish& pub, const Pages& pages) {
+    const uint32_t cpb = cpp * pages.nparts;  // items per block: what the commit counts
     const uint32_t total = n * cpb;
     if (threadIdx.x >= kThreads) {
         if (!pub.recs) return;
@@ -88,8 +96,8 @@ __global__ void __launch_bounds__(kThreads + 32)
     const uint32_t half = lane >> 4, hl = lane & 15;
     constexpr uint32_t kStep = 2 * kRowPairs;  // rows per warp iteration
     for (uint32_t item = blockIdx.x; item < total; item += gridDim.x) {
-        const CopyDesc d = descs[item / cpb];
-        const uint32_t e0 = (item % cpb) * chunk;
+        const CopyDesc d = pages.at(descs, item / cpp);
+        const uint32_t e0 = (item % cpp) * chunk;
         const uint32_t rows = min(chunk, elems - e0) / kRow;
         const uint32_t row0 = e0 / kRow;
         const uint8_t* src = reinterpret_cast<const uint8_t*>(d.src);  // bf16 page
@@ -135,6 +143,30 @@ __global__ void __launch_bounds__(kThreads + 32)
     if (pub.recs) ctrl_barrier_arrive(kThreads + 32);
 }
 
+// Lane hl of the half-warp that owns a row: its 8 e4m3 values (v) times the row's scale, as
+// 8 bf16 (one 16-byte store).  Dequantisation goes through f16x2.
+__device__ __forceinline__ uint4 dequant8(uint2 v, float sc) {
+    const uint32_t w[2] = {v.x, v.y};
+    uint32_t o[4];
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+        const uint32_t h01 = cvt_f16x2_e4m3x2(uint16_t(w[j] & 0xffffu));
+        const uint32_t h23 = cvt_f16x2_e4m3x2(uint16_t(w[j] >> 16));
+        const float2 f01 = __half22float2(*reinterpret_cast<const __half2*>(&h01));
+        const float2 f23 = __half22float2(*reinterpret_cast<const __half2*>(&h23));
+        o[2 * j] = f2_to_bf16x2(f01.x * sc, f01.y * sc);
+        o[2 * j + 1] = f2_to_bf16x2(f23.x * sc, f23.y * sc);
+    }
+    return make_uint4(o[0], o[1], o[2], o[3]);
+}
+
+__global__ void __launch_bounds__(kThreads + 32)
+    kv_write_fp8_kernel(const CopyDesc* __restrict__ descs, uint32_t n, uint32_t elems,
+                        uint32_t chunk, uint32_t cpb, Publish pub) {
+    write_fp8(descs, n, elems, chunk, cpb, pub, OnePage{});
+}
+
+// A missing block (src == 0) counts once in status[kStatMiss]; its page is not written.
 __global__ void __launch_bounds__(kThreads)
     kv_read_fp8_kernel(const CopyDesc* __restrict__ descs, uint32_t n, uint32_t elems,
                        uint32_t chunk, uint32_t cpb, uint32_t* status) {
@@ -169,19 +201,66 @@ __global__ void __launch_bounds__(kThreads)
             for (int u = 0; u < kRowPairs; ++u) {
                 const uint32_t r = r0 + 2 * u + half;
                 if (r >= rows) continue;
-                const uint32_t w[2] = {v[u].x, v[u].y};
-                uint32_t o[4];
-#pragma unroll
-                for (int j = 0; j < 2; ++j) {
-                    const uint32_t h01 = cvt_f16x2_e4m3x2(uint16_t(w[j] & 0xffffu));
-                    const uint32_t h23 = cvt_f16x2_e4m3x2(uint16_t(w[j] >> 16));
-                    const float2 f01 = __half22float2(*reinterpret_cast<const __half2*>(&h01));
-                    const float2 f23 = __half22float2(*reinterpret_cast<const __half2*>(&h23));
-                    o[2 * j] = f2_to_bf16x2(f01.x * sc[u], f01.y * sc[u]);
-                    o[2 * j + 1] = f2_to_bf16x2(f23.x * sc[u], f23.y * sc[u]);
-                }
                 *reinterpret_cast<uint4*>(dst + (size_t(row0 + r) * kRow + hl * 8) * 2) =
-                    make_uint4(o[0], o[1], o[2], o[3]);
+                    dequant8(v[u], sc[u]);
+            }
+        }
+    }
+}
+
+// Gathered blocks (launch_kv_gather_fp8): n blocks of nparts parts, cpp items per part; the
+// part bases travel in the kernel parameters, as for kv_gather_ldst.
+__global__ void __launch_bounds__(kThreads + 32)
+    kv_write_fp8_gather_kernel(const CopyDesc* __restrict__ descs,
+                               const __grid_constant__ GatherParts parts, uint32_t n,
+                               uint32_t nparts, uint32_t elems, uint32_t chunk, uint32_t cpp,
+                               uint64_t stride, Publish pub) {
+    write_fp8(descs, n, elems, chunk, cpp, pub, BlockParts<true>{&parts, nparts, 0, stride});
+}
+
+// The same loop as kv_read_fp8_kernel over the parts of gathered blocks.  A missing block
+// counts once, on its first part's first item; none of its parts is written.  (The two kernels
+// share the row maths, not the loop: inlining one loop body into both changed how the
+// compiler schedules kv_read_fp8_kernel.)
+__global__ void __launch_bounds__(kThreads)
+    kv_read_fp8_scatter_kernel(const CopyDesc* __restrict__ descs,
+                               const __grid_constant__ GatherParts parts, uint32_t n,
+                               uint32_t nparts, uint32_t first_part, uint32_t elems,
+                               uint32_t chunk, uint32_t cpp, uint64_t stride, uint32_t* status) {
+    const BlockParts<false> pages{&parts, nparts, first_part, stride};
+    const uint32_t total = n * nparts * cpp;
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t half = lane >> 4, hl = lane & 15;
+    constexpr uint32_t kStep = 2 * kRowPairs;
+    for (uint32_t item = blockIdx.x; item < total; item += gridDim.x) {
+        const CopyDesc d = pages.at(descs, item / cpp);
+        if (d.src == 0) {
+            if (threadIdx.x == 0 && pages.head(item / cpp) && item % cpp == 0 && status) atomicAdd(status + kStatMiss, 1u);
+            continue;
+        }
+        const uint32_t e0 = (item % cpp) * chunk;
+        const uint32_t rows = min(chunk, elems - e0) / kRow;
+        const uint32_t row0 = e0 / kRow;
+        const uint8_t* q = reinterpret_cast<const uint8_t*>(d.src);
+        const float* scales = reinterpret_cast<const float*>(q + elems);
+        uint8_t* dst = reinterpret_cast<uint8_t*>(d.dst);
+        for (uint32_t r0 = warp * kStep; r0 < rows; r0 += kWarps * kStep) {
+            uint2 v[kRowPairs];
+            float sc[kRowPairs];
+#pragma unroll
+            for (int u = 0; u < kRowPairs; ++u) {
+                const uint32_t r = r0 + 2 * u + half;
+                if (r < rows) {
+                    v[u] = ld_u2(q + size_t(row0 + r) * kRow + hl * 8);
+                    sc[u] = __uint_as_float(ld_u1(scales + row0 + r));
+                }
+            }
+#pragma unroll
+            for (int u = 0; u < kRowPairs; ++u) {
+                const uint32_t r = r0 + 2 * u + half;
+                if (r >= rows) continue;
+                *reinterpret_cast<uint4*>(dst + (size_t(row0 + r) * kRow + hl * 8) * 2) =
+                    dequant8(v[u], sc[u]);
             }
         }
     }
@@ -206,6 +285,25 @@ cudaError_t launch_kv_read_fp8(const Fp8Launch& a, cudaStream_t stream) {
     if (p.kernel != Kernel::kLdStFp8) return launch_kv_fp8_pipe(a, false, stream);
     kv_read_fp8_kernel<<<p.ctas, kThreads, 0, stream>>>(a.descs, a.n, a.elems, p.chunk, p.cpb,
                                                         a.status);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_kv_gather_fp8(const GatherLaunch& a, uint32_t elems, int variant,
+                                 cudaStream_t stream) {
+    if (a.n == 0) return cudaSuccess;
+    if (!a.part_base) return cudaErrorInvalidValue;
+    const LaunchPlan p = plan_gather_fp8(a, elems, variant, sm_count());
+    if (!p.valid) return cudaErrorInvalidValue;  // the caller splits the batch
+    if (p.kernel != Kernel::kLdStFp8) return launch_kv_fp8_pipe_gather(a, elems, stream);
+    GatherParts parts;
+    std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
+    const uint64_t stride = fp8_gather_bytes(1, elems);
+    if (a.write)
+        kv_write_fp8_gather_kernel<<<p.ctas, kThreads + 32, 0, stream>>>(
+            a.descs, parts, a.n, a.nparts, elems, p.chunk, p.cpb, stride, publish_of(a, true));
+    else
+        kv_read_fp8_scatter_kernel<<<p.ctas, kThreads, 0, stream>>>(
+            a.descs, parts, a.n, a.nparts, a.first_part, elems, p.chunk, p.cpb, stride, a.status);
     return cudaGetLastError();
 }
 

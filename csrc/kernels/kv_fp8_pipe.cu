@@ -23,9 +23,11 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
+#include <cstring>
 #include <type_traits>
 
 #include "common.cuh"
+#include "fp8_pages.cuh"
 #include "kernels.h"
 #include "launch_plan.h"
 #include "publish.cuh"
@@ -78,11 +80,14 @@ struct Fp8Shape {
 
 // NCW compute warps (4 or 8) besides the loader, storer and control / resolver warps.
 // FUSED (reads only): descriptors come from the resolver warp's queue instead of `descs`.
-template <bool WRITE, int NCW, bool FUSED>
-__global__ void __launch_bounds__((3 + NCW) * 32)
-    kv_fp8_pipe_kernel(const CopyDesc* __restrict__ descs, const Fp8Shape sh, Publish pub,
-                       uint32_t* status, const __grid_constant__ ResolveArgs ra) {
+// `pages` (fp8_pages.cuh) maps page item / sh.cpb to its descriptor: sh.n pages, grouped into
+// blocks of pages.nparts for the commit and the miss count.
+template <bool WRITE, int NCW, bool FUSED, typename Pages>
+__device__ __forceinline__ void fp8_pipe(const CopyDesc* __restrict__ descs, const Fp8Shape& sh,
+                                         const Publish& pub, uint32_t* status,
+                                         const ResolveArgs& ra, const Pages& pages) {
     static_assert(!(WRITE && FUSED), "only reads resolve keys");
+    static_assert(!(FUSED && Pages::nparts != 1), "the resolver feeds whole pages");
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ Smem bars;
     __shared__ __align__(16) ResolveQueue rq;
@@ -108,7 +113,8 @@ __global__ void __launch_bounds__((3 + NCW) * 32)
     }
     __syncthreads();
     if (warp == 2) {  // control warp: in-band commit (writes) / resolver (fused reads)
-        if (WRITE && pub.recs) control_warp(pub, lane, blockIdx.x, nitems, grid, sh.cpb, 64);
+        if (WRITE && pub.recs)
+            control_warp(pub, lane, blockIdx.x, nitems, grid, sh.cpb * pages.nparts, 64);
         if (FUSED)
             resolver_warp(ra, rq, sh.elems + sh.elems / kRow * 4, blockIdx.x, grid,
                           sh.cpb, nitems, lane);
@@ -123,8 +129,11 @@ __global__ void __launch_bounds__((3 + NCW) * 32)
         for (uint32_t k = 0; k < nitems; ++k) {
             const uint32_t item = blockIdx.x + k * grid;
             CopyDesc d;
-            if constexpr (!FUSED)
-                d = descs[item / sh.cpb];
+            bool head = true;  // a block's first page: its first tile counts a miss
+            if constexpr (!FUSED) {
+                d = pages.at(descs, item / sh.cpb);
+                head = pages.head(item / sh.cpb);
+            }
             else if constexpr (kRole == 2)
                 d = CopyDesc{1, 0};
             else  // one lane per role makes this call: not warp wide
@@ -132,7 +141,7 @@ __global__ void __launch_bounds__((3 + NCW) * 32)
             const uint32_t e0 = (item % sh.cpb) * sh.chunk_elems;
             const uint32_t e1 = min(sh.elems, e0 + sh.chunk_elems);
             for (uint32_t e = e0; e < e1; e += kTileElems, ++q)
-                fn(q, d, e, min(kTileElems, e1 - e) / kRow, e == 0);
+                fn(q, d, e, min(kTileElems, e1 - e) / kRow, head && e == 0);
         }
     };
     if (warp == 0) {  // ---- loader
@@ -255,6 +264,25 @@ __global__ void __launch_bounds__((3 + NCW) * 32)
     });
 }
 
+template <bool WRITE, int NCW, bool FUSED>
+__global__ void __launch_bounds__((3 + NCW) * 32)
+    kv_fp8_pipe_kernel(const CopyDesc* __restrict__ descs, const Fp8Shape sh, Publish pub,
+                       uint32_t* status, const __grid_constant__ ResolveArgs ra) {
+    fp8_pipe<WRITE, NCW, FUSED>(descs, sh, pub, status, ra, OnePage{});
+}
+
+// Gathered blocks (launch_kv_fp8_pipe_gather): part s of block b is page b * nparts + s, the
+// way kv_pipe_gather treats it as a virtual block; sh.n = blocks * nparts, sh.cpb = items per
+// part.  The part bases travel in the kernel parameters.
+template <bool WRITE>
+__global__ void __launch_bounds__((3 + 8) * 32)
+    kv_fp8_pipe_gather_kernel(const CopyDesc* __restrict__ descs, const Fp8Shape sh, Publish pub,
+                              uint32_t* status, const __grid_constant__ GatherParts parts,
+                              uint32_t nparts, uint32_t first_part, uint64_t stride) {
+    fp8_pipe<WRITE, 8, false>(descs, sh, pub, status, ResolveArgs{},
+                              BlockParts<WRITE>{&parts, nparts, first_part, stride});
+}
+
 constexpr size_t kSmemWrite = kInStages * kTileBf16 + kOutStages * (kTileQ + kTileScale);
 constexpr size_t kSmemRead = kInStages * (kTileQ + kTileScale) + kOutStages * kTileBf16;
 
@@ -266,7 +294,9 @@ cudaError_t ensure_attrs() {
          {reinterpret_cast<const void*>(kv_fp8_pipe_kernel<true, 8, false>), int(kSmemWrite)},
          {reinterpret_cast<const void*>(kv_fp8_pipe_kernel<false, 4, false>), int(kSmemRead)},
          {reinterpret_cast<const void*>(kv_fp8_pipe_kernel<false, 8, false>), int(kSmemRead)},
-         {reinterpret_cast<const void*>(kv_fp8_pipe_kernel<false, 8, true>), int(kSmemRead)}});
+         {reinterpret_cast<const void*>(kv_fp8_pipe_kernel<false, 8, true>), int(kSmemRead)},
+         {reinterpret_cast<const void*>(kv_fp8_pipe_gather_kernel<true>), int(kSmemWrite)},
+         {reinterpret_cast<const void*>(kv_fp8_pipe_gather_kernel<false>), int(kSmemRead)}});
 }
 
 }  // namespace
@@ -289,6 +319,26 @@ cudaError_t launch_kv_fp8_pipe(const Fp8Launch& a, bool write, cudaStream_t stre
                                          : go(kv_fp8_pipe_kernel<true, 8, false>, 3 + 8, kSmemWrite);
     return p.kernel == Kernel::kTma4 ? go(kv_fp8_pipe_kernel<false, 4, false>, 3 + 4, kSmemRead)
                                      : go(kv_fp8_pipe_kernel<false, 8, false>, 3 + 8, kSmemRead);
+}
+
+cudaError_t launch_kv_fp8_pipe_gather(const GatherLaunch& a, uint32_t elems, cudaStream_t stream) {
+    if (a.n == 0) return cudaSuccess;
+    if (!a.part_base) return cudaErrorInvalidValue;
+    const LaunchPlan p = plan_gather_fp8(a, elems, kFp8Auto, sm_count());
+    if (!p.valid) return cudaErrorInvalidValue;  // the caller splits the batch
+    cudaError_t e = ensure_attrs();
+    if (e != cudaSuccess) return e;
+    GatherParts parts;
+    std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
+    const Fp8Shape sh{a.n * a.nparts, elems, p.chunk, p.cpb};
+    const uint64_t stride = fp8_gather_bytes(1, elems);
+    if (a.write)
+        kv_fp8_pipe_gather_kernel<true><<<p.ctas, (3 + 8) * 32, kSmemWrite, stream>>>(
+            a.descs, sh, publish_of(a, true), a.status, parts, a.nparts, 0, stride);
+    else
+        kv_fp8_pipe_gather_kernel<false><<<p.ctas, (3 + 8) * 32, kSmemRead, stream>>>(
+            a.descs, sh, Publish{}, a.status, parts, a.nparts, a.first_part, stride);
+    return cudaGetLastError();
 }
 
 // read_cache_fp8 through the device index in one launch: keys -> (resolver warp) -> pool

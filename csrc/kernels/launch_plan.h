@@ -2,7 +2,8 @@
 // many CTAs.  No CUDA in here: the launchers (kv_copy.cu, kv_read_fused.cu, kv_pipe.cu,
 // kv_fp8.cu, kv_fp8_pipe.cu) pass in the SM count and the CTAs per SM the ld/st kernels keep
 // resident (occupancy API), so the choice is unit-tested on the CPU
-// (_infinistore.testing.plan_copy / plan_gather / plan_read_fused / plan_fp8).
+// (_infinistore.testing.plan_copy / plan_gather / plan_read_fused / plan_fp8 /
+// plan_gather_fp8).
 #pragma once
 
 #include <algorithm>
@@ -267,6 +268,27 @@ inline LaunchPlan plan_fp8(const Fp8Launch& a, int sms) {
     p.kernel = Kernel::kLdStFp8;
     ldst_items(p, a.n, a.elems, kFp8Chunk, 1u << 19, sms);
     p.ctas = clamp_grid(a.max_ctas > 0 ? a.max_ctas : 6 * sms, uint64_t(a.n) * p.cpb);
+    return p;
+}
+
+// ---------------------------------------------------------------- launch_kv_gather_fp8
+// Every part of every block is one fp8 page, so the rules of plan_fp8 apply with n * nparts
+// pages: cpb is the items per part.  kFp8LdSt picks the ld/st kernels, anything else the
+// pipeline with 8 compute warps.  Parts of a multiple of 512 elements and 16-byte aligned part
+// bases and offsets only (the pipeline's precondition, and every part starts 16-byte aligned);
+// more than kMaxItems work items are refused (the caller splits the batch).
+inline LaunchPlan plan_gather_fp8(const GatherLaunch& a, uint32_t elems, int variant, int sms) {
+    const uint64_t parts = uint64_t(a.n) * a.nparts;
+    if (a.nparts == 0 || a.nparts > kGatherMaxParts || elems == 0 || elems % 512 != 0 ||
+        (a.align_or & 15) != 0 || parts > kMaxItems)
+        return invalid_plan();
+    Fp8Launch f;
+    f.n = uint32_t(parts);
+    f.elems = elems;
+    f.max_ctas = a.max_ctas;
+    f.variant = variant == kFp8LdSt ? kFp8LdSt : kFp8Auto;
+    LaunchPlan p = plan_fp8(f, sms);
+    if (parts * p.cpb > kMaxItems) return invalid_plan();
     return p;
 }
 

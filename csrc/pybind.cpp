@@ -593,6 +593,46 @@ PYBIND11_MODULE(_infinistore, m) {
             py::arg("device") = -1, py::arg("stream") = 0, py::arg("scale") = 1,
             "scattered read: stored part first_part + s of each block -> part_base[s] + offset")
         .def(
+            "w_rdma_gather_fp8",
+            [](Connection& c, const std::vector<uint64_t>& part_base, int elems,
+               const py::object& offsets, const py::object& remote_blocks, int device,
+               uint64_t stream, uint64_t scale) {
+                BlockSpan rb;
+                OffsetSpan off;
+                blocks_from_py(remote_blocks, rb);
+                offsets_from_py(offsets, off);
+                std::vector<uint64_t> bytes(off.n);
+                for (size_t i = 0; i < off.n; ++i) bytes[i] = off.data[i] * scale;
+                Connection::GatherSpec g;
+                g.part_base = part_base.data();
+                g.nparts = uint32_t(part_base.size());
+                py::gil_scoped_release rel;
+                return c.w_rdma_gather_fp8(g, elems, bytes.data(), bytes.size(), rb.data, rb.n,
+                                           device, stream);
+            },
+            py::arg("part_base"), py::arg("elems"), py::arg("offsets"), py::arg("remote_blocks"),
+            py::arg("device") = -1, py::arg("stream") = 0, py::arg("scale") = 1,
+            "gathered fp8 write: bf16 part s at part_base[s] + offsets[i] * scale is quantised "
+            "into fp8 page s of block i")
+        .def(
+            "r_rdma_scatter_fp8",
+            [](Connection& c, const std::vector<uint64_t>& part_base, int elems,
+               uint32_t first_part, const py::object& blocks, int device, uint64_t stream,
+               uint64_t scale) {
+                std::vector<KeyOffset> kb;
+                blocks_list_from_py(blocks, scale, kb);
+                Connection::GatherSpec g;
+                g.part_base = part_base.data();
+                g.nparts = uint32_t(part_base.size());
+                g.first_part = first_part;
+                py::gil_scoped_release rel;
+                return c.r_rdma_scatter_fp8(g, elems, kb, device, stream);
+            },
+            py::arg("part_base"), py::arg("elems"), py::arg("first_part"), py::arg("blocks"),
+            py::arg("device") = -1, py::arg("stream") = 0, py::arg("scale") = 1,
+            "scattered fp8 read: fp8 page first_part + s of each block, dequantised -> "
+            "part_base[s] + offset")
+        .def(
             "rw_local",
             [](Connection& c, const std::string& op, const py::object& blocks, int block_size,
                uint64_t base_ptr, int device, uint64_t stream, uint64_t scale) {
@@ -891,6 +931,39 @@ PYBIND11_MODULE(_infinistore, m) {
         "gathered blocks: descs[i] = write {local byte offset, block address} / read {block "
         "address or 0, local byte offset}; part s of block i at part_base[s] + local offset");
     k.def(
+        "kv_gather_fp8",
+        [](uint64_t descs, uint32_t n, const std::vector<uint64_t>& part_base, uint32_t elems,
+           uint32_t first_part, bool write, int variant, int max_ctas, uint64_t stream,
+           uint64_t recs, uint64_t table, uint64_t table_mask, uint64_t done, uint64_t status,
+           uint64_t align_or) {
+            if (part_base.empty() || part_base.size() > kernels::kGatherMaxParts)
+                throw std::runtime_error("kv_gather_fp8: 1 to GATHER_MAX_PARTS parts");
+            kernels::GatherLaunch G;
+            G.descs = as_ptr<const kernels::CopyDesc>(descs);
+            G.n = n;
+            G.write = write;
+            G.part_base = part_base.data();
+            G.nparts = uint32_t(part_base.size());
+            G.first_part = first_part;
+            G.align_or = align_or;
+            G.recs = as_ptr<const kernels::IndexEntry>(recs);
+            G.table = as_ptr<kernels::IndexBucket>(table);
+            G.table_mask = table_mask;
+            G.done = as_ptr<uint32_t>(done);
+            G.status = as_ptr<uint32_t>(status);
+            G.max_ctas = max_ctas;
+            const cudaError_t e =
+                kernels::launch_kv_gather_fp8(G, elems, variant, as_ptr<CUstream_st>(stream));
+            if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
+        },
+        py::arg("descs"), py::arg("n"), py::arg("part_base"), py::arg("elems"),
+        py::arg("first_part") = 0, py::arg("write") = true, py::arg("variant") = 0,
+        py::arg("max_ctas") = 0, py::arg("stream") = 0, py::arg("recs") = 0, py::arg("table") = 0,
+        py::arg("table_mask") = 0, py::arg("done") = 0, py::arg("status") = 0,
+        py::arg("align_or") = 0,
+        "gathered fp8 blocks: descs as for kv_gather; part s (elems bf16 elements at "
+        "part_base[s] + local offset) <-> fp8 page s of the block");
+    k.def(
         "kv_pipe_mcast",
         [](uint64_t descs, uint32_t n, uint32_t bytes, const std::vector<int64_t>& delta,
            int max_clusters, uint64_t stream, uint64_t status, uint32_t stage_bytes,
@@ -1031,6 +1104,8 @@ PYBIND11_MODULE(_infinistore, m) {
           py::arg("recs") = 0, py::arg("table") = 0, py::arg("table_mask") = 0,
           py::arg("done") = 0, py::arg("status") = 0, py::arg("variant") = 0);
     k.def("fp8_block_bytes", &kernels::fp8_block_bytes);
+    k.def("fp8_gather_bytes", &kernels::fp8_gather_bytes, py::arg("nparts"), py::arg("elems"),
+          "bytes of nparts fp8 pages of elems elements end to end (a gathered fp8 block)");
     k.def(
         "kv_bcast_nvls",
         [](uint64_t descs, uint32_t n, uint32_t bytes, int max_ctas, uint64_t stream,
@@ -1300,8 +1375,10 @@ PYBIND11_MODULE(_infinistore, m) {
               const DeviceReadPlan p = plan_device_read(DeviceReadIn{
                   n, block_bytes, fp8_elems, gather, fp8_fused_ok, scatter_fused_ok, copy_variant,
                   all_local, all_remote, max_ctas, sm_count});
-              static const char* const kPaths[] = {"fused_copy",  "fused_fp8",  "fused_scatter",
-                                                   "lookup_copy", "lookup_fp8", "lookup_gather"};
+              static const char* const kPaths[] = {"fused_copy",    "fused_fp8",
+                                                   "fused_scatter", "lookup_copy",
+                                                   "lookup_fp8",    "lookup_gather",
+                                                   "lookup_gather_fp8"};
               py::dict d;
               d["path"] = kPaths[int(p.path)];
               d["variant"] = p.variant;
@@ -1400,6 +1477,18 @@ PYBIND11_MODULE(_infinistore, m) {
           },
           py::arg("n"), py::arg("elems"), py::arg("variant") = 0, py::arg("aligned16") = true,
           py::arg("group") = 128, py::arg("max_ctas") = 0, py::arg("sm_count") = 132);
+    t.def("plan_gather_fp8",
+          [plan_dict](uint32_t n, uint32_t nparts, uint32_t elems, int variant, uint64_t align_or,
+                      int max_ctas, int sm_count) {
+              kernels::GatherLaunch a;
+              a.n = n;
+              a.nparts = nparts;
+              a.align_or = align_or;
+              a.max_ctas = max_ctas;
+              return plan_dict(kernels::plan_gather_fp8(a, elems, variant, sm_count));
+          },
+          py::arg("n"), py::arg("nparts"), py::arg("elems"), py::arg("variant") = 0,
+          py::arg("align_or") = 0, py::arg("max_ctas") = 0, py::arg("sm_count") = 132);
     py::class_<MM>(t, "MM")
         .def(py::init<>())
         .def("add_pool", &MM::add_pool)

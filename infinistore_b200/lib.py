@@ -593,9 +593,12 @@ class InfinityConnection:
             raise Exception(f"Failed to read to infinistore, ret = {ret}: {self.conn.last_error()}")
 
     # ------------------------------------------------------------------ gathered blocks
-    def _gather_parts(self, parts, max_offset: int, part_size: int):
+    def _gather_parts(self, parts, max_offset: int, part_size: int, fp8: bool = False,
+                      offsets=None):
         """Checks a parts list ``[(tensor, base), ...]`` before anything is enqueued.  Returns
-        (absolute byte address of every part, device ordinal or -1, element size)."""
+        (absolute byte address of every part, device ordinal or -1, element size).  ``fp8``:
+        the parts are bf16 CUDA tensors, ``part_size`` is a multiple of 512 elements and every
+        part base and offset (``offsets``, elements) is 16-byte aligned."""
         if self._mode != "rdma":
             raise Exception("gathered blocks need a connected rdma connection")
         parts = list(parts)
@@ -609,7 +612,9 @@ class InfinityConnection:
             raise ValueError("part_size must be positive")
         first = parts[0][0]
         es = first.element_size()
-        if len(parts) * int(part_size) * es > _GATHER_MAX_BLOCK_BYTES:
+        block_bytes = (self.fp8_gather_block_bytes(len(parts), int(part_size)) if fp8
+                       else len(parts) * int(part_size) * es)
+        if block_bytes > _GATHER_MAX_BLOCK_BYTES:
             raise ValueError(f"{len(parts)} parts of {int(part_size) * es} bytes exceed the "
                              f"{_GATHER_MAX_BLOCK_BYTES}-byte block limit")
         bases = []
@@ -625,6 +630,21 @@ class InfinityConnection:
                 raise ValueError(f"part {i}: base {base} + offset {max_offset} + part_size "
                                  f"{int(part_size)} runs past the tensor's {t.numel()} elements")
             bases.append(t.data_ptr() + base * es)
+        if fp8:
+            if first.dtype != torch.bfloat16:
+                raise ValueError(f"fp8 gathered blocks take bf16 tensors, not {first.dtype}")
+            if int(part_size) % 512:
+                raise ValueError(f"fp8 gathered blocks need a part_size that is a multiple of "
+                                 f"512 elements, not {int(part_size)}")
+            align = 0
+            for b in bases:
+                align |= b
+            if offsets is not None and len(offsets):
+                align |= int(np.bitwise_or.reduce(np.asarray(offsets, dtype=np.int64) * es))
+            if align & 15:
+                raise ValueError("fp8 gathered blocks need 16-byte aligned part bases and offsets")
+            if first.device.type != "cuda":
+                raise ValueError("fp8 gathered blocks take CUDA tensors")
         dev = _device_of(first)
         if dev < 0 and self.conn.server_has_hbm():
             raise ValueError("gathered blocks of CPU tensors need a host-memory pool "
@@ -659,18 +679,9 @@ class InfinityConnection:
             raise Exception(f"Failed to write to infinistore, ret = {ret}: {self.conn.last_error()}")
         return 0
 
-    def read_cache_scatter(self, parts, blocks, part_size: int, first_part: int = 0,
-                           stream="current"):
-        """Scatter parts ``first_part .. first_part + len(parts) - 1`` of every stored block
-        into the parts list (see ``rdma_write_cache_gather``): stored part ``first_part + s``
-        of block ``(key, offset)`` lands at ``parts[s][1] + offset`` of ``parts[s][0]``.
-
-        ``blocks`` is ``[(key, offset)]`` or ``(keys, offsets)``, offsets in elements.
-        ``first_part`` lets a decoder fetch one layer of all-layer blocks while the previous
-        layer computes.  A missing key raises (with ``device_lookup``, ``sync()`` reports it)
-        and counts once, not once per part; its destination parts are left untouched.  With
-        ``device_lookup`` a stored block shorter than ``(first_part + len(parts)) * part_size``
-        elements is a miss, and a block purged or evicted during the read is reported as one."""
+    @staticmethod
+    def _scatter_blocks(blocks, first_part: int):
+        """``[(key, offset)]`` or ``(keys, offsets)`` -> (keys, int64 offsets), checked."""
         if isinstance(blocks, tuple) and len(blocks) == 2 and isinstance(blocks[1], np.ndarray):
             keys = list(blocks[0])
             offs = np.ascontiguousarray(blocks[1], dtype=np.int64).reshape(-1)
@@ -683,6 +694,21 @@ class InfinityConnection:
             raise ValueError("offsets must not be negative")
         if int(first_part) < 0:
             raise ValueError("first_part must not be negative")
+        return keys, offs
+
+    def read_cache_scatter(self, parts, blocks, part_size: int, first_part: int = 0,
+                           stream="current"):
+        """Scatter parts ``first_part .. first_part + len(parts) - 1`` of every stored block
+        into the parts list (see ``rdma_write_cache_gather``): stored part ``first_part + s``
+        of block ``(key, offset)`` lands at ``parts[s][1] + offset`` of ``parts[s][0]``.
+
+        ``blocks`` is ``[(key, offset)]`` or ``(keys, offsets)``, offsets in elements.
+        ``first_part`` lets a decoder fetch one layer of all-layer blocks while the previous
+        layer computes.  A missing key raises (with ``device_lookup``, ``sync()`` reports it)
+        and counts once, not once per part; its destination parts are left untouched.  With
+        ``device_lookup`` a stored block shorter than ``(first_part + len(parts)) * part_size``
+        elements is a miss, and a block purged or evicted during the read is reported as one."""
+        keys, offs = self._scatter_blocks(blocks, first_part)
         bases, dev, es = self._gather_parts(parts, int(offs.max()) if len(offs) else 0, part_size)
         if (int(first_part) + len(bases)) * int(part_size) * es > _GATHER_MAX_BLOCK_BYTES:
             raise ValueError("first_part + parts run past the block size limit")
@@ -690,6 +716,58 @@ class InfinityConnection:
             return
         ret = self.conn.r_rdma_scatter(bases, int(part_size) * es, int(first_part), (keys, offs),
                                        dev, _stream_of(parts[0][0], stream), es)
+        if ret < 0:
+            raise Exception(f"Failed to read to infinistore, ret = {ret}: {self.conn.last_error()}")
+
+    # ------------------------------------------------------------------ gathered fp8 blocks
+    @staticmethod
+    def fp8_gather_block_bytes(nparts: int, part_size: int) -> int:
+        """Pool bytes of a gathered fp8 block of ``nparts`` parts of ``part_size`` bf16
+        elements (what to pass to ``allocate_rdma``): ``nparts`` fp8 pages end to end, each
+        ``fp8_page_bytes(part_size)``."""
+        return _infinistore.kernels.fp8_gather_bytes(int(nparts), int(part_size))
+
+    def rdma_write_cache_gather_fp8(self, parts, offsets, part_size: int, remote_blocks,
+                                    stream="current"):
+        """``rdma_write_cache_gather`` with every part quantised to e4m3 (one fp32 scale per
+        128 elements) inside the write kernel: part ``s`` of a block is the fp8 page that
+        ``rdma_write_cache_fp8`` would store for it, at byte
+        ``fp8_gather_block_bytes(s, part_size)`` of the block, so a block takes 0.516 of its
+        bf16 bytes.  The parts are bf16 CUDA tensors, ``part_size`` is a multiple of 512
+        elements, and part bases and offsets are 16-byte aligned.  The blocks must have been
+        allocated with ``fp8_gather_block_bytes(len(parts), part_size)`` bytes."""
+        offs = np.ascontiguousarray(offsets, dtype=np.int64).reshape(-1)
+        if len(offs) != len(remote_blocks):
+            raise ValueError(f"{len(offs)} offsets for {len(remote_blocks)} remote blocks")
+        if len(offs) and int(offs.min()) < 0:
+            raise ValueError("offsets must not be negative")
+        bases, dev, _ = self._gather_parts(parts, int(offs.max()) if len(offs) else 0, part_size,
+                                           fp8=True, offsets=offs)
+        if not len(offs):
+            return 0
+        ret = self.conn.w_rdma_gather_fp8(bases, int(part_size), offs, remote_blocks, dev,
+                                          _stream_of(parts[0][0], stream), 2)
+        if ret < 0:
+            raise Exception(f"Failed to write to infinistore, ret = {ret}: {self.conn.last_error()}")
+        return 0
+
+    def read_cache_scatter_fp8(self, parts, blocks, part_size: int, first_part: int = 0,
+                               stream="current"):
+        """Read blocks written by ``rdma_write_cache_gather_fp8``: fp8 page ``first_part + s``
+        of every block is dequantised into part ``s`` (``blocks``, misses and ``first_part`` as
+        for ``read_cache_scatter``).  With ``device_lookup`` a stored block shorter than
+        ``fp8_gather_block_bytes(first_part + len(parts), part_size)`` is a miss.  The same
+        checks as ``rdma_write_cache_gather_fp8``."""
+        keys, offs = self._scatter_blocks(blocks, first_part)
+        bases, dev, _ = self._gather_parts(parts, int(offs.max()) if len(offs) else 0, part_size,
+                                           fp8=True, offsets=offs)
+        if self.fp8_gather_block_bytes(int(first_part) + len(bases),
+                                       int(part_size)) > _GATHER_MAX_BLOCK_BYTES:
+            raise ValueError("first_part + parts run past the block size limit")
+        if not len(offs):
+            return
+        ret = self.conn.r_rdma_scatter_fp8(bases, int(part_size), int(first_part), (keys, offs),
+                                           dev, _stream_of(parts[0][0], stream), 2)
         if ret < 0:
             raise Exception(f"Failed to read to infinistore, ret = {ret}: {self.conn.last_error()}")
 

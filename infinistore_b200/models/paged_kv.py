@@ -96,24 +96,38 @@ class PagedKVCache:
     def _parts(self, layers: range):
         return [(self.data, self.page_offset(layer, kv, 0)) for layer in layers for kv in (0, 1)]
 
+    def _check_fp8(self):
+        if self.data.dtype != torch.bfloat16 or self.data.device.type != "cuda":
+            raise ValueError("fp8 all-layer pages need a bf16 cache on a CUDA device")
+
     def write_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
-                    stream="current") -> int:
-        """Upload every layer's K and V of each page under one key per page.  Returns the
+                    stream="current", fp8: bool = False) -> int:
+        """Upload every layer's K and V of each page under one key per page.  ``fp8``: every
+        part is stored as e4m3 with per-128 scales (``rdma_write_cache_gather_fp8``), about
+        half the pool bytes; read such pages back with ``read_pages(fp8=True)``.  Returns the
         number of blocks written."""
+        if fp8:
+            self._check_fp8()  # before any block is allocated
         self._ensure_registered(conn)
         layers = range(self.layout.layers)
         keys = self.page_keys(page_hashes)
-        blocks = conn.allocate_rdma(keys, 2 * len(layers) * self.layout.page_bytes)
-        offs = np.asarray(pages, dtype=np.int64) * self.layout.page_elems
-        conn.rdma_write_cache_gather(self._parts(layers), offs, self.layout.page_elems, blocks,
-                                     stream=stream)
+        elems = self.layout.page_elems
+        nbytes = (conn.fp8_gather_block_bytes(2 * len(layers), elems) if fp8
+                  else 2 * len(layers) * self.layout.page_bytes)
+        blocks = conn.allocate_rdma(keys, nbytes)
+        offs = np.asarray(pages, dtype=np.int64) * elems
+        write = conn.rdma_write_cache_gather_fp8 if fp8 else conn.rdma_write_cache_gather
+        write(self._parts(layers), offs, elems, blocks, stream=stream)
         return len(keys)
 
     def read_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
-                   layers: Optional[range] = None, stream="current") -> int:
+                   layers: Optional[range] = None, stream="current", fp8: bool = False) -> int:
         """Fetch pages written by ``write_pages`` into pages ``pages``.  ``layers`` (a range
         with step 1, default all) reads only those layers' parts of the blocks, so layer l
-        can be fetched while layer l - 1 computes.  Returns the number of blocks read."""
+        can be fetched while layer l - 1 computes.  ``fp8`` must be what the writer used.
+        Returns the number of blocks read."""
+        if fp8:
+            self._check_fp8()
         self._ensure_registered(conn)
         layers = range(self.layout.layers) if layers is None else layers
         if layers.step != 1 or not len(layers) or layers.start < 0 or layers.stop > self.layout.layers:
@@ -121,8 +135,9 @@ class PagedKVCache:
                              f"0..{self.layout.layers}")
         keys = self.page_keys(page_hashes)
         offs = np.asarray(pages, dtype=np.int64) * self.layout.page_elems
-        conn.read_cache_scatter(self._parts(layers), (keys, offs), self.layout.page_elems,
-                                first_part=2 * layers.start, stream=stream)
+        read = conn.read_cache_scatter_fp8 if fp8 else conn.read_cache_scatter
+        read(self._parts(layers), (keys, offs), self.layout.page_elems,
+             first_part=2 * layers.start, stream=stream)
         return len(keys)
 
     def cached_prefix_pages(self, conn, page_hashes: Sequence[str],

@@ -258,6 +258,36 @@ def kv_read_fp8(descs: torch.Tensor, elems: int, max_ctas: int = 0,
                       status.data_ptr() if status is not None else 0, FP8_VARIANTS[variant])
 
 
+def fp8_gather_bytes(nparts: int, elems: int) -> int:
+    """Bytes of a gathered fp8 block: part s starts at fp8_gather_bytes(s, elems)."""
+    return K.fp8_gather_bytes(nparts, elems)
+
+
+def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, write: bool,
+                  first_part: int = 0, max_ctas: int = 0, status: Optional[torch.Tensor] = None,
+                  align_or: int = 0, publish: Optional[PublishArgs] = None,
+                  variant: str = "auto") -> None:
+    """Gathered fp8 blocks (``kv_gather`` with quantisation): part s of block i is a bf16 page
+    of ``elems`` elements at ``part_base[s] + local offset`` and fp8 page s of the block, at
+    byte ``fp8_gather_bytes(s, elems)``.  ``descs`` as for ``kv_gather``.  ``variant``:
+    "ldst" = the ld/st kernels (kv_fp8.cu), "auto" / "tma" = the TMA pipeline
+    (kv_fp8_pipe.cu).  ``align_or`` must include the local offsets (the part bases are added
+    here): unaligned batches are refused."""
+    assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
+    bases = [int(b) for b in part_base]
+    for b in bases:
+        align_or |= b
+    with torch.cuda.device(descs.device):
+        K.kv_gather_fp8(descs.data_ptr(), descs.shape[0], bases, elems, first_part, write,
+                        FP8_VARIANTS["ldst"] if variant == "ldst" else FP8_VARIANTS["auto"],
+                        max_ctas, _stream(descs.device),
+                        publish.recs.data_ptr() if publish else 0,
+                        publish.table.data_ptr() if publish else 0,
+                        publish.mask if publish else 0,
+                        publish.done.data_ptr() if publish else 0,
+                        status.data_ptr() if status is not None else 0, align_or)
+
+
 def fp8_reference(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """Plain PyTorch fp32 reference of the fused quantiser: per-128 amax scale, e4m3
     round-to-nearest with saturation.  Returns (dequantised fp32, scales, payload)."""
