@@ -266,6 +266,7 @@ void Connection::close() {
     }
     {
         std::lock_guard<std::mutex> lk(mu_);
+        ++session_;  // writers of this session must not touch the released blocks
         for (auto& kv : devs_) kv.second->wait_all();
         devs_.clear();
         host_maps_.clear();

@@ -183,8 +183,44 @@ class Connection {
         const uint64_t* part_base = nullptr;  // absolute addresses, all on `device` (or host)
         uint32_t nparts = 0;
         uint32_t part_bytes = 0;  // pool bytes of a part (fp8: fp8_gather_bytes(1, elems))
-        uint32_t first_part = 0;  // reads: stored part first_part + s lands in part s
+        uint32_t first_part = 0;  // stored part first_part + s is part s (one-shot writes: 0)
     };
+    // Layered gathered write: a fixed set of allocated gathered blocks whose parts are stored
+    // over several calls (write_layered), each a contiguous range of parts of every block -
+    // typically one layer's K and V as prefill produces them.  A block is published (device
+    // index) by the launch that lands its last part, and its server commit is staged by the
+    // call that completes the writer.  Not thread-safe: one caller at a time.
+    struct GatherWriter {
+        std::vector<RemoteBlock> blocks;  // blocks to write (the "already exists" ones dropped)
+        std::vector<uint64_t> offsets;    // their local offsets (elements until the first call)
+        std::vector<KeyHash> hashes;      // their key fingerprints from allocate
+        bool indexed = true;              // every block has a fingerprint: it can be published
+        uint32_t nparts = 0;              // S: parts of a block
+        std::vector<uint8_t> written;     // per part: stored by an earlier call
+        uint32_t parts_written = 0;
+        uint32_t calls = 0;               // calls that launched (the first one claims)
+        int device = -2;                  // fixed by the first call (-1: host tensors)
+        uint64_t scale = 0;               // bytes per offset unit, fixed by the first call
+        int elems = -1;                   // fp8 elements per part (0: raw bytes), first call
+        uint32_t part_bytes = 0;          // pool bytes of a part, first call
+        bool failed = false;
+        void* event = nullptr;            // cudaEvent_t recorded after the last launch
+        uint32_t* state = nullptr;        // device: 3 u32 per block (kernels::GatherLaunch)
+        uint64_t session = 0;             // the connection session that allocated the blocks
+        bool complete() const { return parts_written == nparts; }
+        ~GatherWriter();
+    };
+    // Takes the blocks' fingerprints out of the allocation record, once.
+    std::shared_ptr<GatherWriter> gather_writer(const RemoteBlock* blocks, const uint64_t* offsets,
+                                                size_t n, uint32_t nparts);
+    // Stores parts g.first_part .. g.first_part + g.nparts - 1 of every block of `w`; offsets
+    // are scaled by `scale`.  elems > 0: fp8 parts of `elems` bf16 elements (g.part_bytes is
+    // not read), as w_rdma_gather_fp8.  Refuses part ranges written before, a device, scale or
+    // elems other than the first call's, a complete or failed writer, and a writer made before
+    // the connection was last closed (its blocks and index ways were released).  A refused
+    // call leaves the writer as it was.
+    int write_layered(GatherWriter& w, const GatherSpec& g, int elems, uint64_t scale, int device,
+                      uint64_t stream);
     // offsets in bytes; blocks allocated with nparts * part_bytes bytes (trusted)
     int w_rdma_gather(const GatherSpec& g, const uint64_t* offsets, size_t noffsets,
                       const RemoteBlock* blocks, size_t nblocks, int device, uint64_t stream);
@@ -262,7 +298,7 @@ class Connection {
     int move_blocks(bool write, const uint64_t* local_off, uint64_t scale,
                     const RemoteBlock* blocks, size_t n, int block_size, uint64_t base_ptr,
                     int device, uint64_t stream, int fp8_elems = 0, MoveResult* res = nullptr,
-                    const GatherSpec* gather = nullptr);
+                    const GatherSpec* gather = nullptr, GatherWriter* layered = nullptr);
     // tell the server that the blocks at `addrs` were not (completely) written: it releases
     // them, device-index entries included
     int discard_blocks(const uint64_t* addrs, size_t count);
@@ -332,6 +368,7 @@ class Connection {
     uint32_t publish_failures_ = 0;  // own failures not yet reported to the server
     int streams_ = 4;
     int default_device_ = -1;
+    uint64_t session_ = 0;  // under mu_: close() ends a session (GatherWriter::session)
     ClientStats stats_;
     std::string last_error_;
 

@@ -8,6 +8,7 @@
 #include <cerrno>
 #include <chrono>
 #include <cstring>
+#include <mutex>
 
 #include "../core/log.h"
 #include "../core/trace.h"
@@ -268,6 +269,37 @@ kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n,
     return G;
 }
 
+// Layered writers' state (GatherWriter::state), allocated stream-ordered from a memory pool of
+// the process that keeps up to 64 MB (about 5.6 M blocks' state) once freed.  The device's
+// default pool hands freed memory back to the driver at every synchronise, and mapping it
+// again on a writer's first call stalled that call by up to a few hundred milliseconds
+// (bench/layerwise_gather.py).  The pool lives as long as the process, so a writer that
+// outlives its connection still frees into it.
+static cudaError_t writer_state_alloc(void** p, size_t bytes, int device, cudaStream_t s) {
+    static std::mutex mu;
+    static cudaMemPool_t pools[64] = {};
+    if (device < 0 || device >= 64) return cudaErrorInvalidDevice;
+    cudaMemPool_t pool;
+    {
+        std::lock_guard<std::mutex> lk(mu);
+        if (!pools[device]) {
+            cudaMemPoolProps props{};
+            props.allocType = cudaMemAllocationTypePinned;
+            props.location.type = cudaMemLocationTypeDevice;
+            props.location.id = device;
+            const cudaError_t e = cudaMemPoolCreate(&pools[device], &props);
+            if (e != cudaSuccess) {
+                pools[device] = nullptr;
+                return e;
+            }
+            uint64_t keep = 64ull << 20;
+            cudaMemPoolSetAttribute(pools[device], cudaMemPoolAttrReleaseThreshold, &keep);
+        }
+        pool = pools[device];
+    }
+    return cudaMallocFromPoolAsync(p, bytes, pool, s);
+}
+
 // Blocks per launch of a gathered call (staging.h: gather_max_blocks).  fp8 parts are counted
 // in bf16 bytes: the fp8 kernels cut a part into chunks of at least kFp8Chunk elements (16 KB
 // of bf16), or take it whole.
@@ -298,10 +330,11 @@ static KeyBatch next_key_batch(const std::vector<KeyOffset>& blocks, size_t base
 // byte offset of block i from base_ptr.  With `gather` (base_ptr 0), block i is
 // gather->nparts parts, part s at gather->part_base[s] + local_off[i] * scale, and
 // block_size = nparts * part_bytes.
+// `layered` (with `gather`): a call of a layered writer, whose blocks are exactly `blocks`.
 int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scale,
                             const RemoteBlock* blocks, size_t n, int block_size,
                             uint64_t base_ptr, int device, uint64_t stream_in, int fp8_elems,
-                            MoveResult* res, const GatherSpec* gather) {
+                            MoveResult* res, const GatherSpec* gather, GatherWriter* layered) {
     NvtxRange nvtx(write ? "istore.write_blocks" : "istore.read_blocks");
     std::lock_guard<std::mutex> lk(mu_);
     if (n == 0) return 0;
@@ -312,6 +345,12 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
     // below leaves the sink exactly as the last successful launch left it.
     std::vector<uint64_t>& sink = (res && res->commits) ? *res->commits : pending_commit_;
     std::vector<uint64_t> batch_commits;
+    // a layered writer's blocks are committed by the call that writes their last parts
+    const bool commit_now = !layered || layered->parts_written + gather->nparts == layered->nparts;
+    // bytes moved per block: a gathered call moves its parts, which are the whole block
+    // unless the call is layered
+    const uint64_t moved =
+        gather ? uint64_t(gather->nparts) * gather->part_bytes : uint64_t(uint32_t(block_size));
     int kd = device;
     if (device < 0 && fp8_elems) {
         fail("the fp8 KV path needs a CUDA tensor");
@@ -348,7 +387,7 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
                         uint8_t* local =
                             reinterpret_cast<uint8_t*>(gather->part_base[s] + local_off[i] * scale);
                         if (write)
-                            std::memcpy(pool + s * pb, local, pb);
+                            std::memcpy(pool + (gather->first_part + s) * pb, local, pb);
                         else
                             std::memcpy(local, pool + (gather->first_part + s) * pb, pb);
                     }
@@ -359,10 +398,10 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
                     else
                         std::memcpy(local, pool, size_t(block_size));
                 }
-                if (write) sink.push_back(blocks[i].remote_addr);
+                if (write && commit_now) sink.push_back(blocks[i].remote_addr);
                 stats_.host_copies++;
             }
-            (write ? stats_.bytes_written : stats_.bytes_read) += live * uint64_t(block_size);
+            (write ? stats_.bytes_written : stats_.bytes_read) += live * moved;
             return 0;
         }
         if (gather) {
@@ -409,6 +448,12 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
         }
     }
     if (scope.begin(stream_in, write) != 0) return -1;
+    if (layered && layered->event &&
+        cudaStreamWaitEvent(scope.stream, static_cast<cudaEvent_t>(layered->event), 0) !=
+            cudaSuccess) {
+        fail(std::string("layered write: ") + cudaGetErrorString(cudaGetLastError()));
+        return -1;
+    }
 
     // the device index lives in segment 0
     kernels::IndexBucket* table = nullptr;
@@ -434,9 +479,10 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
             recs = reinterpret_cast<kernels::IndexEntry*>(ctx->ring_h + at_rec);
         }
         uint32_t m = 0;
+        const size_t batch0 = i;  // a layered writer's blocks: its state index of descs[0]
         batch_commits.clear();
         uint32_t n_mc = 0;  // blocks of this batch that live in the NVLS-replicated region
-        bool can_publish = table != nullptr;
+        bool can_publish = table != nullptr && (!layered || layered->indexed);
         bool all_remote = true;
         bool all_local = !ctx->seg_remote.empty() && !ctx->seg_remote[0];  // index table (segment 0)
         uint64_t align_or = 0;
@@ -473,7 +519,8 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
             if (write) {
                 if (recs) {
                     KeyHash kh;
-                    if (pending_hash_.take(rb.remote_addr, &kh))
+                    if (layered) kh = layered->hashes[i];
+                    if (layered || pending_hash_.take(rb.remote_addr, &kh))
                         recs[m] = kernels::IndexEntry{kh.h1, kh.h2, rb.remote_addr, rb.gen,
                                                       uint32_t(block_size)};
                     else
@@ -528,6 +575,23 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
             G.done = L.done;
             G.all_local = L.all_local;
             G.shards = L.shards;
+            if (layered && L.recs) {
+                if (!layered->state) {  // zeroed behind the caller's pages, before any launch
+                    const size_t bytes = layered->blocks.size() * 3 * sizeof(uint32_t);
+                    void* p = nullptr;
+                    cudaError_t ea = writer_state_alloc(&p, bytes, ctx->device, scope.stream);
+                    if (ea == cudaSuccess) ea = cudaMemsetAsync(p, 0, bytes, scope.stream);
+                    if (ea != cudaSuccess) {
+                        if (p) cudaFreeAsync(p, scope.stream);
+                        fail(std::string("layered write state: ") + cudaGetErrorString(ea));
+                        return -1;
+                    }
+                    layered->state = static_cast<uint32_t*>(p);
+                }
+                G.layer_state = layered->state + 3 * batch0;
+                G.layer_parts = layered->nparts;
+                G.layer_claim = layered->calls == 0;
+            }
             // fp8 parts: the variant rule of the per-page fp8 path below
             e = fp8_elems ? kernels::launch_kv_gather_fp8(G, uint32_t(fp8_elems),
                                                           all_local ? kernels::kFp8LdSt
@@ -558,10 +622,25 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
             e = kernels::launch_kv_copy(L, scope.stream);
         }
         stats_.ns_launch += now_ns() - t_launch0;
-        if (scope.launched(e, "page mover launch failed: ", 1, write,
-                           uint64_t(m) * uint64_t(block_size)) != 0)
+        if (scope.launched(e, "page mover launch failed: ", 1, write, uint64_t(m) * moved) != 0)
             return -1;
-        sink.insert(sink.end(), batch_commits.begin(), batch_commits.end());
+        if (commit_now) sink.insert(sink.end(), batch_commits.begin(), batch_commits.end());
+    }
+    if (layered) {  // the writer's next call runs after these launches
+        cudaEvent_t ev = static_cast<cudaEvent_t>(layered->event);
+        cudaError_t e = ev ? cudaSuccess : cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+        if (e == cudaSuccess) {
+            layered->event = ev;
+            e = cudaEventRecord(ev, scope.stream);
+        }
+        if (e == cudaSuccess && commit_now && layered->state) {
+            e = cudaFreeAsync(layered->state, scope.stream);
+            layered->state = nullptr;
+        }
+        if (e != cudaSuccess) {
+            fail(std::string("layered write: ") + cudaGetErrorString(e));
+            return -1;
+        }
     }
     return 0;
 }
@@ -686,6 +765,99 @@ int Connection::w_rdma_gather_fp8(const GatherSpec& g, int elems, const uint64_t
     return move_blocks(true, offsets, 1, blocks, nblocks,
                        int(kernels::fp8_gather_bytes(g.nparts, uint32_t(elems))), 0, device,
                        stream, elems, nullptr, &w);
+}
+
+// Never waits for the device: an abandoned writer's state is freed on the per-thread stream
+// behind the writer's last launch.  Destroying a recorded event is safe while work is queued.
+Connection::GatherWriter::~GatherWriter() {
+    if (!event && !state) return;
+    DeviceGuard g(device);
+    if (state) {
+        if (event) cudaStreamWaitEvent(cudaStreamPerThread, static_cast<cudaEvent_t>(event), 0);
+        cudaFreeAsync(state, cudaStreamPerThread);
+    }
+    if (event) cudaEventDestroy(static_cast<cudaEvent_t>(event));
+    (void)cudaGetLastError();
+}
+
+std::shared_ptr<Connection::GatherWriter> Connection::gather_writer(const RemoteBlock* blocks,
+                                                                    const uint64_t* offsets,
+                                                                    size_t n, uint32_t nparts) {
+    auto w = std::make_shared<GatherWriter>();
+    w->nparts = nparts;
+    w->written.assign(nparts, 0);
+    std::lock_guard<std::mutex> lk(mu_);
+    w->session = session_;
+    for (size_t i = 0; i < n; ++i) {
+        if (is_fake_block(blocks[i])) continue;  // dedup: first writer wins
+        KeyHash kh{0, 0};
+        if (!pending_hash_.take(blocks[i].remote_addr, &kh)) w->indexed = false;
+        w->blocks.push_back(blocks[i]);
+        w->offsets.push_back(offsets[i]);
+        w->hashes.push_back(kh);
+    }
+    return w;
+}
+
+int Connection::write_layered(GatherWriter& w, const GatherSpec& g, int elems, uint64_t scale,
+                              int device, uint64_t stream) {
+    const uint64_t end = uint64_t(g.first_part) + g.nparts;
+    const bool first = w.device == -2;
+    const uint32_t part_bytes =
+        elems > 0 ? uint32_t(kernels::fp8_gather_bytes(1, uint32_t(elems))) : g.part_bytes;
+    uint64_t session;
+    {
+        std::lock_guard<std::mutex> lk(mu_);
+        session = session_;
+    }
+    const char* bad = nullptr;
+    if (w.session != session)
+        bad = "the connection was closed after the writer was made";
+    else if (w.failed || w.complete())
+        bad = "the writer is complete or has failed";
+    else if (!g.part_base || g.nparts < 1 || g.nparts > kernels::kGatherMaxParts || end > w.nparts)
+        bad = "the part range runs past the block";
+    else if (!first && (device != w.device || scale != w.scale || elems != w.elems ||
+                        part_bytes != w.part_bytes))
+        bad = "device, element size or part size differ from the writer's first call";
+    else if (!part_bytes || uint64_t(w.nparts) * part_bytes > uint64_t(INT32_MAX) ||
+             (elems && (elems < 0 || elems % 512 || device < 0)))
+        bad = "bad part size";
+    for (uint64_t s = g.first_part; !bad && s < end; ++s)
+        if (w.written[s]) bad = "the part range overlaps parts written before";
+    // every check before the writer changes: the first call's offsets are still in elements
+    std::vector<uint64_t> scaled;
+    if (!bad && first) {
+        scaled = w.offsets;
+        for (uint64_t& o : scaled) o *= scale;
+    }
+    const std::vector<uint64_t>& offs = first ? scaled : w.offsets;
+    if (!bad && elems && !gather_fp8_ok(g, elems, offs.data(), offs.size(), g.first_part))
+        bad = "fp8 parts need 16-byte aligned part bases and offsets";
+    if (bad) {
+        fail(std::string("write_layered: ") + bad);
+        return -1;
+    }
+    if (first) {
+        w.device = device;
+        w.scale = scale;
+        w.elems = elems;
+        w.part_bytes = part_bytes;
+        w.offsets.swap(scaled);
+    }
+    GatherSpec c = g;
+    c.part_bytes = part_bytes;
+    const int r = move_blocks(true, w.offsets.data(), 1, w.blocks.data(), w.blocks.size(),
+                              int(w.nparts * part_bytes), 0, device, stream, elems, nullptr, &c,
+                              &w);
+    if (r != 0) {
+        w.failed = true;
+        return r;
+    }
+    for (uint64_t s = g.first_part; s < end; ++s) w.written[s] = 1;
+    w.parts_written += g.nparts;
+    ++w.calls;
+    return 0;
 }
 
 int Connection::r_rdma_scatter_fp8(const GatherSpec& g, int elems,

@@ -373,6 +373,16 @@ bool Server::evict_some(size_t want, bool replica) {
     return true;
 }
 
+std::pair<uint64_t, uint64_t> Server::index_table() {
+    std::lock_guard<std::mutex> lk(mu_);
+    if (index_shards_.empty()) return {0, 0};
+    kernels::IndexBucket* table = nullptr;
+    uint64_t mask = 0;
+    kernels::IndexShards shards;
+    fill_index_view(&table, &mask, &shards);
+    return {reinterpret_cast<uint64_t>(table), (mask + 1) * kernels::kIndexWays};
+}
+
 std::vector<SegmentInfo> Server::segments() {
     std::lock_guard<std::mutex> lk(mu_);
     std::vector<SegmentInfo> v;

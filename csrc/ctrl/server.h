@@ -21,6 +21,7 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <utility>
 #include <vector>
 
 #include "../core/config.h"
@@ -98,6 +99,9 @@ class Server {
     size_t purge();
     ServerStats stats();
     std::vector<SegmentInfo> segments();
+    // Shard 0 of the device index: its address on the pool GPU and its slots ({0, 0} when the
+    // pool keeps no device index).  Lets tests of an in-process server inspect the index.
+    std::pair<uint64_t, uint64_t> index_table();
 
     // Checkpoint / resume (the reference has none: a restart loses everything, SURVEY §5.4).
     // dump: every committed block (key, size, bytes) to one file.  load: re-reserve, copy the

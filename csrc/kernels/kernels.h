@@ -134,6 +134,7 @@ cudaError_t launch_kv_pipe_copy(const CopyLaunch& a, cudaStream_t stream);
 // Gathered blocks: pool block i is the concatenation of `nparts` parts of part_bytes each,
 // part s taken from (write) or scattered to (read) part_base[s] + the block's local offset -
 // one page of every layer of a paged KV cache under one key, with no pack/unpack kernel.
+// first_part shifts which stored parts a launch covers, on both sides.
 // Work item = (block, part, chunk), numbered block * nparts * cpp + part * cpp + chunk, so a
 // chunk never crosses a part and the in-band commit (publish.cuh) counts nparts * cpp
 // arrivals per block.  The part bases travel in the kernel parameters.
@@ -147,7 +148,9 @@ struct GatherLaunch {
     const uint64_t* part_base = nullptr;  // host array of nparts absolute addresses
     uint32_t nparts = 0;
     uint32_t part_bytes = 0;
-    uint32_t first_part = 0;  // reads: pool part first_part + s lands in part s
+    // reads: pool part first_part + s lands in part s; writes: part s is stored as pool part
+    // first_part + s (a layered write, below, stores a block's parts over several launches)
+    uint32_t first_part = 0;
     uint64_t align_or = 0;    // OR of every part base and local offset
     // optional in-band commit (writes), as in CopyLaunch; recs[i].size covers all parts
     const IndexEntry* recs = nullptr;
@@ -160,6 +163,14 @@ struct GatherLaunch {
     IndexShards shards;
     uint32_t stage_bytes = 0;  // TMA pipeline geometry, 0 = default
     uint32_t ring_bytes = 0;
+    // Layered write (with recs): this launch stores nparts of the layer_parts parts of each
+    // block, and the block is published by whichever launch lands its last part
+    // (publish.cuh: control_warp_layered).  layer_state: 3 u32 per block, kept by the writer
+    // across its launches and zeroed before its first: slot + 1 | tag | parts landed.
+    // layer_claim: this launch claims the blocks' index ways (the writer's first call).
+    uint32_t* layer_state = nullptr;
+    uint32_t layer_parts = 0;
+    bool layer_claim = false;
 };
 // The TMA pipeline for 16-byte aligned parts of at least kPipeMinBytes, the ld/st kernel
 // (kv_copy.cu) otherwise: the same rule launch_kv_copy applies to whole blocks.

@@ -86,7 +86,7 @@ __global__ void __launch_bounds__(kLdStThreads + 32)
 
 // ---------------------------------------------------------------- gathered blocks (ld/st)
 // Item = chunk c of part s of block b, numbered (b * nparts + s) * cpp + c (GatherLaunch).
-// write: local parts.base[s] + desc.src -> pool desc.dst + s * part_bytes;
+// write: local parts.base[s] + desc.src -> pool desc.dst + (first_part + s) * part_bytes;
 // read:  pool desc.src + (first_part + s) * part_bytes -> local parts.base[s] + desc.dst.
 // The minimum of 3 CTAs per SM lets the 32-byte flavour keep 64 registers; without it ptxas
 // held it to 56 and spilled.
@@ -95,14 +95,14 @@ __global__ void __launch_bounds__(kLdStThreads + 32, 3)
     kv_gather_ldst_kernel(const CopyDesc* __restrict__ descs,
                           const __grid_constant__ GatherParts parts, uint32_t n, uint32_t nparts,
                           uint32_t part_bytes, uint32_t first_part, uint32_t chunk, uint32_t cpp,
-                          bool write, Publish pub) {
+                          bool write, Publish pub, LayerCommit lc) {
     const uint32_t cpb = nparts * cpp;  // items per block: what the commit counter counts
     const uint32_t total = n * cpb;
     if (threadIdx.x >= kLdStThreads) {
         if (!pub.recs) return;
         const uint32_t count = blockIdx.x < total ? (total - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-        control_warp(pub, threadIdx.x - kLdStThreads, blockIdx.x, count, gridDim.x, cpb,
-                     kLdStThreads + 32);
+        gather_control_warp(pub, lc, threadIdx.x - kLdStThreads, blockIdx.x, count, gridDim.x,
+                            cpb, nparts, kLdStThreads + 32);
         return;
     }
     uint32_t item = blockIdx.x;
@@ -120,8 +120,7 @@ __global__ void __launch_bounds__(kLdStThreads + 32, 3)
         const uint32_t off = (in_block % cpp) * chunk;
         const uint32_t len = min(chunk, part_bytes - off);
         const uint64_t local = parts.base[s] + (write ? d.src : d.dst) + off;
-        const uint64_t pool = (write ? d.dst + uint64_t(s) * part_bytes
-                                     : d.src + uint64_t(first_part + s) * part_bytes) + off;
+        const uint64_t pool = (write ? d.dst : d.src) + uint64_t(first_part + s) * part_bytes + off;
         uint8_t* dst = reinterpret_cast<uint8_t*>(write ? pool : local);
         const uint8_t* src = reinterpret_cast<const uint8_t*>(write ? local : pool);
         if constexpr (VEC == 1) {
@@ -208,7 +207,8 @@ cudaError_t launch_kv_gather(const GatherLaunch& a, cudaStream_t stream) {
     std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
     const auto go = [&](auto* kernel) {
         kernel<<<p.ctas, T, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.part_bytes, a.first_part,
-                                         p.chunk, p.cpb, a.write, publish_of(a, a.write));
+                                         p.chunk, p.cpb, a.write, publish_of(a, a.write),
+                                         layer_of(a));
         return cudaGetLastError();
     };
     switch (p.kernel) {

@@ -89,7 +89,7 @@ __device__ __forceinline__ void write_fp8(const CopyDesc* __restrict__ descs, ui
     if (threadIdx.x >= kThreads) {
         if (!pub.recs) return;
         const uint32_t count = blockIdx.x < total ? (total - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-        control_warp(pub, threadIdx.x - kThreads, blockIdx.x, count, gridDim.x, cpb, kThreads + 32);
+        pages.commit(pub, threadIdx.x - kThreads, blockIdx.x, count, gridDim.x, cpb, kThreads + 32);
         return;
     }
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -214,8 +214,10 @@ __global__ void __launch_bounds__(kThreads + 32)
     kv_write_fp8_gather_kernel(const CopyDesc* __restrict__ descs,
                                const __grid_constant__ GatherParts parts, uint32_t n,
                                uint32_t nparts, uint32_t elems, uint32_t chunk, uint32_t cpp,
-                               uint64_t stride, Publish pub) {
-    write_fp8(descs, n, elems, chunk, cpp, pub, BlockParts<true>{&parts, nparts, 0, stride});
+                               uint32_t first_part, uint64_t stride, Publish pub,
+                               LayerCommit lc) {
+    write_fp8(descs, n, elems, chunk, cpp, pub,
+              BlockParts<true>{&parts, nparts, first_part, stride, lc});
 }
 
 // The same loop as kv_read_fp8_kernel over the parts of gathered blocks.  A missing block
@@ -300,7 +302,8 @@ cudaError_t launch_kv_gather_fp8(const GatherLaunch& a, uint32_t elems, int vari
     const uint64_t stride = fp8_gather_bytes(1, elems);
     if (a.write)
         kv_write_fp8_gather_kernel<<<p.ctas, kThreads + 32, 0, stream>>>(
-            a.descs, parts, a.n, a.nparts, elems, p.chunk, p.cpb, stride, publish_of(a, true));
+            a.descs, parts, a.n, a.nparts, elems, p.chunk, p.cpb, a.first_part, stride,
+            publish_of(a, true), layer_of(a));
     else
         kv_read_fp8_scatter_kernel<<<p.ctas, kThreads, 0, stream>>>(
             a.descs, parts, a.n, a.nparts, a.first_part, elems, p.chunk, p.cpb, stride, a.status);

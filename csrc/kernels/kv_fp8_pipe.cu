@@ -114,7 +114,7 @@ __device__ __forceinline__ void fp8_pipe(const CopyDesc* __restrict__ descs, con
     __syncthreads();
     if (warp == 2) {  // control warp: in-band commit (writes) / resolver (fused reads)
         if (WRITE && pub.recs)
-            control_warp(pub, lane, blockIdx.x, nitems, grid, sh.cpb * pages.nparts, 64);
+            pages.commit(pub, lane, blockIdx.x, nitems, grid, sh.cpb * pages.nparts, 64);
         if (FUSED)
             resolver_warp(ra, rq, sh.elems + sh.elems / kRow * 4, blockIdx.x, grid,
                           sh.cpb, nitems, lane);
@@ -278,9 +278,10 @@ template <bool WRITE>
 __global__ void __launch_bounds__((3 + 8) * 32)
     kv_fp8_pipe_gather_kernel(const CopyDesc* __restrict__ descs, const Fp8Shape sh, Publish pub,
                               uint32_t* status, const __grid_constant__ GatherParts parts,
-                              uint32_t nparts, uint32_t first_part, uint64_t stride) {
+                              uint32_t nparts, uint32_t first_part, uint64_t stride,
+                              LayerCommit lc) {
     fp8_pipe<WRITE, 8, false>(descs, sh, pub, status, ResolveArgs{},
-                              BlockParts<WRITE>{&parts, nparts, first_part, stride});
+                              BlockParts<WRITE>{&parts, nparts, first_part, stride, lc});
 }
 
 constexpr size_t kSmemWrite = kInStages * kTileBf16 + kOutStages * (kTileQ + kTileScale);
@@ -334,10 +335,12 @@ cudaError_t launch_kv_fp8_pipe_gather(const GatherLaunch& a, uint32_t elems, cud
     const uint64_t stride = fp8_gather_bytes(1, elems);
     if (a.write)
         kv_fp8_pipe_gather_kernel<true><<<p.ctas, (3 + 8) * 32, kSmemWrite, stream>>>(
-            a.descs, sh, publish_of(a, true), a.status, parts, a.nparts, 0, stride);
+            a.descs, sh, publish_of(a, true), a.status, parts, a.nparts, a.first_part, stride,
+            layer_of(a));
     else
         kv_fp8_pipe_gather_kernel<false><<<p.ctas, (3 + 8) * 32, kSmemRead, stream>>>(
-            a.descs, sh, Publish{}, a.status, parts, a.nparts, a.first_part, stride);
+            a.descs, sh, Publish{}, a.status, parts, a.nparts, a.first_part, stride,
+            LayerCommit{});
     return cudaGetLastError();
 }
 

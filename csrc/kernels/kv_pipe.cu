@@ -221,10 +221,14 @@ __global__ void __launch_bounds__(kPipeThreads)
 // the virtual block b * nparts + s of part_bytes (sh.n virtual blocks, sh.cpb chunks each), so
 // global item numbers are those of GatherLaunch and the control warp counts nparts * sh.cpb
 // arrivals per real block.  The descriptor window walks the real blocks' descriptors.
+// LAYERED: a layered write's launch (publish.cuh: control_warp_layered).  It is a separate
+// instantiation because with both control-warp bodies in one kernel ptxas spilled registers.
+template <bool LAYERED>
 __global__ void __launch_bounds__(kPipeThreads)
     kv_pipe_gather_kernel(const CopyDesc* __restrict__ descs,
                           const __grid_constant__ GatherParts parts, const Shape sh,
-                          uint32_t nparts, uint32_t first_part, bool write, Publish pub) {
+                          uint32_t nparts, uint32_t first_part, bool write, Publish pub,
+                          LayerCommit lc) {
     extern __shared__ __align__(128) uint8_t ring[];
     __shared__ __align__(8) uint64_t full[kPipeMaxStages];
     __shared__ __align__(8) uint64_t empty[kPipeMaxStages];
@@ -242,7 +246,11 @@ __global__ void __launch_bounds__(kPipeThreads)
     }
     __syncthreads();
     if (warp == 2) {  // control warp: in-band commit
-        if (pub.recs) control_warp(pub, lane, blockIdx.x, nitems, grid, cpb, 64);
+        if (!pub.recs) return;
+        if constexpr (LAYERED)
+            control_warp_layered(pub, lc, lane, blockIdx.x, nitems, grid, cpb, nparts, 64);
+        else
+            control_warp(pub, lane, blockIdx.x, nitems, grid, cpb, 64);
         return;
     }
     DescWindow<false> win{descs, nullptr, blockIdx.x, grid, cpb, nitems, lane};
@@ -254,7 +262,7 @@ __global__ void __launch_bounds__(kPipeThreads)
         CopyDesc d;
         if (write) {
             d.src = parts.base[s] + b.src;
-            d.dst = b.dst + uint64_t(s) * sh.bytes;
+            d.dst = b.dst + uint64_t(first_part + s) * sh.bytes;
         } else {
             d.src = b.src ? b.src + uint64_t(first_part + s) * sh.bytes : 0;
             d.dst = parts.base[s] + b.dst;
@@ -599,7 +607,8 @@ cudaError_t ensure_pipe_attrs() {
         done, {{reinterpret_cast<const void*>(kv_pipe_copy_kernel<false>), kMax},
                {reinterpret_cast<const void*>(kv_pipe_copy_kernel<true>), kMax},
                {reinterpret_cast<const void*>(kv_pipe_read_kernel), kMax},
-               {reinterpret_cast<const void*>(kv_pipe_gather_kernel), kMax},
+               {reinterpret_cast<const void*>(kv_pipe_gather_kernel<false>), kMax},
+               {reinterpret_cast<const void*>(kv_pipe_gather_kernel<true>), kMax},
                {reinterpret_cast<const void*>(kv_pipe_scatter_read_kernel), kMax},
                {reinterpret_cast<const void*>(kv_pipe_mcast_kernel<2>), kMax},
                {reinterpret_cast<const void*>(kv_pipe_mcast_kernel<4>), kMax},
@@ -665,8 +674,10 @@ cudaError_t launch_kv_pipe_gather(const GatherLaunch& a, cudaStream_t stream) {
     const Shape sh{a.n * a.nparts, a.part_bytes, p.chunk, p.cpb, p.geo.stage_bytes, p.geo.stages};
     GatherParts parts;
     std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
-    kv_pipe_gather_kernel<<<p.ctas, kPipeThreads, p.geo.smem, stream>>>(
-        a.descs, parts, sh, a.nparts, a.first_part, a.write, publish_of(a, a.write));
+    const LayerCommit lc = layer_of(a);
+    auto* kernel = lc.state ? kv_pipe_gather_kernel<true> : kv_pipe_gather_kernel<false>;
+    kernel<<<p.ctas, kPipeThreads, p.geo.smem, stream>>>(a.descs, parts, sh, a.nparts, a.first_part,
+                                                         a.write, publish_of(a, a.write), lc);
     return cudaGetLastError();
 }
 

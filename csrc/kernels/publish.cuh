@@ -149,4 +149,73 @@ __device__ inline void control_warp(const Publish& pub, uint32_t lane, uint32_t 
     if (tr) tr[4] = globaltimer_ns();
 }
 
+// Layered gathered writes (GatherLaunch::layer_state): a writer stores each block's S parts over
+// several launches, k parts per launch.  The parts' chunking comes from each launch's own plan,
+// so no launch can count arrivals towards a fixed total; the count has two levels:
+//   launch-local  done[block] (the launch's zeroed scratch, as in control_warp) counts this
+//                 launch's cpb = k * cpp arrivals, each made after its lane's fence;
+//   writer-wide   the arrival that completes the launch's share adds k to the block's
+//                 parts-landed word with atom.add.acq_rel.gpu; the add that reaches S
+//                 publishes, with the slot and tag the writer's first launch claimed.
+// Ordering: it is control_warp's argument, extended across launches.  Every CTA of every
+// launch fences its stores before its launch-local increment, so a store is performed
+// system-wide before any increment that depends on it.  The completing arrival acquires
+// every earlier arrival of its launch through the launch-local counter.  The add that reaches
+// S acquires every earlier launch's adds through the writer-wide counter.  Earlier launches
+// were also complete before this one started, because the writer orders its launches.  So
+// when the tag store issues, every part of the block has been performed, as has the claim
+// (of this launch or an earlier one).  The tag needs no second fence.
+struct LayerCommit {
+    uint32_t* state = nullptr;  // 3 u32 per block: slot + 1 | tag | parts landed
+    uint32_t nparts = 0;        // S: parts of a whole block
+    uint32_t claim = 0;         // 1: this launch claims the blocks' index ways
+};
+
+inline LayerCommit layer_of(const GatherLaunch& a) {
+    return LayerCommit{a.write && a.recs ? a.layer_state : nullptr, a.layer_parts,
+                       a.layer_claim ? 1u : 0u};
+}
+
+// `k` parts of each block move in this launch (cpb = k * chunks per part).
+__device__ __forceinline__ void control_warp_layered(const Publish& pub, const LayerCommit& lc,
+                                            uint32_t lane, uint32_t first, uint32_t count,
+                                            uint32_t stride, uint32_t cpb, uint32_t k,
+                                            uint32_t cta_threads) {
+    uint32_t* done = pub.scratch;
+    if (lc.claim) {
+        for (uint32_t j = lane; j < count; j += 32) {
+            const uint32_t item = first + j * stride;
+            if (item % cpb) continue;
+            const uint32_t block = item / cpb;
+            const IndexEntry rec = pub.recs[block];
+            lc.state[3 * size_t(block)] = claim_entry(pub, rec);
+            lc.state[3 * size_t(block) + 1] = rec.tag;
+        }
+    }
+    ctrl_barrier_sync(cta_threads);
+    if (pub.sys)
+        fence_sys();
+    else
+        fence_gpu();
+    for (uint32_t j = lane; j < count; j += 32) {
+        const uint32_t block = (first + j * stride) / cpb;
+        if (atom_add_acq_rel_gpu(done + block, 1u) + 1 != cpb) continue;
+        done[block] = 0;  // leave the launch scratch zeroed for the next launch
+        uint32_t* st = lc.state + 3 * size_t(block);
+        if (atom_add_acq_rel_gpu(st + 2, k) + k != lc.nparts) continue;
+        commit_entry(pub, __ldcg(st), __ldcg(st + 1));
+    }
+}
+
+// The control warp of a gathered write: layered when the launch carries a writer's state.
+__device__ __forceinline__ void gather_control_warp(const Publish& pub, const LayerCommit& lc,
+                                           uint32_t lane, uint32_t first, uint32_t count,
+                                           uint32_t stride, uint32_t cpb, uint32_t k,
+                                           uint32_t cta_threads) {
+    if (lc.state)
+        control_warp_layered(pub, lc, lane, first, count, stride, cpb, k, cta_threads);
+    else
+        control_warp(pub, lane, first, count, stride, cpb, cta_threads);
+}
+
 }  // namespace istore::kernels

@@ -633,6 +633,40 @@ PYBIND11_MODULE(_infinistore, m) {
             "scattered fp8 read: fp8 page first_part + s of each block, dequantised -> "
             "part_base[s] + offset")
         .def(
+            "gather_writer",
+            [](Connection& c, const py::object& remote_blocks, const py::object& offsets,
+               uint32_t nparts) {
+                BlockSpan rb;
+                OffsetSpan off;
+                blocks_from_py(remote_blocks, rb);
+                offsets_from_py(offsets, off);
+                if (off.n != rb.n) throw std::invalid_argument("one offset per remote block");
+                if (nparts < 1 || nparts > kernels::kGatherMaxParts)
+                    throw std::invalid_argument("a block holds 1 to GATHER_MAX_PARTS parts");
+                py::gil_scoped_release rel;
+                return c.gather_writer(rb.data, off.data, rb.n, nparts);
+            },
+            py::arg("remote_blocks"), py::arg("offsets"), py::arg("nparts"),
+            "layered gathered writer over allocated blocks (offsets in elements)")
+        .def(
+            "w_rdma_layered",
+            [](Connection& c, Connection::GatherWriter& w, const std::vector<uint64_t>& part_base,
+               uint32_t part_bytes, int elems, uint32_t first_part, int device, uint64_t stream,
+               uint64_t scale) {
+                Connection::GatherSpec g;
+                g.part_base = part_base.data();
+                g.nparts = uint32_t(part_base.size());
+                g.part_bytes = part_bytes;
+                g.first_part = first_part;
+                py::gil_scoped_release rel;
+                return c.write_layered(w, g, elems, scale, device, stream);
+            },
+            py::arg("writer"), py::arg("part_base"), py::arg("part_bytes"), py::arg("elems"),
+            py::arg("first_part"), py::arg("device") = -1, py::arg("stream") = 0,
+            py::arg("scale") = 1,
+            "layered write: stored part first_part + s of every block of the writer <- "
+            "part_base[s] + offset * scale; elems > 0: fp8 parts of elems bf16 elements")
+        .def(
             "rw_local",
             [](Connection& c, const std::string& op, const py::object& blocks, int block_size,
                uint64_t base_ptr, int device, uint64_t stream, uint64_t scale) {
@@ -680,6 +714,17 @@ PYBIND11_MODULE(_infinistore, m) {
         });
 
     // ------------------------------------------------------------ server
+    py::class_<Connection::GatherWriter, std::shared_ptr<Connection::GatherWriter>>(
+        m, "GatherWriter")
+        .def_property_readonly("complete", &Connection::GatherWriter::complete)
+        .def_readonly("failed", &Connection::GatherWriter::failed)
+        .def_readonly("nparts", &Connection::GatherWriter::nparts)
+        .def_property_readonly("nblocks",
+                               [](const Connection::GatherWriter& w) { return w.blocks.size(); })
+        .def_property_readonly("written", [](const Connection::GatherWriter& w) {
+            return std::vector<bool>(w.written.begin(), w.written.end());
+        });
+
     py::class_<Server, std::shared_ptr<Server>>(m, "Server")
         .def(py::init<const ServerConfig&>())
         .def(
@@ -731,6 +776,8 @@ PYBIND11_MODULE(_infinistore, m) {
             },
             "Load a checkpoint file into the pool (existing keys win); returns blocks loaded")
         .def("stats", [](Server& s) { return stats_dict(s.stats()); })
+        .def("index_table", &Server::index_table,
+             "(address on the pool GPU, slots) of device-index shard 0; (0, 0) without one")
         .def("segments", [](Server& s) {
             py::list l;
             for (auto& i : s.segments()) l.append(segment_dict(i));
@@ -900,9 +947,12 @@ PYBIND11_MODULE(_infinistore, m) {
         [](uint64_t descs, uint32_t n, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
            uint32_t first_part, bool write, int max_ctas, uint64_t stream, uint64_t recs,
            uint64_t table, uint64_t table_mask, uint64_t done, uint64_t status, uint64_t align_or,
-           uint32_t stage_bytes, uint32_t ring_bytes) {
+           uint32_t stage_bytes, uint32_t ring_bytes, uint64_t layer_state, uint32_t layer_parts,
+           bool layer_claim) {
             if (part_base.empty() || part_base.size() > kernels::kGatherMaxParts)
                 throw std::runtime_error("kv_gather: 1 to GATHER_MAX_PARTS parts");
+            if (layer_state && first_part + part_base.size() > layer_parts)
+                throw std::runtime_error("kv_gather: first_part + parts > layer_parts");
             kernels::GatherLaunch G;
             G.descs = as_ptr<const kernels::CopyDesc>(descs);
             G.n = n;
@@ -920,6 +970,9 @@ PYBIND11_MODULE(_infinistore, m) {
             G.max_ctas = max_ctas;
             G.stage_bytes = stage_bytes;
             G.ring_bytes = ring_bytes;
+            G.layer_state = as_ptr<uint32_t>(layer_state);
+            G.layer_parts = layer_parts;
+            G.layer_claim = layer_claim;
             const cudaError_t e = kernels::launch_kv_gather(G, as_ptr<CUstream_st>(stream));
             if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
         },
@@ -928,16 +981,22 @@ PYBIND11_MODULE(_infinistore, m) {
         py::arg("stream") = 0, py::arg("recs") = 0, py::arg("table") = 0,
         py::arg("table_mask") = 0, py::arg("done") = 0, py::arg("status") = 0,
         py::arg("align_or") = 0, py::arg("stage_bytes") = 0, py::arg("ring_bytes") = 0,
+        py::arg("layer_state") = 0, py::arg("layer_parts") = 0, py::arg("layer_claim") = false,
         "gathered blocks: descs[i] = write {local byte offset, block address} / read {block "
-        "address or 0, local byte offset}; part s of block i at part_base[s] + local offset");
+        "address or 0, local byte offset}; part s of block i at part_base[s] + local offset is "
+        "stored part first_part + s.  layer_state (3 zeroed u32 per block, kept across the "
+        "launches of one layered write): the block is published by the launch that lands the "
+        "last of its layer_parts parts; layer_claim: this launch claims the index ways");
     k.def(
         "kv_gather_fp8",
         [](uint64_t descs, uint32_t n, const std::vector<uint64_t>& part_base, uint32_t elems,
            uint32_t first_part, bool write, int variant, int max_ctas, uint64_t stream,
            uint64_t recs, uint64_t table, uint64_t table_mask, uint64_t done, uint64_t status,
-           uint64_t align_or) {
+           uint64_t align_or, uint64_t layer_state, uint32_t layer_parts, bool layer_claim) {
             if (part_base.empty() || part_base.size() > kernels::kGatherMaxParts)
                 throw std::runtime_error("kv_gather_fp8: 1 to GATHER_MAX_PARTS parts");
+            if (layer_state && first_part + part_base.size() > layer_parts)
+                throw std::runtime_error("kv_gather_fp8: first_part + parts > layer_parts");
             kernels::GatherLaunch G;
             G.descs = as_ptr<const kernels::CopyDesc>(descs);
             G.n = n;
@@ -952,6 +1011,9 @@ PYBIND11_MODULE(_infinistore, m) {
             G.done = as_ptr<uint32_t>(done);
             G.status = as_ptr<uint32_t>(status);
             G.max_ctas = max_ctas;
+            G.layer_state = as_ptr<uint32_t>(layer_state);
+            G.layer_parts = layer_parts;
+            G.layer_claim = layer_claim;
             const cudaError_t e =
                 kernels::launch_kv_gather_fp8(G, elems, variant, as_ptr<CUstream_st>(stream));
             if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
@@ -960,9 +1022,11 @@ PYBIND11_MODULE(_infinistore, m) {
         py::arg("first_part") = 0, py::arg("write") = true, py::arg("variant") = 0,
         py::arg("max_ctas") = 0, py::arg("stream") = 0, py::arg("recs") = 0, py::arg("table") = 0,
         py::arg("table_mask") = 0, py::arg("done") = 0, py::arg("status") = 0,
-        py::arg("align_or") = 0,
+        py::arg("align_or") = 0, py::arg("layer_state") = 0, py::arg("layer_parts") = 0,
+        py::arg("layer_claim") = false,
         "gathered fp8 blocks: descs as for kv_gather; part s (elems bf16 elements at "
-        "part_base[s] + local offset) <-> fp8 page s of the block");
+        "part_base[s] + local offset) <-> fp8 page first_part + s of the block; layer_* as "
+        "for kv_gather");
     k.def(
         "kv_pipe_mcast",
         [](uint64_t descs, uint32_t n, uint32_t bytes, const std::vector<int64_t>& delta,

@@ -771,6 +771,32 @@ class InfinityConnection:
         if ret < 0:
             raise Exception(f"Failed to read to infinistore, ret = {ret}: {self.conn.last_error()}")
 
+    # ------------------------------------------------------------------ layered gathered writes
+    def gather_writer(self, remote_blocks, offsets, nparts: int, part_size: int,
+                      fp8: bool = False) -> "GatherWriter":
+        """A writer that stores the ``nparts`` parts of gathered blocks over several calls, as
+        prefill produces them (``GatherWriter.write``), instead of in one call after the last
+        layer.  ``remote_blocks`` were allocated with ``nparts * part_size * element_size``
+        bytes, or ``fp8_gather_block_bytes(nparts, part_size)`` with ``fp8``; ``offsets``
+        (elements) are the blocks' local offsets, the same in every call.  Each block becomes
+        readable once all of its parts have landed; until then it is missing to reads and
+        ``check_exist`` and, like any allocated key, counted by ``get_match_last_index``.
+        Blocks the server marked as already existing are skipped.  A writer that never
+        completes leaves its blocks uncommitted; closing the connection releases them."""
+        if self._mode != "rdma":
+            raise Exception("gathered blocks need a connected rdma connection")
+        offs = np.ascontiguousarray(offsets, dtype=np.int64).reshape(-1)
+        if len(offs) != len(remote_blocks):
+            raise ValueError(f"{len(offs)} offsets for {len(remote_blocks)} remote blocks")
+        if len(offs) and int(offs.min()) < 0:
+            raise ValueError("offsets must not be negative")
+        if not 1 <= int(nparts) <= GATHER_MAX_PARTS:
+            raise ValueError(f"a block holds 1 to {GATHER_MAX_PARTS} parts, not {nparts}")
+        if int(part_size) <= 0:
+            raise ValueError("part_size must be positive")
+        native = self.conn.gather_writer(remote_blocks, offs, int(nparts))
+        return GatherWriter(self, native, offs, int(nparts), int(part_size), bool(fp8))
+
     async def read_cache_async(self, cache: torch.Tensor, blocks: List[Tuple[str, int]],
                                page_size: int, stream="current"):
         if not self.rdma_connected:
@@ -952,3 +978,69 @@ class InfinityConnection:
 
     def segments(self):
         return self.conn.segments()
+
+
+class GatherWriter:
+    """Layered gathered write (``InfinityConnection.gather_writer``).  ``write`` stores a
+    contiguous range of parts of every block; once every part has been written, each block
+    holds exactly what one ``rdma_write_cache_gather`` (``_gather_fp8``) call would have
+    stored.  A call's kernels run after the caller's stream and after this writer's earlier
+    calls; ``sync()`` commits the blocks completed so far."""
+
+    def __init__(self, conn: "InfinityConnection", native, offsets: np.ndarray, nparts: int,
+                 part_size: int, fp8: bool):
+        self._conn = conn
+        self._w = native
+        self._offs = offsets
+        self._max_off = int(offsets.max()) if len(offsets) else 0
+        self.nparts = nparts
+        self.part_size = part_size
+        self.fp8 = fp8
+        self._dev = None  # (device, dtype) of the first call
+
+    @property
+    def complete(self) -> bool:
+        """Every part of every block has been written."""
+        return self._w.complete
+
+    @property
+    def failed(self) -> bool:
+        return self._w.failed
+
+    def write(self, parts, first_part: int, stream="current") -> None:
+        """Store parts ``first_part .. first_part + len(parts) - 1`` of every block: stored
+        part ``first_part + s`` of block i is ``parts[s][0].view(-1)[parts[s][1] + offsets[i]
+        : ... + part_size]``.  ``parts`` is ``[(tensor, base), ...]`` as for
+        ``rdma_write_cache_gather``.  The first call fixes the device and the dtype.  Raises
+        ``ValueError``, with nothing enqueued, for a range that overlaps parts written before
+        or runs past the block, another device or dtype, a complete or failed writer, and
+        everything ``rdma_write_cache_gather`` (``_gather_fp8``) refuses."""
+        if self._w.failed or self._w.complete:
+            raise ValueError("the writer is complete or has failed")
+        parts = list(parts)
+        first_part = int(first_part)
+        if first_part < 0 or first_part + len(parts) > self.nparts:
+            raise ValueError(f"parts {first_part}..{first_part + len(parts) - 1} run past the "
+                             f"block's {self.nparts} parts")
+        written = self._w.written
+        if any(written[first_part:first_part + len(parts)]):
+            raise ValueError("the part range overlaps parts written before")
+        conn = self._conn
+        bases, dev, es = conn._gather_parts(parts, self._max_off, self.part_size, fp8=self.fp8,
+                                            offsets=self._offs)
+        first = parts[0][0]
+        if self._dev is not None and self._dev != (first.device, first.dtype):
+            raise ValueError(f"parts on {first.device} as {first.dtype}, the writer's first call "
+                             f"used {self._dev[0]} as {self._dev[1]}")
+        block_bytes = (conn.fp8_gather_block_bytes(self.nparts, self.part_size) if self.fp8
+                       else self.nparts * self.part_size * es)
+        if block_bytes > _GATHER_MAX_BLOCK_BYTES:
+            raise ValueError(f"{self.nparts} parts of {self.part_size * es} bytes exceed the "
+                             f"{_GATHER_MAX_BLOCK_BYTES}-byte block limit")
+        self._dev = (first.device, first.dtype)
+        ret = conn.conn.w_rdma_layered(self._w, bases, self.part_size * es,
+                                       self.part_size if self.fp8 else 0, first_part, dev,
+                                       _stream_of(first, stream), es)
+        if ret < 0:
+            raise Exception(f"Failed to write to infinistore, ret = {ret}: "
+                            f"{conn.conn.last_error()}")

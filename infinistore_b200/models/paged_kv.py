@@ -120,6 +120,23 @@ class PagedKVCache:
         write(self._parts(layers), offs, elems, blocks, stream=stream)
         return len(keys)
 
+    def page_writer(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
+                    fp8: bool = False) -> "PageWriter":
+        """Allocate all-layer pages (as ``write_pages``) and return a writer that stores them
+        layer by layer: ``write_layers(range(l, l + 1))`` right after layer l has produced its
+        KV, so the upload overlaps the next layer's compute and one key per page is kept.
+        Read the pages back with ``read_pages(fp8=fp8)``."""
+        if fp8:
+            self._check_fp8()  # before any block is allocated
+        self._ensure_registered(conn)
+        nparts = 2 * self.layout.layers
+        elems = self.layout.page_elems
+        nbytes = (conn.fp8_gather_block_bytes(nparts, elems) if fp8
+                  else nparts * self.layout.page_bytes)
+        blocks = conn.allocate_rdma(self.page_keys(page_hashes), nbytes)
+        offs = np.asarray(pages, dtype=np.int64) * elems
+        return PageWriter(self, conn.gather_writer(blocks, offs, nparts, elems, fp8=fp8))
+
     def read_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
                    layers: Optional[range] = None, stream="current", fp8: bool = False) -> int:
         """Fetch pages written by ``write_pages`` into pages ``pages``.  ``layers`` (a range
@@ -169,6 +186,25 @@ class PagedKVCache:
             for kv in (0, 1):
                 keys.extend(self.keys(layer, kv, page_hashes))
         return conn.touch(keys) if keys else 0
+
+
+class PageWriter:
+    """Layer-by-layer upload of all-layer pages (``PagedKVCache.page_writer``)."""
+
+    def __init__(self, cache: PagedKVCache, writer):
+        self.cache = cache
+        self.writer = writer
+
+    @property
+    def complete(self) -> bool:
+        return self.writer.complete
+
+    def write_layers(self, layers: range, stream="current") -> None:
+        """Store the K and V parts of ``layers`` (a non-empty step-1 range) of every page."""
+        n = self.cache.layout.layers
+        if layers.step != 1 or not len(layers) or layers.start < 0 or layers.stop > n:
+            raise ValueError(f"layers must be a non-empty step-1 range within 0..{n}")
+        self.writer.write(self.cache._parts(layers), 2 * layers.start, stream=stream)
 
 
 def read_layer_multi(conn, caches: Sequence[PagedKVCache], layer: int, pages: Sequence[int],

@@ -61,23 +61,44 @@ def kv_copy(descs: torch.Tensor, nbytes: int, variant: str = "auto", max_ctas: i
                   stage_bytes, ring_bytes, [int(d) for d in fan_deltas] if fan_deltas else [])
 
 
+class LayerState:
+    """The per-block state of a layered gathered write (``GatherLaunch::layer_state``), kept
+    across its launches: slot + 1 | tag | parts landed, zeroed before the first launch."""
+
+    def __init__(self, nblocks: int, nparts: int, device):
+        self.state = torch.zeros(3 * nblocks, dtype=torch.int32, device=device)
+        self.nparts = nparts
+
+
+def _publish_args(publish: Optional["PublishArgs"], layer: Optional[LayerState], claim: bool):
+    return ((publish.recs.data_ptr(), publish.table.data_ptr(), publish.mask,
+             publish.done.data_ptr()) if publish else (0, 0, 0, 0),
+            (layer.state.data_ptr(), layer.nparts, bool(claim)) if layer else (0, 0, False))
+
+
 def kv_gather(descs: torch.Tensor, part_base: Sequence[int], part_bytes: int, write: bool,
               first_part: int = 0, max_ctas: int = 0, status: Optional[torch.Tensor] = None,
-              align_or: int = 0, stage_bytes: int = 0, ring_bytes: int = 0) -> None:
+              align_or: int = 0, stage_bytes: int = 0, ring_bytes: int = 0,
+              publish: Optional["PublishArgs"] = None, layer: Optional[LayerState] = None,
+              claim: bool = False) -> None:
     """Gathered blocks (csrc/kernels/kernels.h ``GatherLaunch``): block i is len(part_base)
     parts of ``part_bytes``, part s at ``part_base[s] + local offset``.  ``descs`` is (n, 2)
     int64: write {local byte offset, block address}, read {block address or 0 = miss, local
-    byte offset}; a read moves stored parts first_part... .  ``align_or`` must include the
-    local offsets (the part bases are added here): it picks the vector width."""
+    byte offset}; both move stored parts first_part... .  ``align_or`` must include the
+    local offsets (the part bases are added here): it picks the vector width.  A write with
+    ``publish`` commits its blocks in the index; with ``layer`` too it is one launch of a
+    layered write (``claim``: its first), which publishes a block once all of
+    ``layer.nparts`` parts have landed."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
     bases = [int(b) for b in part_base]
     for b in bases:
         align_or |= b
+    pub, lay = _publish_args(publish, layer, claim)
     with torch.cuda.device(descs.device):
         K.kv_gather(descs.data_ptr(), descs.shape[0], bases, part_bytes, first_part, write,
-                    max_ctas, _stream(descs.device), 0, 0, 0, 0,
+                    max_ctas, _stream(descs.device), *pub,
                     status.data_ptr() if status is not None else 0, align_or, stage_bytes,
-                    ring_bytes)
+                    ring_bytes, *lay)
 
 
 def kv_copy_multicast(descs: torch.Tensor, nbytes: int, dst_deltas: Sequence[int],
@@ -266,26 +287,24 @@ def fp8_gather_bytes(nparts: int, elems: int) -> int:
 def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, write: bool,
                   first_part: int = 0, max_ctas: int = 0, status: Optional[torch.Tensor] = None,
                   align_or: int = 0, publish: Optional[PublishArgs] = None,
-                  variant: str = "auto") -> None:
+                  variant: str = "auto", layer: Optional[LayerState] = None,
+                  claim: bool = False) -> None:
     """Gathered fp8 blocks (``kv_gather`` with quantisation): part s of block i is a bf16 page
-    of ``elems`` elements at ``part_base[s] + local offset`` and fp8 page s of the block, at
-    byte ``fp8_gather_bytes(s, elems)``.  ``descs`` as for ``kv_gather``.  ``variant``:
-    "ldst" = the ld/st kernels (kv_fp8.cu), "auto" / "tma" = the TMA pipeline
-    (kv_fp8_pipe.cu).  ``align_or`` must include the local offsets (the part bases are added
-    here): unaligned batches are refused."""
+    of ``elems`` elements at ``part_base[s] + local offset`` and fp8 page first_part + s of
+    the block, at byte ``fp8_gather_bytes(first_part + s, elems)``.  ``descs``, ``layer`` and
+    ``claim`` as for ``kv_gather``.  ``variant``: "ldst" = the ld/st kernels (kv_fp8.cu),
+    "auto" / "tma" = the TMA pipeline (kv_fp8_pipe.cu).  ``align_or`` must include the local
+    offsets (the part bases are added here): unaligned batches are refused."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
     bases = [int(b) for b in part_base]
     for b in bases:
         align_or |= b
+    pub, lay = _publish_args(publish, layer, claim)
     with torch.cuda.device(descs.device):
         K.kv_gather_fp8(descs.data_ptr(), descs.shape[0], bases, elems, first_part, write,
                         FP8_VARIANTS["ldst"] if variant == "ldst" else FP8_VARIANTS["auto"],
-                        max_ctas, _stream(descs.device),
-                        publish.recs.data_ptr() if publish else 0,
-                        publish.table.data_ptr() if publish else 0,
-                        publish.mask if publish else 0,
-                        publish.done.data_ptr() if publish else 0,
-                        status.data_ptr() if status is not None else 0, align_or)
+                        max_ctas, _stream(descs.device), *pub,
+                        status.data_ptr() if status is not None else 0, align_or, *lay)
 
 
 def fp8_reference(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
