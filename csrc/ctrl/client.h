@@ -177,6 +177,19 @@ class Connection {
                    uint64_t stream);
     int r_rdma_fp8(const std::vector<KeyOffset>& blocks, int elems, uint64_t base_ptr, int device,
                    uint64_t stream);
+    // Layered read (read_scatter_layered): one call whose last page-mover launch releases the
+    // parts group by group, `group_parts` parts per group, each by storing `seq` to its flag
+    // word.  wait(g, stream) makes later work on `stream` wait on the GPU until group g has
+    // landed (cuStreamWaitValue32), with no host synchronisation.
+    struct ScatterReader {
+        uint32_t groups = 0;
+        uint32_t group_parts = 0;
+        int device = -1;
+        uint64_t seq = 0;                 // 0: nothing was launched (no blocks); waits are no-ops
+        const uint32_t* flags = nullptr;  // device: one word per group, in the reader's slot
+        bool failed = false;              // refused or failed: every wait is refused
+        uint64_t session = 0;             // the connection session whose device flags it uses
+    };
     // Gathered blocks (kernels::GatherLaunch): a block is `nparts` parts of part_bytes, part s
     // at part_base[s] + the block's local byte offset (one page of every layer under one key).
     struct GatherSpec {
@@ -184,6 +197,7 @@ class Connection {
         uint32_t nparts = 0;
         uint32_t part_bytes = 0;  // pool bytes of a part (fp8: fp8_gather_bytes(1, elems))
         uint32_t first_part = 0;  // stored part first_part + s is part s (one-shot writes: 0)
+        ScatterReader* reader = nullptr;  // reads: a layered read (read_scatter_layered)
     };
     // Layered gathered write: a fixed set of allocated gathered blocks whose parts are stored
     // over several calls (write_layered), each a contiguous range of parts of every block -
@@ -238,6 +252,18 @@ class Connection {
                           uint64_t stream);
     int r_rdma_scatter_fp8(const GatherSpec& g, int elems, const std::vector<KeyOffset>& blocks,
                            int device, uint64_t stream);
+    // Layered read: r_rdma_scatter (elems == 0) or r_rdma_scatter_fp8 (elems > 0) in one call,
+    // whose parts are released to `r`'s waits in groups of group_parts (which must divide
+    // g.nparts).  Each key is resolved once.  CUDA tensors of an HBM pool only; not on a
+    // doorbell connection.  On failure r.failed is set and every wait is refused.
+    int read_scatter_layered(const GatherSpec& g, int elems, uint32_t group_parts,
+                             const std::vector<KeyOffset>& blocks, int device, uint64_t stream,
+                             ScatterReader& r);
+    // Later work on `stream` waits on the GPU until group `group` of `r` has landed.  0; -1
+    // (and *err) when refused: a failed reader, a group outside the read, or a reader made
+    // before the connection was last closed (its flags were freed with the device context);
+    // -2 (and *err) when the driver refuses the wait.  Nothing is enqueued unless 0.
+    int wait_layered(const ScatterReader& r, uint32_t group, uint64_t stream, std::string* err);
 
     // --- async flavours: the callback runs on the connection's completion thread
     int allocate_async(const std::vector<std::string>& keys, int block_size,
@@ -306,6 +332,10 @@ class Connection {
     kernels_IndexShards index_shards(DevCtx* ctx, bool* all_local);
     kernels::GatherLaunch gather_launch(const GatherSpec& g, uint32_t n, uint64_t align_or,
                                         uint32_t* status, int max_ctas);
+    // a layered read's last launch: takes the reader's slot (0 on failure, else its seq)
+    uint64_t arm_reader(DevCtx* ctx, const ScatterReader& r, kernels::GatherLaunch& G);
+    int reader_launched(DevCtx* ctx, ScatterReader& r, uint64_t seq, void* stream);
+    struct ReaderHold;
     template <typename Launch>
     bool set_index(DevCtx* ctx, Launch& L, bool segs = true);
     const kernels_CopyDesc* resolve_descs(DevCtx* ctx, const std::vector<KeyOffset>& blocks,

@@ -250,6 +250,27 @@ struct Connection::LaunchScope {
     }
 };
 
+// A layered read's slot from arm_reader on (seq != 0).  Whichever way the call ends, the slot
+// is marked live with an event recorded behind everything the call enqueued, so that the next
+// reader of the slot waits for the flagged launch whenever it was enqueued: a later failure
+// (the validate launch, a failed batch) must not hand the slot on while that launch may still
+// store its smaller seq over the next reader's flags.  done() ends a call that succeeded.
+struct Connection::ReaderHold {
+    Connection& c;
+    DevCtx* ctx;
+    ScatterReader* r;
+    cudaStream_t stream;
+    uint64_t seq = 0;
+    int done() {
+        const uint64_t s = seq;
+        seq = 0;
+        return c.reader_launched(ctx, *r, s, stream);
+    }
+    ~ReaderHold() {
+        if (seq) c.reader_launched(ctx, *r, seq, stream);  // the call failed: r is failed too
+    }
+};
+
 // The parts of a gathered launch of n blocks whose local offsets OR to `align_or` (the part
 // bases' alignment counts with theirs); descriptors and commit fields are the caller's.
 kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n, uint64_t align_or,
@@ -448,6 +469,7 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
         }
     }
     if (scope.begin(stream_in, write) != 0) return -1;
+    ReaderHold hold{*this, ctx, gather ? gather->reader : nullptr, scope.stream};
     if (layered && layered->event &&
         cudaStreamWaitEvent(scope.stream, static_cast<cudaEvent_t>(layered->event), 0) !=
             cudaSuccess) {
@@ -592,6 +614,10 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
                 G.layer_parts = layered->nparts;
                 G.layer_claim = layered->calls == 0;
             }
+            if (gather->reader && i >= n) {  // a layered read's flags ride on its last launch
+                hold.seq = arm_reader(ctx, *gather->reader, G);
+                if (!hold.seq) return -1;
+            }
             // fp8 parts: the variant rule of the per-page fp8 path below
             e = fp8_elems ? kernels::launch_kv_gather_fp8(G, uint32_t(fp8_elems),
                                                           all_local ? kernels::kFp8LdSt
@@ -642,7 +668,111 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
             return -1;
         }
     }
+    if (hold.seq) return hold.done();
     return 0;
+}
+
+// The slot flags are zeroed, and the zeroing has completed, before any reader is handed a
+// slot: a consumer's wait runs on its own stream and must never see uninitialised words.
+uint64_t Connection::arm_reader(DevCtx* ctx, const ScatterReader& r, kernels::GatherLaunch& G) {
+    if (!ctx->group_flags) {
+        const size_t bytes = size_t(kReaderSlots) * kernels::kGatherMaxParts * sizeof(uint32_t);
+        void* p = nullptr;
+        cudaError_t e = cudaMalloc(&p, bytes);
+        if (e == cudaSuccess) e = cudaMemsetAsync(p, 0, bytes, ctx->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+        if (e != cudaSuccess) {
+            if (p) cudaFree(p);
+            fail(std::string("layered read flags: ") + cudaGetErrorString(e));
+            return 0;
+        }
+        ctx->group_flags = static_cast<uint32_t*>(p);
+    }
+    // cuStreamWaitValue32's GEQ compares cyclically, (int32_t)(*addr - seq) >= 0: a word
+    // that lags seq by 2^31 or more would satisfy the wait at once, so seq stays below 2^31
+    if (ctx->readers.last() >= uint64_t(INT32_MAX)) {
+        fail("layered read: a connection serves 2^31 - 1 layered reads per device");
+        return 0;
+    }
+    const uint64_t seq = ctx->readers.take([ctx](cudaEvent_t ev) {
+        if (cudaEventQuery(ev) != cudaErrorNotReady) return;  // done, or failed: sync() reports it
+        cudaEventSynchronize(ev);
+        if (ctx->drains) ++*ctx->drains;
+    });
+    G.group_flags = ctx->group_flags + size_t(ctx->readers.slot_of(seq)) * kernels::kGatherMaxParts;
+    G.group_counters =
+        reinterpret_cast<uint32_t*>(ctx->zeros + ctx->zeros_alloc(size_t(r.groups) * 4));
+    G.group_seq = uint32_t(seq);
+    G.group_parts = r.group_parts;
+    return seq;
+}
+
+// After the call's last launch: the slot is held until the reader's launches complete.
+int Connection::reader_launched(DevCtx* ctx, ScatterReader& r, uint64_t seq, void* stream) {
+    const uint32_t slot = ctx->readers.slot_of(seq);
+    cudaEvent_t& ev = ctx->reader_ev[slot];
+    cudaError_t e = ev ? cudaSuccess : cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaEventRecord(ev, static_cast<cudaStream_t>(stream));
+    if (e != cudaSuccess) {
+        fail(std::string("layered read: ") + cudaGetErrorString(e));
+        return -1;
+    }
+    ctx->readers.launched(seq, ev);
+    r.seq = seq;
+    r.flags = ctx->group_flags + size_t(slot) * kernels::kGatherMaxParts;
+    return 0;
+}
+
+int Connection::wait_layered(const ScatterReader& r, uint32_t group, uint64_t stream,
+                             std::string* err) {
+    std::lock_guard<std::mutex> lk(mu_);  // close() cannot free the flags under the wait
+    const char* bad = r.failed               ? "the read failed, so its groups are never released"
+                      : group >= r.groups    ? "the group is outside the read"
+                      : r.session != session_ ? "the connection was closed after the read"
+                                             : nullptr;
+    if (bad) {
+        if (err) *err = bad;
+        return -1;
+    }
+    if (r.seq == 0) return 0;  // nothing was read
+    DeviceGuard g(r.device);
+    const cudaError_t e = kernels::stream_wait_geq(r.flags + group, uint32_t(r.seq),
+                                                   reinterpret_cast<cudaStream_t>(stream));
+    if (e != cudaSuccess) {
+        (void)cudaGetLastError();
+        if (err) *err = std::string("stream wait: ") + cudaGetErrorString(e);
+        return -2;
+    }
+    return 0;
+}
+
+int Connection::read_scatter_layered(const GatherSpec& g, int elems, uint32_t group_parts,
+                                     const std::vector<KeyOffset>& blocks, int device,
+                                     uint64_t stream, ScatterReader& r) {
+    r = ScatterReader{};
+    r.device = device;
+    {
+        std::lock_guard<std::mutex> lk(mu_);
+        r.session = session_;
+    }
+    r.group_parts = group_parts;
+    r.groups = group_parts && g.nparts % group_parts == 0 ? g.nparts / group_parts : 0;
+    const char* bad = device < 0      ? "needs CUDA tensors"
+                      : !server_hbm_  ? "needs a pool in GPU memory"
+                      : cfg_.doorbell ? "is not available on a doorbell connection"
+                      : !r.groups     ? "needs group_parts that divides the part count"
+                                      : nullptr;
+    if (bad) {
+        r.failed = true;
+        fail(std::string("layered read ") + bad);
+        return -1;
+    }
+    GatherSpec l = g;
+    l.reader = &r;
+    const int rc = elems > 0 ? r_rdma_scatter_fp8(l, elems, blocks, device, stream)
+                             : r_rdma_scatter(l, blocks, device, stream);
+    if (rc != 0) r.failed = true;
+    return rc;
 }
 
 int Connection::w_rdma(const uint64_t* offsets, size_t noffsets, uint64_t scale, int block_size,
@@ -929,6 +1059,8 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
     }
     if (scope.begin(stream_in, false) != 0) return -1;
     const size_t max_batch = gather ? gather_batch_cap(*gather, fp8_elems) : kMaxBatch;
+    const bool layered = gather && gather->reader;
+    ReaderHold hold{*this, ctx, layered ? gather->reader : nullptr, scope.stream};
     KeyBatch b;
     for (size_t base = 0; base < blocks.size(); base += b.n) {
         const uint64_t t_build0 = now_ns();
@@ -943,7 +1075,8 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
         DeviceReadIn in{.n = n, .block_bytes = uint32_t(block_size),
                         .fp8_elems = uint32_t(fp8_elems), .gather = gather != nullptr,
                         .copy_variant = copy_variant_, .all_local = true, .all_remote = true,
-                        .max_ctas = max_ctas_, .sm_count = kernels::sm_count()};
+                        .max_ctas = max_ctas_, .sm_count = kernels::sm_count(),
+                        .layered = layered};
         // over every known segment, not only the ones this batch touches: intentional
         for (uint32_t s = 0; s < R.nsegs; ++s) {
             in.all_remote = in.all_remote && ctx->seg_remote[s];
@@ -994,6 +1127,10 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
                 fail("device-index read: cannot resolve the blocks");
                 return -1;
             }
+            if (layered && base + n == blocks.size()) {  // the flags ride on the last launch
+                hold.seq = arm_reader(ctx, *gather->reader, G);
+                if (!hold.seq) return -1;
+            }
             if (plan.path == ReadPath::kLookupGather) {
                 G.descs = descs;  // {pool address or 0, local byte offset} (dst_base 0)
                 e = kernels::launch_kv_gather(G, scope.stream);
@@ -1042,6 +1179,7 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
                            uint64_t(n) * uint64_t(block_size)) != 0)
             return -1;
     }
+    if (hold.seq) return hold.done();
     return 0;
 }
 

@@ -23,6 +23,7 @@ inline constexpr size_t kRingBytes = 16u << 20;     // pinned, mapped staging ri
 inline constexpr size_t kScratchBytes = 8u << 20;   // device scratch per device
 inline constexpr size_t kZeroBytes = 2u << 20;      // self-cleaning zeroed counters per device
 inline constexpr size_t kMaxBatch = 65536;          // blocks per kernel launch
+inline constexpr int kReaderSlots = 64;             // layered reads in flight per device
 
 struct DeviceGuard {
     int prev = -1;
@@ -85,6 +86,12 @@ struct Connection::DevCtx {
     uint32_t* status_d = nullptr;
     std::vector<cudaStream_t> busy;  // streams with launches since the last wait_all()
     bool dirty = false;
+    // Layered reads (Connection::read_scatter_layered): kReaderSlots slots of kGatherMaxParts
+    // group flags, allocated and zeroed on the first such read; reader seq uses slot
+    // seq % kReaderSlots (staging.h: ReaderSlots), whose event completes with its launches.
+    uint32_t* group_flags = nullptr;
+    ReaderSlots<cudaEvent_t, kReaderSlots> readers;
+    cudaEvent_t reader_ev[kReaderSlots] = {};
 
     // Doorbell worker (ClientConfig::doorbell): request ring + control block in pinned,
     // device-mapped host memory; `posted` / `collected` are request numbers.
@@ -177,6 +184,9 @@ struct Connection::DevCtx {
         }
         if (user_ev) cudaEventDestroy(user_ev);
         for (cudaEvent_t ev; staging.take_free(&ev);) cudaEventDestroy(ev);
+        for (cudaEvent_t ev : reader_ev)
+            if (ev) cudaEventDestroy(ev);
+        if (group_flags) cudaFree(group_flags);
         if (stream) {
             cudaStreamSynchronize(stream);
             cudaStreamDestroy(stream);
@@ -209,6 +219,7 @@ struct Connection::DevCtx {
         busy.clear();
         dirty = false;
         staging.retire_all();
+        readers.retire_all();
     }
     cudaStream_t last = nullptr;  // stream of the most recent launch
     // Staging reuse (staging.h): one event per launch, recorded behind it on its stream.  A

@@ -20,6 +20,7 @@ struct DeviceReadIn {
     // over every known segment (up to kMaxSegs), not only the batch's: intentional
     bool all_local = false, all_remote = false;
     int max_ctas = 0, sm_count = 0;  // max_ctas: the connection's grid cap, 0 = none
+    bool layered = false;  // a layered read of gathered blocks (GatherLaunch::group_flags)
 };
 
 enum class ReadPath {
@@ -73,6 +74,13 @@ inline DeviceReadPlan plan_device_read(const DeviceReadIn& in) {
     // lookup + read + validate: 32 calls of 512 pages were launch-bound).
     // gathered fp8 blocks: each key is probed once by the lookup kernel and re-checked after the
     // dequantising scatter; never the bf16 scatter pipeline.
+    // layered reads: lookup, the layered ld/st scatter (the only kernels that release groups),
+    // validate - each key probed once, by the lookup kernel
+    if (in.gather && in.layered) {
+        p.path = in.fp8_elems ? ReadPath::kLookupGatherFp8 : ReadPath::kLookupGather;
+        p.variant = in.fp8_elems ? int(kernels::kFp8LdSt) : int(kernels::kCopyLdSt);
+        return p;
+    }
     if (in.gather && in.fp8_elems)
         p.path = ReadPath::kLookupGatherFp8;
     else if (in.gather)

@@ -86,6 +86,49 @@ class StagingFifo {
     uint64_t first_[R];  // first byte placed since the last push, kNone when there is none
 };
 
+// The flag slots of layered reads (client_dev.h: DevCtx::group_flags).  Reader seq = 1, 2, ...
+// owns slot seq % Slots.  A slot's flag words only grow and a consumer waits for
+// flag >= seq, so a later reader's flags never un-release an earlier reader's wait, and a
+// wait enqueued late is still satisfied.  A slot is handed to the next reader once the
+// launches of the reader that held it one lap earlier have completed: take() passes only that
+// reader to wait(ev).  No CUDA in here (Event is a plain handle), so the ring is unit-tested
+// on the CPU.
+template <typename Event, int Slots>
+class ReaderSlots {
+   public:
+    // The next reader's sequence number; its slot is free to use when take() returns.
+    template <typename Wait>
+    uint64_t take(Wait&& wait) {
+        const uint64_t seq = ++seq_;
+        Slot& s = slots_[seq % Slots];
+        if (s.live) {
+            wait(s.ev);
+            s.live = false;
+        }
+        return seq;
+    }
+    // Reader seq's launches complete with ev.  A reader that launched nothing is never waited for.
+    void launched(uint64_t seq, Event ev) {
+        Slot& s = slots_[seq % Slots];
+        s.ev = ev;
+        s.live = true;
+    }
+    // Every reader has completed (the device context was drained).
+    void retire_all() {
+        for (Slot& s : slots_) s.live = false;
+    }
+    uint64_t last() const { return seq_; }
+    static uint32_t slot_of(uint64_t seq) { return uint32_t(seq % Slots); }
+
+   private:
+    struct Slot {
+        Event ev{};
+        bool live = false;
+    };
+    Slot slots_[Slots];
+    uint64_t seq_ = 0;
+};
+
 // One launch's share of a call's keys, taken from the front of the `left` keys still to go:
 // at most max_blocks keys, whose staged bytes stay within max_bytes.  A key stages its bytes
 // zero padded to a multiple of 8 (an empty key takes 8) plus 16 bytes of offset, length and

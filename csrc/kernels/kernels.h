@@ -171,6 +171,15 @@ struct GatherLaunch {
     uint32_t* layer_state = nullptr;
     uint32_t layer_parts = 0;
     bool layer_claim = false;
+    // Layered read (reads only, ld/st kernels only): the launch walks the parts in groups of
+    // group_parts (2 = one layer's K and V), numbered group-major (launch_plan.h:
+    // layered_item), and releases group g by storing group_seq to group_flags[g] once every
+    // block's parts of g have landed (publish.cuh: leave_group).  A missing block's items count
+    // as landed.  group_counters: nparts / group_parts zeroed u32, left zeroed.
+    uint32_t* group_flags = nullptr;
+    uint32_t* group_counters = nullptr;
+    uint32_t group_seq = 0;
+    uint32_t group_parts = 0;
 };
 // The TMA pipeline for 16-byte aligned parts of at least kPipeMinBytes, the ld/st kernel
 // (kv_copy.cu) otherwise: the same rule launch_kv_copy applies to whole blocks.
@@ -447,6 +456,10 @@ cudaError_t launch_kv_doorbell(const DoorbellLaunch& a, cudaStream_t stream);
 
 // Number of SMs of the current device (cached per device).
 int sm_count();
+// Later work on `stream` waits, on the GPU, until *addr >= value (cuStreamWaitValue32, GEQ):
+// how a consumer waits for a layered read's group flags without a host round trip.
+// cudaErrorNotSupported when the driver does not offer the entry point.
+cudaError_t stream_wait_geq(const uint32_t* addr, uint32_t value, cudaStream_t stream);
 // Raises the dynamic shared-memory limit of each kernel to its `bytes`, once per device:
 // `done` holds the caller's flag of every device.
 struct SmemLimit {

@@ -18,12 +18,15 @@
 //   kCopyLdSt / kCopyLdSt256 : this file - every thread streams 128-bit vectors, 4 (or,
 //               for 32-byte aligned blocks, 8) in flight per thread; used for small or
 //               unaligned blocks and for NVLS multicast stores (multimem.st has no bulk form).
+#include <cuda.h>
+
 #include <cstring>
 #include <mutex>
 
 #include "common.cuh"
 #include "kernels.h"
 #include "copy_span.cuh"
+#include "launch_plan.h"
 #include "publish.cuh"
 
 namespace istore::kernels {
@@ -85,17 +88,66 @@ __global__ void __launch_bounds__(kLdStThreads + 32)
 }
 
 // ---------------------------------------------------------------- gathered blocks (ld/st)
+// The layered read (GatherLaunch::group_flags): items numbered group-major
+// (launch_plan.h: layered_item), group g released by leave_group (publish.cuh) when this
+// CTA's stream leaves it.  A missing block counts once, on its first item (group 0, part 0,
+// chunk 0), and its parts are left untouched; its items still count as arrivals.
+template <int VEC>
+__device__ __forceinline__ void gather_read_layered(const CopyDesc* __restrict__ descs,
+                                                    const GatherParts& parts, uint32_t n,
+                                                    uint32_t nparts, uint32_t part_bytes,
+                                                    uint32_t first_part, uint32_t chunk,
+                                                    uint32_t cpp, uint32_t* status,
+                                                    const GroupRelease& rel) {
+    const uint32_t group_items = n * rel.gp * cpp;
+    const uint32_t total = n * nparts * cpp;
+    uint32_t item = blockIdx.x;
+    CopyDesc next = item < total ? descs[layered_item(item, n, rel.gp, cpp).block] : CopyDesc{0, 0};
+    for (; item < total; item += gridDim.x) {
+        const CopyDesc d = next;
+        const LayeredItem it = layered_item(item, n, rel.gp, cpp);
+        const uint32_t nxt = item + gridDim.x;
+        if (nxt < total) next = descs[layered_item(nxt, n, rel.gp, cpp).block];
+        if (d.src != 0) {
+            const uint32_t off = it.chunk * chunk;
+            const uint32_t len = min(chunk, part_bytes - off);
+            uint8_t* dst = reinterpret_cast<uint8_t*>(parts.base[it.part] + d.dst + off);
+            const uint8_t* src = reinterpret_cast<const uint8_t*>(
+                d.src + uint64_t(first_part + it.part) * part_bytes + off);
+            if constexpr (VEC == 1) {
+                for (uint32_t b = threadIdx.x; b < len; b += kLdStThreads) dst[b] = src[b];
+            } else {
+                copy_span<VEC>(dst, src, len);
+            }
+        } else if (threadIdx.x == 0 && item < group_items && item % (rel.gp * cpp) == 0 && status) {
+            atomicAdd(status + kStatMiss, 1u);
+        }
+        if (nxt >= total || nxt / group_items != it.group) {
+            const uint32_t lo = it.group * group_items;
+            leave_group(rel, it.group, cta_items(lo, lo + group_items, blockIdx.x, gridDim.x),
+                        group_items, kLdStThreads);
+        }
+    }
+}
+
 // Item = chunk c of part s of block b, numbered (b * nparts + s) * cpp + c (GatherLaunch).
 // write: local parts.base[s] + desc.src -> pool desc.dst + (first_part + s) * part_bytes;
 // read:  pool desc.src + (first_part + s) * part_bytes -> local parts.base[s] + desc.dst.
+// LAYERED: a layered read (gather_read_layered above); no publish.
 // The minimum of 3 CTAs per SM lets the 32-byte flavour keep 64 registers; without it ptxas
 // held it to 56 and spilled.
-template <int VEC>
+template <int VEC, bool LAYERED = false>
 __global__ void __launch_bounds__(kLdStThreads + 32, 3)
     kv_gather_ldst_kernel(const CopyDesc* __restrict__ descs,
                           const __grid_constant__ GatherParts parts, uint32_t n, uint32_t nparts,
                           uint32_t part_bytes, uint32_t first_part, uint32_t chunk, uint32_t cpp,
-                          bool write, Publish pub, LayerCommit lc) {
+                          bool write, Publish pub, LayerCommit lc, GroupRelease rel) {
+    if constexpr (LAYERED) {
+        if (threadIdx.x >= kLdStThreads) return;
+        gather_read_layered<VEC>(descs, parts, n, nparts, part_bytes, first_part, chunk, cpp,
+                                 pub.status, rel);
+        return;
+    }
     const uint32_t cpb = nparts * cpp;  // items per block: what the commit counter counts
     const uint32_t total = n * cpb;
     if (threadIdx.x >= kLdStThreads) {
@@ -197,28 +249,53 @@ cudaError_t launch_kv_gather(const GatherLaunch& a, cudaStream_t stream) {
     if (a.n == 0 || a.part_bytes == 0) return cudaSuccess;
     if (a.nparts == 0 || a.nparts > kGatherMaxParts || !a.part_base) return cudaErrorInvalidValue;
     if (uint64_t(a.nparts) * a.part_bytes > 0xffffffffull) return cudaErrorInvalidValue;
+    const bool layered = a.group_flags != nullptr;
+    if (layered && !a.group_counters) return cudaErrorInvalidValue;
     constexpr int T = kLdStThreads + 32;
     static const LdStResident res =
         ldst_resident(kv_gather_ldst_kernel<16>, kv_gather_ldst_kernel<32>, T);
-    const LaunchPlan p = plan_gather(a, sm_count(), res);
+    static const LdStResident res_layered =
+        ldst_resident(kv_gather_ldst_kernel<16, true>, kv_gather_ldst_kernel<32, true>, T);
+    const LaunchPlan p = layered ? plan_gather_layered(a, sm_count(), res_layered)
+                                 : plan_gather(a, sm_count(), res);
     if (!p.valid) return cudaErrorInvalidValue;  // the caller splits the batch
     if (p.kernel == Kernel::kTma) return launch_kv_pipe_gather(a, stream);
     GatherParts parts;
     std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
+    const GroupRelease rel{a.group_flags, a.group_counters, a.group_seq, a.group_parts};
     const auto go = [&](auto* kernel) {
         kernel<<<p.ctas, T, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.part_bytes, a.first_part,
                                          p.chunk, p.cpb, a.write, publish_of(a, a.write),
-                                         layer_of(a));
+                                         layer_of(a), rel);
         return cudaGetLastError();
     };
     switch (p.kernel) {
         case Kernel::kLdSt1:
-            return go(kv_gather_ldst_kernel<1>);
+            return layered ? go(kv_gather_ldst_kernel<1, true>) : go(kv_gather_ldst_kernel<1>);
         case Kernel::kLdSt32:
-            return go(kv_gather_ldst_kernel<32>);
+            return layered ? go(kv_gather_ldst_kernel<32, true>) : go(kv_gather_ldst_kernel<32>);
         default:
-            return go(kv_gather_ldst_kernel<16>);
+            return layered ? go(kv_gather_ldst_kernel<16, true>) : go(kv_gather_ldst_kernel<16>);
     }
+}
+
+// Resolved once per process, as fabric/nvls.cpp resolves its driver entry points.
+cudaError_t stream_wait_geq(const uint32_t* addr, uint32_t value, cudaStream_t stream) {
+    using WaitFn = CUresult (*)(CUstream, CUdeviceptr, cuuint32_t, unsigned int);
+    static const WaitFn fn = [] {
+        void* p = nullptr;
+        cudaDriverEntryPointQueryResult q{};
+        if (cudaGetDriverEntryPoint("cuStreamWaitValue32", &p, cudaEnableDefault, &q) !=
+                cudaSuccess ||
+            q != cudaDriverEntryPointSuccess)
+            p = nullptr;
+        (void)cudaGetLastError();
+        return reinterpret_cast<WaitFn>(p);
+    }();
+    if (!fn) return cudaErrorNotSupported;
+    const CUresult r = fn(stream, reinterpret_cast<CUdeviceptr>(addr), value,
+                          CU_STREAM_WAIT_VALUE_GEQ);
+    return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorNotSupported;
 }
 
 }  // namespace istore::kernels

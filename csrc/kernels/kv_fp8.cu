@@ -220,16 +220,75 @@ __global__ void __launch_bounds__(kThreads + 32)
               BlockParts<true>{&parts, nparts, first_part, stride, lc});
 }
 
+// The layered read (GatherLaunch::group_flags): kv_gather_ldst's gather_read_layered
+// (kv_copy.cu) over fp8 pages.  Item order, miss counting and the group release are the same;
+// the rows of an item are dequantised as in kv_read_fp8_scatter_kernel.
+__device__ __forceinline__ void read_fp8_layered(const CopyDesc* __restrict__ descs,
+                                                 const BlockParts<false>& pages, uint32_t n,
+                                                 uint32_t elems, uint32_t chunk, uint32_t cpp,
+                                                 uint32_t* status, const GroupRelease& rel) {
+    const uint32_t group_items = n * rel.gp * cpp;
+    const uint32_t total = n * pages.nparts * cpp;
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t half = lane >> 4, hl = lane & 15;
+    constexpr uint32_t kStep = 2 * kRowPairs;
+    for (uint32_t item = blockIdx.x; item < total; item += gridDim.x) {
+        const LayeredItem it = layered_item(item, n, rel.gp, cpp);
+        const CopyDesc d = pages.at(descs, it.block * pages.nparts + it.part);
+        if (d.src != 0) {
+            const uint32_t e0 = it.chunk * chunk;
+            const uint32_t rows = min(chunk, elems - e0) / kRow;
+            const uint32_t row0 = e0 / kRow;
+            const uint8_t* q = reinterpret_cast<const uint8_t*>(d.src);
+            const float* scales = reinterpret_cast<const float*>(q + elems);
+            uint8_t* dst = reinterpret_cast<uint8_t*>(d.dst);
+            for (uint32_t r0 = warp * kStep; r0 < rows; r0 += kWarps * kStep) {
+                uint2 v[kRowPairs];
+                float sc[kRowPairs];
+#pragma unroll
+                for (int u = 0; u < kRowPairs; ++u) {
+                    const uint32_t r = r0 + 2 * u + half;
+                    if (r < rows) {
+                        v[u] = ld_u2(q + size_t(row0 + r) * kRow + hl * 8);
+                        sc[u] = __uint_as_float(ld_u1(scales + row0 + r));
+                    }
+                }
+#pragma unroll
+                for (int u = 0; u < kRowPairs; ++u) {
+                    const uint32_t r = r0 + 2 * u + half;
+                    if (r >= rows) continue;
+                    *reinterpret_cast<uint4*>(dst + (size_t(row0 + r) * kRow + hl * 8) * 2) =
+                        dequant8(v[u], sc[u]);
+                }
+            }
+        } else if (threadIdx.x == 0 && item < group_items && item % (rel.gp * cpp) == 0 && status) {
+            atomicAdd(status + kStatMiss, 1u);
+        }
+        const uint32_t nxt = item + gridDim.x;
+        if (nxt >= total || nxt / group_items != it.group) {
+            const uint32_t lo = it.group * group_items;
+            leave_group(rel, it.group, cta_items(lo, lo + group_items, blockIdx.x, gridDim.x),
+                        group_items, kThreads);
+        }
+    }
+}
+
 // The same loop as kv_read_fp8_kernel over the parts of gathered blocks.  A missing block
 // counts once, on its first part's first item; none of its parts is written.  (The two kernels
 // share the row maths, not the loop: inlining one loop body into both changed how the
-// compiler schedules kv_read_fp8_kernel.)
+// compiler schedules kv_read_fp8_kernel.)  LAYERED: a layered read (read_fp8_layered above).
+template <bool LAYERED = false>
 __global__ void __launch_bounds__(kThreads)
     kv_read_fp8_scatter_kernel(const CopyDesc* __restrict__ descs,
                                const __grid_constant__ GatherParts parts, uint32_t n,
                                uint32_t nparts, uint32_t first_part, uint32_t elems,
-                               uint32_t chunk, uint32_t cpp, uint64_t stride, uint32_t* status) {
+                               uint32_t chunk, uint32_t cpp, uint64_t stride, uint32_t* status,
+                               GroupRelease rel) {
     const BlockParts<false> pages{&parts, nparts, first_part, stride};
+    if constexpr (LAYERED) {
+        read_fp8_layered(descs, pages, n, elems, chunk, cpp, status, rel);
+        return;
+    }
     const uint32_t total = n * nparts * cpp;
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t half = lane >> 4, hl = lane & 15;
@@ -294,19 +353,29 @@ cudaError_t launch_kv_gather_fp8(const GatherLaunch& a, uint32_t elems, int vari
                                  cudaStream_t stream) {
     if (a.n == 0) return cudaSuccess;
     if (!a.part_base) return cudaErrorInvalidValue;
-    const LaunchPlan p = plan_gather_fp8(a, elems, variant, sm_count());
+    // a layered read takes the ld/st kernel whatever the variant (no layered pipeline)
+    const bool layered = a.group_flags != nullptr;
+    if (layered && (a.write || !a.group_counters || !a.group_parts || a.nparts % a.group_parts))
+        return cudaErrorInvalidValue;
+    const LaunchPlan p = plan_gather_fp8(a, elems, layered ? int(kFp8LdSt) : variant, sm_count());
     if (!p.valid) return cudaErrorInvalidValue;  // the caller splits the batch
     if (p.kernel != Kernel::kLdStFp8) return launch_kv_fp8_pipe_gather(a, elems, stream);
     GatherParts parts;
     std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
     const uint64_t stride = fp8_gather_bytes(1, elems);
+    const GroupRelease rel{a.group_flags, a.group_counters, a.group_seq, a.group_parts};
     if (a.write)
         kv_write_fp8_gather_kernel<<<p.ctas, kThreads + 32, 0, stream>>>(
             a.descs, parts, a.n, a.nparts, elems, p.chunk, p.cpb, a.first_part, stride,
             publish_of(a, true), layer_of(a));
+    else if (layered)
+        kv_read_fp8_scatter_kernel<true><<<p.ctas, kThreads, 0, stream>>>(
+            a.descs, parts, a.n, a.nparts, a.first_part, elems, p.chunk, p.cpb, stride, a.status,
+            rel);
     else
         kv_read_fp8_scatter_kernel<<<p.ctas, kThreads, 0, stream>>>(
-            a.descs, parts, a.n, a.nparts, a.first_part, elems, p.chunk, p.cpb, stride, a.status);
+            a.descs, parts, a.n, a.nparts, a.first_part, elems, p.chunk, p.cpb, stride, a.status,
+            rel);
     return cudaGetLastError();
 }
 

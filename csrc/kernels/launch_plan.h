@@ -3,7 +3,7 @@
 // kv_fp8.cu, kv_fp8_pipe.cu) pass in the SM count and the CTAs per SM the ld/st kernels keep
 // resident (occupancy API), so the choice is unit-tested on the CPU
 // (_infinistore.testing.plan_copy / plan_gather / plan_read_fused / plan_fp8 /
-// plan_gather_fp8).
+// plan_gather_fp8 / plan_gather_layered).
 #pragma once
 
 #include <algorithm>
@@ -203,6 +203,50 @@ inline LaunchPlan plan_gather(const GatherLaunch& a, int sms, LdStResident res) 
     p.kernel = !aligned16 ? Kernel::kLdSt1 : aligned32 ? Kernel::kLdSt32 : Kernel::kLdSt16;
     const uint64_t parts = uint64_t(a.n) * a.nparts;
     ldst_items(p, parts, a.part_bytes, kLdStChunk, 1u << 20, sms);  // whole parts as items
+    if (parts * p.cpb > kMaxItems) return invalid_plan();
+    p.ctas = ldst_grid(p, a.max_ctas, res, sms, parts * p.cpb);
+    return p;
+}
+
+// ---------------------------------------------------------------- layered reads
+// A layered read (GatherLaunch::group_flags) numbers its work items group-major, so that the
+// persistent grid's stride walks the groups roughly in order:
+//   item = ((g * n + block) * gp + p) * cpp + chunk,   part = g * gp + p,
+// with gp parts per group and G = nparts / gp groups.  Group g's items are the contiguous
+// range [g * n * gp * cpp, (g + 1) * n * gp * cpp).  The kernels (kv_copy.cu, kv_fp8.cu) and
+// the CPU tests (_infinistore.testing.layered_item) share these two functions.
+struct LayeredItem {
+    uint32_t group, block, part, chunk;
+};
+ISTORE_KHD inline LayeredItem layered_item(uint32_t item, uint32_t n, uint32_t gp, uint32_t cpp) {
+    const uint32_t chunk = item % cpp;
+    const uint32_t q = item / cpp;
+    const uint32_t r = q / gp;
+    const uint32_t g = r / n;
+    return LayeredItem{g, r % n, g * gp + q % gp, chunk};
+}
+
+// How many of the items first, first + stride, ... (a CTA's stream) lie in [lo, hi).
+ISTORE_KHD inline uint32_t cta_items_below(uint32_t end, uint32_t first, uint32_t stride) {
+    return end > first ? (end - first + stride - 1) / stride : 0u;
+}
+ISTORE_KHD inline uint32_t cta_items(uint32_t lo, uint32_t hi, uint32_t first, uint32_t stride) {
+    return cta_items_below(hi, first, stride) - cta_items_below(lo, first, stride);
+}
+
+// The layered read runs the ld/st kernels whatever the part size (the TMA pipelines have no
+// layered flavour): 16- or 32-byte vectors, the byte kernel on an unaligned batch.  Whole
+// parts as items as in plan_gather; group_parts must divide nparts.
+inline LaunchPlan plan_gather_layered(const GatherLaunch& a, int sms, LdStResident res) {
+    if (a.nparts == 0 || a.nparts > kGatherMaxParts || a.group_parts == 0 ||
+        a.nparts % a.group_parts != 0 || a.write)
+        return invalid_plan();
+    const bool aligned16 = aligned_to(a.part_bytes, a.align_or, 16);
+    const bool aligned32 = aligned_to(a.part_bytes, a.align_or, 32);
+    LaunchPlan p;
+    p.kernel = !aligned16 ? Kernel::kLdSt1 : aligned32 ? Kernel::kLdSt32 : Kernel::kLdSt16;
+    const uint64_t parts = uint64_t(a.n) * a.nparts;
+    ldst_items(p, parts, a.part_bytes, kLdStChunk, 1u << 20, sms);
     if (parts * p.cpb > kMaxItems) return invalid_plan();
     p.ctas = ldst_grid(p, a.max_ctas, res, sms, parts * p.cpb);
     return p;

@@ -207,6 +207,46 @@ __device__ __forceinline__ void control_warp_layered(const Publish& pub, const L
     }
 }
 
+// Layered reads (GatherLaunch::group_flags): the launch walks the parts group by group
+// (launch_plan.h: layered_item) and releases group g - gp parts of every block, typically one
+// layer's K and V - to a consumer that waits for flag[g] >= seq (cuStreamWaitValue32 on its
+// stream, kernels.h: stream_wait_geq).
+//   Every copy thread calls leave_group when its CTA's item stream leaves group g; items
+// come in increasing order, so that happens once per group the CTA visits.  The copy
+// threads meet on a named barrier; thread 0 then fences and adds the CTA's item count for g
+// (`count`, computed arithmetically) to counter[g].  The add that reaches g's total
+// (n * gp * cpp items) resets the counter and publishes flag[g] = seq.
+// Ordering: each copy thread's stores of group g precede its bar.sync, which orders them at
+// CTA scope before thread 0's fence.acq_rel.gpu; that fence is cumulative, so they are
+// performed at gpu scope before thread 0's atom.add.acq_rel.gpu.  The add that reaches the
+// total acquires every earlier add on the counter (each released its CTA's fenced stores),
+// so every store of group g - from every CTA - happens before it.  fence.acq_rel.sys then
+// a relaxed st.sys of the flag is a release at system scope (the pattern of commit_entry): a
+// waiter that observes flag >= seq observes every part of the group.  A missing block's
+// items count as arrivals without a store, so every group is always released.
+// Copy threads cannot run more than one barrier phase ahead of thread 0: it takes part in
+// every bar.sync, and reaches the next one only after its fence and add.  At most one fence
+// per CTA per group; a CTA that moves no item of g makes no add for it.
+struct GroupRelease {
+    uint32_t* flags = nullptr;     // flag[g], g < nparts / gp; nullptr: not a layered read
+    uint32_t* counters = nullptr;  // zeroed u32 per group, left zeroed
+    uint32_t seq = 0;              // the reader's sequence number
+    uint32_t gp = 0;               // parts per group
+};
+
+constexpr int kGroupBarrier = 2;  // named barrier of a layered read's copy threads
+
+__device__ __forceinline__ void leave_group(const GroupRelease& r, uint32_t g, uint32_t count,
+                                            uint32_t group_items, uint32_t copy_threads) {
+    asm volatile("bar.sync %0, %1;" ::"n"(kGroupBarrier), "r"(copy_threads) : "memory");
+    if (threadIdx.x != 0 || count == 0) return;
+    fence_gpu();
+    if (atom_add_acq_rel_gpu(r.counters + g, count) + count != group_items) return;
+    r.counters[g] = 0;  // the last arrival: nobody adds to it again in this launch
+    fence_sys();
+    asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(r.flags + g), "r"(r.seq) : "memory");
+}
+
 // The control warp of a gathered write: layered when the launch carries a writer's state.
 __device__ __forceinline__ void gather_control_warp(const Publish& pub, const LayerCommit& lc,
                                            uint32_t lane, uint32_t first, uint32_t count,

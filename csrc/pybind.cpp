@@ -633,6 +633,44 @@ PYBIND11_MODULE(_infinistore, m) {
             "scattered fp8 read: fp8 page first_part + s of each block, dequantised -> "
             "part_base[s] + offset")
         .def(
+            "r_rdma_scatter_layered",
+            [](Connection& c, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
+               int elems, uint32_t first_part, uint32_t group_parts, const py::object& blocks,
+               int device, uint64_t stream, uint64_t scale) {
+                std::vector<KeyOffset> kb;
+                blocks_list_from_py(blocks, scale, kb);
+                Connection::GatherSpec g;
+                g.part_base = part_base.data();
+                g.nparts = uint32_t(part_base.size());
+                g.part_bytes = part_bytes;
+                g.first_part = first_part;
+                auto r = std::make_shared<Connection::ScatterReader>();
+                py::gil_scoped_release rel;
+                c.read_scatter_layered(g, elems, group_parts, kb, device, stream, *r);
+                return r;
+            },
+            py::arg("part_base"), py::arg("part_bytes"), py::arg("elems"), py::arg("first_part"),
+            py::arg("group_parts"), py::arg("blocks"), py::arg("device") = -1,
+            py::arg("stream") = 0, py::arg("scale") = 1,
+            "layered scattered read (r_rdma_scatter, or r_rdma_scatter_fp8 with elems > 0) "
+            "whose parts are released in groups of group_parts; check .failed")
+        .def(
+            "wait_layered",
+            [](Connection& c, const Connection::ScatterReader& r, uint32_t group, uint64_t stream) {
+                std::string err;
+                int rc;
+                {
+                    py::gil_scoped_release rel;
+                    rc = c.wait_layered(r, group, stream, &err);
+                }
+                if (rc == -1) throw py::value_error(err);
+                if (rc != 0) throw std::runtime_error(err);
+            },
+            py::arg("reader"), py::arg("group"), py::arg("stream"),
+            "later work on `stream` waits on the GPU until `group` of the reader has landed; "
+            "ValueError when refused (failed reader, group outside the read, connection closed "
+            "since the read)")
+        .def(
             "gather_writer",
             [](Connection& c, const py::object& remote_blocks, const py::object& offsets,
                uint32_t nparts) {
@@ -723,6 +761,15 @@ PYBIND11_MODULE(_infinistore, m) {
                                [](const Connection::GatherWriter& w) { return w.blocks.size(); })
         .def_property_readonly("written", [](const Connection::GatherWriter& w) {
             return std::vector<bool>(w.written.begin(), w.written.end());
+        });
+    py::class_<Connection::ScatterReader, std::shared_ptr<Connection::ScatterReader>>(
+        m, "ScatterReader")
+        .def_readonly("groups", &Connection::ScatterReader::groups)
+        .def_readonly("group_parts", &Connection::ScatterReader::group_parts)
+        .def_readonly("seq", &Connection::ScatterReader::seq)
+        .def_readonly("failed", &Connection::ScatterReader::failed)
+        .def_property_readonly("flags", [](const Connection::ScatterReader& r) {
+            return reinterpret_cast<uint64_t>(r.flags);
         });
 
     py::class_<Server, std::shared_ptr<Server>>(m, "Server")
@@ -948,11 +995,16 @@ PYBIND11_MODULE(_infinistore, m) {
            uint32_t first_part, bool write, int max_ctas, uint64_t stream, uint64_t recs,
            uint64_t table, uint64_t table_mask, uint64_t done, uint64_t status, uint64_t align_or,
            uint32_t stage_bytes, uint32_t ring_bytes, uint64_t layer_state, uint32_t layer_parts,
-           bool layer_claim) {
+           bool layer_claim, uint64_t group_flags, uint64_t group_counters, uint32_t group_seq,
+           uint32_t group_parts) {
             if (part_base.empty() || part_base.size() > kernels::kGatherMaxParts)
                 throw std::runtime_error("kv_gather: 1 to GATHER_MAX_PARTS parts");
             if (layer_state && first_part + part_base.size() > layer_parts)
                 throw std::runtime_error("kv_gather: first_part + parts > layer_parts");
+            if (group_flags && (write || !group_counters || !group_parts ||
+                                part_base.size() % group_parts))
+                throw std::runtime_error(
+                    "kv_gather: a layered read needs counters and group_parts dividing the parts");
             kernels::GatherLaunch G;
             G.descs = as_ptr<const kernels::CopyDesc>(descs);
             G.n = n;
@@ -973,6 +1025,10 @@ PYBIND11_MODULE(_infinistore, m) {
             G.layer_state = as_ptr<uint32_t>(layer_state);
             G.layer_parts = layer_parts;
             G.layer_claim = layer_claim;
+            G.group_flags = as_ptr<uint32_t>(group_flags);
+            G.group_counters = as_ptr<uint32_t>(group_counters);
+            G.group_seq = group_seq;
+            G.group_parts = group_parts;
             const cudaError_t e = kernels::launch_kv_gather(G, as_ptr<CUstream_st>(stream));
             if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
         },
@@ -982,21 +1038,32 @@ PYBIND11_MODULE(_infinistore, m) {
         py::arg("table_mask") = 0, py::arg("done") = 0, py::arg("status") = 0,
         py::arg("align_or") = 0, py::arg("stage_bytes") = 0, py::arg("ring_bytes") = 0,
         py::arg("layer_state") = 0, py::arg("layer_parts") = 0, py::arg("layer_claim") = false,
+        py::arg("group_flags") = 0, py::arg("group_counters") = 0, py::arg("group_seq") = 0,
+        py::arg("group_parts") = 0,
         "gathered blocks: descs[i] = write {local byte offset, block address} / read {block "
         "address or 0, local byte offset}; part s of block i at part_base[s] + local offset is "
         "stored part first_part + s.  layer_state (3 zeroed u32 per block, kept across the "
         "launches of one layered write): the block is published by the launch that lands the "
-        "last of its layer_parts parts; layer_claim: this launch claims the index ways");
+        "last of its layer_parts parts; layer_claim: this launch claims the index ways.  "
+        "group_flags (reads): a layered read that stores group_seq to group_flags[g] once "
+        "group g (group_parts parts of every block) has landed; group_counters: one zeroed "
+        "u32 per group");
     k.def(
         "kv_gather_fp8",
         [](uint64_t descs, uint32_t n, const std::vector<uint64_t>& part_base, uint32_t elems,
            uint32_t first_part, bool write, int variant, int max_ctas, uint64_t stream,
            uint64_t recs, uint64_t table, uint64_t table_mask, uint64_t done, uint64_t status,
-           uint64_t align_or, uint64_t layer_state, uint32_t layer_parts, bool layer_claim) {
+           uint64_t align_or, uint64_t layer_state, uint32_t layer_parts, bool layer_claim,
+           uint64_t group_flags, uint64_t group_counters, uint32_t group_seq,
+           uint32_t group_parts) {
             if (part_base.empty() || part_base.size() > kernels::kGatherMaxParts)
                 throw std::runtime_error("kv_gather_fp8: 1 to GATHER_MAX_PARTS parts");
             if (layer_state && first_part + part_base.size() > layer_parts)
                 throw std::runtime_error("kv_gather_fp8: first_part + parts > layer_parts");
+            if (group_flags && (write || !group_counters || !group_parts ||
+                                part_base.size() % group_parts))
+                throw std::runtime_error("kv_gather_fp8: a layered read needs counters and "
+                                         "group_parts dividing the parts");
             kernels::GatherLaunch G;
             G.descs = as_ptr<const kernels::CopyDesc>(descs);
             G.n = n;
@@ -1014,6 +1081,10 @@ PYBIND11_MODULE(_infinistore, m) {
             G.layer_state = as_ptr<uint32_t>(layer_state);
             G.layer_parts = layer_parts;
             G.layer_claim = layer_claim;
+            G.group_flags = as_ptr<uint32_t>(group_flags);
+            G.group_counters = as_ptr<uint32_t>(group_counters);
+            G.group_seq = group_seq;
+            G.group_parts = group_parts;
             const cudaError_t e =
                 kernels::launch_kv_gather_fp8(G, elems, variant, as_ptr<CUstream_st>(stream));
             if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
@@ -1023,10 +1094,20 @@ PYBIND11_MODULE(_infinistore, m) {
         py::arg("max_ctas") = 0, py::arg("stream") = 0, py::arg("recs") = 0, py::arg("table") = 0,
         py::arg("table_mask") = 0, py::arg("done") = 0, py::arg("status") = 0,
         py::arg("align_or") = 0, py::arg("layer_state") = 0, py::arg("layer_parts") = 0,
-        py::arg("layer_claim") = false,
+        py::arg("layer_claim") = false, py::arg("group_flags") = 0, py::arg("group_counters") = 0,
+        py::arg("group_seq") = 0, py::arg("group_parts") = 0,
         "gathered fp8 blocks: descs as for kv_gather; part s (elems bf16 elements at "
-        "part_base[s] + local offset) <-> fp8 page first_part + s of the block; layer_* as "
-        "for kv_gather");
+        "part_base[s] + local offset) <-> fp8 page first_part + s of the block; layer_* and "
+        "group_* as for kv_gather (a layered read always runs the ld/st kernel)");
+    k.def(
+        "stream_wait_value",
+        [](uint64_t addr, uint32_t value, uint64_t stream) {
+            const cudaError_t e = kernels::stream_wait_geq(as_ptr<const uint32_t>(addr), value,
+                                                           as_ptr<CUstream_st>(stream));
+            if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
+        },
+        py::arg("addr"), py::arg("value"), py::arg("stream"),
+        "later work on `stream` waits on the GPU until the u32 at `addr` is >= value");
     k.def(
         "kv_pipe_mcast",
         [](uint64_t descs, uint32_t n, uint32_t bytes, const std::vector<int64_t>& delta,
@@ -1411,6 +1492,29 @@ PYBIND11_MODULE(_infinistore, m) {
                  return py::int_(ev);
              })
         .def("in_flight", &Staging::in_flight);
+    // flag slots of layered reads (ctrl/staging.h), events as integers
+    using Readers = ReaderSlots<int64_t, kReaderSlots>;
+    t.attr("READER_SLOTS") = kReaderSlots;
+    py::class_<Readers>(t, "ReaderSlots")
+        .def(py::init<>())
+        .def("take",
+             [](Readers& r) {
+                 py::list waited;
+                 const uint64_t seq = r.take([&](int64_t ev) { waited.append(ev); });
+                 return py::make_tuple(seq, Readers::slot_of(seq), waited);
+             })
+        .def("launched", &Readers::launched)
+        .def("retire_all", &Readers::retire_all);
+    // layered reads' work-item numbering (kernels/launch_plan.h)
+    t.def("layered_item", [](uint32_t item, uint32_t n, uint32_t gp, uint32_t cpp) {
+        if (!n || !gp || !cpp) throw py::value_error("needs n, gp, cpp > 0");
+        const kernels::LayeredItem it = kernels::layered_item(item, n, gp, cpp);
+        return py::make_tuple(it.group, it.block, it.part, it.chunk);
+    });
+    t.def("cta_items", [](uint32_t lo, uint32_t hi, uint32_t first, uint32_t stride) {
+        if (!stride || hi < lo) throw py::value_error("needs stride > 0 and lo <= hi");
+        return kernels::cta_items(lo, hi, first, stride);
+    });
     // how a read call is split into launches (ctrl/staging.h), with the client's limits
     t.attr("RING_BYTES") = kRingBytes;
     t.attr("MAX_BATCH") = kMaxBatch;
@@ -1435,10 +1539,10 @@ PYBIND11_MODULE(_infinistore, m) {
     t.def("plan_device_read",
           [](size_t n, uint32_t block_bytes, uint32_t fp8_elems, bool gather, bool fp8_fused_ok,
              bool scatter_fused_ok, int copy_variant, bool all_local, bool all_remote, int max_ctas,
-             int sm_count) {
+             int sm_count, bool layered) {
               const DeviceReadPlan p = plan_device_read(DeviceReadIn{
                   n, block_bytes, fp8_elems, gather, fp8_fused_ok, scatter_fused_ok, copy_variant,
-                  all_local, all_remote, max_ctas, sm_count});
+                  all_local, all_remote, max_ctas, sm_count, layered});
               static const char* const kPaths[] = {"fused_copy",    "fused_fp8",
                                                    "fused_scatter", "lookup_copy",
                                                    "lookup_fp8",    "lookup_gather",
@@ -1452,7 +1556,7 @@ PYBIND11_MODULE(_infinistore, m) {
           py::arg("n"), py::arg("block_bytes"), py::arg("fp8_elems") = 0, py::arg("gather") = false,
           py::arg("fp8_fused_ok") = false, py::arg("scatter_fused_ok") = false,
           py::arg("copy_variant") = 0, py::arg("all_local") = false, py::arg("all_remote") = false,
-          py::arg("max_ctas") = 0, py::arg("sm_count") = 132);
+          py::arg("max_ctas") = 0, py::arg("sm_count") = 132, py::arg("layered") = false);
     // which kernel a page-mover launcher runs, its work split and grid (kernels/launch_plan.h);
     // the resident CTAs per SM of the ld/st kernels are the occupancy API's answer on a GPU
     const auto plan_dict = [](const kernels::LaunchPlan& p) {
@@ -1508,6 +1612,22 @@ PYBIND11_MODULE(_infinistore, m) {
           py::arg("n"), py::arg("nparts"), py::arg("part_bytes"), py::arg("align_or") = 0,
           py::arg("max_ctas") = 0, py::arg("stage_bytes") = 0, py::arg("ring_bytes") = 0,
           py::arg("sm_count") = 132, py::arg("resident16") = 1, py::arg("resident32") = 1);
+    t.def("plan_gather_layered",
+          [plan_dict](uint32_t n, uint32_t nparts, uint32_t part_bytes, uint32_t group_parts,
+                      uint64_t align_or, int max_ctas, int sm_count, int resident16,
+                      int resident32) {
+              kernels::GatherLaunch a;
+              a.n = n;
+              a.nparts = nparts;
+              a.part_bytes = part_bytes;
+              a.group_parts = group_parts;
+              a.align_or = align_or;
+              a.max_ctas = max_ctas;
+              return plan_dict(kernels::plan_gather_layered(a, sm_count, {resident16, resident32}));
+          },
+          py::arg("n"), py::arg("nparts"), py::arg("part_bytes"), py::arg("group_parts") = 2,
+          py::arg("align_or") = 0, py::arg("max_ctas") = 0, py::arg("sm_count") = 132,
+          py::arg("resident16") = 1, py::arg("resident32") = 1);
     t.def("plan_read_fused",
           [plan_dict](uint32_t n, uint32_t bytes, uint64_t align_or, int variant, int max_ctas,
                       uint32_t stage_bytes, uint32_t ring_bytes, int sm_count, int resident16,

@@ -771,6 +771,49 @@ class InfinityConnection:
         if ret < 0:
             raise Exception(f"Failed to read to infinistore, ret = {ret}: {self.conn.last_error()}")
 
+    # ------------------------------------------------------------------ layered scattered reads
+    def read_cache_scatter_layered(self, parts, blocks, part_size: int, group_parts: int = 2,
+                                   first_part: int = 0, fp8: bool = False,
+                                   stream="current") -> "ScatterRead":
+        """``read_cache_scatter`` (``read_cache_scatter_fp8`` with ``fp8``) in one call whose
+        parts are released to consumers group by group: group ``g`` is parts
+        ``g * group_parts .. g * group_parts + group_parts - 1`` of every block (with the
+        default 2 and vLLM's layout, one layer's K and V).  Returns a :class:`ScatterRead`;
+        ``wait(g, stream)`` makes later work on ``stream`` wait, on the GPU, until group g has
+        landed, with no host synchronisation.  Each key is resolved once and one page-mover
+        launch (per 65,536 blocks) walks the groups in order.  The read is enqueued at once,
+        after the caller's stream.  ``parts``, ``blocks``, ``part_size`` and ``first_part`` are
+        as for ``read_cache_scatter[_fp8]``; the parts must be CUDA tensors and the pool in GPU
+        memory.  ``group_parts`` must divide ``len(parts)``.  A group is released before the
+        read's post-copy index check: when ``sync()`` reports a miss, treat the whole read as
+        failed, as for any read.  A missing key on a connection without ``device_lookup``
+        raises here; the exception's ``read`` attribute is the failed reader."""
+        keys, offs = self._scatter_blocks(blocks, first_part)
+        bases, dev, es = self._gather_parts(parts, int(offs.max()) if len(offs) else 0, part_size,
+                                            fp8=fp8, offsets=offs if fp8 else None)
+        if dev < 0:
+            raise ValueError("layered reads take CUDA tensors")
+        if not self.conn.server_has_hbm():
+            raise ValueError("layered reads need a pool in GPU memory")
+        group_parts = int(group_parts)
+        if group_parts < 1 or len(bases) % group_parts:
+            raise ValueError(f"group_parts {group_parts} does not divide the {len(bases)} parts")
+        end = int(first_part) + len(bases)
+        limit = (self.fp8_gather_block_bytes(end, int(part_size)) if fp8
+                 else end * int(part_size) * es)
+        if limit > _GATHER_MAX_BLOCK_BYTES:
+            raise ValueError("first_part + parts run past the block size limit")
+        first = parts[0][0]
+        native = self.conn.r_rdma_scatter_layered(
+            bases, int(part_size) * es, int(part_size) if fp8 else 0, int(first_part), group_parts,
+            (keys, offs), dev, _stream_of(first, stream), es)
+        read = ScatterRead(self, native, first.device)
+        if native.failed:
+            err = Exception(f"Failed to read to infinistore: {self.conn.last_error()}")
+            err.read = read
+            raise err
+        return read
+
     # ------------------------------------------------------------------ layered gathered writes
     def gather_writer(self, remote_blocks, offsets, nparts: int, part_size: int,
                       fp8: bool = False) -> "GatherWriter":
@@ -978,6 +1021,46 @@ class InfinityConnection:
 
     def segments(self):
         return self.conn.segments()
+
+
+class ScatterRead:
+    """A layered scattered read (``InfinityConnection.read_cache_scatter_layered``)."""
+
+    def __init__(self, conn: "InfinityConnection", native, device: torch.device):
+        self._conn = conn
+        self._r = native
+        self._device = device
+
+    @property
+    def groups(self) -> int:
+        """Number of groups: the parts read divided by ``group_parts``."""
+        return self._r.groups
+
+    @property
+    def failed(self) -> bool:
+        """The read was refused or failed to launch: every ``wait`` raises."""
+        return self._r.failed
+
+    def wait(self, group: int, stream="current") -> None:
+        """Later work on ``stream`` (default: the current stream of the parts' device) sees
+        parts ``group * group_parts .. group * group_parts + group_parts - 1`` of every block.
+        The wait is enqueued on the GPU (``cuStreamWaitValue32``); the host does not block.
+        Raises ``ValueError``, with nothing enqueued, for a failed read, a group outside the
+        read, or a connection closed since the read (its flags were released with it)."""
+        if self._r.failed:
+            raise ValueError("the read failed, so its groups are never released")
+        group = int(group)
+        if not 0 <= group < self._r.groups:
+            raise ValueError(f"group {group} is outside the read's {self._r.groups} groups")
+        if stream is None:
+            raise ValueError("wait needs a stream")
+        if stream == "current":
+            handle = torch.cuda.current_stream(self._device).cuda_stream
+        elif isinstance(stream, torch.cuda.Stream):
+            handle = stream.cuda_stream
+        else:
+            handle = int(stream)
+        self._conn.conn.wait_layered(self._r, group, handle if handle != 0 else _CUDA_STREAM_LEGACY)
 
 
 class GatherWriter:

@@ -157,6 +157,28 @@ class PagedKVCache:
              first_part=2 * layers.start, stream=stream)
         return len(keys)
 
+    def read_pages_layered(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
+                           layers: Optional[range] = None, fp8: bool = False,
+                           stream="current") -> "PageRead":
+        """``read_pages`` in one call that releases each layer as it lands: the returned
+        reader's ``wait_layer(l, stream)`` makes later work on ``stream`` wait, on the GPU,
+        for layer l's K and V, so attention on layer 0 can start before the last layer has
+        arrived, with no host synchronisation.  ``layers`` (a step-1 range, default all) and
+        ``fp8`` as for ``read_pages``."""
+        if fp8:
+            self._check_fp8()
+        self._ensure_registered(conn)
+        layers = range(self.layout.layers) if layers is None else layers
+        if layers.step != 1 or not len(layers) or layers.start < 0 or layers.stop > self.layout.layers:
+            raise ValueError(f"layers must be a non-empty step-1 range within "
+                             f"0..{self.layout.layers}")
+        keys = self.page_keys(page_hashes)
+        offs = np.asarray(pages, dtype=np.int64) * self.layout.page_elems
+        read = conn.read_cache_scatter_layered(self._parts(layers), (keys, offs),
+                                               self.layout.page_elems, group_parts=2,
+                                               first_part=2 * layers.start, fp8=fp8, stream=stream)
+        return PageRead(read, layers)
+
     def cached_prefix_pages(self, conn, page_hashes: Sequence[str],
                             layer: Optional[int] = None, all_layer_pages: bool = False) -> int:
         """How many leading pages of this prefix the store already holds (last layer's V
@@ -205,6 +227,21 @@ class PageWriter:
         if layers.step != 1 or not len(layers) or layers.start < 0 or layers.stop > n:
             raise ValueError(f"layers must be a non-empty step-1 range within 0..{n}")
         self.writer.write(self.cache._parts(layers), 2 * layers.start, stream=stream)
+
+
+class PageRead:
+    """A layer-by-layer read of all-layer pages (``PagedKVCache.read_pages_layered``)."""
+
+    def __init__(self, read, layers: range):
+        self.read = read
+        self.layers = layers
+
+    def wait_layer(self, layer: int, stream="current") -> None:
+        """Later work on ``stream`` sees layer ``layer``'s K and V pages.  Raises
+        ``ValueError`` for a layer outside the read or a failed read."""
+        if int(layer) not in self.layers:
+            raise ValueError(f"layer {layer} is outside the read's layers {self.layers}")
+        self.read.wait(int(layer) - self.layers.start, stream=stream)
 
 
 def read_layer_multi(conn, caches: Sequence[PagedKVCache], layer: int, pages: Sequence[int],

@@ -76,11 +76,44 @@ def _publish_args(publish: Optional["PublishArgs"], layer: Optional[LayerState],
             (layer.state.data_ptr(), layer.nparts, bool(claim)) if layer else (0, 0, False))
 
 
+class GroupRelease:
+    """The arguments of a layered read (``GatherLaunch::group_flags``): the launch stores
+    ``seq`` to ``flags[g]`` once group g (``group_parts`` parts of every block) has landed.
+    ``counters`` (one zeroed int32 per group, left zeroed) is allocated when not given."""
+
+    def __init__(self, flags: torch.Tensor, seq: int, group_parts: int,
+                 counters: Optional[torch.Tensor] = None):
+        assert flags.is_cuda and flags.dtype == torch.int32 and flags.is_contiguous()
+        self.flags = flags
+        self.seq = int(seq)
+        self.group_parts = int(group_parts)
+        self.counters = (counters if counters is not None
+                         else torch.zeros(flags.numel(), dtype=torch.int32, device=flags.device))
+
+
+def _release_args(release: Optional[GroupRelease]):
+    if release is None:
+        return (0, 0, 0, 0)
+    return (release.flags.data_ptr(), release.counters.data_ptr(), release.seq,
+            release.group_parts)
+
+
+def stream_wait_value(flags: torch.Tensor, index: int, value: int, stream=None) -> None:
+    """Later work on ``stream`` (default: the current stream of ``flags``' device) waits on
+    the GPU until ``flags[index] >= value`` (``cuStreamWaitValue32``): how a consumer waits for
+    a layered read's group."""
+    assert flags.is_cuda and flags.dtype == torch.int32 and 0 <= index < flags.numel()
+    s = stream if stream is not None else torch.cuda.current_stream(flags.device)
+    h = s.cuda_stream if isinstance(s, torch.cuda.Stream) else int(s)
+    with torch.cuda.device(flags.device):
+        K.stream_wait_value(flags.data_ptr() + 4 * int(index), int(value), h if h != 0 else 1)
+
+
 def kv_gather(descs: torch.Tensor, part_base: Sequence[int], part_bytes: int, write: bool,
               first_part: int = 0, max_ctas: int = 0, status: Optional[torch.Tensor] = None,
               align_or: int = 0, stage_bytes: int = 0, ring_bytes: int = 0,
               publish: Optional["PublishArgs"] = None, layer: Optional[LayerState] = None,
-              claim: bool = False) -> None:
+              claim: bool = False, release: Optional[GroupRelease] = None) -> None:
     """Gathered blocks (csrc/kernels/kernels.h ``GatherLaunch``): block i is len(part_base)
     parts of ``part_bytes``, part s at ``part_base[s] + local offset``.  ``descs`` is (n, 2)
     int64: write {local byte offset, block address}, read {block address or 0 = miss, local
@@ -88,7 +121,8 @@ def kv_gather(descs: torch.Tensor, part_base: Sequence[int], part_bytes: int, wr
     local offsets (the part bases are added here): it picks the vector width.  A write with
     ``publish`` commits its blocks in the index; with ``layer`` too it is one launch of a
     layered write (``claim``: its first), which publishes a block once all of
-    ``layer.nparts`` parts have landed."""
+    ``layer.nparts`` parts have landed.  A read with ``release`` is a layered read: the ld/st
+    kernel walks the parts group by group and releases each group's flag."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
     bases = [int(b) for b in part_base]
     for b in bases:
@@ -98,7 +132,7 @@ def kv_gather(descs: torch.Tensor, part_base: Sequence[int], part_bytes: int, wr
         K.kv_gather(descs.data_ptr(), descs.shape[0], bases, part_bytes, first_part, write,
                     max_ctas, _stream(descs.device), *pub,
                     status.data_ptr() if status is not None else 0, align_or, stage_bytes,
-                    ring_bytes, *lay)
+                    ring_bytes, *lay, *_release_args(release))
 
 
 def kv_copy_multicast(descs: torch.Tensor, nbytes: int, dst_deltas: Sequence[int],
@@ -288,13 +322,14 @@ def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, wri
                   first_part: int = 0, max_ctas: int = 0, status: Optional[torch.Tensor] = None,
                   align_or: int = 0, publish: Optional[PublishArgs] = None,
                   variant: str = "auto", layer: Optional[LayerState] = None,
-                  claim: bool = False) -> None:
+                  claim: bool = False, release: Optional[GroupRelease] = None) -> None:
     """Gathered fp8 blocks (``kv_gather`` with quantisation): part s of block i is a bf16 page
     of ``elems`` elements at ``part_base[s] + local offset`` and fp8 page first_part + s of
     the block, at byte ``fp8_gather_bytes(first_part + s, elems)``.  ``descs``, ``layer`` and
     ``claim`` as for ``kv_gather``.  ``variant``: "ldst" = the ld/st kernels (kv_fp8.cu),
     "auto" / "tma" = the TMA pipeline (kv_fp8_pipe.cu).  ``align_or`` must include the local
-    offsets (the part bases are added here): unaligned batches are refused."""
+    offsets (the part bases are added here): unaligned batches are refused.  ``release`` as for
+    ``kv_gather`` (a layered read always runs the ld/st kernel)."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
     bases = [int(b) for b in part_base]
     for b in bases:
@@ -304,7 +339,8 @@ def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, wri
         K.kv_gather_fp8(descs.data_ptr(), descs.shape[0], bases, elems, first_part, write,
                         FP8_VARIANTS["ldst"] if variant == "ldst" else FP8_VARIANTS["auto"],
                         max_ctas, _stream(descs.device), *pub,
-                        status.data_ptr() if status is not None else 0, align_or, *lay)
+                        status.data_ptr() if status is not None else 0, align_or, *lay,
+                        *_release_args(release))
 
 
 def fp8_reference(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
