@@ -198,6 +198,8 @@ class Connection {
         uint32_t part_bytes = 0;  // pool bytes of a part (fp8: fp8_gather_bytes(1, elems))
         uint32_t first_part = 0;  // stored part first_part + s is part s (one-shot writes: 0)
         ScatterReader* reader = nullptr;  // reads: a layered read (read_scatter_layered)
+        // reads: row-sliced parts (kernels::GatherLaunch::rows, bytes); rows == 0: whole parts
+        uint32_t rows = 0, row_bytes = 0, src_pitch = 0, src_col = 0, dst_pitch = 0;
     };
     // Layered gathered write: a fixed set of allocated gathered blocks whose parts are stored
     // over several calls (write_layered), each a contiguous range of parts of every block -
@@ -238,7 +240,9 @@ class Connection {
     // offsets in bytes; blocks allocated with nparts * part_bytes bytes (trusted)
     int w_rdma_gather(const GatherSpec& g, const uint64_t* offsets, size_t noffsets,
                       const RemoteBlock* blocks, size_t nblocks, int device, uint64_t stream);
-    // a stored block must hold (first_part + nparts) * part_bytes bytes, else it is a miss
+    // a stored block must hold (first_part + nparts) * part_bytes bytes, else it is a miss.
+    // Row-sliced (g.rows): rows >= 1, src_col + row_bytes <= src_pitch and part_bytes ==
+    // rows * src_pitch, else refused before anything is enqueued.
     int r_rdma_scatter(const GatherSpec& g, const std::vector<KeyOffset>& blocks, int device,
                        uint64_t stream);
     // Gathered fp8 blocks: every part is a bf16 page of `elems` elements (a multiple of 512) in

@@ -287,7 +287,17 @@ kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n,
     G.max_ctas = max_ctas;
     G.stage_bytes = pipe_stage_;
     G.ring_bytes = pipe_ring_;
+    G.rows = g.rows;
+    G.row_bytes = g.row_bytes;
+    G.src_pitch = g.src_pitch;
+    G.src_col = g.src_col;
+    G.dst_pitch = g.dst_pitch;
     return G;
+}
+
+// Bytes one block of a gathered call moves: its parts, or their rows when row-sliced.
+static uint64_t gather_moved_bytes(const Connection::GatherSpec& g) {
+    return uint64_t(g.nparts) * (g.rows ? uint64_t(g.rows) * g.row_bytes : g.part_bytes);
 }
 
 // Layered writers' state (GatherWriter::state), allocated stream-ordered from a memory pool of
@@ -370,8 +380,7 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
     const bool commit_now = !layered || layered->parts_written + gather->nparts == layered->nparts;
     // bytes moved per block: a gathered call moves its parts, which are the whole block
     // unless the call is layered
-    const uint64_t moved =
-        gather ? uint64_t(gather->nparts) * gather->part_bytes : uint64_t(uint32_t(block_size));
+    const uint64_t moved = gather ? gather_moved_bytes(*gather) : uint64_t(uint32_t(block_size));
     int kd = device;
     if (device < 0 && fp8_elems) {
         fail("the fp8 KV path needs a CUDA tensor");
@@ -402,12 +411,18 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
                 auto m = mapping(addr_seg(blocks[i].remote_addr), -1);
                 if (!m || !m->host_ptr) return -1;
                 uint8_t* pool = m->host_ptr + addr_off(blocks[i].remote_addr);
-                if (gather) {  // one memcpy per part
+                if (gather) {  // one memcpy per part, or per row of a row-sliced read
                     const size_t pb = gather->part_bytes;
+                    const Connection::GatherSpec& g = *gather;
                     for (uint32_t s = 0; s < gather->nparts; ++s) {
                         uint8_t* local =
                             reinterpret_cast<uint8_t*>(gather->part_base[s] + local_off[i] * scale);
-                        if (write)
+                        if (g.rows) {
+                            const uint8_t* src = pool + (g.first_part + s) * pb + g.src_col;
+                            for (uint32_t r = 0; r < g.rows; ++r)
+                                std::memcpy(local + size_t(r) * g.dst_pitch,
+                                            src + size_t(r) * g.src_pitch, g.row_bytes);
+                        } else if (write)
                             std::memcpy(pool + (gather->first_part + s) * pb, local, pb);
                         else
                             std::memcpy(local, pool + (gather->first_part + s) * pb, pb);
@@ -863,6 +878,12 @@ int Connection::r_rdma_scatter(const GatherSpec& g, const std::vector<KeyOffset>
         fail("r_rdma_scatter: bad parts list");
         return -1;
     }
+    if (g.rows && (!g.row_bytes || uint64_t(g.src_col) + g.row_bytes > g.src_pitch ||
+                   uint64_t(g.rows) * g.src_pitch != g.part_bytes)) {
+        fail("r_rdma_scatter: bad row geometry (rows >= 1, src_col + row_bytes <= src_pitch, "
+             "part_bytes == rows * src_pitch)");
+        return -1;
+    }
     return read_blocks(kOpReadLookup, blocks, int(g.nparts * g.part_bytes), 0, device, stream, 0,
                        nullptr, nullptr, &g);
 }
@@ -996,9 +1017,9 @@ int Connection::r_rdma_scatter_fp8(const GatherSpec& g, int elems,
     if (blocks.empty()) return 0;
     std::vector<uint64_t> offs(blocks.size());
     for (size_t i = 0; i < blocks.size(); ++i) offs[i] = blocks[i].offset;
-    if (device < 0 || !gather_fp8_ok(g, elems, offs.data(), offs.size(), g.first_part)) {
+    if (device < 0 || g.rows || !gather_fp8_ok(g, elems, offs.data(), offs.size(), g.first_part)) {
         fail("r_rdma_scatter_fp8: needs CUDA tensors, parts of a multiple of 512 elements and "
-             "16-byte aligned part bases and offsets");
+             "16-byte aligned part bases and offsets, and reads whole parts");
         return -1;
     }
     GatherSpec r = g;
@@ -1076,7 +1097,7 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
                         .fp8_elems = uint32_t(fp8_elems), .gather = gather != nullptr,
                         .copy_variant = copy_variant_, .all_local = true, .all_remote = true,
                         .max_ctas = max_ctas_, .sm_count = kernels::sm_count(),
-                        .layered = layered};
+                        .layered = layered, .rows = gather && gather->rows};
         // over every known segment, not only the ones this batch touches: intentional
         for (uint32_t s = 0; s < R.nsegs; ++s) {
             in.all_remote = in.all_remote && ctx->seg_remote[s];
@@ -1175,8 +1196,10 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
         stats_.ns_build += t_launch0 - t_build0;
         stats_.ns_launch += now_ns() - t_launch0;
         // lookup + copy + validate: resolve_descs counted the lookup
+        const uint64_t moved = gather && gather->rows ? gather_moved_bytes(*gather)
+                                                      : uint64_t(block_size);
         if (scope.launched(e, "device-index read failed to launch: ", plan.fused() ? 1 : 2, false,
-                           uint64_t(n) * uint64_t(block_size)) != 0)
+                           uint64_t(n) * moved) != 0)
             return -1;
     }
     if (hold.seq) return hold.done();

@@ -21,6 +21,7 @@ struct DeviceReadIn {
     bool all_local = false, all_remote = false;
     int max_ctas = 0, sm_count = 0;  // max_ctas: the connection's grid cap, 0 = none
     bool layered = false;  // a layered read of gathered blocks (GatherLaunch::group_flags)
+    bool rows = false;     // a row-sliced read of gathered blocks (GatherLaunch::rows)
 };
 
 enum class ReadPath {
@@ -75,8 +76,9 @@ inline DeviceReadPlan plan_device_read(const DeviceReadIn& in) {
     // gathered fp8 blocks: each key is probed once by the lookup kernel and re-checked after the
     // dequantising scatter; never the bf16 scatter pipeline.
     // layered reads: lookup, the layered ld/st scatter (the only kernels that release groups),
-    // validate - each key probed once, by the lookup kernel
-    if (in.gather && in.layered) {
+    // validate - each key probed once, by the lookup kernel.  Row-sliced reads the same way:
+    // only the ld/st scatter has a row form.
+    if (in.gather && (in.layered || in.rows)) {
         p.path = in.fp8_elems ? ReadPath::kLookupGatherFp8 : ReadPath::kLookupGather;
         p.variant = in.fp8_elems ? int(kernels::kFp8LdSt) : int(kernels::kCopyLdSt);
         return p;

@@ -68,4 +68,44 @@ __device__ __forceinline__ void copy_span(uint8_t* dst, const uint8_t* src, uint
     for (uint32_t b = nvec * 16 + tid; b < len; b += kLdStThreads) dst[b] = src[b];
 }
 
+// `nrows` rows of row_bytes, row r from src + r * src_pitch to dst + r * dst_pitch.  The 256
+// threads walk the (row, vector) pairs flattened together, so rows much narrower than a CTA's
+// 4 KB per pass (one KV head of 128 bf16 is 256 bytes) still keep every thread busy.  VEC = 16
+// / 32 as for copy_span (row_bytes, both pitches and both bases aligned to VEC); VEC = 1: bytes.
+template <int VEC>
+__device__ __forceinline__ void copy_rows(uint8_t* dst, const uint8_t* src, uint32_t nrows,
+                                          uint32_t row_bytes, uint32_t src_pitch,
+                                          uint32_t dst_pitch) {
+    const uint32_t tid = threadIdx.x;
+    if constexpr (VEC == 1) {
+        const uint32_t len = nrows * row_bytes;
+        for (uint32_t b = tid; b < len; b += kLdStThreads) {
+            const uint32_t r = b / row_bytes, c = b - r * row_bytes;
+            dst[size_t(r) * dst_pitch + c] = src[size_t(r) * src_pitch + c];
+        }
+    } else {
+        static_assert(VEC == 16 || VEC == 32, "vector width");
+        constexpr int U = VEC / 4;
+        const uint32_t vpr = row_bytes / 16;  // vectors per row
+        const uint32_t nvec = nrows * vpr;
+        const auto at = [vpr](uint32_t v, uint32_t pitch) {
+            const uint32_t r = v / vpr;
+            return size_t(r) * pitch + size_t(v - r * vpr) * 16;
+        };
+        uint32_t i = tid;
+        for (; i + (U - 1) * kLdStThreads < nvec; i += U * kLdStThreads) {
+            uint4 v[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                const uint8_t* s = src + at(i + u * kLdStThreads, src_pitch);
+                v[u] = VEC == 16 ? ld_stream_v4(s) : ld_v4(s);
+            }
+#pragma unroll
+            for (int u = 0; u < U; ++u) st_v4(dst + at(i + u * kLdStThreads, dst_pitch), v[u]);
+        }
+        for (; i < nvec; i += kLdStThreads)
+            st_v4(dst + at(i, dst_pitch), ld_stream_v4(src + at(i, src_pitch)));
+    }
+}
+
 }  // namespace istore::kernels

@@ -180,9 +180,20 @@ struct GatherLaunch {
     uint32_t* group_counters = nullptr;
     uint32_t group_seq = 0;
     uint32_t group_parts = 0;
+    // Row-sliced read (reads only, ld/st kernels only; rows == 0: whole contiguous parts): the
+    // reader's share of stored part s is `rows` rows of row_bytes at a pitch of src_pitch,
+    // src_col bytes into each row (part_bytes == rows * src_pitch), and row r lands at
+    // part_base[s] + desc.dst + r * dst_pitch - e.g. a decode rank's KV heads of a page that
+    // a prefill rank at another tensor-parallel degree wrote.  Works with group_flags.
+    uint32_t rows = 0;
+    uint32_t row_bytes = 0;
+    uint32_t src_pitch = 0;
+    uint32_t src_col = 0;
+    uint32_t dst_pitch = 0;
 };
 // The TMA pipeline for 16-byte aligned parts of at least kPipeMinBytes, the ld/st kernel
-// (kv_copy.cu) otherwise: the same rule launch_kv_copy applies to whole blocks.
+// (kv_copy.cu) otherwise: the same rule launch_kv_copy applies to whole blocks.  A row-sliced
+// read runs kv_scatter_rows (kv_copy.cu).
 cudaError_t launch_kv_gather(const GatherLaunch& a, cudaStream_t stream);
 cudaError_t launch_kv_pipe_gather(const GatherLaunch& a, cudaStream_t stream);
 struct GatherParts {

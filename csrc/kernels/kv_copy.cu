@@ -184,6 +184,86 @@ __global__ void __launch_bounds__(kLdStThreads + 32, 3)
     if (pub.recs) ctrl_barrier_arrive(kLdStThreads + 32);
 }
 
+// ---------------------------------------------------------------- row-sliced reads (ld/st)
+struct RowGeometry {
+    uint32_t rows, row_bytes, src_pitch, src_col, dst_pitch, part_bytes;
+};
+
+// GatherLaunch::rows.  Item = run c (`run` rows) of part s of block b, numbered
+// (b * nparts + s) * cpp + c - which is layered_item's numbering with one group of all nparts
+// parts - or, LAYERED, group-major with rel.gp parts per group, each group released by
+// leave_group as in gather_read_layered.  Row r of the run:
+//   pool desc.src + (first_part + s) * part_bytes + r * src_pitch + src_col   (row_bytes)
+//     -> parts.base[s] + desc.dst + r * dst_pitch.
+// A missing block counts once, on its first item, and its parts are left untouched; its items
+// still count as arrivals.  No control warp: reads publish nothing.
+template <int VEC, bool LAYERED>
+__global__ void __launch_bounds__(kLdStThreads, 3)
+    kv_scatter_rows_kernel(const CopyDesc* __restrict__ descs,
+                           const __grid_constant__ GatherParts parts, uint32_t n, uint32_t nparts,
+                           uint32_t first_part, RowGeometry geo, uint32_t run, uint32_t cpp,
+                           uint32_t* status, GroupRelease rel) {
+    const uint32_t gp = LAYERED ? rel.gp : nparts;
+    const uint32_t group_items = n * gp * cpp;
+    const uint32_t total = n * nparts * cpp;
+    uint32_t item = blockIdx.x;
+    CopyDesc next = item < total ? descs[layered_item(item, n, gp, cpp).block] : CopyDesc{0, 0};
+    for (; item < total; item += gridDim.x) {
+        const CopyDesc d = next;
+        const LayeredItem it = layered_item(item, n, gp, cpp);
+        const uint32_t nxt = item + gridDim.x;
+        if (nxt < total) next = descs[layered_item(nxt, n, gp, cpp).block];
+        if (d.src != 0) {
+            const uint32_t r0 = it.chunk * run;
+            const uint8_t* src = reinterpret_cast<const uint8_t*>(
+                d.src + uint64_t(first_part + it.part) * geo.part_bytes +
+                uint64_t(r0) * geo.src_pitch + geo.src_col);
+            uint8_t* dst = reinterpret_cast<uint8_t*>(parts.base[it.part] + d.dst +
+                                                      uint64_t(r0) * geo.dst_pitch);
+            copy_rows<VEC>(dst, src, min(run, geo.rows - r0), geo.row_bytes, geo.src_pitch,
+                           geo.dst_pitch);
+        } else if (threadIdx.x == 0 && item < group_items && item % (gp * cpp) == 0 && status) {
+            atomicAdd(status + kStatMiss, 1u);
+        }
+        if constexpr (LAYERED) {
+            if (nxt >= total || nxt / group_items != it.group) {
+                const uint32_t lo = it.group * group_items;
+                leave_group(rel, it.group, cta_items(lo, lo + group_items, blockIdx.x, gridDim.x),
+                            group_items, kLdStThreads);
+            }
+        }
+    }
+}
+
+cudaError_t launch_kv_scatter_rows(const GatherLaunch& a, cudaStream_t stream) {
+    static const LdStResident res = ldst_resident(kv_scatter_rows_kernel<16, false>,
+                                                  kv_scatter_rows_kernel<32, false>, kLdStThreads);
+    static const LdStResident res_layered = ldst_resident(
+        kv_scatter_rows_kernel<16, true>, kv_scatter_rows_kernel<32, true>, kLdStThreads);
+    const bool layered = a.group_flags != nullptr;
+    const LaunchPlan p = plan_gather_rows(a, sm_count(), layered ? res_layered : res);
+    if (!p.valid) return cudaErrorInvalidValue;  // the caller checks the geometry and splits
+    GatherParts parts;
+    std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
+    const RowGeometry geo{a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.part_bytes};
+    const GroupRelease rel{a.group_flags, a.group_counters, a.group_seq, a.group_parts};
+    const auto go = [&](auto* kernel) {
+        kernel<<<p.ctas, kLdStThreads, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.first_part,
+                                                    geo, p.chunk, p.cpb, a.status, rel);
+        return cudaGetLastError();
+    };
+    switch (p.kernel) {
+        case Kernel::kLdSt1:
+            return layered ? go(kv_scatter_rows_kernel<1, true>) : go(kv_scatter_rows_kernel<1, false>);
+        case Kernel::kLdSt32:
+            return layered ? go(kv_scatter_rows_kernel<32, true>)
+                           : go(kv_scatter_rows_kernel<32, false>);
+        default:
+            return layered ? go(kv_scatter_rows_kernel<16, true>)
+                           : go(kv_scatter_rows_kernel<16, false>);
+    }
+}
+
 }  // namespace
 
 int sm_count() {
@@ -251,6 +331,7 @@ cudaError_t launch_kv_gather(const GatherLaunch& a, cudaStream_t stream) {
     if (uint64_t(a.nparts) * a.part_bytes > 0xffffffffull) return cudaErrorInvalidValue;
     const bool layered = a.group_flags != nullptr;
     if (layered && !a.group_counters) return cudaErrorInvalidValue;
+    if (a.rows) return launch_kv_scatter_rows(a, stream);
     constexpr int T = kLdStThreads + 32;
     static const LdStResident res =
         ldst_resident(kv_gather_ldst_kernel<16>, kv_gather_ldst_kernel<32>, T);

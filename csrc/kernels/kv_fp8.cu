@@ -352,7 +352,7 @@ cudaError_t launch_kv_read_fp8(const Fp8Launch& a, cudaStream_t stream) {
 cudaError_t launch_kv_gather_fp8(const GatherLaunch& a, uint32_t elems, int variant,
                                  cudaStream_t stream) {
     if (a.n == 0) return cudaSuccess;
-    if (!a.part_base) return cudaErrorInvalidValue;
+    if (!a.part_base || a.rows) return cudaErrorInvalidValue;  // no row-sliced fp8 reads
     // a layered read takes the ld/st kernel whatever the variant (no layered pipeline)
     const bool layered = a.group_flags != nullptr;
     if (layered && (a.write || !a.group_counters || !a.group_parts || a.nparts % a.group_parts))

@@ -682,7 +682,7 @@ cudaError_t launch_kv_pipe_gather(const GatherLaunch& a, cudaStream_t stream) {
 }
 
 bool scatter_read_fused_supported(const ReadFusedLaunch& r, const GatherLaunch& g) {
-    return g.nparts >= 1 && g.nparts <= kGatherMaxParts && g.part_base && g.part_bytes &&
+    return g.rows == 0 && g.nparts >= 1 && g.nparts <= kGatherMaxParts && g.part_base && g.part_bytes &&
            (g.part_bytes % 16) == 0 && (g.align_or & 15) == 0 &&
            r.n >= uint32_t(scatter_read_ctas(r, sm_count()));
 }

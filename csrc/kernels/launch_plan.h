@@ -3,7 +3,7 @@
 // kv_fp8.cu, kv_fp8_pipe.cu) pass in the SM count and the CTAs per SM the ld/st kernels keep
 // resident (occupancy API), so the choice is unit-tested on the CPU
 // (_infinistore.testing.plan_copy / plan_gather / plan_read_fused / plan_fp8 /
-// plan_gather_fp8 / plan_gather_layered).
+// plan_gather_fp8 / plan_gather_layered / plan_gather_rows).
 #pragma once
 
 #include <algorithm>
@@ -247,6 +247,32 @@ inline LaunchPlan plan_gather_layered(const GatherLaunch& a, int sms, LdStReside
     p.kernel = !aligned16 ? Kernel::kLdSt1 : aligned32 ? Kernel::kLdSt32 : Kernel::kLdSt16;
     const uint64_t parts = uint64_t(a.n) * a.nparts;
     ldst_items(p, parts, a.part_bytes, kLdStChunk, 1u << 20, sms);
+    if (parts * p.cpb > kMaxItems) return invalid_plan();
+    p.ctas = ldst_grid(p, a.max_ctas, res, sms, parts * p.cpb);
+    return p;
+}
+
+// ---------------------------------------------------------------- row-sliced reads
+// kv_scatter_rows (GatherLaunch::rows != 0), plain or layered: always the ld/st kernels (the
+// TMA pipelines have no row form).  The vector width is the one the OR of row_bytes, both
+// pitches, src_col, the part bases and the local offsets allows (pool blocks are granule
+// aligned and part_bytes is a multiple of src_pitch).  A work item is a run of `chunk` rows of
+// one part, about kLdStChunk of payload, or all of a part's rows under ldst_items' rule; cpb
+// is runs per part, and a layered read numbers items with layered_item as whole parts do.
+inline LaunchPlan plan_gather_rows(const GatherLaunch& a, int sms, LdStResident res) {
+    if (a.write || a.rows == 0 || a.row_bytes == 0 || a.nparts == 0 ||
+        a.nparts > kGatherMaxParts || uint64_t(a.src_col) + a.row_bytes > a.src_pitch ||
+        uint64_t(a.rows) * a.src_pitch != a.part_bytes ||
+        (a.group_flags && (a.group_parts == 0 || a.nparts % a.group_parts != 0)))
+        return invalid_plan();
+    const uint64_t geo_or = a.align_or | a.src_pitch | a.src_col | a.dst_pitch;
+    const bool aligned16 = aligned_to(a.row_bytes, geo_or, 16);
+    const bool aligned32 = aligned_to(a.row_bytes, geo_or, 32);
+    LaunchPlan p;
+    p.kernel = !aligned16 ? Kernel::kLdSt1 : aligned32 ? Kernel::kLdSt32 : Kernel::kLdSt16;
+    const uint64_t parts = uint64_t(a.n) * a.nparts;
+    ldst_items(p, parts, a.rows, std::max(1u, kLdStChunk / a.row_bytes),
+               std::max(1u, (1u << 20) / a.row_bytes), sms);
     if (parts * p.cpb > kMaxItems) return invalid_plan();
     p.ctas = ldst_grid(p, a.max_ctas, res, sms, parts * p.cpb);
     return p;

@@ -180,6 +180,19 @@ struct KeyArena {
 
 thread_local KeyArena t_arena;
 
+// A row-sliced read's geometry, (rows, row_bytes, src_pitch, src_col, dst_pitch) in bytes;
+// empty: whole parts.  The connection checks the values.
+void set_rows(Connection::GatherSpec& g, const std::vector<uint32_t>& rows) {
+    if (rows.empty()) return;
+    if (rows.size() != 5)
+        throw py::value_error("rows is (rows, row_bytes, src_pitch, src_col, dst_pitch)");
+    g.rows = rows[0];
+    g.row_bytes = rows[1];
+    g.src_pitch = rows[2];
+    g.src_col = rows[3];
+    g.dst_pitch = rows[4];
+}
+
 // [(key, offset), ...] -> KeyOffset views (offset * scale bytes).  Also accepted: the pair
 // (keys, offsets) with `keys` a sequence of str / bytes and `offsets` an integer ndarray of the
 // same length - callers that hold their offsets in numpy anyway skip one heap object and one
@@ -578,7 +591,7 @@ PYBIND11_MODULE(_infinistore, m) {
             "r_rdma_scatter",
             [](Connection& c, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
                uint32_t first_part, const py::object& blocks, int device, uint64_t stream,
-               uint64_t scale) {
+               uint64_t scale, const std::vector<uint32_t>& rows) {
                 std::vector<KeyOffset> kb;
                 blocks_list_from_py(blocks, scale, kb);
                 Connection::GatherSpec g;
@@ -586,12 +599,16 @@ PYBIND11_MODULE(_infinistore, m) {
                 g.nparts = uint32_t(part_base.size());
                 g.part_bytes = part_bytes;
                 g.first_part = first_part;
+                set_rows(g, rows);
                 py::gil_scoped_release rel;
                 return c.r_rdma_scatter(g, kb, device, stream);
             },
             py::arg("part_base"), py::arg("part_bytes"), py::arg("first_part"), py::arg("blocks"),
             py::arg("device") = -1, py::arg("stream") = 0, py::arg("scale") = 1,
-            "scattered read: stored part first_part + s of each block -> part_base[s] + offset")
+            py::arg("rows") = std::vector<uint32_t>{},
+            "scattered read: stored part first_part + s of each block -> part_base[s] + offset; "
+            "rows = (rows, row_bytes, src_pitch, src_col, dst_pitch): only those rows of each "
+            "part, row r to part_base[s] + offset + r * dst_pitch")
         .def(
             "w_rdma_gather_fp8",
             [](Connection& c, const std::vector<uint64_t>& part_base, int elems,
@@ -636,7 +653,7 @@ PYBIND11_MODULE(_infinistore, m) {
             "r_rdma_scatter_layered",
             [](Connection& c, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
                int elems, uint32_t first_part, uint32_t group_parts, const py::object& blocks,
-               int device, uint64_t stream, uint64_t scale) {
+               int device, uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows) {
                 std::vector<KeyOffset> kb;
                 blocks_list_from_py(blocks, scale, kb);
                 Connection::GatherSpec g;
@@ -644,6 +661,7 @@ PYBIND11_MODULE(_infinistore, m) {
                 g.nparts = uint32_t(part_base.size());
                 g.part_bytes = part_bytes;
                 g.first_part = first_part;
+                set_rows(g, rows);
                 auto r = std::make_shared<Connection::ScatterReader>();
                 py::gil_scoped_release rel;
                 c.read_scatter_layered(g, elems, group_parts, kb, device, stream, *r);
@@ -651,7 +669,7 @@ PYBIND11_MODULE(_infinistore, m) {
             },
             py::arg("part_base"), py::arg("part_bytes"), py::arg("elems"), py::arg("first_part"),
             py::arg("group_parts"), py::arg("blocks"), py::arg("device") = -1,
-            py::arg("stream") = 0, py::arg("scale") = 1,
+            py::arg("stream") = 0, py::arg("scale") = 1, py::arg("rows") = std::vector<uint32_t>{},
             "layered scattered read (r_rdma_scatter, or r_rdma_scatter_fp8 with elems > 0) "
             "whose parts are released in groups of group_parts; check .failed")
         .def(
@@ -996,7 +1014,7 @@ PYBIND11_MODULE(_infinistore, m) {
            uint64_t table, uint64_t table_mask, uint64_t done, uint64_t status, uint64_t align_or,
            uint32_t stage_bytes, uint32_t ring_bytes, uint64_t layer_state, uint32_t layer_parts,
            bool layer_claim, uint64_t group_flags, uint64_t group_counters, uint32_t group_seq,
-           uint32_t group_parts) {
+           uint32_t group_parts, const std::vector<uint32_t>& rows) {
             if (part_base.empty() || part_base.size() > kernels::kGatherMaxParts)
                 throw std::runtime_error("kv_gather: 1 to GATHER_MAX_PARTS parts");
             if (layer_state && first_part + part_base.size() > layer_parts)
@@ -1029,6 +1047,14 @@ PYBIND11_MODULE(_infinistore, m) {
             G.group_counters = as_ptr<uint32_t>(group_counters);
             G.group_seq = group_seq;
             G.group_parts = group_parts;
+            if (!rows.empty()) {
+                if (rows.size() != 5) throw std::runtime_error("kv_gather: rows is 5 values");
+                G.rows = rows[0];
+                G.row_bytes = rows[1];
+                G.src_pitch = rows[2];
+                G.src_col = rows[3];
+                G.dst_pitch = rows[4];
+            }
             const cudaError_t e = kernels::launch_kv_gather(G, as_ptr<CUstream_st>(stream));
             if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
         },
@@ -1039,7 +1065,7 @@ PYBIND11_MODULE(_infinistore, m) {
         py::arg("align_or") = 0, py::arg("stage_bytes") = 0, py::arg("ring_bytes") = 0,
         py::arg("layer_state") = 0, py::arg("layer_parts") = 0, py::arg("layer_claim") = false,
         py::arg("group_flags") = 0, py::arg("group_counters") = 0, py::arg("group_seq") = 0,
-        py::arg("group_parts") = 0,
+        py::arg("group_parts") = 0, py::arg("rows") = std::vector<uint32_t>{},
         "gathered blocks: descs[i] = write {local byte offset, block address} / read {block "
         "address or 0, local byte offset}; part s of block i at part_base[s] + local offset is "
         "stored part first_part + s.  layer_state (3 zeroed u32 per block, kept across the "
@@ -1539,10 +1565,10 @@ PYBIND11_MODULE(_infinistore, m) {
     t.def("plan_device_read",
           [](size_t n, uint32_t block_bytes, uint32_t fp8_elems, bool gather, bool fp8_fused_ok,
              bool scatter_fused_ok, int copy_variant, bool all_local, bool all_remote, int max_ctas,
-             int sm_count, bool layered) {
+             int sm_count, bool layered, bool rows) {
               const DeviceReadPlan p = plan_device_read(DeviceReadIn{
                   n, block_bytes, fp8_elems, gather, fp8_fused_ok, scatter_fused_ok, copy_variant,
-                  all_local, all_remote, max_ctas, sm_count, layered});
+                  all_local, all_remote, max_ctas, sm_count, layered, rows});
               static const char* const kPaths[] = {"fused_copy",    "fused_fp8",
                                                    "fused_scatter", "lookup_copy",
                                                    "lookup_fp8",    "lookup_gather",
@@ -1556,7 +1582,8 @@ PYBIND11_MODULE(_infinistore, m) {
           py::arg("n"), py::arg("block_bytes"), py::arg("fp8_elems") = 0, py::arg("gather") = false,
           py::arg("fp8_fused_ok") = false, py::arg("scatter_fused_ok") = false,
           py::arg("copy_variant") = 0, py::arg("all_local") = false, py::arg("all_remote") = false,
-          py::arg("max_ctas") = 0, py::arg("sm_count") = 132, py::arg("layered") = false);
+          py::arg("max_ctas") = 0, py::arg("sm_count") = 132, py::arg("layered") = false,
+          py::arg("rows") = false);
     // which kernel a page-mover launcher runs, its work split and grid (kernels/launch_plan.h);
     // the resident CTAs per SM of the ld/st kernels are the occupancy API's answer on a GPU
     const auto plan_dict = [](const kernels::LaunchPlan& p) {
@@ -1628,6 +1655,31 @@ PYBIND11_MODULE(_infinistore, m) {
           py::arg("n"), py::arg("nparts"), py::arg("part_bytes"), py::arg("group_parts") = 2,
           py::arg("align_or") = 0, py::arg("max_ctas") = 0, py::arg("sm_count") = 132,
           py::arg("resident16") = 1, py::arg("resident32") = 1);
+    t.def("plan_gather_rows",
+          [plan_dict](uint32_t n, uint32_t nparts, uint32_t rows, uint32_t row_bytes,
+                      uint32_t src_pitch, uint32_t src_col, uint32_t dst_pitch, uint64_t align_or,
+                      uint32_t group_parts, int max_ctas, int sm_count, int resident16,
+                      int resident32) {
+              static uint32_t flags[1];  // the plan only asks whether the read is layered
+              kernels::GatherLaunch a;
+              a.n = n;
+              a.nparts = nparts;
+              a.part_bytes = uint32_t(uint64_t(rows) * src_pitch);
+              a.rows = rows;
+              a.row_bytes = row_bytes;
+              a.src_pitch = src_pitch;
+              a.src_col = src_col;
+              a.dst_pitch = dst_pitch;
+              a.align_or = align_or;
+              a.group_flags = group_parts ? flags : nullptr;
+              a.group_parts = group_parts;
+              a.max_ctas = max_ctas;
+              return plan_dict(kernels::plan_gather_rows(a, sm_count, {resident16, resident32}));
+          },
+          py::arg("n"), py::arg("nparts"), py::arg("rows"), py::arg("row_bytes"),
+          py::arg("src_pitch"), py::arg("src_col") = 0, py::arg("dst_pitch") = 0,
+          py::arg("align_or") = 0, py::arg("group_parts") = 0, py::arg("max_ctas") = 0,
+          py::arg("sm_count") = 132, py::arg("resident16") = 1, py::arg("resident32") = 1);
     t.def("plan_read_fused",
           [plan_dict](uint32_t n, uint32_t bytes, uint64_t align_or, int variant, int max_ctas,
                       uint32_t stage_bytes, uint32_t ring_bytes, int sm_count, int resident16,

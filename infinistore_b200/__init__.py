@@ -18,8 +18,8 @@ _REFERENCE_SURFACE = (
     "TYPE_RDMA", "TYPE_LOCAL_GPU", "LINK_ETHERNET", "LINK_IB",
     "register_server", "purge_kv_map", "get_kvmap_len", "check_supported",
 )
-# added here: in-process server control, statistics, checkpoint / resume
-_ADDITIONS = ("stop_server", "server_stats", "dump_kv_map", "load_kv_map")
+# added here: in-process server control, statistics, checkpoint / resume, row-sliced reads
+_ADDITIONS = ("stop_server", "server_stats", "dump_kv_map", "load_kv_map", "PartRows")
 
 __all__ = [*_REFERENCE_SURFACE, *_ADDITIONS]
 globals().update({_name: getattr(_lib, _name) for _name in __all__})

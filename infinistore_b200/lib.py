@@ -330,6 +330,53 @@ class DisableTorchCaching:
         return
 
 
+class PartRows:
+    """Row geometry of a row-sliced scattered read (``read_cache_scatter(rows=...)``), in
+    elements: the reader takes ``count`` rows of ``width`` elements from each stored part, row
+    r at ``r * src_pitch + src_offset`` of the part, and stores row r at
+    ``r * dst_pitch`` from the block's destination offset.  The stored part is
+    ``count * src_pitch`` elements.  With token-major KV pages, a row is one token and
+    ``src_offset`` / ``width`` pick a run of KV heads: how a decode rank reads the heads it
+    owns out of pages that a prefill rank at another tensor-parallel degree wrote."""
+
+    __slots__ = ("count", "width", "src_pitch", "src_offset", "dst_pitch")
+
+    def __init__(self, count: int, width: int, src_pitch: int, src_offset: int = 0, *,
+                 dst_pitch: int):
+        self.count, self.width = int(count), int(width)
+        self.src_pitch, self.src_offset, self.dst_pitch = int(src_pitch), int(src_offset), int(dst_pitch)
+
+    def __repr__(self):
+        return (f"PartRows(count={self.count}, width={self.width}, src_pitch={self.src_pitch}, "
+                f"src_offset={self.src_offset}, dst_pitch={self.dst_pitch})")
+
+    def __eq__(self, other):
+        return isinstance(other, PartRows) and all(
+            getattr(self, f) == getattr(other, f) for f in self.__slots__)
+
+    def check(self, part_size: int) -> int:
+        """Raises ``ValueError`` unless the geometry fits a stored part of ``part_size``
+        elements and destination rows do not overlap.  Returns the destination extent of one
+        part in elements, ``(count - 1) * dst_pitch + width``."""
+        if self.count < 1 or self.width < 1 or self.src_offset < 0:
+            raise ValueError(f"{self}: count and width must be positive, src_offset >= 0")
+        if self.src_offset + self.width > self.src_pitch:
+            raise ValueError(f"{self}: src_offset + width runs past src_pitch")
+        if self.count * self.src_pitch != int(part_size):
+            raise ValueError(f"{self}: count * src_pitch must equal part_size {int(part_size)}")
+        if self.dst_pitch < self.width:
+            raise ValueError(f"{self}: dst_pitch must be at least width (rows must not overlap)")
+        return (self.count - 1) * self.dst_pitch + self.width
+
+    def native(self, es: int):
+        """(rows, row_bytes, src_pitch, src_col, dst_pitch) in bytes, for the connection."""
+        out = [self.count, self.width * es, self.src_pitch * es, self.src_offset * es,
+               self.dst_pitch * es]
+        if max(out) >= 1 << 32:
+            raise ValueError(f"{self}: a byte size exceeds 32 bits")
+        return out
+
+
 def _device_of(cache: torch.Tensor) -> int:
     return cache.device.index if cache.device.type == "cuda" else -1
 
@@ -594,7 +641,7 @@ class InfinityConnection:
 
     # ------------------------------------------------------------------ gathered blocks
     def _gather_parts(self, parts, max_offset: int, part_size: int, fp8: bool = False,
-                      offsets=None):
+                      offsets=None, extent=None):
         """Checks a parts list ``[(tensor, base), ...]`` before anything is enqueued.  Returns
         (absolute byte address of every part, device ordinal or -1, element size).  ``fp8``:
         the parts are bf16 CUDA tensors, ``part_size`` is a multiple of 512 elements and every
@@ -626,9 +673,10 @@ class InfinityConnection:
                 raise ValueError(f"part {i}: tensor on {t.device}, part 0 on {first.device}")
             if t.dtype != first.dtype:
                 raise ValueError(f"part {i}: dtype {t.dtype}, part 0 has {first.dtype}")
-            if base < 0 or base + max_offset + int(part_size) > t.numel():
-                raise ValueError(f"part {i}: base {base} + offset {max_offset} + part_size "
-                                 f"{int(part_size)} runs past the tensor's {t.numel()} elements")
+            span = int(part_size) if extent is None else int(extent)
+            if base < 0 or base + max_offset + span > t.numel():
+                raise ValueError(f"part {i}: base {base} + offset {max_offset} + part extent "
+                                 f"{span} runs past the tensor's {t.numel()} elements")
             bases.append(t.data_ptr() + base * es)
         if fp8:
             if first.dtype != torch.bfloat16:
@@ -697,7 +745,7 @@ class InfinityConnection:
         return keys, offs
 
     def read_cache_scatter(self, parts, blocks, part_size: int, first_part: int = 0,
-                           stream="current"):
+                           stream="current", rows: "PartRows | None" = None):
         """Scatter parts ``first_part .. first_part + len(parts) - 1`` of every stored block
         into the parts list (see ``rdma_write_cache_gather``): stored part ``first_part + s``
         of block ``(key, offset)`` lands at ``parts[s][1] + offset`` of ``parts[s][0]``.
@@ -707,15 +755,25 @@ class InfinityConnection:
         layer computes.  A missing key raises (with ``device_lookup``, ``sync()`` reports it)
         and counts once, not once per part; its destination parts are left untouched.  With
         ``device_lookup`` a stored block shorter than ``(first_part + len(parts)) * part_size``
-        elements is a miss, and a block purged or evicted during the read is reported as one."""
+        elements is a miss, and a block purged or evicted during the read is reported as one.
+
+        ``rows`` (a :class:`PartRows`) reads only those rows of every stored part (whose size
+        ``part_size`` still is, ``rows.count * rows.src_pitch``): row r lands at
+        ``parts[s][1] + offset + r * rows.dst_pitch``.  Several blocks may fill disjoint rows
+        of one destination, e.g. one per source rank of a page written at another
+        tensor-parallel degree.  Bad geometry raises ``ValueError`` before anything is
+        enqueued."""
         keys, offs = self._scatter_blocks(blocks, first_part)
-        bases, dev, es = self._gather_parts(parts, int(offs.max()) if len(offs) else 0, part_size)
+        extent = rows.check(part_size) if rows is not None else None
+        bases, dev, es = self._gather_parts(parts, int(offs.max()) if len(offs) else 0, part_size,
+                                            extent=extent)
         if (int(first_part) + len(bases)) * int(part_size) * es > _GATHER_MAX_BLOCK_BYTES:
             raise ValueError("first_part + parts run past the block size limit")
+        native_rows = rows.native(es) if rows is not None else []
         if not len(offs):
             return
         ret = self.conn.r_rdma_scatter(bases, int(part_size) * es, int(first_part), (keys, offs),
-                                       dev, _stream_of(parts[0][0], stream), es)
+                                       dev, _stream_of(parts[0][0], stream), es, native_rows)
         if ret < 0:
             raise Exception(f"Failed to read to infinistore, ret = {ret}: {self.conn.last_error()}")
 
@@ -774,7 +832,8 @@ class InfinityConnection:
     # ------------------------------------------------------------------ layered scattered reads
     def read_cache_scatter_layered(self, parts, blocks, part_size: int, group_parts: int = 2,
                                    first_part: int = 0, fp8: bool = False,
-                                   stream="current") -> "ScatterRead":
+                                   stream="current", rows: "PartRows | None" = None
+                                   ) -> "ScatterRead":
         """``read_cache_scatter`` (``read_cache_scatter_fp8`` with ``fp8``) in one call whose
         parts are released to consumers group by group: group ``g`` is parts
         ``g * group_parts .. g * group_parts + group_parts - 1`` of every block (with the
@@ -787,10 +846,14 @@ class InfinityConnection:
         memory.  ``group_parts`` must divide ``len(parts)``.  A group is released before the
         read's post-copy index check: when ``sync()`` reports a miss, treat the whole read as
         failed, as for any read.  A missing key on a connection without ``device_lookup``
-        raises here; the exception's ``read`` attribute is the failed reader."""
+        raises here; the exception's ``read`` attribute is the failed reader.  ``rows`` as for
+        ``read_cache_scatter`` (not with ``fp8``)."""
+        if rows is not None and fp8:
+            raise ValueError("row-sliced reads of fp8 blocks are not supported")
         keys, offs = self._scatter_blocks(blocks, first_part)
+        extent = rows.check(part_size) if rows is not None else None
         bases, dev, es = self._gather_parts(parts, int(offs.max()) if len(offs) else 0, part_size,
-                                            fp8=fp8, offsets=offs if fp8 else None)
+                                            fp8=fp8, offsets=offs if fp8 else None, extent=extent)
         if dev < 0:
             raise ValueError("layered reads take CUDA tensors")
         if not self.conn.server_has_hbm():
@@ -806,7 +869,8 @@ class InfinityConnection:
         first = parts[0][0]
         native = self.conn.r_rdma_scatter_layered(
             bases, int(part_size) * es, int(part_size) if fp8 else 0, int(first_part), group_parts,
-            (keys, offs), dev, _stream_of(first, stream), es)
+            (keys, offs), dev, _stream_of(first, stream), es,
+            rows.native(es) if rows is not None else [])
         read = ScatterRead(self, native, first.device)
         if native.failed:
             err = Exception(f"Failed to read to infinistore: {self.conn.last_error()}")

@@ -3,7 +3,7 @@ from __future__ import annotations
 
 import hashlib
 from dataclasses import dataclass
-from typing import Dict, List, Sequence
+from typing import Dict, List, Sequence, Tuple
 
 import torch
 
@@ -76,6 +76,47 @@ def chain_hashes(token_ids: Sequence[int], page_tokens: int, salt: str = "") -> 
 
 
 ALL_LAYERS = "all"  # layer field of a key whose block holds one page of every layer
+
+
+def _rank_heads(kv_heads: int, tp: int, rank: int) -> List[int]:
+    """The KV heads TP rank ``rank`` of ``tp`` holds: ``kv_heads // tp`` consecutive heads, or,
+    when ``tp > kv_heads`` (GQA replication), the one head ``rank * kv_heads // tp``."""
+    if tp < 1 or (kv_heads % tp and tp % kv_heads):
+        raise ValueError(f"TP {tp} neither divides nor is a multiple of {kv_heads} KV heads")
+    if not 0 <= rank < tp:
+        raise ValueError(f"TP rank {rank} is outside 0..{tp - 1}")
+    if tp >= kv_heads:
+        return [rank * kv_heads // tp]
+    per = kv_heads // tp
+    return list(range(rank * per, (rank + 1) * per))
+
+
+def tp_sources(layout: KVLayout, reader_tp: int, reader_rank: int,
+               writer_tp: int) -> List[Tuple[int, int, int, int]]:
+    """Where reader rank ``reader_rank`` (of ``reader_tp``) finds its KV heads in pages that
+    ranks at ``writer_tp`` wrote: a list of ``(writer_rank, src_head, dst_head, heads)``, each
+    ``heads`` consecutive heads from head ``src_head`` of that writer's page to head
+    ``dst_head`` of the reader's, in ``dst_head`` order and with equal ``heads``.  A replicated
+    head (``tp > kv_heads``) is taken from its first replica.  One source per page when the
+    reader holds no more heads than a writer rank (``reader_tp >= writer_tp``, and MLA's single
+    latent head), several otherwise.  Raises ``ValueError`` unless both degrees divide, or are
+    multiples of, ``layout.kv_heads``."""
+    h = layout.kv_heads
+    _rank_heads(h, writer_tp, 0)  # checks writer_tp
+    out: List[Tuple[int, int, int, int]] = []
+    for dst, head in enumerate(_rank_heads(h, reader_tp, reader_rank)):
+        if writer_tp >= h:
+            w, src = head * writer_tp // h, 0  # the first rank holding it
+        else:
+            per = h // writer_tp
+            w, src = head // per, head % per
+        last = out[-1] if out else None
+        if last and last[0] == w and last[1] + last[3] == src and last[2] + last[3] == dst:
+            out[-1] = (w, last[1], last[2], last[3] + 1)
+        else:
+            out.append((w, src, dst, 1))
+    assert len({s[3] for s in out}) == 1
+    return out
 
 
 def page_key(model: str, layer, kind: str, tp_rank: int, page_hash: str) -> str:

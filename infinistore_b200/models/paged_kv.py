@@ -6,7 +6,8 @@ from typing import List, Optional, Sequence
 import numpy as np
 import torch
 
-from .kv_layout import ALL_LAYERS, KVLayout, page_key
+from ..lib import PartRows
+from .kv_layout import ALL_LAYERS, KVLayout, page_key, tp_sources
 
 
 def layer_keys(layout: KVLayout, tp_rank: int, layer: int, kv: int,
@@ -137,19 +138,66 @@ class PagedKVCache:
         offs = np.asarray(pages, dtype=np.int64) * elems
         return PageWriter(self, conn.gather_writer(blocks, offs, nparts, elems, fp8=fp8))
 
-    def read_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
-                   layers: Optional[range] = None, stream="current", fp8: bool = False) -> int:
-        """Fetch pages written by ``write_pages`` into pages ``pages``.  ``layers`` (a range
-        with step 1, default all) reads only those layers' parts of the blocks, so layer l
-        can be fetched while layer l - 1 computes.  ``fp8`` must be what the writer used.
-        Returns the number of blocks read."""
+    def _cross_tp(self, source_tp: Optional[int], fp8: bool = False) -> bool:
+        """Whether a read of pages written at ``source_tp`` regroups heads (checked)."""
+        if source_tp is None or int(source_tp) == self.layout.tp:
+            return False
         if fp8:
-            self._check_fp8()
-        self._ensure_registered(conn)
+            raise ValueError("pages written at another TP degree cannot be read as fp8")
+        return True
+
+    def _sources(self, pages: Sequence[int], page_hashes: Sequence[str], source_tp: int):
+        """The blocks of a read of pages written at ``source_tp``: one per (page, source
+        rank), keyed by the writer rank, each landing at its heads of the reader's page, and
+        the rows every block gives (``PartRows``) and the stored part size."""
+        lay = self.layout
+        wl = lay.with_tp(int(source_tp))
+        srcs = tp_sources(lay, lay.tp, self.tp_rank, wl.tp)
+        if len({s[1] for s in srcs}) != 1:  # holds for every pair tp_sources accepts
+            raise ValueError("sources start at different heads of their pages")
+        heads, src_head = srcs[0][3], srcs[0][1]
+        if len(pages) != len(page_hashes):
+            raise ValueError(f"{len(pages)} pages for {len(page_hashes)} page hashes")
+        keys = [page_key(lay.name, ALL_LAYERS, "KV", w, h) for h in page_hashes for w, *_ in srcs]
+        offs = (np.asarray(pages, dtype=np.int64)[:, None] * lay.page_elems
+                + np.asarray([d * lay.head_dim for _, _, d, _ in srcs], dtype=np.int64)[None, :])
+        rows = PartRows(lay.page_tokens, heads * lay.head_dim, wl.heads_per_rank * lay.head_dim,
+                        src_head * lay.head_dim, dst_pitch=lay.heads_per_rank * lay.head_dim)
+        return keys, offs.reshape(-1), rows, wl.page_elems
+
+    def _check_layers(self, layers: Optional[range]) -> range:
         layers = range(self.layout.layers) if layers is None else layers
         if layers.step != 1 or not len(layers) or layers.start < 0 or layers.stop > self.layout.layers:
             raise ValueError(f"layers must be a non-empty step-1 range within "
                              f"0..{self.layout.layers}")
+        return layers
+
+    def read_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
+                   layers: Optional[range] = None, stream="current", fp8: bool = False,
+                   source_tp: Optional[int] = None) -> int:
+        """Fetch pages written by ``write_pages`` into pages ``pages``.  ``layers`` (a range
+        with step 1, default all) reads only those layers' parts of the blocks, so layer l
+        can be fetched while layer l - 1 computes.  ``fp8`` must be what the writer used.
+        Returns the number of blocks read.
+
+        ``source_tp``: the pages were written by ranks at that tensor-parallel degree (e.g. a
+        prefill instance at TP 8 feeding this decode rank at TP 2).  Each page is then read
+        from every writer rank holding some of this rank's KV heads
+        (``kv_layout.tp_sources``), in one call: the read kernel copies each source's heads,
+        token by token, straight into this cache.  Any missing source fails the read (it
+        raises, or with ``device_lookup`` ``sync()`` reports the miss); its heads are left
+        untouched, so treat every page of a failed read as not read.  Not with ``fp8``.
+        Returns the number of (page, source) blocks read."""
+        cross = self._cross_tp(source_tp, fp8)
+        if fp8:
+            self._check_fp8()
+        self._ensure_registered(conn)
+        layers = self._check_layers(layers)
+        if cross:
+            keys, offs, rows, part = self._sources(pages, page_hashes, source_tp)
+            conn.read_cache_scatter(self._parts(layers), (keys, offs), part,
+                                    first_part=2 * layers.start, stream=stream, rows=rows)
+            return len(keys)
         keys = self.page_keys(page_hashes)
         offs = np.asarray(pages, dtype=np.int64) * self.layout.page_elems
         read = conn.read_cache_scatter_fp8 if fp8 else conn.read_cache_scatter
@@ -159,19 +207,24 @@ class PagedKVCache:
 
     def read_pages_layered(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
                            layers: Optional[range] = None, fp8: bool = False,
-                           stream="current") -> "PageRead":
+                           stream="current", source_tp: Optional[int] = None) -> "PageRead":
         """``read_pages`` in one call that releases each layer as it lands: the returned
         reader's ``wait_layer(l, stream)`` makes later work on ``stream`` wait, on the GPU,
         for layer l's K and V, so attention on layer 0 can start before the last layer has
-        arrived, with no host synchronisation.  ``layers`` (a step-1 range, default all) and
-        ``fp8`` as for ``read_pages``."""
+        arrived, with no host synchronisation.  ``layers`` (a step-1 range, default all),
+        ``fp8`` and ``source_tp`` as for ``read_pages``.  A layer is released before the
+        read's post-copy index check: when ``sync()`` reports a miss, the whole read failed."""
+        cross = self._cross_tp(source_tp, fp8)
         if fp8:
             self._check_fp8()
         self._ensure_registered(conn)
-        layers = range(self.layout.layers) if layers is None else layers
-        if layers.step != 1 or not len(layers) or layers.start < 0 or layers.stop > self.layout.layers:
-            raise ValueError(f"layers must be a non-empty step-1 range within "
-                             f"0..{self.layout.layers}")
+        layers = self._check_layers(layers)
+        if cross:
+            keys, offs, rows, part = self._sources(pages, page_hashes, source_tp)
+            read = conn.read_cache_scatter_layered(self._parts(layers), (keys, offs), part,
+                                                   group_parts=2, first_part=2 * layers.start,
+                                                   stream=stream, rows=rows)
+            return PageRead(read, layers)
         keys = self.page_keys(page_hashes)
         offs = np.asarray(pages, dtype=np.int64) * self.layout.page_elems
         read = conn.read_cache_scatter_layered(self._parts(layers), (keys, offs),
@@ -179,13 +232,31 @@ class PagedKVCache:
                                                first_part=2 * layers.start, fp8=fp8, stream=stream)
         return PageRead(read, layers)
 
+    def source_page_keys(self, page_hashes: Sequence[str], source_tp: int) -> List[List[str]]:
+        """All-layer page keys of every writer rank at ``source_tp`` that holds some of this
+        rank's KV heads, one list per source rank."""
+        srcs = tp_sources(self.layout, self.layout.tp, self.tp_rank, int(source_tp))
+        return [[page_key(self.layout.name, ALL_LAYERS, "KV", w, h) for h in page_hashes]
+                for w, *_ in srcs]
+
     def cached_prefix_pages(self, conn, page_hashes: Sequence[str],
-                            layer: Optional[int] = None, all_layer_pages: bool = False) -> int:
+                            layer: Optional[int] = None, all_layer_pages: bool = False,
+                            source_tp: Optional[int] = None) -> int:
         """How many leading pages of this prefix the store already holds (last layer's V
         pages are written last, so probing them answers for the whole stack).
-        ``all_layer_pages``: the pages were written with ``write_pages`` (one key each)."""
+        ``all_layer_pages``: the pages were written with ``write_pages`` (one key each).
+        ``source_tp`` (with ``all_layer_pages``): they were written at that TP degree; the
+        answer is the fewest pages any source rank of ``read_pages(source_tp=)`` holds."""
         if not page_hashes:
             return 0
+        if self._cross_tp(source_tp):
+            if not all_layer_pages:
+                raise ValueError("source_tp needs all_layer_pages")
+            try:
+                return min(conn.get_match_last_index(keys) + 1
+                           for keys in self.source_page_keys(page_hashes, source_tp))
+            except Exception:
+                return 0
         if all_layer_pages:
             keys = self.page_keys(page_hashes)
         else:
@@ -195,11 +266,18 @@ class PagedKVCache:
         except Exception:
             return 0
 
-    def touch_prefix(self, conn, page_hashes: Sequence[str], all_layer_pages: bool = False) -> int:
+    def touch_prefix(self, conn, page_hashes: Sequence[str], all_layer_pages: bool = False,
+                     source_tp: Optional[int] = None) -> int:
         """Tell an evicting store (``--evict``) that these pages were just used: every layer's
         K and V block of every page becomes most-recently-used.  Needed by clients that read
         through the device index, whose reads the server never sees.  Returns the number of
-        blocks refreshed.  ``all_layer_pages``: the pages were written with ``write_pages``."""
+        blocks refreshed.  ``all_layer_pages``: the pages were written with ``write_pages``;
+        ``source_tp`` (with it): at that TP degree, and every source rank's key is touched."""
+        if self._cross_tp(source_tp):
+            if not all_layer_pages:
+                raise ValueError("source_tp needs all_layer_pages")
+            keys = [k for ks in self.source_page_keys(page_hashes, source_tp) for k in ks]
+            return conn.touch(keys) if keys else 0
         if all_layer_pages:
             keys = self.page_keys(page_hashes)
             return conn.touch(keys) if keys else 0

@@ -113,7 +113,8 @@ def kv_gather(descs: torch.Tensor, part_base: Sequence[int], part_bytes: int, wr
               first_part: int = 0, max_ctas: int = 0, status: Optional[torch.Tensor] = None,
               align_or: int = 0, stage_bytes: int = 0, ring_bytes: int = 0,
               publish: Optional["PublishArgs"] = None, layer: Optional[LayerState] = None,
-              claim: bool = False, release: Optional[GroupRelease] = None) -> None:
+              claim: bool = False, release: Optional[GroupRelease] = None,
+              rows: Optional[Sequence[int]] = None) -> None:
     """Gathered blocks (csrc/kernels/kernels.h ``GatherLaunch``): block i is len(part_base)
     parts of ``part_bytes``, part s at ``part_base[s] + local offset``.  ``descs`` is (n, 2)
     int64: write {local byte offset, block address}, read {block address or 0 = miss, local
@@ -122,7 +123,10 @@ def kv_gather(descs: torch.Tensor, part_base: Sequence[int], part_bytes: int, wr
     ``publish`` commits its blocks in the index; with ``layer`` too it is one launch of a
     layered write (``claim``: its first), which publishes a block once all of
     ``layer.nparts`` parts have landed.  A read with ``release`` is a layered read: the ld/st
-    kernel walks the parts group by group and releases each group's flag."""
+    kernel walks the parts group by group and releases each group's flag.  A read with
+    ``rows`` = (rows, row_bytes, src_pitch, src_col, dst_pitch), bytes, is row-sliced
+    (kv_scatter_rows): row r of stored part s at ``r * src_pitch + src_col`` -> part s's
+    destination + ``r * dst_pitch``; ``part_bytes`` must be ``rows * src_pitch``."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
     bases = [int(b) for b in part_base]
     for b in bases:
@@ -132,7 +136,8 @@ def kv_gather(descs: torch.Tensor, part_base: Sequence[int], part_bytes: int, wr
         K.kv_gather(descs.data_ptr(), descs.shape[0], bases, part_bytes, first_part, write,
                     max_ctas, _stream(descs.device), *pub,
                     status.data_ptr() if status is not None else 0, align_or, stage_bytes,
-                    ring_bytes, *lay, *_release_args(release))
+                    ring_bytes, *lay, *_release_args(release),
+                    [int(r) for r in rows] if rows is not None else [])
 
 
 def kv_copy_multicast(descs: torch.Tensor, nbytes: int, dst_deltas: Sequence[int],
