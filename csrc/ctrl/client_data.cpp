@@ -801,11 +801,23 @@ int Connection::w_rdma(const uint64_t* offsets, size_t noffsets, uint64_t scale,
                        stream, 0, res);
 }
 
+// Every fp8 kernel moves bf16 in 16-byte vectors: pages that are not 16-byte aligned are
+// refused before anything is enqueued.
+static bool fp8_pages_aligned(uint64_t base_ptr, const uint64_t* offs, size_t n, uint64_t scale) {
+    uint64_t align_or = base_ptr;
+    for (size_t i = 0; i < n; ++i) align_or |= offs[i] * scale;
+    return (align_or & 15) == 0;
+}
+
 int Connection::w_rdma_fp8(const uint64_t* offsets, size_t noffsets, uint64_t scale, int elems,
                            const RemoteBlock* blocks, size_t nblocks, uint64_t base_ptr,
                            int device, uint64_t stream) {
     if (noffsets != nblocks || elems <= 0 || elems % 128) {
         fail("w_rdma_fp8: page size must be a positive multiple of 128 elements");
+        return -1;
+    }
+    if (!fp8_pages_aligned(base_ptr, offsets, noffsets, scale)) {
+        fail("w_rdma_fp8: pages must start 16-byte aligned");
         return -1;
     }
     return move_blocks(true, offsets, scale, blocks, nblocks,
@@ -818,6 +830,12 @@ int Connection::r_rdma_fp8(const std::vector<KeyOffset>& blocks, int elems, uint
     if (blocks.empty()) return 0;
     if (elems <= 0 || elems % 128 || device < 0) {
         fail("r_rdma_fp8: needs a CUDA tensor and pages of a multiple of 128 elements");
+        return -1;
+    }
+    std::vector<uint64_t> offs(blocks.size());
+    for (size_t i = 0; i < blocks.size(); ++i) offs[i] = blocks[i].offset;
+    if (!fp8_pages_aligned(base_ptr, offs.data(), offs.size(), 1)) {
+        fail("r_rdma_fp8: pages must start 16-byte aligned");
         return -1;
     }
     return read_blocks(kOpReadLookup, blocks, int(kernels::fp8_block_bytes(uint32_t(elems), 128)),

@@ -17,7 +17,7 @@
 // load), reduces |x| max with shuffles inside the half, and emits 8 bytes per lane (one
 // coalesced 128-byte store per row).  Eight rows are in flight per warp to cover the
 // NVLink / HBM latency.
-// There is no direct bf16<->e4m3 cvt on sm_90a: quantise via f32, dequantise via f16x2.
+// The row maths (amax, scale, cvt, dequant8) are fp8_row.cuh's, shared with kv_fp8_pipe.cu.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -25,6 +25,7 @@
 
 #include "common.cuh"
 #include "fp8_pages.cuh"
+#include "fp8_row.cuh"
 #include "kernels.h"
 #include "launch_plan.h"
 #include "publish.cuh"
@@ -33,10 +34,11 @@ namespace istore::kernels {
 
 namespace {
 
+using namespace fp8row;
+
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 constexpr uint32_t kRow = 128;                 // elements sharing a scale
-constexpr float kE4m3Max = 448.f;
 
 __device__ __forceinline__ uint2 ld_u2(const void* p) {
     uint2 r;
@@ -48,24 +50,6 @@ __device__ __forceinline__ uint32_t ld_u1(const void* p) {
     asm volatile("ld.global.L1::no_allocate.u32 %0, [%1];" : "=r"(r) : "l"(p));
     return r;
 }
-__device__ __forceinline__ uint16_t cvt_e4m3x2(float hi, float lo) {  // F2FP.SATFINITE.E4M3.F32
-    uint16_t r;
-    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
-    return r;
-}
-__device__ __forceinline__ uint32_t cvt_f16x2_e4m3x2(uint16_t v) {  // F2FP.F16.E4M3.UNPACK_B
-    uint32_t r;
-    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(r) : "h"(v));
-    return r;
-}
-__device__ __forceinline__ float2 bf16x2_to_f2(uint32_t v) {
-    return make_float2(__uint_as_float(v << 16), __uint_as_float(v & 0xffff0000u));
-}
-__device__ __forceinline__ uint32_t f2_to_bf16x2(float lo, float hi) {
-    const __nv_bfloat162 b = __floats2bfloat162_rn(lo, hi);
-    return *reinterpret_cast<const uint32_t*>(&b);
-}
-
 // A half-warp owns one 128-element row per step (lane l of the half: elements 8l..8l+7, one
 // 16-byte load), so a warp instruction covers two rows; kRowPairs such steps are in flight.
 constexpr int kRowPairs = 4;  // 8 rows = 2 KB of bf16 in flight per warp
@@ -115,49 +99,26 @@ __device__ __forceinline__ void write_fp8(const CopyDesc* __restrict__ descs, ui
                 const uint32_t r = r0 + 2 * u + half;
                 const bool live = r < rows;
                 float2 f[4];
-                f[0] = bf16x2_to_f2(v[u].x);
-                f[1] = bf16x2_to_f2(v[u].y);
-                f[2] = bf16x2_to_f2(v[u].z);
-                f[3] = bf16x2_to_f2(v[u].w);
-                float amax = 0.f;
-                if (live) {
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) amax = fmaxf(amax, fmaxf(fabsf(f[j].x), fabsf(f[j].y)));
-                }
+                float amax = load8(v[u], f);
+                if (!live) amax = 0.f;
 #pragma unroll
                 for (int o = 8; o > 0; o >>= 1)  // reduce within the half-warp that owns the row
                     amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+                if (__any_sync(0xffffffffu, has_inf(amax))) {  // rare: a row holds +-inf
+                    amax = has_inf(amax) ? drop_inf8(f) : amax;
+#pragma unroll
+                    for (int o = 8; o > 0; o >>= 1)
+                        amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+                }
                 if (!live) continue;
-                const float scale = amax > 0.f ? amax * (1.f / kE4m3Max) : 1.f;
-                const float inv = 1.f / scale;
-                uint2 out;
-                out.x = uint32_t(cvt_e4m3x2(f[0].y * inv, f[0].x * inv)) |
-                        (uint32_t(cvt_e4m3x2(f[1].y * inv, f[1].x * inv)) << 16);
-                out.y = uint32_t(cvt_e4m3x2(f[2].y * inv, f[2].x * inv)) |
-                        (uint32_t(cvt_e4m3x2(f[3].y * inv, f[3].x * inv)) << 16);
-                *reinterpret_cast<uint2*>(q + size_t(row0 + r) * kRow + hl * 8) = out;
+                const float scale = row_scale(amax);
+                *reinterpret_cast<uint2*>(q + size_t(row0 + r) * kRow + hl * 8) =
+                    quant8(f, 1.f / scale);
                 if (hl == 0) scales[row0 + r] = scale;
             }
         }
     }
     if (pub.recs) ctrl_barrier_arrive(kThreads + 32);
-}
-
-// Lane hl of the half-warp that owns a row: its 8 e4m3 values (v) times the row's scale, as
-// 8 bf16 (one 16-byte store).  Dequantisation goes through f16x2.
-__device__ __forceinline__ uint4 dequant8(uint2 v, float sc) {
-    const uint32_t w[2] = {v.x, v.y};
-    uint32_t o[4];
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-        const uint32_t h01 = cvt_f16x2_e4m3x2(uint16_t(w[j] & 0xffffu));
-        const uint32_t h23 = cvt_f16x2_e4m3x2(uint16_t(w[j] >> 16));
-        const float2 f01 = __half22float2(*reinterpret_cast<const __half2*>(&h01));
-        const float2 f23 = __half22float2(*reinterpret_cast<const __half2*>(&h23));
-        o[2 * j] = f2_to_bf16x2(f01.x * sc, f01.y * sc);
-        o[2 * j + 1] = f2_to_bf16x2(f23.x * sc, f23.y * sc);
-    }
-    return make_uint4(o[0], o[1], o[2], o[3]);
 }
 
 __global__ void __launch_bounds__(kThreads + 32)
@@ -333,6 +294,7 @@ cudaError_t launch_kv_write_fp8(const Fp8Launch& a, cudaStream_t stream) {
     if (a.n == 0 || a.elems == 0) return cudaSuccess;
     if (a.group != kRow || a.elems % kRow != 0) return cudaErrorInvalidValue;
     const LaunchPlan p = plan_fp8(a, sm_count());
+    if (!p.valid) return cudaErrorInvalidValue;  // pages that are not 16-byte aligned
     if (p.kernel != Kernel::kLdStFp8) return launch_kv_fp8_pipe(a, true, stream);
     kv_write_fp8_kernel<<<p.ctas, kThreads + 32, 0, stream>>>(a.descs, a.n, a.elems, p.chunk, p.cpb,
                                                              publish_of(a, true));
@@ -343,6 +305,7 @@ cudaError_t launch_kv_read_fp8(const Fp8Launch& a, cudaStream_t stream) {
     if (a.n == 0 || a.elems == 0) return cudaSuccess;
     if (a.group != kRow || a.elems % kRow != 0) return cudaErrorInvalidValue;
     const LaunchPlan p = plan_fp8(a, sm_count());
+    if (!p.valid) return cudaErrorInvalidValue;  // pages that are not 16-byte aligned
     if (p.kernel != Kernel::kLdStFp8) return launch_kv_fp8_pipe(a, false, stream);
     kv_read_fp8_kernel<<<p.ctas, kThreads, 0, stream>>>(a.descs, a.n, a.elems, p.chunk, p.cpb,
                                                         a.status);

@@ -18,8 +18,9 @@
 // cast kernel - the reference moves opaque bytes only (infinistore/lib.py:377-379).
 //
 // Pool block layout (unchanged): [elems x e4m3][elems/128 x fp32 scale].
-// Needs elems % 512 == 0 (scale vectors of a tile are 16-byte multiples) and 16-byte aligned
-// pages; launch_kv_{write,read}_fp8 fall back to kv_fp8.cu otherwise.
+// Needs elems % 512 == 0 (scale vectors of a tile are 16-byte multiples); launch_kv_{write,
+// read}_fp8 fall back to kv_fp8.cu otherwise.  Pages that are not 16-byte aligned are refused
+// by plan_fp8 for both flavours.  The row maths are fp8_row.cuh's, shared with kv_fp8.cu.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -28,6 +29,7 @@
 
 #include "common.cuh"
 #include "fp8_pages.cuh"
+#include "fp8_row.cuh"
 #include "kernels.h"
 #include "launch_plan.h"
 #include "publish.cuh"
@@ -38,6 +40,7 @@ namespace istore::kernels {
 namespace {
 
 using namespace dev;
+using namespace fp8row;
 
 constexpr uint32_t kRow = 128;                  // elements sharing a scale
 constexpr uint32_t kTileRows = 64;              // rows per tile
@@ -47,25 +50,6 @@ constexpr uint32_t kTileBf16 = kTileElems * 2;  // 16 KB
 constexpr uint32_t kTileQ = kTileElems;         // 8 KB
 constexpr uint32_t kTileScale = kTileRows * 4;  // 256 B
 constexpr int kInStages = 4, kOutStages = 3, kLag = 2;
-constexpr float kE4m3Max = 448.f;
-
-__device__ __forceinline__ uint16_t cvt_e4m3x2(float hi, float lo) {
-    uint16_t r;
-    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
-    return r;
-}
-__device__ __forceinline__ uint32_t cvt_f16x2_e4m3x2(uint16_t v) {
-    uint32_t r;
-    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(r) : "h"(v));
-    return r;
-}
-__device__ __forceinline__ float2 bf16x2_to_f2(uint32_t v) {
-    return make_float2(__uint_as_float(v << 16), __uint_as_float(v & 0xffff0000u));
-}
-__device__ __forceinline__ uint32_t f2_to_bf16x2(float lo, float hi) {
-    const __nv_bfloat162 b = __floats2bfloat162_rn(lo, hi);
-    return *reinterpret_cast<const uint32_t*>(&b);
-}
 
 struct Smem {
     // [kInStages][in tile] then [kOutStages][out tile]; sizes depend on the direction
@@ -215,41 +199,28 @@ __device__ __forceinline__ void fp8_pipe(const CopyDesc* __restrict__ descs, con
             for (uint32_t r = cw * 2 + half; r < rows; r += NCW * 2) {
                 if constexpr (WRITE) {
                     const uint4 v = *reinterpret_cast<const uint4*>(in + (size_t(r) * kRow + hl * 8) * 2);
-                    float2 f[4] = {bf16x2_to_f2(v.x), bf16x2_to_f2(v.y), bf16x2_to_f2(v.z),
-                                   bf16x2_to_f2(v.w)};
-                    float amax = 0.f;
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) amax = fmaxf(amax, fmaxf(fabsf(f[j].x), fabsf(f[j].y)));
+                    float2 f[4];
+                    float amax = load8(v, f);
                     // the 16 lanes of this half own the row; rows r and r^1 of the two halves
                     // are both live or the loop bound differs only in the last step
                     const uint32_t mask = half ? 0xffff0000u : 0x0000ffffu;
 #pragma unroll
                     for (int o = 8; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(mask, amax, o));
-                    const float scale = amax > 0.f ? amax * (1.f / kE4m3Max) : 1.f;
-                    const float inv = 1.f / scale;
-                    uint2 o2;
-                    o2.x = uint32_t(cvt_e4m3x2(f[0].y * inv, f[0].x * inv)) |
-                           (uint32_t(cvt_e4m3x2(f[1].y * inv, f[1].x * inv)) << 16);
-                    o2.y = uint32_t(cvt_e4m3x2(f[2].y * inv, f[2].x * inv)) |
-                           (uint32_t(cvt_e4m3x2(f[3].y * inv, f[3].x * inv)) << 16);
-                    *reinterpret_cast<uint2*>(out + size_t(r) * kRow + hl * 8) = o2;
+                    if (has_inf(amax)) {  // rare: the row holds +-inf (uniform in the half)
+                        amax = drop_inf8(f);
+#pragma unroll
+                        for (int o = 8; o > 0; o >>= 1)
+                            amax = fmaxf(amax, __shfl_xor_sync(mask, amax, o));
+                    }
+                    const float scale = row_scale(amax);
+                    *reinterpret_cast<uint2*>(out + size_t(r) * kRow + hl * 8) =
+                        quant8(f, 1.f / scale);
                     if (hl == 0) *reinterpret_cast<float*>(out + kTileQ + r * 4) = scale;
                 } else {
                     const uint2 v = *reinterpret_cast<const uint2*>(in + size_t(r) * kRow + hl * 8);
                     const float sc = *reinterpret_cast<const float*>(in + kTileQ + r * 4);
-                    const uint32_t w[2] = {v.x, v.y};
-                    uint32_t o[4];
-#pragma unroll
-                    for (int j = 0; j < 2; ++j) {
-                        const uint32_t h01 = cvt_f16x2_e4m3x2(uint16_t(w[j] & 0xffffu));
-                        const uint32_t h23 = cvt_f16x2_e4m3x2(uint16_t(w[j] >> 16));
-                        const float2 f01 = __half22float2(*reinterpret_cast<const __half2*>(&h01));
-                        const float2 f23 = __half22float2(*reinterpret_cast<const __half2*>(&h23));
-                        o[2 * j] = f2_to_bf16x2(f01.x * sc, f01.y * sc);
-                        o[2 * j + 1] = f2_to_bf16x2(f23.x * sc, f23.y * sc);
-                    }
                     *reinterpret_cast<uint4*>(out + (size_t(r) * kRow + hl * 8) * 2) =
-                        make_uint4(o[0], o[1], o[2], o[3]);
+                        dequant8(v, sc);
                 }
             }
         }

@@ -331,8 +331,10 @@ inline LaunchPlan plan_fp8_pipe(const Fp8Launch& a, int sms) {
 
 // The pipeline unless the ld/st kernels are asked for or the pages do not suit it.  The ld/st
 // kernels: whole pages per CTA when there are enough of them, six CTAs per SM, a caller's cap
-// not bounded.
+// not bounded.  Pages that are not 16-byte aligned are refused: every fp8 kernel moves bf16
+// in 16-byte vectors (the ld/st kernels' loads and stores, the pipeline's bulk copies).
 inline LaunchPlan plan_fp8(const Fp8Launch& a, int sms) {
+    if (!a.aligned16) return invalid_plan();
     if (a.variant != kFp8LdSt && fp8_pipe_supported(a)) return plan_fp8_pipe(a, sms);
     LaunchPlan p;
     p.kernel = Kernel::kLdStFp8;

@@ -1247,9 +1247,10 @@ PYBIND11_MODULE(_infinistore, m) {
     auto fp8 = [](bool write) {
         return [write](uint64_t descs, uint32_t n, uint32_t elems, uint32_t group, int max_ctas,
                        uint64_t stream, uint64_t recs, uint64_t table, uint64_t table_mask,
-                       uint64_t done, uint64_t status, int variant) {
+                       uint64_t done, uint64_t status, int variant, uint64_t align_or) {
             kernels::Fp8Launch L;
             L.variant = variant;
+            L.aligned16 = (align_or & 15) == 0;
             L.descs = as_ptr<const kernels::CopyDesc>(descs);
             L.n = n;
             L.elems = elems;
@@ -1269,11 +1270,13 @@ PYBIND11_MODULE(_infinistore, m) {
     k.def("kv_write_fp8", fp8(true), py::arg("descs"), py::arg("n"), py::arg("elems"),
           py::arg("group") = 128, py::arg("max_ctas") = 0, py::arg("stream") = 0,
           py::arg("recs") = 0, py::arg("table") = 0, py::arg("table_mask") = 0,
-          py::arg("done") = 0, py::arg("status") = 0, py::arg("variant") = 0);
+          py::arg("done") = 0, py::arg("status") = 0, py::arg("variant") = 0,
+          py::arg("align_or") = 0);
     k.def("kv_read_fp8", fp8(false), py::arg("descs"), py::arg("n"), py::arg("elems"),
           py::arg("group") = 128, py::arg("max_ctas") = 0, py::arg("stream") = 0,
           py::arg("recs") = 0, py::arg("table") = 0, py::arg("table_mask") = 0,
-          py::arg("done") = 0, py::arg("status") = 0, py::arg("variant") = 0);
+          py::arg("done") = 0, py::arg("status") = 0, py::arg("variant") = 0,
+          py::arg("align_or") = 0);
     k.def("fp8_block_bytes", &kernels::fp8_block_bytes);
     k.def("fp8_gather_bytes", &kernels::fp8_gather_bytes, py::arg("nparts"), py::arg("elems"),
           "bytes of nparts fp8 pages of elems elements end to end (a gathered fp8 block)");

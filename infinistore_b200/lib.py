@@ -377,6 +377,20 @@ class PartRows:
         return out
 
 
+def _raise_if_fp8_pages_unaligned(cache: torch.Tensor, offsets) -> None:
+    """After a refused fp8 call: ValueError when a page (``offsets`` in elements of ``cache``)
+    does not start 16-byte aligned.  The fp8 kernels move bf16 in 16-byte vectors, so the
+    connection refuses such pages before it enqueues anything; checking here only once the
+    call has failed keeps the per-call cost off the hot path."""
+    align = cache.data_ptr()
+    offs = np.asarray(offsets, dtype=np.int64).reshape(-1)
+    if len(offs):
+        align |= int(np.bitwise_or.reduce(offs * cache.element_size()))
+    if align & 15:
+        raise ValueError("fp8 pages must start 16-byte aligned: the tensor's address and every "
+                         "offset must be multiples of 8 bf16 elements")
+
+
 def _device_of(cache: torch.Tensor) -> int:
     return cache.device.index if cache.device.type == "cuda" else -1
 
@@ -942,6 +956,7 @@ class InfinityConnection:
         ret = self.conn.w_rdma_fp8(offsets, page_size, remote_blocks, cache.data_ptr(),
                                    _device_of(cache), _stream_of(cache, stream), 2)
         if ret < 0:
+            _raise_if_fp8_pages_unaligned(cache, offsets)
             raise Exception(f"Failed to write to infinistore, ret = {ret}")
         return 0
 
@@ -955,6 +970,8 @@ class InfinityConnection:
         ret = self.conn.r_rdma_fp8(blocks, page_size, cache.data_ptr(), _device_of(cache),
                                    _stream_of(cache, stream), 2)
         if ret < 0:
+            _raise_if_fp8_pages_unaligned(cache, blocks[1] if isinstance(blocks, tuple)
+                                          else [b[1] for b in blocks])
             raise Exception(f"Failed to read to infinistore, ret = {ret}")
 
     # the north-star API list names the read entry points rdma_read_cache*: same functions

@@ -297,25 +297,32 @@ FP8_VARIANTS = {"auto": 0, "ldst": 1, "pipe4": 2}
 
 
 def kv_write_fp8(descs: torch.Tensor, elems: int, max_ctas: int = 0,
-                 publish: Optional[PublishArgs] = None, variant: str = "auto") -> None:
+                 publish: Optional[PublishArgs] = None, variant: str = "auto",
+                 align_or: int = 0) -> None:
     """bf16 pages (desc.src) -> e4m3 payload + per-128 scales (desc.dst).  "auto": the
-    TMA-pipelined kernel (kv_fp8_pipe.cu) when elems % 512 == 0, else / "ldst": kv_fp8.cu."""
+    TMA-pipelined kernel (kv_fp8_pipe.cu) when elems % 512 == 0, else / "ldst": kv_fp8.cu;
+    "pipe4": the pipeline with 4 compute warps.  ``align_or``: the OR of every page address;
+    pages that are not 16-byte aligned are refused (RuntimeError), never launched."""
     with torch.cuda.device(descs.device):
         K.kv_write_fp8(descs.data_ptr(), descs.shape[0], elems, 128, max_ctas,
                        _stream(descs.device),
                        publish.recs.data_ptr() if publish else 0,
                        publish.table.data_ptr() if publish else 0,
                        publish.mask if publish else 0,
-                       publish.done.data_ptr() if publish else 0, 0, FP8_VARIANTS[variant])
+                       publish.done.data_ptr() if publish else 0, 0, FP8_VARIANTS[variant],
+                       align_or)
 
 
 def kv_read_fp8(descs: torch.Tensor, elems: int, max_ctas: int = 0,
-                status: Optional[torch.Tensor] = None, variant: str = "auto") -> None:
-    """e4m3 payload + scales (desc.src) -> bf16 pages (desc.dst)."""
+                status: Optional[torch.Tensor] = None, variant: str = "auto",
+                align_or: int = 0) -> None:
+    """e4m3 payload + scales (desc.src) -> bf16 pages (desc.dst); ``variant`` and
+    ``align_or`` as for ``kv_write_fp8``."""
     with torch.cuda.device(descs.device):
         K.kv_read_fp8(descs.data_ptr(), descs.shape[0], elems, 128, max_ctas,
                       _stream(descs.device), 0, 0, 0, 0,
-                      status.data_ptr() if status is not None else 0, FP8_VARIANTS[variant])
+                      status.data_ptr() if status is not None else 0, FP8_VARIANTS[variant],
+                      align_or)
 
 
 def fp8_gather_bytes(nparts: int, elems: int) -> int:
@@ -349,12 +356,20 @@ def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, wri
 
 
 def fp8_reference(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
-    """Plain PyTorch fp32 reference of the fused quantiser: per-128 amax scale, e4m3
-    round-to-nearest with saturation.  Returns (dequantised fp32, scales, payload)."""
+    """Plain PyTorch fp32 reference of the fused quantiser, the row contract of
+    docs/kernels.md: per-128 scale from the |max| of the finite elements, floored at 2^-126,
+    e4m3 round-to-nearest-even with saturation, NaN for a non-finite element.  Returns
+    (dequantised fp32, scales, payload); the dequantised values are e4m3 * scale rounded to
+    fp32, so ``.to(torch.bfloat16)`` of them is what the read kernels store."""
     xf = x.float().reshape(-1, 128)
-    amax = xf.abs().amax(dim=1, keepdim=True)
-    scale = torch.where(amax > 0, amax * (1.0 / 448.0), torch.ones_like(amax))
-    q = (xf * (1.0 / scale)).clamp(-448, 448).to(torch.float8_e4m3fn)
+    finite = torch.isfinite(xf)
+    amax = torch.where(finite, xf.abs(), torch.zeros_like(xf)).amax(dim=1, keepdim=True)
+    inv448 = torch.tensor(1.0 / 448.0, dtype=torch.float32, device=xf.device)
+    floor = torch.tensor(2.0 ** -126, dtype=torch.float32, device=xf.device)
+    scale = torch.where(amax > 0, torch.maximum(amax * inv448, floor), torch.ones_like(amax))
+    inv = torch.ones_like(scale) / scale
+    scaled = torch.where(finite, xf * inv, torch.full_like(xf, float("nan")))
+    q = scaled.clamp(-448, 448).to(torch.float8_e4m3fn)
     return (q.float() * scale).reshape(x.shape), scale.reshape(-1), q.reshape(-1)
 
 
