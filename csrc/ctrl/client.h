@@ -177,10 +177,9 @@ class Connection {
                    uint64_t stream);
     int r_rdma_fp8(const std::vector<KeyOffset>& blocks, int elems, uint64_t base_ptr, int device,
                    uint64_t stream);
-    // Layered read (read_scatter_layered): one call whose last page-mover launch releases the
-    // parts group by group, `group_parts` parts per group, each by storing `seq` to its flag
-    // word.  wait(g, stream) makes later work on `stream` wait on the GPU until group g has
-    // landed (cuStreamWaitValue32), with no host synchronisation.
+    // A layered read's groups (r_rdma_scatter with GatherSpec::reader).  wait_layered(r, g,
+    // stream) makes later work on `stream` wait on the GPU until group g has landed
+    // (cuStreamWaitValue32), with no host synchronisation.
     struct ScatterReader {
         uint32_t groups = 0;
         uint32_t group_parts = 0;
@@ -190,16 +189,27 @@ class Connection {
         bool failed = false;              // refused or failed: every wait is refused
         uint64_t session = 0;             // the connection session whose device flags it uses
     };
-    // Gathered blocks (kernels::GatherLaunch): a block is `nparts` parts of part_bytes, part s
-    // at part_base[s] + the block's local byte offset (one page of every layer under one key).
+    // Gathered blocks (kernels::GatherLaunch): a block is `nparts` parts, part s at
+    // part_base[s] + the block's local byte offset (one page of every layer under one key).
     struct GatherSpec {
         const uint64_t* part_base = nullptr;  // absolute addresses, all on `device` (or host)
         uint32_t nparts = 0;
-        uint32_t part_bytes = 0;  // pool bytes of a part (fp8: fp8_gather_bytes(1, elems))
+        uint32_t part_bytes = 0;  // bytes of a raw part (not read when fp8_elems > 0)
+        // > 0: every part is a bf16 page of fp8_elems elements (a multiple of 512) in the
+        // caller's CUDA tensors and an fp8 page in the pool; part bases and offsets 16-byte
+        // aligned
+        uint32_t fp8_elems = 0;
         uint32_t first_part = 0;  // stored part first_part + s is part s (one-shot writes: 0)
-        ScatterReader* reader = nullptr;  // reads: a layered read (read_scatter_layered)
+        // reads: a layered read, whose parts are released to `reader`'s waits in groups of
+        // group_parts (which must divide nparts)
+        ScatterReader* reader = nullptr;
+        uint32_t group_parts = 0;
         // reads: row-sliced parts (kernels::GatherLaunch::rows, bytes); rows == 0: whole parts
         uint32_t rows = 0, row_bytes = 0, src_pitch = 0, src_col = 0, dst_pitch = 0;
+        // pool bytes of a part: part_bytes, or kernels::fp8_gather_bytes(1, fp8_elems)
+        uint64_t pool_part_bytes() const;
+        // bytes a stored block must hold to serve a read: parts 0 .. first_part + nparts - 1
+        uint64_t need_bytes() const { return (uint64_t(first_part) + nparts) * pool_part_bytes(); }
     };
     // Layered gathered write: a fixed set of allocated gathered blocks whose parts are stored
     // over several calls (write_layered), each a contiguous range of parts of every block -
@@ -217,7 +227,7 @@ class Connection {
         uint32_t calls = 0;               // calls that launched (the first one claims)
         int device = -2;                  // fixed by the first call (-1: host tensors)
         uint64_t scale = 0;               // bytes per offset unit, fixed by the first call
-        int elems = -1;                   // fp8 elements per part (0: raw bytes), first call
+        uint32_t fp8_elems = 0;           // fp8 elements per part (0: raw bytes), first call
         uint32_t part_bytes = 0;          // pool bytes of a part, first call
         bool failed = false;
         void* event = nullptr;            // cudaEvent_t recorded after the last launch
@@ -230,39 +240,23 @@ class Connection {
     std::shared_ptr<GatherWriter> gather_writer(const RemoteBlock* blocks, const uint64_t* offsets,
                                                 size_t n, uint32_t nparts);
     // Stores parts g.first_part .. g.first_part + g.nparts - 1 of every block of `w`; offsets
-    // are scaled by `scale`.  elems > 0: fp8 parts of `elems` bf16 elements (g.part_bytes is
-    // not read), as w_rdma_gather_fp8.  Refuses part ranges written before, a device, scale or
-    // elems other than the first call's, a complete or failed writer, and a writer made before
-    // the connection was last closed (its blocks and index ways were released).  A refused
-    // call leaves the writer as it was.
-    int write_layered(GatherWriter& w, const GatherSpec& g, int elems, uint64_t scale, int device,
+    // are scaled by `scale`.  Refuses part ranges written before, a device, scale, fp8_elems
+    // or part size other than the first call's, a complete or failed writer, and a writer made
+    // before the connection was last closed (its blocks and index ways were released).  A
+    // refused call leaves the writer as it was.
+    int write_layered(GatherWriter& w, const GatherSpec& g, uint64_t scale, int device,
                       uint64_t stream);
-    // offsets in bytes; blocks allocated with nparts * part_bytes bytes (trusted)
+    // offsets in bytes; blocks allocated with nparts * g.pool_part_bytes() bytes (trusted)
     int w_rdma_gather(const GatherSpec& g, const uint64_t* offsets, size_t noffsets,
                       const RemoteBlock* blocks, size_t nblocks, int device, uint64_t stream);
-    // a stored block must hold (first_part + nparts) * part_bytes bytes, else it is a miss.
-    // Row-sliced (g.rows): rows >= 1, src_col + row_bytes <= src_pitch and part_bytes ==
-    // rows * src_pitch, else refused before anything is enqueued.
+    // A stored block must hold g.need_bytes() bytes, else it is a miss.  Row-sliced (g.rows):
+    // bf16 only, rows >= 1, src_col + row_bytes <= src_pitch and part_bytes == rows *
+    // src_pitch.  With g.reader, a layered read: one call whose last page-mover launch
+    // releases the parts group by group, each by storing `seq` to its flag word, and each key
+    // is resolved once; CUDA tensors of an HBM pool only, not on a doorbell connection, and on
+    // failure the reader is failed.  Every refusal comes before anything is enqueued.
     int r_rdma_scatter(const GatherSpec& g, const std::vector<KeyOffset>& blocks, int device,
                        uint64_t stream);
-    // Gathered fp8 blocks: every part is a bf16 page of `elems` elements (a multiple of 512) in
-    // the caller's CUDA tensors and an fp8 page in the pool, part s at byte
-    // kernels::fp8_gather_bytes(s, elems) of the block (g.part_bytes is not read).  Blocks are
-    // allocated with fp8_gather_bytes(nparts, elems) bytes; a stored block must hold
-    // fp8_gather_bytes(first_part + nparts, elems) bytes, else it is a miss.  Part bases and
-    // offsets must be 16-byte aligned.
-    int w_rdma_gather_fp8(const GatherSpec& g, int elems, const uint64_t* offsets,
-                          size_t noffsets, const RemoteBlock* blocks, size_t nblocks, int device,
-                          uint64_t stream);
-    int r_rdma_scatter_fp8(const GatherSpec& g, int elems, const std::vector<KeyOffset>& blocks,
-                           int device, uint64_t stream);
-    // Layered read: r_rdma_scatter (elems == 0) or r_rdma_scatter_fp8 (elems > 0) in one call,
-    // whose parts are released to `r`'s waits in groups of group_parts (which must divide
-    // g.nparts).  Each key is resolved once.  CUDA tensors of an HBM pool only; not on a
-    // doorbell connection.  On failure r.failed is set and every wait is refused.
-    int read_scatter_layered(const GatherSpec& g, int elems, uint32_t group_parts,
-                             const std::vector<KeyOffset>& blocks, int device, uint64_t stream,
-                             ScatterReader& r);
     // Later work on `stream` waits on the GPU until group `group` of `r` has landed.  0; -1
     // (and *err) when refused: a failed reader, a group outside the read, or a reader made
     // before the connection was last closed (its flags were freed with the device context);
@@ -336,6 +330,9 @@ class Connection {
     kernels_IndexShards index_shards(DevCtx* ctx, bool* all_local);
     kernels::GatherLaunch gather_launch(const GatherSpec& g, uint32_t n, uint64_t align_or,
                                         uint32_t* status, int max_ctas);
+    // why a gathered call is refused (nullptr: it is not); `w`: a layered writer's call
+    const char* gather_refusal(const GatherSpec& g, const uint64_t* offs, size_t n, int device,
+                               bool write, const GatherWriter* w = nullptr) const;
     // a layered read's last launch: takes the reader's slot (0 on failure, else its seq)
     uint64_t arm_reader(DevCtx* ctx, const ScatterReader& r, kernels::GatherLaunch& G);
     int reader_launched(DevCtx* ctx, ScatterReader& r, uint64_t seq, void* stream);

@@ -279,7 +279,7 @@ kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n,
     G.n = n;
     G.part_base = g.part_base;
     G.nparts = g.nparts;
-    G.part_bytes = g.part_bytes;
+    G.part_bytes = uint32_t(g.pool_part_bytes());
     G.first_part = g.first_part;
     G.align_or = align_or;
     for (uint32_t s = 0; s < g.nparts; ++s) G.align_or |= g.part_base[s];
@@ -297,7 +297,7 @@ kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n,
 
 // Bytes one block of a gathered call moves: its parts, or their rows when row-sliced.
 static uint64_t gather_moved_bytes(const Connection::GatherSpec& g) {
-    return uint64_t(g.nparts) * (g.rows ? uint64_t(g.rows) * g.row_bytes : g.part_bytes);
+    return uint64_t(g.nparts) * (g.rows ? uint64_t(g.rows) * g.row_bytes : g.pool_part_bytes());
 }
 
 // Layered writers' state (GatherWriter::state), allocated stream-ordered from a memory pool of
@@ -334,8 +334,8 @@ static cudaError_t writer_state_alloc(void** p, size_t bytes, int device, cudaSt
 // Blocks per launch of a gathered call (staging.h: gather_max_blocks).  fp8 parts are counted
 // in bf16 bytes: the fp8 kernels cut a part into chunks of at least kFp8Chunk elements (16 KB
 // of bf16), or take it whole.
-static size_t gather_batch_cap(const Connection::GatherSpec& g, int fp8_elems) {
-    return gather_max_blocks(kMaxBatch, g.nparts, fp8_elems ? 2 * uint32_t(fp8_elems) : g.part_bytes);
+static size_t gather_batch_cap(const Connection::GatherSpec& g) {
+    return gather_max_blocks(kMaxBatch, g.nparts, g.fp8_elems ? 2 * g.fp8_elems : g.part_bytes);
 }
 
 // The blocks of blocks[base, ...) that the next launch stages (staging.h: key_batch) within
@@ -412,7 +412,7 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
                 if (!m || !m->host_ptr) return -1;
                 uint8_t* pool = m->host_ptr + addr_off(blocks[i].remote_addr);
                 if (gather) {  // one memcpy per part, or per row of a row-sliced read
-                    const size_t pb = gather->part_bytes;
+                    const size_t pb = gather->pool_part_bytes();
                     const Connection::GatherSpec& g = *gather;
                     for (uint32_t s = 0; s < gather->nparts; ++s) {
                         uint8_t* local =
@@ -502,7 +502,7 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
         }
     }
 
-    const size_t max_batch = gather ? gather_batch_cap(*gather, fp8_elems) : kMaxBatch;
+    const size_t max_batch = gather ? gather_batch_cap(*gather) : kMaxBatch;
     size_t i = 0;
     while (i < n) {
         const uint64_t t_build0 = now_ns();
@@ -761,35 +761,6 @@ int Connection::wait_layered(const ScatterReader& r, uint32_t group, uint64_t st
     return 0;
 }
 
-int Connection::read_scatter_layered(const GatherSpec& g, int elems, uint32_t group_parts,
-                                     const std::vector<KeyOffset>& blocks, int device,
-                                     uint64_t stream, ScatterReader& r) {
-    r = ScatterReader{};
-    r.device = device;
-    {
-        std::lock_guard<std::mutex> lk(mu_);
-        r.session = session_;
-    }
-    r.group_parts = group_parts;
-    r.groups = group_parts && g.nparts % group_parts == 0 ? g.nparts / group_parts : 0;
-    const char* bad = device < 0      ? "needs CUDA tensors"
-                      : !server_hbm_  ? "needs a pool in GPU memory"
-                      : cfg_.doorbell ? "is not available on a doorbell connection"
-                      : !r.groups     ? "needs group_parts that divides the part count"
-                                      : nullptr;
-    if (bad) {
-        r.failed = true;
-        fail(std::string("layered read ") + bad);
-        return -1;
-    }
-    GatherSpec l = g;
-    l.reader = &r;
-    const int rc = elems > 0 ? r_rdma_scatter_fp8(l, elems, blocks, device, stream)
-                             : r_rdma_scatter(l, blocks, device, stream);
-    if (rc != 0) r.failed = true;
-    return rc;
-}
-
 int Connection::w_rdma(const uint64_t* offsets, size_t noffsets, uint64_t scale, int block_size,
                        const RemoteBlock* blocks, size_t nblocks, uint64_t base_ptr, int device,
                        uint64_t stream, MoveResult* res) {
@@ -848,9 +819,13 @@ int Connection::r_rdma(const std::vector<KeyOffset>& blocks, int block_size, uin
     return read_blocks(kOpReadLookup, blocks, block_size, base_ptr, device, stream, 0, res, packed);
 }
 
+uint64_t Connection::GatherSpec::pool_part_bytes() const {
+    return fp8_elems ? kernels::fp8_gather_bytes(1, fp8_elems) : part_bytes;
+}
+
 // Bytes a stored block must hold to serve the read: every part asked for.
 static uint32_t need_bytes_of(int block_size, const Connection::GatherSpec* g) {
-    return g ? (g->first_part + g->nparts) * g->part_bytes : uint32_t(block_size);
+    return g ? uint32_t(g->need_bytes()) : uint32_t(block_size);
 }
 
 // A read through the device index when this connection can use it from `device`; otherwise
@@ -870,70 +845,83 @@ int Connection::read_blocks(char op, const std::vector<KeyOffset>& blocks, int b
                        stream, fp8_elems, res, gather);
 }
 
-static bool gather_spec_ok(const Connection::GatherSpec& g) {
-    return g.part_base && g.nparts >= 1 && g.nparts <= kernels::kGatherMaxParts && g.part_bytes &&
-           uint64_t(g.nparts) * g.part_bytes <= uint64_t(INT32_MAX);
+// Every check that a launch would fail, or that would let it run past a block, made before
+// anything is enqueued.  The parts a block holds: a one-shot write's nparts, a layered
+// writer's w->nparts, or for a read, the first_part + nparts that a stored block must hold.
+const char* Connection::gather_refusal(const GatherSpec& g, const uint64_t* offs, size_t n,
+                                       int device, bool write, const GatherWriter* w) const {
+    if (!g.part_base || g.nparts < 1 || g.nparts > kernels::kGatherMaxParts)
+        return "bad parts list: 1 to GATHER_MAX_PARTS parts";
+    if (g.fp8_elems ? g.fp8_elems % 512 || g.fp8_elems > uint32_t(INT32_MAX) : !g.part_bytes)
+        return "bad part size: raw parts of 1 byte or more, fp8 parts of a multiple of 512 "
+               "elements";
+    const uint64_t end = uint64_t(g.first_part) + g.nparts;
+    const uint64_t block_parts = w ? w->nparts : write ? g.nparts : end;
+    if (end > block_parts) return "the part range runs past the block";
+    if (block_parts > uint64_t(INT32_MAX) / g.pool_part_bytes())
+        return "bad parts list: a block holds at most 2^31 - 1 bytes";
+    if (g.rows && (write || g.fp8_elems || !g.row_bytes ||
+                   uint64_t(g.src_col) + g.row_bytes > g.src_pitch ||
+                   uint64_t(g.rows) * g.src_pitch != g.part_bytes))
+        return "bad row geometry (bf16 reads only, rows >= 1, src_col + row_bytes <= "
+               "src_pitch, part_bytes == rows * src_pitch)";
+    if (g.reader) {
+        if (!g.group_parts || g.nparts % g.group_parts)
+            return "a layered read needs group_parts that divides the part count";
+        if (device < 0) return "a layered read needs CUDA tensors";
+        if (!server_hbm_) return "a layered read needs a pool in GPU memory";
+        if (cfg_.doorbell) return "a layered read is not available on a doorbell connection";
+    }
+    if (g.fp8_elems) {  // the fp8 kernels move bf16 in 16-byte vectors
+        if (device < 0) return "fp8 parts need CUDA tensors";
+        uint64_t align_or = 0;
+        for (uint32_t s = 0; s < g.nparts; ++s) align_or |= g.part_base[s];
+        for (size_t i = 0; i < n; ++i) align_or |= offs[i];
+        if (align_or & 15) return "fp8 parts need 16-byte aligned part bases and offsets";
+    }
+    return nullptr;
 }
 
 int Connection::w_rdma_gather(const GatherSpec& g, const uint64_t* offsets, size_t noffsets,
                               const RemoteBlock* blocks, size_t nblocks, int device,
                               uint64_t stream) {
-    if (noffsets != nblocks || !gather_spec_ok(g)) {
-        fail("w_rdma_gather: bad parts list, or offsets and remote blocks differ in length");
+    const char* bad = noffsets != nblocks ? "offsets and remote blocks differ in length"
+                                          : gather_refusal(g, offsets, noffsets, device, true);
+    if (bad) {
+        fail(std::string("w_rdma_gather: ") + bad);
         return -1;
     }
-    GatherSpec w = g;
-    w.first_part = 0;
-    return move_blocks(true, offsets, 1, blocks, nblocks, int(g.nparts * g.part_bytes), 0, device,
-                       stream, 0, nullptr, &w);
+    return move_blocks(true, offsets, 1, blocks, nblocks, int(g.nparts * g.pool_part_bytes()), 0,
+                       device, stream, int(g.fp8_elems), nullptr, &g);
 }
 
 int Connection::r_rdma_scatter(const GatherSpec& g, const std::vector<KeyOffset>& blocks,
                                int device, uint64_t stream) {
-    if (blocks.empty()) return 0;
-    if (!gather_spec_ok(g) ||
-        uint64_t(g.first_part) + g.nparts > uint64_t(INT32_MAX) / g.part_bytes) {
-        fail("r_rdma_scatter: bad parts list");
-        return -1;
+    ScatterReader* r = g.reader;
+    if (r) {
+        *r = ScatterReader{};
+        r->device = device;
+        {
+            std::lock_guard<std::mutex> lk(mu_);
+            r->session = session_;
+        }
+        r->group_parts = g.group_parts;
+        r->groups = g.group_parts && g.nparts % g.group_parts == 0 ? g.nparts / g.group_parts : 0;
     }
-    if (g.rows && (!g.row_bytes || uint64_t(g.src_col) + g.row_bytes > g.src_pitch ||
-                   uint64_t(g.rows) * g.src_pitch != g.part_bytes)) {
-        fail("r_rdma_scatter: bad row geometry (rows >= 1, src_col + row_bytes <= src_pitch, "
-             "part_bytes == rows * src_pitch)");
-        return -1;
+    std::vector<uint64_t> offs;  // only the fp8 alignment check reads them
+    if (g.fp8_elems) {
+        offs.resize(blocks.size());
+        for (size_t i = 0; i < blocks.size(); ++i) offs[i] = blocks[i].offset;
     }
-    return read_blocks(kOpReadLookup, blocks, int(g.nparts * g.part_bytes), 0, device, stream, 0,
-                       nullptr, nullptr, &g);
-}
-
-// Gathered fp8 blocks: the checks a launch would fail, made before anything is enqueued.
-static bool gather_fp8_ok(const Connection::GatherSpec& g, int elems, const uint64_t* offs,
-                          size_t n, uint64_t first_part) {
-    if (elems <= 0 || elems % 512 || !g.part_base || g.nparts < 1 ||
-        g.nparts > kernels::kGatherMaxParts ||
-        kernels::fp8_gather_bytes(uint32_t(first_part + g.nparts), uint32_t(elems)) >
-            uint64_t(INT32_MAX))
-        return false;
-    uint64_t align_or = 0;
-    for (uint32_t s = 0; s < g.nparts; ++s) align_or |= g.part_base[s];
-    for (size_t i = 0; i < n; ++i) align_or |= offs[i];
-    return (align_or & 15) == 0;
-}
-
-int Connection::w_rdma_gather_fp8(const GatherSpec& g, int elems, const uint64_t* offsets,
-                                  size_t noffsets, const RemoteBlock* blocks, size_t nblocks,
-                                  int device, uint64_t stream) {
-    if (noffsets != nblocks || device < 0 || !gather_fp8_ok(g, elems, offsets, noffsets, 0)) {
-        fail("w_rdma_gather_fp8: needs CUDA tensors, parts of a multiple of 512 elements, "
-             "16-byte aligned part bases and offsets, and one offset per remote block");
-        return -1;
-    }
-    GatherSpec w = g;
-    w.part_bytes = uint32_t(kernels::fp8_gather_bytes(1, uint32_t(elems)));
-    w.first_part = 0;
-    return move_blocks(true, offsets, 1, blocks, nblocks,
-                       int(kernels::fp8_gather_bytes(g.nparts, uint32_t(elems))), 0, device,
-                       stream, elems, nullptr, &w);
+    const char* bad = gather_refusal(g, offs.data(), offs.size(), device, false);
+    if (bad) fail(std::string("r_rdma_scatter: ") + bad);
+    const int rc = bad              ? -1
+                   : blocks.empty() ? 0
+                                    : read_blocks(kOpReadLookup, blocks,
+                                                  int(g.nparts * g.pool_part_bytes()), 0, device,
+                                                  stream, int(g.fp8_elems), nullptr, nullptr, &g);
+    if (rc != 0 && r) r->failed = true;
+    return rc;
 }
 
 // Never waits for the device: an abandoned writer's state is freed on the per-thread stream
@@ -968,12 +956,10 @@ std::shared_ptr<Connection::GatherWriter> Connection::gather_writer(const Remote
     return w;
 }
 
-int Connection::write_layered(GatherWriter& w, const GatherSpec& g, int elems, uint64_t scale,
-                              int device, uint64_t stream) {
+int Connection::write_layered(GatherWriter& w, const GatherSpec& g, uint64_t scale, int device,
+                              uint64_t stream) {
     const uint64_t end = uint64_t(g.first_part) + g.nparts;
     const bool first = w.device == -2;
-    const uint32_t part_bytes =
-        elems > 0 ? uint32_t(kernels::fp8_gather_bytes(1, uint32_t(elems))) : g.part_bytes;
     uint64_t session;
     {
         std::lock_guard<std::mutex> lk(mu_);
@@ -984,16 +970,9 @@ int Connection::write_layered(GatherWriter& w, const GatherSpec& g, int elems, u
         bad = "the connection was closed after the writer was made";
     else if (w.failed || w.complete())
         bad = "the writer is complete or has failed";
-    else if (!g.part_base || g.nparts < 1 || g.nparts > kernels::kGatherMaxParts || end > w.nparts)
-        bad = "the part range runs past the block";
-    else if (!first && (device != w.device || scale != w.scale || elems != w.elems ||
-                        part_bytes != w.part_bytes))
+    else if (!first && (device != w.device || scale != w.scale || g.fp8_elems != w.fp8_elems ||
+                        g.pool_part_bytes() != w.part_bytes))
         bad = "device, element size or part size differ from the writer's first call";
-    else if (!part_bytes || uint64_t(w.nparts) * part_bytes > uint64_t(INT32_MAX) ||
-             (elems && (elems < 0 || elems % 512 || device < 0)))
-        bad = "bad part size";
-    for (uint64_t s = g.first_part; !bad && s < end; ++s)
-        if (w.written[s]) bad = "the part range overlaps parts written before";
     // every check before the writer changes: the first call's offsets are still in elements
     std::vector<uint64_t> scaled;
     if (!bad && first) {
@@ -1001,8 +980,9 @@ int Connection::write_layered(GatherWriter& w, const GatherSpec& g, int elems, u
         for (uint64_t& o : scaled) o *= scale;
     }
     const std::vector<uint64_t>& offs = first ? scaled : w.offsets;
-    if (!bad && elems && !gather_fp8_ok(g, elems, offs.data(), offs.size(), g.first_part))
-        bad = "fp8 parts need 16-byte aligned part bases and offsets";
+    if (!bad) bad = gather_refusal(g, offs.data(), offs.size(), device, true, &w);
+    for (uint64_t s = g.first_part; !bad && s < end; ++s)
+        if (w.written[s]) bad = "the part range overlaps parts written before";
     if (bad) {
         fail(std::string("write_layered: ") + bad);
         return -1;
@@ -1010,15 +990,13 @@ int Connection::write_layered(GatherWriter& w, const GatherSpec& g, int elems, u
     if (first) {
         w.device = device;
         w.scale = scale;
-        w.elems = elems;
-        w.part_bytes = part_bytes;
+        w.fp8_elems = g.fp8_elems;
+        w.part_bytes = uint32_t(g.pool_part_bytes());
         w.offsets.swap(scaled);
     }
-    GatherSpec c = g;
-    c.part_bytes = part_bytes;
     const int r = move_blocks(true, w.offsets.data(), 1, w.blocks.data(), w.blocks.size(),
-                              int(w.nparts * part_bytes), 0, device, stream, elems, nullptr, &c,
-                              &w);
+                              int(w.nparts * w.part_bytes), 0, device, stream, int(g.fp8_elems),
+                              nullptr, &g, &w);
     if (r != 0) {
         w.failed = true;
         return r;
@@ -1027,24 +1005,6 @@ int Connection::write_layered(GatherWriter& w, const GatherSpec& g, int elems, u
     w.parts_written += g.nparts;
     ++w.calls;
     return 0;
-}
-
-int Connection::r_rdma_scatter_fp8(const GatherSpec& g, int elems,
-                                   const std::vector<KeyOffset>& blocks, int device,
-                                   uint64_t stream) {
-    if (blocks.empty()) return 0;
-    std::vector<uint64_t> offs(blocks.size());
-    for (size_t i = 0; i < blocks.size(); ++i) offs[i] = blocks[i].offset;
-    if (device < 0 || g.rows || !gather_fp8_ok(g, elems, offs.data(), offs.size(), g.first_part)) {
-        fail("r_rdma_scatter_fp8: needs CUDA tensors, parts of a multiple of 512 elements and "
-             "16-byte aligned part bases and offsets, and reads whole parts");
-        return -1;
-    }
-    GatherSpec r = g;
-    r.part_bytes = uint32_t(kernels::fp8_gather_bytes(1, uint32_t(elems)));
-    return read_blocks(kOpReadLookup, blocks,
-                       int(kernels::fp8_gather_bytes(g.nparts, uint32_t(elems))), 0, device,
-                       stream, elems, nullptr, nullptr, &r);
 }
 
 int Connection::rw_local(char op, const std::vector<KeyOffset>& blocks, int block_size,
@@ -1097,7 +1057,7 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
         return 0;
     }
     if (scope.begin(stream_in, false) != 0) return -1;
-    const size_t max_batch = gather ? gather_batch_cap(*gather, fp8_elems) : kMaxBatch;
+    const size_t max_batch = gather ? gather_batch_cap(*gather) : kMaxBatch;
     const bool layered = gather && gather->reader;
     ReaderHold hold{*this, ctx, layered ? gather->reader : nullptr, scope.stream};
     KeyBatch b;

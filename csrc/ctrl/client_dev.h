@@ -86,9 +86,9 @@ struct Connection::DevCtx {
     uint32_t* status_d = nullptr;
     std::vector<cudaStream_t> busy;  // streams with launches since the last wait_all()
     bool dirty = false;
-    // Layered reads (Connection::read_scatter_layered): kReaderSlots slots of kGatherMaxParts
-    // group flags, allocated and zeroed on the first such read; reader seq uses slot
-    // seq % kReaderSlots (staging.h: ReaderSlots), whose event completes with its launches.
+    // Layered reads (Connection::r_rdma_scatter with a reader): kReaderSlots slots of
+    // kGatherMaxParts group flags, allocated and zeroed on the first such read; reader seq uses
+    // slot seq % kReaderSlots (staging.h: ReaderSlots), whose event completes with its launches.
     uint32_t* group_flags = nullptr;
     ReaderSlots<cudaEvent_t, kReaderSlots> readers;
     cudaEvent_t reader_ev[kReaderSlots] = {};

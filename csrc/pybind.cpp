@@ -180,10 +180,20 @@ struct KeyArena {
 
 thread_local KeyArena t_arena;
 
-// A row-sliced read's geometry, (rows, row_bytes, src_pitch, src_col, dst_pitch) in bytes;
-// empty: whole parts.  The connection checks the values.
-void set_rows(Connection::GatherSpec& g, const std::vector<uint32_t>& rows) {
-    if (rows.empty()) return;
+// A gathered call's parts: part s at part_base[s] (which must outlive the spec); elems > 0:
+// bf16 parts of elems elements stored as fp8 pages.  rows: a row-sliced read's geometry,
+// (rows, row_bytes, src_pitch, src_col, dst_pitch) in bytes; empty: whole parts.  The
+// connection checks the values.
+Connection::GatherSpec gather_spec(const std::vector<uint64_t>& part_base, uint32_t part_bytes,
+                                   uint32_t elems, uint32_t first_part,
+                                   const std::vector<uint32_t>& rows = {}) {
+    Connection::GatherSpec g;
+    g.part_base = part_base.data();
+    g.nparts = uint32_t(part_base.size());
+    g.part_bytes = part_bytes;
+    g.fp8_elems = elems;
+    g.first_part = first_part;
+    if (rows.empty()) return g;
     if (rows.size() != 5)
         throw py::value_error("rows is (rows, row_bytes, src_pitch, src_col, dst_pitch)");
     g.rows = rows[0];
@@ -191,6 +201,7 @@ void set_rows(Connection::GatherSpec& g, const std::vector<uint32_t>& rows) {
     g.src_pitch = rows[2];
     g.src_col = rows[3];
     g.dst_pitch = rows[4];
+    return g;
 }
 
 // [(key, offset), ...] -> KeyOffset views (offset * scale bytes).  Also accepted: the pair
@@ -568,110 +579,47 @@ PYBIND11_MODULE(_infinistore, m) {
         .def(
             "w_rdma_gather",
             [](Connection& c, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
-               const py::object& offsets, const py::object& remote_blocks, int device,
-               uint64_t stream, uint64_t scale) {
+               uint32_t elems, const py::object& offsets, const py::object& remote_blocks,
+               int device, uint64_t stream, uint64_t scale) {
                 BlockSpan rb;
                 OffsetSpan off;
                 blocks_from_py(remote_blocks, rb);
                 offsets_from_py(offsets, off);
                 std::vector<uint64_t> bytes(off.n);
                 for (size_t i = 0; i < off.n; ++i) bytes[i] = off.data[i] * scale;
-                Connection::GatherSpec g;
-                g.part_base = part_base.data();
-                g.nparts = uint32_t(part_base.size());
-                g.part_bytes = part_bytes;
+                const Connection::GatherSpec g = gather_spec(part_base, part_bytes, elems, 0);
                 py::gil_scoped_release rel;
                 return c.w_rdma_gather(g, bytes.data(), bytes.size(), rb.data, rb.n, device, stream);
             },
-            py::arg("part_base"), py::arg("part_bytes"), py::arg("offsets"),
+            py::arg("part_base"), py::arg("part_bytes"), py::arg("elems"), py::arg("offsets"),
             py::arg("remote_blocks"), py::arg("device") = -1, py::arg("stream") = 0,
             py::arg("scale") = 1,
-            "gathered write: block i = part s at part_base[s] + offsets[i] * scale, s = 0..S-1")
+            "gathered write: block i = part s at part_base[s] + offsets[i] * scale, s = 0..S-1; "
+            "elems > 0: bf16 parts of elems elements, quantised into fp8 page s of block i")
         .def(
             "r_rdma_scatter",
             [](Connection& c, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
-               uint32_t first_part, const py::object& blocks, int device, uint64_t stream,
-               uint64_t scale, const std::vector<uint32_t>& rows) {
+               uint32_t elems, uint32_t first_part, const py::object& blocks, int device,
+               uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows,
+               Connection::ScatterReader* reader, uint32_t group_parts) {
                 std::vector<KeyOffset> kb;
                 blocks_list_from_py(blocks, scale, kb);
-                Connection::GatherSpec g;
-                g.part_base = part_base.data();
-                g.nparts = uint32_t(part_base.size());
-                g.part_bytes = part_bytes;
-                g.first_part = first_part;
-                set_rows(g, rows);
+                Connection::GatherSpec g =
+                    gather_spec(part_base, part_bytes, elems, first_part, rows);
+                g.reader = reader;
+                g.group_parts = group_parts;
                 py::gil_scoped_release rel;
                 return c.r_rdma_scatter(g, kb, device, stream);
             },
-            py::arg("part_base"), py::arg("part_bytes"), py::arg("first_part"), py::arg("blocks"),
-            py::arg("device") = -1, py::arg("stream") = 0, py::arg("scale") = 1,
-            py::arg("rows") = std::vector<uint32_t>{},
-            "scattered read: stored part first_part + s of each block -> part_base[s] + offset; "
-            "rows = (rows, row_bytes, src_pitch, src_col, dst_pitch): only those rows of each "
-            "part, row r to part_base[s] + offset + r * dst_pitch")
-        .def(
-            "w_rdma_gather_fp8",
-            [](Connection& c, const std::vector<uint64_t>& part_base, int elems,
-               const py::object& offsets, const py::object& remote_blocks, int device,
-               uint64_t stream, uint64_t scale) {
-                BlockSpan rb;
-                OffsetSpan off;
-                blocks_from_py(remote_blocks, rb);
-                offsets_from_py(offsets, off);
-                std::vector<uint64_t> bytes(off.n);
-                for (size_t i = 0; i < off.n; ++i) bytes[i] = off.data[i] * scale;
-                Connection::GatherSpec g;
-                g.part_base = part_base.data();
-                g.nparts = uint32_t(part_base.size());
-                py::gil_scoped_release rel;
-                return c.w_rdma_gather_fp8(g, elems, bytes.data(), bytes.size(), rb.data, rb.n,
-                                           device, stream);
-            },
-            py::arg("part_base"), py::arg("elems"), py::arg("offsets"), py::arg("remote_blocks"),
-            py::arg("device") = -1, py::arg("stream") = 0, py::arg("scale") = 1,
-            "gathered fp8 write: bf16 part s at part_base[s] + offsets[i] * scale is quantised "
-            "into fp8 page s of block i")
-        .def(
-            "r_rdma_scatter_fp8",
-            [](Connection& c, const std::vector<uint64_t>& part_base, int elems,
-               uint32_t first_part, const py::object& blocks, int device, uint64_t stream,
-               uint64_t scale) {
-                std::vector<KeyOffset> kb;
-                blocks_list_from_py(blocks, scale, kb);
-                Connection::GatherSpec g;
-                g.part_base = part_base.data();
-                g.nparts = uint32_t(part_base.size());
-                g.first_part = first_part;
-                py::gil_scoped_release rel;
-                return c.r_rdma_scatter_fp8(g, elems, kb, device, stream);
-            },
-            py::arg("part_base"), py::arg("elems"), py::arg("first_part"), py::arg("blocks"),
-            py::arg("device") = -1, py::arg("stream") = 0, py::arg("scale") = 1,
-            "scattered fp8 read: fp8 page first_part + s of each block, dequantised -> "
-            "part_base[s] + offset")
-        .def(
-            "r_rdma_scatter_layered",
-            [](Connection& c, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
-               int elems, uint32_t first_part, uint32_t group_parts, const py::object& blocks,
-               int device, uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows) {
-                std::vector<KeyOffset> kb;
-                blocks_list_from_py(blocks, scale, kb);
-                Connection::GatherSpec g;
-                g.part_base = part_base.data();
-                g.nparts = uint32_t(part_base.size());
-                g.part_bytes = part_bytes;
-                g.first_part = first_part;
-                set_rows(g, rows);
-                auto r = std::make_shared<Connection::ScatterReader>();
-                py::gil_scoped_release rel;
-                c.read_scatter_layered(g, elems, group_parts, kb, device, stream, *r);
-                return r;
-            },
             py::arg("part_base"), py::arg("part_bytes"), py::arg("elems"), py::arg("first_part"),
-            py::arg("group_parts"), py::arg("blocks"), py::arg("device") = -1,
-            py::arg("stream") = 0, py::arg("scale") = 1, py::arg("rows") = std::vector<uint32_t>{},
-            "layered scattered read (r_rdma_scatter, or r_rdma_scatter_fp8 with elems > 0) "
-            "whose parts are released in groups of group_parts; check .failed")
+            py::arg("blocks"), py::arg("device") = -1, py::arg("stream") = 0,
+            py::arg("scale") = 1, py::arg("rows") = std::vector<uint32_t>{},
+            py::arg("reader") = py::none(), py::arg("group_parts") = 0,
+            "scattered read: stored part first_part + s of each block -> part_base[s] + offset; "
+            "elems > 0: fp8 pages dequantised into bf16 parts of elems elements; rows = (rows, "
+            "row_bytes, src_pitch, src_col, dst_pitch): only those rows of each part, row r to "
+            "part_base[s] + offset + r * dst_pitch; reader: a layered read whose parts are "
+            "released in groups of group_parts (check reader.failed)")
         .def(
             "wait_layered",
             [](Connection& c, const Connection::ScatterReader& r, uint32_t group, uint64_t stream) {
@@ -707,15 +655,12 @@ PYBIND11_MODULE(_infinistore, m) {
         .def(
             "w_rdma_layered",
             [](Connection& c, Connection::GatherWriter& w, const std::vector<uint64_t>& part_base,
-               uint32_t part_bytes, int elems, uint32_t first_part, int device, uint64_t stream,
-               uint64_t scale) {
-                Connection::GatherSpec g;
-                g.part_base = part_base.data();
-                g.nparts = uint32_t(part_base.size());
-                g.part_bytes = part_bytes;
-                g.first_part = first_part;
+               uint32_t part_bytes, uint32_t elems, uint32_t first_part, int device,
+               uint64_t stream, uint64_t scale) {
+                const Connection::GatherSpec g =
+                    gather_spec(part_base, part_bytes, elems, first_part);
                 py::gil_scoped_release rel;
-                return c.write_layered(w, g, elems, scale, device, stream);
+                return c.write_layered(w, g, scale, device, stream);
             },
             py::arg("writer"), py::arg("part_base"), py::arg("part_bytes"), py::arg("elems"),
             py::arg("first_part"), py::arg("device") = -1, py::arg("stream") = 0,
@@ -782,6 +727,7 @@ PYBIND11_MODULE(_infinistore, m) {
         });
     py::class_<Connection::ScatterReader, std::shared_ptr<Connection::ScatterReader>>(
         m, "ScatterReader")
+        .def(py::init<>())
         .def_readonly("groups", &Connection::ScatterReader::groups)
         .def_readonly("group_parts", &Connection::ScatterReader::group_parts)
         .def_readonly("seq", &Connection::ScatterReader::seq)

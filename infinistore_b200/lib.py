@@ -391,6 +391,14 @@ def _raise_if_fp8_pages_unaligned(cache: torch.Tensor, offsets) -> None:
                          "offset must be multiples of 8 bf16 elements")
 
 
+def _split_blocks(blocks):
+    """``[(key, offset)]`` or ``(keys, offsets)`` with ``offsets`` an ndarray -> (keys,
+    offsets)."""
+    if isinstance(blocks, tuple) and len(blocks) == 2 and isinstance(blocks[1], np.ndarray):
+        return list(blocks[0]), blocks[1]
+    return [b[0] for b in blocks], [int(b[1]) for b in blocks]
+
+
 def _device_of(cache: torch.Tensor) -> int:
     return cache.device.index if cache.device.type == "cuda" else -1
 
@@ -654,14 +662,28 @@ class InfinityConnection:
             raise Exception(f"Failed to read to infinistore, ret = {ret}: {self.conn.last_error()}")
 
     # ------------------------------------------------------------------ gathered blocks
-    def _gather_parts(self, parts, max_offset: int, part_size: int, fp8: bool = False,
-                      offsets=None, extent=None):
-        """Checks a parts list ``[(tensor, base), ...]`` before anything is enqueued.  Returns
-        (absolute byte address of every part, device ordinal or -1, element size).  ``fp8``:
+    def _gather_parts(self, parts, offsets, part_size: int, first_part: int = 0,
+                      block_parts=None, fp8: bool = False, rows: "PartRows | None" = None, *,
+                      nblocks=None, stream="current"):
+        """Checks a gathered call before anything is enqueued: parts ``first_part ..
+        first_part + len(parts) - 1`` of the blocks at ``offsets`` (elements, a list or an int64
+        ndarray; ``nblocks`` of them when given), in a parts list ``[(tensor, base), ...]``, of
+        blocks that hold ``block_parts`` parts (default ``first_part + len(parts)``).  ``fp8``:
         the parts are bf16 CUDA tensors, ``part_size`` is a multiple of 512 elements and every
-        part base and offset (``offsets``, elements) is 16-byte aligned."""
+        part base and offset is 16-byte aligned.  ``rows``: a row-sliced read.  Returns
+        (absolute byte address of every part, device ordinal or -1, element size, int64
+        offsets, stream handle)."""
         if self._mode != "rdma":
             raise Exception("gathered blocks need a connected rdma connection")
+        offs = np.ascontiguousarray(offsets, dtype=np.int64).reshape(-1)
+        if nblocks is not None and len(offs) != nblocks:
+            raise ValueError(f"{len(offs)} offsets for {nblocks} blocks")
+        if len(offs) and int(offs.min()) < 0:
+            raise ValueError("offsets must not be negative")
+        first_part = int(first_part)
+        if first_part < 0:
+            raise ValueError("first_part must not be negative")
+        extent = rows.check(part_size) if rows is not None else int(part_size)
         parts = list(parts)
         if not 1 <= len(parts) <= GATHER_MAX_PARTS:
             raise ValueError(f"a parts list holds 1 to {GATHER_MAX_PARTS} parts, not {len(parts)}")
@@ -669,15 +691,17 @@ class InfinityConnection:
             if not (isinstance(part, (tuple, list)) and len(part) == 2
                     and isinstance(part[0], torch.Tensor)):
                 raise ValueError(f"part {i} is not a (tensor, base) pair")
-        if int(part_size) <= 0:
+        part_size = int(part_size)
+        if part_size <= 0:
             raise ValueError("part_size must be positive")
         first = parts[0][0]
         es = first.element_size()
-        block_bytes = (self.fp8_gather_block_bytes(len(parts), int(part_size)) if fp8
-                       else len(parts) * int(part_size) * es)
-        if block_bytes > _GATHER_MAX_BLOCK_BYTES:
-            raise ValueError(f"{len(parts)} parts of {int(part_size) * es} bytes exceed the "
+        pool_part = self.fp8_gather_block_bytes(1, part_size) if fp8 else part_size * es
+        nparts = first_part + len(parts) if block_parts is None else int(block_parts)
+        if nparts * pool_part > _GATHER_MAX_BLOCK_BYTES:
+            raise ValueError(f"{nparts} parts of {pool_part} bytes exceed the "
                              f"{_GATHER_MAX_BLOCK_BYTES}-byte block limit")
+        max_offset = int(offs.max()) if len(offs) else 0
         bases = []
         for i, (t, base) in enumerate(parts):
             base = int(base)
@@ -687,22 +711,21 @@ class InfinityConnection:
                 raise ValueError(f"part {i}: tensor on {t.device}, part 0 on {first.device}")
             if t.dtype != first.dtype:
                 raise ValueError(f"part {i}: dtype {t.dtype}, part 0 has {first.dtype}")
-            span = int(part_size) if extent is None else int(extent)
-            if base < 0 or base + max_offset + span > t.numel():
+            if base < 0 or base + max_offset + extent > t.numel():
                 raise ValueError(f"part {i}: base {base} + offset {max_offset} + part extent "
-                                 f"{span} runs past the tensor's {t.numel()} elements")
+                                 f"{extent} runs past the tensor's {t.numel()} elements")
             bases.append(t.data_ptr() + base * es)
         if fp8:
             if first.dtype != torch.bfloat16:
                 raise ValueError(f"fp8 gathered blocks take bf16 tensors, not {first.dtype}")
-            if int(part_size) % 512:
+            if part_size % 512:
                 raise ValueError(f"fp8 gathered blocks need a part_size that is a multiple of "
-                                 f"512 elements, not {int(part_size)}")
+                                 f"512 elements, not {part_size}")
             align = 0
             for b in bases:
                 align |= b
-            if offsets is not None and len(offsets):
-                align |= int(np.bitwise_or.reduce(np.asarray(offsets, dtype=np.int64) * es))
+            if len(offs):
+                align |= int(np.bitwise_or.reduce(offs * es))
             if align & 15:
                 raise ValueError("fp8 gathered blocks need 16-byte aligned part bases and offsets")
             if first.device.type != "cuda":
@@ -711,7 +734,7 @@ class InfinityConnection:
         if dev < 0 and self.conn.server_has_hbm():
             raise ValueError("gathered blocks of CPU tensors need a host-memory pool "
                              "(--pool-backend host)")
-        return bases, dev, es
+        return bases, dev, es, offs, _stream_of(first, stream)
 
     def rdma_write_cache_gather(self, parts, offsets, part_size: int, remote_blocks,
                                 stream="current"):
@@ -727,36 +750,15 @@ class InfinityConnection:
         ``rdma_write_cache`` trusts ``page_size``.  Blocks the server marked as already
         existing are skipped (first writer wins); the in-band commit publishes a block once,
         after all of its parts have landed.  CPU tensors need a host-memory pool."""
-        offs = np.ascontiguousarray(offsets, dtype=np.int64).reshape(-1)
-        if len(offs) != len(remote_blocks):
-            raise ValueError(f"{len(offs)} offsets for {len(remote_blocks)} remote blocks")
-        if len(offs) and int(offs.min()) < 0:
-            raise ValueError("offsets must not be negative")
-        bases, dev, es = self._gather_parts(parts, int(offs.max()) if len(offs) else 0, part_size)
+        bases, dev, es, offs, s = self._gather_parts(parts, offsets, part_size,
+                                                     nblocks=len(remote_blocks), stream=stream)
         if not len(offs):
             return 0
-        ret = self.conn.w_rdma_gather(bases, int(part_size) * es, offs, remote_blocks, dev,
-                                      _stream_of(parts[0][0], stream), es)
+        ret = self.conn.w_rdma_gather(bases, int(part_size) * es, 0, offs, remote_blocks, dev, s,
+                                      es)
         if ret < 0:
             raise Exception(f"Failed to write to infinistore, ret = {ret}: {self.conn.last_error()}")
         return 0
-
-    @staticmethod
-    def _scatter_blocks(blocks, first_part: int):
-        """``[(key, offset)]`` or ``(keys, offsets)`` -> (keys, int64 offsets), checked."""
-        if isinstance(blocks, tuple) and len(blocks) == 2 and isinstance(blocks[1], np.ndarray):
-            keys = list(blocks[0])
-            offs = np.ascontiguousarray(blocks[1], dtype=np.int64).reshape(-1)
-            if len(keys) != len(offs):
-                raise ValueError(f"{len(keys)} keys for {len(offs)} offsets")
-        else:
-            keys = [b[0] for b in blocks]
-            offs = np.asarray([int(b[1]) for b in blocks], dtype=np.int64)
-        if len(offs) and int(offs.min()) < 0:
-            raise ValueError("offsets must not be negative")
-        if int(first_part) < 0:
-            raise ValueError("first_part must not be negative")
-        return keys, offs
 
     def read_cache_scatter(self, parts, blocks, part_size: int, first_part: int = 0,
                            stream="current", rows: "PartRows | None" = None):
@@ -777,17 +779,14 @@ class InfinityConnection:
         of one destination, e.g. one per source rank of a page written at another
         tensor-parallel degree.  Bad geometry raises ``ValueError`` before anything is
         enqueued."""
-        keys, offs = self._scatter_blocks(blocks, first_part)
-        extent = rows.check(part_size) if rows is not None else None
-        bases, dev, es = self._gather_parts(parts, int(offs.max()) if len(offs) else 0, part_size,
-                                            extent=extent)
-        if (int(first_part) + len(bases)) * int(part_size) * es > _GATHER_MAX_BLOCK_BYTES:
-            raise ValueError("first_part + parts run past the block size limit")
+        keys, offs = _split_blocks(blocks)
+        bases, dev, es, offs, s = self._gather_parts(parts, offs, part_size, first_part,
+                                                     rows=rows, nblocks=len(keys), stream=stream)
         native_rows = rows.native(es) if rows is not None else []
         if not len(offs):
             return
-        ret = self.conn.r_rdma_scatter(bases, int(part_size) * es, int(first_part), (keys, offs),
-                                       dev, _stream_of(parts[0][0], stream), es, native_rows)
+        ret = self.conn.r_rdma_scatter(bases, int(part_size) * es, 0, int(first_part),
+                                       (keys, offs), dev, s, es, native_rows)
         if ret < 0:
             raise Exception(f"Failed to read to infinistore, ret = {ret}: {self.conn.last_error()}")
 
@@ -808,17 +807,12 @@ class InfinityConnection:
         bf16 bytes.  The parts are bf16 CUDA tensors, ``part_size`` is a multiple of 512
         elements, and part bases and offsets are 16-byte aligned.  The blocks must have been
         allocated with ``fp8_gather_block_bytes(len(parts), part_size)`` bytes."""
-        offs = np.ascontiguousarray(offsets, dtype=np.int64).reshape(-1)
-        if len(offs) != len(remote_blocks):
-            raise ValueError(f"{len(offs)} offsets for {len(remote_blocks)} remote blocks")
-        if len(offs) and int(offs.min()) < 0:
-            raise ValueError("offsets must not be negative")
-        bases, dev, _ = self._gather_parts(parts, int(offs.max()) if len(offs) else 0, part_size,
-                                           fp8=True, offsets=offs)
+        bases, dev, es, offs, s = self._gather_parts(parts, offsets, part_size, fp8=True,
+                                                     nblocks=len(remote_blocks), stream=stream)
         if not len(offs):
             return 0
-        ret = self.conn.w_rdma_gather_fp8(bases, int(part_size), offs, remote_blocks, dev,
-                                          _stream_of(parts[0][0], stream), 2)
+        ret = self.conn.w_rdma_gather(bases, int(part_size) * es, int(part_size), offs,
+                                      remote_blocks, dev, s, es)
         if ret < 0:
             raise Exception(f"Failed to write to infinistore, ret = {ret}: {self.conn.last_error()}")
         return 0
@@ -830,16 +824,13 @@ class InfinityConnection:
         for ``read_cache_scatter``).  With ``device_lookup`` a stored block shorter than
         ``fp8_gather_block_bytes(first_part + len(parts), part_size)`` is a miss.  The same
         checks as ``rdma_write_cache_gather_fp8``."""
-        keys, offs = self._scatter_blocks(blocks, first_part)
-        bases, dev, _ = self._gather_parts(parts, int(offs.max()) if len(offs) else 0, part_size,
-                                           fp8=True, offsets=offs)
-        if self.fp8_gather_block_bytes(int(first_part) + len(bases),
-                                       int(part_size)) > _GATHER_MAX_BLOCK_BYTES:
-            raise ValueError("first_part + parts run past the block size limit")
+        keys, offs = _split_blocks(blocks)
+        bases, dev, es, offs, s = self._gather_parts(parts, offs, part_size, first_part,
+                                                     fp8=True, nblocks=len(keys), stream=stream)
         if not len(offs):
             return
-        ret = self.conn.r_rdma_scatter_fp8(bases, int(part_size), int(first_part), (keys, offs),
-                                           dev, _stream_of(parts[0][0], stream), 2)
+        ret = self.conn.r_rdma_scatter(bases, int(part_size) * es, int(part_size), int(first_part),
+                                       (keys, offs), dev, s, es)
         if ret < 0:
             raise Exception(f"Failed to read to infinistore, ret = {ret}: {self.conn.last_error()}")
 
@@ -864,10 +855,10 @@ class InfinityConnection:
         ``read_cache_scatter`` (not with ``fp8``)."""
         if rows is not None and fp8:
             raise ValueError("row-sliced reads of fp8 blocks are not supported")
-        keys, offs = self._scatter_blocks(blocks, first_part)
-        extent = rows.check(part_size) if rows is not None else None
-        bases, dev, es = self._gather_parts(parts, int(offs.max()) if len(offs) else 0, part_size,
-                                            fp8=fp8, offsets=offs if fp8 else None, extent=extent)
+        keys, offs = _split_blocks(blocks)
+        bases, dev, es, offs, s = self._gather_parts(parts, offs, part_size, first_part,
+                                                     fp8=fp8, rows=rows, nblocks=len(keys),
+                                                     stream=stream)
         if dev < 0:
             raise ValueError("layered reads take CUDA tensors")
         if not self.conn.server_has_hbm():
@@ -875,17 +866,11 @@ class InfinityConnection:
         group_parts = int(group_parts)
         if group_parts < 1 or len(bases) % group_parts:
             raise ValueError(f"group_parts {group_parts} does not divide the {len(bases)} parts")
-        end = int(first_part) + len(bases)
-        limit = (self.fp8_gather_block_bytes(end, int(part_size)) if fp8
-                 else end * int(part_size) * es)
-        if limit > _GATHER_MAX_BLOCK_BYTES:
-            raise ValueError("first_part + parts run past the block size limit")
-        first = parts[0][0]
-        native = self.conn.r_rdma_scatter_layered(
-            bases, int(part_size) * es, int(part_size) if fp8 else 0, int(first_part), group_parts,
-            (keys, offs), dev, _stream_of(first, stream), es,
-            rows.native(es) if rows is not None else [])
-        read = ScatterRead(self, native, first.device)
+        native = _infinistore.ScatterReader()
+        self.conn.r_rdma_scatter(bases, int(part_size) * es, int(part_size) if fp8 else 0,
+                                 int(first_part), (keys, offs), dev, s, es,
+                                 rows.native(es) if rows is not None else [], native, group_parts)
+        read = ScatterRead(self, native, parts[0][0].device)
         if native.failed:
             err = Exception(f"Failed to read to infinistore: {self.conn.last_error()}")
             err.read = read
@@ -1156,7 +1141,6 @@ class GatherWriter:
         self._conn = conn
         self._w = native
         self._offs = offsets
-        self._max_off = int(offsets.max()) if len(offsets) else 0
         self.nparts = nparts
         self.part_size = part_size
         self.fp8 = fp8
@@ -1190,21 +1174,15 @@ class GatherWriter:
         if any(written[first_part:first_part + len(parts)]):
             raise ValueError("the part range overlaps parts written before")
         conn = self._conn
-        bases, dev, es = conn._gather_parts(parts, self._max_off, self.part_size, fp8=self.fp8,
-                                            offsets=self._offs)
+        bases, dev, es, _, s = conn._gather_parts(parts, self._offs, self.part_size, first_part,
+                                                  self.nparts, self.fp8, stream=stream)
         first = parts[0][0]
         if self._dev is not None and self._dev != (first.device, first.dtype):
             raise ValueError(f"parts on {first.device} as {first.dtype}, the writer's first call "
                              f"used {self._dev[0]} as {self._dev[1]}")
-        block_bytes = (conn.fp8_gather_block_bytes(self.nparts, self.part_size) if self.fp8
-                       else self.nparts * self.part_size * es)
-        if block_bytes > _GATHER_MAX_BLOCK_BYTES:
-            raise ValueError(f"{self.nparts} parts of {self.part_size * es} bytes exceed the "
-                             f"{_GATHER_MAX_BLOCK_BYTES}-byte block limit")
         self._dev = (first.device, first.dtype)
         ret = conn.conn.w_rdma_layered(self._w, bases, self.part_size * es,
-                                       self.part_size if self.fp8 else 0, first_part, dev,
-                                       _stream_of(first, stream), es)
+                                       self.part_size if self.fp8 else 0, first_part, dev, s, es)
         if ret < 0:
             raise Exception(f"Failed to write to infinistore, ret = {ret}: "
                             f"{conn.conn.last_error()}")
