@@ -24,7 +24,14 @@ the median.  The layered flavour (read_pages_layered(source_tp=W)) is timed to t
 layer 0 and of the last layer, as seen by a consumer stream that waits for them.  Every
 round's pages are checked bit for bit against the full-head source.  Prints the card's name,
 power limit and SM clock from the same run, then one JSON line.  Over NVLink (a pool on
-another GPU) the numbers may differ; that is not measured here."""
+another GPU) the numbers may differ; that is not measured here.
+
+--fp8: the pages are written as fp8 (write_pages(fp8=True)) and every arm reads with fp8=True:
+rows is then the dequantising row-sliced read (kv_read_fp8_rows), staging a same-TP fp8 read
+per source rank and a torch copy of its heads, same_tp a same-TP fp8 read.  A head of 128
+elements is one scale group, so all three give the same bits; every round is checked against
+a same-TP fp8 read taken before the timed rounds.  Each arm also reports the pool bytes it
+reads (e4m3 payload and scales), from the shapes."""
 from __future__ import annotations
 
 import argparse
@@ -40,6 +47,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "bench"))
 import infinistore_b200 as ist  # noqa: E402
 from infinistore_b200 import _infinistore as native  # noqa: E402
+from infinistore_b200.lib import InfinityConnection  # noqa: E402
 from infinistore_b200.models.kv_layout import KVLayout, tp_sources  # noqa: E402
 from infinistore_b200.models.paged_kv import PagedKVCache  # noqa: E402
 from gather_fp8 import card  # noqa: E402
@@ -60,6 +68,20 @@ def view(cache):
                            lay.head_dim)
 
 
+def same_bits(a, b):
+    """Equal bf16 bits (NaN included)."""
+    return torch.equal(a.contiguous().view(torch.int16), b.contiguous().view(torch.int16))
+
+
+def pool_bytes(rl, wl, n, nsrc):
+    """fp8 pool bytes each arm reads for n pages: payload and scales of what it touches."""
+    parts = 2 * LAYERS
+    rows = PagedKVCache(rl, 1, "meta")._sources([0], ["p"], wl.tp)[2].native(2)
+    return {"rows": n * nsrc * parts * native.testing.fp8_rows_read_bytes(*rows[:4]),
+            "staging": n * nsrc * parts * InfinityConnection.fp8_page_bytes(wl.page_elems),
+            "same_tp": n * parts * InfinityConnection.fp8_page_bytes(rl.page_elems)}
+
+
 def timed(fn):
     """Device milliseconds of fn() on the current stream."""
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -77,7 +99,9 @@ def main():
     ap.add_argument("--reps", type=int, default=9)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--pool-gb", type=int, default=8)
+    ap.add_argument("--fp8", action="store_true", help="fp8 pages (write_pages(fp8=True))")
     a = ap.parse_args()
+    fp8 = a.fp8
     if not torch.cuda.is_available():
         raise SystemExit("tp_regroup_read.py needs a CUDA device")
     dev = torch.device("cuda", 0)
@@ -99,6 +123,8 @@ def main():
     port = srv.start()
     out = {"card": info, "layout": "llama-3-70b", "pages": n, "page_tokens": TOKENS,
            "reps": a.reps, "directions": {}}
+    if fp8:
+        out["fp8"] = True
     try:
         conn = ist.InfinityConnection(ist.ClientConfig(
             host_addr="127.0.0.1", service_port=port, connection_type=ist.TYPE_RDMA,
@@ -112,7 +138,7 @@ def main():
             for w in range(tp):
                 c = PagedKVCache(base.with_tp(tp), n, dev, tp_rank=w)
                 view(c).copy_(full[:, :, :, :, heads_of(tp, w), :])
-                c.write_pages(conn, pages, hashes[tp])
+                c.write_pages(conn, pages, hashes[tp], fp8=fp8)
                 conn.sync()
                 del c
         torch.cuda.empty_cache()
@@ -122,20 +148,24 @@ def main():
             srcs = tp_sources(rl, rt, 0, wt)
             want = full[:, :, :, :, heads_of(rt, 0), :]
             reader = PagedKVCache(rl, n, dev, tp_rank=0)
+            if fp8:  # the dequantised pages: a same-TP fp8 read, outside the timed rounds
+                reader.read_pages(conn, pages, hashes[rt], fp8=True)
+                conn.sync()
+                want = view(reader).clone()
             staging = [PagedKVCache(wl, n, dev, tp_rank=w) for w, *_ in srcs]
             dst_bytes = n * LAYERS * 2 * rl.page_bytes
 
             def rows():
-                reader.read_pages(conn, pages, hashes[wt], source_tp=wt)
+                reader.read_pages(conn, pages, hashes[wt], source_tp=wt, fp8=fp8)
 
             def stage():
                 v = view(reader)
                 for st, (w, sh, dh, k) in zip(staging, srcs):
-                    st.read_pages(conn, pages, hashes[wt])
+                    st.read_pages(conn, pages, hashes[wt], fp8=fp8)
                     v[:, :, :, :, dh:dh + k].copy_(view(st)[:, :, :, :, sh:sh + k])
 
             def same():
-                reader.read_pages(conn, pages, hashes[rt])
+                reader.read_pages(conn, pages, hashes[rt], fp8=fp8)
 
             arms = {"rows": rows, "staging": stage, "same_tp": same}
             ms = {k: [] for k in ARMS}
@@ -144,12 +174,14 @@ def main():
                     reader.data.zero_()
                     t = timed(arms[k])
                     conn.sync()
-                    assert torch.equal(view(reader), want), f"{wt}->{rt} {k}: wrong pages"
+                    assert same_bits(view(reader), want), f"{wt}->{rt} {k}: wrong pages"
                     if rep >= a.warmup:
                         ms[k].append(t)
             res = {"writer_tp": wt, "reader_tp": rt, "sources_per_page": len(srcs),
                    "blocks": n * len(srcs), "dst_bytes": dst_bytes,
                    "staging_bytes": sum(s.data.numel() * 2 for s in staging)}
+            if fp8:
+                res["pool_bytes"] = pool_bytes(rl, wl, n, len(srcs))
             for k in ARMS:
                 med = statistics.median(ms[k])
                 res[k] = {"ms_median": round(med, 4), "ms_min": round(min(ms[k]), 4),
@@ -167,14 +199,14 @@ def main():
                 torch.cuda.synchronize()
                 e0, e1, e2 = (torch.cuda.Event(enable_timing=True) for _ in range(3))
                 e0.record()
-                read = reader.read_pages_layered(conn, pages, hashes[wt], source_tp=wt)
+                read = reader.read_pages_layered(conn, pages, hashes[wt], source_tp=wt, fp8=fp8)
                 read.wait_layer(0, stream=cons)
                 e1.record(cons)
                 read.wait_layer(LAYERS - 1, stream=cons)
                 e2.record(cons)
                 torch.cuda.synchronize()
                 conn.sync()
-                assert torch.equal(view(reader), want), f"{wt}->{rt} layered: wrong pages"
+                assert same_bits(view(reader), want), f"{wt}->{rt} layered: wrong pages"
                 if rep >= a.warmup:
                     first.append(e0.elapsed_time(e1))
                     last.append(e0.elapsed_time(e2))

@@ -279,7 +279,8 @@ kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n,
     G.n = n;
     G.part_base = g.part_base;
     G.nparts = g.nparts;
-    G.part_bytes = uint32_t(g.pool_part_bytes());
+    // a row-sliced read's geometry counts bytes of the caller's view of a part (bf16 for fp8)
+    G.part_bytes = uint32_t(g.rows ? g.view_part_bytes() : g.pool_part_bytes());
     G.first_part = g.first_part;
     G.align_or = align_or;
     for (uint32_t s = 0; s < g.nparts; ++s) G.align_or |= g.part_base[s];
@@ -295,9 +296,14 @@ kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n,
     return G;
 }
 
-// Bytes one block of a gathered call moves: its parts, or their rows when row-sliced.
+// Bytes one block of a gathered call moves: its parts, or their rows when row-sliced (of fp8
+// parts: the pool bytes of those rows, read_plan.h: fp8_rows_read_bytes).
 static uint64_t gather_moved_bytes(const Connection::GatherSpec& g) {
-    return uint64_t(g.nparts) * (g.rows ? uint64_t(g.rows) * g.row_bytes : g.pool_part_bytes());
+    const uint64_t part = !g.rows ? g.pool_part_bytes()
+                          : g.fp8_elems
+                              ? fp8_rows_read_bytes(g.rows, g.row_bytes, g.src_pitch, g.src_col)
+                              : uint64_t(g.rows) * g.row_bytes;
+    return uint64_t(g.nparts) * part;
 }
 
 // Layered writers' state (GatherWriter::state), allocated stream-ordered from a memory pool of
@@ -860,11 +866,13 @@ const char* Connection::gather_refusal(const GatherSpec& g, const uint64_t* offs
     if (end > block_parts) return "the part range runs past the block";
     if (block_parts > uint64_t(INT32_MAX) / g.pool_part_bytes())
         return "bad parts list: a block holds at most 2^31 - 1 bytes";
-    if (g.rows && (write || g.fp8_elems || !g.row_bytes ||
-                   uint64_t(g.src_col) + g.row_bytes > g.src_pitch ||
-                   uint64_t(g.rows) * g.src_pitch != g.part_bytes))
-        return "bad row geometry (bf16 reads only, rows >= 1, src_col + row_bytes <= "
-               "src_pitch, part_bytes == rows * src_pitch)";
+    if (g.rows && (write || !g.row_bytes || uint64_t(g.src_col) + g.row_bytes > g.src_pitch ||
+                   uint64_t(g.rows) * g.src_pitch != g.view_part_bytes()))
+        return "bad row geometry (reads only, rows >= 1, src_col + row_bytes <= src_pitch, "
+               "part_bytes == rows * src_pitch)";
+    if (g.rows && g.fp8_elems && ((g.row_bytes | g.src_pitch | g.src_col | g.dst_pitch) & 15))
+        return "bad row geometry for fp8 parts: row_bytes, src_pitch, src_col and dst_pitch "
+               "must be multiples of 16 bytes (8 bf16 elements)";
     if (g.reader) {
         if (!g.group_parts || g.nparts % g.group_parts)
             return "a layered read needs group_parts that divides the part count";

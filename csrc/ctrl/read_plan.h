@@ -3,6 +3,7 @@
 // the caller, so the choice is unit-tested on the CPU (_infinistore.testing.plan_device_read).
 #pragma once
 
+#include <algorithm>
 #include <cstddef>
 #include <cstdint>
 
@@ -53,6 +54,26 @@ inline int device_read_grid_cap(int max_ctas, bool all_remote, bool fp8, int sm_
 // read phase (docs/kernels.md); pools behind NVLink keep the TMA pipeline.
 inline int local_auto_variant(int variant, bool local) {
     return variant == kernels::kCopyAuto && local ? int(kernels::kCopyLdSt256) : variant;
+}
+
+// What a row-sliced read of one stored fp8 part counts in bytes_read: the pool bytes it reads,
+// which are the e4m3 bytes of its rows plus 4 bytes for every 128-element scale group they
+// touch, each group counted once however many rows share it.  The geometry is in bytes of the
+// part's bf16 view (GatherLaunch::rows); rows never overlap and come in increasing order.
+// Full-width rows touch every group once: fp8_block_bytes(elems, 128), what a read of the
+// whole part counts.
+inline uint64_t fp8_rows_read_bytes(uint32_t rows, uint32_t row_bytes, uint32_t src_pitch,
+                                    uint32_t src_col) {
+    const uint64_t width = row_bytes / 2, pitch = src_pitch / 2, col = src_col / 2;
+    if (rows == 0 || width == 0) return 0;
+    uint64_t groups = 0, next = 0;  // next: the first group not counted yet
+    for (uint64_t r = 0; r < rows; ++r) {
+        const uint64_t lo = std::max((r * pitch + col) / 128, next);
+        const uint64_t hi = (r * pitch + col + width - 1) / 128;
+        if (hi >= lo) groups += hi - lo + 1;
+        next = std::max(next, hi + 1);
+    }
+    return uint64_t(rows) * width + 4 * groups;
 }
 
 inline DeviceReadPlan plan_device_read(const DeviceReadIn& in) {

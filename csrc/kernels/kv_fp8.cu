@@ -288,6 +288,118 @@ __global__ void __launch_bounds__(kThreads)
     }
 }
 
+// ---------------------------------------------------------------- row-sliced reads
+// The geometry of launch_kv_gather_fp8 with GatherLaunch::rows, in elements of the part's bf16
+// view (GatherLaunch counts bytes): row r of stored part s takes vpr 8-element vectors from
+// element r * src_pitch + src_col, and lands at r * dst_pitch bytes from the part's destination.
+struct Fp8Rows {
+    uint32_t rows, vpr, src_pitch, src_col, dst_pitch, elems;
+};
+
+constexpr int kRowVecs = 4;  // (row, vector) pairs in flight per thread: 4 x 16 B of bf16
+
+// `nrows` rows of one stored fp8 part `q` (scales at q + elems) from element e0 on, dequantised
+// to dst.  The 256 threads walk the (row, vector) pairs flattened together, as copy_rows
+// (copy_span.cuh) does, so one 128-element KV head (16 vectors) per row keeps every thread
+// busy.  A vector is 8 e4m3 bytes at q + e and the scale of its group at scales[e / 128]: the
+// geometry keeps e a multiple of 8, so a vector never straddles two scale groups.
+__device__ __forceinline__ void read_fp8_rows(uint8_t* dst, const uint8_t* q, const float* scales,
+                                              uint32_t e0, uint32_t nrows, const Fp8Rows& g) {
+    const uint32_t nvec = nrows * g.vpr;
+    uint32_t i = threadIdx.x;
+    for (; i < nvec; i += kRowVecs * kThreads) {
+        uint2 v[kRowVecs];
+        float sc[kRowVecs];
+        size_t out[kRowVecs];
+#pragma unroll
+        for (int u = 0; u < kRowVecs; ++u) {
+            const uint32_t k = i + u * kThreads;
+            if (k >= nvec) continue;
+            const uint32_t r = k / g.vpr, c = k - r * g.vpr;
+            const uint32_t e = e0 + r * g.src_pitch + 8 * c;
+            v[u] = ld_u2(q + e);
+            sc[u] = __uint_as_float(ld_u1(scales + e / kRow));
+            out[u] = size_t(r) * g.dst_pitch + 16 * c;
+        }
+#pragma unroll
+        for (int u = 0; u < kRowVecs; ++u) {
+            if (i + u * kThreads >= nvec) continue;
+            *reinterpret_cast<uint4*>(dst + out[u]) = dequant8(v[u], sc[u]);
+        }
+    }
+}
+
+// Item = run c (`run` rows) of part s of block b, numbered with layered_item: one group of all
+// nparts parts for a plain read, rel.gp parts per group for a layered one, each group released
+// by leave_group - the numbering, miss counting and release of kv_scatter_rows_kernel
+// (kv_copy.cu).  Stored part first_part + s starts at desc.src + (first_part + s) * stride.
+// A missing block counts once, on its first item, and its parts are left untouched; its items
+// still count as arrivals.
+template <bool LAYERED>
+__global__ void __launch_bounds__(kThreads)
+    kv_read_fp8_rows_kernel(const CopyDesc* __restrict__ descs,
+                            const __grid_constant__ GatherParts parts, uint32_t n, uint32_t nparts,
+                            uint32_t first_part, Fp8Rows geo, uint32_t run, uint32_t cpp,
+                            uint64_t stride, uint32_t* status, GroupRelease rel) {
+    const uint32_t gp = LAYERED ? rel.gp : nparts;
+    const uint32_t group_items = n * gp * cpp;
+    const uint32_t total = n * nparts * cpp;
+    uint32_t item = blockIdx.x;
+    CopyDesc next = item < total ? descs[layered_item(item, n, gp, cpp).block] : CopyDesc{0, 0};
+    for (; item < total; item += gridDim.x) {
+        const CopyDesc d = next;
+        const LayeredItem it = layered_item(item, n, gp, cpp);
+        const uint32_t nxt = item + gridDim.x;
+        if (nxt < total) next = descs[layered_item(nxt, n, gp, cpp).block];
+        if (d.src != 0) {
+            const uint32_t r0 = it.chunk * run;
+            const uint8_t* q =
+                reinterpret_cast<const uint8_t*>(d.src + uint64_t(first_part + it.part) * stride);
+            uint8_t* dst = reinterpret_cast<uint8_t*>(parts.base[it.part] + d.dst +
+                                                      uint64_t(r0) * geo.dst_pitch);
+            read_fp8_rows(dst, q, reinterpret_cast<const float*>(q + geo.elems),
+                          r0 * geo.src_pitch + geo.src_col, min(run, geo.rows - r0), geo);
+        } else if (threadIdx.x == 0 && item < group_items && item % (gp * cpp) == 0 && status) {
+            atomicAdd(status + kStatMiss, 1u);
+        }
+        if constexpr (LAYERED) {
+            if (nxt >= total || nxt / group_items != it.group) {
+                const uint32_t lo = it.group * group_items;
+                leave_group(rel, it.group, cta_items(lo, lo + group_items, blockIdx.x, gridDim.x),
+                            group_items, kThreads);
+            }
+        }
+    }
+}
+
+int fp8_rows_resident(const void* kernel) {
+    int r = 1;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&r, kernel, kThreads, 0);
+    return r > 0 ? r : 1;
+}
+
+cudaError_t launch_kv_read_fp8_rows(const GatherLaunch& a, uint32_t elems, cudaStream_t stream) {
+    const bool layered = a.group_flags != nullptr;
+    if (layered && !a.group_counters) return cudaErrorInvalidValue;
+    static const int res = fp8_rows_resident(reinterpret_cast<const void*>(kv_read_fp8_rows_kernel<false>));
+    static const int res_layered =
+        fp8_rows_resident(reinterpret_cast<const void*>(kv_read_fp8_rows_kernel<true>));
+    const int r = layered ? res_layered : res;
+    const LaunchPlan p = plan_gather_fp8_rows(a, elems, sm_count(), {r, r});
+    if (!p.valid) return cudaErrorInvalidValue;  // the caller checks the geometry and splits
+    GatherParts parts;
+    std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
+    const Fp8Rows geo{a.rows, a.row_bytes / 16, a.src_pitch / 2, a.src_col / 2, a.dst_pitch, elems};
+    const uint64_t stride = fp8_gather_bytes(1, elems);
+    const GroupRelease rel{a.group_flags, a.group_counters, a.group_seq, a.group_parts};
+    const auto go = [&](auto* kernel) {
+        kernel<<<p.ctas, kThreads, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.first_part, geo,
+                                                p.chunk, p.cpb, stride, a.status, rel);
+        return cudaGetLastError();
+    };
+    return layered ? go(kv_read_fp8_rows_kernel<true>) : go(kv_read_fp8_rows_kernel<false>);
+}
+
 }  // namespace
 
 cudaError_t launch_kv_write_fp8(const Fp8Launch& a, cudaStream_t stream) {
@@ -315,7 +427,8 @@ cudaError_t launch_kv_read_fp8(const Fp8Launch& a, cudaStream_t stream) {
 cudaError_t launch_kv_gather_fp8(const GatherLaunch& a, uint32_t elems, int variant,
                                  cudaStream_t stream) {
     if (a.n == 0) return cudaSuccess;
-    if (!a.part_base || a.rows) return cudaErrorInvalidValue;  // no row-sliced fp8 reads
+    if (!a.part_base) return cudaErrorInvalidValue;
+    if (a.rows) return launch_kv_read_fp8_rows(a, elems, stream);
     // a layered read takes the ld/st kernel whatever the variant (no layered pipeline)
     const bool layered = a.group_flags != nullptr;
     if (layered && (a.write || !a.group_counters || !a.group_parts || a.nparts % a.group_parts))

@@ -3,7 +3,7 @@
 // kv_fp8.cu, kv_fp8_pipe.cu) pass in the SM count and the CTAs per SM the ld/st kernels keep
 // resident (occupancy API), so the choice is unit-tested on the CPU
 // (_infinistore.testing.plan_copy / plan_gather / plan_read_fused / plan_fp8 /
-// plan_gather_fp8 / plan_gather_layered / plan_gather_rows).
+// plan_gather_fp8 / plan_gather_layered / plan_gather_rows / plan_gather_fp8_rows).
 #pragma once
 
 #include <algorithm>
@@ -361,6 +361,35 @@ inline LaunchPlan plan_gather_fp8(const GatherLaunch& a, uint32_t elems, int var
     f.variant = variant == kFp8LdSt ? kFp8LdSt : kFp8Auto;
     LaunchPlan p = plan_fp8(f, sms);
     if (parts * p.cpb > kMaxItems) return invalid_plan();
+    return p;
+}
+
+// ---------------------------------------------------------------- row-sliced fp8 reads
+// kv_read_fp8_rows (launch_kv_gather_fp8 with GatherLaunch::rows), plain or layered.  The
+// geometry is plan_gather_rows' and counts bytes of the part's bf16 view (part_bytes == rows *
+// src_pitch == 2 * elems); elems is a multiple of 512, and row_bytes, both pitches, src_col,
+// the part bases and the local offsets are multiples of 16 bytes, so every 8-element vector is
+// one 8-byte e4m3 load inside one 128-element scale group and one 16-byte store.  Runs of rows
+// as in plan_gather_rows (about kLdStChunk of destination bytes, or all of a part's rows under
+// ldst_items' rule).  The grid follows the ld/st residency rule: one wave of the CTAs the
+// kernel keeps resident (res.r16, the occupancy API's answer for it).
+inline LaunchPlan plan_gather_fp8_rows(const GatherLaunch& a, uint32_t elems, int sms,
+                                       LdStResident res) {
+    if (a.write || a.rows == 0 || a.row_bytes == 0 || a.nparts == 0 ||
+        a.nparts > kGatherMaxParts || uint64_t(a.src_col) + a.row_bytes > a.src_pitch ||
+        uint64_t(a.rows) * a.src_pitch != a.part_bytes ||
+        (a.group_flags && (a.group_parts == 0 || a.nparts % a.group_parts != 0)))
+        return invalid_plan();
+    if (elems == 0 || elems % 512 != 0 || uint64_t(a.part_bytes) != 2ull * elems ||
+        ((a.align_or | a.row_bytes | a.src_pitch | a.src_col | a.dst_pitch) & 15) != 0)
+        return invalid_plan();
+    LaunchPlan p;
+    p.kernel = Kernel::kLdStFp8;
+    const uint64_t parts = uint64_t(a.n) * a.nparts;
+    ldst_items(p, parts, a.rows, std::max(1u, kLdStChunk / a.row_bytes),
+               std::max(1u, (1u << 20) / a.row_bytes), sms);
+    if (parts * p.cpb > kMaxItems) return invalid_plan();
+    p.ctas = clamp_grid(a.max_ctas > 0 ? a.max_ctas : res.r16 * sms, parts * p.cpb);
     return p;
 }
 

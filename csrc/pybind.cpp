@@ -1027,7 +1027,7 @@ PYBIND11_MODULE(_infinistore, m) {
            uint64_t recs, uint64_t table, uint64_t table_mask, uint64_t done, uint64_t status,
            uint64_t align_or, uint64_t layer_state, uint32_t layer_parts, bool layer_claim,
            uint64_t group_flags, uint64_t group_counters, uint32_t group_seq,
-           uint32_t group_parts) {
+           uint32_t group_parts, const std::vector<uint32_t>& rows) {
             if (part_base.empty() || part_base.size() > kernels::kGatherMaxParts)
                 throw std::runtime_error("kv_gather_fp8: 1 to GATHER_MAX_PARTS parts");
             if (layer_state && first_part + part_base.size() > layer_parts)
@@ -1057,6 +1057,15 @@ PYBIND11_MODULE(_infinistore, m) {
             G.group_counters = as_ptr<uint32_t>(group_counters);
             G.group_seq = group_seq;
             G.group_parts = group_parts;
+            if (!rows.empty()) {  // bytes of the parts' bf16 view: part_bytes is 2 * elems
+                if (rows.size() != 5) throw std::runtime_error("kv_gather_fp8: rows is 5 values");
+                G.part_bytes = 2 * elems;
+                G.rows = rows[0];
+                G.row_bytes = rows[1];
+                G.src_pitch = rows[2];
+                G.src_col = rows[3];
+                G.dst_pitch = rows[4];
+            }
             const cudaError_t e =
                 kernels::launch_kv_gather_fp8(G, elems, variant, as_ptr<CUstream_st>(stream));
             if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
@@ -1068,9 +1077,12 @@ PYBIND11_MODULE(_infinistore, m) {
         py::arg("align_or") = 0, py::arg("layer_state") = 0, py::arg("layer_parts") = 0,
         py::arg("layer_claim") = false, py::arg("group_flags") = 0, py::arg("group_counters") = 0,
         py::arg("group_seq") = 0, py::arg("group_parts") = 0,
+        py::arg("rows") = std::vector<uint32_t>{},
         "gathered fp8 blocks: descs as for kv_gather; part s (elems bf16 elements at "
         "part_base[s] + local offset) <-> fp8 page first_part + s of the block; layer_* and "
-        "group_* as for kv_gather (a layered read always runs the ld/st kernel)");
+        "group_* as for kv_gather (a layered read always runs the ld/st kernel); rows (reads) "
+        "as for kv_gather, in bytes of the parts' bf16 view: those rows of each fp8 page, "
+        "dequantised (kv_read_fp8_rows)");
     k.def(
         "stream_wait_value",
         [](uint64_t addr, uint32_t value, uint64_t stream) {
@@ -1674,6 +1686,36 @@ PYBIND11_MODULE(_infinistore, m) {
           },
           py::arg("n"), py::arg("nparts"), py::arg("elems"), py::arg("variant") = 0,
           py::arg("align_or") = 0, py::arg("max_ctas") = 0, py::arg("sm_count") = 132);
+    t.def("plan_gather_fp8_rows",
+          [plan_dict](uint32_t n, uint32_t nparts, uint32_t elems, uint32_t rows,
+                      uint32_t row_bytes, uint32_t src_pitch, uint32_t src_col, uint32_t dst_pitch,
+                      uint64_t align_or, uint32_t group_parts, bool write, int max_ctas,
+                      int sm_count, int resident) {
+              static uint32_t flags[1];  // the plan only asks whether the read is layered
+              kernels::GatherLaunch a;
+              a.n = n;
+              a.nparts = nparts;
+              a.write = write;
+              a.part_bytes = uint32_t(uint64_t(rows) * src_pitch);
+              a.rows = rows;
+              a.row_bytes = row_bytes;
+              a.src_pitch = src_pitch;
+              a.src_col = src_col;
+              a.dst_pitch = dst_pitch;
+              a.align_or = align_or;
+              a.group_flags = group_parts ? flags : nullptr;
+              a.group_parts = group_parts;
+              a.max_ctas = max_ctas;
+              return plan_dict(
+                  kernels::plan_gather_fp8_rows(a, elems, sm_count, {resident, resident}));
+          },
+          py::arg("n"), py::arg("nparts"), py::arg("elems"), py::arg("rows"), py::arg("row_bytes"),
+          py::arg("src_pitch"), py::arg("src_col") = 0, py::arg("dst_pitch") = 0,
+          py::arg("align_or") = 0, py::arg("group_parts") = 0, py::arg("write") = false,
+          py::arg("max_ctas") = 0, py::arg("sm_count") = 132, py::arg("resident") = 1);
+    t.def("fp8_rows_read_bytes", &fp8_rows_read_bytes, py::arg("rows"), py::arg("row_bytes"),
+          py::arg("src_pitch"), py::arg("src_col") = 0,
+          "bytes_read of a row-sliced read of one stored fp8 part (geometry in bf16 bytes)");
     py::class_<MM>(t, "MM")
         .def(py::init<>())
         .def("add_pool", &MM::add_pool)

@@ -670,7 +670,8 @@ class InfinityConnection:
         ndarray; ``nblocks`` of them when given), in a parts list ``[(tensor, base), ...]``, of
         blocks that hold ``block_parts`` parts (default ``first_part + len(parts)``).  ``fp8``:
         the parts are bf16 CUDA tensors, ``part_size`` is a multiple of 512 elements and every
-        part base and offset is 16-byte aligned.  ``rows``: a row-sliced read.  Returns
+        part base and offset is 16-byte aligned.  ``rows``: a row-sliced read (with ``fp8``,
+        its geometry in multiples of 8 elements).  Returns
         (absolute byte address of every part, device ordinal or -1, element size, int64
         offsets, stream handle)."""
         if self._mode != "rdma":
@@ -721,6 +722,11 @@ class InfinityConnection:
             if part_size % 512:
                 raise ValueError(f"fp8 gathered blocks need a part_size that is a multiple of "
                                  f"512 elements, not {part_size}")
+            if rows is not None and any(v % 8 for v in (rows.width, rows.src_pitch,
+                                                         rows.src_offset, rows.dst_pitch)):
+                raise ValueError(f"{rows}: row-sliced reads of fp8 blocks need width, "
+                                 f"src_pitch, src_offset and dst_pitch in multiples of 8 "
+                                 f"elements (one 16-byte vector)")
             align = 0
             for b in bases:
                 align |= b
@@ -818,19 +824,27 @@ class InfinityConnection:
         return 0
 
     def read_cache_scatter_fp8(self, parts, blocks, part_size: int, first_part: int = 0,
-                               stream="current"):
+                               stream="current", rows: "PartRows | None" = None):
         """Read blocks written by ``rdma_write_cache_gather_fp8``: fp8 page ``first_part + s``
         of every block is dequantised into part ``s`` (``blocks``, misses and ``first_part`` as
         for ``read_cache_scatter``).  With ``device_lookup`` a stored block shorter than
         ``fp8_gather_block_bytes(first_part + len(parts), part_size)`` is a miss.  The same
-        checks as ``rdma_write_cache_gather_fp8``."""
+        checks as ``rdma_write_cache_gather_fp8``.
+
+        ``rows`` (a :class:`PartRows` over the ``part_size`` bf16 elements of a part) reads
+        only those rows, as ``read_cache_scatter(rows=...)`` does, dequantising each with its
+        128-element group's scale: the result is bit for bit the same rows of a whole-part
+        read.  ``width``, ``src_pitch``, ``src_offset`` and ``dst_pitch`` must be multiples of 8
+        elements; rows need not line up with the scale groups."""
         keys, offs = _split_blocks(blocks)
         bases, dev, es, offs, s = self._gather_parts(parts, offs, part_size, first_part,
-                                                     fp8=True, nblocks=len(keys), stream=stream)
+                                                     fp8=True, rows=rows, nblocks=len(keys),
+                                                     stream=stream)
+        native_rows = rows.native(es) if rows is not None else []
         if not len(offs):
             return
         ret = self.conn.r_rdma_scatter(bases, int(part_size) * es, int(part_size), int(first_part),
-                                       (keys, offs), dev, s, es)
+                                       (keys, offs), dev, s, es, native_rows)
         if ret < 0:
             raise Exception(f"Failed to read to infinistore, ret = {ret}: {self.conn.last_error()}")
 
@@ -852,9 +866,7 @@ class InfinityConnection:
         read's post-copy index check: when ``sync()`` reports a miss, treat the whole read as
         failed, as for any read.  A missing key on a connection without ``device_lookup``
         raises here; the exception's ``read`` attribute is the failed reader.  ``rows`` as for
-        ``read_cache_scatter`` (not with ``fp8``)."""
-        if rows is not None and fp8:
-            raise ValueError("row-sliced reads of fp8 blocks are not supported")
+        ``read_cache_scatter[_fp8]``."""
         keys, offs = _split_blocks(blocks)
         bases, dev, es, offs, s = self._gather_parts(parts, offs, part_size, first_part,
                                                      fp8=fp8, rows=rows, nblocks=len(keys),

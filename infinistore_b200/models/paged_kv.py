@@ -97,9 +97,14 @@ class PagedKVCache:
     def _parts(self, layers: range):
         return [(self.data, self.page_offset(layer, kv, 0)) for layer in layers for kv in (0, 1)]
 
-    def _check_fp8(self):
+    def _check_fp8(self, cross_tp: bool = False):
         if self.data.dtype != torch.bfloat16 or self.data.device.type != "cuda":
             raise ValueError("fp8 all-layer pages need a bf16 cache on a CUDA device")
+        # a cross-TP read dequantises each source's heads in 8-element vectors; a head need
+        # not fill a 128-element scale group
+        if cross_tp and self.layout.head_dim % 8:
+            raise ValueError(f"fp8 pages written at another TP degree need a head_dim that is "
+                             f"a multiple of 8, not {self.layout.head_dim}")
 
     def write_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
                     stream="current", fp8: bool = False) -> int:
@@ -138,13 +143,9 @@ class PagedKVCache:
         offs = np.asarray(pages, dtype=np.int64) * elems
         return PageWriter(self, conn.gather_writer(blocks, offs, nparts, elems, fp8=fp8))
 
-    def _cross_tp(self, source_tp: Optional[int], fp8: bool = False) -> bool:
-        """Whether a read of pages written at ``source_tp`` regroups heads (checked)."""
-        if source_tp is None or int(source_tp) == self.layout.tp:
-            return False
-        if fp8:
-            raise ValueError("pages written at another TP degree cannot be read as fp8")
-        return True
+    def _cross_tp(self, source_tp: Optional[int]) -> bool:
+        """Whether a read of pages written at ``source_tp`` regroups heads."""
+        return source_tp is not None and int(source_tp) != self.layout.tp
 
     def _sources(self, pages: Sequence[int], page_hashes: Sequence[str], source_tp: int):
         """The blocks of a read of pages written at ``source_tp``: one per (page, source
@@ -186,17 +187,19 @@ class PagedKVCache:
         (``kv_layout.tp_sources``), in one call: the read kernel copies each source's heads,
         token by token, straight into this cache.  Any missing source fails the read (it
         raises, or with ``device_lookup`` ``sync()`` reports the miss); its heads are left
-        untouched, so treat every page of a failed read as not read.  Not with ``fp8``.
-        Returns the number of (page, source) blocks read."""
-        cross = self._cross_tp(source_tp, fp8)
+        untouched, so treat every page of a failed read as not read.  With ``fp8`` the read
+        kernel dequantises each source's heads out of its fp8 pages in the same way
+        (``head_dim`` a multiple of 8).  Returns the number of (page, source) blocks read."""
+        cross = self._cross_tp(source_tp)
         if fp8:
-            self._check_fp8()
+            self._check_fp8(cross)
         self._ensure_registered(conn)
         layers = self._check_layers(layers)
         if cross:
             keys, offs, rows, part = self._sources(pages, page_hashes, source_tp)
-            conn.read_cache_scatter(self._parts(layers), (keys, offs), part,
-                                    first_part=2 * layers.start, stream=stream, rows=rows)
+            read = conn.read_cache_scatter_fp8 if fp8 else conn.read_cache_scatter
+            read(self._parts(layers), (keys, offs), part, first_part=2 * layers.start,
+                 stream=stream, rows=rows)
             return len(keys)
         keys = self.page_keys(page_hashes)
         offs = np.asarray(pages, dtype=np.int64) * self.layout.page_elems
@@ -214,16 +217,16 @@ class PagedKVCache:
         arrived, with no host synchronisation.  ``layers`` (a step-1 range, default all),
         ``fp8`` and ``source_tp`` as for ``read_pages``.  A layer is released before the
         read's post-copy index check: when ``sync()`` reports a miss, the whole read failed."""
-        cross = self._cross_tp(source_tp, fp8)
+        cross = self._cross_tp(source_tp)
         if fp8:
-            self._check_fp8()
+            self._check_fp8(cross)
         self._ensure_registered(conn)
         layers = self._check_layers(layers)
         if cross:
             keys, offs, rows, part = self._sources(pages, page_hashes, source_tp)
             read = conn.read_cache_scatter_layered(self._parts(layers), (keys, offs), part,
                                                    group_parts=2, first_part=2 * layers.start,
-                                                   stream=stream, rows=rows)
+                                                   fp8=fp8, stream=stream, rows=rows)
             return PageRead(read, layers)
         keys = self.page_keys(page_hashes)
         offs = np.asarray(pages, dtype=np.int64) * self.layout.page_elems

@@ -334,14 +334,19 @@ def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, wri
                   first_part: int = 0, max_ctas: int = 0, status: Optional[torch.Tensor] = None,
                   align_or: int = 0, publish: Optional[PublishArgs] = None,
                   variant: str = "auto", layer: Optional[LayerState] = None,
-                  claim: bool = False, release: Optional[GroupRelease] = None) -> None:
+                  claim: bool = False, release: Optional[GroupRelease] = None,
+                  rows: Optional[Sequence[int]] = None) -> None:
     """Gathered fp8 blocks (``kv_gather`` with quantisation): part s of block i is a bf16 page
     of ``elems`` elements at ``part_base[s] + local offset`` and fp8 page first_part + s of
     the block, at byte ``fp8_gather_bytes(first_part + s, elems)``.  ``descs``, ``layer`` and
     ``claim`` as for ``kv_gather``.  ``variant``: "ldst" = the ld/st kernels (kv_fp8.cu),
     "auto" / "tma" = the TMA pipeline (kv_fp8_pipe.cu).  ``align_or`` must include the local
     offsets (the part bases are added here): unaligned batches are refused.  ``release`` as for
-    ``kv_gather`` (a layered read always runs the ld/st kernel)."""
+    ``kv_gather`` (a layered read always runs the ld/st kernel).  A read with ``rows`` =
+    (rows, row_bytes, src_pitch, src_col, dst_pitch), in bytes of the part's bf16 view
+    (``rows * src_pitch == 2 * elems``, every value a multiple of 16), dequantises only those
+    rows (kv_read_fp8_rows, whatever the variant): row r from bf16 byte
+    ``r * src_pitch + src_col`` of the page -> part s's destination + ``r * dst_pitch``."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
     bases = [int(b) for b in part_base]
     for b in bases:
@@ -352,7 +357,8 @@ def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, wri
                         FP8_VARIANTS["ldst"] if variant == "ldst" else FP8_VARIANTS["auto"],
                         max_ctas, _stream(descs.device), *pub,
                         status.data_ptr() if status is not None else 0, align_or, *lay,
-                        *_release_args(release))
+                        *_release_args(release),
+                        [int(r) for r in rows] if rows is not None else [])
 
 
 def fp8_reference(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
