@@ -205,8 +205,10 @@ class Connection {
         ScatterReader* reader = nullptr;
         uint32_t group_parts = 0;
         // reads: row-sliced parts (kernels::GatherLaunch::rows, bytes of the caller's view of a
-        // part, view_part_bytes()); rows == 0: whole parts
+        // part, view_part_bytes()); rows == 0: whole parts.  slices > 1: sliced rows
+        // (kernels::GatherLaunch::slices), e.g. a token's KV heads into a head-major page
         uint32_t rows = 0, row_bytes = 0, src_pitch = 0, src_col = 0, dst_pitch = 0;
+        uint32_t slices = 1, dst_slice_pitch = 0;
         // pool bytes of a part: part_bytes, or kernels::fp8_gather_bytes(1, fp8_elems)
         uint64_t pool_part_bytes() const;
         // bytes of a part in the caller's tensors: part_bytes, or 2 * fp8_elems (bf16)
@@ -253,9 +255,10 @@ class Connection {
     int w_rdma_gather(const GatherSpec& g, const uint64_t* offsets, size_t noffsets,
                       const RemoteBlock* blocks, size_t nblocks, int device, uint64_t stream);
     // A stored block must hold g.need_bytes() bytes, else it is a miss.  Row-sliced (g.rows):
-    // rows >= 1, src_col + row_bytes <= src_pitch and g.view_part_bytes() == rows * src_pitch;
-    // fp8 parts also need row_bytes, both pitches and src_col in multiples of 16 bytes (the
-    // rows are picked out of the part's bf16 view and dequantised).  With g.reader, a layered read: one call whose last page-mover launch
+    // the geometry kernels::row_geometry_ok accepts for g.view_part_bytes() (launch_plan.h);
+    // fp8 parts also need row_bytes, both pitches, src_col and, with slices > 1,
+    // dst_slice_pitch in multiples of 16 bytes (the rows are picked out of the part's bf16
+    // view and dequantised).  With g.reader, a layered read: one call whose last page-mover launch
     // releases the parts group by group, each by storing `seq` to its flag word, and each key
     // is resolved once; CUDA tensors of an HBM pool only, not on a doorbell connection, and on
     // failure the reader is failed.  Every refusal comes before anything is enqueued.

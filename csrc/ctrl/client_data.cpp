@@ -13,6 +13,7 @@
 #include "../core/log.h"
 #include "../core/trace.h"
 #include "../kernels/kernels.h"
+#include "../kernels/launch_plan.h"
 #include "../wire/messages.h"
 #include "client_dev.h"
 #include "read_plan.h"
@@ -293,16 +294,20 @@ kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n,
     G.src_pitch = g.src_pitch;
     G.src_col = g.src_col;
     G.dst_pitch = g.dst_pitch;
+    G.slices = g.slices;
+    G.dst_slice_pitch = g.dst_slice_pitch;
     return G;
 }
 
 // Bytes one block of a gathered call moves: its parts, or their rows when row-sliced (of fp8
-// parts: the pool bytes of those rows, read_plan.h: fp8_rows_read_bytes).
+// parts: the pool bytes of those rows, read_plan.h: fp8_rows_read_bytes; a row's slices are
+// adjacent in the stored row, so they count as one run of slices * row_bytes).
 static uint64_t gather_moved_bytes(const Connection::GatherSpec& g) {
+    const uint64_t width = uint64_t(g.slices) * g.row_bytes;
     const uint64_t part = !g.rows ? g.pool_part_bytes()
                           : g.fp8_elems
-                              ? fp8_rows_read_bytes(g.rows, g.row_bytes, g.src_pitch, g.src_col)
-                              : uint64_t(g.rows) * g.row_bytes;
+                              ? fp8_rows_read_bytes(g.rows, uint32_t(width), g.src_pitch, g.src_col)
+                              : uint64_t(g.rows) * width;
     return uint64_t(g.nparts) * part;
 }
 
@@ -417,7 +422,7 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
                 auto m = mapping(addr_seg(blocks[i].remote_addr), -1);
                 if (!m || !m->host_ptr) return -1;
                 uint8_t* pool = m->host_ptr + addr_off(blocks[i].remote_addr);
-                if (gather) {  // one memcpy per part, or per row of a row-sliced read
+                if (gather) {  // one memcpy per part, or per (row, slice) of a row-sliced read
                     const size_t pb = gather->pool_part_bytes();
                     const Connection::GatherSpec& g = *gather;
                     for (uint32_t s = 0; s < gather->nparts; ++s) {
@@ -426,8 +431,12 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
                         if (g.rows) {
                             const uint8_t* src = pool + (g.first_part + s) * pb + g.src_col;
                             for (uint32_t r = 0; r < g.rows; ++r)
-                                std::memcpy(local + size_t(r) * g.dst_pitch,
-                                            src + size_t(r) * g.src_pitch, g.row_bytes);
+                                for (uint32_t j = 0; j < g.slices; ++j)
+                                    std::memcpy(local + size_t(r) * g.dst_pitch +
+                                                    size_t(j) * g.dst_slice_pitch,
+                                                src + size_t(r) * g.src_pitch +
+                                                    size_t(j) * g.row_bytes,
+                                                g.row_bytes);
                         } else if (write)
                             std::memcpy(pool + (gather->first_part + s) * pb, local, pb);
                         else
@@ -866,13 +875,17 @@ const char* Connection::gather_refusal(const GatherSpec& g, const uint64_t* offs
     if (end > block_parts) return "the part range runs past the block";
     if (block_parts > uint64_t(INT32_MAX) / g.pool_part_bytes())
         return "bad parts list: a block holds at most 2^31 - 1 bytes";
-    if (g.rows && (write || !g.row_bytes || uint64_t(g.src_col) + g.row_bytes > g.src_pitch ||
-                   uint64_t(g.rows) * g.src_pitch != g.view_part_bytes()))
-        return "bad row geometry (reads only, rows >= 1, src_col + row_bytes <= src_pitch, "
-               "part_bytes == rows * src_pitch)";
-    if (g.rows && g.fp8_elems && ((g.row_bytes | g.src_pitch | g.src_col | g.dst_pitch) & 15))
-        return "bad row geometry for fp8 parts: row_bytes, src_pitch, src_col and dst_pitch "
-               "must be multiples of 16 bytes (8 bf16 elements)";
+    if (g.rows && (write || !kernels::row_geometry_ok(g.rows, g.row_bytes, g.src_pitch,
+                                                      g.src_col, g.dst_pitch, g.slices,
+                                                      g.dst_slice_pitch, g.view_part_bytes())))
+        return "bad row geometry (reads only, rows >= 1, slices >= 1, src_col + slices * "
+               "row_bytes <= src_pitch, part_bytes == rows * src_pitch; with slices > 1, "
+               "disjoint destination slices within 2^32 bytes)";
+    if (g.rows && g.fp8_elems &&
+        ((g.row_bytes | g.src_pitch | g.src_col | g.dst_pitch |
+          (g.slices > 1 ? g.dst_slice_pitch : 0u)) & 15))
+        return "bad row geometry for fp8 parts: row_bytes, src_pitch, src_col, dst_pitch and "
+               "dst_slice_pitch must be multiples of 16 bytes (8 bf16 elements)";
     if (g.reader) {
         if (!g.group_parts || g.nparts % g.group_parts)
             return "a layered read needs group_parts that divides the part count";

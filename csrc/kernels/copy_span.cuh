@@ -72,12 +72,62 @@ __device__ __forceinline__ void copy_span(uint8_t* dst, const uint8_t* src, uint
 // threads walk the (row, vector) pairs flattened together, so rows much narrower than a CTA's
 // 4 KB per pass (one KV head of 128 bf16 is 256 bytes) still keep every thread busy.  VEC = 16
 // / 32 as for copy_span (row_bytes, both pitches and both bases aligned to VEC); VEC = 1: bytes.
-template <int VEC>
+// SLICED (GatherLaunch::slices > 1): src and dst are the part's stored start and destination,
+// and the nrows units are the (slice, row) pairs sl.q0 .. sl.q0 + nrows - 1 of the part, each
+// placed by slice_pair (launch_plan.h): the threads walk (slice, row, vector) triples flattened
+// together (sl.slice_pitch aligned to VEC as well).
+struct RowSlices {
+    uint32_t q0, rows, src_col, slice_pitch;
+};
+template <int VEC, bool SLICED = false>
 __device__ __forceinline__ void copy_rows(uint8_t* dst, const uint8_t* src, uint32_t nrows,
                                           uint32_t row_bytes, uint32_t src_pitch,
-                                          uint32_t dst_pitch) {
+                                          uint32_t dst_pitch, RowSlices sl = {}) {
     const uint32_t tid = threadIdx.x;
-    if constexpr (VEC == 1) {
+    if constexpr (SLICED) {
+        // pair p of the run: offsets of its byte c from src and dst
+        const auto at = [&](uint32_t p, uint32_t c) {
+            PairOffsets o = slice_pair(sl.q0 + p, sl.rows, row_bytes, src_pitch, sl.src_col,
+                                       dst_pitch, sl.slice_pitch);
+            o.src += c;
+            o.dst += c;
+            return o;
+        };
+        if constexpr (VEC == 1) {
+            const uint32_t len = nrows * row_bytes;
+            for (uint32_t b = tid; b < len; b += kLdStThreads) {
+                const uint32_t p = b / row_bytes;
+                const PairOffsets o = at(p, b - p * row_bytes);
+                dst[o.dst] = src[o.src];
+            }
+        } else {
+            static_assert(VEC == 16 || VEC == 32, "vector width");
+            constexpr int U = VEC / 4;
+            const uint32_t vpr = row_bytes / 16;
+            const uint32_t nvec = nrows * vpr;
+            const auto vec_at = [&](uint32_t v) {
+                const uint32_t p = v / vpr;
+                return at(p, (v - p * vpr) * 16);
+            };
+            uint32_t i = tid;
+            for (; i + (U - 1) * kLdStThreads < nvec; i += U * kLdStThreads) {
+                uint4 v[U];
+                uint32_t out[U];
+#pragma unroll
+                for (int u = 0; u < U; ++u) {
+                    const PairOffsets o = vec_at(i + u * kLdStThreads);
+                    v[u] = VEC == 16 ? ld_stream_v4(src + o.src) : ld_v4(src + o.src);
+                    out[u] = o.dst;
+                }
+#pragma unroll
+                for (int u = 0; u < U; ++u) st_v4(dst + out[u], v[u]);
+            }
+            for (; i < nvec; i += kLdStThreads) {
+                const PairOffsets o = vec_at(i);
+                st_v4(dst + o.dst, ld_stream_v4(src + o.src));
+            }
+        }
+    } else if constexpr (VEC == 1) {
         const uint32_t len = nrows * row_bytes;
         for (uint32_t b = tid; b < len; b += kLdStThreads) {
             const uint32_t r = b / row_bytes, c = b - r * row_bytes;

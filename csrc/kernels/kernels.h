@@ -190,6 +190,13 @@ struct GatherLaunch {
     uint32_t src_pitch = 0;
     uint32_t src_col = 0;
     uint32_t dst_pitch = 0;
+    // Sliced rows (slices > 1): each stored row holds `slices` slices of row_bytes side by side
+    // from src_col, and slice j of row r lands at part_base[s] + desc.dst + r * dst_pitch +
+    // j * dst_slice_pitch - e.g. a token's KV heads into a head-major page [head][token][dim]
+    // (launch_plan.h: slice_pair, row_geometry_ok).  slices == 1: the rows above, and
+    // dst_slice_pitch is not read.
+    uint32_t slices = 1;
+    uint32_t dst_slice_pitch = 0;
 };
 // The TMA pipeline for 16-byte aligned parts of at least kPipeMinBytes, the ld/st kernel
 // (kv_copy.cu) otherwise: the same rule launch_kv_copy applies to whole blocks.  A row-sliced

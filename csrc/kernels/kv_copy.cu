@@ -197,12 +197,15 @@ struct RowGeometry {
 //     -> parts.base[s] + desc.dst + r * dst_pitch.
 // A missing block counts once, on its first item, and its parts are left untouched; its items
 // still count as arrivals.  No control warp: reads publish nothing.
-template <int VEC, bool LAYERED>
-__global__ void __launch_bounds__(kLdStThreads, 3)
-    kv_scatter_rows_kernel(const CopyDesc* __restrict__ descs,
-                           const __grid_constant__ GatherParts parts, uint32_t n, uint32_t nparts,
-                           uint32_t first_part, RowGeometry geo, uint32_t run, uint32_t cpp,
-                           uint32_t* status, GroupRelease rel) {
+// SLICED (kv_scatter_slices_kernel, GatherLaunch::slices > 1): a run is `run` (slice, row)
+// pairs of the part, numbered slice-major, each placed by slice_pair (launch_plan.h).
+template <int VEC, bool LAYERED, bool SLICED>
+__device__ __forceinline__ void scatter_rows(const CopyDesc* __restrict__ descs,
+                                             const GatherParts& parts, uint32_t n,
+                                             uint32_t nparts, uint32_t first_part,
+                                             const RowGeometry& geo, uint32_t slices,
+                                             uint32_t slice_pitch, uint32_t run, uint32_t cpp,
+                                             uint32_t* status, const GroupRelease& rel) {
     const uint32_t gp = LAYERED ? rel.gp : nparts;
     const uint32_t group_items = n * gp * cpp;
     const uint32_t total = n * nparts * cpp;
@@ -213,7 +216,15 @@ __global__ void __launch_bounds__(kLdStThreads, 3)
         const LayeredItem it = layered_item(item, n, gp, cpp);
         const uint32_t nxt = item + gridDim.x;
         if (nxt < total) next = descs[layered_item(nxt, n, gp, cpp).block];
-        if (d.src != 0) {
+        if (d.src != 0 && SLICED) {
+            const uint32_t q0 = it.chunk * run;
+            const uint8_t* src = reinterpret_cast<const uint8_t*>(
+                d.src + uint64_t(first_part + it.part) * geo.part_bytes);
+            uint8_t* dst = reinterpret_cast<uint8_t*>(parts.base[it.part] + d.dst);
+            copy_rows<VEC, true>(dst, src, min(run, geo.rows * slices - q0), geo.row_bytes,
+                                 geo.src_pitch, geo.dst_pitch,
+                                 RowSlices{q0, geo.rows, geo.src_col, slice_pitch});
+        } else if (d.src != 0) {
             const uint32_t r0 = it.chunk * run;
             const uint8_t* src = reinterpret_cast<const uint8_t*>(
                 d.src + uint64_t(first_part + it.part) * geo.part_bytes +
@@ -235,18 +246,72 @@ __global__ void __launch_bounds__(kLdStThreads, 3)
     }
 }
 
+template <int VEC, bool LAYERED>
+__global__ void __launch_bounds__(kLdStThreads, 3)
+    kv_scatter_rows_kernel(const CopyDesc* __restrict__ descs,
+                           const __grid_constant__ GatherParts parts, uint32_t n, uint32_t nparts,
+                           uint32_t first_part, RowGeometry geo, uint32_t run, uint32_t cpp,
+                           uint32_t* status, GroupRelease rel) {
+    scatter_rows<VEC, LAYERED, false>(descs, parts, n, nparts, first_part, geo, 1, 0, run, cpp,
+                                      status, rel);
+}
+
+// GatherLaunch::slices > 1: runs of (slice, row) pairs (scatter_rows above).
+template <int VEC, bool LAYERED>
+__global__ void __launch_bounds__(kLdStThreads, 3)
+    kv_scatter_slices_kernel(const CopyDesc* __restrict__ descs,
+                             const __grid_constant__ GatherParts parts, uint32_t n,
+                             uint32_t nparts, uint32_t first_part, RowGeometry geo,
+                             uint32_t slices, uint32_t slice_pitch, uint32_t run, uint32_t cpp,
+                             uint32_t* status, GroupRelease rel) {
+    scatter_rows<VEC, LAYERED, true>(descs, parts, n, nparts, first_part, geo, slices,
+                                     slice_pitch, run, cpp, status, rel);
+}
+
+cudaError_t launch_kv_scatter_slices(const GatherLaunch& a, const LaunchPlan& p,
+                                     const GatherParts& parts, const RowGeometry& geo,
+                                     const GroupRelease& rel, cudaStream_t stream) {
+    const bool layered = a.group_flags != nullptr;
+    const auto go = [&](auto* kernel) {
+        kernel<<<p.ctas, kLdStThreads, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.first_part,
+                                                    geo, a.slices, a.dst_slice_pitch, p.chunk,
+                                                    p.cpb, a.status, rel);
+        return cudaGetLastError();
+    };
+    switch (p.kernel) {
+        case Kernel::kLdSt1:
+            return layered ? go(kv_scatter_slices_kernel<1, true>)
+                           : go(kv_scatter_slices_kernel<1, false>);
+        case Kernel::kLdSt32:
+            return layered ? go(kv_scatter_slices_kernel<32, true>)
+                           : go(kv_scatter_slices_kernel<32, false>);
+        default:
+            return layered ? go(kv_scatter_slices_kernel<16, true>)
+                           : go(kv_scatter_slices_kernel<16, false>);
+    }
+}
+
 cudaError_t launch_kv_scatter_rows(const GatherLaunch& a, cudaStream_t stream) {
     static const LdStResident res = ldst_resident(kv_scatter_rows_kernel<16, false>,
                                                   kv_scatter_rows_kernel<32, false>, kLdStThreads);
     static const LdStResident res_layered = ldst_resident(
         kv_scatter_rows_kernel<16, true>, kv_scatter_rows_kernel<32, true>, kLdStThreads);
+    static const LdStResident res_sliced = ldst_resident(
+        kv_scatter_slices_kernel<16, false>, kv_scatter_slices_kernel<32, false>, kLdStThreads);
+    static const LdStResident res_sliced_layered = ldst_resident(
+        kv_scatter_slices_kernel<16, true>, kv_scatter_slices_kernel<32, true>, kLdStThreads);
     const bool layered = a.group_flags != nullptr;
-    const LaunchPlan p = plan_gather_rows(a, sm_count(), layered ? res_layered : res);
+    const bool sliced = a.slices > 1;
+    const LaunchPlan p = plan_gather_rows(a, sm_count(),
+                                          sliced ? (layered ? res_sliced_layered : res_sliced)
+                                          : layered ? res_layered
+                                                    : res);
     if (!p.valid) return cudaErrorInvalidValue;  // the caller checks the geometry and splits
     GatherParts parts;
     std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
     const RowGeometry geo{a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.part_bytes};
     const GroupRelease rel{a.group_flags, a.group_counters, a.group_seq, a.group_parts};
+    if (sliced) return launch_kv_scatter_slices(a, p, parts, geo, rel, stream);
     const auto go = [&](auto* kernel) {
         kernel<<<p.ctas, kLdStThreads, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.first_part,
                                                     geo, p.chunk, p.cpb, a.status, rel);

@@ -303,10 +303,40 @@ constexpr int kRowVecs = 4;  // (row, vector) pairs in flight per thread: 4 x 16
 // (copy_span.cuh) does, so one 128-element KV head (16 vectors) per row keeps every thread
 // busy.  A vector is 8 e4m3 bytes at q + e and the scale of its group at scales[e / 128]: the
 // geometry keeps e a multiple of 8, so a vector never straddles two scale groups.
+// SLICED (GatherLaunch::slices > 1): dst is the part's destination and the nrows units are the
+// (slice, row) pairs e0 .. e0 + nrows - 1 of the part, placed by slice_pair (launch_plan.h) with
+// slice_pitch bytes between destination slices: (slice, row, vector) triples flattened.
+template <bool SLICED = false>
 __device__ __forceinline__ void read_fp8_rows(uint8_t* dst, const uint8_t* q, const float* scales,
-                                              uint32_t e0, uint32_t nrows, const Fp8Rows& g) {
+                                              uint32_t e0, uint32_t nrows, const Fp8Rows& g,
+                                              uint32_t slice_pitch = 0) {
     const uint32_t nvec = nrows * g.vpr;
     uint32_t i = threadIdx.x;
+    if constexpr (SLICED) {
+        for (; i < nvec; i += kRowVecs * kThreads) {
+            uint2 v[kRowVecs];
+            float sc[kRowVecs];
+            uint32_t out[kRowVecs];
+#pragma unroll
+            for (int u = 0; u < kRowVecs; ++u) {
+                const uint32_t k = i + u * kThreads;
+                if (k >= nvec) continue;
+                const uint32_t p = k / g.vpr, c = k - p * g.vpr;
+                const PairOffsets o = slice_pair(e0 + p, g.rows, 8 * g.vpr, g.src_pitch,
+                                                 g.src_col, g.dst_pitch, slice_pitch);
+                const uint32_t e = o.src + 8 * c;
+                v[u] = ld_u2(q + e);
+                sc[u] = __uint_as_float(ld_u1(scales + e / kRow));
+                out[u] = o.dst + 16 * c;
+            }
+#pragma unroll
+            for (int u = 0; u < kRowVecs; ++u) {
+                if (i + u * kThreads >= nvec) continue;
+                *reinterpret_cast<uint4*>(dst + out[u]) = dequant8(v[u], sc[u]);
+            }
+        }
+        return;
+    }
     for (; i < nvec; i += kRowVecs * kThreads) {
         uint2 v[kRowVecs];
         float sc[kRowVecs];
@@ -334,13 +364,16 @@ __device__ __forceinline__ void read_fp8_rows(uint8_t* dst, const uint8_t* q, co
 // by leave_group - the numbering, miss counting and release of kv_scatter_rows_kernel
 // (kv_copy.cu).  Stored part first_part + s starts at desc.src + (first_part + s) * stride.
 // A missing block counts once, on its first item, and its parts are left untouched; its items
-// still count as arrivals.
-template <bool LAYERED>
-__global__ void __launch_bounds__(kThreads)
-    kv_read_fp8_rows_kernel(const CopyDesc* __restrict__ descs,
-                            const __grid_constant__ GatherParts parts, uint32_t n, uint32_t nparts,
-                            uint32_t first_part, Fp8Rows geo, uint32_t run, uint32_t cpp,
-                            uint64_t stride, uint32_t* status, GroupRelease rel) {
+// still count as arrivals.  SLICED (kv_read_fp8_slices_kernel, GatherLaunch::slices > 1): a
+// run is `run` (slice, row) pairs of the part, numbered slice-major.
+template <bool LAYERED, bool SLICED>
+__device__ __forceinline__ void read_fp8_row_items(const CopyDesc* __restrict__ descs,
+                                                   const GatherParts& parts, uint32_t n,
+                                                   uint32_t nparts, uint32_t first_part,
+                                                   const Fp8Rows& geo, uint32_t slices,
+                                                   uint32_t slice_pitch, uint32_t run,
+                                                   uint32_t cpp, uint64_t stride,
+                                                   uint32_t* status, const GroupRelease& rel) {
     const uint32_t gp = LAYERED ? rel.gp : nparts;
     const uint32_t group_items = n * gp * cpp;
     const uint32_t total = n * nparts * cpp;
@@ -351,7 +384,14 @@ __global__ void __launch_bounds__(kThreads)
         const LayeredItem it = layered_item(item, n, gp, cpp);
         const uint32_t nxt = item + gridDim.x;
         if (nxt < total) next = descs[layered_item(nxt, n, gp, cpp).block];
-        if (d.src != 0) {
+        if (d.src != 0 && SLICED) {
+            const uint32_t q0 = it.chunk * run;
+            const uint8_t* q =
+                reinterpret_cast<const uint8_t*>(d.src + uint64_t(first_part + it.part) * stride);
+            read_fp8_rows<true>(reinterpret_cast<uint8_t*>(parts.base[it.part] + d.dst), q,
+                                reinterpret_cast<const float*>(q + geo.elems), q0,
+                                min(run, geo.rows * slices - q0), geo, slice_pitch);
+        } else if (d.src != 0) {
             const uint32_t r0 = it.chunk * run;
             const uint8_t* q =
                 reinterpret_cast<const uint8_t*>(d.src + uint64_t(first_part + it.part) * stride);
@@ -372,6 +412,28 @@ __global__ void __launch_bounds__(kThreads)
     }
 }
 
+template <bool LAYERED>
+__global__ void __launch_bounds__(kThreads)
+    kv_read_fp8_rows_kernel(const CopyDesc* __restrict__ descs,
+                            const __grid_constant__ GatherParts parts, uint32_t n, uint32_t nparts,
+                            uint32_t first_part, Fp8Rows geo, uint32_t run, uint32_t cpp,
+                            uint64_t stride, uint32_t* status, GroupRelease rel) {
+    read_fp8_row_items<LAYERED, false>(descs, parts, n, nparts, first_part, geo, 1, 0, run, cpp,
+                                       stride, status, rel);
+}
+
+// GatherLaunch::slices > 1: runs of (slice, row) pairs (read_fp8_row_items above).
+template <bool LAYERED>
+__global__ void __launch_bounds__(kThreads)
+    kv_read_fp8_slices_kernel(const CopyDesc* __restrict__ descs,
+                              const __grid_constant__ GatherParts parts, uint32_t n,
+                              uint32_t nparts, uint32_t first_part, Fp8Rows geo, uint32_t slices,
+                              uint32_t slice_pitch, uint32_t run, uint32_t cpp, uint64_t stride,
+                              uint32_t* status, GroupRelease rel) {
+    read_fp8_row_items<LAYERED, true>(descs, parts, n, nparts, first_part, geo, slices,
+                                      slice_pitch, run, cpp, stride, status, rel);
+}
+
 int fp8_rows_resident(const void* kernel) {
     int r = 1;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&r, kernel, kThreads, 0);
@@ -384,7 +446,13 @@ cudaError_t launch_kv_read_fp8_rows(const GatherLaunch& a, uint32_t elems, cudaS
     static const int res = fp8_rows_resident(reinterpret_cast<const void*>(kv_read_fp8_rows_kernel<false>));
     static const int res_layered =
         fp8_rows_resident(reinterpret_cast<const void*>(kv_read_fp8_rows_kernel<true>));
-    const int r = layered ? res_layered : res;
+    static const int res_sliced =
+        fp8_rows_resident(reinterpret_cast<const void*>(kv_read_fp8_slices_kernel<false>));
+    static const int res_sliced_layered =
+        fp8_rows_resident(reinterpret_cast<const void*>(kv_read_fp8_slices_kernel<true>));
+    const bool sliced = a.slices > 1;
+    const int r = sliced ? (layered ? res_sliced_layered : res_sliced)
+                         : (layered ? res_layered : res);
     const LaunchPlan p = plan_gather_fp8_rows(a, elems, sm_count(), {r, r});
     if (!p.valid) return cudaErrorInvalidValue;  // the caller checks the geometry and splits
     GatherParts parts;
@@ -392,6 +460,15 @@ cudaError_t launch_kv_read_fp8_rows(const GatherLaunch& a, uint32_t elems, cudaS
     const Fp8Rows geo{a.rows, a.row_bytes / 16, a.src_pitch / 2, a.src_col / 2, a.dst_pitch, elems};
     const uint64_t stride = fp8_gather_bytes(1, elems);
     const GroupRelease rel{a.group_flags, a.group_counters, a.group_seq, a.group_parts};
+    if (sliced) {
+        const auto go = [&](auto* kernel) {
+            kernel<<<p.ctas, kThreads, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.first_part,
+                                                    geo, a.slices, a.dst_slice_pitch, p.chunk,
+                                                    p.cpb, stride, a.status, rel);
+            return cudaGetLastError();
+        };
+        return layered ? go(kv_read_fp8_slices_kernel<true>) : go(kv_read_fp8_slices_kernel<false>);
+    }
     const auto go = [&](auto* kernel) {
         kernel<<<p.ctas, kThreads, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.first_part, geo,
                                                 p.chunk, p.cpb, stride, a.status, rel);

@@ -252,26 +252,69 @@ inline LaunchPlan plan_gather_layered(const GatherLaunch& a, int sms, LdStReside
     return p;
 }
 
+// ---------------------------------------------------------------- row geometry
+// The row geometry of a row-sliced read (GatherLaunch::rows, ::slices), in bytes of the
+// caller's view of a part (part_bytes), as the connection (Connection::gather_refusal) and the
+// plans below accept it: the row's slices lie inside the stored row, the rows cover the part,
+// and with slices > 1 the destination rectangles are disjoint under one of two nestings -
+// head-major (a slice's rows inside dst_slice_pitch) or token-major (a row's slices inside
+// dst_pitch) - and the destination extent, (rows - 1) * dst_pitch + (slices - 1) *
+// dst_slice_pitch + row_bytes, fits 32 bits.  slices == 1 checks what it always did.
+inline bool row_geometry_ok(uint32_t rows, uint32_t row_bytes, uint32_t src_pitch,
+                            uint32_t src_col, uint32_t dst_pitch, uint32_t slices,
+                            uint32_t dst_slice_pitch, uint64_t part_bytes) {
+    if (rows == 0 || row_bytes == 0 || slices == 0 ||
+        uint64_t(src_col) + uint64_t(slices) * row_bytes > src_pitch ||
+        uint64_t(rows) * src_pitch != part_bytes)
+        return false;
+    if (slices == 1) return true;
+    const uint64_t rb = row_bytes, r1 = rows - 1, s1 = slices - 1;
+    const bool head_major = dst_pitch >= rb && dst_slice_pitch >= r1 * dst_pitch + rb;
+    const bool token_major = dst_slice_pitch >= rb && dst_pitch >= s1 * dst_slice_pitch + rb;
+    return (head_major || token_major) &&
+           r1 * dst_pitch + s1 * dst_slice_pitch + rb <= 0xffffffffull;
+}
+
+// Where (slice, row) pair q of a part goes: the kernels' unit of work with slices > 1.  Pairs
+// are numbered slice-major (q = j * rows + r), so a run of pairs of a head-major destination
+// writes contiguous bytes.  Slice j of row r moves `row` units from r * src_pitch + src_col +
+// j * row of the stored part to r * dst_pitch + j * dst_slice_pitch of the part's destination.
+// Units are the caller's: bytes, or for fp8 parts elements of the bf16 view on the source side
+// and bytes on the destination side.  row_geometry_ok keeps both offsets within 32 bits.  The
+// kernels (copy_span.cuh: copy_rows, kv_fp8.cu: read_fp8_rows) and the CPU tests
+// (_infinistore.testing.slice_pair) share this function.
+struct PairOffsets {
+    uint32_t src, dst;
+};
+ISTORE_KHD inline PairOffsets slice_pair(uint32_t q, uint32_t rows, uint32_t row,
+                                         uint32_t src_pitch, uint32_t src_col, uint32_t dst_pitch,
+                                         uint32_t dst_slice_pitch) {
+    const uint32_t j = q / rows, r = q - j * rows;
+    return PairOffsets{r * src_pitch + src_col + j * row, r * dst_pitch + j * dst_slice_pitch};
+}
+
 // ---------------------------------------------------------------- row-sliced reads
 // kv_scatter_rows (GatherLaunch::rows != 0), plain or layered: always the ld/st kernels (the
 // TMA pipelines have no row form).  The vector width is the one the OR of row_bytes, both
-// pitches, src_col, the part bases and the local offsets allows (pool blocks are granule
-// aligned and part_bytes is a multiple of src_pitch).  A work item is a run of `chunk` rows of
-// one part, about kLdStChunk of payload, or all of a part's rows under ldst_items' rule; cpb
-// is runs per part, and a layered read numbers items with layered_item as whole parts do.
+// pitches (with slices > 1, dst_slice_pitch too), src_col, the part bases and the local
+// offsets allows (pool blocks are granule aligned and part_bytes is a multiple of src_pitch).
+// A work item is a run of `chunk` (slice, row) pairs of one part (rows with slices == 1),
+// about kLdStChunk of payload, or all of a part's pairs under ldst_items' rule; cpb is runs per
+// part, and a layered read numbers items with layered_item as whole parts do.
 inline LaunchPlan plan_gather_rows(const GatherLaunch& a, int sms, LdStResident res) {
-    if (a.write || a.rows == 0 || a.row_bytes == 0 || a.nparts == 0 ||
-        a.nparts > kGatherMaxParts || uint64_t(a.src_col) + a.row_bytes > a.src_pitch ||
-        uint64_t(a.rows) * a.src_pitch != a.part_bytes ||
+    if (a.write || a.nparts == 0 || a.nparts > kGatherMaxParts ||
+        !row_geometry_ok(a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.slices,
+                         a.dst_slice_pitch, a.part_bytes) ||
         (a.group_flags && (a.group_parts == 0 || a.nparts % a.group_parts != 0)))
         return invalid_plan();
-    const uint64_t geo_or = a.align_or | a.src_pitch | a.src_col | a.dst_pitch;
+    const uint64_t geo_or = a.align_or | a.src_pitch | a.src_col | a.dst_pitch |
+                            (a.slices > 1 ? a.dst_slice_pitch : 0u);
     const bool aligned16 = aligned_to(a.row_bytes, geo_or, 16);
     const bool aligned32 = aligned_to(a.row_bytes, geo_or, 32);
     LaunchPlan p;
     p.kernel = !aligned16 ? Kernel::kLdSt1 : aligned32 ? Kernel::kLdSt32 : Kernel::kLdSt16;
     const uint64_t parts = uint64_t(a.n) * a.nparts;
-    ldst_items(p, parts, a.rows, std::max(1u, kLdStChunk / a.row_bytes),
+    ldst_items(p, parts, a.rows * a.slices, std::max(1u, kLdStChunk / a.row_bytes),
                std::max(1u, (1u << 20) / a.row_bytes), sms);
     if (parts * p.cpb > kMaxItems) return invalid_plan();
     p.ctas = ldst_grid(p, a.max_ctas, res, sms, parts * p.cpb);
@@ -367,26 +410,29 @@ inline LaunchPlan plan_gather_fp8(const GatherLaunch& a, uint32_t elems, int var
 // ---------------------------------------------------------------- row-sliced fp8 reads
 // kv_read_fp8_rows (launch_kv_gather_fp8 with GatherLaunch::rows), plain or layered.  The
 // geometry is plan_gather_rows' and counts bytes of the part's bf16 view (part_bytes == rows *
-// src_pitch == 2 * elems); elems is a multiple of 512, and row_bytes, both pitches, src_col,
-// the part bases and the local offsets are multiples of 16 bytes, so every 8-element vector is
-// one 8-byte e4m3 load inside one 128-element scale group and one 16-byte store.  Runs of rows
-// as in plan_gather_rows (about kLdStChunk of destination bytes, or all of a part's rows under
-// ldst_items' rule).  The grid follows the ld/st residency rule: one wave of the CTAs the
-// kernel keeps resident (res.r16, the occupancy API's answer for it).
+// src_pitch == 2 * elems); elems is a multiple of 512, and row_bytes, both pitches (with
+// slices > 1, dst_slice_pitch too), src_col, the part bases and the local offsets are multiples
+// of 16 bytes, so every 8-element vector is one 8-byte e4m3 load inside one 128-element scale
+// group and one 16-byte store.  Runs of (slice, row) pairs as in plan_gather_rows (about
+// kLdStChunk of destination bytes, or all of a part's pairs under ldst_items' rule).  The grid
+// follows the ld/st residency rule: one wave of the CTAs the kernel keeps resident (res.r16,
+// the occupancy API's answer for it).
 inline LaunchPlan plan_gather_fp8_rows(const GatherLaunch& a, uint32_t elems, int sms,
                                        LdStResident res) {
-    if (a.write || a.rows == 0 || a.row_bytes == 0 || a.nparts == 0 ||
-        a.nparts > kGatherMaxParts || uint64_t(a.src_col) + a.row_bytes > a.src_pitch ||
-        uint64_t(a.rows) * a.src_pitch != a.part_bytes ||
+    if (a.write || a.nparts == 0 || a.nparts > kGatherMaxParts ||
+        !row_geometry_ok(a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.slices,
+                         a.dst_slice_pitch, a.part_bytes) ||
         (a.group_flags && (a.group_parts == 0 || a.nparts % a.group_parts != 0)))
         return invalid_plan();
+    const uint64_t geo_or = a.align_or | a.row_bytes | a.src_pitch | a.src_col | a.dst_pitch |
+                            (a.slices > 1 ? a.dst_slice_pitch : 0u);
     if (elems == 0 || elems % 512 != 0 || uint64_t(a.part_bytes) != 2ull * elems ||
-        ((a.align_or | a.row_bytes | a.src_pitch | a.src_col | a.dst_pitch) & 15) != 0)
+        (geo_or & 15) != 0)
         return invalid_plan();
     LaunchPlan p;
     p.kernel = Kernel::kLdStFp8;
     const uint64_t parts = uint64_t(a.n) * a.nparts;
-    ldst_items(p, parts, a.rows, std::max(1u, kLdStChunk / a.row_bytes),
+    ldst_items(p, parts, a.rows * a.slices, std::max(1u, kLdStChunk / a.row_bytes),
                std::max(1u, (1u << 20) / a.row_bytes), sms);
     if (parts * p.cpb > kMaxItems) return invalid_plan();
     p.ctas = clamp_grid(a.max_ctas > 0 ? a.max_ctas : res.r16 * sms, parts * p.cpb);

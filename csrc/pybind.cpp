@@ -180,10 +180,27 @@ struct KeyArena {
 
 thread_local KeyArena t_arena;
 
+// A row-sliced read's geometry from its native list, in bytes: (rows, row_bytes, src_pitch,
+// src_col, dst_pitch) or the same followed by (slices, dst_slice_pitch) into a GatherSpec or a
+// GatherLaunch.  False unless the list has 5 or 7 entries; an empty list is for the caller.
+template <typename G>
+bool set_rows(G& g, const std::vector<uint32_t>& rows) {
+    if (rows.size() != 5 && rows.size() != 7) return false;
+    g.rows = rows[0];
+    g.row_bytes = rows[1];
+    g.src_pitch = rows[2];
+    g.src_col = rows[3];
+    g.dst_pitch = rows[4];
+    if (rows.size() == 7) {
+        g.slices = rows[5];
+        g.dst_slice_pitch = rows[6];
+    }
+    return true;
+}
+
 // A gathered call's parts: part s at part_base[s] (which must outlive the spec); elems > 0:
-// bf16 parts of elems elements stored as fp8 pages.  rows: a row-sliced read's geometry,
-// (rows, row_bytes, src_pitch, src_col, dst_pitch) in bytes; empty: whole parts.  The
-// connection checks the values.
+// bf16 parts of elems elements stored as fp8 pages.  rows: a row-sliced read's geometry
+// (set_rows); empty: whole parts.  The connection checks the values.
 Connection::GatherSpec gather_spec(const std::vector<uint64_t>& part_base, uint32_t part_bytes,
                                    uint32_t elems, uint32_t first_part,
                                    const std::vector<uint32_t>& rows = {}) {
@@ -193,14 +210,9 @@ Connection::GatherSpec gather_spec(const std::vector<uint64_t>& part_base, uint3
     g.part_bytes = part_bytes;
     g.fp8_elems = elems;
     g.first_part = first_part;
-    if (rows.empty()) return g;
-    if (rows.size() != 5)
-        throw py::value_error("rows is (rows, row_bytes, src_pitch, src_col, dst_pitch)");
-    g.rows = rows[0];
-    g.row_bytes = rows[1];
-    g.src_pitch = rows[2];
-    g.src_col = rows[3];
-    g.dst_pitch = rows[4];
+    if (!rows.empty() && !set_rows(g, rows))
+        throw py::value_error("rows is (rows, row_bytes, src_pitch, src_col, dst_pitch[, "
+                              "slices, dst_slice_pitch])");
     return g;
 }
 
@@ -617,8 +629,9 @@ PYBIND11_MODULE(_infinistore, m) {
             py::arg("reader") = py::none(), py::arg("group_parts") = 0,
             "scattered read: stored part first_part + s of each block -> part_base[s] + offset; "
             "elems > 0: fp8 pages dequantised into bf16 parts of elems elements; rows = (rows, "
-            "row_bytes, src_pitch, src_col, dst_pitch): only those rows of each part, row r to "
-            "part_base[s] + offset + r * dst_pitch; reader: a layered read whose parts are "
+            "row_bytes, src_pitch, src_col, dst_pitch[, slices, dst_slice_pitch]): only those "
+            "rows of each part, slice j of row r to part_base[s] + offset + r * dst_pitch + j * "
+            "dst_slice_pitch; reader: a layered read whose parts are "
             "released in groups of group_parts (check reader.failed)")
         .def(
             "wait_layered",
@@ -993,14 +1006,8 @@ PYBIND11_MODULE(_infinistore, m) {
             G.group_counters = as_ptr<uint32_t>(group_counters);
             G.group_seq = group_seq;
             G.group_parts = group_parts;
-            if (!rows.empty()) {
-                if (rows.size() != 5) throw std::runtime_error("kv_gather: rows is 5 values");
-                G.rows = rows[0];
-                G.row_bytes = rows[1];
-                G.src_pitch = rows[2];
-                G.src_col = rows[3];
-                G.dst_pitch = rows[4];
-            }
+            if (!rows.empty() && !set_rows(G, rows))
+                throw std::runtime_error("kv_gather: rows is 5 or 7 values");
             const cudaError_t e = kernels::launch_kv_gather(G, as_ptr<CUstream_st>(stream));
             if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
         },
@@ -1058,13 +1065,9 @@ PYBIND11_MODULE(_infinistore, m) {
             G.group_seq = group_seq;
             G.group_parts = group_parts;
             if (!rows.empty()) {  // bytes of the parts' bf16 view: part_bytes is 2 * elems
-                if (rows.size() != 5) throw std::runtime_error("kv_gather_fp8: rows is 5 values");
+                if (!set_rows(G, rows))
+                    throw std::runtime_error("kv_gather_fp8: rows is 5 or 7 values");
                 G.part_bytes = 2 * elems;
-                G.rows = rows[0];
-                G.row_bytes = rows[1];
-                G.src_pitch = rows[2];
-                G.src_col = rows[3];
-                G.dst_pitch = rows[4];
             }
             const cudaError_t e =
                 kernels::launch_kv_gather_fp8(G, elems, variant, as_ptr<CUstream_st>(stream));
@@ -1502,6 +1505,21 @@ PYBIND11_MODULE(_infinistore, m) {
         if (!stride || hi < lo) throw py::value_error("needs stride > 0 and lo <= hi");
         return kernels::cta_items(lo, hi, first, stride);
     });
+    // sliced rows: where (slice, row) pair q of a part goes, and the geometry the plans and the
+    // connection accept (kernels/launch_plan.h)
+    t.def("slice_pair",
+          [](uint32_t q, uint32_t rows, uint32_t row, uint32_t src_pitch, uint32_t src_col,
+             uint32_t dst_pitch, uint32_t dst_slice_pitch) {
+              if (!rows) throw py::value_error("needs rows > 0");
+              const kernels::PairOffsets o = kernels::slice_pair(q, rows, row, src_pitch, src_col,
+                                                                 dst_pitch, dst_slice_pitch);
+              return py::make_tuple(o.src, o.dst);
+          },
+          py::arg("q"), py::arg("rows"), py::arg("row"), py::arg("src_pitch"),
+          py::arg("src_col"), py::arg("dst_pitch"), py::arg("dst_slice_pitch"));
+    t.def("row_geometry_ok", &kernels::row_geometry_ok, py::arg("rows"), py::arg("row_bytes"),
+          py::arg("src_pitch"), py::arg("src_col"), py::arg("dst_pitch"), py::arg("slices"),
+          py::arg("dst_slice_pitch"), py::arg("part_bytes"));
     // how a read call is split into launches (ctrl/staging.h), with the client's limits
     t.attr("RING_BYTES") = kRingBytes;
     t.attr("MAX_BATCH") = kMaxBatch;
@@ -1620,7 +1638,7 @@ PYBIND11_MODULE(_infinistore, m) {
           [plan_dict](uint32_t n, uint32_t nparts, uint32_t rows, uint32_t row_bytes,
                       uint32_t src_pitch, uint32_t src_col, uint32_t dst_pitch, uint64_t align_or,
                       uint32_t group_parts, int max_ctas, int sm_count, int resident16,
-                      int resident32) {
+                      int resident32, uint32_t slices, uint32_t dst_slice_pitch) {
               static uint32_t flags[1];  // the plan only asks whether the read is layered
               kernels::GatherLaunch a;
               a.n = n;
@@ -1631,6 +1649,8 @@ PYBIND11_MODULE(_infinistore, m) {
               a.src_pitch = src_pitch;
               a.src_col = src_col;
               a.dst_pitch = dst_pitch;
+              a.slices = slices;
+              a.dst_slice_pitch = dst_slice_pitch;
               a.align_or = align_or;
               a.group_flags = group_parts ? flags : nullptr;
               a.group_parts = group_parts;
@@ -1640,7 +1660,8 @@ PYBIND11_MODULE(_infinistore, m) {
           py::arg("n"), py::arg("nparts"), py::arg("rows"), py::arg("row_bytes"),
           py::arg("src_pitch"), py::arg("src_col") = 0, py::arg("dst_pitch") = 0,
           py::arg("align_or") = 0, py::arg("group_parts") = 0, py::arg("max_ctas") = 0,
-          py::arg("sm_count") = 132, py::arg("resident16") = 1, py::arg("resident32") = 1);
+          py::arg("sm_count") = 132, py::arg("resident16") = 1, py::arg("resident32") = 1,
+          py::arg("slices") = 1, py::arg("dst_slice_pitch") = 0);
     t.def("plan_read_fused",
           [plan_dict](uint32_t n, uint32_t bytes, uint64_t align_or, int variant, int max_ctas,
                       uint32_t stage_bytes, uint32_t ring_bytes, int sm_count, int resident16,
@@ -1690,7 +1711,7 @@ PYBIND11_MODULE(_infinistore, m) {
           [plan_dict](uint32_t n, uint32_t nparts, uint32_t elems, uint32_t rows,
                       uint32_t row_bytes, uint32_t src_pitch, uint32_t src_col, uint32_t dst_pitch,
                       uint64_t align_or, uint32_t group_parts, bool write, int max_ctas,
-                      int sm_count, int resident) {
+                      int sm_count, int resident, uint32_t slices, uint32_t dst_slice_pitch) {
               static uint32_t flags[1];  // the plan only asks whether the read is layered
               kernels::GatherLaunch a;
               a.n = n;
@@ -1702,6 +1723,8 @@ PYBIND11_MODULE(_infinistore, m) {
               a.src_pitch = src_pitch;
               a.src_col = src_col;
               a.dst_pitch = dst_pitch;
+              a.slices = slices;
+              a.dst_slice_pitch = dst_slice_pitch;
               a.align_or = align_or;
               a.group_flags = group_parts ? flags : nullptr;
               a.group_parts = group_parts;
@@ -1712,7 +1735,8 @@ PYBIND11_MODULE(_infinistore, m) {
           py::arg("n"), py::arg("nparts"), py::arg("elems"), py::arg("rows"), py::arg("row_bytes"),
           py::arg("src_pitch"), py::arg("src_col") = 0, py::arg("dst_pitch") = 0,
           py::arg("align_or") = 0, py::arg("group_parts") = 0, py::arg("write") = false,
-          py::arg("max_ctas") = 0, py::arg("sm_count") = 132, py::arg("resident") = 1);
+          py::arg("max_ctas") = 0, py::arg("sm_count") = 132, py::arg("resident") = 1,
+          py::arg("slices") = 1, py::arg("dst_slice_pitch") = 0);
     t.def("fp8_rows_read_bytes", &fp8_rows_read_bytes, py::arg("rows"), py::arg("row_bytes"),
           py::arg("src_pitch"), py::arg("src_col") = 0,
           "bytes_read of a row-sliced read of one stored fp8 part (geometry in bf16 bytes)");

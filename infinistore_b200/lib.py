@@ -337,18 +337,28 @@ class PartRows:
     ``r * dst_pitch`` from the block's destination offset.  The stored part is
     ``count * src_pitch`` elements.  With token-major KV pages, a row is one token and
     ``src_offset`` / ``width`` pick a run of KV heads: how a decode rank reads the heads it
-    owns out of pages that a prefill rank at another tensor-parallel degree wrote."""
+    owns out of pages that a prefill rank at another tensor-parallel degree wrote.
 
-    __slots__ = ("count", "width", "src_pitch", "src_offset", "dst_pitch")
+    ``slices`` > 1 splits each row into that many slices of ``width`` elements, side by side
+    from ``src_offset``: slice j of row r lands at ``r * dst_pitch + j * dst_slice_pitch``.
+    With one KV head per slice, ``dst_pitch = head_dim`` and ``dst_slice_pitch = tokens *
+    head_dim`` land a token-major page's heads in a head-major ``[head][token][dim]`` page
+    (``HeadMajorKVCache``).  With ``slices == 1``, ``dst_slice_pitch`` is not used."""
+
+    __slots__ = ("count", "width", "src_pitch", "src_offset", "dst_pitch", "slices",
+                 "dst_slice_pitch")
 
     def __init__(self, count: int, width: int, src_pitch: int, src_offset: int = 0, *,
-                 dst_pitch: int):
+                 dst_pitch: int, slices: int = 1, dst_slice_pitch: int = 0):
         self.count, self.width = int(count), int(width)
         self.src_pitch, self.src_offset, self.dst_pitch = int(src_pitch), int(src_offset), int(dst_pitch)
+        self.slices, self.dst_slice_pitch = int(slices), int(dst_slice_pitch)
 
     def __repr__(self):
+        sliced = (f", slices={self.slices}, dst_slice_pitch={self.dst_slice_pitch}"
+                  if (self.slices, self.dst_slice_pitch) != (1, 0) else "")
         return (f"PartRows(count={self.count}, width={self.width}, src_pitch={self.src_pitch}, "
-                f"src_offset={self.src_offset}, dst_pitch={self.dst_pitch})")
+                f"src_offset={self.src_offset}, dst_pitch={self.dst_pitch}{sliced})")
 
     def __eq__(self, other):
         return isinstance(other, PartRows) and all(
@@ -356,22 +366,43 @@ class PartRows:
 
     def check(self, part_size: int) -> int:
         """Raises ``ValueError`` unless the geometry fits a stored part of ``part_size``
-        elements and destination rows do not overlap.  Returns the destination extent of one
-        part in elements, ``(count - 1) * dst_pitch + width``."""
-        if self.count < 1 or self.width < 1 or self.src_offset < 0:
-            raise ValueError(f"{self}: count and width must be positive, src_offset >= 0")
-        if self.src_offset + self.width > self.src_pitch:
-            raise ValueError(f"{self}: src_offset + width runs past src_pitch")
+        elements and destination rows (and slices) do not overlap.  Returns the destination
+        extent of one part in elements, ``(count - 1) * dst_pitch + (slices - 1) *
+        dst_slice_pitch + width``."""
+        if self.count < 1 or self.width < 1 or self.src_offset < 0 or self.slices < 1:
+            raise ValueError(f"{self}: count, width and slices must be positive, "
+                             f"src_offset >= 0")
+        if self.src_offset + self.slices * self.width > self.src_pitch:
+            raise ValueError(f"{self}: src_offset + slices * width runs past src_pitch")
         if self.count * self.src_pitch != int(part_size):
             raise ValueError(f"{self}: count * src_pitch must equal part_size {int(part_size)}")
-        if self.dst_pitch < self.width:
-            raise ValueError(f"{self}: dst_pitch must be at least width (rows must not overlap)")
-        return (self.count - 1) * self.dst_pitch + self.width
+        if self.slices == 1:
+            if self.dst_pitch < self.width:
+                raise ValueError(f"{self}: dst_pitch must be at least width "
+                                 f"(rows must not overlap)")
+            return (self.count - 1) * self.dst_pitch + self.width
+        # disjoint when a slice's rows nest inside dst_slice_pitch (head-major) or a row's
+        # slices inside dst_pitch (token-major)
+        w, r1, s1 = self.width, self.count - 1, self.slices - 1
+        head_major = self.dst_pitch >= w and self.dst_slice_pitch >= r1 * self.dst_pitch + w
+        token_major = self.dst_slice_pitch >= w and self.dst_pitch >= s1 * self.dst_slice_pitch + w
+        if not (head_major or token_major):
+            raise ValueError(f"{self}: destination slices overlap (need dst_slice_pitch >= "
+                             f"(count - 1) * dst_pitch + width, or dst_pitch >= "
+                             f"(slices - 1) * dst_slice_pitch + width)")
+        return r1 * self.dst_pitch + s1 * self.dst_slice_pitch + w
 
     def native(self, es: int):
-        """(rows, row_bytes, src_pitch, src_col, dst_pitch) in bytes, for the connection."""
+        """(rows, row_bytes, src_pitch, src_col, dst_pitch) in bytes, for the connection,
+        followed by (slices, dst_slice_pitch) when ``slices > 1``."""
         out = [self.count, self.width * es, self.src_pitch * es, self.src_offset * es,
                self.dst_pitch * es]
+        if self.slices != 1:
+            out += [self.slices, self.dst_slice_pitch * es]
+            extent = ((self.count - 1) * self.dst_pitch + (self.slices - 1) * self.dst_slice_pitch
+                      + self.width) * es
+            if extent >= 1 << 32:
+                raise ValueError(f"{self}: the destination extent exceeds 32 bits")
         if max(out) >= 1 << 32:
             raise ValueError(f"{self}: a byte size exceeds 32 bits")
         return out
@@ -722,11 +753,12 @@ class InfinityConnection:
             if part_size % 512:
                 raise ValueError(f"fp8 gathered blocks need a part_size that is a multiple of "
                                  f"512 elements, not {part_size}")
-            if rows is not None and any(v % 8 for v in (rows.width, rows.src_pitch,
-                                                         rows.src_offset, rows.dst_pitch)):
+            if rows is not None and any(v % 8 for v in (
+                    rows.width, rows.src_pitch, rows.src_offset, rows.dst_pitch,
+                    rows.dst_slice_pitch if rows.slices > 1 else 0)):
                 raise ValueError(f"{rows}: row-sliced reads of fp8 blocks need width, "
-                                 f"src_pitch, src_offset and dst_pitch in multiples of 8 "
-                                 f"elements (one 16-byte vector)")
+                                 f"src_pitch, src_offset, dst_pitch and dst_slice_pitch in "
+                                 f"multiples of 8 elements (one 16-byte vector)")
             align = 0
             for b in bases:
                 align |= b

@@ -17,33 +17,25 @@ def layer_keys(layout: KVLayout, tp_rank: int, layer: int, kv: int,
     return [page_key(layout.name, layer, kind, tp_rank, h) for h in page_hashes]
 
 
-class PagedKVCache:
-    """``cache[layer, kv, page]`` is one contiguous page of ``layout.page_elems`` elements.
+class _PagedCache:
+    """What the token-major :class:`PagedKVCache` and the head-major :class:`HeadMajorKVCache`
+    share: ``data[layer, kv, page]`` is one page of ``layout.page_elems`` elements, per-layer
+    and all-layer keys, and the reads of all-layer pages (one key per page, parts 2l (K) and
+    2l + 1 (V)), from ranks at this or another tensor-parallel degree.  The pages are
+    byte-identical in the store whichever cache wrote them; a subclass gives only where a
+    source rank's heads land in its page layout (``_source_rows``)."""
 
-    The whole cache is one tensor, registered once with the connection (``register_mr``) and
-    addressed by element offset, the calling convention of the reference
-    (infinistore/lib.py:645-667, SURVEY C10).
-
-    Layer-wise streaming (docs/source/design.rst:56-63): ``write_layer`` is called right
-    after layer l's KV has been produced, on the producing stream; the page mover runs on
-    the connection's own streams behind it, so the upload overlaps the next layer's compute.
-    """
-
-    def __init__(self, layout: KVLayout, num_pages: int, device, tp_rank: int = 0):
+    def __init__(self, layout: KVLayout, num_pages: int, tp_rank: int, data: torch.Tensor):
         self.layout = layout
         self.num_pages = num_pages
         self.tp_rank = tp_rank
-        self.data = torch.zeros(layout.layers, 2, num_pages, layout.page_elems,
-                                dtype=layout.dtype, device=device)
+        self.data = data
         self._registered = set()
 
     # ------------------------------------------------------------------ geometry
     def page_offset(self, layer: int, kv: int, page: int) -> int:
         """Element offset of a page from the start of the cache tensor."""
         return ((layer * 2 + kv) * self.num_pages + page) * self.layout.page_elems
-
-    def page(self, layer: int, kv: int, page: int) -> torch.Tensor:
-        return self.data[layer, kv, page]
 
     def keys(self, layer: int, kv: int, page_hashes: Sequence[str]) -> List[str]:
         return layer_keys(self.layout, self.tp_rank, layer, kv, page_hashes)
@@ -53,118 +45,59 @@ class PagedKVCache:
             conn.register_mr(self.data)
             self._registered.add(id(conn))
 
-    # ------------------------------------------------------------------ store I/O
-    def write_layer(self, conn, layer: int, pages: Sequence[int], page_hashes: Sequence[str],
-                    fp8: bool = False, stream="current") -> int:
-        """Upload K and V pages of one layer.  Returns the number of blocks written."""
-        self._ensure_registered(conn)
-        elems = self.layout.page_elems
-        nbytes = conn.fp8_page_bytes(elems) if fp8 else self.layout.page_bytes
-        n = 0
-        for kv in (0, 1):
-            keys = self.keys(layer, kv, page_hashes)
-            blocks = conn.allocate_rdma(keys, nbytes)
-            offs = np.asarray([self.page_offset(layer, kv, p) for p in pages], dtype=np.int64)
-            if fp8:
-                conn.rdma_write_cache_fp8(self.data, offs, elems, blocks, stream=stream)
-            else:
-                conn.rdma_write_cache(self.data, offs, elems, blocks, stream=stream)
-            n += len(keys)
-        return n
-
-    def read_layer(self, conn, layer: int, pages: Sequence[int], page_hashes: Sequence[str],
-                   fp8: bool = False, stream="current") -> int:
-        self._ensure_registered(conn)
-        elems = self.layout.page_elems
-        n = 0
-        for kv in (0, 1):
-            keys = self.keys(layer, kv, page_hashes)
-            blocks = [(k, self.page_offset(layer, kv, p)) for k, p in zip(keys, pages)]
-            if fp8:
-                conn.read_cache_fp8(self.data, blocks, elems, stream=stream)
-            else:
-                conn.read_cache(self.data, blocks, elems, stream=stream)
-            n += len(keys)
-        return n
-
     # ------------------------------------------------------------------ all-layer pages
-    # One key per page: the block is the page's K and V of every layer, parts 2l (K) and
-    # 2l + 1 (V), gathered by the write kernel and scattered by the read kernel.
     def page_keys(self, page_hashes: Sequence[str]) -> List[str]:
-        """Store keys of all-layer pages (``write_pages``)."""
+        """Store keys of all-layer pages (``PagedKVCache.write_pages``)."""
         return [page_key(self.layout.name, ALL_LAYERS, "KV", self.tp_rank, h) for h in page_hashes]
 
     def _parts(self, layers: range):
         return [(self.data, self.page_offset(layer, kv, 0)) for layer in layers for kv in (0, 1)]
 
-    def _check_fp8(self, cross_tp: bool = False):
+    def _check_fp8(self, rows: bool = False):
         if self.data.dtype != torch.bfloat16 or self.data.device.type != "cuda":
             raise ValueError("fp8 all-layer pages need a bf16 cache on a CUDA device")
-        # a cross-TP read dequantises each source's heads in 8-element vectors; a head need
-        # not fill a 128-element scale group
-        if cross_tp and self.layout.head_dim % 8:
-            raise ValueError(f"fp8 pages written at another TP degree need a head_dim that is "
-                             f"a multiple of 8, not {self.layout.head_dim}")
-
-    def write_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
-                    stream="current", fp8: bool = False) -> int:
-        """Upload every layer's K and V of each page under one key per page.  ``fp8``: every
-        part is stored as e4m3 with per-128 scales (``rdma_write_cache_gather_fp8``), about
-        half the pool bytes; read such pages back with ``read_pages(fp8=True)``.  Returns the
-        number of blocks written."""
-        if fp8:
-            self._check_fp8()  # before any block is allocated
-        self._ensure_registered(conn)
-        layers = range(self.layout.layers)
-        keys = self.page_keys(page_hashes)
-        elems = self.layout.page_elems
-        nbytes = (conn.fp8_gather_block_bytes(2 * len(layers), elems) if fp8
-                  else 2 * len(layers) * self.layout.page_bytes)
-        blocks = conn.allocate_rdma(keys, nbytes)
-        offs = np.asarray(pages, dtype=np.int64) * elems
-        write = conn.rdma_write_cache_gather_fp8 if fp8 else conn.rdma_write_cache_gather
-        write(self._parts(layers), offs, elems, blocks, stream=stream)
-        return len(keys)
-
-    def page_writer(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
-                    fp8: bool = False) -> "PageWriter":
-        """Allocate all-layer pages (as ``write_pages``) and return a writer that stores them
-        layer by layer: ``write_layers(range(l, l + 1))`` right after layer l has produced its
-        KV, so the upload overlaps the next layer's compute and one key per page is kept.
-        Read the pages back with ``read_pages(fp8=fp8)``."""
-        if fp8:
-            self._check_fp8()  # before any block is allocated
-        self._ensure_registered(conn)
-        nparts = 2 * self.layout.layers
-        elems = self.layout.page_elems
-        nbytes = (conn.fp8_gather_block_bytes(nparts, elems) if fp8
-                  else nparts * self.layout.page_bytes)
-        blocks = conn.allocate_rdma(self.page_keys(page_hashes), nbytes)
-        offs = np.asarray(pages, dtype=np.int64) * elems
-        return PageWriter(self, conn.gather_writer(blocks, offs, nparts, elems, fp8=fp8))
+        # a read that regroups heads dequantises them in 8-element vectors; a head need not
+        # fill a 128-element scale group
+        if rows and self.layout.head_dim % 8:
+            raise ValueError(f"fp8 pages read head by head (written at another TP degree, or "
+                             f"into a head-major cache) need a head_dim that is a multiple of "
+                             f"8, not {self.layout.head_dim}")
 
     def _cross_tp(self, source_tp: Optional[int]) -> bool:
         """Whether a read of pages written at ``source_tp`` regroups heads."""
         return source_tp is not None and int(source_tp) != self.layout.tp
 
-    def _sources(self, pages: Sequence[int], page_hashes: Sequence[str], source_tp: int):
-        """The blocks of a read of pages written at ``source_tp``: one per (page, source
-        rank), keyed by the writer rank, each landing at its heads of the reader's page, and
-        the rows every block gives (``PartRows``) and the stored part size."""
+    def _source_rows(self, wl: KVLayout, src_head: int, heads: int):
+        """How ``heads`` consecutive heads from head ``src_head`` of a page written with
+        layout ``wl`` land in this cache's page: the ``PartRows`` of the read (None: the whole
+        stored part, contiguously) and the elements between two heads of a destination page."""
+        raise NotImplementedError
+
+    def _sources(self, pages: Sequence[int], page_hashes: Sequence[str],
+                 source_tp: Optional[int]):
+        """The blocks of a read of pages written at ``source_tp`` (None: this TP degree, by
+        this rank): one per (page, source rank), keyed by the writer rank, each landing at its
+        heads of the reader's page, and the rows every block gives (``PartRows``, or None for
+        whole parts) and the stored part size."""
         lay = self.layout
-        wl = lay.with_tp(int(source_tp))
-        srcs = tp_sources(lay, lay.tp, self.tp_rank, wl.tp)
+        wl = lay if source_tp is None else lay.with_tp(int(source_tp))
+        srcs = (tp_sources(lay, lay.tp, self.tp_rank, wl.tp) if self._cross_tp(source_tp)
+                else [(self.tp_rank, 0, 0, lay.heads_per_rank)])
         if len({s[1] for s in srcs}) != 1:  # holds for every pair tp_sources accepts
             raise ValueError("sources start at different heads of their pages")
         heads, src_head = srcs[0][3], srcs[0][1]
         if len(pages) != len(page_hashes):
             raise ValueError(f"{len(pages)} pages for {len(page_hashes)} page hashes")
+        rows, head_elems = self._source_rows(wl, src_head, heads)
         keys = [page_key(lay.name, ALL_LAYERS, "KV", w, h) for h in page_hashes for w, *_ in srcs]
         offs = (np.asarray(pages, dtype=np.int64)[:, None] * lay.page_elems
-                + np.asarray([d * lay.head_dim for _, _, d, _ in srcs], dtype=np.int64)[None, :])
-        rows = PartRows(lay.page_tokens, heads * lay.head_dim, wl.heads_per_rank * lay.head_dim,
-                        src_head * lay.head_dim, dst_pitch=lay.heads_per_rank * lay.head_dim)
+                + np.asarray([d * head_elems for _, _, d, _ in srcs], dtype=np.int64)[None, :])
         return keys, offs.reshape(-1), rows, wl.page_elems
+
+    def _blocks(self, pages: Sequence[int], page_hashes: Sequence[str],
+                source_tp: Optional[int]):
+        """keys, offsets, rows and stored part size of a read of all-layer pages."""
+        return self._sources(pages, page_hashes, source_tp)
 
     def _check_layers(self, layers: Optional[range]) -> range:
         layers = range(self.layout.layers) if layers is None else layers
@@ -176,10 +109,10 @@ class PagedKVCache:
     def read_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
                    layers: Optional[range] = None, stream="current", fp8: bool = False,
                    source_tp: Optional[int] = None) -> int:
-        """Fetch pages written by ``write_pages`` into pages ``pages``.  ``layers`` (a range
-        with step 1, default all) reads only those layers' parts of the blocks, so layer l
-        can be fetched while layer l - 1 computes.  ``fp8`` must be what the writer used.
-        Returns the number of blocks read.
+        """Fetch pages written by ``PagedKVCache.write_pages`` (or ``page_writer``) into
+        pages ``pages``.  ``layers`` (a range with step 1, default all) reads only those
+        layers' parts of the blocks, so layer l can be fetched while layer l - 1 computes.
+        ``fp8`` must be what the writer used.  Returns the number of blocks read.
 
         ``source_tp``: the pages were written by ranks at that tensor-parallel degree (e.g. a
         prefill instance at TP 8 feeding this decode rank at TP 2).  Each page is then read
@@ -190,22 +123,14 @@ class PagedKVCache:
         untouched, so treat every page of a failed read as not read.  With ``fp8`` the read
         kernel dequantises each source's heads out of its fp8 pages in the same way
         (``head_dim`` a multiple of 8).  Returns the number of (page, source) blocks read."""
-        cross = self._cross_tp(source_tp)
+        keys, offs, rows, part = self._blocks(pages, page_hashes, source_tp)
         if fp8:
-            self._check_fp8(cross)
+            self._check_fp8(rows is not None)
         self._ensure_registered(conn)
         layers = self._check_layers(layers)
-        if cross:
-            keys, offs, rows, part = self._sources(pages, page_hashes, source_tp)
-            read = conn.read_cache_scatter_fp8 if fp8 else conn.read_cache_scatter
-            read(self._parts(layers), (keys, offs), part, first_part=2 * layers.start,
-                 stream=stream, rows=rows)
-            return len(keys)
-        keys = self.page_keys(page_hashes)
-        offs = np.asarray(pages, dtype=np.int64) * self.layout.page_elems
         read = conn.read_cache_scatter_fp8 if fp8 else conn.read_cache_scatter
-        read(self._parts(layers), (keys, offs), self.layout.page_elems,
-             first_part=2 * layers.start, stream=stream)
+        read(self._parts(layers), (keys, offs), part, first_part=2 * layers.start,
+             stream=stream, rows=rows)
         return len(keys)
 
     def read_pages_layered(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
@@ -217,22 +142,14 @@ class PagedKVCache:
         arrived, with no host synchronisation.  ``layers`` (a step-1 range, default all),
         ``fp8`` and ``source_tp`` as for ``read_pages``.  A layer is released before the
         read's post-copy index check: when ``sync()`` reports a miss, the whole read failed."""
-        cross = self._cross_tp(source_tp)
+        keys, offs, rows, part = self._blocks(pages, page_hashes, source_tp)
         if fp8:
-            self._check_fp8(cross)
+            self._check_fp8(rows is not None)
         self._ensure_registered(conn)
         layers = self._check_layers(layers)
-        if cross:
-            keys, offs, rows, part = self._sources(pages, page_hashes, source_tp)
-            read = conn.read_cache_scatter_layered(self._parts(layers), (keys, offs), part,
-                                                   group_parts=2, first_part=2 * layers.start,
-                                                   fp8=fp8, stream=stream, rows=rows)
-            return PageRead(read, layers)
-        keys = self.page_keys(page_hashes)
-        offs = np.asarray(pages, dtype=np.int64) * self.layout.page_elems
-        read = conn.read_cache_scatter_layered(self._parts(layers), (keys, offs),
-                                               self.layout.page_elems, group_parts=2,
-                                               first_part=2 * layers.start, fp8=fp8, stream=stream)
+        read = conn.read_cache_scatter_layered(self._parts(layers), (keys, offs), part,
+                                               group_parts=2, first_part=2 * layers.start,
+                                               fp8=fp8, stream=stream, rows=rows)
         return PageRead(read, layers)
 
     def source_page_keys(self, page_hashes: Sequence[str], source_tp: int) -> List[List[str]]:
@@ -291,6 +208,114 @@ class PagedKVCache:
         return conn.touch(keys) if keys else 0
 
 
+class PagedKVCache(_PagedCache):
+    """``cache[layer, kv, page]`` is one contiguous page of ``layout.page_elems`` elements.
+
+    The whole cache is one tensor, registered once with the connection (``register_mr``) and
+    addressed by element offset, the calling convention of the reference
+    (infinistore/lib.py:645-667, SURVEY C10).
+
+    Layer-wise streaming (docs/source/design.rst:56-63): ``write_layer`` is called right
+    after layer l's KV has been produced, on the producing stream; the page mover runs on
+    the connection's own streams behind it, so the upload overlaps the next layer's compute.
+    """
+
+    def __init__(self, layout: KVLayout, num_pages: int, device, tp_rank: int = 0):
+        super().__init__(layout, num_pages, tp_rank,
+                         torch.zeros(layout.layers, 2, num_pages, layout.page_elems,
+                                     dtype=layout.dtype, device=device))
+
+    def page(self, layer: int, kv: int, page: int) -> torch.Tensor:
+        return self.data[layer, kv, page]
+
+    # ------------------------------------------------------------------ store I/O
+    def write_layer(self, conn, layer: int, pages: Sequence[int], page_hashes: Sequence[str],
+                    fp8: bool = False, stream="current") -> int:
+        """Upload K and V pages of one layer.  Returns the number of blocks written."""
+        self._ensure_registered(conn)
+        elems = self.layout.page_elems
+        nbytes = conn.fp8_page_bytes(elems) if fp8 else self.layout.page_bytes
+        n = 0
+        for kv in (0, 1):
+            keys = self.keys(layer, kv, page_hashes)
+            blocks = conn.allocate_rdma(keys, nbytes)
+            offs = np.asarray([self.page_offset(layer, kv, p) for p in pages], dtype=np.int64)
+            if fp8:
+                conn.rdma_write_cache_fp8(self.data, offs, elems, blocks, stream=stream)
+            else:
+                conn.rdma_write_cache(self.data, offs, elems, blocks, stream=stream)
+            n += len(keys)
+        return n
+
+    def read_layer(self, conn, layer: int, pages: Sequence[int], page_hashes: Sequence[str],
+                   fp8: bool = False, stream="current") -> int:
+        self._ensure_registered(conn)
+        elems = self.layout.page_elems
+        n = 0
+        for kv in (0, 1):
+            keys = self.keys(layer, kv, page_hashes)
+            blocks = [(k, self.page_offset(layer, kv, p)) for k, p in zip(keys, pages)]
+            if fp8:
+                conn.read_cache_fp8(self.data, blocks, elems, stream=stream)
+            else:
+                conn.read_cache(self.data, blocks, elems, stream=stream)
+            n += len(keys)
+        return n
+
+    # ------------------------------------------------------------------ all-layer pages
+    def _source_rows(self, wl: KVLayout, src_head: int, heads: int):
+        lay = self.layout
+        rows = PartRows(lay.page_tokens, heads * lay.head_dim, wl.heads_per_rank * lay.head_dim,
+                        src_head * lay.head_dim, dst_pitch=lay.heads_per_rank * lay.head_dim)
+        return rows, lay.head_dim
+
+    def _blocks(self, pages: Sequence[int], page_hashes: Sequence[str],
+                source_tp: Optional[int]):
+        if self._cross_tp(source_tp):
+            return self._sources(pages, page_hashes, source_tp)
+        # this rank's own pages land whole: the same token-major layout
+        return (self.page_keys(page_hashes),
+                np.asarray(pages, dtype=np.int64) * self.layout.page_elems, None,
+                self.layout.page_elems)
+
+    def write_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
+                    stream="current", fp8: bool = False) -> int:
+        """Upload every layer's K and V of each page under one key per page.  ``fp8``: every
+        part is stored as e4m3 with per-128 scales (``rdma_write_cache_gather_fp8``), about
+        half the pool bytes; read such pages back with ``read_pages(fp8=True)``.  Returns the
+        number of blocks written."""
+        if fp8:
+            self._check_fp8()  # before any block is allocated
+        self._ensure_registered(conn)
+        layers = range(self.layout.layers)
+        keys = self.page_keys(page_hashes)
+        elems = self.layout.page_elems
+        nbytes = (conn.fp8_gather_block_bytes(2 * len(layers), elems) if fp8
+                  else 2 * len(layers) * self.layout.page_bytes)
+        blocks = conn.allocate_rdma(keys, nbytes)
+        offs = np.asarray(pages, dtype=np.int64) * elems
+        write = conn.rdma_write_cache_gather_fp8 if fp8 else conn.rdma_write_cache_gather
+        write(self._parts(layers), offs, elems, blocks, stream=stream)
+        return len(keys)
+
+    def page_writer(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
+                    fp8: bool = False) -> "PageWriter":
+        """Allocate all-layer pages (as ``write_pages``) and return a writer that stores them
+        layer by layer: ``write_layers(range(l, l + 1))`` right after layer l has produced its
+        KV, so the upload overlaps the next layer's compute and one key per page is kept.
+        Read the pages back with ``read_pages(fp8=fp8)``."""
+        if fp8:
+            self._check_fp8()  # before any block is allocated
+        self._ensure_registered(conn)
+        nparts = 2 * self.layout.layers
+        elems = self.layout.page_elems
+        nbytes = (conn.fp8_gather_block_bytes(nparts, elems) if fp8
+                  else nparts * self.layout.page_bytes)
+        blocks = conn.allocate_rdma(self.page_keys(page_hashes), nbytes)
+        offs = np.asarray(pages, dtype=np.int64) * elems
+        return PageWriter(self, conn.gather_writer(blocks, offs, nparts, elems, fp8=fp8))
+
+
 class PageWriter:
     """Layer-by-layer upload of all-layer pages (``PagedKVCache.page_writer``)."""
 
@@ -347,26 +372,29 @@ def read_layer_multi(conn, caches: Sequence[PagedKVCache], layer: int, pages: Se
     return n
 
 
-class HeadMajorKVCache:
+
+
+class HeadMajorKVCache(_PagedCache):
     """Decode-side cache in the layout a paged-attention kernel streams:
     ``data[layer, kv]`` is ``[num_pages, heads, page_tokens, head_dim]`` - one head's tokens
     of a page are contiguous.  Prefill writes pages token-major (``[tokens, heads, dim]``,
-    :class:`PagedKVCache`); ``read_layer`` fetches them with
+    :class:`PagedKVCache`); ``read_layer`` fetches per-layer pages with
     ``InfinityConnection.read_cache_hnd``, whose store is a 4-D tensor-map TMA: the
     transposition happens inside the read, the page crosses HBM once and no permute kernel
     runs on the decode GPU.  The reference hands opaque bytes to the consumer
-    (infinistore/lib.py:377-379), which then repacks them itself."""
+    (infinistore/lib.py:377-379), which then repacks them itself.
+
+    All-layer pages (``PagedKVCache.write_pages`` / ``page_writer``, one key per page) are
+    read with ``read_pages`` / ``read_pages_layered``, in bf16 or fp8 and from writers at any
+    TP degree, with the semantics and refusals of the ``PagedKVCache`` methods: the read
+    kernel lands each source's heads as ``[head][token][dim]`` itself (sliced rows,
+    ``PartRows(slices=)``), one block per (page, source rank)."""
 
     def __init__(self, layout: KVLayout, num_pages: int, device, tp_rank: int = 0):
-        self.layout = layout
-        self.num_pages = num_pages
-        self.tp_rank = tp_rank
-        self.data = torch.zeros(layout.layers, 2, num_pages, layout.heads_per_rank,
-                                layout.page_tokens, layout.head_dim, dtype=layout.dtype,
-                                device=device)
-
-    def keys(self, layer: int, kv: int, page_hashes: Sequence[str]) -> List[str]:
-        return layer_keys(self.layout, self.tp_rank, layer, kv, page_hashes)
+        super().__init__(layout, num_pages, tp_rank,
+                         torch.zeros(layout.layers, 2, num_pages, layout.heads_per_rank,
+                                     layout.page_tokens, layout.head_dim, dtype=layout.dtype,
+                                     device=device))
 
     def page_token_major(self, layer: int, kv: int, page: int) -> torch.Tensor:
         """A page as prefill laid it out, ``[tokens, heads, dim]`` (a permuted view)."""
@@ -382,3 +410,15 @@ class HeadMajorKVCache:
                                 stream=stream)
             n += len(keys)
         return n
+
+    # ------------------------------------------------------------------ all-layer pages
+    def _source_rows(self, wl: KVLayout, src_head: int, heads: int):
+        """Token r of the source's heads is row r; head j of it is slice j, landing at
+        ``r * head_dim + j * page_tokens * head_dim`` of the destination.  A writer rank with
+        one head stores it as ``[token][dim]``, which is already head-major: whole parts."""
+        tokens, dim = self.layout.page_tokens, self.layout.head_dim
+        if wl.heads_per_rank == 1:
+            return None, tokens * dim
+        rows = PartRows(tokens, dim, wl.heads_per_rank * dim, src_head * dim, dst_pitch=dim,
+                        slices=heads, dst_slice_pitch=tokens * dim)
+        return rows, tokens * dim

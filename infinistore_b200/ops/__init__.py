@@ -126,7 +126,10 @@ def kv_gather(descs: torch.Tensor, part_base: Sequence[int], part_bytes: int, wr
     kernel walks the parts group by group and releases each group's flag.  A read with
     ``rows`` = (rows, row_bytes, src_pitch, src_col, dst_pitch), bytes, is row-sliced
     (kv_scatter_rows): row r of stored part s at ``r * src_pitch + src_col`` -> part s's
-    destination + ``r * dst_pitch``; ``part_bytes`` must be ``rows * src_pitch``."""
+    destination + ``r * dst_pitch``; ``part_bytes`` must be ``rows * src_pitch``.  Seven
+    values, (..., slices, dst_slice_pitch), make it sliced: slice j of row r at
+    ``r * src_pitch + src_col + j * row_bytes`` -> destination + ``r * dst_pitch + j *
+    dst_slice_pitch`` (e.g. token-major KV heads into a head-major page)."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
     bases = [int(b) for b in part_base]
     for b in bases:
@@ -346,7 +349,9 @@ def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, wri
     (rows, row_bytes, src_pitch, src_col, dst_pitch), in bytes of the part's bf16 view
     (``rows * src_pitch == 2 * elems``, every value a multiple of 16), dequantises only those
     rows (kv_read_fp8_rows, whatever the variant): row r from bf16 byte
-    ``r * src_pitch + src_col`` of the page -> part s's destination + ``r * dst_pitch``."""
+    ``r * src_pitch + src_col`` of the page -> part s's destination + ``r * dst_pitch``.
+    Seven values slice the rows as for ``kv_gather`` (``dst_slice_pitch`` a multiple of 16
+    too)."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
     bases = [int(b) for b in part_base]
     for b in bases:
