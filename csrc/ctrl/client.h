@@ -204,9 +204,11 @@ class Connection {
         // group_parts (which must divide nparts)
         ScatterReader* reader = nullptr;
         uint32_t group_parts = 0;
-        // reads: row-sliced parts (kernels::GatherLaunch::rows, bytes of the caller's view of a
-        // part, view_part_bytes()); rows == 0: whole parts.  slices > 1: sliced rows
-        // (kernels::GatherLaunch::slices), e.g. a token's KV heads into a head-major page
+        // row-sliced parts (kernels::GatherLaunch::rows, bytes of the caller's view of a part,
+        // view_part_bytes()); rows == 0: whole parts.  slices > 1: sliced rows
+        // (kernels::GatherLaunch::slices), e.g. a token's KV heads into a head-major page.  A
+        // write takes the geometry that reads the same local layout back, and its rows must
+        // fill the stored part (kernels::row_write_covers)
         uint32_t rows = 0, row_bytes = 0, src_pitch = 0, src_col = 0, dst_pitch = 0;
         uint32_t slices = 1, dst_slice_pitch = 0;
         // pool bytes of a part: part_bytes, or kernels::fp8_gather_bytes(1, fp8_elems)
@@ -251,7 +253,10 @@ class Connection {
     // refused call leaves the writer as it was.
     int write_layered(GatherWriter& w, const GatherSpec& g, uint64_t scale, int device,
                       uint64_t stream);
-    // offsets in bytes; blocks allocated with nparts * g.pool_part_bytes() bytes (trusted)
+    // offsets in bytes; blocks allocated with nparts * g.pool_part_bytes() bytes (trusted).
+    // Row-sliced (g.rows): the geometry of r_rdma_scatter below, filling every stored part;
+    // bytes_written counts whole parts, as without rows.  write_layered takes rows the same
+    // way, on any of a writer's calls.
     int w_rdma_gather(const GatherSpec& g, const uint64_t* offsets, size_t noffsets,
                       const RemoteBlock* blocks, size_t nblocks, int device, uint64_t stream);
     // A stored block must hold g.need_bytes() bytes, else it is a miss.  Row-sliced (g.rows):

@@ -299,12 +299,13 @@ kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n,
     return G;
 }
 
-// Bytes one block of a gathered call moves: its parts, or their rows when row-sliced (of fp8
-// parts: the pool bytes of those rows, read_plan.h: fp8_rows_read_bytes; a row's slices are
-// adjacent in the stored row, so they count as one run of slices * row_bytes).
-static uint64_t gather_moved_bytes(const Connection::GatherSpec& g) {
+// Bytes one block of a gathered call moves: its parts, or their rows when a read is row-sliced
+// (of fp8 parts: the pool bytes of those rows, read_plan.h: fp8_rows_read_bytes; a row's slices
+// are adjacent in the stored row, so they count as one run of slices * row_bytes).  A
+// row-sliced write fills whole stored parts, so it counts them as the write without rows does.
+static uint64_t gather_moved_bytes(const Connection::GatherSpec& g, bool write) {
     const uint64_t width = uint64_t(g.slices) * g.row_bytes;
-    const uint64_t part = !g.rows ? g.pool_part_bytes()
+    const uint64_t part = !g.rows || write ? g.pool_part_bytes()
                           : g.fp8_elems
                               ? fp8_rows_read_bytes(g.rows, uint32_t(width), g.src_pitch, g.src_col)
                               : uint64_t(g.rows) * width;
@@ -391,7 +392,8 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
     const bool commit_now = !layered || layered->parts_written + gather->nparts == layered->nparts;
     // bytes moved per block: a gathered call moves its parts, which are the whole block
     // unless the call is layered
-    const uint64_t moved = gather ? gather_moved_bytes(*gather) : uint64_t(uint32_t(block_size));
+    const uint64_t moved =
+        gather ? gather_moved_bytes(*gather, write) : uint64_t(uint32_t(block_size));
     int kd = device;
     if (device < 0 && fp8_elems) {
         fail("the fp8 KV path needs a CUDA tensor");
@@ -422,21 +424,25 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
                 auto m = mapping(addr_seg(blocks[i].remote_addr), -1);
                 if (!m || !m->host_ptr) return -1;
                 uint8_t* pool = m->host_ptr + addr_off(blocks[i].remote_addr);
-                if (gather) {  // one memcpy per part, or per (row, slice) of a row-sliced read
+                if (gather) {  // one memcpy per part, or per (row, slice) of a row-sliced call
                     const size_t pb = gather->pool_part_bytes();
                     const Connection::GatherSpec& g = *gather;
                     for (uint32_t s = 0; s < gather->nparts; ++s) {
                         uint8_t* local =
                             reinterpret_cast<uint8_t*>(gather->part_base[s] + local_off[i] * scale);
                         if (g.rows) {
-                            const uint8_t* src = pool + (g.first_part + s) * pb + g.src_col;
+                            uint8_t* stored = pool + (g.first_part + s) * pb + g.src_col;
                             for (uint32_t r = 0; r < g.rows; ++r)
-                                for (uint32_t j = 0; j < g.slices; ++j)
-                                    std::memcpy(local + size_t(r) * g.dst_pitch +
-                                                    size_t(j) * g.dst_slice_pitch,
-                                                src + size_t(r) * g.src_pitch +
-                                                    size_t(j) * g.row_bytes,
-                                                g.row_bytes);
+                                for (uint32_t j = 0; j < g.slices; ++j) {
+                                    uint8_t* l = local + size_t(r) * g.dst_pitch +
+                                                 size_t(j) * g.dst_slice_pitch;
+                                    uint8_t* p = stored + size_t(r) * g.src_pitch +
+                                                 size_t(j) * g.row_bytes;
+                                    if (write)
+                                        std::memcpy(p, l, g.row_bytes);
+                                    else
+                                        std::memcpy(l, p, g.row_bytes);
+                                }
                         } else if (write)
                             std::memcpy(pool + (gather->first_part + s) * pb, local, pb);
                         else
@@ -875,12 +881,17 @@ const char* Connection::gather_refusal(const GatherSpec& g, const uint64_t* offs
     if (end > block_parts) return "the part range runs past the block";
     if (block_parts > uint64_t(INT32_MAX) / g.pool_part_bytes())
         return "bad parts list: a block holds at most 2^31 - 1 bytes";
-    if (g.rows && (write || !kernels::row_geometry_ok(g.rows, g.row_bytes, g.src_pitch,
-                                                      g.src_col, g.dst_pitch, g.slices,
-                                                      g.dst_slice_pitch, g.view_part_bytes())))
-        return "bad row geometry (reads only, rows >= 1, slices >= 1, src_col + slices * "
-               "row_bytes <= src_pitch, part_bytes == rows * src_pitch; with slices > 1, "
-               "disjoint destination slices within 2^32 bytes)";
+    if (g.rows && !kernels::row_geometry_ok(g.rows, g.row_bytes, g.src_pitch, g.src_col,
+                                            g.dst_pitch, g.slices, g.dst_slice_pitch,
+                                            g.view_part_bytes()))
+        return "bad row geometry (rows >= 1, slices >= 1, src_col + slices * row_bytes <= "
+               "src_pitch, part_bytes == rows * src_pitch; with slices > 1, disjoint local "
+               "slices within 2^32 bytes)";
+    // the in-band commit publishes whole blocks: a write fills every byte of a stored part
+    if (g.rows && write &&
+        !kernels::row_write_covers(g.row_bytes, g.src_pitch, g.src_col, g.slices))
+        return "bad row geometry for a write: the rows must fill the stored part (src_col == 0, "
+               "slices * row_bytes == src_pitch)";
     if (g.rows && g.fp8_elems &&
         ((g.row_bytes | g.src_pitch | g.src_col | g.dst_pitch |
           (g.slices > 1 ? g.dst_slice_pitch : 0u)) & 15))
@@ -1195,7 +1206,7 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
         stats_.ns_build += t_launch0 - t_build0;
         stats_.ns_launch += now_ns() - t_launch0;
         // lookup + copy + validate: resolve_descs counted the lookup
-        const uint64_t moved = gather && gather->rows ? gather_moved_bytes(*gather)
+        const uint64_t moved = gather && gather->rows ? gather_moved_bytes(*gather, false)
                                                       : uint64_t(block_size);
         if (scope.launched(e, "device-index read failed to launch: ", plan.fused() ? 1 : 2, false,
                            uint64_t(n) * moved) != 0)

@@ -68,6 +68,43 @@ __device__ __forceinline__ void copy_span(uint8_t* dst, const uint8_t* src, uint
     for (uint32_t b = nvec * 16 + tid; b < len; b += kLdStThreads) dst[b] = src[b];
 }
 
+// A row-sliced write (GatherLaunch::rows with write): stored bytes [off, off + len) of a part
+// to dst (the pool, contiguous), each loaded from the caller's part `src` at row_write_offset
+// (launch_plan.h) of its stored offset.  copy_span's shape: VEC = 16 / 32 keep four / eight
+// 16-byte vectors in flight per thread (row_bytes, dst_pitch, slice_pitch, off, len and both
+// bases aligned to 16; a vector never straddles two slices); VEC = 1: bytes.
+struct RowWrite {
+    uint32_t row_bytes, src_pitch, dst_pitch, slice_pitch;
+};
+template <int VEC>
+__device__ __forceinline__ void copy_span_rows(uint8_t* dst, const uint8_t* src, uint32_t off,
+                                               uint32_t len, const RowWrite& w) {
+    const uint32_t tid = threadIdx.x;
+    const auto at = [&](uint32_t o) {
+        return row_write_offset(o, w.row_bytes, w.src_pitch, w.dst_pitch, w.slice_pitch);
+    };
+    if constexpr (VEC == 1) {
+        for (uint32_t b = tid; b < len; b += kLdStThreads) dst[b] = src[at(off + b)];
+    } else {
+        static_assert(VEC == 16 || VEC == 32, "vector width");
+        constexpr int U = VEC / 4;
+        const uint32_t nvec = len / 16;
+        uint32_t i = tid;
+        for (; i + (U - 1) * kLdStThreads < nvec; i += U * kLdStThreads) {
+            uint4 v[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                const uint8_t* s = src + at(off + (i + u * kLdStThreads) * 16);
+                v[u] = VEC == 16 ? ld_stream_v4(s) : ld_v4(s);
+            }
+#pragma unroll
+            for (int u = 0; u < U; ++u) st_v4(dst + size_t(i + u * kLdStThreads) * 16, v[u]);
+        }
+        for (; i < nvec; i += kLdStThreads)
+            st_v4(dst + size_t(i) * 16, ld_stream_v4(src + at(off + i * 16)));
+    }
+}
+
 // `nrows` rows of row_bytes, row r from src + r * src_pitch to dst + r * dst_pitch.  The 256
 // threads walk the (row, vector) pairs flattened together, so rows much narrower than a CTA's
 // 4 KB per pass (one KV head of 128 bf16 is 256 bytes) still keep every thread busy.  VEC = 16

@@ -195,12 +195,17 @@ struct GatherLaunch {
     // j * dst_slice_pitch - e.g. a token's KV heads into a head-major page [head][token][dim]
     // (launch_plan.h: slice_pair, row_geometry_ok).  slices == 1: the rows above, and
     // dst_slice_pitch is not read.
+    // With write, the same geometry runs the other way (ld/st kernels only, no layered read):
+    // slice j of stored row r is taken from part_base[s] + desc.src + r * dst_pitch + j *
+    // dst_slice_pitch, and the rows must fill the stored part (src_col == 0, slices *
+    // row_bytes == src_pitch; launch_plan.h: row_write_covers, row_write_offset) - e.g. a
+    // head-major page stored token-major.  Works with recs and a layered writer's layer_state.
     uint32_t slices = 1;
     uint32_t dst_slice_pitch = 0;
 };
 // The TMA pipeline for 16-byte aligned parts of at least kPipeMinBytes, the ld/st kernel
 // (kv_copy.cu) otherwise: the same rule launch_kv_copy applies to whole blocks.  A row-sliced
-// read runs kv_scatter_rows (kv_copy.cu).
+// read runs kv_scatter_rows (kv_copy.cu), a row-sliced write kv_gather_rows_write.
 cudaError_t launch_kv_gather(const GatherLaunch& a, cudaStream_t stream);
 cudaError_t launch_kv_pipe_gather(const GatherLaunch& a, cudaStream_t stream);
 struct GatherParts {

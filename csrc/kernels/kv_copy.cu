@@ -329,6 +329,70 @@ cudaError_t launch_kv_scatter_rows(const GatherLaunch& a, cudaStream_t stream) {
     }
 }
 
+// ---------------------------------------------------------------- row-sliced writes (ld/st)
+// GatherLaunch::rows with write: kv_gather_ldst_kernel's items, (block, part, chunk of the
+// stored part) numbered (b * nparts + s) * cpp + c, each storing one contiguous run of pool
+// bytes, so the control warp (publish, or a layered writer's LayerCommit) counts arrivals
+// exactly as for kv_gather_ldst.  Only the local load address differs: stored byte o of part
+// s comes from parts.base[s] + desc.src + row_write_offset(o) (copy_span_rows).
+template <int VEC>
+__global__ void __launch_bounds__(kLdStThreads + 32, 3)
+    kv_gather_rows_write_kernel(const CopyDesc* __restrict__ descs,
+                                const __grid_constant__ GatherParts parts, uint32_t n,
+                                uint32_t nparts, uint32_t part_bytes, uint32_t first_part,
+                                uint32_t chunk, uint32_t cpp, RowWrite geo, Publish pub,
+                                LayerCommit lc) {
+    const uint32_t cpb = nparts * cpp;  // items per block: what the commit counter counts
+    const uint32_t total = n * cpb;
+    if (threadIdx.x >= kLdStThreads) {
+        if (!pub.recs) return;
+        const uint32_t count = blockIdx.x < total ? (total - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+        gather_control_warp(pub, lc, threadIdx.x - kLdStThreads, blockIdx.x, count, gridDim.x,
+                            cpb, nparts, kLdStThreads + 32);
+        return;
+    }
+    uint32_t item = blockIdx.x;
+    CopyDesc next = item < total ? descs[item / cpb] : CopyDesc{0, 0};
+    for (; item < total; item += gridDim.x) {
+        const CopyDesc d = next;
+        const uint32_t nxt = item + gridDim.x;
+        if (nxt < total) next = descs[nxt / cpb];  // prefetch: descriptors may sit in host memory
+        const uint32_t in_block = item % cpb;
+        const uint32_t s = in_block / cpp;
+        const uint32_t off = (in_block % cpp) * chunk;
+        const uint32_t len = min(chunk, part_bytes - off);
+        const uint8_t* src = reinterpret_cast<const uint8_t*>(parts.base[s] + d.src);
+        uint8_t* dst =
+            reinterpret_cast<uint8_t*>(d.dst + uint64_t(first_part + s) * part_bytes + off);
+        copy_span_rows<VEC>(dst, src, off, len, geo);
+    }
+    if (pub.recs) ctrl_barrier_arrive(kLdStThreads + 32);
+}
+
+cudaError_t launch_kv_gather_rows_write(const GatherLaunch& a, cudaStream_t stream) {
+    constexpr int T = kLdStThreads + 32;
+    static const LdStResident res =
+        ldst_resident(kv_gather_rows_write_kernel<16>, kv_gather_rows_write_kernel<32>, T);
+    const LaunchPlan p = plan_gather_rows_write(a, sm_count(), res);
+    if (!p.valid) return cudaErrorInvalidValue;  // the caller checks the geometry and splits
+    GatherParts parts;
+    std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
+    const RowWrite geo{a.row_bytes, a.src_pitch, a.dst_pitch, a.dst_slice_pitch};
+    const auto go = [&](auto* kernel) {
+        kernel<<<p.ctas, T, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.part_bytes, a.first_part,
+                                         p.chunk, p.cpb, geo, publish_of(a, true), layer_of(a));
+        return cudaGetLastError();
+    };
+    switch (p.kernel) {
+        case Kernel::kLdSt1:
+            return go(kv_gather_rows_write_kernel<1>);
+        case Kernel::kLdSt32:
+            return go(kv_gather_rows_write_kernel<32>);
+        default:
+            return go(kv_gather_rows_write_kernel<16>);
+    }
+}
+
 }  // namespace
 
 int sm_count() {
@@ -396,7 +460,8 @@ cudaError_t launch_kv_gather(const GatherLaunch& a, cudaStream_t stream) {
     if (uint64_t(a.nparts) * a.part_bytes > 0xffffffffull) return cudaErrorInvalidValue;
     const bool layered = a.group_flags != nullptr;
     if (layered && !a.group_counters) return cudaErrorInvalidValue;
-    if (a.rows) return launch_kv_scatter_rows(a, stream);
+    if (a.rows)
+        return a.write ? launch_kv_gather_rows_write(a, stream) : launch_kv_scatter_rows(a, stream);
     constexpr int T = kLdStThreads + 32;
     static const LdStResident res =
         ldst_resident(kv_gather_ldst_kernel<16>, kv_gather_ldst_kernel<32>, T);

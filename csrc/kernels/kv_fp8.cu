@@ -9,6 +9,10 @@
 //   kv_read_fp8  : pool block -> dequantised bf16 scattered into the destination pages.
 //   kv_write_fp8_gather / kv_read_fp8_scatter : the same for gathered blocks, whose parts are
 //                  fp8 pages end to end (launch_kv_gather_fp8, fp8_pages.cuh).
+//   kv_read_fp8_rows / _slices, kv_write_fp8_rows : the gathered forms with row geometry
+//                  (GatherLaunch::rows): a read dequantises rows (and slices) of each stored
+//                  page, a write quantises a stored page whose rows are loaded from a strided
+//                  local layout (e.g. a head-major page).
 // The reference moves raw bytes only (dtype-agnostic, infinistore/lib.py:377-379); this is
 // the "write fused with fp8 cast / read fused with gather" item of the north star.
 //
@@ -62,12 +66,34 @@ __device__ __forceinline__ uint4 ld_u4(const void* p) {
     return r;
 }
 
+// Where a lane's 16-byte bf16 load comes from: byte offset from the page's local address of
+// elements 8 * hl .. 8 * hl + 7 of 128-element row `row` of the stored page.  A template
+// policy rather than a runtime branch, so the existing kernels' loop is compiled as before.
+//   DenseRows  the page is contiguous bf16 (every kernel but kv_write_fp8_rows).
+//   SlicedRows a row-sliced write (GatherLaunch::rows): row_write_offset (launch_plan.h) of the
+//              vector's byte in the part's bf16 view; the geometry is in multiples of 16 bytes,
+//              so the 8 elements never straddle two slices.
+struct DenseRows {
+    __device__ __forceinline__ size_t operator()(uint32_t row, uint32_t hl) const {
+        return (size_t(row) * kRow + hl * 8) * 2;
+    }
+};
+struct SlicedRows {
+    uint32_t row_bytes, src_pitch, dst_pitch, slice_pitch;
+    __device__ __forceinline__ size_t operator()(uint32_t row, uint32_t hl) const {
+        return row_write_offset((row * kRow + hl * 8) * 2, row_bytes, src_pitch, dst_pitch,
+                                slice_pitch);
+    }
+};
+
 // Threads [0, 256) quantise + store; warp 8 is the control warp (in-band commit).  Work item
 // k is chunk k % cpp of page k / cpp (`pages`, fp8_pages.cuh); n blocks of pages.nparts pages.
-template <typename Pages>
+// `load_at` places each lane's bf16 load (DenseRows / SlicedRows above).
+template <typename Pages, typename LoadAt = DenseRows>
 __device__ __forceinline__ void write_fp8(const CopyDesc* __restrict__ descs, uint32_t n,
                                           uint32_t elems, uint32_t chunk, uint32_t cpp,
-                                          const Publish& pub, const Pages& pages) {
+                                          const Publish& pub, const Pages& pages,
+                                          const LoadAt& load_at = {}) {
     const uint32_t cpb = cpp * pages.nparts;  // items per block: what the commit counts
     const uint32_t total = n * cpb;
     if (threadIdx.x >= kThreads) {
@@ -92,7 +118,7 @@ __device__ __forceinline__ void write_fp8(const CopyDesc* __restrict__ descs, ui
 #pragma unroll
             for (int u = 0; u < kRowPairs; ++u) {
                 const uint32_t r = r0 + 2 * u + half;
-                if (r < rows) v[u] = ld_u4(src + (size_t(row0 + r) * kRow + hl * 8) * 2);
+                if (r < rows) v[u] = ld_u4(src + load_at(row0 + r, hl));
             }
 #pragma unroll
             for (int u = 0; u < kRowPairs; ++u) {
@@ -179,6 +205,18 @@ __global__ void __launch_bounds__(kThreads + 32)
                                LayerCommit lc) {
     write_fp8(descs, n, elems, chunk, cpp, pub,
               BlockParts<true>{&parts, nparts, first_part, stride, lc});
+}
+
+// GatherLaunch::rows with write: kv_write_fp8_gather_kernel's items and commit
+// (BlockParts<true>), each lane's bf16 vector loaded from its row_write_offset in the part.
+__global__ void __launch_bounds__(kThreads + 32)
+    kv_write_fp8_rows_kernel(const CopyDesc* __restrict__ descs,
+                             const __grid_constant__ GatherParts parts, uint32_t n,
+                             uint32_t nparts, uint32_t elems, uint32_t chunk, uint32_t cpp,
+                             uint32_t first_part, uint64_t stride, SlicedRows geo, Publish pub,
+                             LayerCommit lc) {
+    write_fp8(descs, n, elems, chunk, cpp, pub,
+              BlockParts<true>{&parts, nparts, first_part, stride, lc}, geo);
 }
 
 // The layered read (GatherLaunch::group_flags): kv_gather_ldst's gather_read_layered
@@ -477,6 +515,23 @@ cudaError_t launch_kv_read_fp8_rows(const GatherLaunch& a, uint32_t elems, cudaS
     return layered ? go(kv_read_fp8_rows_kernel<true>) : go(kv_read_fp8_rows_kernel<false>);
 }
 
+cudaError_t launch_kv_write_fp8_rows(const GatherLaunch& a, uint32_t elems, cudaStream_t stream) {
+    static const int res = [] {
+        int r = 1;
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&r, kv_write_fp8_rows_kernel, kThreads + 32, 0);
+        return r > 0 ? r : 1;
+    }();
+    const LaunchPlan p = plan_gather_fp8_rows_write(a, elems, sm_count(), {res, res});
+    if (!p.valid) return cudaErrorInvalidValue;  // the caller checks the geometry and splits
+    GatherParts parts;
+    std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
+    const SlicedRows geo{a.row_bytes, a.src_pitch, a.dst_pitch, a.dst_slice_pitch};
+    kv_write_fp8_rows_kernel<<<p.ctas, kThreads + 32, 0, stream>>>(
+        a.descs, parts, a.n, a.nparts, elems, p.chunk, p.cpb, a.first_part,
+        fp8_gather_bytes(1, elems), geo, publish_of(a, true), layer_of(a));
+    return cudaGetLastError();
+}
+
 }  // namespace
 
 cudaError_t launch_kv_write_fp8(const Fp8Launch& a, cudaStream_t stream) {
@@ -505,7 +560,9 @@ cudaError_t launch_kv_gather_fp8(const GatherLaunch& a, uint32_t elems, int vari
                                  cudaStream_t stream) {
     if (a.n == 0) return cudaSuccess;
     if (!a.part_base) return cudaErrorInvalidValue;
-    if (a.rows) return launch_kv_read_fp8_rows(a, elems, stream);
+    if (a.rows)
+        return a.write ? launch_kv_write_fp8_rows(a, elems, stream)
+                       : launch_kv_read_fp8_rows(a, elems, stream);
     // a layered read takes the ld/st kernel whatever the variant (no layered pipeline)
     const bool layered = a.group_flags != nullptr;
     if (layered && (a.write || !a.group_counters || !a.group_parts || a.nparts % a.group_parts))

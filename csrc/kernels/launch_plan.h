@@ -3,7 +3,8 @@
 // kv_fp8.cu, kv_fp8_pipe.cu) pass in the SM count and the CTAs per SM the ld/st kernels keep
 // resident (occupancy API), so the choice is unit-tested on the CPU
 // (_infinistore.testing.plan_copy / plan_gather / plan_read_fused / plan_fp8 /
-// plan_gather_fp8 / plan_gather_layered / plan_gather_rows / plan_gather_fp8_rows).
+// plan_gather_fp8 / plan_gather_layered / plan_gather_rows / plan_gather_fp8_rows /
+// plan_gather_rows_write / plan_gather_fp8_rows_write).
 #pragma once
 
 #include <algorithm>
@@ -318,6 +319,84 @@ inline LaunchPlan plan_gather_rows(const GatherLaunch& a, int sms, LdStResident 
                std::max(1u, (1u << 20) / a.row_bytes), sms);
     if (parts * p.cpb > kMaxItems) return invalid_plan();
     p.ctas = ldst_grid(p, a.max_ctas, res, sms, parts * p.cpb);
+    return p;
+}
+
+// ---------------------------------------------------------------- row-sliced writes
+// A row-sliced write (GatherLaunch::rows with write) takes the geometry that reads the same
+// local layout back: the stored part is src_pitch-byte rows, the caller's part holds slice j of
+// row r at r * dst_pitch + j * dst_slice_pitch - e.g. a head-major page [head][token][dim]
+// stored token-major.  The in-band commit publishes whole blocks, so a write must fill every
+// byte of the stored part: on top of row_geometry_ok, src_col == 0 and slices * row_bytes ==
+// src_pitch.
+inline bool row_write_covers(uint32_t row_bytes, uint32_t src_pitch, uint32_t src_col,
+                             uint32_t slices) {
+    return src_col == 0 && uint64_t(slices) * row_bytes == src_pitch;
+}
+
+// Where byte o of a fully covered stored part comes from in the caller's part: row r =
+// o / src_pitch, slice j of it, column c - j * row_bytes of that slice.  Over a covering
+// geometry it is the inverse of slice_pair: row_write_offset(slice_pair(q).src + w) ==
+// slice_pair(q).dst + w for every byte w < row_bytes.  The kernels (copy_span.cuh:
+// copy_span_rows, kv_fp8.cu: kv_write_fp8_rows) and the CPU tests
+// (_infinistore.testing.row_write_offset) share this function.
+ISTORE_KHD inline uint32_t row_write_offset(uint32_t o, uint32_t row_bytes, uint32_t src_pitch,
+                                            uint32_t dst_pitch, uint32_t dst_slice_pitch) {
+    const uint32_t r = o / src_pitch, c = o - r * src_pitch, j = c / row_bytes;
+    return r * dst_pitch + j * dst_slice_pitch + (c - j * row_bytes);
+}
+
+// kv_gather_rows_write (launch_kv_gather with rows and write): the work items of the
+// whole-part write, (block, part, chunk of the stored part) numbered (b * nparts + s) * cpp + c
+// with plan_gather's ld/st chunks, so every item stores one contiguous run of pool bytes and
+// the commit counts arrivals as for kv_gather_ldst; only the local load address goes through
+// row_write_offset.  Always the ld/st kernels (no TMA form), never layered reads.  The vector
+// width is the one the OR of row_bytes, dst_pitch, dst_slice_pitch (with slices > 1), the part
+// bases and the local offsets allows (src_pitch is slices * row_bytes).
+inline LaunchPlan plan_gather_rows_write(const GatherLaunch& a, int sms, LdStResident res) {
+    if (!a.write || a.group_flags || a.nparts == 0 || a.nparts > kGatherMaxParts ||
+        !row_geometry_ok(a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.slices,
+                         a.dst_slice_pitch, a.part_bytes) ||
+        !row_write_covers(a.row_bytes, a.src_pitch, a.src_col, a.slices))
+        return invalid_plan();
+    const uint64_t geo_or =
+        a.align_or | a.dst_pitch | (a.slices > 1 ? a.dst_slice_pitch : 0u);
+    const bool aligned16 = aligned_to(a.row_bytes, geo_or, 16);
+    const bool aligned32 = aligned_to(a.row_bytes, geo_or, 32);
+    LaunchPlan p;
+    p.kernel = !aligned16 ? Kernel::kLdSt1 : aligned32 ? Kernel::kLdSt32 : Kernel::kLdSt16;
+    const uint64_t parts = uint64_t(a.n) * a.nparts;
+    ldst_items(p, parts, a.part_bytes, kLdStChunk, 1u << 20, sms);
+    if (parts * p.cpb > kMaxItems) return invalid_plan();
+    p.ctas = ldst_grid(p, a.max_ctas, res, sms, parts * p.cpb);
+    return p;
+}
+
+// kv_write_fp8_rows (launch_kv_gather_fp8 with rows and write): the items of the gathered fp8
+// ld/st write (plan_gather_fp8 with kFp8LdSt: chunks of kFp8Chunk elements of the stored fp8
+// page, or whole pages under ldst_items' rule), the geometry of plan_gather_rows_write in bytes
+// of the part's bf16 view (part_bytes == rows * src_pitch == 2 * elems), and every geometry
+// value, part base and local offset a multiple of 16 bytes, so a lane's 8-element vector never
+// straddles two slices.  The grid is one wave of the CTAs the kernel keeps resident (res.r16,
+// the occupancy API's answer for it).
+inline LaunchPlan plan_gather_fp8_rows_write(const GatherLaunch& a, uint32_t elems, int sms,
+                                             LdStResident res) {
+    if (!a.write || a.group_flags || a.nparts == 0 || a.nparts > kGatherMaxParts ||
+        !row_geometry_ok(a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.slices,
+                         a.dst_slice_pitch, a.part_bytes) ||
+        !row_write_covers(a.row_bytes, a.src_pitch, a.src_col, a.slices))
+        return invalid_plan();
+    const uint64_t geo_or = a.align_or | a.row_bytes | a.src_pitch | a.dst_pitch |
+                            (a.slices > 1 ? a.dst_slice_pitch : 0u);
+    const uint64_t parts = uint64_t(a.n) * a.nparts;
+    if (elems == 0 || elems % 512 != 0 || uint64_t(a.part_bytes) != 2ull * elems ||
+        (geo_or & 15) != 0 || parts > kMaxItems)
+        return invalid_plan();
+    LaunchPlan p;
+    p.kernel = Kernel::kLdStFp8;
+    ldst_items(p, parts, elems, kFp8Chunk, 1u << 19, sms);
+    if (parts * p.cpb > kMaxItems) return invalid_plan();
+    p.ctas = clamp_grid(a.max_ctas > 0 ? a.max_ctas : res.r16 * sms, parts * p.cpb);
     return p;
 }
 

@@ -180,7 +180,7 @@ struct KeyArena {
 
 thread_local KeyArena t_arena;
 
-// A row-sliced read's geometry from its native list, in bytes: (rows, row_bytes, src_pitch,
+// A row-sliced call's geometry from its native list, in bytes: (rows, row_bytes, src_pitch,
 // src_col, dst_pitch) or the same followed by (slices, dst_slice_pitch) into a GatherSpec or a
 // GatherLaunch.  False unless the list has 5 or 7 entries; an empty list is for the caller.
 template <typename G>
@@ -199,8 +199,8 @@ bool set_rows(G& g, const std::vector<uint32_t>& rows) {
 }
 
 // A gathered call's parts: part s at part_base[s] (which must outlive the spec); elems > 0:
-// bf16 parts of elems elements stored as fp8 pages.  rows: a row-sliced read's geometry
-// (set_rows); empty: whole parts.  The connection checks the values.
+// bf16 parts of elems elements stored as fp8 pages.  rows: a row-sliced read's or write's
+// geometry (set_rows); empty: whole parts.  The connection checks the values.
 Connection::GatherSpec gather_spec(const std::vector<uint64_t>& part_base, uint32_t part_bytes,
                                    uint32_t elems, uint32_t first_part,
                                    const std::vector<uint32_t>& rows = {}) {
@@ -214,6 +214,33 @@ Connection::GatherSpec gather_spec(const std::vector<uint64_t>& part_base, uint3
         throw py::value_error("rows is (rows, row_bytes, src_pitch, src_col, dst_pitch[, "
                               "slices, dst_slice_pitch])");
     return g;
+}
+
+// A row-sliced launch as the plan bindings of _infinistore.testing describe it: part_bytes is
+// rows * src_pitch, and group_parts > 0 makes it a layered read (the plans only ask whether
+// group_flags is set).
+kernels::GatherLaunch rows_launch(uint32_t n, uint32_t nparts, bool write, uint32_t rows,
+                                  uint32_t row_bytes, uint32_t src_pitch, uint32_t src_col,
+                                  uint32_t dst_pitch, uint32_t slices, uint32_t dst_slice_pitch,
+                                  uint64_t align_or, uint32_t group_parts, int max_ctas) {
+    static uint32_t flags[1];
+    kernels::GatherLaunch a;
+    a.n = n;
+    a.nparts = nparts;
+    a.write = write;
+    a.part_bytes = uint32_t(uint64_t(rows) * src_pitch);
+    a.rows = rows;
+    a.row_bytes = row_bytes;
+    a.src_pitch = src_pitch;
+    a.src_col = src_col;
+    a.dst_pitch = dst_pitch;
+    a.slices = slices;
+    a.dst_slice_pitch = dst_slice_pitch;
+    a.align_or = align_or;
+    a.group_flags = group_parts ? flags : nullptr;
+    a.group_parts = group_parts;
+    a.max_ctas = max_ctas;
+    return a;
 }
 
 // [(key, offset), ...] -> KeyOffset views (offset * scale bytes).  Also accepted: the pair
@@ -592,22 +619,25 @@ PYBIND11_MODULE(_infinistore, m) {
             "w_rdma_gather",
             [](Connection& c, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
                uint32_t elems, const py::object& offsets, const py::object& remote_blocks,
-               int device, uint64_t stream, uint64_t scale) {
+               int device, uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows) {
                 BlockSpan rb;
                 OffsetSpan off;
                 blocks_from_py(remote_blocks, rb);
                 offsets_from_py(offsets, off);
                 std::vector<uint64_t> bytes(off.n);
                 for (size_t i = 0; i < off.n; ++i) bytes[i] = off.data[i] * scale;
-                const Connection::GatherSpec g = gather_spec(part_base, part_bytes, elems, 0);
+                const Connection::GatherSpec g = gather_spec(part_base, part_bytes, elems, 0, rows);
                 py::gil_scoped_release rel;
                 return c.w_rdma_gather(g, bytes.data(), bytes.size(), rb.data, rb.n, device, stream);
             },
             py::arg("part_base"), py::arg("part_bytes"), py::arg("elems"), py::arg("offsets"),
             py::arg("remote_blocks"), py::arg("device") = -1, py::arg("stream") = 0,
-            py::arg("scale") = 1,
+            py::arg("scale") = 1, py::arg("rows") = std::vector<uint32_t>{},
             "gathered write: block i = part s at part_base[s] + offsets[i] * scale, s = 0..S-1; "
-            "elems > 0: bf16 parts of elems elements, quantised into fp8 page s of block i")
+            "elems > 0: bf16 parts of elems elements, quantised into fp8 page s of block i; "
+            "rows = (rows, row_bytes, src_pitch, 0, dst_pitch[, slices, dst_slice_pitch]) filling "
+            "each stored part: slice j of stored row r from part_base[s] + offset + r * "
+            "dst_pitch + j * dst_slice_pitch")
         .def(
             "r_rdma_scatter",
             [](Connection& c, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
@@ -669,17 +699,18 @@ PYBIND11_MODULE(_infinistore, m) {
             "w_rdma_layered",
             [](Connection& c, Connection::GatherWriter& w, const std::vector<uint64_t>& part_base,
                uint32_t part_bytes, uint32_t elems, uint32_t first_part, int device,
-               uint64_t stream, uint64_t scale) {
+               uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows) {
                 const Connection::GatherSpec g =
-                    gather_spec(part_base, part_bytes, elems, first_part);
+                    gather_spec(part_base, part_bytes, elems, first_part, rows);
                 py::gil_scoped_release rel;
                 return c.write_layered(w, g, scale, device, stream);
             },
             py::arg("writer"), py::arg("part_base"), py::arg("part_bytes"), py::arg("elems"),
             py::arg("first_part"), py::arg("device") = -1, py::arg("stream") = 0,
-            py::arg("scale") = 1,
+            py::arg("scale") = 1, py::arg("rows") = std::vector<uint32_t>{},
             "layered write: stored part first_part + s of every block of the writer <- "
-            "part_base[s] + offset * scale; elems > 0: fp8 parts of elems bf16 elements")
+            "part_base[s] + offset * scale; elems > 0: fp8 parts of elems bf16 elements; rows "
+            "as for w_rdma_gather")
         .def(
             "rw_local",
             [](Connection& c, const std::string& op, const py::object& blocks, int block_size,
@@ -1026,7 +1057,8 @@ PYBIND11_MODULE(_infinistore, m) {
         "last of its layer_parts parts; layer_claim: this launch claims the index ways.  "
         "group_flags (reads): a layered read that stores group_seq to group_flags[g] once "
         "group g (group_parts parts of every block) has landed; group_counters: one zeroed "
-        "u32 per group");
+        "u32 per group.  rows (5 or 7 values): a row-sliced read, or a write whose rows fill "
+        "each stored part");
     k.def(
         "kv_gather_fp8",
         [](uint64_t descs, uint32_t n, const std::vector<uint64_t>& part_base, uint32_t elems,
@@ -1083,9 +1115,10 @@ PYBIND11_MODULE(_infinistore, m) {
         py::arg("rows") = std::vector<uint32_t>{},
         "gathered fp8 blocks: descs as for kv_gather; part s (elems bf16 elements at "
         "part_base[s] + local offset) <-> fp8 page first_part + s of the block; layer_* and "
-        "group_* as for kv_gather (a layered read always runs the ld/st kernel); rows (reads) "
-        "as for kv_gather, in bytes of the parts' bf16 view: those rows of each fp8 page, "
-        "dequantised (kv_read_fp8_rows)");
+        "group_* as for kv_gather (a layered read always runs the ld/st kernel); rows as for "
+        "kv_gather, in bytes of the parts' bf16 view: a read dequantises those rows of each "
+        "fp8 page (kv_read_fp8_rows), a write quantises stored pages whose rows it loads from "
+        "the strided parts (kv_write_fp8_rows)");
     k.def(
         "stream_wait_value",
         [](uint64_t addr, uint32_t value, uint64_t stream) {
@@ -1517,6 +1550,17 @@ PYBIND11_MODULE(_infinistore, m) {
           },
           py::arg("q"), py::arg("rows"), py::arg("row"), py::arg("src_pitch"),
           py::arg("src_col"), py::arg("dst_pitch"), py::arg("dst_slice_pitch"));
+    // row-sliced writes: where byte o of a fully covered stored part comes from
+    t.def("row_write_offset",
+          [](uint32_t o, uint32_t row_bytes, uint32_t src_pitch, uint32_t dst_pitch,
+             uint32_t dst_slice_pitch) {
+              if (!row_bytes || !src_pitch) throw py::value_error("needs row_bytes, src_pitch > 0");
+              return kernels::row_write_offset(o, row_bytes, src_pitch, dst_pitch, dst_slice_pitch);
+          },
+          py::arg("o"), py::arg("row_bytes"), py::arg("src_pitch"), py::arg("dst_pitch"),
+          py::arg("dst_slice_pitch"));
+    t.def("row_write_covers", &kernels::row_write_covers, py::arg("row_bytes"),
+          py::arg("src_pitch"), py::arg("src_col"), py::arg("slices"));
     t.def("row_geometry_ok", &kernels::row_geometry_ok, py::arg("rows"), py::arg("row_bytes"),
           py::arg("src_pitch"), py::arg("src_col"), py::arg("dst_pitch"), py::arg("slices"),
           py::arg("dst_slice_pitch"), py::arg("part_bytes"));
@@ -1639,22 +1683,9 @@ PYBIND11_MODULE(_infinistore, m) {
                       uint32_t src_pitch, uint32_t src_col, uint32_t dst_pitch, uint64_t align_or,
                       uint32_t group_parts, int max_ctas, int sm_count, int resident16,
                       int resident32, uint32_t slices, uint32_t dst_slice_pitch) {
-              static uint32_t flags[1];  // the plan only asks whether the read is layered
-              kernels::GatherLaunch a;
-              a.n = n;
-              a.nparts = nparts;
-              a.part_bytes = uint32_t(uint64_t(rows) * src_pitch);
-              a.rows = rows;
-              a.row_bytes = row_bytes;
-              a.src_pitch = src_pitch;
-              a.src_col = src_col;
-              a.dst_pitch = dst_pitch;
-              a.slices = slices;
-              a.dst_slice_pitch = dst_slice_pitch;
-              a.align_or = align_or;
-              a.group_flags = group_parts ? flags : nullptr;
-              a.group_parts = group_parts;
-              a.max_ctas = max_ctas;
+              const kernels::GatherLaunch a =
+                  rows_launch(n, nparts, false, rows, row_bytes, src_pitch, src_col, dst_pitch,
+                              slices, dst_slice_pitch, align_or, group_parts, max_ctas);
               return plan_dict(kernels::plan_gather_rows(a, sm_count, {resident16, resident32}));
           },
           py::arg("n"), py::arg("nparts"), py::arg("rows"), py::arg("row_bytes"),
@@ -1712,23 +1743,9 @@ PYBIND11_MODULE(_infinistore, m) {
                       uint32_t row_bytes, uint32_t src_pitch, uint32_t src_col, uint32_t dst_pitch,
                       uint64_t align_or, uint32_t group_parts, bool write, int max_ctas,
                       int sm_count, int resident, uint32_t slices, uint32_t dst_slice_pitch) {
-              static uint32_t flags[1];  // the plan only asks whether the read is layered
-              kernels::GatherLaunch a;
-              a.n = n;
-              a.nparts = nparts;
-              a.write = write;
-              a.part_bytes = uint32_t(uint64_t(rows) * src_pitch);
-              a.rows = rows;
-              a.row_bytes = row_bytes;
-              a.src_pitch = src_pitch;
-              a.src_col = src_col;
-              a.dst_pitch = dst_pitch;
-              a.slices = slices;
-              a.dst_slice_pitch = dst_slice_pitch;
-              a.align_or = align_or;
-              a.group_flags = group_parts ? flags : nullptr;
-              a.group_parts = group_parts;
-              a.max_ctas = max_ctas;
+              const kernels::GatherLaunch a =
+                  rows_launch(n, nparts, write, rows, row_bytes, src_pitch, src_col, dst_pitch,
+                              slices, dst_slice_pitch, align_or, group_parts, max_ctas);
               return plan_dict(
                   kernels::plan_gather_fp8_rows(a, elems, sm_count, {resident, resident}));
           },
@@ -1737,6 +1754,41 @@ PYBIND11_MODULE(_infinistore, m) {
           py::arg("align_or") = 0, py::arg("group_parts") = 0, py::arg("write") = false,
           py::arg("max_ctas") = 0, py::arg("sm_count") = 132, py::arg("resident") = 1,
           py::arg("slices") = 1, py::arg("dst_slice_pitch") = 0);
+    // row-sliced writes (kernels/launch_plan.h); group_parts > 0 asks for a layered read, which
+    // the write plans refuse
+    t.def("plan_gather_rows_write",
+          [plan_dict](uint32_t n, uint32_t nparts, uint32_t rows, uint32_t row_bytes,
+                      uint32_t src_pitch, uint32_t src_col, uint32_t dst_pitch, uint32_t slices,
+                      uint32_t dst_slice_pitch, uint64_t align_or, bool write,
+                      uint32_t group_parts, int max_ctas, int sm_count, int resident16,
+                      int resident32) {
+              const kernels::GatherLaunch a =
+                  rows_launch(n, nparts, write, rows, row_bytes, src_pitch, src_col, dst_pitch,
+                              slices, dst_slice_pitch, align_or, group_parts, max_ctas);
+              return plan_dict(
+                  kernels::plan_gather_rows_write(a, sm_count, {resident16, resident32}));
+          },
+          py::arg("n"), py::arg("nparts"), py::arg("rows"), py::arg("row_bytes"),
+          py::arg("src_pitch"), py::arg("src_col") = 0, py::arg("dst_pitch") = 0,
+          py::arg("slices") = 1, py::arg("dst_slice_pitch") = 0, py::arg("align_or") = 0,
+          py::arg("write") = true, py::arg("group_parts") = 0, py::arg("max_ctas") = 0,
+          py::arg("sm_count") = 132, py::arg("resident16") = 1, py::arg("resident32") = 1);
+    t.def("plan_gather_fp8_rows_write",
+          [plan_dict](uint32_t n, uint32_t nparts, uint32_t elems, uint32_t rows,
+                      uint32_t row_bytes, uint32_t src_pitch, uint32_t src_col, uint32_t dst_pitch,
+                      uint32_t slices, uint32_t dst_slice_pitch, uint64_t align_or, bool write,
+                      uint32_t group_parts, int max_ctas, int sm_count, int resident) {
+              const kernels::GatherLaunch a =
+                  rows_launch(n, nparts, write, rows, row_bytes, src_pitch, src_col, dst_pitch,
+                              slices, dst_slice_pitch, align_or, group_parts, max_ctas);
+              return plan_dict(
+                  kernels::plan_gather_fp8_rows_write(a, elems, sm_count, {resident, resident}));
+          },
+          py::arg("n"), py::arg("nparts"), py::arg("elems"), py::arg("rows"), py::arg("row_bytes"),
+          py::arg("src_pitch"), py::arg("src_col") = 0, py::arg("dst_pitch") = 0,
+          py::arg("slices") = 1, py::arg("dst_slice_pitch") = 0, py::arg("align_or") = 0,
+          py::arg("write") = true, py::arg("group_parts") = 0, py::arg("max_ctas") = 0,
+          py::arg("sm_count") = 132, py::arg("resident") = 1);
     t.def("fp8_rows_read_bytes", &fp8_rows_read_bytes, py::arg("rows"), py::arg("row_bytes"),
           py::arg("src_pitch"), py::arg("src_col") = 0,
           "bytes_read of a row-sliced read of one stored fp8 part (geometry in bf16 bytes)");

@@ -343,7 +343,12 @@ class PartRows:
     from ``src_offset``: slice j of row r lands at ``r * dst_pitch + j * dst_slice_pitch``.
     With one KV head per slice, ``dst_pitch = head_dim`` and ``dst_slice_pitch = tokens *
     head_dim`` land a token-major page's heads in a head-major ``[head][token][dim]`` page
-    (``HeadMajorKVCache``).  With ``slices == 1``, ``dst_slice_pitch`` is not used."""
+    (``HeadMajorKVCache``).  With ``slices == 1``, ``dst_slice_pitch`` is not used.
+
+    A gathered write (``rdma_write_cache_gather(rows=...)``, ``GatherWriter.write``) takes the
+    geometry that reads the same local layout back and runs it the other way: stored row r is
+    filled from ``r * dst_pitch + j * dst_slice_pitch`` for its slices j.  Its rows must fill
+    the stored part: ``src_offset == 0`` and ``slices * width == src_pitch``."""
 
     __slots__ = ("count", "width", "src_pitch", "src_offset", "dst_pitch", "slices",
                  "dst_slice_pitch")
@@ -695,14 +700,15 @@ class InfinityConnection:
     # ------------------------------------------------------------------ gathered blocks
     def _gather_parts(self, parts, offsets, part_size: int, first_part: int = 0,
                       block_parts=None, fp8: bool = False, rows: "PartRows | None" = None, *,
-                      nblocks=None, stream="current"):
+                      nblocks=None, stream="current", write: bool = False):
         """Checks a gathered call before anything is enqueued: parts ``first_part ..
         first_part + len(parts) - 1`` of the blocks at ``offsets`` (elements, a list or an int64
         ndarray; ``nblocks`` of them when given), in a parts list ``[(tensor, base), ...]``, of
         blocks that hold ``block_parts`` parts (default ``first_part + len(parts)``).  ``fp8``:
         the parts are bf16 CUDA tensors, ``part_size`` is a multiple of 512 elements and every
-        part base and offset is 16-byte aligned.  ``rows``: a row-sliced read (with ``fp8``,
-        its geometry in multiples of 8 elements).  Returns
+        part base and offset is 16-byte aligned.  ``rows``: a row-sliced call (with ``fp8``,
+        its geometry in multiples of 8 elements); with ``write`` its rows must fill the stored
+        part (``src_offset == 0`` and ``slices * width == src_pitch``).  Returns
         (absolute byte address of every part, device ordinal or -1, element size, int64
         offsets, stream handle)."""
         if self._mode != "rdma":
@@ -716,6 +722,10 @@ class InfinityConnection:
         if first_part < 0:
             raise ValueError("first_part must not be negative")
         extent = rows.check(part_size) if rows is not None else int(part_size)
+        if write and rows is not None and (rows.src_offset != 0
+                                           or rows.slices * rows.width != rows.src_pitch):
+            raise ValueError(f"{rows}: a row-sliced write must fill the stored part "
+                             f"(src_offset == 0 and slices * width == src_pitch)")
         parts = list(parts)
         if not 1 <= len(parts) <= GATHER_MAX_PARTS:
             raise ValueError(f"a parts list holds 1 to {GATHER_MAX_PARTS} parts, not {len(parts)}")
@@ -756,7 +766,7 @@ class InfinityConnection:
             if rows is not None and any(v % 8 for v in (
                     rows.width, rows.src_pitch, rows.src_offset, rows.dst_pitch,
                     rows.dst_slice_pitch if rows.slices > 1 else 0)):
-                raise ValueError(f"{rows}: row-sliced reads of fp8 blocks need width, "
+                raise ValueError(f"{rows}: row-sliced fp8 blocks need width, "
                                  f"src_pitch, src_offset, dst_pitch and dst_slice_pitch in "
                                  f"multiples of 8 elements (one 16-byte vector)")
             align = 0
@@ -775,7 +785,7 @@ class InfinityConnection:
         return bases, dev, es, offs, _stream_of(first, stream)
 
     def rdma_write_cache_gather(self, parts, offsets, part_size: int, remote_blocks,
-                                stream="current"):
+                                stream="current", rows: "PartRows | None" = None):
         """Write block ``i`` as the concatenation over ``s`` of
         ``parts[s][0].view(-1)[parts[s][1] + offsets[i] : ... + part_size]``.
 
@@ -787,13 +797,24 @@ class InfinityConnection:
         ``len(parts) * part_size * element_size`` bytes; that is trusted, as
         ``rdma_write_cache`` trusts ``page_size``.  Blocks the server marked as already
         existing are skipped (first writer wins); the in-band commit publishes a block once,
-        after all of its parts have landed.  CPU tensors need a host-memory pool."""
-        bases, dev, es, offs, s = self._gather_parts(parts, offsets, part_size,
-                                                     nblocks=len(remote_blocks), stream=stream)
+        after all of its parts have landed.  CPU tensors need a host-memory pool.
+
+        ``rows`` (a :class:`PartRows`, the geometry that reads the same layout back with
+        ``read_cache_scatter(rows=...)``) fills each stored part of ``part_size`` elements from
+        a strided local layout: slice j of stored row r is taken from ``parts[s][1] + offset +
+        r * rows.dst_pitch + j * rows.dst_slice_pitch``.  The rows must fill the stored part
+        (``src_offset == 0``, ``slices * width == src_pitch``), e.g. a head-major page
+        ``[head][token][dim]`` stored token-major.  The stored bytes are those of a write
+        without rows from the transposed page.  Bad geometry raises ``ValueError`` before
+        anything is enqueued."""
+        bases, dev, es, offs, s = self._gather_parts(parts, offsets, part_size, rows=rows,
+                                                     nblocks=len(remote_blocks), stream=stream,
+                                                     write=True)
+        native_rows = rows.native(es) if rows is not None else []
         if not len(offs):
             return 0
         ret = self.conn.w_rdma_gather(bases, int(part_size) * es, 0, offs, remote_blocks, dev, s,
-                                      es)
+                                      es, native_rows)
         if ret < 0:
             raise Exception(f"Failed to write to infinistore, ret = {ret}: {self.conn.last_error()}")
         return 0
@@ -837,20 +858,24 @@ class InfinityConnection:
         return _infinistore.kernels.fp8_gather_bytes(int(nparts), int(part_size))
 
     def rdma_write_cache_gather_fp8(self, parts, offsets, part_size: int, remote_blocks,
-                                    stream="current"):
+                                    stream="current", rows: "PartRows | None" = None):
         """``rdma_write_cache_gather`` with every part quantised to e4m3 (one fp32 scale per
         128 elements) inside the write kernel: part ``s`` of a block is the fp8 page that
         ``rdma_write_cache_fp8`` would store for it, at byte
         ``fp8_gather_block_bytes(s, part_size)`` of the block, so a block takes 0.516 of its
         bf16 bytes.  The parts are bf16 CUDA tensors, ``part_size`` is a multiple of 512
         elements, and part bases and offsets are 16-byte aligned.  The blocks must have been
-        allocated with ``fp8_gather_block_bytes(len(parts), part_size)`` bytes."""
+        allocated with ``fp8_gather_block_bytes(len(parts), part_size)`` bytes.  ``rows`` as
+        for ``rdma_write_cache_gather``, in multiples of 8 elements: each stored page is the
+        one the write without rows stores for the transposed page."""
         bases, dev, es, offs, s = self._gather_parts(parts, offsets, part_size, fp8=True,
-                                                     nblocks=len(remote_blocks), stream=stream)
+                                                     rows=rows, nblocks=len(remote_blocks),
+                                                     stream=stream, write=True)
+        native_rows = rows.native(es) if rows is not None else []
         if not len(offs):
             return 0
         ret = self.conn.w_rdma_gather(bases, int(part_size) * es, int(part_size), offs,
-                                      remote_blocks, dev, s, es)
+                                      remote_blocks, dev, s, es, native_rows)
         if ret < 0:
             raise Exception(f"Failed to write to infinistore, ret = {ret}: {self.conn.last_error()}")
         return 0
@@ -1199,14 +1224,17 @@ class GatherWriter:
     def failed(self) -> bool:
         return self._w.failed
 
-    def write(self, parts, first_part: int, stream="current") -> None:
+    def write(self, parts, first_part: int, stream="current",
+              rows: "PartRows | None" = None) -> None:
         """Store parts ``first_part .. first_part + len(parts) - 1`` of every block: stored
         part ``first_part + s`` of block i is ``parts[s][0].view(-1)[parts[s][1] + offsets[i]
         : ... + part_size]``.  ``parts`` is ``[(tensor, base), ...]`` as for
         ``rdma_write_cache_gather``.  The first call fixes the device and the dtype.  Raises
         ``ValueError``, with nothing enqueued, for a range that overlaps parts written before
         or runs past the block, another device or dtype, a complete or failed writer, and
-        everything ``rdma_write_cache_gather`` (``_gather_fp8``) refuses."""
+        everything ``rdma_write_cache_gather`` (``_gather_fp8``) refuses.  ``rows`` as for
+        ``rdma_write_cache_gather``; one call may take rows and another not, and every call
+        stores whole parts."""
         if self._w.failed or self._w.complete:
             raise ValueError("the writer is complete or has failed")
         parts = list(parts)
@@ -1219,14 +1247,17 @@ class GatherWriter:
             raise ValueError("the part range overlaps parts written before")
         conn = self._conn
         bases, dev, es, _, s = conn._gather_parts(parts, self._offs, self.part_size, first_part,
-                                                  self.nparts, self.fp8, stream=stream)
+                                                  self.nparts, self.fp8, rows, stream=stream,
+                                                  write=True)
+        native_rows = rows.native(es) if rows is not None else []
         first = parts[0][0]
         if self._dev is not None and self._dev != (first.device, first.dtype):
             raise ValueError(f"parts on {first.device} as {first.dtype}, the writer's first call "
                              f"used {self._dev[0]} as {self._dev[1]}")
         self._dev = (first.device, first.dtype)
         ret = conn.conn.w_rdma_layered(self._w, bases, self.part_size * es,
-                                       self.part_size if self.fp8 else 0, first_part, dev, s, es)
+                                       self.part_size if self.fp8 else 0, first_part, dev, s, es,
+                                       native_rows)
         if ret < 0:
             raise Exception(f"Failed to write to infinistore, ret = {ret}: "
                             f"{conn.conn.last_error()}")

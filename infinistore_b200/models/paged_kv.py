@@ -20,10 +20,11 @@ def layer_keys(layout: KVLayout, tp_rank: int, layer: int, kv: int,
 class _PagedCache:
     """What the token-major :class:`PagedKVCache` and the head-major :class:`HeadMajorKVCache`
     share: ``data[layer, kv, page]`` is one page of ``layout.page_elems`` elements, per-layer
-    and all-layer keys, and the reads of all-layer pages (one key per page, parts 2l (K) and
-    2l + 1 (V)), from ranks at this or another tensor-parallel degree.  The pages are
-    byte-identical in the store whichever cache wrote them; a subclass gives only where a
-    source rank's heads land in its page layout (``_source_rows``)."""
+    and all-layer keys, and the writes and reads of all-layer pages (one key per page, parts
+    2l (K) and 2l + 1 (V)), read from ranks at this or another tensor-parallel degree.  The
+    pages are byte-identical in the store whichever cache wrote them; a subclass gives only
+    where a source rank's heads land in its page layout (``_source_rows``) and how its page
+    fills a stored part (``_write_rows``)."""
 
     def __init__(self, layout: KVLayout, num_pages: int, tp_rank: int, data: torch.Tensor):
         self.layout = layout
@@ -56,12 +57,12 @@ class _PagedCache:
     def _check_fp8(self, rows: bool = False):
         if self.data.dtype != torch.bfloat16 or self.data.device.type != "cuda":
             raise ValueError("fp8 all-layer pages need a bf16 cache on a CUDA device")
-        # a read that regroups heads dequantises them in 8-element vectors; a head need not
+        # a read or write that regroups heads moves them in 8-element vectors; a head need not
         # fill a 128-element scale group
         if rows and self.layout.head_dim % 8:
-            raise ValueError(f"fp8 pages read head by head (written at another TP degree, or "
-                             f"into a head-major cache) need a head_dim that is a multiple of "
-                             f"8, not {self.layout.head_dim}")
+            raise ValueError(f"fp8 pages moved head by head (read from another TP degree, or "
+                             f"into or out of a head-major cache) need a head_dim that is a "
+                             f"multiple of 8, not {self.layout.head_dim}")
 
     def _cross_tp(self, source_tp: Optional[int]) -> bool:
         """Whether a read of pages written at ``source_tp`` regroups heads."""
@@ -105,6 +106,50 @@ class _PagedCache:
             raise ValueError(f"layers must be a non-empty step-1 range within "
                              f"0..{self.layout.layers}")
         return layers
+
+    def _write_rows(self) -> Optional[PartRows]:
+        """How this cache's page fills a stored token-major part on a write: the ``PartRows``
+        (None: the page is the stored part, written whole)."""
+        raise NotImplementedError
+
+    def write_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
+                    stream="current", fp8: bool = False) -> int:
+        """Upload every layer's K and V of each page under one key per page.  ``fp8``: every
+        part is stored as e4m3 with per-128 scales (``rdma_write_cache_gather_fp8``), about
+        half the pool bytes; read such pages back with ``read_pages(fp8=True)``.  The stored
+        pages are the same whichever cache writes them.  Blocks whose key already exists are
+        skipped (first writer wins).  Returns the number of blocks written."""
+        rows = self._write_rows()
+        if fp8:
+            self._check_fp8(rows is not None)  # before any block is allocated
+        self._ensure_registered(conn)
+        layers = range(self.layout.layers)
+        keys = self.page_keys(page_hashes)
+        elems = self.layout.page_elems
+        nbytes = (conn.fp8_gather_block_bytes(2 * len(layers), elems) if fp8
+                  else 2 * len(layers) * self.layout.page_bytes)
+        blocks = conn.allocate_rdma(keys, nbytes)
+        offs = np.asarray(pages, dtype=np.int64) * elems
+        write = conn.rdma_write_cache_gather_fp8 if fp8 else conn.rdma_write_cache_gather
+        write(self._parts(layers), offs, elems, blocks, stream=stream, rows=rows)
+        return len(keys)
+
+    def page_writer(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
+                    fp8: bool = False) -> "PageWriter":
+        """Allocate all-layer pages (as ``write_pages``) and return a writer that stores them
+        layer by layer: ``write_layers(range(l, l + 1))`` right after layer l has produced its
+        KV, so the upload overlaps the next layer's compute and one key per page is kept.
+        Read the pages back with ``read_pages(fp8=fp8)``."""
+        if fp8:
+            self._check_fp8(self._write_rows() is not None)  # before any block is allocated
+        self._ensure_registered(conn)
+        nparts = 2 * self.layout.layers
+        elems = self.layout.page_elems
+        nbytes = (conn.fp8_gather_block_bytes(nparts, elems) if fp8
+                  else nparts * self.layout.page_bytes)
+        blocks = conn.allocate_rdma(self.page_keys(page_hashes), nbytes)
+        offs = np.asarray(pages, dtype=np.int64) * elems
+        return PageWriter(self, conn.gather_writer(blocks, offs, nparts, elems, fp8=fp8))
 
     def read_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
                    layers: Optional[range] = None, stream="current", fp8: bool = False,
@@ -278,48 +323,14 @@ class PagedKVCache(_PagedCache):
                 np.asarray(pages, dtype=np.int64) * self.layout.page_elems, None,
                 self.layout.page_elems)
 
-    def write_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
-                    stream="current", fp8: bool = False) -> int:
-        """Upload every layer's K and V of each page under one key per page.  ``fp8``: every
-        part is stored as e4m3 with per-128 scales (``rdma_write_cache_gather_fp8``), about
-        half the pool bytes; read such pages back with ``read_pages(fp8=True)``.  Returns the
-        number of blocks written."""
-        if fp8:
-            self._check_fp8()  # before any block is allocated
-        self._ensure_registered(conn)
-        layers = range(self.layout.layers)
-        keys = self.page_keys(page_hashes)
-        elems = self.layout.page_elems
-        nbytes = (conn.fp8_gather_block_bytes(2 * len(layers), elems) if fp8
-                  else 2 * len(layers) * self.layout.page_bytes)
-        blocks = conn.allocate_rdma(keys, nbytes)
-        offs = np.asarray(pages, dtype=np.int64) * elems
-        write = conn.rdma_write_cache_gather_fp8 if fp8 else conn.rdma_write_cache_gather
-        write(self._parts(layers), offs, elems, blocks, stream=stream)
-        return len(keys)
-
-    def page_writer(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
-                    fp8: bool = False) -> "PageWriter":
-        """Allocate all-layer pages (as ``write_pages``) and return a writer that stores them
-        layer by layer: ``write_layers(range(l, l + 1))`` right after layer l has produced its
-        KV, so the upload overlaps the next layer's compute and one key per page is kept.
-        Read the pages back with ``read_pages(fp8=fp8)``."""
-        if fp8:
-            self._check_fp8()  # before any block is allocated
-        self._ensure_registered(conn)
-        nparts = 2 * self.layout.layers
-        elems = self.layout.page_elems
-        nbytes = (conn.fp8_gather_block_bytes(nparts, elems) if fp8
-                  else nparts * self.layout.page_bytes)
-        blocks = conn.allocate_rdma(self.page_keys(page_hashes), nbytes)
-        offs = np.asarray(pages, dtype=np.int64) * elems
-        return PageWriter(self, conn.gather_writer(blocks, offs, nparts, elems, fp8=fp8))
+    def _write_rows(self):
+        return None  # the stored layout: whole parts
 
 
 class PageWriter:
-    """Layer-by-layer upload of all-layer pages (``PagedKVCache.page_writer``)."""
+    """Layer-by-layer upload of all-layer pages (``page_writer`` of either cache)."""
 
-    def __init__(self, cache: PagedKVCache, writer):
+    def __init__(self, cache: _PagedCache, writer):
         self.cache = cache
         self.writer = writer
 
@@ -332,7 +343,8 @@ class PageWriter:
         n = self.cache.layout.layers
         if layers.step != 1 or not len(layers) or layers.start < 0 or layers.stop > n:
             raise ValueError(f"layers must be a non-empty step-1 range within 0..{n}")
-        self.writer.write(self.cache._parts(layers), 2 * layers.start, stream=stream)
+        self.writer.write(self.cache._parts(layers), 2 * layers.start, stream=stream,
+                          rows=self.cache._write_rows())
 
 
 class PageRead:
@@ -384,11 +396,13 @@ class HeadMajorKVCache(_PagedCache):
     runs on the decode GPU.  The reference hands opaque bytes to the consumer
     (infinistore/lib.py:377-379), which then repacks them itself.
 
-    All-layer pages (``PagedKVCache.write_pages`` / ``page_writer``, one key per page) are
-    read with ``read_pages`` / ``read_pages_layered``, in bf16 or fp8 and from writers at any
-    TP degree, with the semantics and refusals of the ``PagedKVCache`` methods: the read
+    All-layer pages (one key per page) are written with ``write_pages`` / ``page_writer`` and
+    read with ``read_pages`` / ``read_pages_layered``, in bf16 or fp8, read from writers at
+    any TP degree, with the semantics and refusals of the ``PagedKVCache`` methods: the read
     kernel lands each source's heads as ``[head][token][dim]`` itself (sliced rows,
-    ``PartRows(slices=)``), one block per (page, source rank)."""
+    ``PartRows(slices=)``), one block per (page, source rank), and the write kernel gathers
+    each stored token-major part from the head-major page with the same geometry, so the
+    stored pages are the ones ``PagedKVCache`` stores for the transposed data."""
 
     def __init__(self, layout: KVLayout, num_pages: int, device, tp_rank: int = 0):
         super().__init__(layout, num_pages, tp_rank,
@@ -422,3 +436,14 @@ class HeadMajorKVCache(_PagedCache):
         rows = PartRows(tokens, dim, wl.heads_per_rank * dim, src_head * dim, dst_pitch=dim,
                         slices=heads, dst_slice_pitch=tokens * dim)
         return rows, tokens * dim
+
+    def _write_rows(self):
+        """This rank's own read geometry, run the other way: stored row r (a token) takes head
+        j from ``r * head_dim + j * page_tokens * head_dim``.  A rank with one head already
+        stores ``[token][dim]``: whole parts."""
+        lay = self.layout
+        tokens, dim, heads = lay.page_tokens, lay.head_dim, lay.heads_per_rank
+        if heads == 1:
+            return None
+        return PartRows(tokens, dim, heads * dim, 0, dst_pitch=dim, slices=heads,
+                        dst_slice_pitch=tokens * dim)

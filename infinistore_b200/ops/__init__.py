@@ -129,7 +129,11 @@ def kv_gather(descs: torch.Tensor, part_base: Sequence[int], part_bytes: int, wr
     destination + ``r * dst_pitch``; ``part_bytes`` must be ``rows * src_pitch``.  Seven
     values, (..., slices, dst_slice_pitch), make it sliced: slice j of row r at
     ``r * src_pitch + src_col + j * row_bytes`` -> destination + ``r * dst_pitch + j *
-    dst_slice_pitch`` (e.g. token-major KV heads into a head-major page)."""
+    dst_slice_pitch`` (e.g. token-major KV heads into a head-major page).  A write with
+    ``rows`` runs the same geometry the other way (kv_gather_rows_write): slice j of stored row
+    r is taken from part s's local address + ``r * dst_pitch + j * dst_slice_pitch``; the rows
+    must fill the stored part (``src_col == 0``, ``slices * row_bytes == src_pitch``), and
+    ``publish`` / ``layer`` / ``claim`` work as without rows."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
     bases = [int(b) for b in part_base]
     for b in bases:
@@ -351,7 +355,10 @@ def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, wri
     rows (kv_read_fp8_rows, whatever the variant): row r from bf16 byte
     ``r * src_pitch + src_col`` of the page -> part s's destination + ``r * dst_pitch``.
     Seven values slice the rows as for ``kv_gather`` (``dst_slice_pitch`` a multiple of 16
-    too)."""
+    too).  A write with ``rows`` quantises each stored page whose bf16 rows it loads from the
+    strided local part, as ``kv_gather``'s row write does (kv_write_fp8_rows, whatever the
+    variant); the rows must fill the stored part, and ``publish`` / ``layer`` / ``claim`` work
+    as without rows."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
     bases = [int(b) for b in part_base]
     for b in bases:
