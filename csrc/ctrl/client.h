@@ -211,6 +211,12 @@ class Connection {
         // fill the stored part (kernels::row_write_covers)
         uint32_t rows = 0, row_bytes = 0, src_pitch = 0, src_col = 0, dst_pitch = 0;
         uint32_t slices = 1, dst_slice_pitch = 0;
+        // pieces > 1 (with rows): block i's local layout is `pieces` runs of rows / pieces rows,
+        // run t at part_base[s] + the block's offset + piece_off[i * pieces + t], a host array
+        // in the units of the call's offsets (kernels::GatherLaunch::pieces) - e.g. a chunk of
+        // k engine pages under one key, each page where the caller's block table puts it
+        const uint64_t* piece_off = nullptr;
+        uint32_t pieces = 1;
         // pool bytes of a part: part_bytes, or kernels::fp8_gather_bytes(1, fp8_elems)
         uint64_t pool_part_bytes() const;
         // bytes of a part in the caller's tensors: part_bytes, or 2 * fp8_elems (bf16)
@@ -227,6 +233,8 @@ class Connection {
         std::vector<RemoteBlock> blocks;  // blocks to write (the "already exists" ones dropped)
         std::vector<uint64_t> offsets;    // their local offsets (elements until the first call)
         std::vector<KeyHash> hashes;      // their key fingerprints from allocate
+        uint32_t pieces = 1;              // GatherSpec::pieces of every call
+        std::vector<uint64_t> piece_off;  // their piece tables, scaled as offsets
         bool indexed = true;              // every block has a fingerprint: it can be published
         uint32_t nparts = 0;              // S: parts of a block
         std::vector<uint8_t> written;     // per part: stored by an earlier call
@@ -243,9 +251,12 @@ class Connection {
         bool complete() const { return parts_written == nparts; }
         ~GatherWriter();
     };
-    // Takes the blocks' fingerprints out of the allocation record, once.
+    // Takes the blocks' fingerprints out of the allocation record, once.  pieces > 1:
+    // piece_off holds n * pieces piece offsets (GatherSpec::piece_off), used by every call.
     std::shared_ptr<GatherWriter> gather_writer(const RemoteBlock* blocks, const uint64_t* offsets,
-                                                size_t n, uint32_t nparts);
+                                                size_t n, uint32_t nparts,
+                                                const uint64_t* piece_off = nullptr,
+                                                uint32_t pieces = 1);
     // Stores parts g.first_part .. g.first_part + g.nparts - 1 of every block of `w`; offsets
     // are scaled by `scale`.  Refuses part ranges written before, a device, scale, fp8_elems
     // or part size other than the first call's, a complete or failed writer, and a writer made

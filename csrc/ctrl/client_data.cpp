@@ -296,6 +296,7 @@ kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n,
     G.dst_pitch = g.dst_pitch;
     G.slices = g.slices;
     G.dst_slice_pitch = g.dst_slice_pitch;
+    G.pieces = g.pieces;  // the caller stages the piece table beside the descriptors
     return G;
 }
 
@@ -346,8 +347,11 @@ static cudaError_t writer_state_alloc(void** p, size_t bytes, int device, cudaSt
 // Blocks per launch of a gathered call (staging.h: gather_max_blocks).  fp8 parts are counted
 // in bf16 bytes: the fp8 kernels cut a part into chunks of at least kFp8Chunk elements (16 KB
 // of bf16), or take it whole.
+// A piece table (GatherSpec::pieces) bounds it to the blocks whose tables fit kPieceRingBytes.
 static size_t gather_batch_cap(const Connection::GatherSpec& g) {
-    return gather_max_blocks(kMaxBatch, g.nparts, g.fp8_elems ? 2 * g.fp8_elems : g.part_bytes);
+    const size_t cap =
+        gather_max_blocks(kMaxBatch, g.nparts, g.fp8_elems ? 2 * g.fp8_elems : g.part_bytes);
+    return g.pieces > 1 ? std::min(cap, kPieceRingBytes / (sizeof(uint64_t) * g.pieces)) : cap;
 }
 
 // The blocks of blocks[base, ...) that the next launch stages (staging.h: key_batch) within
@@ -430,11 +434,15 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
                     for (uint32_t s = 0; s < gather->nparts; ++s) {
                         uint8_t* local =
                             reinterpret_cast<uint8_t*>(gather->part_base[s] + local_off[i] * scale);
-                        if (g.rows) {
+                        if (g.rows) {  // pieces: row r in piece r / piece_rows
                             uint8_t* stored = pool + (g.first_part + s) * pb + g.src_col;
+                            const uint32_t pr = g.rows / g.pieces;
                             for (uint32_t r = 0; r < g.rows; ++r)
                                 for (uint32_t j = 0; j < g.slices; ++j) {
-                                    uint8_t* l = local + size_t(r) * g.dst_pitch +
+                                    const uint64_t piece =
+                                        g.pieces > 1 ? g.piece_off[i * g.pieces + r / pr] * scale
+                                                     : 0;
+                                    uint8_t* l = local + piece + size_t(r % pr) * g.dst_pitch +
                                                  size_t(j) * g.dst_slice_pitch;
                                     uint8_t* p = stored + size_t(r) * g.src_pitch +
                                                  size_t(j) * g.row_bytes;
@@ -536,6 +544,13 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
             at_rec = ctx->ring_alloc(batch_cap * sizeof(kernels::IndexEntry));
             recs = reinterpret_cast<kernels::IndexEntry*>(ctx->ring_h + at_rec);
         }
+        const uint32_t k = gather ? gather->pieces : 1;  // piece table: one row per descriptor
+        size_t at_piece = 0;
+        uint64_t* pieces = nullptr;
+        if (k > 1) {
+            at_piece = ctx->ring_alloc(batch_cap * k * sizeof(uint64_t));
+            pieces = reinterpret_cast<uint64_t*>(ctx->ring_h + at_piece);
+        }
         uint32_t m = 0;
         const size_t batch0 = i;  // a layered writer's blocks: its state index of descs[0]
         batch_commits.clear();
@@ -574,6 +589,10 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
             align_or |= local;
             descs[m].src = write ? local : pool;
             descs[m].dst = write ? pool : local;
+            for (uint32_t t = 0; t < k && pieces; ++t) {
+                pieces[size_t(m) * k + t] = gather->piece_off[i * k + t] * scale;
+                align_or |= pieces[size_t(m) * k + t];
+            }
             if (write) {
                 if (recs) {
                     KeyHash kh;
@@ -626,6 +645,7 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
         if (gather) {
             kernels::GatherLaunch G = gather_launch(*gather, m, align_or, L.status, L.max_ctas);
             G.descs = L.descs;
+            if (pieces) G.piece_off = reinterpret_cast<const uint64_t*>(ctx->ring_d + at_piece);
             G.write = write;
             G.recs = L.recs;
             G.table = L.table;
@@ -881,12 +901,18 @@ const char* Connection::gather_refusal(const GatherSpec& g, const uint64_t* offs
     if (end > block_parts) return "the part range runs past the block";
     if (block_parts > uint64_t(INT32_MAX) / g.pool_part_bytes())
         return "bad parts list: a block holds at most 2^31 - 1 bytes";
+    if (g.pieces == 0 || (g.pieces > 1 && (!g.rows || !g.piece_off)))
+        return "bad pieces: pieces >= 1, and pieces > 1 need row geometry and a piece table";
+    if (g.pieces > 1 && g.rows % g.pieces)
+        return "bad pieces: the piece count must divide the rows";
+    if (uint64_t(g.pieces) * sizeof(uint64_t) > kPieceRingBytes)
+        return "bad pieces: one block's piece table does not fit the staging ring";
     if (g.rows && !kernels::row_geometry_ok(g.rows, g.row_bytes, g.src_pitch, g.src_col,
                                             g.dst_pitch, g.slices, g.dst_slice_pitch,
-                                            g.view_part_bytes()))
+                                            g.view_part_bytes(), g.pieces))
         return "bad row geometry (rows >= 1, slices >= 1, src_col + slices * row_bytes <= "
                "src_pitch, part_bytes == rows * src_pitch; with slices > 1, disjoint local "
-               "slices within 2^32 bytes)";
+               "slices within 2^32 bytes; with pieces, per piece)";
     // the in-band commit publishes whole blocks: a write fills every byte of a stored part
     if (g.rows && write &&
         !kernels::row_write_covers(g.row_bytes, g.src_pitch, g.src_col, g.slices))
@@ -909,7 +935,10 @@ const char* Connection::gather_refusal(const GatherSpec& g, const uint64_t* offs
         uint64_t align_or = 0;
         for (uint32_t s = 0; s < g.nparts; ++s) align_or |= g.part_base[s];
         for (size_t i = 0; i < n; ++i) align_or |= offs[i];
-        if (align_or & 15) return "fp8 parts need 16-byte aligned part bases and offsets";
+        if (g.pieces > 1)
+            for (size_t i = 0; i < n * g.pieces; ++i) align_or |= g.piece_off[i];
+        if (align_or & 15)
+            return "fp8 parts need 16-byte aligned part bases, offsets and piece offsets";
     }
     return nullptr;
 }
@@ -971,9 +1000,12 @@ Connection::GatherWriter::~GatherWriter() {
 
 std::shared_ptr<Connection::GatherWriter> Connection::gather_writer(const RemoteBlock* blocks,
                                                                     const uint64_t* offsets,
-                                                                    size_t n, uint32_t nparts) {
+                                                                    size_t n, uint32_t nparts,
+                                                                    const uint64_t* piece_off,
+                                                                    uint32_t pieces) {
     auto w = std::make_shared<GatherWriter>();
     w->nparts = nparts;
+    w->pieces = piece_off ? pieces : 1;
     w->written.assign(nparts, 0);
     std::lock_guard<std::mutex> lk(mu_);
     w->session = session_;
@@ -984,6 +1016,9 @@ std::shared_ptr<Connection::GatherWriter> Connection::gather_writer(const Remote
         w->blocks.push_back(blocks[i]);
         w->offsets.push_back(offsets[i]);
         w->hashes.push_back(kh);
+        if (w->pieces > 1)
+            w->piece_off.insert(w->piece_off.end(), piece_off + i * pieces,
+                                piece_off + (i + 1) * pieces);
     }
     return w;
 }
@@ -1006,13 +1041,20 @@ int Connection::write_layered(GatherWriter& w, const GatherSpec& g, uint64_t sca
                         g.pool_part_bytes() != w.part_bytes))
         bad = "device, element size or part size differ from the writer's first call";
     // every check before the writer changes: the first call's offsets are still in elements
-    std::vector<uint64_t> scaled;
+    std::vector<uint64_t> scaled, scaled_pieces;
     if (!bad && first) {
         scaled = w.offsets;
         for (uint64_t& o : scaled) o *= scale;
+        scaled_pieces = w.piece_off;
+        for (uint64_t& o : scaled_pieces) o *= scale;
     }
     const std::vector<uint64_t>& offs = first ? scaled : w.offsets;
-    if (!bad) bad = gather_refusal(g, offs.data(), offs.size(), device, true, &w);
+    GatherSpec gp = g;  // the writer's piece table goes with every call
+    if (!bad && (g.pieces != 1 || g.piece_off))
+        bad = "a layered writer takes its pieces when it is made";
+    gp.pieces = w.pieces;
+    gp.piece_off = w.pieces > 1 ? (first ? scaled_pieces : w.piece_off).data() : nullptr;
+    if (!bad) bad = gather_refusal(gp, offs.data(), offs.size(), device, true, &w);
     for (uint64_t s = g.first_part; !bad && s < end; ++s)
         if (w.written[s]) bad = "the part range overlaps parts written before";
     if (bad) {
@@ -1025,10 +1067,12 @@ int Connection::write_layered(GatherWriter& w, const GatherSpec& g, uint64_t sca
         w.fp8_elems = g.fp8_elems;
         w.part_bytes = uint32_t(g.pool_part_bytes());
         w.offsets.swap(scaled);
+        w.piece_off.swap(scaled_pieces);
+        if (w.pieces > 1) gp.piece_off = w.piece_off.data();
     }
     const int r = move_blocks(true, w.offsets.data(), 1, w.blocks.data(), w.blocks.size(),
                               int(w.nparts * w.part_bytes), 0, device, stream, int(g.fp8_elems),
-                              nullptr, &g, &w);
+                              nullptr, &gp, &w);
     if (r != 0) {
         w.failed = true;
         return r;
@@ -1115,12 +1159,24 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
         }
         uint64_t align_or = base_ptr;
         for (size_t i = 0; i < n; ++i) align_or |= blocks[base + i].offset;
+        const uint32_t k = gather ? gather->pieces : 1;  // piece table, beside the keys
+        const uint64_t* pieces_d = nullptr;
+        if (k > 1) {
+            const size_t at = ctx->ring_alloc(n * k * sizeof(uint64_t));
+            auto* pieces = reinterpret_cast<uint64_t*>(ctx->ring_h + at);
+            for (size_t t = 0; t < n * k; ++t) {
+                pieces[t] = gather->piece_off[base * k + t];
+                align_or |= pieces[t];
+            }
+            pieces_d = reinterpret_cast<const uint64_t*>(ctx->ring_d + at);
+        }
         // the fused kernels' support checks see the batch as it would be launched
         R.n = uint32_t(n);
         R.align_or = align_or;
         R.max_ctas = device_read_grid_cap(max_ctas_, in.all_remote, fp8_elems != 0, in.sm_count);
         kernels::GatherLaunch G;
         if (gather) G = gather_launch(*gather, uint32_t(n), align_or, ctx->status_d, R.max_ctas);
+        G.piece_off = pieces_d;
         in.fp8_fused_ok = fp8_elems && kernels::fp8_read_fused_supported(R, uint32_t(fp8_elems));
         in.scatter_fused_ok = gather && kernels::scatter_read_fused_supported(R, G);
         const DeviceReadPlan plan = plan_device_read(in);

@@ -202,6 +202,14 @@ struct GatherLaunch {
     // head-major page stored token-major.  Works with recs and a layered writer's layer_state.
     uint32_t slices = 1;
     uint32_t dst_slice_pitch = 0;
+    // Pieces (with rows, reads and writes; pieces == 1: one local offset per block, desc's):
+    // block i's local layout is `pieces` runs of rows / pieces rows, run t at part_base[s] +
+    // the descriptor's local offset + piece_off[i * pieces + t] (device-addressable byte
+    // offsets, one table row per descriptor) - e.g. a chunk of k engine pages stored under one
+    // key, each page where the caller's block table puts it (launch_plan.h: piece_pair,
+    // piece_write_offset).  align_or covers every piece offset.
+    const uint64_t* piece_off = nullptr;
+    uint32_t pieces = 1;
 };
 // The TMA pipeline for 16-byte aligned parts of at least kPipeMinBytes, the ld/st kernel
 // (kv_copy.cu) otherwise: the same rule launch_kv_copy applies to whole blocks.  A row-sliced

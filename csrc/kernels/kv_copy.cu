@@ -199,13 +199,19 @@ struct RowGeometry {
 // still count as arrivals.  No control warp: reads publish nothing.
 // SLICED (kv_scatter_slices_kernel, GatherLaunch::slices > 1): a run is `run` (slice, row)
 // pairs of the part, numbered slice-major, each placed by slice_pair (launch_plan.h).
-template <int VEC, bool LAYERED, bool SLICED>
+// PIECES (kv_scatter_pieces_kernel, GatherLaunch::pieces > 1, any slices): the same items; the
+// run's pairs are cut where q / piece_rows changes, and each cut, one slice's rows inside one
+// piece, is copied as plain rows to desc.dst + piece_off[block * pieces + t] + the place
+// piece_pair gives its first pair - one piece-offset load per cut.
+template <int VEC, bool LAYERED, bool SLICED, bool PIECES = false>
 __device__ __forceinline__ void scatter_rows(const CopyDesc* __restrict__ descs,
                                              const GatherParts& parts, uint32_t n,
                                              uint32_t nparts, uint32_t first_part,
                                              const RowGeometry& geo, uint32_t slices,
                                              uint32_t slice_pitch, uint32_t run, uint32_t cpp,
-                                             uint32_t* status, const GroupRelease& rel) {
+                                             uint32_t* status, const GroupRelease& rel,
+                                             const uint64_t* piece_off = nullptr,
+                                             uint32_t pieces = 1) {
     const uint32_t gp = LAYERED ? rel.gp : nparts;
     const uint32_t group_items = n * gp * cpp;
     const uint32_t total = n * nparts * cpp;
@@ -216,7 +222,23 @@ __device__ __forceinline__ void scatter_rows(const CopyDesc* __restrict__ descs,
         const LayeredItem it = layered_item(item, n, gp, cpp);
         const uint32_t nxt = item + gridDim.x;
         if (nxt < total) next = descs[layered_item(nxt, n, gp, cpp).block];
-        if (d.src != 0 && SLICED) {
+        if (d.src != 0 && PIECES) {
+            const uint32_t piece_rows = geo.rows / pieces;
+            const uint32_t q0 = it.chunk * run, q1 = min(q0 + run, geo.rows * slices);
+            const uint8_t* src = reinterpret_cast<const uint8_t*>(
+                d.src + uint64_t(first_part + it.part) * geo.part_bytes);
+            const uint64_t* off = piece_off + uint64_t(it.block) * pieces;
+            for (uint32_t q = q0; q < q1;) {
+                const uint32_t e = min(q1, (q / piece_rows + 1) * piece_rows);
+                const PieceOffsets o = piece_pair(q, geo.rows, geo.row_bytes, geo.src_pitch,
+                                                  geo.src_col, geo.dst_pitch, slice_pitch,
+                                                  piece_rows);
+                copy_rows<VEC>(
+                    reinterpret_cast<uint8_t*>(parts.base[it.part] + d.dst + off[o.piece] + o.dst),
+                    src + o.src, e - q, geo.row_bytes, geo.src_pitch, geo.dst_pitch);
+                q = e;
+            }
+        } else if (d.src != 0 && SLICED) {
             const uint32_t q0 = it.chunk * run;
             const uint8_t* src = reinterpret_cast<const uint8_t*>(
                 d.src + uint64_t(first_part + it.part) * geo.part_bytes);
@@ -268,6 +290,43 @@ __global__ void __launch_bounds__(kLdStThreads, 3)
                                      slice_pitch, run, cpp, status, rel);
 }
 
+// GatherLaunch::pieces > 1, one or more slices: runs cut at piece boundaries (scatter_rows).
+template <int VEC, bool LAYERED>
+__global__ void __launch_bounds__(kLdStThreads, 3)
+    kv_scatter_pieces_kernel(const CopyDesc* __restrict__ descs,
+                             const __grid_constant__ GatherParts parts, uint32_t n,
+                             uint32_t nparts, uint32_t first_part, RowGeometry geo,
+                             uint32_t slices, uint32_t slice_pitch, uint32_t run, uint32_t cpp,
+                             uint32_t* status, GroupRelease rel, const uint64_t* piece_off,
+                             uint32_t pieces) {
+    scatter_rows<VEC, LAYERED, false, true>(descs, parts, n, nparts, first_part, geo, slices,
+                                            slice_pitch, run, cpp, status, rel, piece_off,
+                                            pieces);
+}
+
+cudaError_t launch_kv_scatter_pieces(const GatherLaunch& a, const LaunchPlan& p,
+                                     const GatherParts& parts, const RowGeometry& geo,
+                                     const GroupRelease& rel, cudaStream_t stream) {
+    const bool layered = a.group_flags != nullptr;
+    const auto go = [&](auto* kernel) {
+        kernel<<<p.ctas, kLdStThreads, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.first_part,
+                                                    geo, a.slices, a.dst_slice_pitch, p.chunk,
+                                                    p.cpb, a.status, rel, a.piece_off, a.pieces);
+        return cudaGetLastError();
+    };
+    switch (p.kernel) {
+        case Kernel::kLdSt1:
+            return layered ? go(kv_scatter_pieces_kernel<1, true>)
+                           : go(kv_scatter_pieces_kernel<1, false>);
+        case Kernel::kLdSt32:
+            return layered ? go(kv_scatter_pieces_kernel<32, true>)
+                           : go(kv_scatter_pieces_kernel<32, false>);
+        default:
+            return layered ? go(kv_scatter_pieces_kernel<16, true>)
+                           : go(kv_scatter_pieces_kernel<16, false>);
+    }
+}
+
 cudaError_t launch_kv_scatter_slices(const GatherLaunch& a, const LaunchPlan& p,
                                      const GatherParts& parts, const RowGeometry& geo,
                                      const GroupRelease& rel, cudaStream_t stream) {
@@ -300,10 +359,17 @@ cudaError_t launch_kv_scatter_rows(const GatherLaunch& a, cudaStream_t stream) {
         kv_scatter_slices_kernel<16, false>, kv_scatter_slices_kernel<32, false>, kLdStThreads);
     static const LdStResident res_sliced_layered = ldst_resident(
         kv_scatter_slices_kernel<16, true>, kv_scatter_slices_kernel<32, true>, kLdStThreads);
+    static const LdStResident res_pieces = ldst_resident(
+        kv_scatter_pieces_kernel<16, false>, kv_scatter_pieces_kernel<32, false>, kLdStThreads);
+    static const LdStResident res_pieces_layered = ldst_resident(
+        kv_scatter_pieces_kernel<16, true>, kv_scatter_pieces_kernel<32, true>, kLdStThreads);
     const bool layered = a.group_flags != nullptr;
     const bool sliced = a.slices > 1;
+    const bool pieced = a.pieces > 1;
+    if (pieced && !a.piece_off) return cudaErrorInvalidValue;
     const LaunchPlan p = plan_gather_rows(a, sm_count(),
-                                          sliced ? (layered ? res_sliced_layered : res_sliced)
+                                          pieced   ? (layered ? res_pieces_layered : res_pieces)
+                                          : sliced ? (layered ? res_sliced_layered : res_sliced)
                                           : layered ? res_layered
                                                     : res);
     if (!p.valid) return cudaErrorInvalidValue;  // the caller checks the geometry and splits
@@ -311,6 +377,7 @@ cudaError_t launch_kv_scatter_rows(const GatherLaunch& a, cudaStream_t stream) {
     std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
     const RowGeometry geo{a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.part_bytes};
     const GroupRelease rel{a.group_flags, a.group_counters, a.group_seq, a.group_parts};
+    if (pieced) return launch_kv_scatter_pieces(a, p, parts, geo, rel, stream);
     if (sliced) return launch_kv_scatter_slices(a, p, parts, geo, rel, stream);
     const auto go = [&](auto* kernel) {
         kernel<<<p.ctas, kLdStThreads, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.first_part,
@@ -335,13 +402,19 @@ cudaError_t launch_kv_scatter_rows(const GatherLaunch& a, cudaStream_t stream) {
 // bytes, so the control warp (publish, or a layered writer's LayerCommit) counts arrivals
 // exactly as for kv_gather_ldst.  Only the local load address differs: stored byte o of part
 // s comes from parts.base[s] + desc.src + row_write_offset(o) (copy_span_rows).
-template <int VEC>
-__global__ void __launch_bounds__(kLdStThreads + 32, 3)
-    kv_gather_rows_write_kernel(const CopyDesc* __restrict__ descs,
-                                const __grid_constant__ GatherParts parts, uint32_t n,
-                                uint32_t nparts, uint32_t part_bytes, uint32_t first_part,
-                                uint32_t chunk, uint32_t cpp, RowWrite geo, Publish pub,
-                                LayerCommit lc) {
+// PIECES (kv_gather_pieces_write_kernel, GatherLaunch::pieces > 1): the item's stored bytes are
+// cut at piece boundaries (piece_rows * src_pitch bytes), and each cut is loaded from
+// parts.base[s] + desc.src + piece_off[block * pieces + t] (piece_write_offset's geometry) -
+// one piece-offset load per cut.
+template <int VEC, bool PIECES>
+__device__ __forceinline__ void gather_rows_write(const CopyDesc* __restrict__ descs,
+                                                  const GatherParts& parts, uint32_t n,
+                                                  uint32_t nparts, uint32_t part_bytes,
+                                                  uint32_t first_part, uint32_t chunk, uint32_t cpp,
+                                                  const RowWrite& geo, const Publish& pub,
+                                                  const LayerCommit& lc,
+                                                  const uint64_t* piece_off = nullptr,
+                                                  uint32_t pieces = 1) {
     const uint32_t cpb = nparts * cpp;  // items per block: what the commit counter counts
     const uint32_t total = n * cpb;
     if (threadIdx.x >= kLdStThreads) {
@@ -361,23 +434,75 @@ __global__ void __launch_bounds__(kLdStThreads + 32, 3)
         const uint32_t s = in_block / cpp;
         const uint32_t off = (in_block % cpp) * chunk;
         const uint32_t len = min(chunk, part_bytes - off);
-        const uint8_t* src = reinterpret_cast<const uint8_t*>(parts.base[s] + d.src);
-        uint8_t* dst =
-            reinterpret_cast<uint8_t*>(d.dst + uint64_t(first_part + s) * part_bytes + off);
-        copy_span_rows<VEC>(dst, src, off, len, geo);
+        if constexpr (!PIECES) {
+            const uint8_t* src = reinterpret_cast<const uint8_t*>(parts.base[s] + d.src);
+            uint8_t* dst =
+                reinterpret_cast<uint8_t*>(d.dst + uint64_t(first_part + s) * part_bytes + off);
+            copy_span_rows<VEC>(dst, src, off, len, geo);
+        } else {
+            uint8_t* dst =
+                reinterpret_cast<uint8_t*>(d.dst + uint64_t(first_part + s) * part_bytes + off);
+            const uint32_t piece_bytes = part_bytes / pieces;
+            const uint64_t* poff = piece_off + uint64_t(item / cpb) * pieces;
+            for (uint32_t o = off; o < off + len;) {
+                const uint32_t t = o / piece_bytes;
+                const uint32_t e = min(off + len, (t + 1) * piece_bytes);
+                copy_span_rows<VEC>(
+                    dst + (o - off), reinterpret_cast<const uint8_t*>(parts.base[s] + d.src + poff[t]),
+                    o - t * piece_bytes, e - o, geo);
+                o = e;
+            }
+        }
     }
     if (pub.recs) ctrl_barrier_arrive(kLdStThreads + 32);
+}
+
+template <int VEC>
+__global__ void __launch_bounds__(kLdStThreads + 32, 3)
+    kv_gather_rows_write_kernel(const CopyDesc* __restrict__ descs,
+                                const __grid_constant__ GatherParts parts, uint32_t n,
+                                uint32_t nparts, uint32_t part_bytes, uint32_t first_part,
+                                uint32_t chunk, uint32_t cpp, RowWrite geo, Publish pub,
+                                LayerCommit lc) {
+    gather_rows_write<VEC, false>(descs, parts, n, nparts, part_bytes, first_part, chunk, cpp,
+                                  geo, pub, lc);
+}
+
+template <int VEC>
+__global__ void __launch_bounds__(kLdStThreads + 32, 3)
+    kv_gather_pieces_write_kernel(const CopyDesc* __restrict__ descs,
+                                  const __grid_constant__ GatherParts parts, uint32_t n,
+                                  uint32_t nparts, uint32_t part_bytes, uint32_t first_part,
+                                  uint32_t chunk, uint32_t cpp, RowWrite geo, Publish pub,
+                                  LayerCommit lc, const uint64_t* piece_off, uint32_t pieces) {
+    gather_rows_write<VEC, true>(descs, parts, n, nparts, part_bytes, first_part, chunk, cpp, geo,
+                                 pub, lc, piece_off, pieces);
 }
 
 cudaError_t launch_kv_gather_rows_write(const GatherLaunch& a, cudaStream_t stream) {
     constexpr int T = kLdStThreads + 32;
     static const LdStResident res =
         ldst_resident(kv_gather_rows_write_kernel<16>, kv_gather_rows_write_kernel<32>, T);
-    const LaunchPlan p = plan_gather_rows_write(a, sm_count(), res);
+    static const LdStResident res_pieces =
+        ldst_resident(kv_gather_pieces_write_kernel<16>, kv_gather_pieces_write_kernel<32>, T);
+    const bool pieced = a.pieces > 1;
+    if (pieced && !a.piece_off) return cudaErrorInvalidValue;
+    const LaunchPlan p = plan_gather_rows_write(a, sm_count(), pieced ? res_pieces : res);
     if (!p.valid) return cudaErrorInvalidValue;  // the caller checks the geometry and splits
     GatherParts parts;
     std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
     const RowWrite geo{a.row_bytes, a.src_pitch, a.dst_pitch, a.dst_slice_pitch};
+    if (pieced) {
+        const auto go = [&](auto* kernel) {
+            kernel<<<p.ctas, T, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.part_bytes,
+                                             a.first_part, p.chunk, p.cpb, geo, publish_of(a, true),
+                                             layer_of(a), a.piece_off, a.pieces);
+            return cudaGetLastError();
+        };
+        return p.kernel == Kernel::kLdSt1    ? go(kv_gather_pieces_write_kernel<1>)
+               : p.kernel == Kernel::kLdSt32 ? go(kv_gather_pieces_write_kernel<32>)
+                                             : go(kv_gather_pieces_write_kernel<16>);
+    }
     const auto go = [&](auto* kernel) {
         kernel<<<p.ctas, T, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.part_bytes, a.first_part,
                                          p.chunk, p.cpb, geo, publish_of(a, true), layer_of(a));
@@ -462,6 +587,7 @@ cudaError_t launch_kv_gather(const GatherLaunch& a, cudaStream_t stream) {
     if (layered && !a.group_counters) return cudaErrorInvalidValue;
     if (a.rows)
         return a.write ? launch_kv_gather_rows_write(a, stream) : launch_kv_scatter_rows(a, stream);
+    if (a.pieces != 1) return cudaErrorInvalidValue;  // pieces split rows
     constexpr int T = kLdStThreads + 32;
     static const LdStResident res =
         ldst_resident(kv_gather_ldst_kernel<16>, kv_gather_ldst_kernel<32>, T);

@@ -13,6 +13,8 @@
 //                  (GatherLaunch::rows): a read dequantises rows (and slices) of each stored
 //                  page, a write quantises a stored page whose rows are loaded from a strided
 //                  local layout (e.g. a head-major page).
+//   kv_read_fp8_pieces, kv_write_fp8_pieces : the same with GatherLaunch::pieces > 1, each
+//                  block's rows in runs at the offsets of its row of the piece table.
 // The reference moves raw bytes only (dtype-agnostic, infinistore/lib.py:377-379); this is
 // the "write fused with fp8 cast / read fused with gather" item of the north star.
 //
@@ -73,16 +75,40 @@ __device__ __forceinline__ uint4 ld_u4(const void* p) {
 //   SlicedRows a row-sliced write (GatherLaunch::rows): row_write_offset (launch_plan.h) of the
 //              vector's byte in the part's bf16 view; the geometry is in multiples of 16 bytes,
 //              so the 8 elements never straddle two slices.
+//   PiecedRows a row-sliced write with pieces (GatherLaunch::pieces > 1): piece_write_offset,
+//              plus the piece's offset from block b's row of the piece table (block(b)).
+//              Pieces split at row boundaries, rows are multiples of 8 elements, so a vector
+//              never straddles two pieces; a 128-element scale group may, and each of its
+//              vectors is placed on its own.
+// block(b) is the policy for the items of block b.
 struct DenseRows {
     __device__ __forceinline__ size_t operator()(uint32_t row, uint32_t hl) const {
         return (size_t(row) * kRow + hl * 8) * 2;
     }
+    __device__ __forceinline__ DenseRows block(uint32_t) const { return *this; }
 };
 struct SlicedRows {
     uint32_t row_bytes, src_pitch, dst_pitch, slice_pitch;
     __device__ __forceinline__ size_t operator()(uint32_t row, uint32_t hl) const {
         return row_write_offset((row * kRow + hl * 8) * 2, row_bytes, src_pitch, dst_pitch,
                                 slice_pitch);
+    }
+    __device__ __forceinline__ SlicedRows block(uint32_t) const { return *this; }
+};
+struct PiecedRows {
+    SlicedRows geo;
+    uint32_t piece_rows, pieces;
+    const uint64_t* off;  // block b's row of the piece table once bound by block(b)
+    __device__ __forceinline__ size_t operator()(uint32_t row, uint32_t hl) const {
+        const PieceOffset p = piece_write_offset((row * kRow + hl * 8) * 2, geo.row_bytes,
+                                                 geo.src_pitch, geo.dst_pitch, geo.slice_pitch,
+                                                 piece_rows);
+        return off[p.piece] + p.off;
+    }
+    __device__ __forceinline__ PiecedRows block(uint32_t b) const {
+        PiecedRows r = *this;
+        r.off += uint64_t(b) * pieces;
+        return r;
     }
 };
 
@@ -107,6 +133,7 @@ __device__ __forceinline__ void write_fp8(const CopyDesc* __restrict__ descs, ui
     constexpr uint32_t kStep = 2 * kRowPairs;  // rows per warp iteration
     for (uint32_t item = blockIdx.x; item < total; item += gridDim.x) {
         const CopyDesc d = pages.at(descs, item / cpp);
+        const LoadAt at = load_at.block(item / cpb);
         const uint32_t e0 = (item % cpp) * chunk;
         const uint32_t rows = min(chunk, elems - e0) / kRow;
         const uint32_t row0 = e0 / kRow;
@@ -118,7 +145,7 @@ __device__ __forceinline__ void write_fp8(const CopyDesc* __restrict__ descs, ui
 #pragma unroll
             for (int u = 0; u < kRowPairs; ++u) {
                 const uint32_t r = r0 + 2 * u + half;
-                if (r < rows) v[u] = ld_u4(src + load_at(row0 + r, hl));
+                if (r < rows) v[u] = ld_u4(src + at(row0 + r, hl));
             }
 #pragma unroll
             for (int u = 0; u < kRowPairs; ++u) {
@@ -215,6 +242,17 @@ __global__ void __launch_bounds__(kThreads + 32)
                              uint32_t nparts, uint32_t elems, uint32_t chunk, uint32_t cpp,
                              uint32_t first_part, uint64_t stride, SlicedRows geo, Publish pub,
                              LayerCommit lc) {
+    write_fp8(descs, n, elems, chunk, cpp, pub,
+              BlockParts<true>{&parts, nparts, first_part, stride, lc}, geo);
+}
+
+// GatherLaunch::pieces > 1: kv_write_fp8_rows_kernel with each vector loaded from its piece.
+__global__ void __launch_bounds__(kThreads + 32)
+    kv_write_fp8_pieces_kernel(const CopyDesc* __restrict__ descs,
+                               const __grid_constant__ GatherParts parts, uint32_t n,
+                               uint32_t nparts, uint32_t elems, uint32_t chunk, uint32_t cpp,
+                               uint32_t first_part, uint64_t stride, PiecedRows geo, Publish pub,
+                               LayerCommit lc) {
     write_fp8(descs, n, elems, chunk, cpp, pub,
               BlockParts<true>{&parts, nparts, first_part, stride, lc}, geo);
 }
@@ -403,15 +441,21 @@ __device__ __forceinline__ void read_fp8_rows(uint8_t* dst, const uint8_t* q, co
 // (kv_copy.cu).  Stored part first_part + s starts at desc.src + (first_part + s) * stride.
 // A missing block counts once, on its first item, and its parts are left untouched; its items
 // still count as arrivals.  SLICED (kv_read_fp8_slices_kernel, GatherLaunch::slices > 1): a
-// run is `run` (slice, row) pairs of the part, numbered slice-major.
-template <bool LAYERED, bool SLICED>
+// run is `run` (slice, row) pairs of the part, numbered slice-major.  PIECES
+// (kv_read_fp8_pieces_kernel, GatherLaunch::pieces > 1, any slices): the run is cut where
+// q / piece_rows changes, as in kv_scatter_pieces_kernel (kv_copy.cu), and each cut is read as
+// plain rows to desc.dst + piece_off[block * pieces + t] + the place piece_pair gives its first
+// pair - one piece-offset load per cut.
+template <bool LAYERED, bool SLICED, bool PIECES = false>
 __device__ __forceinline__ void read_fp8_row_items(const CopyDesc* __restrict__ descs,
                                                    const GatherParts& parts, uint32_t n,
                                                    uint32_t nparts, uint32_t first_part,
                                                    const Fp8Rows& geo, uint32_t slices,
                                                    uint32_t slice_pitch, uint32_t run,
                                                    uint32_t cpp, uint64_t stride,
-                                                   uint32_t* status, const GroupRelease& rel) {
+                                                   uint32_t* status, const GroupRelease& rel,
+                                                   const uint64_t* piece_off = nullptr,
+                                                   uint32_t pieces = 1) {
     const uint32_t gp = LAYERED ? rel.gp : nparts;
     const uint32_t group_items = n * gp * cpp;
     const uint32_t total = n * nparts * cpp;
@@ -422,7 +466,23 @@ __device__ __forceinline__ void read_fp8_row_items(const CopyDesc* __restrict__ 
         const LayeredItem it = layered_item(item, n, gp, cpp);
         const uint32_t nxt = item + gridDim.x;
         if (nxt < total) next = descs[layered_item(nxt, n, gp, cpp).block];
-        if (d.src != 0 && SLICED) {
+        if (d.src != 0 && PIECES) {
+            const uint32_t piece_rows = geo.rows / pieces;
+            const uint32_t q0 = it.chunk * run, q1 = min(q0 + run, geo.rows * slices);
+            const uint8_t* q =
+                reinterpret_cast<const uint8_t*>(d.src + uint64_t(first_part + it.part) * stride);
+            const uint64_t* off = piece_off + uint64_t(it.block) * pieces;
+            for (uint32_t p = q0; p < q1;) {
+                const uint32_t e = min(q1, (p / piece_rows + 1) * piece_rows);
+                const PieceOffsets o = piece_pair(p, geo.rows, 8 * geo.vpr, geo.src_pitch,
+                                                  geo.src_col, geo.dst_pitch, slice_pitch,
+                                                  piece_rows);
+                read_fp8_rows(
+                    reinterpret_cast<uint8_t*>(parts.base[it.part] + d.dst + off[o.piece] + o.dst),
+                    q, reinterpret_cast<const float*>(q + geo.elems), o.src, e - p, geo);
+                p = e;
+            }
+        } else if (d.src != 0 && SLICED) {
             const uint32_t q0 = it.chunk * run;
             const uint8_t* q =
                 reinterpret_cast<const uint8_t*>(d.src + uint64_t(first_part + it.part) * stride);
@@ -472,6 +532,21 @@ __global__ void __launch_bounds__(kThreads)
                                       slice_pitch, run, cpp, stride, status, rel);
 }
 
+// GatherLaunch::pieces > 1, one or more slices: runs cut at piece boundaries
+// (read_fp8_row_items above).
+template <bool LAYERED>
+__global__ void __launch_bounds__(kThreads)
+    kv_read_fp8_pieces_kernel(const CopyDesc* __restrict__ descs,
+                              const __grid_constant__ GatherParts parts, uint32_t n,
+                              uint32_t nparts, uint32_t first_part, Fp8Rows geo, uint32_t slices,
+                              uint32_t slice_pitch, uint32_t run, uint32_t cpp, uint64_t stride,
+                              uint32_t* status, GroupRelease rel, const uint64_t* piece_off,
+                              uint32_t pieces) {
+    read_fp8_row_items<LAYERED, false, true>(descs, parts, n, nparts, first_part, geo, slices,
+                                             slice_pitch, run, cpp, stride, status, rel,
+                                             piece_off, pieces);
+}
+
 int fp8_rows_resident(const void* kernel) {
     int r = 1;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&r, kernel, kThreads, 0);
@@ -488,9 +563,16 @@ cudaError_t launch_kv_read_fp8_rows(const GatherLaunch& a, uint32_t elems, cudaS
         fp8_rows_resident(reinterpret_cast<const void*>(kv_read_fp8_slices_kernel<false>));
     static const int res_sliced_layered =
         fp8_rows_resident(reinterpret_cast<const void*>(kv_read_fp8_slices_kernel<true>));
+    static const int res_pieces =
+        fp8_rows_resident(reinterpret_cast<const void*>(kv_read_fp8_pieces_kernel<false>));
+    static const int res_pieces_layered =
+        fp8_rows_resident(reinterpret_cast<const void*>(kv_read_fp8_pieces_kernel<true>));
     const bool sliced = a.slices > 1;
-    const int r = sliced ? (layered ? res_sliced_layered : res_sliced)
-                         : (layered ? res_layered : res);
+    const bool pieced = a.pieces > 1;
+    if (pieced && !a.piece_off) return cudaErrorInvalidValue;
+    const int r = pieced   ? (layered ? res_pieces_layered : res_pieces)
+                  : sliced ? (layered ? res_sliced_layered : res_sliced)
+                           : (layered ? res_layered : res);
     const LaunchPlan p = plan_gather_fp8_rows(a, elems, sm_count(), {r, r});
     if (!p.valid) return cudaErrorInvalidValue;  // the caller checks the geometry and splits
     GatherParts parts;
@@ -498,6 +580,16 @@ cudaError_t launch_kv_read_fp8_rows(const GatherLaunch& a, uint32_t elems, cudaS
     const Fp8Rows geo{a.rows, a.row_bytes / 16, a.src_pitch / 2, a.src_col / 2, a.dst_pitch, elems};
     const uint64_t stride = fp8_gather_bytes(1, elems);
     const GroupRelease rel{a.group_flags, a.group_counters, a.group_seq, a.group_parts};
+    if (pieced) {
+        const auto go = [&](auto* kernel) {
+            kernel<<<p.ctas, kThreads, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.first_part,
+                                                    geo, a.slices, a.dst_slice_pitch, p.chunk,
+                                                    p.cpb, stride, a.status, rel, a.piece_off,
+                                                    a.pieces);
+            return cudaGetLastError();
+        };
+        return layered ? go(kv_read_fp8_pieces_kernel<true>) : go(kv_read_fp8_pieces_kernel<false>);
+    }
     if (sliced) {
         const auto go = [&](auto* kernel) {
             kernel<<<p.ctas, kThreads, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.first_part,
@@ -521,11 +613,27 @@ cudaError_t launch_kv_write_fp8_rows(const GatherLaunch& a, uint32_t elems, cuda
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&r, kv_write_fp8_rows_kernel, kThreads + 32, 0);
         return r > 0 ? r : 1;
     }();
-    const LaunchPlan p = plan_gather_fp8_rows_write(a, elems, sm_count(), {res, res});
+    static const int res_pieces = [] {
+        int r = 1;
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&r, kv_write_fp8_pieces_kernel,
+                                                      kThreads + 32, 0);
+        return r > 0 ? r : 1;
+    }();
+    const bool pieced = a.pieces > 1;
+    if (pieced && !a.piece_off) return cudaErrorInvalidValue;
+    const int r = pieced ? res_pieces : res;
+    const LaunchPlan p = plan_gather_fp8_rows_write(a, elems, sm_count(), {r, r});
     if (!p.valid) return cudaErrorInvalidValue;  // the caller checks the geometry and splits
     GatherParts parts;
     std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
     const SlicedRows geo{a.row_bytes, a.src_pitch, a.dst_pitch, a.dst_slice_pitch};
+    if (pieced) {
+        kv_write_fp8_pieces_kernel<<<p.ctas, kThreads + 32, 0, stream>>>(
+            a.descs, parts, a.n, a.nparts, elems, p.chunk, p.cpb, a.first_part,
+            fp8_gather_bytes(1, elems), PiecedRows{geo, a.rows / a.pieces, a.pieces, a.piece_off},
+            publish_of(a, true), layer_of(a));
+        return cudaGetLastError();
+    }
     kv_write_fp8_rows_kernel<<<p.ctas, kThreads + 32, 0, stream>>>(
         a.descs, parts, a.n, a.nparts, elems, p.chunk, p.cpb, a.first_part,
         fp8_gather_bytes(1, elems), geo, publish_of(a, true), layer_of(a));
@@ -563,6 +671,7 @@ cudaError_t launch_kv_gather_fp8(const GatherLaunch& a, uint32_t elems, int vari
     if (a.rows)
         return a.write ? launch_kv_write_fp8_rows(a, elems, stream)
                        : launch_kv_read_fp8_rows(a, elems, stream);
+    if (a.pieces != 1) return cudaErrorInvalidValue;  // pieces split rows
     // a layered read takes the ld/st kernel whatever the variant (no layered pipeline)
     const bool layered = a.group_flags != nullptr;
     if (layered && (a.write || !a.group_counters || !a.group_parts || a.nparts % a.group_parts))

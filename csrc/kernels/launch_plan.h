@@ -261,15 +261,18 @@ inline LaunchPlan plan_gather_layered(const GatherLaunch& a, int sms, LdStReside
 // head-major (a slice's rows inside dst_slice_pitch) or token-major (a row's slices inside
 // dst_pitch) - and the destination extent, (rows - 1) * dst_pitch + (slices - 1) *
 // dst_slice_pitch + row_bytes, fits 32 bits.  slices == 1 checks what it always did.
+// pieces > 1 (GatherLaunch::pieces): the rows land in `pieces` runs of rows / pieces rows, each
+// at its own local offset, so the nesting and the 32-bit extent hold per run (piece_rows rows)
+// rather than over all rows, and pieces must divide rows.
 inline bool row_geometry_ok(uint32_t rows, uint32_t row_bytes, uint32_t src_pitch,
                             uint32_t src_col, uint32_t dst_pitch, uint32_t slices,
-                            uint32_t dst_slice_pitch, uint64_t part_bytes) {
-    if (rows == 0 || row_bytes == 0 || slices == 0 ||
+                            uint32_t dst_slice_pitch, uint64_t part_bytes, uint32_t pieces = 1) {
+    if (rows == 0 || row_bytes == 0 || slices == 0 || pieces == 0 || rows % pieces != 0 ||
         uint64_t(src_col) + uint64_t(slices) * row_bytes > src_pitch ||
         uint64_t(rows) * src_pitch != part_bytes)
         return false;
-    if (slices == 1) return true;
-    const uint64_t rb = row_bytes, r1 = rows - 1, s1 = slices - 1;
+    const uint64_t rb = row_bytes, r1 = rows / pieces - 1, s1 = slices - 1;
+    if (slices == 1) return pieces == 1 || r1 * dst_pitch + rb <= 0xffffffffull;
     const bool head_major = dst_pitch >= rb && dst_slice_pitch >= r1 * dst_pitch + rb;
     const bool token_major = dst_slice_pitch >= rb && dst_pitch >= s1 * dst_slice_pitch + rb;
     return (head_major || token_major) &&
@@ -294,6 +297,29 @@ ISTORE_KHD inline PairOffsets slice_pair(uint32_t q, uint32_t rows, uint32_t row
     return PairOffsets{r * src_pitch + src_col + j * row, r * dst_pitch + j * dst_slice_pitch};
 }
 
+// ---------------------------------------------------------------- pieces
+// A block whose destination is `pieces` local offsets off[0..pieces-1] (GatherLaunch::pieces,
+// piece_off) instead of one: each part's rows split into pieces runs of piece_rows = rows /
+// pieces rows, and run t lands at off[t] - e.g. a chunk of k engine pages stored under one key,
+// page t of it at the offset the caller's block table names.  Slice j of stored row r goes to
+// off[r / piece_rows] + (r % piece_rows) * dst_pitch + j * dst_slice_pitch.  piece_pair is
+// slice_pair with the destination inside its piece; piece_rows == rows is slice_pair with
+// piece 0.  Pairs q with the same q / piece_rows share their slice and their piece (rows is a
+// multiple of piece_rows), so the kernels copy each such run as plain rows from the place
+// piece_pair gives its first pair, loading its piece offset once.  The kernels (kv_copy.cu:
+// scatter_rows, kv_fp8.cu: read_fp8_row_items) and the CPU tests (_infinistore.testing.piece_pair)
+// share this function.
+struct PieceOffsets {
+    uint32_t src, dst, piece;
+};
+ISTORE_KHD inline PieceOffsets piece_pair(uint32_t q, uint32_t rows, uint32_t row,
+                                          uint32_t src_pitch, uint32_t src_col, uint32_t dst_pitch,
+                                          uint32_t dst_slice_pitch, uint32_t piece_rows) {
+    const uint32_t j = q / rows, r = q - j * rows, t = r / piece_rows;
+    return PieceOffsets{r * src_pitch + src_col + j * row,
+                        (r - t * piece_rows) * dst_pitch + j * dst_slice_pitch, t};
+}
+
 // ---------------------------------------------------------------- row-sliced reads
 // kv_scatter_rows (GatherLaunch::rows != 0), plain or layered: always the ld/st kernels (the
 // TMA pipelines have no row form).  The vector width is the one the OR of row_bytes, both
@@ -305,7 +331,7 @@ ISTORE_KHD inline PairOffsets slice_pair(uint32_t q, uint32_t rows, uint32_t row
 inline LaunchPlan plan_gather_rows(const GatherLaunch& a, int sms, LdStResident res) {
     if (a.write || a.nparts == 0 || a.nparts > kGatherMaxParts ||
         !row_geometry_ok(a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.slices,
-                         a.dst_slice_pitch, a.part_bytes) ||
+                         a.dst_slice_pitch, a.part_bytes, a.pieces) ||
         (a.group_flags && (a.group_parts == 0 || a.nparts % a.group_parts != 0)))
         return invalid_plan();
     const uint64_t geo_or = a.align_or | a.src_pitch | a.src_col | a.dst_pitch |
@@ -346,6 +372,23 @@ ISTORE_KHD inline uint32_t row_write_offset(uint32_t o, uint32_t row_bytes, uint
     return r * dst_pitch + j * dst_slice_pitch + (c - j * row_bytes);
 }
 
+// The pieced form (GatherLaunch::pieces): byte o of a covered stored part comes from piece
+// o / (piece_rows * src_pitch), at row_write_offset of o within that piece's rows.  Over a
+// covering geometry it is the inverse of piece_pair.  The kernels cut a work item's stored
+// bytes at piece boundaries and load each run from its piece (copy_span.cuh: copy_span_rows)
+// or place each vector with it (kv_fp8.cu: PiecedRows); the CPU tests call it through
+// _infinistore.testing.piece_write_offset.
+struct PieceOffset {
+    uint32_t piece, off;
+};
+ISTORE_KHD inline PieceOffset piece_write_offset(uint32_t o, uint32_t row_bytes, uint32_t src_pitch,
+                                                 uint32_t dst_pitch, uint32_t dst_slice_pitch,
+                                                 uint32_t piece_rows) {
+    const uint32_t piece_bytes = piece_rows * src_pitch, t = o / piece_bytes;
+    return PieceOffset{t, row_write_offset(o - t * piece_bytes, row_bytes, src_pitch, dst_pitch,
+                                           dst_slice_pitch)};
+}
+
 // kv_gather_rows_write (launch_kv_gather with rows and write): the work items of the
 // whole-part write, (block, part, chunk of the stored part) numbered (b * nparts + s) * cpp + c
 // with plan_gather's ld/st chunks, so every item stores one contiguous run of pool bytes and
@@ -356,7 +399,7 @@ ISTORE_KHD inline uint32_t row_write_offset(uint32_t o, uint32_t row_bytes, uint
 inline LaunchPlan plan_gather_rows_write(const GatherLaunch& a, int sms, LdStResident res) {
     if (!a.write || a.group_flags || a.nparts == 0 || a.nparts > kGatherMaxParts ||
         !row_geometry_ok(a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.slices,
-                         a.dst_slice_pitch, a.part_bytes) ||
+                         a.dst_slice_pitch, a.part_bytes, a.pieces) ||
         !row_write_covers(a.row_bytes, a.src_pitch, a.src_col, a.slices))
         return invalid_plan();
     const uint64_t geo_or =
@@ -383,7 +426,7 @@ inline LaunchPlan plan_gather_fp8_rows_write(const GatherLaunch& a, uint32_t ele
                                              LdStResident res) {
     if (!a.write || a.group_flags || a.nparts == 0 || a.nparts > kGatherMaxParts ||
         !row_geometry_ok(a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.slices,
-                         a.dst_slice_pitch, a.part_bytes) ||
+                         a.dst_slice_pitch, a.part_bytes, a.pieces) ||
         !row_write_covers(a.row_bytes, a.src_pitch, a.src_col, a.slices))
         return invalid_plan();
     const uint64_t geo_or = a.align_or | a.row_bytes | a.src_pitch | a.dst_pitch |
@@ -500,7 +543,7 @@ inline LaunchPlan plan_gather_fp8_rows(const GatherLaunch& a, uint32_t elems, in
                                        LdStResident res) {
     if (a.write || a.nparts == 0 || a.nparts > kGatherMaxParts ||
         !row_geometry_ok(a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.slices,
-                         a.dst_slice_pitch, a.part_bytes) ||
+                         a.dst_slice_pitch, a.part_bytes, a.pieces) ||
         (a.group_flags && (a.group_parts == 0 || a.nparts % a.group_parts != 0)))
         return invalid_plan();
     const uint64_t geo_or = a.align_or | a.row_bytes | a.src_pitch | a.src_col | a.dst_pitch |

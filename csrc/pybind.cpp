@@ -203,8 +203,12 @@ bool set_rows(G& g, const std::vector<uint32_t>& rows) {
 // geometry (set_rows); empty: whole parts.  The connection checks the values.
 Connection::GatherSpec gather_spec(const std::vector<uint64_t>& part_base, uint32_t part_bytes,
                                    uint32_t elems, uint32_t first_part,
-                                   const std::vector<uint32_t>& rows = {}) {
+                                   const std::vector<uint32_t>& rows = {},
+                                   const std::vector<uint64_t>* piece_off = nullptr,
+                                   uint32_t pieces = 1) {
     Connection::GatherSpec g;
+    g.pieces = pieces;
+    if (pieces > 1) g.piece_off = piece_off->data();
     g.part_base = part_base.data();
     g.nparts = uint32_t(part_base.size());
     g.part_bytes = part_bytes;
@@ -216,15 +220,33 @@ Connection::GatherSpec gather_spec(const std::vector<uint64_t>& part_base, uint3
     return g;
 }
 
+// A gathered call's piece table: `pieces` local offsets per block of n blocks (a flat int64
+// ndarray or list, n * pieces values), times `scale`.  pieces <= 1: none (empty).
+std::vector<uint64_t> piece_table(const py::object& obj, size_t n, uint32_t pieces,
+                                  uint64_t scale) {
+    std::vector<uint64_t> out;
+    if (pieces <= 1) return out;
+    if (obj.is_none()) throw py::value_error("pieces > 1 need piece_off");
+    OffsetSpan off;
+    offsets_from_py(obj, off);
+    if (off.n != n * pieces)
+        throw py::value_error("piece_off holds `pieces` offsets for every block");
+    out.resize(off.n);
+    for (size_t i = 0; i < off.n; ++i) out[i] = off.data[i] * scale;
+    return out;
+}
+
 // A row-sliced launch as the plan bindings of _infinistore.testing describe it: part_bytes is
 // rows * src_pitch, and group_parts > 0 makes it a layered read (the plans only ask whether
 // group_flags is set).
 kernels::GatherLaunch rows_launch(uint32_t n, uint32_t nparts, bool write, uint32_t rows,
                                   uint32_t row_bytes, uint32_t src_pitch, uint32_t src_col,
                                   uint32_t dst_pitch, uint32_t slices, uint32_t dst_slice_pitch,
-                                  uint64_t align_or, uint32_t group_parts, int max_ctas) {
+                                  uint64_t align_or, uint32_t group_parts, int max_ctas,
+                                  uint32_t pieces = 1) {
     static uint32_t flags[1];
     kernels::GatherLaunch a;
+    a.pieces = pieces;
     a.n = n;
     a.nparts = nparts;
     a.write = write;
@@ -619,35 +641,43 @@ PYBIND11_MODULE(_infinistore, m) {
             "w_rdma_gather",
             [](Connection& c, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
                uint32_t elems, const py::object& offsets, const py::object& remote_blocks,
-               int device, uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows) {
+               int device, uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows,
+               const py::object& piece_off, uint32_t pieces) {
                 BlockSpan rb;
                 OffsetSpan off;
                 blocks_from_py(remote_blocks, rb);
                 offsets_from_py(offsets, off);
                 std::vector<uint64_t> bytes(off.n);
                 for (size_t i = 0; i < off.n; ++i) bytes[i] = off.data[i] * scale;
-                const Connection::GatherSpec g = gather_spec(part_base, part_bytes, elems, 0, rows);
+                const std::vector<uint64_t> table = piece_table(piece_off, off.n, pieces, scale);
+                const Connection::GatherSpec g =
+                    gather_spec(part_base, part_bytes, elems, 0, rows, &table, pieces);
                 py::gil_scoped_release rel;
                 return c.w_rdma_gather(g, bytes.data(), bytes.size(), rb.data, rb.n, device, stream);
             },
             py::arg("part_base"), py::arg("part_bytes"), py::arg("elems"), py::arg("offsets"),
             py::arg("remote_blocks"), py::arg("device") = -1, py::arg("stream") = 0,
             py::arg("scale") = 1, py::arg("rows") = std::vector<uint32_t>{},
+            py::arg("piece_off") = py::none(), py::arg("pieces") = 1,
             "gathered write: block i = part s at part_base[s] + offsets[i] * scale, s = 0..S-1; "
             "elems > 0: bf16 parts of elems elements, quantised into fp8 page s of block i; "
             "rows = (rows, row_bytes, src_pitch, 0, dst_pitch[, slices, dst_slice_pitch]) filling "
             "each stored part: slice j of stored row r from part_base[s] + offset + r * "
-            "dst_pitch + j * dst_slice_pitch")
+            "dst_pitch + j * dst_slice_pitch; pieces > 1 (with rows): piece_off holds pieces "
+            "offsets per block (times scale), and run t of rows / pieces rows comes from "
+            "part_base[s] + offset + piece_off[i * pieces + t]")
         .def(
             "r_rdma_scatter",
             [](Connection& c, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
                uint32_t elems, uint32_t first_part, const py::object& blocks, int device,
                uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows,
-               Connection::ScatterReader* reader, uint32_t group_parts) {
+               Connection::ScatterReader* reader, uint32_t group_parts, const py::object& piece_off,
+               uint32_t pieces) {
                 std::vector<KeyOffset> kb;
                 blocks_list_from_py(blocks, scale, kb);
+                const std::vector<uint64_t> table = piece_table(piece_off, kb.size(), pieces, scale);
                 Connection::GatherSpec g =
-                    gather_spec(part_base, part_bytes, elems, first_part, rows);
+                    gather_spec(part_base, part_bytes, elems, first_part, rows, &table, pieces);
                 g.reader = reader;
                 g.group_parts = group_parts;
                 py::gil_scoped_release rel;
@@ -657,12 +687,14 @@ PYBIND11_MODULE(_infinistore, m) {
             py::arg("blocks"), py::arg("device") = -1, py::arg("stream") = 0,
             py::arg("scale") = 1, py::arg("rows") = std::vector<uint32_t>{},
             py::arg("reader") = py::none(), py::arg("group_parts") = 0,
+            py::arg("piece_off") = py::none(), py::arg("pieces") = 1,
             "scattered read: stored part first_part + s of each block -> part_base[s] + offset; "
             "elems > 0: fp8 pages dequantised into bf16 parts of elems elements; rows = (rows, "
             "row_bytes, src_pitch, src_col, dst_pitch[, slices, dst_slice_pitch]): only those "
             "rows of each part, slice j of row r to part_base[s] + offset + r * dst_pitch + j * "
             "dst_slice_pitch; reader: a layered read whose parts are "
-            "released in groups of group_parts (check reader.failed)")
+            "released in groups of group_parts (check reader.failed); pieces as for "
+            "w_rdma_gather")
         .def(
             "wait_layered",
             [](Connection& c, const Connection::ScatterReader& r, uint32_t group, uint64_t stream) {
@@ -682,7 +714,7 @@ PYBIND11_MODULE(_infinistore, m) {
         .def(
             "gather_writer",
             [](Connection& c, const py::object& remote_blocks, const py::object& offsets,
-               uint32_t nparts) {
+               uint32_t nparts, const py::object& piece_off, uint32_t pieces) {
                 BlockSpan rb;
                 OffsetSpan off;
                 blocks_from_py(remote_blocks, rb);
@@ -690,11 +722,16 @@ PYBIND11_MODULE(_infinistore, m) {
                 if (off.n != rb.n) throw std::invalid_argument("one offset per remote block");
                 if (nparts < 1 || nparts > kernels::kGatherMaxParts)
                     throw std::invalid_argument("a block holds 1 to GATHER_MAX_PARTS parts");
+                if (pieces < 1) throw std::invalid_argument("pieces must be at least 1");
+                const std::vector<uint64_t> table = piece_table(piece_off, off.n, pieces, 1);
                 py::gil_scoped_release rel;
-                return c.gather_writer(rb.data, off.data, rb.n, nparts);
+                return c.gather_writer(rb.data, off.data, rb.n, nparts,
+                                       pieces > 1 ? table.data() : nullptr, pieces);
             },
             py::arg("remote_blocks"), py::arg("offsets"), py::arg("nparts"),
-            "layered gathered writer over allocated blocks (offsets in elements)")
+            py::arg("piece_off") = py::none(), py::arg("pieces") = 1,
+            "layered gathered writer over allocated blocks (offsets in elements); pieces > 1: "
+            "piece_off (elements) as for w_rdma_gather, used by every call")
         .def(
             "w_rdma_layered",
             [](Connection& c, Connection::GatherWriter& w, const std::vector<uint64_t>& part_base,
@@ -1004,7 +1041,8 @@ PYBIND11_MODULE(_infinistore, m) {
            uint64_t table, uint64_t table_mask, uint64_t done, uint64_t status, uint64_t align_or,
            uint32_t stage_bytes, uint32_t ring_bytes, uint64_t layer_state, uint32_t layer_parts,
            bool layer_claim, uint64_t group_flags, uint64_t group_counters, uint32_t group_seq,
-           uint32_t group_parts, const std::vector<uint32_t>& rows) {
+           uint32_t group_parts, const std::vector<uint32_t>& rows, uint64_t piece_off,
+           uint32_t pieces) {
             if (part_base.empty() || part_base.size() > kernels::kGatherMaxParts)
                 throw std::runtime_error("kv_gather: 1 to GATHER_MAX_PARTS parts");
             if (layer_state && first_part + part_base.size() > layer_parts)
@@ -1039,6 +1077,8 @@ PYBIND11_MODULE(_infinistore, m) {
             G.group_parts = group_parts;
             if (!rows.empty() && !set_rows(G, rows))
                 throw std::runtime_error("kv_gather: rows is 5 or 7 values");
+            G.piece_off = as_ptr<const uint64_t>(piece_off);
+            G.pieces = pieces;
             const cudaError_t e = kernels::launch_kv_gather(G, as_ptr<CUstream_st>(stream));
             if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
         },
@@ -1050,6 +1090,7 @@ PYBIND11_MODULE(_infinistore, m) {
         py::arg("layer_state") = 0, py::arg("layer_parts") = 0, py::arg("layer_claim") = false,
         py::arg("group_flags") = 0, py::arg("group_counters") = 0, py::arg("group_seq") = 0,
         py::arg("group_parts") = 0, py::arg("rows") = std::vector<uint32_t>{},
+        py::arg("piece_off") = 0, py::arg("pieces") = 1,
         "gathered blocks: descs[i] = write {local byte offset, block address} / read {block "
         "address or 0, local byte offset}; part s of block i at part_base[s] + local offset is "
         "stored part first_part + s.  layer_state (3 zeroed u32 per block, kept across the "
@@ -1058,7 +1099,9 @@ PYBIND11_MODULE(_infinistore, m) {
         "group_flags (reads): a layered read that stores group_seq to group_flags[g] once "
         "group g (group_parts parts of every block) has landed; group_counters: one zeroed "
         "u32 per group.  rows (5 or 7 values): a row-sliced read, or a write whose rows fill "
-        "each stored part");
+        "each stored part.  pieces > 1 (with rows): piece_off is the device address of n * "
+        "pieces byte offsets, and run t of block i's rows / pieces rows is at part_base[s] + "
+        "local offset + piece_off[i * pieces + t]");
     k.def(
         "kv_gather_fp8",
         [](uint64_t descs, uint32_t n, const std::vector<uint64_t>& part_base, uint32_t elems,
@@ -1066,7 +1109,8 @@ PYBIND11_MODULE(_infinistore, m) {
            uint64_t recs, uint64_t table, uint64_t table_mask, uint64_t done, uint64_t status,
            uint64_t align_or, uint64_t layer_state, uint32_t layer_parts, bool layer_claim,
            uint64_t group_flags, uint64_t group_counters, uint32_t group_seq,
-           uint32_t group_parts, const std::vector<uint32_t>& rows) {
+           uint32_t group_parts, const std::vector<uint32_t>& rows, uint64_t piece_off,
+           uint32_t pieces) {
             if (part_base.empty() || part_base.size() > kernels::kGatherMaxParts)
                 throw std::runtime_error("kv_gather_fp8: 1 to GATHER_MAX_PARTS parts");
             if (layer_state && first_part + part_base.size() > layer_parts)
@@ -1101,6 +1145,8 @@ PYBIND11_MODULE(_infinistore, m) {
                     throw std::runtime_error("kv_gather_fp8: rows is 5 or 7 values");
                 G.part_bytes = 2 * elems;
             }
+            G.piece_off = as_ptr<const uint64_t>(piece_off);
+            G.pieces = pieces;
             const cudaError_t e =
                 kernels::launch_kv_gather_fp8(G, elems, variant, as_ptr<CUstream_st>(stream));
             if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
@@ -1112,8 +1158,8 @@ PYBIND11_MODULE(_infinistore, m) {
         py::arg("align_or") = 0, py::arg("layer_state") = 0, py::arg("layer_parts") = 0,
         py::arg("layer_claim") = false, py::arg("group_flags") = 0, py::arg("group_counters") = 0,
         py::arg("group_seq") = 0, py::arg("group_parts") = 0,
-        py::arg("rows") = std::vector<uint32_t>{},
-        "gathered fp8 blocks: descs as for kv_gather; part s (elems bf16 elements at "
+        py::arg("rows") = std::vector<uint32_t>{}, py::arg("piece_off") = 0, py::arg("pieces") = 1,
+        "gathered fp8 blocks: descs as for kv_gather; pieces as for kv_gather; part s (elems bf16 elements at "
         "part_base[s] + local offset) <-> fp8 page first_part + s of the block; layer_* and "
         "group_* as for kv_gather (a layered read always runs the ld/st kernel); rows as for "
         "kv_gather, in bytes of the parts' bf16 view: a read dequantises those rows of each "
@@ -1563,7 +1609,32 @@ PYBIND11_MODULE(_infinistore, m) {
           py::arg("src_pitch"), py::arg("src_col"), py::arg("slices"));
     t.def("row_geometry_ok", &kernels::row_geometry_ok, py::arg("rows"), py::arg("row_bytes"),
           py::arg("src_pitch"), py::arg("src_col"), py::arg("dst_pitch"), py::arg("slices"),
-          py::arg("dst_slice_pitch"), py::arg("part_bytes"));
+          py::arg("dst_slice_pitch"), py::arg("part_bytes"), py::arg("pieces") = 1);
+    // pieces: where (slice, row) pair q goes (piece, offset inside it), and where byte o of a
+    // covered stored part comes from
+    t.def("piece_pair",
+          [](uint32_t q, uint32_t rows, uint32_t row, uint32_t src_pitch, uint32_t src_col,
+             uint32_t dst_pitch, uint32_t dst_slice_pitch, uint32_t piece_rows) {
+              if (!rows || !piece_rows) throw py::value_error("needs rows, piece_rows > 0");
+              const kernels::PieceOffsets o = kernels::piece_pair(
+                  q, rows, row, src_pitch, src_col, dst_pitch, dst_slice_pitch, piece_rows);
+              return py::make_tuple(o.src, o.dst, o.piece);
+          },
+          py::arg("q"), py::arg("rows"), py::arg("row"), py::arg("src_pitch"),
+          py::arg("src_col"), py::arg("dst_pitch"), py::arg("dst_slice_pitch"),
+          py::arg("piece_rows"));
+    t.def("piece_write_offset",
+          [](uint32_t o, uint32_t row_bytes, uint32_t src_pitch, uint32_t dst_pitch,
+             uint32_t dst_slice_pitch, uint32_t piece_rows) {
+              if (!row_bytes || !src_pitch || !piece_rows)
+                  throw py::value_error("needs row_bytes, src_pitch, piece_rows > 0");
+              const kernels::PieceOffset p = kernels::piece_write_offset(
+                  o, row_bytes, src_pitch, dst_pitch, dst_slice_pitch, piece_rows);
+              return py::make_tuple(p.piece, p.off);
+          },
+          py::arg("o"), py::arg("row_bytes"), py::arg("src_pitch"), py::arg("dst_pitch"),
+          py::arg("dst_slice_pitch"), py::arg("piece_rows"));
+    t.attr("PIECE_RING_BYTES") = kPieceRingBytes;
     // how a read call is split into launches (ctrl/staging.h), with the client's limits
     t.attr("RING_BYTES") = kRingBytes;
     t.attr("MAX_BATCH") = kMaxBatch;
@@ -1682,17 +1753,17 @@ PYBIND11_MODULE(_infinistore, m) {
           [plan_dict](uint32_t n, uint32_t nparts, uint32_t rows, uint32_t row_bytes,
                       uint32_t src_pitch, uint32_t src_col, uint32_t dst_pitch, uint64_t align_or,
                       uint32_t group_parts, int max_ctas, int sm_count, int resident16,
-                      int resident32, uint32_t slices, uint32_t dst_slice_pitch) {
+                      int resident32, uint32_t slices, uint32_t dst_slice_pitch, uint32_t pieces) {
               const kernels::GatherLaunch a =
                   rows_launch(n, nparts, false, rows, row_bytes, src_pitch, src_col, dst_pitch,
-                              slices, dst_slice_pitch, align_or, group_parts, max_ctas);
+                              slices, dst_slice_pitch, align_or, group_parts, max_ctas, pieces);
               return plan_dict(kernels::plan_gather_rows(a, sm_count, {resident16, resident32}));
           },
           py::arg("n"), py::arg("nparts"), py::arg("rows"), py::arg("row_bytes"),
           py::arg("src_pitch"), py::arg("src_col") = 0, py::arg("dst_pitch") = 0,
           py::arg("align_or") = 0, py::arg("group_parts") = 0, py::arg("max_ctas") = 0,
           py::arg("sm_count") = 132, py::arg("resident16") = 1, py::arg("resident32") = 1,
-          py::arg("slices") = 1, py::arg("dst_slice_pitch") = 0);
+          py::arg("slices") = 1, py::arg("dst_slice_pitch") = 0, py::arg("pieces") = 1);
     t.def("plan_read_fused",
           [plan_dict](uint32_t n, uint32_t bytes, uint64_t align_or, int variant, int max_ctas,
                       uint32_t stage_bytes, uint32_t ring_bytes, int sm_count, int resident16,
@@ -1742,10 +1813,11 @@ PYBIND11_MODULE(_infinistore, m) {
           [plan_dict](uint32_t n, uint32_t nparts, uint32_t elems, uint32_t rows,
                       uint32_t row_bytes, uint32_t src_pitch, uint32_t src_col, uint32_t dst_pitch,
                       uint64_t align_or, uint32_t group_parts, bool write, int max_ctas,
-                      int sm_count, int resident, uint32_t slices, uint32_t dst_slice_pitch) {
+                      int sm_count, int resident, uint32_t slices, uint32_t dst_slice_pitch,
+                      uint32_t pieces) {
               const kernels::GatherLaunch a =
                   rows_launch(n, nparts, write, rows, row_bytes, src_pitch, src_col, dst_pitch,
-                              slices, dst_slice_pitch, align_or, group_parts, max_ctas);
+                              slices, dst_slice_pitch, align_or, group_parts, max_ctas, pieces);
               return plan_dict(
                   kernels::plan_gather_fp8_rows(a, elems, sm_count, {resident, resident}));
           },
@@ -1753,7 +1825,7 @@ PYBIND11_MODULE(_infinistore, m) {
           py::arg("src_pitch"), py::arg("src_col") = 0, py::arg("dst_pitch") = 0,
           py::arg("align_or") = 0, py::arg("group_parts") = 0, py::arg("write") = false,
           py::arg("max_ctas") = 0, py::arg("sm_count") = 132, py::arg("resident") = 1,
-          py::arg("slices") = 1, py::arg("dst_slice_pitch") = 0);
+          py::arg("slices") = 1, py::arg("dst_slice_pitch") = 0, py::arg("pieces") = 1);
     // row-sliced writes (kernels/launch_plan.h); group_parts > 0 asks for a layered read, which
     // the write plans refuse
     t.def("plan_gather_rows_write",
@@ -1761,10 +1833,10 @@ PYBIND11_MODULE(_infinistore, m) {
                       uint32_t src_pitch, uint32_t src_col, uint32_t dst_pitch, uint32_t slices,
                       uint32_t dst_slice_pitch, uint64_t align_or, bool write,
                       uint32_t group_parts, int max_ctas, int sm_count, int resident16,
-                      int resident32) {
+                      int resident32, uint32_t pieces) {
               const kernels::GatherLaunch a =
                   rows_launch(n, nparts, write, rows, row_bytes, src_pitch, src_col, dst_pitch,
-                              slices, dst_slice_pitch, align_or, group_parts, max_ctas);
+                              slices, dst_slice_pitch, align_or, group_parts, max_ctas, pieces);
               return plan_dict(
                   kernels::plan_gather_rows_write(a, sm_count, {resident16, resident32}));
           },
@@ -1772,15 +1844,17 @@ PYBIND11_MODULE(_infinistore, m) {
           py::arg("src_pitch"), py::arg("src_col") = 0, py::arg("dst_pitch") = 0,
           py::arg("slices") = 1, py::arg("dst_slice_pitch") = 0, py::arg("align_or") = 0,
           py::arg("write") = true, py::arg("group_parts") = 0, py::arg("max_ctas") = 0,
-          py::arg("sm_count") = 132, py::arg("resident16") = 1, py::arg("resident32") = 1);
+          py::arg("sm_count") = 132, py::arg("resident16") = 1, py::arg("resident32") = 1,
+          py::arg("pieces") = 1);
     t.def("plan_gather_fp8_rows_write",
           [plan_dict](uint32_t n, uint32_t nparts, uint32_t elems, uint32_t rows,
                       uint32_t row_bytes, uint32_t src_pitch, uint32_t src_col, uint32_t dst_pitch,
                       uint32_t slices, uint32_t dst_slice_pitch, uint64_t align_or, bool write,
-                      uint32_t group_parts, int max_ctas, int sm_count, int resident) {
+                      uint32_t group_parts, int max_ctas, int sm_count, int resident,
+                      uint32_t pieces) {
               const kernels::GatherLaunch a =
                   rows_launch(n, nparts, write, rows, row_bytes, src_pitch, src_col, dst_pitch,
-                              slices, dst_slice_pitch, align_or, group_parts, max_ctas);
+                              slices, dst_slice_pitch, align_or, group_parts, max_ctas, pieces);
               return plan_dict(
                   kernels::plan_gather_fp8_rows_write(a, elems, sm_count, {resident, resident}));
           },
@@ -1788,7 +1862,7 @@ PYBIND11_MODULE(_infinistore, m) {
           py::arg("src_pitch"), py::arg("src_col") = 0, py::arg("dst_pitch") = 0,
           py::arg("slices") = 1, py::arg("dst_slice_pitch") = 0, py::arg("align_or") = 0,
           py::arg("write") = true, py::arg("group_parts") = 0, py::arg("max_ctas") = 0,
-          py::arg("sm_count") = 132, py::arg("resident") = 1);
+          py::arg("sm_count") = 132, py::arg("resident") = 1, py::arg("pieces") = 1);
     t.def("fp8_rows_read_bytes", &fp8_rows_read_bytes, py::arg("rows"), py::arg("row_bytes"),
           py::arg("src_pitch"), py::arg("src_col") = 0,
           "bytes_read of a row-sliced read of one stored fp8 part (geometry in bf16 bytes)");

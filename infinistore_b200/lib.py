@@ -435,6 +435,13 @@ def _split_blocks(blocks):
     return [b[0] for b in blocks], [int(b[1]) for b in blocks]
 
 
+def _piece_args(table) -> dict:
+    """The native calls' piece arguments for a piece table (``_gather_parts``; None: none)."""
+    if table is None:
+        return {}
+    return {"piece_off": np.ascontiguousarray(table.reshape(-1)), "pieces": int(table.shape[1])}
+
+
 def _device_of(cache: torch.Tensor) -> int:
     return cache.device.index if cache.device.type == "cuda" else -1
 
@@ -708,12 +715,28 @@ class InfinityConnection:
         the parts are bf16 CUDA tensors, ``part_size`` is a multiple of 512 elements and every
         part base and offset is 16-byte aligned.  ``rows``: a row-sliced call (with ``fp8``,
         its geometry in multiples of 8 elements); with ``write`` its rows must fill the stored
-        part (``src_offset == 0`` and ``slices * width == src_pitch``).  Returns
-        (absolute byte address of every part, device ordinal or -1, element size, int64
-        offsets, stream handle)."""
+        part (``src_offset == 0`` and ``slices * width == src_pitch``).  2-D ``offsets``
+        ``(n, k)`` (with ``rows``, ``k`` dividing ``rows.count``): piece i of every part of
+        block b, rows ``i * count / k .. (i + 1) * count / k - 1``, is at ``offsets[b, i]``;
+        ``k == 1`` is the 1-D call.  Returns (absolute byte address of every part, device
+        ordinal or -1, element size, int64 offsets, stream handle, piece table): with pieces
+        the offsets are zeros and the piece table is the ``(n, k)`` offsets, else None."""
         if self._mode != "rdma":
             raise Exception("gathered blocks need a connected rdma connection")
-        offs = np.ascontiguousarray(offsets, dtype=np.int64).reshape(-1)
+        offs = np.ascontiguousarray(offsets, dtype=np.int64)
+        table = None
+        if offs.ndim == 2 and offs.shape[1] == 1:
+            offs = offs[:, 0]
+        elif offs.ndim == 2:
+            if rows is None:
+                raise ValueError("2-D offsets (one per piece of a block) need rows=")
+            if rows.count % offs.shape[1]:
+                raise ValueError(f"{offs.shape[1]} pieces do not divide the {rows.count} rows")
+            table = offs
+            offs = np.zeros(len(table), dtype=np.int64)
+        elif offs.ndim > 2:
+            raise ValueError("offsets are 1-D, or 2-D with one column per piece")
+        offs = offs.reshape(-1)
         if nblocks is not None and len(offs) != nblocks:
             raise ValueError(f"{len(offs)} offsets for {nblocks} blocks")
         if len(offs) and int(offs.min()) < 0:
@@ -721,7 +744,15 @@ class InfinityConnection:
         first_part = int(first_part)
         if first_part < 0:
             raise ValueError("first_part must not be negative")
-        extent = rows.check(part_size) if rows is not None else int(part_size)
+        if table is not None:  # each piece is count / k rows of part_size / k elements
+            k = table.shape[1]
+            extent = PartRows(rows.count // k, rows.width, rows.src_pitch, rows.src_offset,
+                              dst_pitch=rows.dst_pitch, slices=rows.slices,
+                              dst_slice_pitch=rows.dst_slice_pitch).check(int(part_size) // k)
+            if table.size and int(table.min()) < 0:
+                raise ValueError("offsets must not be negative")
+        else:
+            extent = rows.check(part_size) if rows is not None else int(part_size)
         if write and rows is not None and (rows.src_offset != 0
                                            or rows.slices * rows.width != rows.src_pitch):
             raise ValueError(f"{rows}: a row-sliced write must fill the stored part "
@@ -743,7 +774,8 @@ class InfinityConnection:
         if nparts * pool_part > _GATHER_MAX_BLOCK_BYTES:
             raise ValueError(f"{nparts} parts of {pool_part} bytes exceed the "
                              f"{_GATHER_MAX_BLOCK_BYTES}-byte block limit")
-        max_offset = int(offs.max()) if len(offs) else 0
+        local = offs if table is None else table
+        max_offset = int(local.max()) if local.size else 0
         bases = []
         for i, (t, base) in enumerate(parts):
             base = int(base)
@@ -772,8 +804,8 @@ class InfinityConnection:
             align = 0
             for b in bases:
                 align |= b
-            if len(offs):
-                align |= int(np.bitwise_or.reduce(offs * es))
+            if local.size:
+                align |= int(np.bitwise_or.reduce(local.reshape(-1) * es))
             if align & 15:
                 raise ValueError("fp8 gathered blocks need 16-byte aligned part bases and offsets")
             if first.device.type != "cuda":
@@ -782,7 +814,7 @@ class InfinityConnection:
         if dev < 0 and self.conn.server_has_hbm():
             raise ValueError("gathered blocks of CPU tensors need a host-memory pool "
                              "(--pool-backend host)")
-        return bases, dev, es, offs, _stream_of(first, stream)
+        return bases, dev, es, offs, _stream_of(first, stream), table
 
     def rdma_write_cache_gather(self, parts, offsets, part_size: int, remote_blocks,
                                 stream="current", rows: "PartRows | None" = None):
@@ -806,15 +838,20 @@ class InfinityConnection:
         (``src_offset == 0``, ``slices * width == src_pitch``), e.g. a head-major page
         ``[head][token][dim]`` stored token-major.  The stored bytes are those of a write
         without rows from the transposed page.  Bad geometry raises ``ValueError`` before
-        anything is enqueued."""
-        bases, dev, es, offs, s = self._gather_parts(parts, offsets, part_size, rows=rows,
-                                                     nblocks=len(remote_blocks), stream=stream,
-                                                     write=True)
+        anything is enqueued.
+
+        With ``rows``, ``offsets`` may be an ``(n, k)`` int64 array (pieces): the ``rows.count``
+        rows of every stored part split into k runs, and run i of block b is taken from
+        ``offsets[b, i]`` - e.g. a chunk of k engine pages stored under one key, each page where
+        the block table puts it.  k must divide ``rows.count``; ``(n, 1)`` is the 1-D call."""
+        bases, dev, es, offs, s, table = self._gather_parts(parts, offsets, part_size, rows=rows,
+                                                            nblocks=len(remote_blocks),
+                                                            stream=stream, write=True)
         native_rows = rows.native(es) if rows is not None else []
         if not len(offs):
             return 0
         ret = self.conn.w_rdma_gather(bases, int(part_size) * es, 0, offs, remote_blocks, dev, s,
-                                      es, native_rows)
+                                      es, native_rows, **_piece_args(table))
         if ret < 0:
             raise Exception(f"Failed to write to infinistore, ret = {ret}: {self.conn.last_error()}")
         return 0
@@ -837,15 +874,19 @@ class InfinityConnection:
         ``parts[s][1] + offset + r * rows.dst_pitch``.  Several blocks may fill disjoint rows
         of one destination, e.g. one per source rank of a page written at another
         tensor-parallel degree.  Bad geometry raises ``ValueError`` before anything is
-        enqueued."""
+        enqueued.  With ``rows``, ``(keys, offsets)`` may carry an ``(n, k)`` int64 array
+        (pieces, as for ``rdma_write_cache_gather``): run i of the rows of block b lands at
+        ``offsets[b, i]``."""
         keys, offs = _split_blocks(blocks)
-        bases, dev, es, offs, s = self._gather_parts(parts, offs, part_size, first_part,
-                                                     rows=rows, nblocks=len(keys), stream=stream)
+        bases, dev, es, offs, s, table = self._gather_parts(parts, offs, part_size, first_part,
+                                                            rows=rows, nblocks=len(keys),
+                                                            stream=stream)
         native_rows = rows.native(es) if rows is not None else []
         if not len(offs):
             return
         ret = self.conn.r_rdma_scatter(bases, int(part_size) * es, 0, int(first_part),
-                                       (keys, offs), dev, s, es, native_rows)
+                                       (keys, offs), dev, s, es, native_rows,
+                                       **_piece_args(table))
         if ret < 0:
             raise Exception(f"Failed to read to infinistore, ret = {ret}: {self.conn.last_error()}")
 
@@ -868,14 +909,15 @@ class InfinityConnection:
         allocated with ``fp8_gather_block_bytes(len(parts), part_size)`` bytes.  ``rows`` as
         for ``rdma_write_cache_gather``, in multiples of 8 elements: each stored page is the
         one the write without rows stores for the transposed page."""
-        bases, dev, es, offs, s = self._gather_parts(parts, offsets, part_size, fp8=True,
-                                                     rows=rows, nblocks=len(remote_blocks),
-                                                     stream=stream, write=True)
+        bases, dev, es, offs, s, table = self._gather_parts(parts, offsets, part_size, fp8=True,
+                                                            rows=rows, nblocks=len(remote_blocks),
+                                                            stream=stream, write=True)
         native_rows = rows.native(es) if rows is not None else []
         if not len(offs):
             return 0
         ret = self.conn.w_rdma_gather(bases, int(part_size) * es, int(part_size), offs,
-                                      remote_blocks, dev, s, es, native_rows)
+                                      remote_blocks, dev, s, es, native_rows,
+                                      **_piece_args(table))
         if ret < 0:
             raise Exception(f"Failed to write to infinistore, ret = {ret}: {self.conn.last_error()}")
         return 0
@@ -894,14 +936,15 @@ class InfinityConnection:
         read.  ``width``, ``src_pitch``, ``src_offset`` and ``dst_pitch`` must be multiples of 8
         elements; rows need not line up with the scale groups."""
         keys, offs = _split_blocks(blocks)
-        bases, dev, es, offs, s = self._gather_parts(parts, offs, part_size, first_part,
-                                                     fp8=True, rows=rows, nblocks=len(keys),
-                                                     stream=stream)
+        bases, dev, es, offs, s, table = self._gather_parts(parts, offs, part_size, first_part,
+                                                            fp8=True, rows=rows,
+                                                            nblocks=len(keys), stream=stream)
         native_rows = rows.native(es) if rows is not None else []
         if not len(offs):
             return
         ret = self.conn.r_rdma_scatter(bases, int(part_size) * es, int(part_size), int(first_part),
-                                       (keys, offs), dev, s, es, native_rows)
+                                       (keys, offs), dev, s, es, native_rows,
+                                       **_piece_args(table))
         if ret < 0:
             raise Exception(f"Failed to read to infinistore, ret = {ret}: {self.conn.last_error()}")
 
@@ -925,9 +968,9 @@ class InfinityConnection:
         raises here; the exception's ``read`` attribute is the failed reader.  ``rows`` as for
         ``read_cache_scatter[_fp8]``."""
         keys, offs = _split_blocks(blocks)
-        bases, dev, es, offs, s = self._gather_parts(parts, offs, part_size, first_part,
-                                                     fp8=fp8, rows=rows, nblocks=len(keys),
-                                                     stream=stream)
+        bases, dev, es, offs, s, table = self._gather_parts(parts, offs, part_size, first_part,
+                                                            fp8=fp8, rows=rows, nblocks=len(keys),
+                                                            stream=stream)
         if dev < 0:
             raise ValueError("layered reads take CUDA tensors")
         if not self.conn.server_has_hbm():
@@ -938,7 +981,8 @@ class InfinityConnection:
         native = _infinistore.ScatterReader()
         self.conn.r_rdma_scatter(bases, int(part_size) * es, int(part_size) if fp8 else 0,
                                  int(first_part), (keys, offs), dev, s, es,
-                                 rows.native(es) if rows is not None else [], native, group_parts)
+                                 rows.native(es) if rows is not None else [], native, group_parts,
+                                 **_piece_args(table))
         read = ScatterRead(self, native, parts[0][0].device)
         if native.failed:
             err = Exception(f"Failed to read to infinistore: {self.conn.last_error()}")
@@ -960,16 +1004,23 @@ class InfinityConnection:
         completes leaves its blocks uncommitted; closing the connection releases them."""
         if self._mode != "rdma":
             raise Exception("gathered blocks need a connected rdma connection")
-        offs = np.ascontiguousarray(offsets, dtype=np.int64).reshape(-1)
+        offs = np.ascontiguousarray(offsets, dtype=np.int64)
+        if offs.ndim == 2 and offs.shape[1] == 1:
+            offs = offs[:, 0]
+        if offs.ndim not in (1, 2):
+            raise ValueError("offsets are 1-D, or 2-D with one column per piece")
         if len(offs) != len(remote_blocks):
             raise ValueError(f"{len(offs)} offsets for {len(remote_blocks)} remote blocks")
-        if len(offs) and int(offs.min()) < 0:
+        if offs.size and int(offs.min()) < 0:
             raise ValueError("offsets must not be negative")
         if not 1 <= int(nparts) <= GATHER_MAX_PARTS:
             raise ValueError(f"a block holds 1 to {GATHER_MAX_PARTS} parts, not {nparts}")
         if int(part_size) <= 0:
             raise ValueError("part_size must be positive")
-        native = self.conn.gather_writer(remote_blocks, offs, int(nparts))
+        table = offs if offs.ndim == 2 else None
+        native = self.conn.gather_writer(
+            remote_blocks, offs if table is None else np.zeros(len(offs), dtype=np.int64),
+            int(nparts), **_piece_args(table))
         return GatherWriter(self, native, offs, int(nparts), int(part_size), bool(fp8))
 
     async def read_cache_async(self, cache: torch.Tensor, blocks: List[Tuple[str, int]],
@@ -1246,9 +1297,11 @@ class GatherWriter:
         if any(written[first_part:first_part + len(parts)]):
             raise ValueError("the part range overlaps parts written before")
         conn = self._conn
-        bases, dev, es, _, s = conn._gather_parts(parts, self._offs, self.part_size, first_part,
-                                                  self.nparts, self.fp8, rows, stream=stream,
-                                                  write=True)
+        if self._offs.ndim == 2 and rows is None:
+            raise ValueError("a writer made with 2-D offsets (pieces) needs rows= on every call")
+        bases, dev, es, _, s, _ = conn._gather_parts(parts, self._offs, self.part_size, first_part,
+                                                     self.nparts, self.fp8, rows, stream=stream,
+                                                     write=True)
         native_rows = rows.native(es) if rows is not None else []
         first = parts[0][0]
         if self._dev is not None and self._dev != (first.device, first.dtype):

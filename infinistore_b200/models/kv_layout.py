@@ -123,3 +123,11 @@ def page_key(model: str, layer, kind: str, tp_rank: int, page_hash: str) -> str:
     """Key of one page: model / layer (or ``ALL_LAYERS``) / K|V|KV / TP rank / chained
     prefix hash."""
     return f"{model}/L{layer}/{kind}/tp{tp_rank}/{page_hash}"
+
+
+def chunk_key(model: str, chunk_tokens: int, tp_rank: int, chunk_hash: str) -> str:
+    """Key of one all-layer chunk of ``chunk_tokens`` tokens (``_PagedCache.write_chunks``):
+    like an all-layer ``page_key``, with the token count in the kind field (``KVx256``), so
+    keys of different chunk sizes, and page keys, never resolve to each other's blocks.
+    ``chunk_hash`` comes from ``chain_hashes(token_ids, chunk_tokens)``."""
+    return f"{model}/L{ALL_LAYERS}/KVx{int(chunk_tokens)}/tp{tp_rank}/{chunk_hash}"

@@ -6,8 +6,8 @@ from typing import List, Optional, Sequence
 import numpy as np
 import torch
 
-from ..lib import PartRows
-from .kv_layout import ALL_LAYERS, KVLayout, page_key, tp_sources
+from ..lib import _GATHER_MAX_BLOCK_BYTES, PartRows
+from .kv_layout import ALL_LAYERS, KVLayout, chunk_key, page_key, tp_sources
 
 
 def layer_keys(layout: KVLayout, tp_rank: int, layer: int, kv: int,
@@ -24,7 +24,14 @@ class _PagedCache:
     2l (K) and 2l + 1 (V)), read from ranks at this or another tensor-parallel degree.  The
     pages are byte-identical in the store whichever cache wrote them; a subclass gives only
     where a source rank's heads land in its page layout (``_source_rows``) and how its page
-    fills a stored part (``_write_rows``)."""
+    fills a stored part (``_write_rows``).
+
+    Chunks (``write_chunks``, ``chunk_writer``, ``read_chunks[_layered]``) store k pages under
+    one key: the stored block is the all-layer page of ``k * page_tokens`` tokens that a cache
+    of that page size would store, and page i of chunk b is this cache's page
+    ``block_table[b, i]``.  The kernels land each page's rows through the block table
+    (``PartRows`` with 2-D offsets), with the rows of ``_source_rows`` / ``_write_rows``
+    stretched over the chunk."""
 
     def __init__(self, layout: KVLayout, num_pages: int, tp_rank: int, data: torch.Tensor):
         self.layout = layout
@@ -75,11 +82,13 @@ class _PagedCache:
         raise NotImplementedError
 
     def _sources(self, pages: Sequence[int], page_hashes: Sequence[str],
-                 source_tp: Optional[int]):
+                 source_tp: Optional[int], chunk_pages: int = 0):
         """The blocks of a read of pages written at ``source_tp`` (None: this TP degree, by
         this rank): one per (page, source rank), keyed by the writer rank, each landing at its
         heads of the reader's page, and the rows every block gives (``PartRows``, or None for
-        whole parts) and the stored part size."""
+        whole parts) and the stored part size.  ``chunk_pages`` k > 0: ``pages`` is an (n, k)
+        block table of chunks, and the blocks are one per (chunk, source rank), with (blocks,
+        k) offsets and the chunk's rows (``_chunk_rows``)."""
         lay = self.layout
         wl = lay if source_tp is None else lay.with_tp(int(source_tp))
         srcs = (tp_sources(lay, lay.tp, self.tp_rank, wl.tp) if self._cross_tp(source_tp)
@@ -90,9 +99,17 @@ class _PagedCache:
         if len(pages) != len(page_hashes):
             raise ValueError(f"{len(pages)} pages for {len(page_hashes)} page hashes")
         rows, head_elems = self._source_rows(wl, src_head, heads)
+        dst = np.asarray([d * head_elems for _, _, d, _ in srcs], dtype=np.int64)
+        if chunk_pages:
+            keys = [chunk_key(lay.name, chunk_pages * lay.page_tokens, w, h)
+                    for h in page_hashes for w, *_ in srcs]
+            offs = (np.asarray(pages, dtype=np.int64)[:, None, :] * lay.page_elems
+                    + dst[None, :, None])
+            return (keys, offs.reshape(-1, chunk_pages),
+                    self._chunk_rows(rows, chunk_pages, wl.page_elems),
+                    chunk_pages * wl.page_elems)
         keys = [page_key(lay.name, ALL_LAYERS, "KV", w, h) for h in page_hashes for w, *_ in srcs]
-        offs = (np.asarray(pages, dtype=np.int64)[:, None] * lay.page_elems
-                + np.asarray([d * head_elems for _, _, d, _ in srcs], dtype=np.int64)[None, :])
+        offs = np.asarray(pages, dtype=np.int64)[:, None] * lay.page_elems + dst[None, :]
         return keys, offs.reshape(-1), rows, wl.page_elems
 
     def _blocks(self, pages: Sequence[int], page_hashes: Sequence[str],
@@ -206,14 +223,23 @@ class _PagedCache:
 
     def cached_prefix_pages(self, conn, page_hashes: Sequence[str],
                             layer: Optional[int] = None, all_layer_pages: bool = False,
-                            source_tp: Optional[int] = None) -> int:
+                            source_tp: Optional[int] = None, chunk_pages: int = 0) -> int:
         """How many leading pages of this prefix the store already holds (last layer's V
         pages are written last, so probing them answers for the whole stack).
         ``all_layer_pages``: the pages were written with ``write_pages`` (one key each).
         ``source_tp`` (with ``all_layer_pages``): they were written at that TP degree; the
-        answer is the fewest pages any source rank of ``read_pages(source_tp=)`` holds."""
+        answer is the fewest pages any source rank of ``read_pages(source_tp=)`` holds.
+        ``chunk_pages`` k > 0: ``page_hashes`` are chunk hashes of chunks of k pages
+        (``write_chunks``), and the answer counts chunks."""
         if not page_hashes:
             return 0
+        if chunk_pages:
+            groups = (self.source_chunk_keys(page_hashes, chunk_pages, source_tp)
+                      if self._cross_tp(source_tp) else [self.chunk_keys(page_hashes, chunk_pages)])
+            try:
+                return min(conn.get_match_last_index(keys) + 1 for keys in groups)
+            except Exception:
+                return 0
         if self._cross_tp(source_tp):
             if not all_layer_pages:
                 raise ValueError("source_tp needs all_layer_pages")
@@ -232,12 +258,18 @@ class _PagedCache:
             return 0
 
     def touch_prefix(self, conn, page_hashes: Sequence[str], all_layer_pages: bool = False,
-                     source_tp: Optional[int] = None) -> int:
+                     source_tp: Optional[int] = None, chunk_pages: int = 0) -> int:
         """Tell an evicting store (``--evict``) that these pages were just used: every layer's
         K and V block of every page becomes most-recently-used.  Needed by clients that read
         through the device index, whose reads the server never sees.  Returns the number of
         blocks refreshed.  ``all_layer_pages``: the pages were written with ``write_pages``;
-        ``source_tp`` (with it): at that TP degree, and every source rank's key is touched."""
+        ``source_tp`` (with it): at that TP degree, and every source rank's key is touched.
+        ``chunk_pages`` k > 0: chunk hashes of chunks of k pages (``write_chunks``)."""
+        if chunk_pages:
+            keys = ([k for ks in self.source_chunk_keys(page_hashes, chunk_pages, source_tp)
+                     for k in ks] if self._cross_tp(source_tp)
+                    else self.chunk_keys(page_hashes, chunk_pages))
+            return conn.touch(keys) if keys else 0
         if self._cross_tp(source_tp):
             if not all_layer_pages:
                 raise ValueError("source_tp needs all_layer_pages")
@@ -251,6 +283,130 @@ class _PagedCache:
             for kv in (0, 1):
                 keys.extend(self.keys(layer, kv, page_hashes))
         return conn.touch(keys) if keys else 0
+
+
+    # ------------------------------------------------------------------ all-layer chunks
+    @staticmethod
+    def _chunk_rows(rows: Optional[PartRows], k: int, part: int) -> PartRows:
+        """The rows of a k-page chunk from one page's rows (``_source_rows``, ``_write_rows``):
+        ``k * count`` rows with the same pitches, one piece per page.  A page that is its
+        stored part of ``part`` elements, contiguously, is one row of ``part`` elements."""
+        if rows is None or (rows.slices == 1 and rows.src_offset == 0
+                            and rows.width == rows.src_pitch == rows.dst_pitch):
+            return PartRows(k, part, part, 0, dst_pitch=part)
+        return PartRows(rows.count * k, rows.width, rows.src_pitch, rows.src_offset,
+                        dst_pitch=rows.dst_pitch, slices=rows.slices,
+                        dst_slice_pitch=rows.dst_slice_pitch)
+
+    def chunk_keys(self, chunk_hashes: Sequence[str], chunk_pages: int) -> List[str]:
+        """Store keys of chunks of ``chunk_pages`` pages (``kv_layout.chunk_key``)."""
+        tokens = int(chunk_pages) * self.layout.page_tokens
+        return [chunk_key(self.layout.name, tokens, self.tp_rank, h) for h in chunk_hashes]
+
+    def source_chunk_keys(self, chunk_hashes: Sequence[str], chunk_pages: int,
+                          source_tp: int) -> List[List[str]]:
+        """``source_page_keys`` for chunks of ``chunk_pages`` pages."""
+        tokens = int(chunk_pages) * self.layout.page_tokens
+        srcs = tp_sources(self.layout, self.layout.tp, self.tp_rank, int(source_tp))
+        return [[chunk_key(self.layout.name, tokens, w, h) for h in chunk_hashes]
+                for w, *_ in srcs]
+
+    def _chunk_table(self, block_table, chunk_hashes: Sequence[str], read: bool) -> np.ndarray:
+        """The checked (n, k) block table of chunks; ValueError before anything happens."""
+        table = np.asarray(block_table, dtype=np.int64)
+        if table.ndim != 2 or table.shape[1] < 1:
+            raise ValueError("block_table is an (n, k) array of page indices, k >= 1")
+        if table.shape[0] != len(chunk_hashes):
+            raise ValueError(f"{table.shape[0]} block-table rows for {len(chunk_hashes)} chunk "
+                             f"hashes")
+        if table.size and (int(table.min()) < 0 or int(table.max()) >= self.num_pages):
+            raise ValueError(f"a page index is outside 0..{self.num_pages - 1}")
+        if read and len(np.unique(table)) != table.size:
+            raise ValueError("a page appears twice in the block table: two chunks would land "
+                             "on it")
+        return table
+
+    def _chunk_block_bytes(self, conn, k: int, fp8: bool) -> int:
+        """Pool bytes of one chunk; ValueError over the block limit."""
+        nparts, elems = 2 * self.layout.layers, k * self.layout.page_elems
+        nbytes = (conn.fp8_gather_block_bytes(nparts, elems) if fp8
+                  else nparts * k * self.layout.page_bytes)
+        if nbytes > _GATHER_MAX_BLOCK_BYTES:
+            raise ValueError(f"a chunk of {k} pages takes {nbytes} bytes, over the "
+                             f"{_GATHER_MAX_BLOCK_BYTES}-byte block limit")
+        return nbytes
+
+    def _chunk_write(self, conn, block_table, chunk_hashes: Sequence[str], fp8: bool):
+        """Checks, allocates and returns (blocks, offsets, rows, stored part size) of a chunk
+        write."""
+        table = self._chunk_table(block_table, chunk_hashes, read=False)
+        k, elems = table.shape[1], self.layout.page_elems
+        rows = self._chunk_rows(self._write_rows(), k, elems)
+        if fp8:  # heads move row by row unless each page is one row
+            self._check_fp8(rows.count != k)
+        nbytes = self._chunk_block_bytes(conn, k, fp8)
+        self._ensure_registered(conn)
+        blocks = conn.allocate_rdma(self.chunk_keys(chunk_hashes, k), nbytes)
+        return blocks, table * elems, rows, k * elems
+
+    def write_chunks(self, conn, block_table, chunk_hashes: Sequence[str], stream="current",
+                     fp8: bool = False) -> int:
+        """``write_pages`` for chunks: chunk b, pages ``block_table[b, 0..k-1]`` of this cache
+        in token order (``k * page_tokens`` tokens), is stored under ``chunk_keys`` as the
+        all-layer page a cache with ``page_tokens = k * page_tokens`` stores for the same
+        tokens.  ``chunk_hashes`` come from ``chain_hashes(token_ids, k * page_tokens)``; only
+        full chunks are stored.  Blocks whose key already exists are skipped.  Raises
+        ``ValueError`` before any block is allocated for a table whose row count differs from
+        the hashes, a page index outside the cache, a chunk over the block limit and every
+        ``write_pages`` refusal.  Returns the number of blocks written."""
+        blocks, offs, rows, part = self._chunk_write(conn, block_table, chunk_hashes, fp8)
+        write = conn.rdma_write_cache_gather_fp8 if fp8 else conn.rdma_write_cache_gather
+        write(self._parts(range(self.layout.layers)), offs, part, blocks, stream=stream, rows=rows)
+        return len(blocks)
+
+    def chunk_writer(self, conn, block_table, chunk_hashes: Sequence[str],
+                     fp8: bool = False) -> "PageWriter":
+        """``page_writer`` for chunks (``write_chunks``): ``write_layers`` stores layers of
+        every chunk as they are produced."""
+        blocks, offs, rows, part = self._chunk_write(conn, block_table, chunk_hashes, fp8)
+        writer = conn.gather_writer(blocks, offs, 2 * self.layout.layers, part, fp8=fp8)
+        return PageWriter(self, writer, rows)
+
+    def _chunk_read(self, block_table, chunk_hashes: Sequence[str], layers, fp8: bool,
+                    source_tp: Optional[int]):
+        table = self._chunk_table(block_table, chunk_hashes, read=True)
+        keys, offs, rows, part = self._sources(table, chunk_hashes, source_tp,
+                                               chunk_pages=table.shape[1])
+        if fp8:  # heads move row by row unless each page is one row
+            self._check_fp8(rows.count != table.shape[1])
+        return keys, offs, rows, part, self._check_layers(layers)
+
+    def read_chunks(self, conn, block_table, chunk_hashes: Sequence[str],
+                    layers: Optional[range] = None, stream="current", fp8: bool = False,
+                    source_tp: Optional[int] = None) -> int:
+        """``read_pages`` for chunks written by ``write_chunks`` / ``chunk_writer`` (at
+        ``source_tp``, as for ``read_pages``): page i of chunk b lands in this cache's page
+        ``block_table[b, i]``.  A page that appears twice in the table raises ``ValueError``
+        (two chunks would race on it).  Returns the number of (chunk, source) blocks read."""
+        keys, offs, rows, part, layers = self._chunk_read(block_table, chunk_hashes, layers, fp8,
+                                                          source_tp)
+        self._ensure_registered(conn)
+        read = conn.read_cache_scatter_fp8 if fp8 else conn.read_cache_scatter
+        read(self._parts(layers), (keys, offs), part, first_part=2 * layers.start,
+             stream=stream, rows=rows)
+        return len(keys)
+
+    def read_chunks_layered(self, conn, block_table, chunk_hashes: Sequence[str],
+                            layers: Optional[range] = None, fp8: bool = False,
+                            stream="current", source_tp: Optional[int] = None) -> "PageRead":
+        """``read_pages_layered`` for chunks (``read_chunks``)."""
+        keys, offs, rows, part, layers = self._chunk_read(block_table, chunk_hashes, layers, fp8,
+                                                          source_tp)
+        self._ensure_registered(conn)
+        read = conn.read_cache_scatter_layered(self._parts(layers), (keys, offs), part,
+                                               group_parts=2, first_part=2 * layers.start,
+                                               fp8=fp8, stream=stream, rows=rows)
+        return PageRead(read, layers)
 
 
 class PagedKVCache(_PagedCache):
@@ -330,9 +486,10 @@ class PagedKVCache(_PagedCache):
 class PageWriter:
     """Layer-by-layer upload of all-layer pages (``page_writer`` of either cache)."""
 
-    def __init__(self, cache: _PagedCache, writer):
+    def __init__(self, cache: _PagedCache, writer, rows: Optional[PartRows] = None):
         self.cache = cache
         self.writer = writer
+        self._chunk_rows = rows  # a chunk writer's rows (chunk_writer); None: the page's
 
     @property
     def complete(self) -> bool:
@@ -343,8 +500,8 @@ class PageWriter:
         n = self.cache.layout.layers
         if layers.step != 1 or not len(layers) or layers.start < 0 or layers.stop > n:
             raise ValueError(f"layers must be a non-empty step-1 range within 0..{n}")
-        self.writer.write(self.cache._parts(layers), 2 * layers.start, stream=stream,
-                          rows=self.cache._write_rows())
+        rows = self._chunk_rows if self._chunk_rows is not None else self.cache._write_rows()
+        self.writer.write(self.cache._parts(layers), 2 * layers.start, stream=stream, rows=rows)
 
 
 class PageRead:

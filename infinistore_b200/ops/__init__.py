@@ -109,12 +109,21 @@ def stream_wait_value(flags: torch.Tensor, index: int, value: int, stream=None) 
         K.stream_wait_value(flags.data_ptr() + 4 * int(index), int(value), h if h != 0 else 1)
 
 
+def _piece_args(pieces: Optional[torch.Tensor]):
+    """(device address, k) of an (n, k) piece table for the native gathers; (0, 1): none."""
+    if pieces is None:
+        return 0, 1
+    assert (pieces.is_cuda and pieces.dtype == torch.int64 and pieces.is_contiguous()
+            and pieces.dim() == 2)
+    return pieces.data_ptr(), pieces.shape[1]
+
+
 def kv_gather(descs: torch.Tensor, part_base: Sequence[int], part_bytes: int, write: bool,
               first_part: int = 0, max_ctas: int = 0, status: Optional[torch.Tensor] = None,
               align_or: int = 0, stage_bytes: int = 0, ring_bytes: int = 0,
               publish: Optional["PublishArgs"] = None, layer: Optional[LayerState] = None,
               claim: bool = False, release: Optional[GroupRelease] = None,
-              rows: Optional[Sequence[int]] = None) -> None:
+              rows: Optional[Sequence[int]] = None, pieces: Optional[torch.Tensor] = None) -> None:
     """Gathered blocks (csrc/kernels/kernels.h ``GatherLaunch``): block i is len(part_base)
     parts of ``part_bytes``, part s at ``part_base[s] + local offset``.  ``descs`` is (n, 2)
     int64: write {local byte offset, block address}, read {block address or 0 = miss, local
@@ -133,7 +142,10 @@ def kv_gather(descs: torch.Tensor, part_base: Sequence[int], part_bytes: int, wr
     ``rows`` runs the same geometry the other way (kv_gather_rows_write): slice j of stored row
     r is taken from part s's local address + ``r * dst_pitch + j * dst_slice_pitch``; the rows
     must fill the stored part (``src_col == 0``, ``slices * row_bytes == src_pitch``), and
-    ``publish`` / ``layer`` / ``claim`` work as without rows."""
+    ``publish`` / ``layer`` / ``claim`` work as without rows.  ``pieces`` (with ``rows``), an
+    (n, k) int64 CUDA tensor of local byte offsets: block i's rows are k runs of rows / k
+    rows, run t at part s's local address + ``pieces[i, t]`` (kv_scatter_pieces,
+    kv_gather_pieces_write); ``align_or`` must include them."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
     bases = [int(b) for b in part_base]
     for b in bases:
@@ -144,7 +156,7 @@ def kv_gather(descs: torch.Tensor, part_base: Sequence[int], part_bytes: int, wr
                     max_ctas, _stream(descs.device), *pub,
                     status.data_ptr() if status is not None else 0, align_or, stage_bytes,
                     ring_bytes, *lay, *_release_args(release),
-                    [int(r) for r in rows] if rows is not None else [])
+                    [int(r) for r in rows] if rows is not None else [], *_piece_args(pieces))
 
 
 def kv_copy_multicast(descs: torch.Tensor, nbytes: int, dst_deltas: Sequence[int],
@@ -342,7 +354,8 @@ def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, wri
                   align_or: int = 0, publish: Optional[PublishArgs] = None,
                   variant: str = "auto", layer: Optional[LayerState] = None,
                   claim: bool = False, release: Optional[GroupRelease] = None,
-                  rows: Optional[Sequence[int]] = None) -> None:
+                  rows: Optional[Sequence[int]] = None,
+                  pieces: Optional[torch.Tensor] = None) -> None:
     """Gathered fp8 blocks (``kv_gather`` with quantisation): part s of block i is a bf16 page
     of ``elems`` elements at ``part_base[s] + local offset`` and fp8 page first_part + s of
     the block, at byte ``fp8_gather_bytes(first_part + s, elems)``.  ``descs``, ``layer`` and
@@ -358,7 +371,8 @@ def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, wri
     too).  A write with ``rows`` quantises each stored page whose bf16 rows it loads from the
     strided local part, as ``kv_gather``'s row write does (kv_write_fp8_rows, whatever the
     variant); the rows must fill the stored part, and ``publish`` / ``layer`` / ``claim`` work
-    as without rows."""
+    as without rows.  ``pieces`` as for ``kv_gather`` (kv_read_fp8_pieces,
+    kv_write_fp8_pieces)."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
     bases = [int(b) for b in part_base]
     for b in bases:
@@ -370,7 +384,7 @@ def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, wri
                         max_ctas, _stream(descs.device), *pub,
                         status.data_ptr() if status is not None else 0, align_or, *lay,
                         *_release_args(release),
-                        [int(r) for r in rows] if rows is not None else [])
+                        [int(r) for r in rows] if rows is not None else [], *_piece_args(pieces))
 
 
 def fp8_reference(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
