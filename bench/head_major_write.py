@@ -28,10 +28,11 @@ checks them bit for bit against the token-major arm's, then purges the store.
 
 Kernels alone.  The page movers the store calls launch, on pre-allocated pool blocks with no
 allocation, lookup or publish: ops.kv_gather / ops.kv_gather_fp8 with rows= from the head-major
-pages (kv_gather_rows_write, kv_write_fp8_rows) against the same call without rows from the
-token-major pages (kv_gather_ldst; fp8: the ld/st kernel and the TMA pipeline), and the staging
-arm's torch permute-copy alone.  Events around --launches back-to-back launches per window,
-arms rotated every round as above; the pool bytes of the two writes are checked equal.
+pages (kv_gather_ldst<VEC, kRows>, kv_write_fp8_gather<SlicedRows>) against the same call
+without rows from the token-major pages (kv_gather_ldst<VEC, kWhole>; fp8: the ld/st kernel
+and the TMA pipeline), and the staging arm's torch permute-copy alone.  Events around
+--launches back-to-back launches per window, arms rotated every round as above; the pool
+bytes of the two writes are checked equal.
 
 Reported per arm: the median window over --reps rounds (per launch for kernels) with its
 minimum and maximum, and GB/s of stored bytes at the median.  Prints the card's name, power

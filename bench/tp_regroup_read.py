@@ -27,11 +27,11 @@ power limit and SM clock from the same run, then one JSON line.  Over NVLink (a 
 another GPU) the numbers may differ; that is not measured here.
 
 --fp8: the pages are written as fp8 (write_pages(fp8=True)) and every arm reads with fp8=True:
-rows is then the dequantising row-sliced read (kv_read_fp8_rows), staging a same-TP fp8 read
-per source rank and a torch copy of its heads, same_tp a same-TP fp8 read.  A head of 128
-elements is one scale group, so all three give the same bits; every round is checked against
-a same-TP fp8 read taken before the timed rounds.  Each arm also reports the pool bytes it
-reads (e4m3 payload and scales), from the shapes."""
+rows is then the dequantising row-sliced read (kv_read_fp8_scatter<LAYERED, kRows>), staging
+a same-TP fp8 read per source rank and a torch copy of its heads, same_tp a same-TP fp8 read.
+A head of 128 elements is one scale group, so all three give the same bits; every round is
+checked against a same-TP fp8 read taken before the timed rounds.  Each arm also reports the
+pool bytes it reads (e4m3 payload and scales), from the shapes."""
 from __future__ import annotations
 
 import argparse

@@ -28,6 +28,14 @@ LdStResident ldst_resident(K16* k16, K32* k32, int threads) {
     return r;
 }
 
+// ldst_resident of one pair of kernels, asked once per process.  A kernel with a single flavour
+// passes itself as both (r16 == r32).
+template <auto K16, auto K32, int THREADS>
+const LdStResident& cached_resident() {
+    static const LdStResident r = ldst_resident(K16, K32, THREADS);
+    return r;
+}
+
 // NVLS: one 16-byte store to a multicast address lands in every replica  (multimem.st)
 __device__ __forceinline__ void st_multicast_v4(void* mc, const uint4& v) {
     asm volatile("multimem.st.relaxed.sys.global.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(mc),

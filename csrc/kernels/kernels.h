@@ -212,8 +212,9 @@ struct GatherLaunch {
     uint32_t pieces = 1;
 };
 // The TMA pipeline for 16-byte aligned parts of at least kPipeMinBytes, the ld/st kernel
-// (kv_copy.cu) otherwise: the same rule launch_kv_copy applies to whole blocks.  A row-sliced
-// read runs kv_scatter_rows (kv_copy.cu), a row-sliced write kv_gather_rows_write.
+// (kv_copy.cu) otherwise: the same rule launch_kv_copy applies to whole blocks.  Reads run
+// kv_scatter_ldst and writes kv_gather_ldst, with one body per part shape (whole parts, rows,
+// slices, pieces) around the item walks of gather_items.cuh.
 cudaError_t launch_kv_gather(const GatherLaunch& a, cudaStream_t stream);
 cudaError_t launch_kv_pipe_gather(const GatherLaunch& a, cudaStream_t stream);
 struct GatherParts {

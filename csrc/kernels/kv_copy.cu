@@ -26,6 +26,7 @@
 #include "common.cuh"
 #include "kernels.h"
 #include "copy_span.cuh"
+#include "gather_items.cuh"
 #include "launch_plan.h"
 #include "publish.cuh"
 
@@ -88,434 +89,154 @@ __global__ void __launch_bounds__(kLdStThreads + 32)
 }
 
 // ---------------------------------------------------------------- gathered blocks (ld/st)
-// The layered read (GatherLaunch::group_flags): items numbered group-major
-// (launch_plan.h: layered_item), group g released by leave_group (publish.cuh) when this
-// CTA's stream leaves it.  A missing block counts once, on its first item (group 0, part 0,
-// chunk 0), and its parts are left untouched; its items still count as arrivals.
-template <int VEC>
-__device__ __forceinline__ void gather_read_layered(const CopyDesc* __restrict__ descs,
-                                                    const GatherParts& parts, uint32_t n,
-                                                    uint32_t nparts, uint32_t part_bytes,
-                                                    uint32_t first_part, uint32_t chunk,
-                                                    uint32_t cpp, uint32_t* status,
-                                                    const GroupRelease& rel) {
-    const uint32_t group_items = n * rel.gp * cpp;
-    const uint32_t total = n * nparts * cpp;
-    uint32_t item = blockIdx.x;
-    CopyDesc next = item < total ? descs[layered_item(item, n, rel.gp, cpp).block] : CopyDesc{0, 0};
-    for (; item < total; item += gridDim.x) {
-        const CopyDesc d = next;
-        const LayeredItem it = layered_item(item, n, rel.gp, cpp);
-        const uint32_t nxt = item + gridDim.x;
-        if (nxt < total) next = descs[layered_item(nxt, n, rel.gp, cpp).block];
-        if (d.src != 0) {
+// The launch's part geometry, every shape's fields in one kernel parameter (GatherLaunch):
+// each body reads the fields of its own shape.
+struct PartGeometry {
+    uint32_t part_bytes, rows, row_bytes, src_pitch, src_col, dst_pitch, slices, slice_pitch,
+        pieces;
+    const uint64_t* piece_off;
+};
+
+// Reads: gather_items.cuh's scatter_items walk, one body per part shape.  Item chunk c of part s
+// of block b copies, from pool desc.src + (first_part + s) * part_bytes to local
+// parts.base[s] + desc.dst:
+//   kWhole   bytes [c * chunk, +chunk) of the part (copy_span);
+//   kRows    rows [c * chunk, +chunk) (GatherLaunch::rows): row r from r * src_pitch + src_col
+//            (row_bytes) to r * dst_pitch (copy_rows);
+//   kSlices  (slice, row) pairs [c * chunk, +chunk) of the part (GatherLaunch::slices > 1),
+//            numbered slice-major, each placed by slice_pair (launch_plan.h: copy_rows<VEC, true>);
+//   kPieces  the same pairs (GatherLaunch::pieces > 1, any slices), cut where q / piece_rows
+//            changes; each cut, one slice's rows inside one piece, is copied as plain rows to
+//            desc.dst + piece_off[block * pieces + t] + the place piece_pair gives its first pair
+//            - one piece-offset load per cut.
+// No control warp: reads publish nothing.  The minimum of 3 CTAs per SM holds every flavour to
+// 80 registers, which the 32-byte row reads use.
+template <int VEC, bool LAYERED, PartShape S>
+__global__ void __launch_bounds__(kLdStThreads, 3)
+    kv_scatter_ldst_kernel(const CopyDesc* __restrict__ descs,
+                           const __grid_constant__ GatherParts parts, uint32_t n, uint32_t nparts,
+                           uint32_t first_part, uint32_t chunk, uint32_t cpp, PartGeometry g,
+                           uint32_t* status, GroupRelease rel) {
+    scatter_items<LAYERED>(descs, n, nparts, cpp, status, rel, [&](const CopyDesc& d,
+                                                                  const LayeredItem& it) {
+        const uint64_t src = d.src + uint64_t(first_part + it.part) * g.part_bytes;
+        const uint64_t dst = parts.base[it.part] + d.dst;
+        const auto at = [](uint64_t a) { return reinterpret_cast<uint8_t*>(a); };
+        if constexpr (S == PartShape::kWhole) {
             const uint32_t off = it.chunk * chunk;
-            const uint32_t len = min(chunk, part_bytes - off);
-            uint8_t* dst = reinterpret_cast<uint8_t*>(parts.base[it.part] + d.dst + off);
-            const uint8_t* src = reinterpret_cast<const uint8_t*>(
-                d.src + uint64_t(first_part + it.part) * part_bytes + off);
+            const uint32_t len = min(chunk, g.part_bytes - off);
             if constexpr (VEC == 1) {
-                for (uint32_t b = threadIdx.x; b < len; b += kLdStThreads) dst[b] = src[b];
+                for (uint32_t b = threadIdx.x; b < len; b += kLdStThreads)
+                    at(dst + off)[b] = at(src + off)[b];
             } else {
-                copy_span<VEC>(dst, src, len);
+                copy_span<VEC>(at(dst + off), at(src + off), len);
             }
-        } else if (threadIdx.x == 0 && item < group_items && item % (rel.gp * cpp) == 0 && status) {
-            atomicAdd(status + kStatMiss, 1u);
+        } else if constexpr (S == PartShape::kRows) {
+            const uint32_t r0 = it.chunk * chunk;
+            copy_rows<VEC>(at(dst + uint64_t(r0) * g.dst_pitch),
+                           at(src + uint64_t(r0) * g.src_pitch + g.src_col),
+                           min(chunk, g.rows - r0), g.row_bytes, g.src_pitch, g.dst_pitch);
+        } else if constexpr (S == PartShape::kSlices) {
+            const uint32_t q0 = it.chunk * chunk;
+            copy_rows<VEC, true>(at(dst), at(src), min(chunk, g.rows * g.slices - q0), g.row_bytes,
+                                 g.src_pitch, g.dst_pitch,
+                                 RowSlices{q0, g.rows, g.src_col, g.slice_pitch});
+        } else {
+            const uint32_t piece_rows = g.rows / g.pieces;
+            const uint32_t q0 = it.chunk * chunk, q1 = min(q0 + chunk, g.rows * g.slices);
+            const uint64_t* off = g.piece_off + uint64_t(it.block) * g.pieces;
+            for (uint32_t q = q0; q < q1;) {
+                const uint32_t e = min(q1, (q / piece_rows + 1) * piece_rows);
+                const PieceOffsets o = piece_pair(q, g.rows, g.row_bytes, g.src_pitch, g.src_col,
+                                                  g.dst_pitch, g.slice_pitch, piece_rows);
+                copy_rows<VEC>(at(dst + off[o.piece] + o.dst), at(src + o.src), e - q,
+                               g.row_bytes, g.src_pitch, g.dst_pitch);
+                q = e;
+            }
         }
-        if (nxt >= total || nxt / group_items != it.group) {
-            const uint32_t lo = it.group * group_items;
-            leave_group(rel, it.group, cta_items(lo, lo + group_items, blockIdx.x, gridDim.x),
-                        group_items, kLdStThreads);
-        }
-    }
+    });
 }
 
-// Item = chunk c of part s of block b, numbered (b * nparts + s) * cpp + c (GatherLaunch).
-// write: local parts.base[s] + desc.src -> pool desc.dst + (first_part + s) * part_bytes;
-// read:  pool desc.src + (first_part + s) * part_bytes -> local parts.base[s] + desc.dst.
-// LAYERED: a layered read (gather_read_layered above); no publish.
+// bf16 writes: gather_items.cuh's gather_items walk.  Item chunk c of part s of block b stores
+// bytes [off, off + len) of pool part first_part + s of desc.dst, each loaded from local
+// parts.base[s] + desc.src:
+//   kWhole   at the same offset (copy_span);
+//   kRows    at row_write_offset of its stored offset (GatherLaunch::rows with write, any
+//            slices: copy_span_rows), so every item still stores one contiguous run of pool
+//            bytes and the commit counts arrivals as for whole parts;
+//   kPieces  the same, with the item's stored bytes cut at piece boundaries (piece_rows *
+//            src_pitch bytes) and each cut loaded from desc.src + piece_off[block * pieces + t]
+//            (piece_write_offset's geometry) - one piece-offset load per cut.
 // The minimum of 3 CTAs per SM lets the 32-byte flavour keep 64 registers; without it ptxas
 // held it to 56 and spilled.
-template <int VEC, bool LAYERED = false>
+template <int VEC, PartShape S>
 __global__ void __launch_bounds__(kLdStThreads + 32, 3)
     kv_gather_ldst_kernel(const CopyDesc* __restrict__ descs,
                           const __grid_constant__ GatherParts parts, uint32_t n, uint32_t nparts,
-                          uint32_t part_bytes, uint32_t first_part, uint32_t chunk, uint32_t cpp,
-                          bool write, Publish pub, LayerCommit lc, GroupRelease rel) {
-    if constexpr (LAYERED) {
-        if (threadIdx.x >= kLdStThreads) return;
-        gather_read_layered<VEC>(descs, parts, n, nparts, part_bytes, first_part, chunk, cpp,
-                                 pub.status, rel);
-        return;
-    }
-    const uint32_t cpb = nparts * cpp;  // items per block: what the commit counter counts
-    const uint32_t total = n * cpb;
-    if (threadIdx.x >= kLdStThreads) {
-        if (!pub.recs) return;
-        const uint32_t count = blockIdx.x < total ? (total - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-        gather_control_warp(pub, lc, threadIdx.x - kLdStThreads, blockIdx.x, count, gridDim.x,
-                            cpb, nparts, kLdStThreads + 32);
-        return;
-    }
-    uint32_t item = blockIdx.x;
-    CopyDesc next = item < total ? descs[item / cpb] : CopyDesc{0, 0};
-    for (; item < total; item += gridDim.x) {
-        const CopyDesc d = next;
-        const uint32_t nxt = item + gridDim.x;
-        if (nxt < total) next = descs[nxt / cpb];  // prefetch: descriptors may sit in host memory
-        const uint32_t in_block = item % cpb;
-        if (!write && d.src == 0) {  // key not found: one miss per block, parts left untouched
-            if (threadIdx.x == 0 && in_block == 0 && pub.status) atomicAdd(pub.status + kStatMiss, 1u);
-            continue;
-        }
-        const uint32_t s = in_block / cpp;
-        const uint32_t off = (in_block % cpp) * chunk;
-        const uint32_t len = min(chunk, part_bytes - off);
-        const uint64_t local = parts.base[s] + (write ? d.src : d.dst) + off;
-        const uint64_t pool = (write ? d.dst : d.src) + uint64_t(first_part + s) * part_bytes + off;
-        uint8_t* dst = reinterpret_cast<uint8_t*>(write ? pool : local);
-        const uint8_t* src = reinterpret_cast<const uint8_t*>(write ? local : pool);
-        if constexpr (VEC == 1) {
-            for (uint32_t b = threadIdx.x; b < len; b += kLdStThreads) dst[b] = src[b];
-        } else {
-            copy_span<VEC>(dst, src, len);
-        }
-    }
-    if (pub.recs) ctrl_barrier_arrive(kLdStThreads + 32);
-}
-
-// ---------------------------------------------------------------- row-sliced reads (ld/st)
-struct RowGeometry {
-    uint32_t rows, row_bytes, src_pitch, src_col, dst_pitch, part_bytes;
-};
-
-// GatherLaunch::rows.  Item = run c (`run` rows) of part s of block b, numbered
-// (b * nparts + s) * cpp + c - which is layered_item's numbering with one group of all nparts
-// parts - or, LAYERED, group-major with rel.gp parts per group, each group released by
-// leave_group as in gather_read_layered.  Row r of the run:
-//   pool desc.src + (first_part + s) * part_bytes + r * src_pitch + src_col   (row_bytes)
-//     -> parts.base[s] + desc.dst + r * dst_pitch.
-// A missing block counts once, on its first item, and its parts are left untouched; its items
-// still count as arrivals.  No control warp: reads publish nothing.
-// SLICED (kv_scatter_slices_kernel, GatherLaunch::slices > 1): a run is `run` (slice, row)
-// pairs of the part, numbered slice-major, each placed by slice_pair (launch_plan.h).
-// PIECES (kv_scatter_pieces_kernel, GatherLaunch::pieces > 1, any slices): the same items; the
-// run's pairs are cut where q / piece_rows changes, and each cut, one slice's rows inside one
-// piece, is copied as plain rows to desc.dst + piece_off[block * pieces + t] + the place
-// piece_pair gives its first pair - one piece-offset load per cut.
-template <int VEC, bool LAYERED, bool SLICED, bool PIECES = false>
-__device__ __forceinline__ void scatter_rows(const CopyDesc* __restrict__ descs,
-                                             const GatherParts& parts, uint32_t n,
-                                             uint32_t nparts, uint32_t first_part,
-                                             const RowGeometry& geo, uint32_t slices,
-                                             uint32_t slice_pitch, uint32_t run, uint32_t cpp,
-                                             uint32_t* status, const GroupRelease& rel,
-                                             const uint64_t* piece_off = nullptr,
-                                             uint32_t pieces = 1) {
-    const uint32_t gp = LAYERED ? rel.gp : nparts;
-    const uint32_t group_items = n * gp * cpp;
-    const uint32_t total = n * nparts * cpp;
-    uint32_t item = blockIdx.x;
-    CopyDesc next = item < total ? descs[layered_item(item, n, gp, cpp).block] : CopyDesc{0, 0};
-    for (; item < total; item += gridDim.x) {
-        const CopyDesc d = next;
-        const LayeredItem it = layered_item(item, n, gp, cpp);
-        const uint32_t nxt = item + gridDim.x;
-        if (nxt < total) next = descs[layered_item(nxt, n, gp, cpp).block];
-        if (d.src != 0 && PIECES) {
-            const uint32_t piece_rows = geo.rows / pieces;
-            const uint32_t q0 = it.chunk * run, q1 = min(q0 + run, geo.rows * slices);
-            const uint8_t* src = reinterpret_cast<const uint8_t*>(
-                d.src + uint64_t(first_part + it.part) * geo.part_bytes);
-            const uint64_t* off = piece_off + uint64_t(it.block) * pieces;
-            for (uint32_t q = q0; q < q1;) {
-                const uint32_t e = min(q1, (q / piece_rows + 1) * piece_rows);
-                const PieceOffsets o = piece_pair(q, geo.rows, geo.row_bytes, geo.src_pitch,
-                                                  geo.src_col, geo.dst_pitch, slice_pitch,
-                                                  piece_rows);
-                copy_rows<VEC>(
-                    reinterpret_cast<uint8_t*>(parts.base[it.part] + d.dst + off[o.piece] + o.dst),
-                    src + o.src, e - q, geo.row_bytes, geo.src_pitch, geo.dst_pitch);
-                q = e;
+                          uint32_t first_part, uint32_t chunk, uint32_t cpp, PartGeometry g,
+                          Publish pub, LayerCommit lc) {
+    gather_items(descs, n, nparts, g.part_bytes, chunk, cpp, pub, lc, [&](const CopyDesc& d,
+                                                                        uint32_t block,
+                                                                        uint32_t s, uint32_t off,
+                                                                        uint32_t len) {
+        uint8_t* dst =
+            reinterpret_cast<uint8_t*>(d.dst + uint64_t(first_part + s) * g.part_bytes + off);
+        const uint64_t src = parts.base[s] + d.src;
+        const auto at = [](uint64_t a) { return reinterpret_cast<const uint8_t*>(a); };
+        const RowWrite w{g.row_bytes, g.src_pitch, g.dst_pitch, g.slice_pitch};
+        if constexpr (S == PartShape::kWhole) {
+            if constexpr (VEC == 1) {
+                for (uint32_t b = threadIdx.x; b < len; b += kLdStThreads)
+                    dst[b] = at(src + off)[b];
+            } else {
+                copy_span<VEC>(dst, at(src + off), len);
             }
-        } else if (d.src != 0 && SLICED) {
-            const uint32_t q0 = it.chunk * run;
-            const uint8_t* src = reinterpret_cast<const uint8_t*>(
-                d.src + uint64_t(first_part + it.part) * geo.part_bytes);
-            uint8_t* dst = reinterpret_cast<uint8_t*>(parts.base[it.part] + d.dst);
-            copy_rows<VEC, true>(dst, src, min(run, geo.rows * slices - q0), geo.row_bytes,
-                                 geo.src_pitch, geo.dst_pitch,
-                                 RowSlices{q0, geo.rows, geo.src_col, slice_pitch});
-        } else if (d.src != 0) {
-            const uint32_t r0 = it.chunk * run;
-            const uint8_t* src = reinterpret_cast<const uint8_t*>(
-                d.src + uint64_t(first_part + it.part) * geo.part_bytes +
-                uint64_t(r0) * geo.src_pitch + geo.src_col);
-            uint8_t* dst = reinterpret_cast<uint8_t*>(parts.base[it.part] + d.dst +
-                                                      uint64_t(r0) * geo.dst_pitch);
-            copy_rows<VEC>(dst, src, min(run, geo.rows - r0), geo.row_bytes, geo.src_pitch,
-                           geo.dst_pitch);
-        } else if (threadIdx.x == 0 && item < group_items && item % (gp * cpp) == 0 && status) {
-            atomicAdd(status + kStatMiss, 1u);
-        }
-        if constexpr (LAYERED) {
-            if (nxt >= total || nxt / group_items != it.group) {
-                const uint32_t lo = it.group * group_items;
-                leave_group(rel, it.group, cta_items(lo, lo + group_items, blockIdx.x, gridDim.x),
-                            group_items, kLdStThreads);
-            }
-        }
-    }
-}
-
-template <int VEC, bool LAYERED>
-__global__ void __launch_bounds__(kLdStThreads, 3)
-    kv_scatter_rows_kernel(const CopyDesc* __restrict__ descs,
-                           const __grid_constant__ GatherParts parts, uint32_t n, uint32_t nparts,
-                           uint32_t first_part, RowGeometry geo, uint32_t run, uint32_t cpp,
-                           uint32_t* status, GroupRelease rel) {
-    scatter_rows<VEC, LAYERED, false>(descs, parts, n, nparts, first_part, geo, 1, 0, run, cpp,
-                                      status, rel);
-}
-
-// GatherLaunch::slices > 1: runs of (slice, row) pairs (scatter_rows above).
-template <int VEC, bool LAYERED>
-__global__ void __launch_bounds__(kLdStThreads, 3)
-    kv_scatter_slices_kernel(const CopyDesc* __restrict__ descs,
-                             const __grid_constant__ GatherParts parts, uint32_t n,
-                             uint32_t nparts, uint32_t first_part, RowGeometry geo,
-                             uint32_t slices, uint32_t slice_pitch, uint32_t run, uint32_t cpp,
-                             uint32_t* status, GroupRelease rel) {
-    scatter_rows<VEC, LAYERED, true>(descs, parts, n, nparts, first_part, geo, slices,
-                                     slice_pitch, run, cpp, status, rel);
-}
-
-// GatherLaunch::pieces > 1, one or more slices: runs cut at piece boundaries (scatter_rows).
-template <int VEC, bool LAYERED>
-__global__ void __launch_bounds__(kLdStThreads, 3)
-    kv_scatter_pieces_kernel(const CopyDesc* __restrict__ descs,
-                             const __grid_constant__ GatherParts parts, uint32_t n,
-                             uint32_t nparts, uint32_t first_part, RowGeometry geo,
-                             uint32_t slices, uint32_t slice_pitch, uint32_t run, uint32_t cpp,
-                             uint32_t* status, GroupRelease rel, const uint64_t* piece_off,
-                             uint32_t pieces) {
-    scatter_rows<VEC, LAYERED, false, true>(descs, parts, n, nparts, first_part, geo, slices,
-                                            slice_pitch, run, cpp, status, rel, piece_off,
-                                            pieces);
-}
-
-cudaError_t launch_kv_scatter_pieces(const GatherLaunch& a, const LaunchPlan& p,
-                                     const GatherParts& parts, const RowGeometry& geo,
-                                     const GroupRelease& rel, cudaStream_t stream) {
-    const bool layered = a.group_flags != nullptr;
-    const auto go = [&](auto* kernel) {
-        kernel<<<p.ctas, kLdStThreads, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.first_part,
-                                                    geo, a.slices, a.dst_slice_pitch, p.chunk,
-                                                    p.cpb, a.status, rel, a.piece_off, a.pieces);
-        return cudaGetLastError();
-    };
-    switch (p.kernel) {
-        case Kernel::kLdSt1:
-            return layered ? go(kv_scatter_pieces_kernel<1, true>)
-                           : go(kv_scatter_pieces_kernel<1, false>);
-        case Kernel::kLdSt32:
-            return layered ? go(kv_scatter_pieces_kernel<32, true>)
-                           : go(kv_scatter_pieces_kernel<32, false>);
-        default:
-            return layered ? go(kv_scatter_pieces_kernel<16, true>)
-                           : go(kv_scatter_pieces_kernel<16, false>);
-    }
-}
-
-cudaError_t launch_kv_scatter_slices(const GatherLaunch& a, const LaunchPlan& p,
-                                     const GatherParts& parts, const RowGeometry& geo,
-                                     const GroupRelease& rel, cudaStream_t stream) {
-    const bool layered = a.group_flags != nullptr;
-    const auto go = [&](auto* kernel) {
-        kernel<<<p.ctas, kLdStThreads, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.first_part,
-                                                    geo, a.slices, a.dst_slice_pitch, p.chunk,
-                                                    p.cpb, a.status, rel);
-        return cudaGetLastError();
-    };
-    switch (p.kernel) {
-        case Kernel::kLdSt1:
-            return layered ? go(kv_scatter_slices_kernel<1, true>)
-                           : go(kv_scatter_slices_kernel<1, false>);
-        case Kernel::kLdSt32:
-            return layered ? go(kv_scatter_slices_kernel<32, true>)
-                           : go(kv_scatter_slices_kernel<32, false>);
-        default:
-            return layered ? go(kv_scatter_slices_kernel<16, true>)
-                           : go(kv_scatter_slices_kernel<16, false>);
-    }
-}
-
-cudaError_t launch_kv_scatter_rows(const GatherLaunch& a, cudaStream_t stream) {
-    static const LdStResident res = ldst_resident(kv_scatter_rows_kernel<16, false>,
-                                                  kv_scatter_rows_kernel<32, false>, kLdStThreads);
-    static const LdStResident res_layered = ldst_resident(
-        kv_scatter_rows_kernel<16, true>, kv_scatter_rows_kernel<32, true>, kLdStThreads);
-    static const LdStResident res_sliced = ldst_resident(
-        kv_scatter_slices_kernel<16, false>, kv_scatter_slices_kernel<32, false>, kLdStThreads);
-    static const LdStResident res_sliced_layered = ldst_resident(
-        kv_scatter_slices_kernel<16, true>, kv_scatter_slices_kernel<32, true>, kLdStThreads);
-    static const LdStResident res_pieces = ldst_resident(
-        kv_scatter_pieces_kernel<16, false>, kv_scatter_pieces_kernel<32, false>, kLdStThreads);
-    static const LdStResident res_pieces_layered = ldst_resident(
-        kv_scatter_pieces_kernel<16, true>, kv_scatter_pieces_kernel<32, true>, kLdStThreads);
-    const bool layered = a.group_flags != nullptr;
-    const bool sliced = a.slices > 1;
-    const bool pieced = a.pieces > 1;
-    if (pieced && !a.piece_off) return cudaErrorInvalidValue;
-    const LaunchPlan p = plan_gather_rows(a, sm_count(),
-                                          pieced   ? (layered ? res_pieces_layered : res_pieces)
-                                          : sliced ? (layered ? res_sliced_layered : res_sliced)
-                                          : layered ? res_layered
-                                                    : res);
-    if (!p.valid) return cudaErrorInvalidValue;  // the caller checks the geometry and splits
-    GatherParts parts;
-    std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
-    const RowGeometry geo{a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.part_bytes};
-    const GroupRelease rel{a.group_flags, a.group_counters, a.group_seq, a.group_parts};
-    if (pieced) return launch_kv_scatter_pieces(a, p, parts, geo, rel, stream);
-    if (sliced) return launch_kv_scatter_slices(a, p, parts, geo, rel, stream);
-    const auto go = [&](auto* kernel) {
-        kernel<<<p.ctas, kLdStThreads, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.first_part,
-                                                    geo, p.chunk, p.cpb, a.status, rel);
-        return cudaGetLastError();
-    };
-    switch (p.kernel) {
-        case Kernel::kLdSt1:
-            return layered ? go(kv_scatter_rows_kernel<1, true>) : go(kv_scatter_rows_kernel<1, false>);
-        case Kernel::kLdSt32:
-            return layered ? go(kv_scatter_rows_kernel<32, true>)
-                           : go(kv_scatter_rows_kernel<32, false>);
-        default:
-            return layered ? go(kv_scatter_rows_kernel<16, true>)
-                           : go(kv_scatter_rows_kernel<16, false>);
-    }
-}
-
-// ---------------------------------------------------------------- row-sliced writes (ld/st)
-// GatherLaunch::rows with write: kv_gather_ldst_kernel's items, (block, part, chunk of the
-// stored part) numbered (b * nparts + s) * cpp + c, each storing one contiguous run of pool
-// bytes, so the control warp (publish, or a layered writer's LayerCommit) counts arrivals
-// exactly as for kv_gather_ldst.  Only the local load address differs: stored byte o of part
-// s comes from parts.base[s] + desc.src + row_write_offset(o) (copy_span_rows).
-// PIECES (kv_gather_pieces_write_kernel, GatherLaunch::pieces > 1): the item's stored bytes are
-// cut at piece boundaries (piece_rows * src_pitch bytes), and each cut is loaded from
-// parts.base[s] + desc.src + piece_off[block * pieces + t] (piece_write_offset's geometry) -
-// one piece-offset load per cut.
-template <int VEC, bool PIECES>
-__device__ __forceinline__ void gather_rows_write(const CopyDesc* __restrict__ descs,
-                                                  const GatherParts& parts, uint32_t n,
-                                                  uint32_t nparts, uint32_t part_bytes,
-                                                  uint32_t first_part, uint32_t chunk, uint32_t cpp,
-                                                  const RowWrite& geo, const Publish& pub,
-                                                  const LayerCommit& lc,
-                                                  const uint64_t* piece_off = nullptr,
-                                                  uint32_t pieces = 1) {
-    const uint32_t cpb = nparts * cpp;  // items per block: what the commit counter counts
-    const uint32_t total = n * cpb;
-    if (threadIdx.x >= kLdStThreads) {
-        if (!pub.recs) return;
-        const uint32_t count = blockIdx.x < total ? (total - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-        gather_control_warp(pub, lc, threadIdx.x - kLdStThreads, blockIdx.x, count, gridDim.x,
-                            cpb, nparts, kLdStThreads + 32);
-        return;
-    }
-    uint32_t item = blockIdx.x;
-    CopyDesc next = item < total ? descs[item / cpb] : CopyDesc{0, 0};
-    for (; item < total; item += gridDim.x) {
-        const CopyDesc d = next;
-        const uint32_t nxt = item + gridDim.x;
-        if (nxt < total) next = descs[nxt / cpb];  // prefetch: descriptors may sit in host memory
-        const uint32_t in_block = item % cpb;
-        const uint32_t s = in_block / cpp;
-        const uint32_t off = (in_block % cpp) * chunk;
-        const uint32_t len = min(chunk, part_bytes - off);
-        if constexpr (!PIECES) {
-            const uint8_t* src = reinterpret_cast<const uint8_t*>(parts.base[s] + d.src);
-            uint8_t* dst =
-                reinterpret_cast<uint8_t*>(d.dst + uint64_t(first_part + s) * part_bytes + off);
-            copy_span_rows<VEC>(dst, src, off, len, geo);
+        } else if constexpr (S == PartShape::kRows) {
+            copy_span_rows<VEC>(dst, at(src), off, len, w);
         } else {
-            uint8_t* dst =
-                reinterpret_cast<uint8_t*>(d.dst + uint64_t(first_part + s) * part_bytes + off);
-            const uint32_t piece_bytes = part_bytes / pieces;
-            const uint64_t* poff = piece_off + uint64_t(item / cpb) * pieces;
+            const uint32_t piece_bytes = g.part_bytes / g.pieces;
+            const uint64_t* poff = g.piece_off + uint64_t(block) * g.pieces;
             for (uint32_t o = off; o < off + len;) {
                 const uint32_t t = o / piece_bytes;
                 const uint32_t e = min(off + len, (t + 1) * piece_bytes);
-                copy_span_rows<VEC>(
-                    dst + (o - off), reinterpret_cast<const uint8_t*>(parts.base[s] + d.src + poff[t]),
-                    o - t * piece_bytes, e - o, geo);
+                copy_span_rows<VEC>(dst + (o - off), at(src + poff[t]), o - t * piece_bytes,
+                                    e - o, w);
                 o = e;
             }
         }
-    }
-    if (pub.recs) ctrl_barrier_arrive(kLdStThreads + 32);
+    });
 }
 
-template <int VEC>
-__global__ void __launch_bounds__(kLdStThreads + 32, 3)
-    kv_gather_rows_write_kernel(const CopyDesc* __restrict__ descs,
-                                const __grid_constant__ GatherParts parts, uint32_t n,
-                                uint32_t nparts, uint32_t part_bytes, uint32_t first_part,
-                                uint32_t chunk, uint32_t cpp, RowWrite geo, Publish pub,
-                                LayerCommit lc) {
-    gather_rows_write<VEC, false>(descs, parts, n, nparts, part_bytes, first_part, chunk, cpp,
-                                  geo, pub, lc);
-}
-
-template <int VEC>
-__global__ void __launch_bounds__(kLdStThreads + 32, 3)
-    kv_gather_pieces_write_kernel(const CopyDesc* __restrict__ descs,
-                                  const __grid_constant__ GatherParts parts, uint32_t n,
-                                  uint32_t nparts, uint32_t part_bytes, uint32_t first_part,
-                                  uint32_t chunk, uint32_t cpp, RowWrite geo, Publish pub,
-                                  LayerCommit lc, const uint64_t* piece_off, uint32_t pieces) {
-    gather_rows_write<VEC, true>(descs, parts, n, nparts, part_bytes, first_part, chunk, cpp, geo,
-                                 pub, lc, piece_off, pieces);
-}
-
-cudaError_t launch_kv_gather_rows_write(const GatherLaunch& a, cudaStream_t stream) {
-    constexpr int T = kLdStThreads + 32;
-    static const LdStResident res =
-        ldst_resident(kv_gather_rows_write_kernel<16>, kv_gather_rows_write_kernel<32>, T);
-    static const LdStResident res_pieces =
-        ldst_resident(kv_gather_pieces_write_kernel<16>, kv_gather_pieces_write_kernel<32>, T);
-    const bool pieced = a.pieces > 1;
-    if (pieced && !a.piece_off) return cudaErrorInvalidValue;
-    const LaunchPlan p = plan_gather_rows_write(a, sm_count(), pieced ? res_pieces : res);
+// One launch of a gathered ld/st kernel: the plan for its shape and direction, then the plan's
+// vector width.  The residency is the launched kernel's own; whole parts take the TMA
+// pipeline where plan_gather says so.
+template <bool WRITE, bool LAYERED, PartShape S>
+cudaError_t launch_ldst_gather(const GatherLaunch& a, const GatherParts& parts,
+                               const PartGeometry& g, cudaStream_t stream) {
+    constexpr int T = WRITE ? kLdStThreads + 32 : kLdStThreads;
+    const LdStResident* res;
+    if constexpr (WRITE)
+        res = &cached_resident<kv_gather_ldst_kernel<16, S>, kv_gather_ldst_kernel<32, S>, T>();
+    else
+        res = &cached_resident<kv_scatter_ldst_kernel<16, LAYERED, S>,
+                               kv_scatter_ldst_kernel<32, LAYERED, S>, T>();
+    const LaunchPlan p = S == PartShape::kWhole ? plan_gather(a, sm_count(), *res)
+                         : WRITE                ? plan_gather_rows_write(a, sm_count(), *res)
+                                                : plan_gather_rows(a, sm_count(), *res);
     if (!p.valid) return cudaErrorInvalidValue;  // the caller checks the geometry and splits
-    GatherParts parts;
-    std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
-    const RowWrite geo{a.row_bytes, a.src_pitch, a.dst_pitch, a.dst_slice_pitch};
-    if (pieced) {
-        const auto go = [&](auto* kernel) {
-            kernel<<<p.ctas, T, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.part_bytes,
-                                             a.first_part, p.chunk, p.cpb, geo, publish_of(a, true),
-                                             layer_of(a), a.piece_off, a.pieces);
-            return cudaGetLastError();
-        };
-        return p.kernel == Kernel::kLdSt1    ? go(kv_gather_pieces_write_kernel<1>)
-               : p.kernel == Kernel::kLdSt32 ? go(kv_gather_pieces_write_kernel<32>)
-                                             : go(kv_gather_pieces_write_kernel<16>);
-    }
-    const auto go = [&](auto* kernel) {
-        kernel<<<p.ctas, T, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.part_bytes, a.first_part,
-                                         p.chunk, p.cpb, geo, publish_of(a, true), layer_of(a));
+    if (p.kernel == Kernel::kTma) return launch_kv_pipe_gather(a, stream);
+    return with_vec(p.kernel, [&](auto vec) {
+        constexpr int V = decltype(vec)::value;
+        if constexpr (WRITE)
+            kv_gather_ldst_kernel<V, S><<<p.ctas, T, 0, stream>>>(
+                a.descs, parts, a.n, a.nparts, a.first_part, p.chunk, p.cpb, g,
+                publish_of(a, true), layer_of(a));
+        else
+            kv_scatter_ldst_kernel<V, LAYERED, S><<<p.ctas, T, 0, stream>>>(
+                a.descs, parts, a.n, a.nparts, a.first_part, p.chunk, p.cpb, g, a.status,
+                release_of(a));
         return cudaGetLastError();
-    };
-    switch (p.kernel) {
-        case Kernel::kLdSt1:
-            return go(kv_gather_rows_write_kernel<1>);
-        case Kernel::kLdSt32:
-            return go(kv_gather_rows_write_kernel<32>);
-        default:
-            return go(kv_gather_rows_write_kernel<16>);
-    }
+    });
 }
 
 }  // namespace
@@ -585,35 +306,19 @@ cudaError_t launch_kv_gather(const GatherLaunch& a, cudaStream_t stream) {
     if (uint64_t(a.nparts) * a.part_bytes > 0xffffffffull) return cudaErrorInvalidValue;
     const bool layered = a.group_flags != nullptr;
     if (layered && !a.group_counters) return cudaErrorInvalidValue;
-    if (a.rows)
-        return a.write ? launch_kv_gather_rows_write(a, stream) : launch_kv_scatter_rows(a, stream);
-    if (a.pieces != 1) return cudaErrorInvalidValue;  // pieces split rows
-    constexpr int T = kLdStThreads + 32;
-    static const LdStResident res =
-        ldst_resident(kv_gather_ldst_kernel<16>, kv_gather_ldst_kernel<32>, T);
-    static const LdStResident res_layered =
-        ldst_resident(kv_gather_ldst_kernel<16, true>, kv_gather_ldst_kernel<32, true>, T);
-    const LaunchPlan p = layered ? plan_gather_layered(a, sm_count(), res_layered)
-                                 : plan_gather(a, sm_count(), res);
-    if (!p.valid) return cudaErrorInvalidValue;  // the caller splits the batch
-    if (p.kernel == Kernel::kTma) return launch_kv_pipe_gather(a, stream);
-    GatherParts parts;
-    std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
-    const GroupRelease rel{a.group_flags, a.group_counters, a.group_seq, a.group_parts};
-    const auto go = [&](auto* kernel) {
-        kernel<<<p.ctas, T, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.part_bytes, a.first_part,
-                                         p.chunk, p.cpb, a.write, publish_of(a, a.write),
-                                         layer_of(a), rel);
-        return cudaGetLastError();
-    };
-    switch (p.kernel) {
-        case Kernel::kLdSt1:
-            return layered ? go(kv_gather_ldst_kernel<1, true>) : go(kv_gather_ldst_kernel<1>);
-        case Kernel::kLdSt32:
-            return layered ? go(kv_gather_ldst_kernel<32, true>) : go(kv_gather_ldst_kernel<32>);
-        default:
-            return layered ? go(kv_gather_ldst_kernel<16, true>) : go(kv_gather_ldst_kernel<16>);
-    }
+    // pieces split rows, at the offsets of the piece table
+    if (a.pieces != 1 && (!a.rows || !a.piece_off)) return cudaErrorInvalidValue;
+    const GatherParts parts = parts_of(a);
+    const PartGeometry g{a.part_bytes, a.rows,  a.row_bytes,       a.src_pitch, a.src_col,
+                         a.dst_pitch,  a.slices, a.dst_slice_pitch, a.pieces,    a.piece_off};
+    if (a.write)
+        return with_shape<true>(a, [&](auto s) {
+            return launch_ldst_gather<true, false, decltype(s)::value>(a, parts, g, stream);
+        });
+    return with_shape<false>(a, [&](auto s) {
+        return layered ? launch_ldst_gather<false, true, decltype(s)::value>(a, parts, g, stream)
+                       : launch_ldst_gather<false, false, decltype(s)::value>(a, parts, g, stream);
+    });
 }
 
 // Resolved once per process, as fabric/nvls.cpp resolves its driver entry points.

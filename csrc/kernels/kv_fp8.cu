@@ -8,13 +8,13 @@
 //                  no separate cast kernel / staging buffer.
 //   kv_read_fp8  : pool block -> dequantised bf16 scattered into the destination pages.
 //   kv_write_fp8_gather / kv_read_fp8_scatter : the same for gathered blocks, whose parts are
-//                  fp8 pages end to end (launch_kv_gather_fp8, fp8_pages.cuh).
-//   kv_read_fp8_rows / _slices, kv_write_fp8_rows : the gathered forms with row geometry
-//                  (GatherLaunch::rows): a read dequantises rows (and slices) of each stored
-//                  page, a write quantises a stored page whose rows are loaded from a strided
-//                  local layout (e.g. a head-major page).
-//   kv_read_fp8_pieces, kv_write_fp8_pieces : the same with GatherLaunch::pieces > 1, each
-//                  block's rows in runs at the offsets of its row of the piece table.
+//                  fp8 pages end to end (launch_kv_gather_fp8, fp8_pages.cuh), in every part
+//                  shape.  With row geometry (GatherLaunch::rows) a read dequantises rows (and
+//                  slices) of each stored page, a write quantises a stored page whose rows are
+//                  loaded from a strided local layout (e.g. a head-major page); with
+//                  GatherLaunch::pieces > 1 each block's rows are in runs at the offsets of its
+//                  row of the piece table.  Reads walk their items in gather_items.cuh
+//                  (scatter_items), writes in write_fp8 below.
 // The reference moves raw bytes only (dtype-agnostic, infinistore/lib.py:377-379); this is
 // the "write fused with fp8 cast / read fused with gather" item of the north star.
 //
@@ -27,11 +27,10 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
-#include <cstring>
-
 #include "common.cuh"
 #include "fp8_pages.cuh"
 #include "fp8_row.cuh"
+#include "gather_items.cuh"
 #include "kernels.h"
 #include "launch_plan.h"
 #include "publish.cuh"
@@ -71,7 +70,7 @@ __device__ __forceinline__ uint4 ld_u4(const void* p) {
 // Where a lane's 16-byte bf16 load comes from: byte offset from the page's local address of
 // elements 8 * hl .. 8 * hl + 7 of 128-element row `row` of the stored page.  A template
 // policy rather than a runtime branch, so the existing kernels' loop is compiled as before.
-//   DenseRows  the page is contiguous bf16 (every kernel but kv_write_fp8_rows).
+//   DenseRows  the page is contiguous bf16 (kv_write_fp8 and whole gathered parts).
 //   SlicedRows a row-sliced write (GatherLaunch::rows): row_write_offset (launch_plan.h) of the
 //              vector's byte in the part's bf16 view; the geometry is in multiples of 16 bytes,
 //              so the 8 elements never straddle two slices.
@@ -222,154 +221,30 @@ __global__ void __launch_bounds__(kThreads)
     }
 }
 
-// Gathered blocks (launch_kv_gather_fp8): n blocks of nparts parts, cpp items per part; the
-// part bases travel in the kernel parameters, as for kv_gather_ldst.
+// Gathered writes (launch_kv_gather_fp8): n blocks of nparts parts, cpp items per part, the
+// part bases in the kernel parameters; write_fp8's items and commit (BlockParts<true>), each
+// lane's bf16 vector placed by `load_at`: DenseRows for whole parts, SlicedRows with
+// GatherLaunch::rows, PiecedRows with GatherLaunch::pieces > 1.
+template <typename LoadAt>
 __global__ void __launch_bounds__(kThreads + 32)
     kv_write_fp8_gather_kernel(const CopyDesc* __restrict__ descs,
                                const __grid_constant__ GatherParts parts, uint32_t n,
                                uint32_t nparts, uint32_t elems, uint32_t chunk, uint32_t cpp,
-                               uint32_t first_part, uint64_t stride, Publish pub,
+                               uint32_t first_part, uint64_t stride, LoadAt load_at, Publish pub,
                                LayerCommit lc) {
     write_fp8(descs, n, elems, chunk, cpp, pub,
-              BlockParts<true>{&parts, nparts, first_part, stride, lc});
+              BlockParts<true>{&parts, nparts, first_part, stride, lc}, load_at);
 }
 
-// GatherLaunch::rows with write: kv_write_fp8_gather_kernel's items and commit
-// (BlockParts<true>), each lane's bf16 vector loaded from its row_write_offset in the part.
-__global__ void __launch_bounds__(kThreads + 32)
-    kv_write_fp8_rows_kernel(const CopyDesc* __restrict__ descs,
-                             const __grid_constant__ GatherParts parts, uint32_t n,
-                             uint32_t nparts, uint32_t elems, uint32_t chunk, uint32_t cpp,
-                             uint32_t first_part, uint64_t stride, SlicedRows geo, Publish pub,
-                             LayerCommit lc) {
-    write_fp8(descs, n, elems, chunk, cpp, pub,
-              BlockParts<true>{&parts, nparts, first_part, stride, lc}, geo);
-}
-
-// GatherLaunch::pieces > 1: kv_write_fp8_rows_kernel with each vector loaded from its piece.
-__global__ void __launch_bounds__(kThreads + 32)
-    kv_write_fp8_pieces_kernel(const CopyDesc* __restrict__ descs,
-                               const __grid_constant__ GatherParts parts, uint32_t n,
-                               uint32_t nparts, uint32_t elems, uint32_t chunk, uint32_t cpp,
-                               uint32_t first_part, uint64_t stride, PiecedRows geo, Publish pub,
-                               LayerCommit lc) {
-    write_fp8(descs, n, elems, chunk, cpp, pub,
-              BlockParts<true>{&parts, nparts, first_part, stride, lc}, geo);
-}
-
-// The layered read (GatherLaunch::group_flags): kv_gather_ldst's gather_read_layered
-// (kv_copy.cu) over fp8 pages.  Item order, miss counting and the group release are the same;
-// the rows of an item are dequantised as in kv_read_fp8_scatter_kernel.
-__device__ __forceinline__ void read_fp8_layered(const CopyDesc* __restrict__ descs,
-                                                 const BlockParts<false>& pages, uint32_t n,
-                                                 uint32_t elems, uint32_t chunk, uint32_t cpp,
-                                                 uint32_t* status, const GroupRelease& rel) {
-    const uint32_t group_items = n * rel.gp * cpp;
-    const uint32_t total = n * pages.nparts * cpp;
-    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t half = lane >> 4, hl = lane & 15;
-    constexpr uint32_t kStep = 2 * kRowPairs;
-    for (uint32_t item = blockIdx.x; item < total; item += gridDim.x) {
-        const LayeredItem it = layered_item(item, n, rel.gp, cpp);
-        const CopyDesc d = pages.at(descs, it.block * pages.nparts + it.part);
-        if (d.src != 0) {
-            const uint32_t e0 = it.chunk * chunk;
-            const uint32_t rows = min(chunk, elems - e0) / kRow;
-            const uint32_t row0 = e0 / kRow;
-            const uint8_t* q = reinterpret_cast<const uint8_t*>(d.src);
-            const float* scales = reinterpret_cast<const float*>(q + elems);
-            uint8_t* dst = reinterpret_cast<uint8_t*>(d.dst);
-            for (uint32_t r0 = warp * kStep; r0 < rows; r0 += kWarps * kStep) {
-                uint2 v[kRowPairs];
-                float sc[kRowPairs];
-#pragma unroll
-                for (int u = 0; u < kRowPairs; ++u) {
-                    const uint32_t r = r0 + 2 * u + half;
-                    if (r < rows) {
-                        v[u] = ld_u2(q + size_t(row0 + r) * kRow + hl * 8);
-                        sc[u] = __uint_as_float(ld_u1(scales + row0 + r));
-                    }
-                }
-#pragma unroll
-                for (int u = 0; u < kRowPairs; ++u) {
-                    const uint32_t r = r0 + 2 * u + half;
-                    if (r >= rows) continue;
-                    *reinterpret_cast<uint4*>(dst + (size_t(row0 + r) * kRow + hl * 8) * 2) =
-                        dequant8(v[u], sc[u]);
-                }
-            }
-        } else if (threadIdx.x == 0 && item < group_items && item % (rel.gp * cpp) == 0 && status) {
-            atomicAdd(status + kStatMiss, 1u);
-        }
-        const uint32_t nxt = item + gridDim.x;
-        if (nxt >= total || nxt / group_items != it.group) {
-            const uint32_t lo = it.group * group_items;
-            leave_group(rel, it.group, cta_items(lo, lo + group_items, blockIdx.x, gridDim.x),
-                        group_items, kThreads);
-        }
-    }
-}
-
-// The same loop as kv_read_fp8_kernel over the parts of gathered blocks.  A missing block
-// counts once, on its first part's first item; none of its parts is written.  (The two kernels
-// share the row maths, not the loop: inlining one loop body into both changed how the
-// compiler schedules kv_read_fp8_kernel.)  LAYERED: a layered read (read_fp8_layered above).
-template <bool LAYERED = false>
-__global__ void __launch_bounds__(kThreads)
-    kv_read_fp8_scatter_kernel(const CopyDesc* __restrict__ descs,
-                               const __grid_constant__ GatherParts parts, uint32_t n,
-                               uint32_t nparts, uint32_t first_part, uint32_t elems,
-                               uint32_t chunk, uint32_t cpp, uint64_t stride, uint32_t* status,
-                               GroupRelease rel) {
-    const BlockParts<false> pages{&parts, nparts, first_part, stride};
-    if constexpr (LAYERED) {
-        read_fp8_layered(descs, pages, n, elems, chunk, cpp, status, rel);
-        return;
-    }
-    const uint32_t total = n * nparts * cpp;
-    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t half = lane >> 4, hl = lane & 15;
-    constexpr uint32_t kStep = 2 * kRowPairs;
-    for (uint32_t item = blockIdx.x; item < total; item += gridDim.x) {
-        const CopyDesc d = pages.at(descs, item / cpp);
-        if (d.src == 0) {
-            if (threadIdx.x == 0 && pages.head(item / cpp) && item % cpp == 0 && status) atomicAdd(status + kStatMiss, 1u);
-            continue;
-        }
-        const uint32_t e0 = (item % cpp) * chunk;
-        const uint32_t rows = min(chunk, elems - e0) / kRow;
-        const uint32_t row0 = e0 / kRow;
-        const uint8_t* q = reinterpret_cast<const uint8_t*>(d.src);
-        const float* scales = reinterpret_cast<const float*>(q + elems);
-        uint8_t* dst = reinterpret_cast<uint8_t*>(d.dst);
-        for (uint32_t r0 = warp * kStep; r0 < rows; r0 += kWarps * kStep) {
-            uint2 v[kRowPairs];
-            float sc[kRowPairs];
-#pragma unroll
-            for (int u = 0; u < kRowPairs; ++u) {
-                const uint32_t r = r0 + 2 * u + half;
-                if (r < rows) {
-                    v[u] = ld_u2(q + size_t(row0 + r) * kRow + hl * 8);
-                    sc[u] = __uint_as_float(ld_u1(scales + row0 + r));
-                }
-            }
-#pragma unroll
-            for (int u = 0; u < kRowPairs; ++u) {
-                const uint32_t r = r0 + 2 * u + half;
-                if (r >= rows) continue;
-                *reinterpret_cast<uint4*>(dst + (size_t(row0 + r) * kRow + hl * 8) * 2) =
-                    dequant8(v[u], sc[u]);
-            }
-        }
-    }
-}
-
-// ---------------------------------------------------------------- row-sliced reads
-// The geometry of launch_kv_gather_fp8 with GatherLaunch::rows, in elements of the part's bf16
-// view (GatherLaunch counts bytes): row r of stored part s takes vpr 8-element vectors from
-// element r * src_pitch + src_col, and lands at r * dst_pitch bytes from the part's destination.
+// ---------------------------------------------------------------- gathered reads
+// The geometry of launch_kv_gather_fp8's reads, in elements of the part's bf16 view
+// (GatherLaunch counts bytes): a stored part holds `elems` e4m3 elements and their scales; with
+// GatherLaunch::rows, row r of it takes vpr 8-element vectors from element r * src_pitch +
+// src_col, and lands at r * dst_pitch bytes from the part's destination (slices, slice_pitch,
+// pieces and piece_off as in GatherLaunch).
 struct Fp8Rows {
-    uint32_t rows, vpr, src_pitch, src_col, dst_pitch, elems;
+    uint32_t rows, vpr, src_pitch, src_col, dst_pitch, elems, slices, slice_pitch, pieces;
+    const uint64_t* piece_off;
 };
 
 constexpr int kRowVecs = 4;  // (row, vector) pairs in flight per thread: 4 x 16 B of bf16
@@ -435,208 +310,125 @@ __device__ __forceinline__ void read_fp8_rows(uint8_t* dst, const uint8_t* q, co
     }
 }
 
-// Item = run c (`run` rows) of part s of block b, numbered with layered_item: one group of all
-// nparts parts for a plain read, rel.gp parts per group for a layered one, each group released
-// by leave_group - the numbering, miss counting and release of kv_scatter_rows_kernel
-// (kv_copy.cu).  Stored part first_part + s starts at desc.src + (first_part + s) * stride.
-// A missing block counts once, on its first item, and its parts are left untouched; its items
-// still count as arrivals.  SLICED (kv_read_fp8_slices_kernel, GatherLaunch::slices > 1): a
-// run is `run` (slice, row) pairs of the part, numbered slice-major.  PIECES
-// (kv_read_fp8_pieces_kernel, GatherLaunch::pieces > 1, any slices): the run is cut where
-// q / piece_rows changes, as in kv_scatter_pieces_kernel (kv_copy.cu), and each cut is read as
-// plain rows to desc.dst + piece_off[block * pieces + t] + the place piece_pair gives its first
-// pair - one piece-offset load per cut.
-template <bool LAYERED, bool SLICED, bool PIECES = false>
-__device__ __forceinline__ void read_fp8_row_items(const CopyDesc* __restrict__ descs,
-                                                   const GatherParts& parts, uint32_t n,
-                                                   uint32_t nparts, uint32_t first_part,
-                                                   const Fp8Rows& geo, uint32_t slices,
-                                                   uint32_t slice_pitch, uint32_t run,
-                                                   uint32_t cpp, uint64_t stride,
-                                                   uint32_t* status, const GroupRelease& rel,
-                                                   const uint64_t* piece_off = nullptr,
-                                                   uint32_t pieces = 1) {
-    const uint32_t gp = LAYERED ? rel.gp : nparts;
-    const uint32_t group_items = n * gp * cpp;
-    const uint32_t total = n * nparts * cpp;
-    uint32_t item = blockIdx.x;
-    CopyDesc next = item < total ? descs[layered_item(item, n, gp, cpp).block] : CopyDesc{0, 0};
-    for (; item < total; item += gridDim.x) {
-        const CopyDesc d = next;
-        const LayeredItem it = layered_item(item, n, gp, cpp);
-        const uint32_t nxt = item + gridDim.x;
-        if (nxt < total) next = descs[layered_item(nxt, n, gp, cpp).block];
-        if (d.src != 0 && PIECES) {
-            const uint32_t piece_rows = geo.rows / pieces;
-            const uint32_t q0 = it.chunk * run, q1 = min(q0 + run, geo.rows * slices);
-            const uint8_t* q =
-                reinterpret_cast<const uint8_t*>(d.src + uint64_t(first_part + it.part) * stride);
-            const uint64_t* off = piece_off + uint64_t(it.block) * pieces;
+// Reads: gather_items.cuh's scatter_items walk, one body per part shape.  Item chunk c of part s
+// of block b reads stored part first_part + s, at desc.src + (first_part + s) * stride, into
+// local parts.base[s] + desc.dst:
+//   kWhole   rows [c * chunk, +chunk) / 128 of the page, a half-warp per 128-element row as in
+//            kv_read_fp8_kernel;
+//   kRows    rows [c * chunk, +chunk) (GatherLaunch::rows: read_fp8_rows);
+//   kSlices  (slice, row) pairs [c * chunk, +chunk), numbered slice-major (read_fp8_rows<true>);
+//   kPieces  the same pairs (GatherLaunch::pieces > 1, any slices), cut where q / piece_rows
+//            changes as in kv_copy.cu's kv_scatter_ldst_kernel; each cut is read as plain rows to
+//            desc.dst + piece_off[block * pieces + t] + the place piece_pair gives its first pair
+//            - one piece-offset load per cut.
+// (This kernel and kv_read_fp8_kernel share the row maths, not the loop: inlining one loop body
+// into both changed how the compiler schedules kv_read_fp8_kernel.)
+static_assert(kThreads == kLdStThreads, "scatter_items releases groups on kLdStThreads threads");
+template <bool LAYERED, PartShape S>
+__global__ void __launch_bounds__(kThreads)
+    kv_read_fp8_scatter_kernel(const CopyDesc* __restrict__ descs,
+                               const __grid_constant__ GatherParts parts, uint32_t n,
+                               uint32_t nparts, uint32_t first_part, uint32_t chunk, uint32_t cpp,
+                               uint64_t stride, Fp8Rows g, uint32_t* status, GroupRelease rel) {
+    scatter_items<LAYERED>(descs, n, nparts, cpp, status, rel, [&](const CopyDesc& d,
+                                                                  const LayeredItem& it) {
+        const uint8_t* q =
+            reinterpret_cast<const uint8_t*>(d.src + uint64_t(first_part + it.part) * stride);
+        const float* scales = reinterpret_cast<const float*>(q + g.elems);
+        uint8_t* dst = reinterpret_cast<uint8_t*>(parts.base[it.part] + d.dst);
+        if constexpr (S == PartShape::kWhole) {
+            const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+            const uint32_t half = lane >> 4, hl = lane & 15;
+            constexpr uint32_t kStep = 2 * kRowPairs;
+            const uint32_t e0 = it.chunk * chunk;
+            const uint32_t rows = min(chunk, g.elems - e0) / kRow;
+            const uint32_t row0 = e0 / kRow;
+            for (uint32_t r0 = warp * kStep; r0 < rows; r0 += kWarps * kStep) {
+                uint2 v[kRowPairs];
+                float sc[kRowPairs];
+#pragma unroll
+                for (int u = 0; u < kRowPairs; ++u) {
+                    const uint32_t r = r0 + 2 * u + half;
+                    if (r < rows) {
+                        v[u] = ld_u2(q + size_t(row0 + r) * kRow + hl * 8);
+                        sc[u] = __uint_as_float(ld_u1(scales + row0 + r));
+                    }
+                }
+#pragma unroll
+                for (int u = 0; u < kRowPairs; ++u) {
+                    const uint32_t r = r0 + 2 * u + half;
+                    if (r >= rows) continue;
+                    *reinterpret_cast<uint4*>(dst + (size_t(row0 + r) * kRow + hl * 8) * 2) =
+                        dequant8(v[u], sc[u]);
+                }
+            }
+        } else if constexpr (S == PartShape::kRows) {
+            const uint32_t r0 = it.chunk * chunk;
+            read_fp8_rows(dst + uint64_t(r0) * g.dst_pitch, q, scales, r0 * g.src_pitch + g.src_col,
+                          min(chunk, g.rows - r0), g);
+        } else if constexpr (S == PartShape::kSlices) {
+            const uint32_t q0 = it.chunk * chunk;
+            read_fp8_rows<true>(dst, q, scales, q0, min(chunk, g.rows * g.slices - q0), g,
+                                g.slice_pitch);
+        } else {
+            const uint32_t piece_rows = g.rows / g.pieces;
+            const uint32_t q0 = it.chunk * chunk, q1 = min(q0 + chunk, g.rows * g.slices);
+            const uint64_t* off = g.piece_off + uint64_t(it.block) * g.pieces;
             for (uint32_t p = q0; p < q1;) {
                 const uint32_t e = min(q1, (p / piece_rows + 1) * piece_rows);
-                const PieceOffsets o = piece_pair(p, geo.rows, 8 * geo.vpr, geo.src_pitch,
-                                                  geo.src_col, geo.dst_pitch, slice_pitch,
-                                                  piece_rows);
-                read_fp8_rows(
-                    reinterpret_cast<uint8_t*>(parts.base[it.part] + d.dst + off[o.piece] + o.dst),
-                    q, reinterpret_cast<const float*>(q + geo.elems), o.src, e - p, geo);
+                const PieceOffsets o = piece_pair(p, g.rows, 8 * g.vpr, g.src_pitch, g.src_col,
+                                                  g.dst_pitch, g.slice_pitch, piece_rows);
+                read_fp8_rows(dst + off[o.piece] + o.dst, q, scales, o.src, e - p, g);
                 p = e;
             }
-        } else if (d.src != 0 && SLICED) {
-            const uint32_t q0 = it.chunk * run;
-            const uint8_t* q =
-                reinterpret_cast<const uint8_t*>(d.src + uint64_t(first_part + it.part) * stride);
-            read_fp8_rows<true>(reinterpret_cast<uint8_t*>(parts.base[it.part] + d.dst), q,
-                                reinterpret_cast<const float*>(q + geo.elems), q0,
-                                min(run, geo.rows * slices - q0), geo, slice_pitch);
-        } else if (d.src != 0) {
-            const uint32_t r0 = it.chunk * run;
-            const uint8_t* q =
-                reinterpret_cast<const uint8_t*>(d.src + uint64_t(first_part + it.part) * stride);
-            uint8_t* dst = reinterpret_cast<uint8_t*>(parts.base[it.part] + d.dst +
-                                                      uint64_t(r0) * geo.dst_pitch);
-            read_fp8_rows(dst, q, reinterpret_cast<const float*>(q + geo.elems),
-                          r0 * geo.src_pitch + geo.src_col, min(run, geo.rows - r0), geo);
-        } else if (threadIdx.x == 0 && item < group_items && item % (gp * cpp) == 0 && status) {
-            atomicAdd(status + kStatMiss, 1u);
         }
-        if constexpr (LAYERED) {
-            if (nxt >= total || nxt / group_items != it.group) {
-                const uint32_t lo = it.group * group_items;
-                leave_group(rel, it.group, cta_items(lo, lo + group_items, blockIdx.x, gridDim.x),
-                            group_items, kThreads);
-            }
-        }
-    }
+    });
 }
 
-template <bool LAYERED>
-__global__ void __launch_bounds__(kThreads)
-    kv_read_fp8_rows_kernel(const CopyDesc* __restrict__ descs,
-                            const __grid_constant__ GatherParts parts, uint32_t n, uint32_t nparts,
-                            uint32_t first_part, Fp8Rows geo, uint32_t run, uint32_t cpp,
-                            uint64_t stride, uint32_t* status, GroupRelease rel) {
-    read_fp8_row_items<LAYERED, false>(descs, parts, n, nparts, first_part, geo, 1, 0, run, cpp,
-                                       stride, status, rel);
-}
-
-// GatherLaunch::slices > 1: runs of (slice, row) pairs (read_fp8_row_items above).
-template <bool LAYERED>
-__global__ void __launch_bounds__(kThreads)
-    kv_read_fp8_slices_kernel(const CopyDesc* __restrict__ descs,
-                              const __grid_constant__ GatherParts parts, uint32_t n,
-                              uint32_t nparts, uint32_t first_part, Fp8Rows geo, uint32_t slices,
-                              uint32_t slice_pitch, uint32_t run, uint32_t cpp, uint64_t stride,
-                              uint32_t* status, GroupRelease rel) {
-    read_fp8_row_items<LAYERED, true>(descs, parts, n, nparts, first_part, geo, slices,
-                                      slice_pitch, run, cpp, stride, status, rel);
-}
-
-// GatherLaunch::pieces > 1, one or more slices: runs cut at piece boundaries
-// (read_fp8_row_items above).
-template <bool LAYERED>
-__global__ void __launch_bounds__(kThreads)
-    kv_read_fp8_pieces_kernel(const CopyDesc* __restrict__ descs,
-                              const __grid_constant__ GatherParts parts, uint32_t n,
-                              uint32_t nparts, uint32_t first_part, Fp8Rows geo, uint32_t slices,
-                              uint32_t slice_pitch, uint32_t run, uint32_t cpp, uint64_t stride,
-                              uint32_t* status, GroupRelease rel, const uint64_t* piece_off,
-                              uint32_t pieces) {
-    read_fp8_row_items<LAYERED, false, true>(descs, parts, n, nparts, first_part, geo, slices,
-                                             slice_pitch, run, cpp, stride, status, rel,
-                                             piece_off, pieces);
-}
-
-int fp8_rows_resident(const void* kernel) {
-    int r = 1;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&r, kernel, kThreads, 0);
-    return r > 0 ? r : 1;
-}
-
-cudaError_t launch_kv_read_fp8_rows(const GatherLaunch& a, uint32_t elems, cudaStream_t stream) {
-    const bool layered = a.group_flags != nullptr;
-    if (layered && !a.group_counters) return cudaErrorInvalidValue;
-    static const int res = fp8_rows_resident(reinterpret_cast<const void*>(kv_read_fp8_rows_kernel<false>));
-    static const int res_layered =
-        fp8_rows_resident(reinterpret_cast<const void*>(kv_read_fp8_rows_kernel<true>));
-    static const int res_sliced =
-        fp8_rows_resident(reinterpret_cast<const void*>(kv_read_fp8_slices_kernel<false>));
-    static const int res_sliced_layered =
-        fp8_rows_resident(reinterpret_cast<const void*>(kv_read_fp8_slices_kernel<true>));
-    static const int res_pieces =
-        fp8_rows_resident(reinterpret_cast<const void*>(kv_read_fp8_pieces_kernel<false>));
-    static const int res_pieces_layered =
-        fp8_rows_resident(reinterpret_cast<const void*>(kv_read_fp8_pieces_kernel<true>));
-    const bool sliced = a.slices > 1;
-    const bool pieced = a.pieces > 1;
-    if (pieced && !a.piece_off) return cudaErrorInvalidValue;
-    const int r = pieced   ? (layered ? res_pieces_layered : res_pieces)
-                  : sliced ? (layered ? res_sliced_layered : res_sliced)
-                           : (layered ? res_layered : res);
-    const LaunchPlan p = plan_gather_fp8_rows(a, elems, sm_count(), {r, r});
-    if (!p.valid) return cudaErrorInvalidValue;  // the caller checks the geometry and splits
-    GatherParts parts;
-    std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
-    const Fp8Rows geo{a.rows, a.row_bytes / 16, a.src_pitch / 2, a.src_col / 2, a.dst_pitch, elems};
+// One gathered fp8 ld/st launch of shape S: its plan (whole pages may take the TMA pipeline of
+// kv_fp8_pipe.cu), then the kernel.  The row plans' grid follows the launched kernel's residency.
+template <bool WRITE, bool LAYERED, PartShape S>
+cudaError_t launch_fp8_gather(const GatherLaunch& a, uint32_t elems, int variant,
+                              const GatherParts& parts, cudaStream_t stream) {
     const uint64_t stride = fp8_gather_bytes(1, elems);
-    const GroupRelease rel{a.group_flags, a.group_counters, a.group_seq, a.group_parts};
-    if (pieced) {
-        const auto go = [&](auto* kernel) {
-            kernel<<<p.ctas, kThreads, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.first_part,
-                                                    geo, a.slices, a.dst_slice_pitch, p.chunk,
-                                                    p.cpb, stride, a.status, rel, a.piece_off,
-                                                    a.pieces);
-            return cudaGetLastError();
-        };
-        return layered ? go(kv_read_fp8_pieces_kernel<true>) : go(kv_read_fp8_pieces_kernel<false>);
-    }
-    if (sliced) {
-        const auto go = [&](auto* kernel) {
-            kernel<<<p.ctas, kThreads, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.first_part,
-                                                    geo, a.slices, a.dst_slice_pitch, p.chunk,
-                                                    p.cpb, stride, a.status, rel);
-            return cudaGetLastError();
-        };
-        return layered ? go(kv_read_fp8_slices_kernel<true>) : go(kv_read_fp8_slices_kernel<false>);
-    }
-    const auto go = [&](auto* kernel) {
-        kernel<<<p.ctas, kThreads, 0, stream>>>(a.descs, parts, a.n, a.nparts, a.first_part, geo,
-                                                p.chunk, p.cpb, stride, a.status, rel);
-        return cudaGetLastError();
-    };
-    return layered ? go(kv_read_fp8_rows_kernel<true>) : go(kv_read_fp8_rows_kernel<false>);
-}
-
-cudaError_t launch_kv_write_fp8_rows(const GatherLaunch& a, uint32_t elems, cudaStream_t stream) {
-    static const int res = [] {
-        int r = 1;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&r, kv_write_fp8_rows_kernel, kThreads + 32, 0);
-        return r > 0 ? r : 1;
+    const SlicedRows rows{a.row_bytes, a.src_pitch, a.dst_pitch, a.dst_slice_pitch};
+    const auto load_at = [&] {
+        if constexpr (S == PartShape::kWhole)
+            return DenseRows{};
+        else if constexpr (S == PartShape::kRows)
+            return rows;
+        else
+            return PiecedRows{rows, a.rows / a.pieces, a.pieces, a.piece_off};
     }();
-    static const int res_pieces = [] {
-        int r = 1;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&r, kv_write_fp8_pieces_kernel,
-                                                      kThreads + 32, 0);
-        return r > 0 ? r : 1;
-    }();
-    const bool pieced = a.pieces > 1;
-    if (pieced && !a.piece_off) return cudaErrorInvalidValue;
-    const int r = pieced ? res_pieces : res;
-    const LaunchPlan p = plan_gather_fp8_rows_write(a, elems, sm_count(), {r, r});
+    using LoadAt = std::decay_t<decltype(load_at)>;
+    LaunchPlan p;
+    if constexpr (S == PartShape::kWhole) {
+        p = plan_gather_fp8(a, elems, variant, sm_count());
+    } else if constexpr (WRITE) {
+        p = plan_gather_fp8_rows_write(
+            a, elems, sm_count(),
+            cached_resident<kv_write_fp8_gather_kernel<LoadAt>, kv_write_fp8_gather_kernel<LoadAt>,
+                            kThreads + 32>());
+    } else {
+        p = plan_gather_fp8_rows(
+            a, elems, sm_count(),
+            cached_resident<kv_read_fp8_scatter_kernel<LAYERED, S>,
+                            kv_read_fp8_scatter_kernel<LAYERED, S>, kThreads>());
+    }
     if (!p.valid) return cudaErrorInvalidValue;  // the caller checks the geometry and splits
-    GatherParts parts;
-    std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
-    const SlicedRows geo{a.row_bytes, a.src_pitch, a.dst_pitch, a.dst_slice_pitch};
-    if (pieced) {
-        kv_write_fp8_pieces_kernel<<<p.ctas, kThreads + 32, 0, stream>>>(
-            a.descs, parts, a.n, a.nparts, elems, p.chunk, p.cpb, a.first_part,
-            fp8_gather_bytes(1, elems), PiecedRows{geo, a.rows / a.pieces, a.pieces, a.piece_off},
+    if (p.kernel != Kernel::kLdStFp8) return launch_kv_fp8_pipe_gather(a, elems, stream);
+    if constexpr (WRITE) {
+        kv_write_fp8_gather_kernel<<<p.ctas, kThreads + 32, 0, stream>>>(
+            a.descs, parts, a.n, a.nparts, elems, p.chunk, p.cpb, a.first_part, stride, load_at,
             publish_of(a, true), layer_of(a));
-        return cudaGetLastError();
+    } else {
+        const Fp8Rows g{a.rows,          a.row_bytes / 16, a.src_pitch / 2, a.src_col / 2,
+                        a.dst_pitch,     elems,            a.slices,        a.dst_slice_pitch,
+                        a.pieces,        a.piece_off};
+        kv_read_fp8_scatter_kernel<LAYERED, S><<<p.ctas, kThreads, 0, stream>>>(
+            a.descs, parts, a.n, a.nparts, a.first_part, p.chunk, p.cpb, stride, g, a.status,
+            release_of(a));
     }
-    kv_write_fp8_rows_kernel<<<p.ctas, kThreads + 32, 0, stream>>>(
-        a.descs, parts, a.n, a.nparts, elems, p.chunk, p.cpb, a.first_part,
-        fp8_gather_bytes(1, elems), geo, publish_of(a, true), layer_of(a));
     return cudaGetLastError();
 }
 
@@ -668,34 +460,21 @@ cudaError_t launch_kv_gather_fp8(const GatherLaunch& a, uint32_t elems, int vari
                                  cudaStream_t stream) {
     if (a.n == 0) return cudaSuccess;
     if (!a.part_base) return cudaErrorInvalidValue;
-    if (a.rows)
-        return a.write ? launch_kv_write_fp8_rows(a, elems, stream)
-                       : launch_kv_read_fp8_rows(a, elems, stream);
-    if (a.pieces != 1) return cudaErrorInvalidValue;  // pieces split rows
-    // a layered read takes the ld/st kernel whatever the variant (no layered pipeline)
     const bool layered = a.group_flags != nullptr;
-    if (layered && (a.write || !a.group_counters || !a.group_parts || a.nparts % a.group_parts))
-        return cudaErrorInvalidValue;
-    const LaunchPlan p = plan_gather_fp8(a, elems, layered ? int(kFp8LdSt) : variant, sm_count());
-    if (!p.valid) return cudaErrorInvalidValue;  // the caller splits the batch
-    if (p.kernel != Kernel::kLdStFp8) return launch_kv_fp8_pipe_gather(a, elems, stream);
-    GatherParts parts;
-    std::memcpy(parts.base, a.part_base, size_t(a.nparts) * sizeof(uint64_t));
-    const uint64_t stride = fp8_gather_bytes(1, elems);
-    const GroupRelease rel{a.group_flags, a.group_counters, a.group_seq, a.group_parts};
+    if (layered && !a.group_counters) return cudaErrorInvalidValue;
+    // pieces split rows, at the offsets of the piece table
+    if (a.pieces != 1 && (!a.rows || !a.piece_off)) return cudaErrorInvalidValue;
+    const GatherParts parts = parts_of(a);
     if (a.write)
-        kv_write_fp8_gather_kernel<<<p.ctas, kThreads + 32, 0, stream>>>(
-            a.descs, parts, a.n, a.nparts, elems, p.chunk, p.cpb, a.first_part, stride,
-            publish_of(a, true), layer_of(a));
-    else if (layered)
-        kv_read_fp8_scatter_kernel<true><<<p.ctas, kThreads, 0, stream>>>(
-            a.descs, parts, a.n, a.nparts, a.first_part, elems, p.chunk, p.cpb, stride, a.status,
-            rel);
-    else
-        kv_read_fp8_scatter_kernel<<<p.ctas, kThreads, 0, stream>>>(
-            a.descs, parts, a.n, a.nparts, a.first_part, elems, p.chunk, p.cpb, stride, a.status,
-            rel);
-    return cudaGetLastError();
+        return with_shape<true>(a, [&](auto s) {
+            return launch_fp8_gather<true, false, decltype(s)::value>(a, elems, variant, parts,
+                                                                      stream);
+        });
+    return with_shape<false>(a, [&](auto s) {
+        constexpr PartShape S = decltype(s)::value;
+        return layered ? launch_fp8_gather<false, true, S>(a, elems, variant, parts, stream)
+                       : launch_fp8_gather<false, false, S>(a, elems, variant, parts, stream);
+    });
 }
 
 }  // namespace istore::kernels

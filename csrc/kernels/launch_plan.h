@@ -3,8 +3,9 @@
 // kv_fp8.cu, kv_fp8_pipe.cu) pass in the SM count and the CTAs per SM the ld/st kernels keep
 // resident (occupancy API), so the choice is unit-tested on the CPU
 // (_infinistore.testing.plan_copy / plan_gather / plan_read_fused / plan_fp8 /
-// plan_gather_fp8 / plan_gather_layered / plan_gather_rows / plan_gather_fp8_rows /
-// plan_gather_rows_write / plan_gather_fp8_rows_write).
+// plan_gather_fp8 / plan_gather_rows / plan_gather_fp8_rows / plan_gather_rows_write /
+// plan_gather_fp8_rows_write; plan_gather_layered is plan_gather of a layered read).  The
+// gathered ld/st kernels these plans choose walk their items in gather_items.cuh.
 #pragma once
 
 #include <algorithm>
@@ -193,13 +194,22 @@ inline LaunchPlan plan_pipe_gather(const GatherLaunch& a, int sms) {
     return p;
 }
 
+// A layered read's groups (GatherLaunch::group_flags): only reads are layered, and group_parts
+// divides nparts.  Every gathered plan refuses a launch that breaks this.
+inline bool groups_ok(const GatherLaunch& a) {
+    return !a.group_flags || (!a.write && a.group_parts != 0 && a.nparts % a.group_parts == 0);
+}
+
 // Gathers take no variant: 16-byte aligned parts of at least kPipeMinBytes go to the TMA
 // pipeline (the per-part form of launch_kv_copy's auto rule), even on a local pool or an ldst
-// connection.
+// connection.  A layered read always runs the ld/st kernels (the TMA pipelines have no layered
+// flavour): 16- or 32-byte vectors, the byte kernel on an unaligned batch.
 inline LaunchPlan plan_gather(const GatherLaunch& a, int sms, LdStResident res) {
+    if (!groups_ok(a)) return invalid_plan();
     const bool aligned16 = aligned_to(a.part_bytes, a.align_or, 16);
     const bool aligned32 = aligned_to(a.part_bytes, a.align_or, 32);
-    if (aligned16 && a.part_bytes >= kPipeMinBytes) return plan_pipe_gather(a, sms);
+    if (!a.group_flags && aligned16 && a.part_bytes >= kPipeMinBytes)
+        return plan_pipe_gather(a, sms);
     LaunchPlan p;
     p.kernel = !aligned16 ? Kernel::kLdSt1 : aligned32 ? Kernel::kLdSt32 : Kernel::kLdSt16;
     const uint64_t parts = uint64_t(a.n) * a.nparts;
@@ -233,24 +243,6 @@ ISTORE_KHD inline uint32_t cta_items_below(uint32_t end, uint32_t first, uint32_
 }
 ISTORE_KHD inline uint32_t cta_items(uint32_t lo, uint32_t hi, uint32_t first, uint32_t stride) {
     return cta_items_below(hi, first, stride) - cta_items_below(lo, first, stride);
-}
-
-// The layered read runs the ld/st kernels whatever the part size (the TMA pipelines have no
-// layered flavour): 16- or 32-byte vectors, the byte kernel on an unaligned batch.  Whole
-// parts as items as in plan_gather; group_parts must divide nparts.
-inline LaunchPlan plan_gather_layered(const GatherLaunch& a, int sms, LdStResident res) {
-    if (a.nparts == 0 || a.nparts > kGatherMaxParts || a.group_parts == 0 ||
-        a.nparts % a.group_parts != 0 || a.write)
-        return invalid_plan();
-    const bool aligned16 = aligned_to(a.part_bytes, a.align_or, 16);
-    const bool aligned32 = aligned_to(a.part_bytes, a.align_or, 32);
-    LaunchPlan p;
-    p.kernel = !aligned16 ? Kernel::kLdSt1 : aligned32 ? Kernel::kLdSt32 : Kernel::kLdSt16;
-    const uint64_t parts = uint64_t(a.n) * a.nparts;
-    ldst_items(p, parts, a.part_bytes, kLdStChunk, 1u << 20, sms);
-    if (parts * p.cpb > kMaxItems) return invalid_plan();
-    p.ctas = ldst_grid(p, a.max_ctas, res, sms, parts * p.cpb);
-    return p;
 }
 
 // ---------------------------------------------------------------- row geometry
@@ -307,8 +299,8 @@ ISTORE_KHD inline PairOffsets slice_pair(uint32_t q, uint32_t rows, uint32_t row
 // piece 0.  Pairs q with the same q / piece_rows share their slice and their piece (rows is a
 // multiple of piece_rows), so the kernels copy each such run as plain rows from the place
 // piece_pair gives its first pair, loading its piece offset once.  The kernels (kv_copy.cu:
-// scatter_rows, kv_fp8.cu: read_fp8_row_items) and the CPU tests (_infinistore.testing.piece_pair)
-// share this function.
+// kv_scatter_ldst_kernel, kv_fp8.cu: kv_read_fp8_scatter_kernel) and the CPU tests
+// (_infinistore.testing.piece_pair) share this function.
 struct PieceOffsets {
     uint32_t src, dst, piece;
 };
@@ -320,8 +312,30 @@ ISTORE_KHD inline PieceOffsets piece_pair(uint32_t q, uint32_t rows, uint32_t ro
                         (r - t * piece_rows) * dst_pitch + j * dst_slice_pitch, t};
 }
 
+// A row-sliced write (GatherLaunch::rows with write) takes the geometry that reads the same
+// local layout back: the stored part is src_pitch-byte rows, the caller's part holds slice j of
+// row r at r * dst_pitch + j * dst_slice_pitch - e.g. a head-major page [head][token][dim]
+// stored token-major.  The in-band commit publishes whole blocks, so a write must fill every
+// byte of the stored part: on top of row_geometry_ok, src_col == 0 and slices * row_bytes ==
+// src_pitch.
+inline bool row_write_covers(uint32_t row_bytes, uint32_t src_pitch, uint32_t src_col,
+                             uint32_t slices) {
+    return src_col == 0 && uint64_t(slices) * row_bytes == src_pitch;
+}
+
+// What the four row plans (bf16 and fp8, reads and writes) admit: a launch of `write`'s
+// direction, 1 to kGatherMaxParts parts, a row geometry row_geometry_ok accepts, and the
+// groups of a layered read (groups_ok; writes are never layered).  A write's rows must cover
+// the stored part (row_write_covers).
+inline bool rows_admitted(const GatherLaunch& a, bool write) {
+    return a.write == write && a.nparts != 0 && a.nparts <= kGatherMaxParts && groups_ok(a) &&
+           row_geometry_ok(a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.slices,
+                           a.dst_slice_pitch, a.part_bytes, a.pieces) &&
+           (!write || row_write_covers(a.row_bytes, a.src_pitch, a.src_col, a.slices));
+}
+
 // ---------------------------------------------------------------- row-sliced reads
-// kv_scatter_rows (GatherLaunch::rows != 0), plain or layered: always the ld/st kernels (the
+// Row reads (GatherLaunch::rows != 0), plain or layered: always the ld/st kernels (the
 // TMA pipelines have no row form).  The vector width is the one the OR of row_bytes, both
 // pitches (with slices > 1, dst_slice_pitch too), src_col, the part bases and the local
 // offsets allows (pool blocks are granule aligned and part_bytes is a multiple of src_pitch).
@@ -329,11 +343,7 @@ ISTORE_KHD inline PieceOffsets piece_pair(uint32_t q, uint32_t rows, uint32_t ro
 // about kLdStChunk of payload, or all of a part's pairs under ldst_items' rule; cpb is runs per
 // part, and a layered read numbers items with layered_item as whole parts do.
 inline LaunchPlan plan_gather_rows(const GatherLaunch& a, int sms, LdStResident res) {
-    if (a.write || a.nparts == 0 || a.nparts > kGatherMaxParts ||
-        !row_geometry_ok(a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.slices,
-                         a.dst_slice_pitch, a.part_bytes, a.pieces) ||
-        (a.group_flags && (a.group_parts == 0 || a.nparts % a.group_parts != 0)))
-        return invalid_plan();
+    if (!rows_admitted(a, false)) return invalid_plan();
     const uint64_t geo_or = a.align_or | a.src_pitch | a.src_col | a.dst_pitch |
                             (a.slices > 1 ? a.dst_slice_pitch : 0u);
     const bool aligned16 = aligned_to(a.row_bytes, geo_or, 16);
@@ -349,22 +359,11 @@ inline LaunchPlan plan_gather_rows(const GatherLaunch& a, int sms, LdStResident 
 }
 
 // ---------------------------------------------------------------- row-sliced writes
-// A row-sliced write (GatherLaunch::rows with write) takes the geometry that reads the same
-// local layout back: the stored part is src_pitch-byte rows, the caller's part holds slice j of
-// row r at r * dst_pitch + j * dst_slice_pitch - e.g. a head-major page [head][token][dim]
-// stored token-major.  The in-band commit publishes whole blocks, so a write must fill every
-// byte of the stored part: on top of row_geometry_ok, src_col == 0 and slices * row_bytes ==
-// src_pitch.
-inline bool row_write_covers(uint32_t row_bytes, uint32_t src_pitch, uint32_t src_col,
-                             uint32_t slices) {
-    return src_col == 0 && uint64_t(slices) * row_bytes == src_pitch;
-}
-
 // Where byte o of a fully covered stored part comes from in the caller's part: row r =
 // o / src_pitch, slice j of it, column c - j * row_bytes of that slice.  Over a covering
 // geometry it is the inverse of slice_pair: row_write_offset(slice_pair(q).src + w) ==
 // slice_pair(q).dst + w for every byte w < row_bytes.  The kernels (copy_span.cuh:
-// copy_span_rows, kv_fp8.cu: kv_write_fp8_rows) and the CPU tests
+// copy_span_rows, kv_fp8.cu: SlicedRows) and the CPU tests
 // (_infinistore.testing.row_write_offset) share this function.
 ISTORE_KHD inline uint32_t row_write_offset(uint32_t o, uint32_t row_bytes, uint32_t src_pitch,
                                             uint32_t dst_pitch, uint32_t dst_slice_pitch) {
@@ -389,19 +388,15 @@ ISTORE_KHD inline PieceOffset piece_write_offset(uint32_t o, uint32_t row_bytes,
                                            dst_slice_pitch)};
 }
 
-// kv_gather_rows_write (launch_kv_gather with rows and write): the work items of the
+// Row writes (launch_kv_gather with rows and write): the work items of the
 // whole-part write, (block, part, chunk of the stored part) numbered (b * nparts + s) * cpp + c
 // with plan_gather's ld/st chunks, so every item stores one contiguous run of pool bytes and
-// the commit counts arrivals as for kv_gather_ldst; only the local load address goes through
+// the commit counts arrivals as for whole parts; only the local load address goes through
 // row_write_offset.  Always the ld/st kernels (no TMA form), never layered reads.  The vector
 // width is the one the OR of row_bytes, dst_pitch, dst_slice_pitch (with slices > 1), the part
 // bases and the local offsets allows (src_pitch is slices * row_bytes).
 inline LaunchPlan plan_gather_rows_write(const GatherLaunch& a, int sms, LdStResident res) {
-    if (!a.write || a.group_flags || a.nparts == 0 || a.nparts > kGatherMaxParts ||
-        !row_geometry_ok(a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.slices,
-                         a.dst_slice_pitch, a.part_bytes, a.pieces) ||
-        !row_write_covers(a.row_bytes, a.src_pitch, a.src_col, a.slices))
-        return invalid_plan();
+    if (!rows_admitted(a, true)) return invalid_plan();
     const uint64_t geo_or =
         a.align_or | a.dst_pitch | (a.slices > 1 ? a.dst_slice_pitch : 0u);
     const bool aligned16 = aligned_to(a.row_bytes, geo_or, 16);
@@ -415,7 +410,7 @@ inline LaunchPlan plan_gather_rows_write(const GatherLaunch& a, int sms, LdStRes
     return p;
 }
 
-// kv_write_fp8_rows (launch_kv_gather_fp8 with rows and write): the items of the gathered fp8
+// fp8 row writes (launch_kv_gather_fp8 with rows and write): the items of the gathered fp8
 // ld/st write (plan_gather_fp8 with kFp8LdSt: chunks of kFp8Chunk elements of the stored fp8
 // page, or whole pages under ldst_items' rule), the geometry of plan_gather_rows_write in bytes
 // of the part's bf16 view (part_bytes == rows * src_pitch == 2 * elems), and every geometry
@@ -424,11 +419,7 @@ inline LaunchPlan plan_gather_rows_write(const GatherLaunch& a, int sms, LdStRes
 // the occupancy API's answer for it).
 inline LaunchPlan plan_gather_fp8_rows_write(const GatherLaunch& a, uint32_t elems, int sms,
                                              LdStResident res) {
-    if (!a.write || a.group_flags || a.nparts == 0 || a.nparts > kGatherMaxParts ||
-        !row_geometry_ok(a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.slices,
-                         a.dst_slice_pitch, a.part_bytes, a.pieces) ||
-        !row_write_covers(a.row_bytes, a.src_pitch, a.src_col, a.slices))
-        return invalid_plan();
+    if (!rows_admitted(a, true)) return invalid_plan();
     const uint64_t geo_or = a.align_or | a.row_bytes | a.src_pitch | a.dst_pitch |
                             (a.slices > 1 ? a.dst_slice_pitch : 0u);
     const uint64_t parts = uint64_t(a.n) * a.nparts;
@@ -510,27 +501,28 @@ inline LaunchPlan plan_fp8(const Fp8Launch& a, int sms) {
 
 // ---------------------------------------------------------------- launch_kv_gather_fp8
 // Every part of every block is one fp8 page, so the rules of plan_fp8 apply with n * nparts
-// pages: cpb is the items per part.  kFp8LdSt picks the ld/st kernels, anything else the
-// pipeline with 8 compute warps.  Parts of a multiple of 512 elements and 16-byte aligned part
-// bases and offsets only (the pipeline's precondition, and every part starts 16-byte aligned);
-// more than kMaxItems work items are refused (the caller splits the batch).
+// pages: cpb is the items per part.  kFp8LdSt, or a layered read (groups_ok), picks the ld/st
+// kernels, anything else the pipeline with 8 compute warps.  Parts of a multiple of 512
+// elements and 16-byte aligned part bases and offsets only (the pipeline's precondition, and
+// every part starts 16-byte aligned); more than kMaxItems work items are refused (the caller
+// splits the batch).
 inline LaunchPlan plan_gather_fp8(const GatherLaunch& a, uint32_t elems, int variant, int sms) {
     const uint64_t parts = uint64_t(a.n) * a.nparts;
-    if (a.nparts == 0 || a.nparts > kGatherMaxParts || elems == 0 || elems % 512 != 0 ||
-        (a.align_or & 15) != 0 || parts > kMaxItems)
+    if (a.nparts == 0 || a.nparts > kGatherMaxParts || !groups_ok(a) || elems == 0 ||
+        elems % 512 != 0 || (a.align_or & 15) != 0 || parts > kMaxItems)
         return invalid_plan();
     Fp8Launch f;
     f.n = uint32_t(parts);
     f.elems = elems;
     f.max_ctas = a.max_ctas;
-    f.variant = variant == kFp8LdSt ? kFp8LdSt : kFp8Auto;
+    f.variant = variant == kFp8LdSt || a.group_flags ? kFp8LdSt : kFp8Auto;
     LaunchPlan p = plan_fp8(f, sms);
     if (parts * p.cpb > kMaxItems) return invalid_plan();
     return p;
 }
 
 // ---------------------------------------------------------------- row-sliced fp8 reads
-// kv_read_fp8_rows (launch_kv_gather_fp8 with GatherLaunch::rows), plain or layered.  The
+// fp8 row reads (launch_kv_gather_fp8 with GatherLaunch::rows), plain or layered.  The
 // geometry is plan_gather_rows' and counts bytes of the part's bf16 view (part_bytes == rows *
 // src_pitch == 2 * elems); elems is a multiple of 512, and row_bytes, both pitches (with
 // slices > 1, dst_slice_pitch too), src_col, the part bases and the local offsets are multiples
@@ -541,11 +533,7 @@ inline LaunchPlan plan_gather_fp8(const GatherLaunch& a, uint32_t elems, int var
 // the occupancy API's answer for it).
 inline LaunchPlan plan_gather_fp8_rows(const GatherLaunch& a, uint32_t elems, int sms,
                                        LdStResident res) {
-    if (a.write || a.nparts == 0 || a.nparts > kGatherMaxParts ||
-        !row_geometry_ok(a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.slices,
-                         a.dst_slice_pitch, a.part_bytes, a.pieces) ||
-        (a.group_flags && (a.group_parts == 0 || a.nparts % a.group_parts != 0)))
-        return invalid_plan();
+    if (!rows_admitted(a, false)) return invalid_plan();
     const uint64_t geo_or = a.align_or | a.row_bytes | a.src_pitch | a.src_col | a.dst_pitch |
                             (a.slices > 1 ? a.dst_slice_pitch : 0u);
     if (elems == 0 || elems % 512 != 0 || uint64_t(a.part_bytes) != 2ull * elems ||

@@ -1741,10 +1741,12 @@ PYBIND11_MODULE(_infinistore, m) {
               a.n = n;
               a.nparts = nparts;
               a.part_bytes = part_bytes;
+              static uint32_t flags[1];
+              a.group_flags = flags;
               a.group_parts = group_parts;
               a.align_or = align_or;
               a.max_ctas = max_ctas;
-              return plan_dict(kernels::plan_gather_layered(a, sm_count, {resident16, resident32}));
+              return plan_dict(kernels::plan_gather(a, sm_count, {resident16, resident32}));
           },
           py::arg("n"), py::arg("nparts"), py::arg("part_bytes"), py::arg("group_parts") = 2,
           py::arg("align_or") = 0, py::arg("max_ctas") = 0, py::arg("sm_count") = 132,

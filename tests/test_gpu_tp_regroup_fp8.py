@@ -1,7 +1,7 @@
-"""Row-sliced reads of fp8 all-layer pages, on the H100: kv_read_fp8_rows (plain and layered)
-bit for bit against the whole-page fp8 read sliced by torch and against the exact e4m3
-reference of tests/fp8_exact.py, and the store's fp8 cross-TP reads in the Llama-3-8B layout
-against same-TP fp8 reads of the writers' pages, sliced by torch."""
+"""Row-sliced reads of fp8 all-layer pages, on the H100: kv_read_fp8_scatter<LAYERED, kRows>
+(plain and layered) bit for bit against the whole-page fp8 read sliced by torch and against
+the exact e4m3 reference of tests/fp8_exact.py, and the store's fp8 cross-TP reads in the
+Llama-3-8B layout against same-TP fp8 reads of the writers' pages, sliced by torch."""
 import numpy as np
 import pytest
 import torch
