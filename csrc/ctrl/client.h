@@ -28,16 +28,11 @@
 #include "../core/config.h"
 #include "../core/hash.h"
 #include "../fabric/segment.h"
+#include "../kernels/kernels.h"
 #include "../wire/protocol.h"
 
 namespace istore {
 
-namespace kernels {
-struct CopyDesc;
-struct IndexShards;
-struct LookupLaunch;
-struct GatherLaunch;
-}
 using kernels_CopyDesc = kernels::CopyDesc;
 using kernels_IndexShards = kernels::IndexShards;
 struct KeyBatch;
@@ -204,19 +199,14 @@ class Connection {
         // group_parts (which must divide nparts)
         ScatterReader* reader = nullptr;
         uint32_t group_parts = 0;
-        // row-sliced parts (kernels::GatherLaunch::rows, bytes of the caller's view of a part,
-        // view_part_bytes()); rows == 0: whole parts.  slices > 1: sliced rows
-        // (kernels::GatherLaunch::slices), e.g. a token's KV heads into a head-major page.  A
-        // write takes the geometry that reads the same local layout back, and its rows must
-        // fill the stored part (kernels::row_write_covers)
-        uint32_t rows = 0, row_bytes = 0, src_pitch = 0, src_col = 0, dst_pitch = 0;
-        uint32_t slices = 1, dst_slice_pitch = 0;
-        // pieces > 1 (with rows): block i's local layout is `pieces` runs of rows / pieces rows,
-        // run t at part_base[s] + the block's offset + piece_off[i * pieces + t], a host array
-        // in the units of the call's offsets (kernels::GatherLaunch::pieces) - e.g. a chunk of
-        // k engine pages under one key, each page where the caller's block table puts it
+        // row geometry (kernels::PartRows, in bytes of the caller's view of a part,
+        // view_part_bytes()); rows.rows == 0: whole parts.  A write's rows must fill the stored
+        // part (kernels::PartRows::covers)
+        kernels::PartRows rows;
+        // rows.pieces > 1: a host array of rows.pieces offsets per block, in the units of the
+        // call's offsets; run t of block i is at part_base[s] + the block's offset +
+        // piece_off[i * rows.pieces + t]
         const uint64_t* piece_off = nullptr;
-        uint32_t pieces = 1;
         // pool bytes of a part: part_bytes, or kernels::fp8_gather_bytes(1, fp8_elems)
         uint64_t pool_part_bytes() const;
         // bytes of a part in the caller's tensors: part_bytes, or 2 * fp8_elems (bf16)
@@ -233,7 +223,7 @@ class Connection {
         std::vector<RemoteBlock> blocks;  // blocks to write (the "already exists" ones dropped)
         std::vector<uint64_t> offsets;    // their local offsets (elements until the first call)
         std::vector<KeyHash> hashes;      // their key fingerprints from allocate
-        uint32_t pieces = 1;              // GatherSpec::pieces of every call
+        uint32_t pieces = 1;              // GatherSpec::rows.pieces of every call
         std::vector<uint64_t> piece_off;  // their piece tables, scaled as offsets
         bool indexed = true;              // every block has a fingerprint: it can be published
         uint32_t nparts = 0;              // S: parts of a block
@@ -271,7 +261,7 @@ class Connection {
     int w_rdma_gather(const GatherSpec& g, const uint64_t* offsets, size_t noffsets,
                       const RemoteBlock* blocks, size_t nblocks, int device, uint64_t stream);
     // A stored block must hold g.need_bytes() bytes, else it is a miss.  Row-sliced (g.rows):
-    // the geometry kernels::row_geometry_ok accepts for g.view_part_bytes() (launch_plan.h);
+    // the geometry kernels::PartRows::ok accepts for g.view_part_bytes();
     // fp8 parts also need row_bytes, both pitches, src_col and, with slices > 1,
     // dst_slice_pitch in multiples of 16 bytes (the rows are picked out of the part's bf16
     // view and dequantised).  With g.reader, a layered read: one call whose last page-mover launch

@@ -281,7 +281,7 @@ kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n,
     G.part_base = g.part_base;
     G.nparts = g.nparts;
     // a row-sliced read's geometry counts bytes of the caller's view of a part (bf16 for fp8)
-    G.part_bytes = uint32_t(g.rows ? g.view_part_bytes() : g.pool_part_bytes());
+    G.part_bytes = uint32_t(g.rows.rows ? g.view_part_bytes() : g.pool_part_bytes());
     G.first_part = g.first_part;
     G.align_or = align_or;
     for (uint32_t s = 0; s < g.nparts; ++s) G.align_or |= g.part_base[s];
@@ -289,14 +289,7 @@ kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n,
     G.max_ctas = max_ctas;
     G.stage_bytes = pipe_stage_;
     G.ring_bytes = pipe_ring_;
-    G.rows = g.rows;
-    G.row_bytes = g.row_bytes;
-    G.src_pitch = g.src_pitch;
-    G.src_col = g.src_col;
-    G.dst_pitch = g.dst_pitch;
-    G.slices = g.slices;
-    G.dst_slice_pitch = g.dst_slice_pitch;
-    G.pieces = g.pieces;  // the caller stages the piece table beside the descriptors
+    G.rows = g.rows;  // the caller stages the piece table beside the descriptors
     return G;
 }
 
@@ -305,11 +298,12 @@ kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n,
 // are adjacent in the stored row, so they count as one run of slices * row_bytes).  A
 // row-sliced write fills whole stored parts, so it counts them as the write without rows does.
 static uint64_t gather_moved_bytes(const Connection::GatherSpec& g, bool write) {
-    const uint64_t width = uint64_t(g.slices) * g.row_bytes;
-    const uint64_t part = !g.rows || write ? g.pool_part_bytes()
+    const kernels::PartRows& r = g.rows;
+    const uint64_t width = uint64_t(r.slices) * r.row_bytes;
+    const uint64_t part = !r.rows || write ? g.pool_part_bytes()
                           : g.fp8_elems
-                              ? fp8_rows_read_bytes(g.rows, uint32_t(width), g.src_pitch, g.src_col)
-                              : uint64_t(g.rows) * width;
+                              ? fp8_rows_read_bytes(r.rows, uint32_t(width), r.src_pitch, r.src_col)
+                              : uint64_t(r.rows) * width;
     return uint64_t(g.nparts) * part;
 }
 
@@ -347,11 +341,13 @@ static cudaError_t writer_state_alloc(void** p, size_t bytes, int device, cudaSt
 // Blocks per launch of a gathered call (staging.h: gather_max_blocks).  fp8 parts are counted
 // in bf16 bytes: the fp8 kernels cut a part into chunks of at least kFp8Chunk elements (16 KB
 // of bf16), or take it whole.
-// A piece table (GatherSpec::pieces) bounds it to the blocks whose tables fit kPieceRingBytes.
+// A piece table (GatherSpec::rows.pieces) bounds it to the blocks whose tables fit
+// kPieceRingBytes.
 static size_t gather_batch_cap(const Connection::GatherSpec& g) {
     const size_t cap =
         gather_max_blocks(kMaxBatch, g.nparts, g.fp8_elems ? 2 * g.fp8_elems : g.part_bytes);
-    return g.pieces > 1 ? std::min(cap, kPieceRingBytes / (sizeof(uint64_t) * g.pieces)) : cap;
+    const uint32_t k = g.rows.pieces;
+    return k > 1 ? std::min(cap, kPieceRingBytes / (sizeof(uint64_t) * k)) : cap;
 }
 
 // The blocks of blocks[base, ...) that the next launch stages (staging.h: key_batch) within
@@ -430,27 +426,27 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
                 uint8_t* pool = m->host_ptr + addr_off(blocks[i].remote_addr);
                 if (gather) {  // one memcpy per part, or per (row, slice) of a row-sliced call
                     const size_t pb = gather->pool_part_bytes();
-                    const Connection::GatherSpec& g = *gather;
+                    const kernels::PartRows& R = gather->rows;
                     for (uint32_t s = 0; s < gather->nparts; ++s) {
                         uint8_t* local =
                             reinterpret_cast<uint8_t*>(gather->part_base[s] + local_off[i] * scale);
-                        if (g.rows) {  // pieces: row r in piece r / piece_rows
-                            uint8_t* stored = pool + (g.first_part + s) * pb + g.src_col;
-                            const uint32_t pr = g.rows / g.pieces;
-                            for (uint32_t r = 0; r < g.rows; ++r)
-                                for (uint32_t j = 0; j < g.slices; ++j) {
-                                    const uint64_t piece =
-                                        g.pieces > 1 ? g.piece_off[i * g.pieces + r / pr] * scale
-                                                     : 0;
-                                    uint8_t* l = local + piece + size_t(r % pr) * g.dst_pitch +
-                                                 size_t(j) * g.dst_slice_pitch;
-                                    uint8_t* p = stored + size_t(r) * g.src_pitch +
-                                                 size_t(j) * g.row_bytes;
+                        if (R.rows) {  // as the kernels do: runs of rows of one slice and piece
+                            uint8_t* stored = pool + (gather->first_part + s) * pb;
+                            const uint32_t pr = R.rows / R.pieces;
+                            for (uint32_t q = 0; q < R.rows * R.slices; q += pr) {
+                                const kernels::PairOffsets o = R.pair(q, pr);
+                                uint8_t* l = local + o.dst;
+                                if (R.pieces > 1)
+                                    l += gather->piece_off[i * R.pieces + o.piece] * scale;
+                                for (uint32_t r = 0; r < pr; ++r) {
+                                    uint8_t* lr = l + size_t(r) * R.dst_pitch;
+                                    uint8_t* p = stored + o.src + size_t(r) * R.src_pitch;
                                     if (write)
-                                        std::memcpy(p, l, g.row_bytes);
+                                        std::memcpy(p, lr, R.row_bytes);
                                     else
-                                        std::memcpy(l, p, g.row_bytes);
+                                        std::memcpy(lr, p, R.row_bytes);
                                 }
+                            }
                         } else if (write)
                             std::memcpy(pool + (gather->first_part + s) * pb, local, pb);
                         else
@@ -544,7 +540,7 @@ int Connection::move_blocks(bool write, const uint64_t* local_off, uint64_t scal
             at_rec = ctx->ring_alloc(batch_cap * sizeof(kernels::IndexEntry));
             recs = reinterpret_cast<kernels::IndexEntry*>(ctx->ring_h + at_rec);
         }
-        const uint32_t k = gather ? gather->pieces : 1;  // piece table: one row per descriptor
+        const uint32_t k = gather ? gather->rows.pieces : 1;  // piece table: one row per descriptor
         size_t at_piece = 0;
         uint64_t* pieces = nullptr;
         if (k > 1) {
@@ -901,26 +897,22 @@ const char* Connection::gather_refusal(const GatherSpec& g, const uint64_t* offs
     if (end > block_parts) return "the part range runs past the block";
     if (block_parts > uint64_t(INT32_MAX) / g.pool_part_bytes())
         return "bad parts list: a block holds at most 2^31 - 1 bytes";
-    if (g.pieces == 0 || (g.pieces > 1 && (!g.rows || !g.piece_off)))
+    const kernels::PartRows& r = g.rows;
+    if (r.pieces == 0 || (r.pieces > 1 && (!r.rows || !g.piece_off)))
         return "bad pieces: pieces >= 1, and pieces > 1 need row geometry and a piece table";
-    if (g.pieces > 1 && g.rows % g.pieces)
+    if (r.pieces > 1 && r.rows % r.pieces)
         return "bad pieces: the piece count must divide the rows";
-    if (uint64_t(g.pieces) * sizeof(uint64_t) > kPieceRingBytes)
+    if (uint64_t(r.pieces) * sizeof(uint64_t) > kPieceRingBytes)
         return "bad pieces: one block's piece table does not fit the staging ring";
-    if (g.rows && !kernels::row_geometry_ok(g.rows, g.row_bytes, g.src_pitch, g.src_col,
-                                            g.dst_pitch, g.slices, g.dst_slice_pitch,
-                                            g.view_part_bytes(), g.pieces))
+    if (r.rows && !r.ok(g.view_part_bytes()))
         return "bad row geometry (rows >= 1, slices >= 1, src_col + slices * row_bytes <= "
                "src_pitch, part_bytes == rows * src_pitch; with slices > 1, disjoint local "
                "slices within 2^32 bytes; with pieces, per piece)";
     // the in-band commit publishes whole blocks: a write fills every byte of a stored part
-    if (g.rows && write &&
-        !kernels::row_write_covers(g.row_bytes, g.src_pitch, g.src_col, g.slices))
+    if (r.rows && write && !r.covers())
         return "bad row geometry for a write: the rows must fill the stored part (src_col == 0, "
                "slices * row_bytes == src_pitch)";
-    if (g.rows && g.fp8_elems &&
-        ((g.row_bytes | g.src_pitch | g.src_col | g.dst_pitch |
-          (g.slices > 1 ? g.dst_slice_pitch : 0u)) & 15))
+    if (r.rows && g.fp8_elems && (r.align_or() & 15))
         return "bad row geometry for fp8 parts: row_bytes, src_pitch, src_col, dst_pitch and "
                "dst_slice_pitch must be multiples of 16 bytes (8 bf16 elements)";
     if (g.reader) {
@@ -935,8 +927,8 @@ const char* Connection::gather_refusal(const GatherSpec& g, const uint64_t* offs
         uint64_t align_or = 0;
         for (uint32_t s = 0; s < g.nparts; ++s) align_or |= g.part_base[s];
         for (size_t i = 0; i < n; ++i) align_or |= offs[i];
-        if (g.pieces > 1)
-            for (size_t i = 0; i < n * g.pieces; ++i) align_or |= g.piece_off[i];
+        if (r.pieces > 1)
+            for (size_t i = 0; i < n * r.pieces; ++i) align_or |= g.piece_off[i];
         if (align_or & 15)
             return "fp8 parts need 16-byte aligned part bases, offsets and piece offsets";
     }
@@ -1050,9 +1042,9 @@ int Connection::write_layered(GatherWriter& w, const GatherSpec& g, uint64_t sca
     }
     const std::vector<uint64_t>& offs = first ? scaled : w.offsets;
     GatherSpec gp = g;  // the writer's piece table goes with every call
-    if (!bad && (g.pieces != 1 || g.piece_off))
+    if (!bad && (g.rows.pieces != 1 || g.piece_off))
         bad = "a layered writer takes its pieces when it is made";
-    gp.pieces = w.pieces;
+    gp.rows.pieces = w.pieces;
     gp.piece_off = w.pieces > 1 ? (first ? scaled_pieces : w.piece_off).data() : nullptr;
     if (!bad) bad = gather_refusal(gp, offs.data(), offs.size(), device, true, &w);
     for (uint64_t s = g.first_part; !bad && s < end; ++s)
@@ -1151,7 +1143,7 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
                         .fp8_elems = uint32_t(fp8_elems), .gather = gather != nullptr,
                         .copy_variant = copy_variant_, .all_local = true, .all_remote = true,
                         .max_ctas = max_ctas_, .sm_count = kernels::sm_count(),
-                        .layered = layered, .rows = gather && gather->rows};
+                        .layered = layered, .rows = gather && gather->rows.rows};
         // over every known segment, not only the ones this batch touches: intentional
         for (uint32_t s = 0; s < R.nsegs; ++s) {
             in.all_remote = in.all_remote && ctx->seg_remote[s];
@@ -1159,7 +1151,7 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
         }
         uint64_t align_or = base_ptr;
         for (size_t i = 0; i < n; ++i) align_or |= blocks[base + i].offset;
-        const uint32_t k = gather ? gather->pieces : 1;  // piece table, beside the keys
+        const uint32_t k = gather ? gather->rows.pieces : 1;  // piece table, beside the keys
         const uint64_t* pieces_d = nullptr;
         if (k > 1) {
             const size_t at = ctx->ring_alloc(n * k * sizeof(uint64_t));
@@ -1262,8 +1254,8 @@ int Connection::read_via_device_index(const std::vector<KeyOffset>& blocks, int 
         stats_.ns_build += t_launch0 - t_build0;
         stats_.ns_launch += now_ns() - t_launch0;
         // lookup + copy + validate: resolve_descs counted the lookup
-        const uint64_t moved = gather && gather->rows ? gather_moved_bytes(*gather, false)
-                                                      : uint64_t(block_size);
+        const uint64_t moved = gather && gather->rows.rows ? gather_moved_bytes(*gather, false)
+                                                           : uint64_t(block_size);
         if (scope.launched(e, "device-index read failed to launch: ", plan.fused() ? 1 : 2, false,
                            uint64_t(n) * moved) != 0)
             return -1;

@@ -23,8 +23,8 @@ inline constexpr size_t kRingBytes = 16u << 20;     // pinned, mapped staging ri
 inline constexpr size_t kScratchBytes = 8u << 20;   // device scratch per device
 inline constexpr size_t kZeroBytes = 2u << 20;      // self-cleaning zeroed counters per device
 inline constexpr size_t kMaxBatch = 65536;          // blocks per kernel launch
-// ring bytes one launch's piece tables may take (GatherSpec::pieces): with a key batch's half
-// of the ring, a launch's placements still never come round to each other
+// ring bytes one launch's piece tables may take (GatherSpec::rows.pieces): with a key batch's
+// half of the ring, a launch's placements still never come round to each other
 inline constexpr size_t kPieceRingBytes = kRingBytes / 4;
 inline constexpr int kReaderSlots = 64;             // layered reads in flight per device
 

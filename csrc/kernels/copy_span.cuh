@@ -77,22 +77,16 @@ __device__ __forceinline__ void copy_span(uint8_t* dst, const uint8_t* src, uint
 }
 
 // A row-sliced write (GatherLaunch::rows with write): stored bytes [off, off + len) of a part
-// to dst (the pool, contiguous), each loaded from the caller's part `src` at row_write_offset
-// (launch_plan.h) of its stored offset.  copy_span's shape: VEC = 16 / 32 keep four / eight
-// 16-byte vectors in flight per thread (row_bytes, dst_pitch, slice_pitch, off, len and both
-// bases aligned to 16; a vector never straddles two slices); VEC = 1: bytes.
-struct RowWrite {
-    uint32_t row_bytes, src_pitch, dst_pitch, slice_pitch;
-};
+// to dst (the pool, contiguous), each loaded from the caller's part `src` at g.write_offset of
+// its stored offset.  copy_span's shape: VEC = 16 / 32 keep four / eight 16-byte vectors in
+// flight per thread (row_bytes, dst_pitch, dst_slice_pitch, off, len and both bases aligned to
+// 16; a vector never straddles two slices); VEC = 1: bytes.
 template <int VEC>
 __device__ __forceinline__ void copy_span_rows(uint8_t* dst, const uint8_t* src, uint32_t off,
-                                               uint32_t len, const RowWrite& w) {
+                                               uint32_t len, const PartRows& g) {
     const uint32_t tid = threadIdx.x;
-    const auto at = [&](uint32_t o) {
-        return row_write_offset(o, w.row_bytes, w.src_pitch, w.dst_pitch, w.slice_pitch);
-    };
     if constexpr (VEC == 1) {
-        for (uint32_t b = tid; b < len; b += kLdStThreads) dst[b] = src[at(off + b)];
+        for (uint32_t b = tid; b < len; b += kLdStThreads) dst[b] = src[g.write_offset(off + b)];
     } else {
         static_assert(VEC == 16 || VEC == 32, "vector width");
         constexpr int U = VEC / 4;
@@ -102,38 +96,35 @@ __device__ __forceinline__ void copy_span_rows(uint8_t* dst, const uint8_t* src,
             uint4 v[U];
 #pragma unroll
             for (int u = 0; u < U; ++u) {
-                const uint8_t* s = src + at(off + (i + u * kLdStThreads) * 16);
+                const uint8_t* s = src + g.write_offset(off + (i + u * kLdStThreads) * 16);
                 v[u] = VEC == 16 ? ld_stream_v4(s) : ld_v4(s);
             }
 #pragma unroll
             for (int u = 0; u < U; ++u) st_v4(dst + size_t(i + u * kLdStThreads) * 16, v[u]);
         }
         for (; i < nvec; i += kLdStThreads)
-            st_v4(dst + size_t(i) * 16, ld_stream_v4(src + at(off + i * 16)));
+            st_v4(dst + size_t(i) * 16, ld_stream_v4(src + g.write_offset(off + i * 16)));
     }
 }
 
-// `nrows` rows of row_bytes, row r from src + r * src_pitch to dst + r * dst_pitch.  The 256
-// threads walk the (row, vector) pairs flattened together, so rows much narrower than a CTA's
-// 4 KB per pass (one KV head of 128 bf16 is 256 bytes) still keep every thread busy.  VEC = 16
-// / 32 as for copy_span (row_bytes, both pitches and both bases aligned to VEC); VEC = 1: bytes.
-// SLICED (GatherLaunch::slices > 1): src and dst are the part's stored start and destination,
-// and the nrows units are the (slice, row) pairs sl.q0 .. sl.q0 + nrows - 1 of the part, each
-// placed by slice_pair (launch_plan.h): the threads walk (slice, row, vector) triples flattened
-// together (sl.slice_pitch aligned to VEC as well).
-struct RowSlices {
-    uint32_t q0, rows, src_col, slice_pitch;
-};
+// `nrows` rows of g.row_bytes, row r from src + r * g.src_pitch to dst + r * g.dst_pitch.  The
+// 256 threads walk the (row, vector) pairs flattened together, so rows much narrower than a
+// CTA's 4 KB per pass (one KV head of 128 bf16 is 256 bytes) still keep every thread busy.
+// VEC = 16 / 32 as for copy_span (row_bytes, both pitches and both bases aligned to VEC);
+// VEC = 1: bytes.
+// SLICED (GatherLaunch::rows.slices > 1): src and dst are the part's stored start and
+// destination, and the nrows units are the (slice, row) pairs q0 .. q0 + nrows - 1 of the part,
+// each placed by g.pair: the threads walk (slice, row, vector) triples flattened together
+// (dst_slice_pitch aligned to VEC as well).
 template <int VEC, bool SLICED = false>
 __device__ __forceinline__ void copy_rows(uint8_t* dst, const uint8_t* src, uint32_t nrows,
-                                          uint32_t row_bytes, uint32_t src_pitch,
-                                          uint32_t dst_pitch, RowSlices sl = {}) {
+                                          const PartRows& g, uint32_t q0 = 0) {
     const uint32_t tid = threadIdx.x;
+    const uint32_t row_bytes = g.row_bytes;
     if constexpr (SLICED) {
         // pair p of the run: offsets of its byte c from src and dst
         const auto at = [&](uint32_t p, uint32_t c) {
-            PairOffsets o = slice_pair(sl.q0 + p, sl.rows, row_bytes, src_pitch, sl.src_col,
-                                       dst_pitch, sl.slice_pitch);
+            PairOffsets o = g.pair(q0 + p);
             o.src += c;
             o.dst += c;
             return o;
@@ -176,7 +167,7 @@ __device__ __forceinline__ void copy_rows(uint8_t* dst, const uint8_t* src, uint
         const uint32_t len = nrows * row_bytes;
         for (uint32_t b = tid; b < len; b += kLdStThreads) {
             const uint32_t r = b / row_bytes, c = b - r * row_bytes;
-            dst[size_t(r) * dst_pitch + c] = src[size_t(r) * src_pitch + c];
+            dst[size_t(r) * g.dst_pitch + c] = src[size_t(r) * g.src_pitch + c];
         }
     } else {
         static_assert(VEC == 16 || VEC == 32, "vector width");
@@ -192,14 +183,14 @@ __device__ __forceinline__ void copy_rows(uint8_t* dst, const uint8_t* src, uint
             uint4 v[U];
 #pragma unroll
             for (int u = 0; u < U; ++u) {
-                const uint8_t* s = src + at(i + u * kLdStThreads, src_pitch);
+                const uint8_t* s = src + at(i + u * kLdStThreads, g.src_pitch);
                 v[u] = VEC == 16 ? ld_stream_v4(s) : ld_v4(s);
             }
 #pragma unroll
-            for (int u = 0; u < U; ++u) st_v4(dst + at(i + u * kLdStThreads, dst_pitch), v[u]);
+            for (int u = 0; u < U; ++u) st_v4(dst + at(i + u * kLdStThreads, g.dst_pitch), v[u]);
         }
         for (; i < nvec; i += kLdStThreads)
-            st_v4(dst + at(i, dst_pitch), ld_stream_v4(src + at(i, src_pitch)));
+            st_v4(dst + at(i, g.dst_pitch), ld_stream_v4(src + at(i, g.src_pitch)));
     }
 }
 

@@ -17,7 +17,7 @@
 
 namespace istore::kernels {
 
-// How a gathered launch lays out each part (GatherLaunch::rows, ::slices, ::pieces).
+// How a gathered launch lays out each part (GatherLaunch::rows: PartRows).
 enum class PartShape { kWhole, kRows, kSlices, kPieces };
 
 // Calls go with the launch's shape as a compile-time constant.  Writes have no sliced body:
@@ -25,10 +25,10 @@ enum class PartShape { kWhole, kRows, kSlices, kPieces };
 template <bool WRITE, typename Go>
 cudaError_t with_shape(const GatherLaunch& a, Go&& go) {
     using S = PartShape;
-    if (!a.rows) return go(std::integral_constant<S, S::kWhole>{});
-    if (a.pieces > 1) return go(std::integral_constant<S, S::kPieces>{});
+    if (!a.rows.rows) return go(std::integral_constant<S, S::kWhole>{});
+    if (a.rows.pieces > 1) return go(std::integral_constant<S, S::kPieces>{});
     if constexpr (!WRITE)
-        if (a.slices > 1) return go(std::integral_constant<S, S::kSlices>{});
+        if (a.rows.slices > 1) return go(std::integral_constant<S, S::kSlices>{});
     return go(std::integral_constant<S, S::kRows>{});
 }
 

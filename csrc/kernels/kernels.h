@@ -14,6 +14,12 @@
 
 namespace istore::kernels {
 
+#if defined(__CUDACC__)
+#define ISTORE_KHD __host__ __device__
+#else
+#define ISTORE_KHD
+#endif
+
 // One block to move: absolute, device-addressable source and destination.  For a write
 // `dst` is a peer-mapped pool address, for a read `src` is.  src == 0 marks a block the
 // device lookup did not find: it is skipped and counted in status[kStatMiss].
@@ -139,6 +145,101 @@ cudaError_t launch_kv_pipe_copy(const CopyLaunch& a, cudaStream_t stream);
 // chunk never crosses a part and the in-band commit (publish.cuh) counts nparts * cpp
 // arrivals per block.  The part bases travel in the kernel parameters.
 constexpr uint32_t kGatherMaxParts = 256;
+
+// Where a (slice, row) pair or a stored byte of a PartRows geometry lies: `src` in the stored
+// part, `dst` from the start of its piece of the caller's part, and which piece that is (0
+// without pieces).
+struct PairOffsets {
+    uint32_t src, dst, piece;
+};
+
+// The row geometry of a gathered launch (GatherLaunch::rows, the connection's
+// GatherSpec::rows), in bytes of the caller's view of a part (part_bytes; bf16 for fp8 parts).
+// rows == 0: whole contiguous parts, and the other fields are not read.
+//   Rows: the reader's share of stored part s is `rows` rows of row_bytes at a pitch of
+//   src_pitch, src_col bytes into each row (part_bytes == rows * src_pitch), and row r lands at
+//   part_base[s] + desc.dst + r * dst_pitch - e.g. a decode rank's KV heads of a page that a
+//   prefill rank at another tensor-parallel degree wrote.
+//   Slices (slices > 1): each stored row holds `slices` slices of row_bytes side by side from
+//   src_col, and slice j of row r lands at r * dst_pitch + j * dst_slice_pitch - e.g. a
+//   token's KV heads into a head-major page [head][token][dim].  slices == 1: dst_slice_pitch
+//   is not read.
+//   Pieces (pieces > 1): block i's local layout is `pieces` runs of piece_rows = rows / pieces
+//   rows, run t at the descriptor's local offset + piece_off[i * pieces + t] - e.g. a chunk of
+//   k engine pages stored under one key, each page where the caller's block table puts it.
+// A write takes the geometry that reads the same local layout back: slice j of stored row r is
+// loaded from r * dst_pitch + j * dst_slice_pitch of the caller's part (covers()).
+struct PartRows {
+    uint32_t rows = 0, row_bytes = 0, src_pitch = 0, src_col = 0, dst_pitch = 0;
+    uint32_t slices = 1, dst_slice_pitch = 0, pieces = 1;
+
+    // The geometry as the connection (Connection::gather_refusal) and the row plans accept it:
+    // the row's slices lie inside the stored row, the rows cover the part, and with slices > 1
+    // the destination rectangles are disjoint under one of two nestings - head-major (a
+    // slice's rows inside dst_slice_pitch) or token-major (a row's slices inside dst_pitch) -
+    // and the destination extent, (rows - 1) * dst_pitch + (slices - 1) * dst_slice_pitch +
+    // row_bytes, fits 32 bits.  With pieces > 1 the nesting and the 32-bit extent hold per
+    // piece (piece_rows rows) rather than over all rows, and pieces must divide rows.
+    bool ok(uint64_t part_bytes) const {
+        if (rows == 0 || row_bytes == 0 || slices == 0 || pieces == 0 || rows % pieces != 0 ||
+            uint64_t(src_col) + uint64_t(slices) * row_bytes > src_pitch ||
+            uint64_t(rows) * src_pitch != part_bytes)
+            return false;
+        const uint64_t rb = row_bytes, r1 = rows / pieces - 1, s1 = slices - 1;
+        if (slices == 1) return pieces == 1 || r1 * dst_pitch + rb <= 0xffffffffull;
+        const bool head_major = dst_pitch >= rb && dst_slice_pitch >= r1 * dst_pitch + rb;
+        const bool token_major = dst_slice_pitch >= rb && dst_pitch >= s1 * dst_slice_pitch + rb;
+        return (head_major || token_major) &&
+               r1 * dst_pitch + s1 * dst_slice_pitch + rb <= 0xffffffffull;
+    }
+
+    // A write's rows must fill every byte of the stored part, because the in-band commit
+    // publishes whole blocks: on top of ok(), src_col == 0 and slices * row_bytes == src_pitch.
+    bool covers() const { return src_col == 0 && uint64_t(slices) * row_bytes == src_pitch; }
+
+    // The OR of every geometry value that offsets a vector: with the part bases and local
+    // offsets, it decides the vector width (launch_plan.h) and the fp8 kernels' 16-byte rule.
+    uint32_t align_or() const {
+        return row_bytes | src_pitch | src_col | dst_pitch | (slices > 1 ? dst_slice_pitch : 0u);
+    }
+
+    // Where (slice, row) pair q of a part goes.  Pairs are numbered slice-major (q = j * rows +
+    // r), so a run of pairs of a head-major destination writes contiguous bytes.  Slice j of row
+    // r moves row_bytes from r * src_pitch + src_col + j * row_bytes of the stored part to
+    // r * dst_pitch + j * dst_slice_pitch of the part's destination.  Units are the caller's:
+    // bytes, or for the fp8 reads elements of the bf16 view on the source side and bytes on the
+    // destination side.  ok() keeps both offsets within 32 bits once slices > 1 or pieces > 1.
+    ISTORE_KHD PairOffsets pair(uint32_t q) const {
+        const uint32_t j = q / rows, r = q - j * rows;
+        return PairOffsets{r * src_pitch + src_col + j * row_bytes,
+                           r * dst_pitch + j * dst_slice_pitch, 0};
+    }
+    // The same with pieces of piece_rows (rows / pieces) rows: row r is in piece r / piece_rows
+    // and lands at its row r % piece_rows.  Pairs q with the same q / piece_rows share their
+    // slice and their piece, so the kernels copy each such run as plain rows from the place
+    // this gives its first pair, loading its piece offset once.
+    ISTORE_KHD PairOffsets pair(uint32_t q, uint32_t piece_rows) const {
+        const uint32_t j = q / rows, r = q - j * rows, t = r / piece_rows;
+        return PairOffsets{r * src_pitch + src_col + j * row_bytes,
+                           (r - t * piece_rows) * dst_pitch + j * dst_slice_pitch, t};
+    }
+
+    // Where byte o of a covered stored part comes from in the caller's part: row r =
+    // o / src_pitch, slice j of it, column c - j * row_bytes of that slice.  Over a covering
+    // geometry it is the inverse of pair(): write_offset(pair(q).src + w) == pair(q).dst + w
+    // for every byte w < row_bytes.
+    ISTORE_KHD uint32_t write_offset(uint32_t o) const {
+        const uint32_t r = o / src_pitch, c = o - r * src_pitch, j = c / row_bytes;
+        return r * dst_pitch + j * dst_slice_pitch + (c - j * row_bytes);
+    }
+    // The same with pieces of piece_rows rows: byte o is in piece o / (piece_rows * src_pitch),
+    // and {o, its offset in that piece, the piece} is the inverse of pair(q, piece_rows).
+    ISTORE_KHD PairOffsets write_offset(uint32_t o, uint32_t piece_rows) const {
+        const uint32_t piece_bytes = piece_rows * src_pitch, t = o / piece_bytes;
+        return PairOffsets{o, write_offset(o - t * piece_bytes), t};
+    }
+};
+
 struct GatherLaunch {
     // per block, device-addressable: write {local byte offset, pool address},
     // read {pool address or 0 = miss, local byte offset}
@@ -180,36 +281,13 @@ struct GatherLaunch {
     uint32_t* group_counters = nullptr;
     uint32_t group_seq = 0;
     uint32_t group_parts = 0;
-    // Row-sliced read (reads only, ld/st kernels only; rows == 0: whole contiguous parts): the
-    // reader's share of stored part s is `rows` rows of row_bytes at a pitch of src_pitch,
-    // src_col bytes into each row (part_bytes == rows * src_pitch), and row r lands at
-    // part_base[s] + desc.dst + r * dst_pitch - e.g. a decode rank's KV heads of a page that
-    // a prefill rank at another tensor-parallel degree wrote.  Works with group_flags.
-    uint32_t rows = 0;
-    uint32_t row_bytes = 0;
-    uint32_t src_pitch = 0;
-    uint32_t src_col = 0;
-    uint32_t dst_pitch = 0;
-    // Sliced rows (slices > 1): each stored row holds `slices` slices of row_bytes side by side
-    // from src_col, and slice j of row r lands at part_base[s] + desc.dst + r * dst_pitch +
-    // j * dst_slice_pitch - e.g. a token's KV heads into a head-major page [head][token][dim]
-    // (launch_plan.h: slice_pair, row_geometry_ok).  slices == 1: the rows above, and
-    // dst_slice_pitch is not read.
-    // With write, the same geometry runs the other way (ld/st kernels only, no layered read):
-    // slice j of stored row r is taken from part_base[s] + desc.src + r * dst_pitch + j *
-    // dst_slice_pitch, and the rows must fill the stored part (src_col == 0, slices *
-    // row_bytes == src_pitch; launch_plan.h: row_write_covers, row_write_offset) - e.g. a
-    // head-major page stored token-major.  Works with recs and a layered writer's layer_state.
-    uint32_t slices = 1;
-    uint32_t dst_slice_pitch = 0;
-    // Pieces (with rows, reads and writes; pieces == 1: one local offset per block, desc's):
-    // block i's local layout is `pieces` runs of rows / pieces rows, run t at part_base[s] +
-    // the descriptor's local offset + piece_off[i * pieces + t] (device-addressable byte
-    // offsets, one table row per descriptor) - e.g. a chunk of k engine pages stored under one
-    // key, each page where the caller's block table puts it (launch_plan.h: piece_pair,
-    // piece_write_offset).  align_or covers every piece offset.
+    // Row geometry (PartRows; rows.rows == 0: whole contiguous parts).  Ld/st kernels only.
+    // Reads work with group_flags; writes (e.g. a head-major page stored token-major) with
+    // recs and a layered writer's layer_state.
+    PartRows rows;
+    // rows.pieces > 1: device-addressable byte offsets, one row of rows.pieces per descriptor.
+    // align_or covers every piece offset.
     const uint64_t* piece_off = nullptr;
-    uint32_t pieces = 1;
 };
 // The TMA pipeline for 16-byte aligned parts of at least kPipeMinBytes, the ld/st kernel
 // (kv_copy.cu) otherwise: the same rule launch_kv_copy applies to whole blocks.  Reads run
@@ -443,11 +521,6 @@ cudaError_t launch_kv_read_when_ready(const ReadyLaunch& a, cudaStream_t stream)
 // ---------------------------------------------------------------- doorbell worker (kv_doorbell.cu)
 // One persistent CTA that serves single-block writes / reads posted into a ring in pinned
 // host memory: no launch, no event, no stream poll on the caller's path.
-#if defined(__CUDACC__)
-#define ISTORE_KHD __host__ __device__
-#else
-#define ISTORE_KHD
-#endif
 constexpr int kDoorbellMaxSlots = 64;
 constexpr uint32_t kDoorbellMaxBytes = 256u << 10;  // larger blocks want more than one CTA
 constexpr uint64_t kDoorbellMagic = 0x646f6f7262656c6cull;

@@ -92,8 +92,8 @@ __global__ void __launch_bounds__(kLdStThreads + 32)
 // The launch's part geometry, every shape's fields in one kernel parameter (GatherLaunch):
 // each body reads the fields of its own shape.
 struct PartGeometry {
-    uint32_t part_bytes, rows, row_bytes, src_pitch, src_col, dst_pitch, slices, slice_pitch,
-        pieces;
+    uint32_t part_bytes;
+    PartRows rows;
     const uint64_t* piece_off;
 };
 
@@ -103,12 +103,12 @@ struct PartGeometry {
 //   kWhole   bytes [c * chunk, +chunk) of the part (copy_span);
 //   kRows    rows [c * chunk, +chunk) (GatherLaunch::rows): row r from r * src_pitch + src_col
 //            (row_bytes) to r * dst_pitch (copy_rows);
-//   kSlices  (slice, row) pairs [c * chunk, +chunk) of the part (GatherLaunch::slices > 1),
-//            numbered slice-major, each placed by slice_pair (launch_plan.h: copy_rows<VEC, true>);
-//   kPieces  the same pairs (GatherLaunch::pieces > 1, any slices), cut where q / piece_rows
-//            changes; each cut, one slice's rows inside one piece, is copied as plain rows to
-//            desc.dst + piece_off[block * pieces + t] + the place piece_pair gives its first pair
-//            - one piece-offset load per cut.
+//   kSlices  (slice, row) pairs [c * chunk, +chunk) of the part (rows.slices > 1), numbered
+//            slice-major, each placed by PartRows::pair (copy_rows<VEC, true>);
+//   kPieces  the same pairs (rows.pieces > 1, any slices), cut where q / piece_rows changes;
+//            each cut, one slice's rows inside one piece, is copied as plain rows to desc.dst +
+//            piece_off[block * pieces + t] + the place PartRows::pair gives its first pair - one
+//            piece-offset load per cut.
 // No control warp: reads publish nothing.  The minimum of 3 CTAs per SM holds every flavour to
 // 80 registers, which the 32-byte row reads use.
 template <int VEC, bool LAYERED, PartShape S>
@@ -133,24 +133,21 @@ __global__ void __launch_bounds__(kLdStThreads, 3)
             }
         } else if constexpr (S == PartShape::kRows) {
             const uint32_t r0 = it.chunk * chunk;
-            copy_rows<VEC>(at(dst + uint64_t(r0) * g.dst_pitch),
-                           at(src + uint64_t(r0) * g.src_pitch + g.src_col),
-                           min(chunk, g.rows - r0), g.row_bytes, g.src_pitch, g.dst_pitch);
+            copy_rows<VEC>(at(dst + uint64_t(r0) * g.rows.dst_pitch),
+                           at(src + uint64_t(r0) * g.rows.src_pitch + g.rows.src_col),
+                           min(chunk, g.rows.rows - r0), g.rows);
         } else if constexpr (S == PartShape::kSlices) {
             const uint32_t q0 = it.chunk * chunk;
-            copy_rows<VEC, true>(at(dst), at(src), min(chunk, g.rows * g.slices - q0), g.row_bytes,
-                                 g.src_pitch, g.dst_pitch,
-                                 RowSlices{q0, g.rows, g.src_col, g.slice_pitch});
+            copy_rows<VEC, true>(at(dst), at(src), min(chunk, g.rows.rows * g.rows.slices - q0),
+                                 g.rows, q0);
         } else {
-            const uint32_t piece_rows = g.rows / g.pieces;
-            const uint32_t q0 = it.chunk * chunk, q1 = min(q0 + chunk, g.rows * g.slices);
-            const uint64_t* off = g.piece_off + uint64_t(it.block) * g.pieces;
+            const uint32_t piece_rows = g.rows.rows / g.rows.pieces;
+            const uint32_t q0 = it.chunk * chunk, q1 = min(q0 + chunk, g.rows.rows * g.rows.slices);
+            const uint64_t* off = g.piece_off + uint64_t(it.block) * g.rows.pieces;
             for (uint32_t q = q0; q < q1;) {
                 const uint32_t e = min(q1, (q / piece_rows + 1) * piece_rows);
-                const PieceOffsets o = piece_pair(q, g.rows, g.row_bytes, g.src_pitch, g.src_col,
-                                                  g.dst_pitch, g.slice_pitch, piece_rows);
-                copy_rows<VEC>(at(dst + off[o.piece] + o.dst), at(src + o.src), e - q,
-                               g.row_bytes, g.src_pitch, g.dst_pitch);
+                const PairOffsets o = g.rows.pair(q, piece_rows);
+                copy_rows<VEC>(at(dst + off[o.piece] + o.dst), at(src + o.src), e - q, g.rows);
                 q = e;
             }
         }
@@ -161,12 +158,12 @@ __global__ void __launch_bounds__(kLdStThreads, 3)
 // bytes [off, off + len) of pool part first_part + s of desc.dst, each loaded from local
 // parts.base[s] + desc.src:
 //   kWhole   at the same offset (copy_span);
-//   kRows    at row_write_offset of its stored offset (GatherLaunch::rows with write, any
+//   kRows    at PartRows::write_offset of its stored offset (GatherLaunch::rows with write, any
 //            slices: copy_span_rows), so every item still stores one contiguous run of pool
 //            bytes and the commit counts arrivals as for whole parts;
 //   kPieces  the same, with the item's stored bytes cut at piece boundaries (piece_rows *
 //            src_pitch bytes) and each cut loaded from desc.src + piece_off[block * pieces + t]
-//            (piece_write_offset's geometry) - one piece-offset load per cut.
+//            - one piece-offset load per cut.
 // The minimum of 3 CTAs per SM lets the 32-byte flavour keep 64 registers; without it ptxas
 // held it to 56 and spilled.
 template <int VEC, PartShape S>
@@ -183,7 +180,6 @@ __global__ void __launch_bounds__(kLdStThreads + 32, 3)
             reinterpret_cast<uint8_t*>(d.dst + uint64_t(first_part + s) * g.part_bytes + off);
         const uint64_t src = parts.base[s] + d.src;
         const auto at = [](uint64_t a) { return reinterpret_cast<const uint8_t*>(a); };
-        const RowWrite w{g.row_bytes, g.src_pitch, g.dst_pitch, g.slice_pitch};
         if constexpr (S == PartShape::kWhole) {
             if constexpr (VEC == 1) {
                 for (uint32_t b = threadIdx.x; b < len; b += kLdStThreads)
@@ -192,15 +188,15 @@ __global__ void __launch_bounds__(kLdStThreads + 32, 3)
                 copy_span<VEC>(dst, at(src + off), len);
             }
         } else if constexpr (S == PartShape::kRows) {
-            copy_span_rows<VEC>(dst, at(src), off, len, w);
+            copy_span_rows<VEC>(dst, at(src), off, len, g.rows);
         } else {
-            const uint32_t piece_bytes = g.part_bytes / g.pieces;
-            const uint64_t* poff = g.piece_off + uint64_t(block) * g.pieces;
+            const uint32_t piece_bytes = g.part_bytes / g.rows.pieces;
+            const uint64_t* poff = g.piece_off + uint64_t(block) * g.rows.pieces;
             for (uint32_t o = off; o < off + len;) {
                 const uint32_t t = o / piece_bytes;
                 const uint32_t e = min(off + len, (t + 1) * piece_bytes);
                 copy_span_rows<VEC>(dst + (o - off), at(src + poff[t]), o - t * piece_bytes,
-                                    e - o, w);
+                                    e - o, g.rows);
                 o = e;
             }
         }
@@ -307,10 +303,9 @@ cudaError_t launch_kv_gather(const GatherLaunch& a, cudaStream_t stream) {
     const bool layered = a.group_flags != nullptr;
     if (layered && !a.group_counters) return cudaErrorInvalidValue;
     // pieces split rows, at the offsets of the piece table
-    if (a.pieces != 1 && (!a.rows || !a.piece_off)) return cudaErrorInvalidValue;
+    if (a.rows.pieces != 1 && (!a.rows.rows || !a.piece_off)) return cudaErrorInvalidValue;
     const GatherParts parts = parts_of(a);
-    const PartGeometry g{a.part_bytes, a.rows,  a.row_bytes,       a.src_pitch, a.src_col,
-                         a.dst_pitch,  a.slices, a.dst_slice_pitch, a.pieces,    a.piece_off};
+    const PartGeometry g{a.part_bytes, a.rows, a.piece_off};
     if (a.write)
         return with_shape<true>(a, [&](auto s) {
             return launch_ldst_gather<true, false, decltype(s)::value>(a, parts, g, stream);

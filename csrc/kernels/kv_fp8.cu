@@ -12,8 +12,8 @@
 //                  shape.  With row geometry (GatherLaunch::rows) a read dequantises rows (and
 //                  slices) of each stored page, a write quantises a stored page whose rows are
 //                  loaded from a strided local layout (e.g. a head-major page); with
-//                  GatherLaunch::pieces > 1 each block's rows are in runs at the offsets of its
-//                  row of the piece table.  Reads walk their items in gather_items.cuh
+//                  rows.pieces > 1 each block's rows are in runs at the offsets of its row of
+//                  the piece table.  Reads walk their items in gather_items.cuh
 //                  (scatter_items), writes in write_fp8 below.
 // The reference moves raw bytes only (dtype-agnostic, infinistore/lib.py:377-379); this is
 // the "write fused with fp8 cast / read fused with gather" item of the north star.
@@ -71,11 +71,11 @@ __device__ __forceinline__ uint4 ld_u4(const void* p) {
 // elements 8 * hl .. 8 * hl + 7 of 128-element row `row` of the stored page.  A template
 // policy rather than a runtime branch, so the existing kernels' loop is compiled as before.
 //   DenseRows  the page is contiguous bf16 (kv_write_fp8 and whole gathered parts).
-//   SlicedRows a row-sliced write (GatherLaunch::rows): row_write_offset (launch_plan.h) of the
-//              vector's byte in the part's bf16 view; the geometry is in multiples of 16 bytes,
-//              so the 8 elements never straddle two slices.
-//   PiecedRows a row-sliced write with pieces (GatherLaunch::pieces > 1): piece_write_offset,
-//              plus the piece's offset from block b's row of the piece table (block(b)).
+//   SlicedRows a row-sliced write (GatherLaunch::rows): PartRows::write_offset of the vector's
+//              byte in the part's bf16 view; the geometry is in multiples of 16 bytes, so the 8
+//              elements never straddle two slices.
+//   PiecedRows a row-sliced write with pieces (rows.pieces > 1): the pieced write_offset, plus
+//              the piece's offset from block b's row of the piece table (block(b)).
 //              Pieces split at row boundaries, rows are multiples of 8 elements, so a vector
 //              never straddles two pieces; a 128-element scale group may, and each of its
 //              vectors is placed on its own.
@@ -87,26 +87,23 @@ struct DenseRows {
     __device__ __forceinline__ DenseRows block(uint32_t) const { return *this; }
 };
 struct SlicedRows {
-    uint32_t row_bytes, src_pitch, dst_pitch, slice_pitch;
+    PartRows g;
     __device__ __forceinline__ size_t operator()(uint32_t row, uint32_t hl) const {
-        return row_write_offset((row * kRow + hl * 8) * 2, row_bytes, src_pitch, dst_pitch,
-                                slice_pitch);
+        return g.write_offset((row * kRow + hl * 8) * 2);
     }
     __device__ __forceinline__ SlicedRows block(uint32_t) const { return *this; }
 };
 struct PiecedRows {
-    SlicedRows geo;
-    uint32_t piece_rows, pieces;
+    PartRows g;
+    uint32_t piece_rows;  // g.rows / g.pieces
     const uint64_t* off;  // block b's row of the piece table once bound by block(b)
     __device__ __forceinline__ size_t operator()(uint32_t row, uint32_t hl) const {
-        const PieceOffset p = piece_write_offset((row * kRow + hl * 8) * 2, geo.row_bytes,
-                                                 geo.src_pitch, geo.dst_pitch, geo.slice_pitch,
-                                                 piece_rows);
-        return off[p.piece] + p.off;
+        const PairOffsets p = g.write_offset((row * kRow + hl * 8) * 2, piece_rows);
+        return off[p.piece] + p.dst;
     }
     __device__ __forceinline__ PiecedRows block(uint32_t b) const {
         PiecedRows r = *this;
-        r.off += uint64_t(b) * pieces;
+        r.off += uint64_t(b) * g.pieces;
         return r;
     }
 };
@@ -224,7 +221,7 @@ __global__ void __launch_bounds__(kThreads)
 // Gathered writes (launch_kv_gather_fp8): n blocks of nparts parts, cpp items per part, the
 // part bases in the kernel parameters; write_fp8's items and commit (BlockParts<true>), each
 // lane's bf16 vector placed by `load_at`: DenseRows for whole parts, SlicedRows with
-// GatherLaunch::rows, PiecedRows with GatherLaunch::pieces > 1.
+// GatherLaunch::rows, PiecedRows with rows.pieces > 1.
 template <typename LoadAt>
 __global__ void __launch_bounds__(kThreads + 32)
     kv_write_fp8_gather_kernel(const CopyDesc* __restrict__ descs,
@@ -237,70 +234,56 @@ __global__ void __launch_bounds__(kThreads + 32)
 }
 
 // ---------------------------------------------------------------- gathered reads
-// The geometry of launch_kv_gather_fp8's reads, in elements of the part's bf16 view
-// (GatherLaunch counts bytes): a stored part holds `elems` e4m3 elements and their scales; with
-// GatherLaunch::rows, row r of it takes vpr 8-element vectors from element r * src_pitch +
-// src_col, and lands at r * dst_pitch bytes from the part's destination (slices, slice_pitch,
-// pieces and piece_off as in GatherLaunch).
-struct Fp8Rows {
-    uint32_t rows, vpr, src_pitch, src_col, dst_pitch, elems, slices, slice_pitch, pieces;
-    const uint64_t* piece_off;
-};
+// The units of the fp8 reads' row loops: a geometry's source side (row_bytes, src_pitch,
+// src_col) in elements of the part's bf16 view, its destination side in bytes.  Built once per
+// launch from its byte geometry (GatherLaunch::rows): derived inside the kernel, the halved
+// values took registers that the parameter bank holds for free.
+PartRows fp8_source_elems(const PartRows& g) {
+    PartRows e = g;
+    e.row_bytes = g.row_bytes / 2;
+    e.src_pitch = g.src_pitch / 2;
+    e.src_col = g.src_col / 2;
+    return e;
+}
 
 constexpr int kRowVecs = 4;  // (row, vector) pairs in flight per thread: 4 x 16 B of bf16
 
 // `nrows` rows of one stored fp8 part `q` (scales at q + elems) from element e0 on, dequantised
-// to dst.  The 256 threads walk the (row, vector) pairs flattened together, as copy_rows
-// (copy_span.cuh) does, so one 128-element KV head (16 vectors) per row keeps every thread
-// busy.  A vector is 8 e4m3 bytes at q + e and the scale of its group at scales[e / 128]: the
-// geometry keeps e a multiple of 8, so a vector never straddles two scale groups.
-// SLICED (GatherLaunch::slices > 1): dst is the part's destination and the nrows units are the
-// (slice, row) pairs e0 .. e0 + nrows - 1 of the part, placed by slice_pair (launch_plan.h) with
-// slice_pitch bytes between destination slices: (slice, row, vector) triples flattened.
+// to dst, in the units of fp8_source_elems: row r of the run takes e.row_bytes / 8 8-element
+// vectors from element e0 + r * e.src_pitch and lands at r * e.dst_pitch bytes from dst.  The
+// 256 threads walk the (row, vector) pairs flattened together, as copy_rows (copy_span.cuh)
+// does, so one 128-element KV head (16 vectors) per row keeps every thread busy.  A vector is 8
+// e4m3 bytes at q + e and the scale of its group at scales[e / 128]: the geometry keeps e a
+// multiple of 8, so a vector never straddles two scale groups.
+// SLICED (rows.slices > 1): dst is the part's destination and the nrows units are the (slice,
+// row) pairs e0 .. e0 + nrows - 1 of the part, placed by e.pair: (slice, row, vector) triples
+// flattened.
 template <bool SLICED = false>
 __device__ __forceinline__ void read_fp8_rows(uint8_t* dst, const uint8_t* q, const float* scales,
-                                              uint32_t e0, uint32_t nrows, const Fp8Rows& g,
-                                              uint32_t slice_pitch = 0) {
-    const uint32_t nvec = nrows * g.vpr;
-    uint32_t i = threadIdx.x;
-    if constexpr (SLICED) {
-        for (; i < nvec; i += kRowVecs * kThreads) {
-            uint2 v[kRowVecs];
-            float sc[kRowVecs];
-            uint32_t out[kRowVecs];
-#pragma unroll
-            for (int u = 0; u < kRowVecs; ++u) {
-                const uint32_t k = i + u * kThreads;
-                if (k >= nvec) continue;
-                const uint32_t p = k / g.vpr, c = k - p * g.vpr;
-                const PairOffsets o = slice_pair(e0 + p, g.rows, 8 * g.vpr, g.src_pitch,
-                                                 g.src_col, g.dst_pitch, slice_pitch);
-                const uint32_t e = o.src + 8 * c;
-                v[u] = ld_u2(q + e);
-                sc[u] = __uint_as_float(ld_u1(scales + e / kRow));
-                out[u] = o.dst + 16 * c;
-            }
-#pragma unroll
-            for (int u = 0; u < kRowVecs; ++u) {
-                if (i + u * kThreads >= nvec) continue;
-                *reinterpret_cast<uint4*>(dst + out[u]) = dequant8(v[u], sc[u]);
-            }
-        }
-        return;
-    }
-    for (; i < nvec; i += kRowVecs * kThreads) {
+                                              uint32_t e0, uint32_t nrows, const PartRows& e) {
+    const uint32_t vpr = e.row_bytes / 8;
+    const uint32_t nvec = nrows * vpr;
+    for (uint32_t i = threadIdx.x; i < nvec; i += kRowVecs * kThreads) {
         uint2 v[kRowVecs];
         float sc[kRowVecs];
-        size_t out[kRowVecs];
+        // a sliced destination lies within 32 bits (PartRows::ok), plain rows may not
+        std::conditional_t<SLICED, uint32_t, size_t> out[kRowVecs];
 #pragma unroll
         for (int u = 0; u < kRowVecs; ++u) {
             const uint32_t k = i + u * kThreads;
             if (k >= nvec) continue;
-            const uint32_t r = k / g.vpr, c = k - r * g.vpr;
-            const uint32_t e = e0 + r * g.src_pitch + 8 * c;
-            v[u] = ld_u2(q + e);
-            sc[u] = __uint_as_float(ld_u1(scales + e / kRow));
-            out[u] = size_t(r) * g.dst_pitch + 16 * c;
+            const uint32_t p = k / vpr, c = k - p * vpr;
+            uint32_t el;
+            if constexpr (SLICED) {
+                const PairOffsets o = e.pair(e0 + p);
+                el = o.src + 8 * c;
+                out[u] = o.dst + 16 * c;
+            } else {
+                el = e0 + p * e.src_pitch + 8 * c;
+                out[u] = size_t(p) * e.dst_pitch + 16 * c;
+            }
+            v[u] = ld_u2(q + el);
+            sc[u] = __uint_as_float(ld_u1(scales + el / kRow));
         }
 #pragma unroll
         for (int u = 0; u < kRowVecs; ++u) {
@@ -317,10 +300,11 @@ __device__ __forceinline__ void read_fp8_rows(uint8_t* dst, const uint8_t* q, co
 //            kv_read_fp8_kernel;
 //   kRows    rows [c * chunk, +chunk) (GatherLaunch::rows: read_fp8_rows);
 //   kSlices  (slice, row) pairs [c * chunk, +chunk), numbered slice-major (read_fp8_rows<true>);
-//   kPieces  the same pairs (GatherLaunch::pieces > 1, any slices), cut where q / piece_rows
-//            changes as in kv_copy.cu's kv_scatter_ldst_kernel; each cut is read as plain rows to
-//            desc.dst + piece_off[block * pieces + t] + the place piece_pair gives its first pair
-//            - one piece-offset load per cut.
+//   kPieces  the same pairs (rows.pieces > 1, any slices), cut where q / piece_rows changes as
+//            in kv_copy.cu's kv_scatter_ldst_kernel; each cut is read as plain rows to desc.dst +
+//            piece_off[block * pieces + t] + the place PartRows::pair gives its first pair - one
+//            piece-offset load per cut.
+// `e` is the launch's row geometry in fp8_source_elems' units.
 // (This kernel and kv_read_fp8_kernel share the row maths, not the loop: inlining one loop body
 // into both changed how the compiler schedules kv_read_fp8_kernel.)
 static_assert(kThreads == kLdStThreads, "scatter_items releases groups on kLdStThreads threads");
@@ -329,19 +313,20 @@ __global__ void __launch_bounds__(kThreads)
     kv_read_fp8_scatter_kernel(const CopyDesc* __restrict__ descs,
                                const __grid_constant__ GatherParts parts, uint32_t n,
                                uint32_t nparts, uint32_t first_part, uint32_t chunk, uint32_t cpp,
-                               uint64_t stride, Fp8Rows g, uint32_t* status, GroupRelease rel) {
+                               uint64_t stride, uint32_t elems, PartRows e,
+                               const uint64_t* piece_off, uint32_t* status, GroupRelease rel) {
     scatter_items<LAYERED>(descs, n, nparts, cpp, status, rel, [&](const CopyDesc& d,
                                                                   const LayeredItem& it) {
         const uint8_t* q =
             reinterpret_cast<const uint8_t*>(d.src + uint64_t(first_part + it.part) * stride);
-        const float* scales = reinterpret_cast<const float*>(q + g.elems);
+        const float* scales = reinterpret_cast<const float*>(q + elems);
         uint8_t* dst = reinterpret_cast<uint8_t*>(parts.base[it.part] + d.dst);
         if constexpr (S == PartShape::kWhole) {
             const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
             const uint32_t half = lane >> 4, hl = lane & 15;
             constexpr uint32_t kStep = 2 * kRowPairs;
             const uint32_t e0 = it.chunk * chunk;
-            const uint32_t rows = min(chunk, g.elems - e0) / kRow;
+            const uint32_t rows = min(chunk, elems - e0) / kRow;
             const uint32_t row0 = e0 / kRow;
             for (uint32_t r0 = warp * kStep; r0 < rows; r0 += kWarps * kStep) {
                 uint2 v[kRowPairs];
@@ -364,22 +349,20 @@ __global__ void __launch_bounds__(kThreads)
             }
         } else if constexpr (S == PartShape::kRows) {
             const uint32_t r0 = it.chunk * chunk;
-            read_fp8_rows(dst + uint64_t(r0) * g.dst_pitch, q, scales, r0 * g.src_pitch + g.src_col,
-                          min(chunk, g.rows - r0), g);
+            read_fp8_rows(dst + uint64_t(r0) * e.dst_pitch, q, scales, r0 * e.src_pitch + e.src_col,
+                          min(chunk, e.rows - r0), e);
         } else if constexpr (S == PartShape::kSlices) {
             const uint32_t q0 = it.chunk * chunk;
-            read_fp8_rows<true>(dst, q, scales, q0, min(chunk, g.rows * g.slices - q0), g,
-                                g.slice_pitch);
+            read_fp8_rows<true>(dst, q, scales, q0, min(chunk, e.rows * e.slices - q0), e);
         } else {
-            const uint32_t piece_rows = g.rows / g.pieces;
-            const uint32_t q0 = it.chunk * chunk, q1 = min(q0 + chunk, g.rows * g.slices);
-            const uint64_t* off = g.piece_off + uint64_t(it.block) * g.pieces;
+            const uint32_t piece_rows = e.rows / e.pieces;
+            const uint32_t q0 = it.chunk * chunk, q1 = min(q0 + chunk, e.rows * e.slices);
+            const uint64_t* off = piece_off + uint64_t(it.block) * e.pieces;
             for (uint32_t p = q0; p < q1;) {
-                const uint32_t e = min(q1, (p / piece_rows + 1) * piece_rows);
-                const PieceOffsets o = piece_pair(p, g.rows, 8 * g.vpr, g.src_pitch, g.src_col,
-                                                  g.dst_pitch, g.slice_pitch, piece_rows);
-                read_fp8_rows(dst + off[o.piece] + o.dst, q, scales, o.src, e - p, g);
-                p = e;
+                const uint32_t end = min(q1, (p / piece_rows + 1) * piece_rows);
+                const PairOffsets o = e.pair(p, piece_rows);
+                read_fp8_rows(dst + off[o.piece] + o.dst, q, scales, o.src, end - p, e);
+                p = end;
             }
         }
     });
@@ -391,14 +374,13 @@ template <bool WRITE, bool LAYERED, PartShape S>
 cudaError_t launch_fp8_gather(const GatherLaunch& a, uint32_t elems, int variant,
                               const GatherParts& parts, cudaStream_t stream) {
     const uint64_t stride = fp8_gather_bytes(1, elems);
-    const SlicedRows rows{a.row_bytes, a.src_pitch, a.dst_pitch, a.dst_slice_pitch};
     const auto load_at = [&] {
         if constexpr (S == PartShape::kWhole)
             return DenseRows{};
         else if constexpr (S == PartShape::kRows)
-            return rows;
+            return SlicedRows{a.rows};
         else
-            return PiecedRows{rows, a.rows / a.pieces, a.pieces, a.piece_off};
+            return PiecedRows{a.rows, a.rows.rows / a.rows.pieces, a.piece_off};
     }();
     using LoadAt = std::decay_t<decltype(load_at)>;
     LaunchPlan p;
@@ -422,12 +404,9 @@ cudaError_t launch_fp8_gather(const GatherLaunch& a, uint32_t elems, int variant
             a.descs, parts, a.n, a.nparts, elems, p.chunk, p.cpb, a.first_part, stride, load_at,
             publish_of(a, true), layer_of(a));
     } else {
-        const Fp8Rows g{a.rows,          a.row_bytes / 16, a.src_pitch / 2, a.src_col / 2,
-                        a.dst_pitch,     elems,            a.slices,        a.dst_slice_pitch,
-                        a.pieces,        a.piece_off};
         kv_read_fp8_scatter_kernel<LAYERED, S><<<p.ctas, kThreads, 0, stream>>>(
-            a.descs, parts, a.n, a.nparts, a.first_part, p.chunk, p.cpb, stride, g, a.status,
-            release_of(a));
+            a.descs, parts, a.n, a.nparts, a.first_part, p.chunk, p.cpb, stride, elems,
+            fp8_source_elems(a.rows), a.piece_off, a.status, release_of(a));
     }
     return cudaGetLastError();
 }
@@ -463,7 +442,7 @@ cudaError_t launch_kv_gather_fp8(const GatherLaunch& a, uint32_t elems, int vari
     const bool layered = a.group_flags != nullptr;
     if (layered && !a.group_counters) return cudaErrorInvalidValue;
     // pieces split rows, at the offsets of the piece table
-    if (a.pieces != 1 && (!a.rows || !a.piece_off)) return cudaErrorInvalidValue;
+    if (a.rows.pieces != 1 && (!a.rows.rows || !a.piece_off)) return cudaErrorInvalidValue;
     const GatherParts parts = parts_of(a);
     if (a.write)
         return with_shape<true>(a, [&](auto s) {

@@ -246,163 +246,54 @@ ISTORE_KHD inline uint32_t cta_items(uint32_t lo, uint32_t hi, uint32_t first, u
 }
 
 // ---------------------------------------------------------------- row geometry
-// The row geometry of a row-sliced read (GatherLaunch::rows, ::slices), in bytes of the
-// caller's view of a part (part_bytes), as the connection (Connection::gather_refusal) and the
-// plans below accept it: the row's slices lie inside the stored row, the rows cover the part,
-// and with slices > 1 the destination rectangles are disjoint under one of two nestings -
-// head-major (a slice's rows inside dst_slice_pitch) or token-major (a row's slices inside
-// dst_pitch) - and the destination extent, (rows - 1) * dst_pitch + (slices - 1) *
-// dst_slice_pitch + row_bytes, fits 32 bits.  slices == 1 checks what it always did.
-// pieces > 1 (GatherLaunch::pieces): the rows land in `pieces` runs of rows / pieces rows, each
-// at its own local offset, so the nesting and the 32-bit extent hold per run (piece_rows rows)
-// rather than over all rows, and pieces must divide rows.
-inline bool row_geometry_ok(uint32_t rows, uint32_t row_bytes, uint32_t src_pitch,
-                            uint32_t src_col, uint32_t dst_pitch, uint32_t slices,
-                            uint32_t dst_slice_pitch, uint64_t part_bytes, uint32_t pieces = 1) {
-    if (rows == 0 || row_bytes == 0 || slices == 0 || pieces == 0 || rows % pieces != 0 ||
-        uint64_t(src_col) + uint64_t(slices) * row_bytes > src_pitch ||
-        uint64_t(rows) * src_pitch != part_bytes)
-        return false;
-    const uint64_t rb = row_bytes, r1 = rows / pieces - 1, s1 = slices - 1;
-    if (slices == 1) return pieces == 1 || r1 * dst_pitch + rb <= 0xffffffffull;
-    const bool head_major = dst_pitch >= rb && dst_slice_pitch >= r1 * dst_pitch + rb;
-    const bool token_major = dst_slice_pitch >= rb && dst_pitch >= s1 * dst_slice_pitch + rb;
-    return (head_major || token_major) &&
-           r1 * dst_pitch + s1 * dst_slice_pitch + rb <= 0xffffffffull;
-}
-
-// Where (slice, row) pair q of a part goes: the kernels' unit of work with slices > 1.  Pairs
-// are numbered slice-major (q = j * rows + r), so a run of pairs of a head-major destination
-// writes contiguous bytes.  Slice j of row r moves `row` units from r * src_pitch + src_col +
-// j * row of the stored part to r * dst_pitch + j * dst_slice_pitch of the part's destination.
-// Units are the caller's: bytes, or for fp8 parts elements of the bf16 view on the source side
-// and bytes on the destination side.  row_geometry_ok keeps both offsets within 32 bits.  The
-// kernels (copy_span.cuh: copy_rows, kv_fp8.cu: read_fp8_rows) and the CPU tests
-// (_infinistore.testing.slice_pair) share this function.
-struct PairOffsets {
-    uint32_t src, dst;
-};
-ISTORE_KHD inline PairOffsets slice_pair(uint32_t q, uint32_t rows, uint32_t row,
-                                         uint32_t src_pitch, uint32_t src_col, uint32_t dst_pitch,
-                                         uint32_t dst_slice_pitch) {
-    const uint32_t j = q / rows, r = q - j * rows;
-    return PairOffsets{r * src_pitch + src_col + j * row, r * dst_pitch + j * dst_slice_pitch};
-}
-
-// ---------------------------------------------------------------- pieces
-// A block whose destination is `pieces` local offsets off[0..pieces-1] (GatherLaunch::pieces,
-// piece_off) instead of one: each part's rows split into pieces runs of piece_rows = rows /
-// pieces rows, and run t lands at off[t] - e.g. a chunk of k engine pages stored under one key,
-// page t of it at the offset the caller's block table names.  Slice j of stored row r goes to
-// off[r / piece_rows] + (r % piece_rows) * dst_pitch + j * dst_slice_pitch.  piece_pair is
-// slice_pair with the destination inside its piece; piece_rows == rows is slice_pair with
-// piece 0.  Pairs q with the same q / piece_rows share their slice and their piece (rows is a
-// multiple of piece_rows), so the kernels copy each such run as plain rows from the place
-// piece_pair gives its first pair, loading its piece offset once.  The kernels (kv_copy.cu:
-// kv_scatter_ldst_kernel, kv_fp8.cu: kv_read_fp8_scatter_kernel) and the CPU tests
-// (_infinistore.testing.piece_pair) share this function.
-struct PieceOffsets {
-    uint32_t src, dst, piece;
-};
-ISTORE_KHD inline PieceOffsets piece_pair(uint32_t q, uint32_t rows, uint32_t row,
-                                          uint32_t src_pitch, uint32_t src_col, uint32_t dst_pitch,
-                                          uint32_t dst_slice_pitch, uint32_t piece_rows) {
-    const uint32_t j = q / rows, r = q - j * rows, t = r / piece_rows;
-    return PieceOffsets{r * src_pitch + src_col + j * row,
-                        (r - t * piece_rows) * dst_pitch + j * dst_slice_pitch, t};
-}
-
-// A row-sliced write (GatherLaunch::rows with write) takes the geometry that reads the same
-// local layout back: the stored part is src_pitch-byte rows, the caller's part holds slice j of
-// row r at r * dst_pitch + j * dst_slice_pitch - e.g. a head-major page [head][token][dim]
-// stored token-major.  The in-band commit publishes whole blocks, so a write must fill every
-// byte of the stored part: on top of row_geometry_ok, src_col == 0 and slices * row_bytes ==
-// src_pitch.
-inline bool row_write_covers(uint32_t row_bytes, uint32_t src_pitch, uint32_t src_col,
-                             uint32_t slices) {
-    return src_col == 0 && uint64_t(slices) * row_bytes == src_pitch;
-}
-
 // What the four row plans (bf16 and fp8, reads and writes) admit: a launch of `write`'s
-// direction, 1 to kGatherMaxParts parts, a row geometry row_geometry_ok accepts, and the
-// groups of a layered read (groups_ok; writes are never layered).  A write's rows must cover
-// the stored part (row_write_covers).
+// direction, 1 to kGatherMaxParts parts, a row geometry PartRows::ok accepts, and the groups of
+// a layered read (groups_ok; writes are never layered).  A write's rows must cover the stored
+// part (PartRows::covers).
 inline bool rows_admitted(const GatherLaunch& a, bool write) {
     return a.write == write && a.nparts != 0 && a.nparts <= kGatherMaxParts && groups_ok(a) &&
-           row_geometry_ok(a.rows, a.row_bytes, a.src_pitch, a.src_col, a.dst_pitch, a.slices,
-                           a.dst_slice_pitch, a.part_bytes, a.pieces) &&
-           (!write || row_write_covers(a.row_bytes, a.src_pitch, a.src_col, a.slices));
+           a.rows.ok(a.part_bytes) && (!write || a.rows.covers());
+}
+
+// The bf16 row kernels' vector width: the one the OR of the geometry (PartRows::align_or), the
+// part bases and the local offsets allows (pool blocks are granule aligned and part_bytes is a
+// multiple of src_pitch).
+inline Kernel rows_kernel(const GatherLaunch& a) {
+    const uint64_t align_or = a.align_or | a.rows.align_or();
+    return !aligned_to(a.rows.row_bytes, align_or, 16)   ? Kernel::kLdSt1
+           : aligned_to(a.rows.row_bytes, align_or, 32)  ? Kernel::kLdSt32
+                                                         : Kernel::kLdSt16;
 }
 
 // ---------------------------------------------------------------- row-sliced reads
 // Row reads (GatherLaunch::rows != 0), plain or layered: always the ld/st kernels (the
-// TMA pipelines have no row form).  The vector width is the one the OR of row_bytes, both
-// pitches (with slices > 1, dst_slice_pitch too), src_col, the part bases and the local
-// offsets allows (pool blocks are granule aligned and part_bytes is a multiple of src_pitch).
-// A work item is a run of `chunk` (slice, row) pairs of one part (rows with slices == 1),
-// about kLdStChunk of payload, or all of a part's pairs under ldst_items' rule; cpb is runs per
-// part, and a layered read numbers items with layered_item as whole parts do.
+// TMA pipelines have no row form), at rows_kernel's vector width.  A work item is a run of
+// `chunk` (slice, row) pairs of one part (rows with slices == 1), about kLdStChunk of payload,
+// or all of a part's pairs under ldst_items' rule; cpb is runs per part, and a layered read
+// numbers items with layered_item as whole parts do.
 inline LaunchPlan plan_gather_rows(const GatherLaunch& a, int sms, LdStResident res) {
     if (!rows_admitted(a, false)) return invalid_plan();
-    const uint64_t geo_or = a.align_or | a.src_pitch | a.src_col | a.dst_pitch |
-                            (a.slices > 1 ? a.dst_slice_pitch : 0u);
-    const bool aligned16 = aligned_to(a.row_bytes, geo_or, 16);
-    const bool aligned32 = aligned_to(a.row_bytes, geo_or, 32);
     LaunchPlan p;
-    p.kernel = !aligned16 ? Kernel::kLdSt1 : aligned32 ? Kernel::kLdSt32 : Kernel::kLdSt16;
+    p.kernel = rows_kernel(a);
     const uint64_t parts = uint64_t(a.n) * a.nparts;
-    ldst_items(p, parts, a.rows * a.slices, std::max(1u, kLdStChunk / a.row_bytes),
-               std::max(1u, (1u << 20) / a.row_bytes), sms);
+    ldst_items(p, parts, a.rows.rows * a.rows.slices, std::max(1u, kLdStChunk / a.rows.row_bytes),
+               std::max(1u, (1u << 20) / a.rows.row_bytes), sms);
     if (parts * p.cpb > kMaxItems) return invalid_plan();
     p.ctas = ldst_grid(p, a.max_ctas, res, sms, parts * p.cpb);
     return p;
 }
 
 // ---------------------------------------------------------------- row-sliced writes
-// Where byte o of a fully covered stored part comes from in the caller's part: row r =
-// o / src_pitch, slice j of it, column c - j * row_bytes of that slice.  Over a covering
-// geometry it is the inverse of slice_pair: row_write_offset(slice_pair(q).src + w) ==
-// slice_pair(q).dst + w for every byte w < row_bytes.  The kernels (copy_span.cuh:
-// copy_span_rows, kv_fp8.cu: SlicedRows) and the CPU tests
-// (_infinistore.testing.row_write_offset) share this function.
-ISTORE_KHD inline uint32_t row_write_offset(uint32_t o, uint32_t row_bytes, uint32_t src_pitch,
-                                            uint32_t dst_pitch, uint32_t dst_slice_pitch) {
-    const uint32_t r = o / src_pitch, c = o - r * src_pitch, j = c / row_bytes;
-    return r * dst_pitch + j * dst_slice_pitch + (c - j * row_bytes);
-}
-
-// The pieced form (GatherLaunch::pieces): byte o of a covered stored part comes from piece
-// o / (piece_rows * src_pitch), at row_write_offset of o within that piece's rows.  Over a
-// covering geometry it is the inverse of piece_pair.  The kernels cut a work item's stored
-// bytes at piece boundaries and load each run from its piece (copy_span.cuh: copy_span_rows)
-// or place each vector with it (kv_fp8.cu: PiecedRows); the CPU tests call it through
-// _infinistore.testing.piece_write_offset.
-struct PieceOffset {
-    uint32_t piece, off;
-};
-ISTORE_KHD inline PieceOffset piece_write_offset(uint32_t o, uint32_t row_bytes, uint32_t src_pitch,
-                                                 uint32_t dst_pitch, uint32_t dst_slice_pitch,
-                                                 uint32_t piece_rows) {
-    const uint32_t piece_bytes = piece_rows * src_pitch, t = o / piece_bytes;
-    return PieceOffset{t, row_write_offset(o - t * piece_bytes, row_bytes, src_pitch, dst_pitch,
-                                           dst_slice_pitch)};
-}
-
 // Row writes (launch_kv_gather with rows and write): the work items of the
 // whole-part write, (block, part, chunk of the stored part) numbered (b * nparts + s) * cpp + c
 // with plan_gather's ld/st chunks, so every item stores one contiguous run of pool bytes and
 // the commit counts arrivals as for whole parts; only the local load address goes through
-// row_write_offset.  Always the ld/st kernels (no TMA form), never layered reads.  The vector
-// width is the one the OR of row_bytes, dst_pitch, dst_slice_pitch (with slices > 1), the part
-// bases and the local offsets allows (src_pitch is slices * row_bytes).
+// PartRows::write_offset.  Always the ld/st kernels (no TMA form), at rows_kernel's vector
+// width, never layered reads.
 inline LaunchPlan plan_gather_rows_write(const GatherLaunch& a, int sms, LdStResident res) {
     if (!rows_admitted(a, true)) return invalid_plan();
-    const uint64_t geo_or =
-        a.align_or | a.dst_pitch | (a.slices > 1 ? a.dst_slice_pitch : 0u);
-    const bool aligned16 = aligned_to(a.row_bytes, geo_or, 16);
-    const bool aligned32 = aligned_to(a.row_bytes, geo_or, 32);
     LaunchPlan p;
-    p.kernel = !aligned16 ? Kernel::kLdSt1 : aligned32 ? Kernel::kLdSt32 : Kernel::kLdSt16;
+    p.kernel = rows_kernel(a);
     const uint64_t parts = uint64_t(a.n) * a.nparts;
     ldst_items(p, parts, a.part_bytes, kLdStChunk, 1u << 20, sms);
     if (parts * p.cpb > kMaxItems) return invalid_plan();
@@ -420,11 +311,9 @@ inline LaunchPlan plan_gather_rows_write(const GatherLaunch& a, int sms, LdStRes
 inline LaunchPlan plan_gather_fp8_rows_write(const GatherLaunch& a, uint32_t elems, int sms,
                                              LdStResident res) {
     if (!rows_admitted(a, true)) return invalid_plan();
-    const uint64_t geo_or = a.align_or | a.row_bytes | a.src_pitch | a.dst_pitch |
-                            (a.slices > 1 ? a.dst_slice_pitch : 0u);
     const uint64_t parts = uint64_t(a.n) * a.nparts;
     if (elems == 0 || elems % 512 != 0 || uint64_t(a.part_bytes) != 2ull * elems ||
-        (geo_or & 15) != 0 || parts > kMaxItems)
+        ((a.align_or | a.rows.align_or()) & 15) != 0 || parts > kMaxItems)
         return invalid_plan();
     LaunchPlan p;
     p.kernel = Kernel::kLdStFp8;
@@ -534,16 +423,14 @@ inline LaunchPlan plan_gather_fp8(const GatherLaunch& a, uint32_t elems, int var
 inline LaunchPlan plan_gather_fp8_rows(const GatherLaunch& a, uint32_t elems, int sms,
                                        LdStResident res) {
     if (!rows_admitted(a, false)) return invalid_plan();
-    const uint64_t geo_or = a.align_or | a.row_bytes | a.src_pitch | a.src_col | a.dst_pitch |
-                            (a.slices > 1 ? a.dst_slice_pitch : 0u);
     if (elems == 0 || elems % 512 != 0 || uint64_t(a.part_bytes) != 2ull * elems ||
-        (geo_or & 15) != 0)
+        ((a.align_or | a.rows.align_or()) & 15) != 0)
         return invalid_plan();
     LaunchPlan p;
     p.kernel = Kernel::kLdStFp8;
     const uint64_t parts = uint64_t(a.n) * a.nparts;
-    ldst_items(p, parts, a.rows * a.slices, std::max(1u, kLdStChunk / a.row_bytes),
-               std::max(1u, (1u << 20) / a.row_bytes), sms);
+    ldst_items(p, parts, a.rows.rows * a.rows.slices, std::max(1u, kLdStChunk / a.rows.row_bytes),
+               std::max(1u, (1u << 20) / a.rows.row_bytes), sms);
     if (parts * p.cpb > kMaxItems) return invalid_plan();
     p.ctas = clamp_grid(a.max_ctas > 0 ? a.max_ctas : res.r16 * sms, parts * p.cpb);
     return p;

@@ -180,41 +180,42 @@ struct KeyArena {
 
 thread_local KeyArena t_arena;
 
-// A row-sliced call's geometry from its native list, in bytes: (rows, row_bytes, src_pitch,
-// src_col, dst_pitch) or the same followed by (slices, dst_slice_pitch) into a GatherSpec or a
-// GatherLaunch.  False unless the list has 5 or 7 entries; an empty list is for the caller.
-template <typename G>
-bool set_rows(G& g, const std::vector<uint32_t>& rows) {
-    if (rows.size() != 5 && rows.size() != 7) return false;
-    g.rows = rows[0];
-    g.row_bytes = rows[1];
-    g.src_pitch = rows[2];
-    g.src_col = rows[3];
-    g.dst_pitch = rows[4];
-    if (rows.size() == 7) {
-        g.slices = rows[5];
-        g.dst_slice_pitch = rows[6];
+// A gathered call's row geometry from its native list, in bytes: (rows, row_bytes, src_pitch,
+// src_col, dst_pitch) or the same followed by (slices, dst_slice_pitch); an empty list is whole
+// parts.  `pieces` comes from its own argument.  False unless the list has 0, 5 or 7 entries.
+bool parse_rows(const std::vector<uint32_t>& v, uint32_t pieces, kernels::PartRows& r) {
+    if (!v.empty() && v.size() != 5 && v.size() != 7) return false;
+    r = kernels::PartRows{};
+    r.pieces = pieces;
+    if (v.empty()) return true;
+    r.rows = v[0];
+    r.row_bytes = v[1];
+    r.src_pitch = v[2];
+    r.src_col = v[3];
+    r.dst_pitch = v[4];
+    if (v.size() == 7) {
+        r.slices = v[5];
+        r.dst_slice_pitch = v[6];
     }
     return true;
 }
 
 // A gathered call's parts: part s at part_base[s] (which must outlive the spec); elems > 0:
 // bf16 parts of elems elements stored as fp8 pages.  rows: a row-sliced read's or write's
-// geometry (set_rows); empty: whole parts.  The connection checks the values.
+// geometry (parse_rows); empty: whole parts.  The connection checks the values.
 Connection::GatherSpec gather_spec(const std::vector<uint64_t>& part_base, uint32_t part_bytes,
                                    uint32_t elems, uint32_t first_part,
                                    const std::vector<uint32_t>& rows = {},
                                    const std::vector<uint64_t>* piece_off = nullptr,
                                    uint32_t pieces = 1) {
     Connection::GatherSpec g;
-    g.pieces = pieces;
     if (pieces > 1) g.piece_off = piece_off->data();
     g.part_base = part_base.data();
     g.nparts = uint32_t(part_base.size());
     g.part_bytes = part_bytes;
     g.fp8_elems = elems;
     g.first_part = first_part;
-    if (!rows.empty() && !set_rows(g, rows))
+    if (!parse_rows(rows, pieces, g.rows))
         throw py::value_error("rows is (rows, row_bytes, src_pitch, src_col, dst_pitch[, "
                               "slices, dst_slice_pitch])");
     return g;
@@ -239,25 +240,16 @@ std::vector<uint64_t> piece_table(const py::object& obj, size_t n, uint32_t piec
 // A row-sliced launch as the plan bindings of _infinistore.testing describe it: part_bytes is
 // rows * src_pitch, and group_parts > 0 makes it a layered read (the plans only ask whether
 // group_flags is set).
-kernels::GatherLaunch rows_launch(uint32_t n, uint32_t nparts, bool write, uint32_t rows,
-                                  uint32_t row_bytes, uint32_t src_pitch, uint32_t src_col,
-                                  uint32_t dst_pitch, uint32_t slices, uint32_t dst_slice_pitch,
-                                  uint64_t align_or, uint32_t group_parts, int max_ctas,
-                                  uint32_t pieces = 1) {
+kernels::GatherLaunch rows_launch(uint32_t n, uint32_t nparts, bool write,
+                                  const kernels::PartRows& rows, uint64_t align_or,
+                                  uint32_t group_parts, int max_ctas) {
     static uint32_t flags[1];
     kernels::GatherLaunch a;
-    a.pieces = pieces;
     a.n = n;
     a.nparts = nparts;
     a.write = write;
-    a.part_bytes = uint32_t(uint64_t(rows) * src_pitch);
+    a.part_bytes = uint32_t(uint64_t(rows.rows) * rows.src_pitch);
     a.rows = rows;
-    a.row_bytes = row_bytes;
-    a.src_pitch = src_pitch;
-    a.src_col = src_col;
-    a.dst_pitch = dst_pitch;
-    a.slices = slices;
-    a.dst_slice_pitch = dst_slice_pitch;
     a.align_or = align_or;
     a.group_flags = group_parts ? flags : nullptr;
     a.group_parts = group_parts;
@@ -1075,10 +1067,9 @@ PYBIND11_MODULE(_infinistore, m) {
             G.group_counters = as_ptr<uint32_t>(group_counters);
             G.group_seq = group_seq;
             G.group_parts = group_parts;
-            if (!rows.empty() && !set_rows(G, rows))
+            if (!parse_rows(rows, pieces, G.rows))
                 throw std::runtime_error("kv_gather: rows is 5 or 7 values");
             G.piece_off = as_ptr<const uint64_t>(piece_off);
-            G.pieces = pieces;
             const cudaError_t e = kernels::launch_kv_gather(G, as_ptr<CUstream_st>(stream));
             if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
         },
@@ -1140,13 +1131,10 @@ PYBIND11_MODULE(_infinistore, m) {
             G.group_counters = as_ptr<uint32_t>(group_counters);
             G.group_seq = group_seq;
             G.group_parts = group_parts;
-            if (!rows.empty()) {  // bytes of the parts' bf16 view: part_bytes is 2 * elems
-                if (!set_rows(G, rows))
-                    throw std::runtime_error("kv_gather_fp8: rows is 5 or 7 values");
-                G.part_bytes = 2 * elems;
-            }
+            if (!parse_rows(rows, pieces, G.rows))
+                throw std::runtime_error("kv_gather_fp8: rows is 5 or 7 values");
+            if (!rows.empty()) G.part_bytes = 2 * elems;  // bytes of the parts' bf16 view
             G.piece_off = as_ptr<const uint64_t>(piece_off);
-            G.pieces = pieces;
             const cudaError_t e =
                 kernels::launch_kv_gather_fp8(G, elems, variant, as_ptr<CUstream_st>(stream));
             if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
@@ -1584,40 +1572,60 @@ PYBIND11_MODULE(_infinistore, m) {
         if (!stride || hi < lo) throw py::value_error("needs stride > 0 and lo <= hi");
         return kernels::cta_items(lo, hi, first, stride);
     });
-    // sliced rows: where (slice, row) pair q of a part goes, and the geometry the plans and the
-    // connection accept (kernels/launch_plan.h)
+    // row geometry (kernels::PartRows): where (slice, row) pair q of a part goes, where byte o
+    // of a covered stored part comes from (with pieces: which piece, and where inside it), and
+    // the geometry the plans and the connection accept
+    using kernels::PartRows;
     t.def("slice_pair",
           [](uint32_t q, uint32_t rows, uint32_t row, uint32_t src_pitch, uint32_t src_col,
              uint32_t dst_pitch, uint32_t dst_slice_pitch) {
               if (!rows) throw py::value_error("needs rows > 0");
-              const kernels::PairOffsets o = kernels::slice_pair(q, rows, row, src_pitch, src_col,
-                                                                 dst_pitch, dst_slice_pitch);
+              const kernels::PairOffsets o =
+                  PartRows{.rows = rows, .row_bytes = row, .src_pitch = src_pitch,
+                           .src_col = src_col, .dst_pitch = dst_pitch,
+                           .dst_slice_pitch = dst_slice_pitch}
+                      .pair(q);
               return py::make_tuple(o.src, o.dst);
           },
           py::arg("q"), py::arg("rows"), py::arg("row"), py::arg("src_pitch"),
           py::arg("src_col"), py::arg("dst_pitch"), py::arg("dst_slice_pitch"));
-    // row-sliced writes: where byte o of a fully covered stored part comes from
     t.def("row_write_offset",
           [](uint32_t o, uint32_t row_bytes, uint32_t src_pitch, uint32_t dst_pitch,
              uint32_t dst_slice_pitch) {
               if (!row_bytes || !src_pitch) throw py::value_error("needs row_bytes, src_pitch > 0");
-              return kernels::row_write_offset(o, row_bytes, src_pitch, dst_pitch, dst_slice_pitch);
+              return PartRows{.row_bytes = row_bytes, .src_pitch = src_pitch,
+                              .dst_pitch = dst_pitch, .dst_slice_pitch = dst_slice_pitch}
+                  .write_offset(o);
           },
           py::arg("o"), py::arg("row_bytes"), py::arg("src_pitch"), py::arg("dst_pitch"),
           py::arg("dst_slice_pitch"));
-    t.def("row_write_covers", &kernels::row_write_covers, py::arg("row_bytes"),
-          py::arg("src_pitch"), py::arg("src_col"), py::arg("slices"));
-    t.def("row_geometry_ok", &kernels::row_geometry_ok, py::arg("rows"), py::arg("row_bytes"),
-          py::arg("src_pitch"), py::arg("src_col"), py::arg("dst_pitch"), py::arg("slices"),
-          py::arg("dst_slice_pitch"), py::arg("part_bytes"), py::arg("pieces") = 1);
-    // pieces: where (slice, row) pair q goes (piece, offset inside it), and where byte o of a
-    // covered stored part comes from
+    t.def("row_write_covers",
+          [](uint32_t row_bytes, uint32_t src_pitch, uint32_t src_col, uint32_t slices) {
+              return PartRows{.row_bytes = row_bytes, .src_pitch = src_pitch, .src_col = src_col,
+                              .slices = slices}
+                  .covers();
+          },
+          py::arg("row_bytes"), py::arg("src_pitch"), py::arg("src_col"), py::arg("slices"));
+    t.def("row_geometry_ok",
+          [](uint32_t rows, uint32_t row_bytes, uint32_t src_pitch, uint32_t src_col,
+             uint32_t dst_pitch, uint32_t slices, uint32_t dst_slice_pitch, uint64_t part_bytes,
+             uint32_t pieces) {
+              return PartRows{rows,   row_bytes,       src_pitch, src_col, dst_pitch,
+                              slices, dst_slice_pitch, pieces}
+                  .ok(part_bytes);
+          },
+          py::arg("rows"), py::arg("row_bytes"), py::arg("src_pitch"), py::arg("src_col"),
+          py::arg("dst_pitch"), py::arg("slices"), py::arg("dst_slice_pitch"),
+          py::arg("part_bytes"), py::arg("pieces") = 1);
     t.def("piece_pair",
           [](uint32_t q, uint32_t rows, uint32_t row, uint32_t src_pitch, uint32_t src_col,
              uint32_t dst_pitch, uint32_t dst_slice_pitch, uint32_t piece_rows) {
               if (!rows || !piece_rows) throw py::value_error("needs rows, piece_rows > 0");
-              const kernels::PieceOffsets o = kernels::piece_pair(
-                  q, rows, row, src_pitch, src_col, dst_pitch, dst_slice_pitch, piece_rows);
+              const kernels::PairOffsets o =
+                  PartRows{.rows = rows, .row_bytes = row, .src_pitch = src_pitch,
+                           .src_col = src_col, .dst_pitch = dst_pitch,
+                           .dst_slice_pitch = dst_slice_pitch}
+                      .pair(q, piece_rows);
               return py::make_tuple(o.src, o.dst, o.piece);
           },
           py::arg("q"), py::arg("rows"), py::arg("row"), py::arg("src_pitch"),
@@ -1628,9 +1636,11 @@ PYBIND11_MODULE(_infinistore, m) {
              uint32_t dst_slice_pitch, uint32_t piece_rows) {
               if (!row_bytes || !src_pitch || !piece_rows)
                   throw py::value_error("needs row_bytes, src_pitch, piece_rows > 0");
-              const kernels::PieceOffset p = kernels::piece_write_offset(
-                  o, row_bytes, src_pitch, dst_pitch, dst_slice_pitch, piece_rows);
-              return py::make_tuple(p.piece, p.off);
+              const kernels::PairOffsets p =
+                  PartRows{.row_bytes = row_bytes, .src_pitch = src_pitch,
+                           .dst_pitch = dst_pitch, .dst_slice_pitch = dst_slice_pitch}
+                      .write_offset(o, piece_rows);
+              return py::make_tuple(p.piece, p.dst);
           },
           py::arg("o"), py::arg("row_bytes"), py::arg("src_pitch"), py::arg("dst_pitch"),
           py::arg("dst_slice_pitch"), py::arg("piece_rows"));
@@ -1756,9 +1766,10 @@ PYBIND11_MODULE(_infinistore, m) {
                       uint32_t src_pitch, uint32_t src_col, uint32_t dst_pitch, uint64_t align_or,
                       uint32_t group_parts, int max_ctas, int sm_count, int resident16,
                       int resident32, uint32_t slices, uint32_t dst_slice_pitch, uint32_t pieces) {
-              const kernels::GatherLaunch a =
-                  rows_launch(n, nparts, false, rows, row_bytes, src_pitch, src_col, dst_pitch,
-                              slices, dst_slice_pitch, align_or, group_parts, max_ctas, pieces);
+              const kernels::GatherLaunch a = rows_launch(
+                  n, nparts, false,
+                  {rows, row_bytes, src_pitch, src_col, dst_pitch, slices, dst_slice_pitch, pieces},
+                  align_or, group_parts, max_ctas);
               return plan_dict(kernels::plan_gather_rows(a, sm_count, {resident16, resident32}));
           },
           py::arg("n"), py::arg("nparts"), py::arg("rows"), py::arg("row_bytes"),
@@ -1817,9 +1828,10 @@ PYBIND11_MODULE(_infinistore, m) {
                       uint64_t align_or, uint32_t group_parts, bool write, int max_ctas,
                       int sm_count, int resident, uint32_t slices, uint32_t dst_slice_pitch,
                       uint32_t pieces) {
-              const kernels::GatherLaunch a =
-                  rows_launch(n, nparts, write, rows, row_bytes, src_pitch, src_col, dst_pitch,
-                              slices, dst_slice_pitch, align_or, group_parts, max_ctas, pieces);
+              const kernels::GatherLaunch a = rows_launch(
+                  n, nparts, write,
+                  {rows, row_bytes, src_pitch, src_col, dst_pitch, slices, dst_slice_pitch, pieces},
+                  align_or, group_parts, max_ctas);
               return plan_dict(
                   kernels::plan_gather_fp8_rows(a, elems, sm_count, {resident, resident}));
           },
@@ -1836,9 +1848,10 @@ PYBIND11_MODULE(_infinistore, m) {
                       uint32_t dst_slice_pitch, uint64_t align_or, bool write,
                       uint32_t group_parts, int max_ctas, int sm_count, int resident16,
                       int resident32, uint32_t pieces) {
-              const kernels::GatherLaunch a =
-                  rows_launch(n, nparts, write, rows, row_bytes, src_pitch, src_col, dst_pitch,
-                              slices, dst_slice_pitch, align_or, group_parts, max_ctas, pieces);
+              const kernels::GatherLaunch a = rows_launch(
+                  n, nparts, write,
+                  {rows, row_bytes, src_pitch, src_col, dst_pitch, slices, dst_slice_pitch, pieces},
+                  align_or, group_parts, max_ctas);
               return plan_dict(
                   kernels::plan_gather_rows_write(a, sm_count, {resident16, resident32}));
           },
@@ -1854,9 +1867,10 @@ PYBIND11_MODULE(_infinistore, m) {
                       uint32_t slices, uint32_t dst_slice_pitch, uint64_t align_or, bool write,
                       uint32_t group_parts, int max_ctas, int sm_count, int resident,
                       uint32_t pieces) {
-              const kernels::GatherLaunch a =
-                  rows_launch(n, nparts, write, rows, row_bytes, src_pitch, src_col, dst_pitch,
-                              slices, dst_slice_pitch, align_or, group_parts, max_ctas, pieces);
+              const kernels::GatherLaunch a = rows_launch(
+                  n, nparts, write,
+                  {rows, row_bytes, src_pitch, src_col, dst_pitch, slices, dst_slice_pitch, pieces},
+                  align_or, group_parts, max_ctas);
               return plan_dict(
                   kernels::plan_gather_fp8_rows_write(a, elems, sm_count, {resident, resident}));
           },
