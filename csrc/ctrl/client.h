@@ -207,7 +207,11 @@ class Connection {
         // call's offsets; run t of block i is at part_base[s] + the block's offset +
         // piece_off[i * rows.pieces + t]
         const uint64_t* piece_off = nullptr;
-        // pool bytes of a part: part_bytes, or kernels::fp8_gather_bytes(1, fp8_elems)
+        // fp8 parts only: records.latent != 0 stores every part as fp8_elems / token_elems()
+        // token records (kernels::Fp8Records) instead of an fp8 page; whole parts only
+        kernels::Fp8Records records;
+        // pool bytes of a part: part_bytes, kernels::fp8_gather_bytes(1, fp8_elems), or with
+        // records kernels::fp8_records_bytes(1, fp8_elems, records)
         uint64_t pool_part_bytes() const;
         // bytes of a part in the caller's tensors: part_bytes, or 2 * fp8_elems (bf16)
         uint64_t view_part_bytes() const { return fp8_elems ? 2ull * fp8_elems : part_bytes; }
@@ -233,6 +237,7 @@ class Connection {
         int device = -2;                  // fixed by the first call (-1: host tensors)
         uint64_t scale = 0;               // bytes per offset unit, fixed by the first call
         uint32_t fp8_elems = 0;           // fp8 elements per part (0: raw bytes), first call
+        kernels::Fp8Records records;      // GatherSpec::records of the first call
         uint32_t part_bytes = 0;          // pool bytes of a part, first call
         bool failed = false;
         void* event = nullptr;            // cudaEvent_t recorded after the last launch
@@ -248,8 +253,8 @@ class Connection {
                                                 const uint64_t* piece_off = nullptr,
                                                 uint32_t pieces = 1);
     // Stores parts g.first_part .. g.first_part + g.nparts - 1 of every block of `w`; offsets
-    // are scaled by `scale`.  Refuses part ranges written before, a device, scale, fp8_elems
-    // or part size other than the first call's, a complete or failed writer, and a writer made
+    // are scaled by `scale`.  Refuses part ranges written before, a device, scale, fp8_elems,
+    // records or part size other than the first call's, a complete or failed writer, and a writer made
     // before the connection was last closed (its blocks and index ways were released).  A
     // refused call leaves the writer as it was.
     int write_layered(GatherWriter& w, const GatherSpec& g, uint64_t scale, int device,

@@ -290,6 +290,7 @@ kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n,
     G.stage_bytes = pipe_stage_;
     G.ring_bytes = pipe_ring_;
     G.rows = g.rows;  // the caller stages the piece table beside the descriptors
+    G.records = g.records;
     return G;
 }
 
@@ -857,7 +858,9 @@ int Connection::r_rdma(const std::vector<KeyOffset>& blocks, int block_size, uin
 }
 
 uint64_t Connection::GatherSpec::pool_part_bytes() const {
-    return fp8_elems ? kernels::fp8_gather_bytes(1, fp8_elems) : part_bytes;
+    if (!fp8_elems) return part_bytes;
+    return records.latent ? kernels::fp8_records_bytes(1, fp8_elems, records)
+                          : kernels::fp8_gather_bytes(1, fp8_elems);
 }
 
 // Bytes a stored block must hold to serve the read: every part asked for.
@@ -889,9 +892,21 @@ const char* Connection::gather_refusal(const GatherSpec& g, const uint64_t* offs
                                        int device, bool write, const GatherWriter* w) const {
     if (!g.part_base || g.nparts < 1 || g.nparts > kernels::kGatherMaxParts)
         return "bad parts list: 1 to GATHER_MAX_PARTS parts";
-    if (g.fp8_elems ? g.fp8_elems % 512 || g.fp8_elems > uint32_t(INT32_MAX) : !g.part_bytes)
+    if (g.records.latent) {  // token records: whole parts of whole tokens, bf16 in the tensors
+        if (!g.fp8_elems) return "fp8 records need fp8 parts (bf16 elements in the tensors)";
+        if (!g.records.ok())
+            return "bad fp8 records: latent a positive multiple of 128, rope a multiple of 8, and "
+                   "a record (latent + 4 * latent / 128 + 2 * rope bytes) a multiple of 16 bytes";
+        if (g.fp8_elems % g.records.token_elems() || g.fp8_elems > uint32_t(INT32_MAX))
+            return "bad part size for fp8 records: a whole number of tokens of latent + rope "
+                   "elements";
+        if (g.rows.rows || g.rows.pieces != 1 || g.piece_off)
+            return "fp8 records take whole parts: no row geometry or pieces";
+    } else if (g.fp8_elems ? g.fp8_elems % 512 || g.fp8_elems > uint32_t(INT32_MAX)
+                           : !g.part_bytes) {
         return "bad part size: raw parts of 1 byte or more, fp8 parts of a multiple of 512 "
                "elements";
+    }
     const uint64_t end = uint64_t(g.first_part) + g.nparts;
     const uint64_t block_parts = w ? w->nparts : write ? g.nparts : end;
     if (end > block_parts) return "the part range runs past the block";
@@ -1030,8 +1045,9 @@ int Connection::write_layered(GatherWriter& w, const GatherSpec& g, uint64_t sca
     else if (w.failed || w.complete())
         bad = "the writer is complete or has failed";
     else if (!first && (device != w.device || scale != w.scale || g.fp8_elems != w.fp8_elems ||
+                        g.records.latent != w.records.latent || g.records.rope != w.records.rope ||
                         g.pool_part_bytes() != w.part_bytes))
-        bad = "device, element size or part size differ from the writer's first call";
+        bad = "device, element size, records or part size differ from the writer's first call";
     // every check before the writer changes: the first call's offsets are still in elements
     std::vector<uint64_t> scaled, scaled_pieces;
     if (!bad && first) {
@@ -1057,6 +1073,7 @@ int Connection::write_layered(GatherWriter& w, const GatherSpec& g, uint64_t sca
         w.device = device;
         w.scale = scale;
         w.fp8_elems = g.fp8_elems;
+        w.records = g.records;
         w.part_bytes = uint32_t(g.pool_part_bytes());
         w.offsets.swap(scaled);
         w.piece_off.swap(scaled_pieces);

@@ -240,6 +240,30 @@ struct PartRows {
     }
 };
 
+// fp8 token records (GatherLaunch::records, the connection's GatherSpec::records): the stored
+// form of an MLA latent page.  A part is `tokens` tokens of latent + rope bf16 elements,
+// [token][latent + rope] in the caller's tensors, and each token is stored as one record
+//   [latent x e4m3][latent / 128 x fp32 scale][rope x bf16, verbatim]
+// (656 bytes for 512 + 64).  Each 128-element run of a token's latent is one row of the fp8 row
+// contract (fp8_row.cuh).  Token t of stored part s lies at (s * tokens + t) * record_bytes()
+// from the block (launch_plan.h: fp8_record_offset).  latent == 0: no records.
+struct Fp8Records {
+    uint32_t latent = 0, rope = 0;
+
+    ISTORE_KHD uint32_t token_elems() const { return latent + rope; }
+    // byte offsets inside a record: the scales, then the rope elements
+    ISTORE_KHD uint32_t scale_offset() const { return latent; }
+    ISTORE_KHD uint32_t rope_offset() const { return latent + 4 * (latent / 128); }
+    ISTORE_KHD uint32_t record_bytes() const { return rope_offset() + 2 * rope; }
+    // Every access of the movers is a 16-byte vector (bf16 tokens, rope runs) or lies inside
+    // one (e4m3 runs, scales): latent a positive multiple of 128, rope a multiple of 8, and a
+    // record of a multiple of 16 bytes (which makes the rope offset one too).
+    bool ok() const {
+        return latent != 0 && latent % 128 == 0 && rope % 8 == 0 && latent <= (1u << 20) &&
+               rope <= (1u << 20) && record_bytes() % 16 == 0;
+    }
+};
+
 struct GatherLaunch {
     // per block, device-addressable: write {local byte offset, pool address},
     // read {pool address or 0 = miss, local byte offset}
@@ -288,6 +312,9 @@ struct GatherLaunch {
     // rows.pieces > 1: device-addressable byte offsets, one row of rows.pieces per descriptor.
     // align_or covers every piece offset.
     const uint64_t* piece_off = nullptr;
+    // fp8 launches only (launch_kv_gather_fp8): records.latent != 0 stores each part as token
+    // records (Fp8Records) instead of an fp8 page.  Whole parts only (rows.rows == 0).
+    Fp8Records records;
 };
 // The TMA pipeline for 16-byte aligned parts of at least kPipeMinBytes, the ld/st kernel
 // (kv_copy.cu) otherwise: the same rule launch_kv_copy applies to whole blocks.  Reads run
@@ -353,8 +380,13 @@ cudaError_t launch_kv_read_fp8(const Fp8Launch& a, cudaStream_t stream);
 // Every part of a block is byte-identical to the block launch_kv_write_fp8 stores for that
 // page.  variant kFp8LdSt: the ld/st kernels (kv_fp8.cu), anything else: the TMA pipeline with
 // 8 compute warps (kv_fp8_pipe.cu).  Part bases and local offsets must be 16-byte aligned.
+// With a.records.latent != 0 the parts are token records instead (kv_fp8_records.cu): elems is
+// a whole number of tokens, the ld/st kernels run whatever the variant, and the block holds
+// fp8_records_bytes(nparts, elems, a.records) bytes.
 cudaError_t launch_kv_gather_fp8(const GatherLaunch& a, uint32_t elems, int variant,
                                  cudaStream_t stream);
+cudaError_t launch_kv_gather_fp8_records(const GatherLaunch& a, uint32_t elems,
+                                         cudaStream_t stream);
 cudaError_t launch_kv_fp8_pipe_gather(const GatherLaunch& a, uint32_t elems, cudaStream_t stream);
 
 // Device-side key lookup: hash the packed key bytes, probe the index, and either build

@@ -436,4 +436,42 @@ inline LaunchPlan plan_gather_fp8_rows(const GatherLaunch& a, uint32_t elems, in
     return p;
 }
 
+// ---------------------------------------------------------------- fp8 token records
+// The geometry of gathered fp8 records (GatherLaunch::records, kv_fp8_records.cu), shared with
+// the connection and the CPU tests (_infinistore.testing.fp8_record_offset /
+// fp8_records_bytes / plan_gather_fp8_records).  A part of `elems` bf16 elements is
+// elems / token_elems tokens, stored as that many records end to end, part after part.
+ISTORE_KHD inline uint64_t fp8_record_offset(const Fp8Records& r, uint32_t tokens, uint32_t s,
+                                             uint32_t t) {
+    return (uint64_t(s) * tokens + t) * r.record_bytes();
+}
+inline uint64_t fp8_records_bytes(uint32_t nparts, uint32_t elems, const Fp8Records& r) {
+    return r.token_elems() ? fp8_record_offset(r, elems / r.token_elems(), nparts, 0) : 0;
+}
+
+// Reads (plain or layered) and writes of whole parts as records: always the ld/st kernels.
+// A work item is a run of `chunk` tokens of one part, about kFp8Chunk elements, or every token
+// of the part under ldst_items' rule; cpb is runs per part, and a layered read numbers items with
+// layered_item as whole parts do.  Refused: bad records (Fp8Records::ok), a part that is not a
+// whole number of tokens, row geometry, part bases or local offsets that are not 16-byte
+// aligned, and more than kMaxItems work items.  The grid is one wave of the CTAs the kernel
+// keeps resident (res.r16).
+inline LaunchPlan plan_gather_fp8_records(const GatherLaunch& a, uint32_t elems, int sms,
+                                          LdStResident res) {
+    const Fp8Records& r = a.records;
+    const uint64_t parts = uint64_t(a.n) * a.nparts;
+    if (!r.ok() || elems == 0 || elems % r.token_elems() != 0 || a.rows.rows != 0 ||
+        a.rows.pieces != 1 || a.nparts == 0 || a.nparts > kGatherMaxParts || !groups_ok(a) ||
+        (a.align_or & 15) != 0 || parts > kMaxItems)
+        return invalid_plan();
+    const uint32_t te = r.token_elems();
+    LaunchPlan p;
+    p.kernel = Kernel::kLdStFp8;
+    ldst_items(p, parts, elems / te, std::max(1u, kFp8Chunk / te), std::max(1u, (1u << 19) / te),
+               sms);
+    if (parts * p.cpb > kMaxItems) return invalid_plan();
+    p.ctas = clamp_grid(a.max_ctas > 0 ? a.max_ctas : res.r16 * sms, parts * p.cpb);
+    return p;
+}
+
 }  // namespace istore::kernels

@@ -200,15 +200,26 @@ bool parse_rows(const std::vector<uint32_t>& v, uint32_t pieces, kernels::PartRo
     return true;
 }
 
+// fp8 token records from their native list: (latent, rope) elements, or empty for none.
+kernels::Fp8Records parse_records(const std::vector<uint32_t>& v) {
+    if (v.empty()) return {};
+    if (v.size() != 2 || v[0] == 0)
+        throw py::value_error("records is (latent, rope) with latent > 0, or empty");
+    return kernels::Fp8Records{v[0], v[1]};
+}
+
 // A gathered call's parts: part s at part_base[s] (which must outlive the spec); elems > 0:
-// bf16 parts of elems elements stored as fp8 pages.  rows: a row-sliced read's or write's
-// geometry (parse_rows); empty: whole parts.  The connection checks the values.
+// bf16 parts of elems elements stored as fp8 pages, or with records (parse_records) as token
+// records.  rows: a row-sliced read's or write's geometry (parse_rows); empty: whole parts.
+// The connection checks the values.
 Connection::GatherSpec gather_spec(const std::vector<uint64_t>& part_base, uint32_t part_bytes,
                                    uint32_t elems, uint32_t first_part,
                                    const std::vector<uint32_t>& rows = {},
                                    const std::vector<uint64_t>* piece_off = nullptr,
-                                   uint32_t pieces = 1) {
+                                   uint32_t pieces = 1,
+                                   const std::vector<uint32_t>& records = {}) {
     Connection::GatherSpec g;
+    g.records = parse_records(records);
     if (pieces > 1) g.piece_off = piece_off->data();
     g.part_base = part_base.data();
     g.nparts = uint32_t(part_base.size());
@@ -634,7 +645,7 @@ PYBIND11_MODULE(_infinistore, m) {
             [](Connection& c, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
                uint32_t elems, const py::object& offsets, const py::object& remote_blocks,
                int device, uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows,
-               const py::object& piece_off, uint32_t pieces) {
+               const py::object& piece_off, uint32_t pieces, const std::vector<uint32_t>& records) {
                 BlockSpan rb;
                 OffsetSpan off;
                 blocks_from_py(remote_blocks, rb);
@@ -643,7 +654,7 @@ PYBIND11_MODULE(_infinistore, m) {
                 for (size_t i = 0; i < off.n; ++i) bytes[i] = off.data[i] * scale;
                 const std::vector<uint64_t> table = piece_table(piece_off, off.n, pieces, scale);
                 const Connection::GatherSpec g =
-                    gather_spec(part_base, part_bytes, elems, 0, rows, &table, pieces);
+                    gather_spec(part_base, part_bytes, elems, 0, rows, &table, pieces, records);
                 py::gil_scoped_release rel;
                 return c.w_rdma_gather(g, bytes.data(), bytes.size(), rb.data, rb.n, device, stream);
             },
@@ -651,8 +662,10 @@ PYBIND11_MODULE(_infinistore, m) {
             py::arg("remote_blocks"), py::arg("device") = -1, py::arg("stream") = 0,
             py::arg("scale") = 1, py::arg("rows") = std::vector<uint32_t>{},
             py::arg("piece_off") = py::none(), py::arg("pieces") = 1,
+            py::arg("records") = std::vector<uint32_t>{},
             "gathered write: block i = part s at part_base[s] + offsets[i] * scale, s = 0..S-1; "
-            "elems > 0: bf16 parts of elems elements, quantised into fp8 page s of block i; "
+            "elems > 0: bf16 parts of elems elements, quantised into fp8 page s of block i, or "
+            "with records = (latent, rope) into elems / (latent + rope) fp8 token records; "
             "rows = (rows, row_bytes, src_pitch, 0, dst_pitch[, slices, dst_slice_pitch]) filling "
             "each stored part: slice j of stored row r from part_base[s] + offset + r * "
             "dst_pitch + j * dst_slice_pitch; pieces > 1 (with rows): piece_off holds pieces "
@@ -664,12 +677,12 @@ PYBIND11_MODULE(_infinistore, m) {
                uint32_t elems, uint32_t first_part, const py::object& blocks, int device,
                uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows,
                Connection::ScatterReader* reader, uint32_t group_parts, const py::object& piece_off,
-               uint32_t pieces) {
+               uint32_t pieces, const std::vector<uint32_t>& records) {
                 std::vector<KeyOffset> kb;
                 blocks_list_from_py(blocks, scale, kb);
                 const std::vector<uint64_t> table = piece_table(piece_off, kb.size(), pieces, scale);
-                Connection::GatherSpec g =
-                    gather_spec(part_base, part_bytes, elems, first_part, rows, &table, pieces);
+                Connection::GatherSpec g = gather_spec(part_base, part_bytes, elems, first_part,
+                                                       rows, &table, pieces, records);
                 g.reader = reader;
                 g.group_parts = group_parts;
                 py::gil_scoped_release rel;
@@ -680,8 +693,10 @@ PYBIND11_MODULE(_infinistore, m) {
             py::arg("scale") = 1, py::arg("rows") = std::vector<uint32_t>{},
             py::arg("reader") = py::none(), py::arg("group_parts") = 0,
             py::arg("piece_off") = py::none(), py::arg("pieces") = 1,
+            py::arg("records") = std::vector<uint32_t>{},
             "scattered read: stored part first_part + s of each block -> part_base[s] + offset; "
-            "elems > 0: fp8 pages dequantised into bf16 parts of elems elements; rows = (rows, "
+            "elems > 0: fp8 pages (or with records, token records) dequantised into bf16 parts "
+            "of elems elements; rows = (rows, "
             "row_bytes, src_pitch, src_col, dst_pitch[, slices, dst_slice_pitch]): only those "
             "rows of each part, slice j of row r to part_base[s] + offset + r * dst_pitch + j * "
             "dst_slice_pitch; reader: a layered read whose parts are "
@@ -728,18 +743,20 @@ PYBIND11_MODULE(_infinistore, m) {
             "w_rdma_layered",
             [](Connection& c, Connection::GatherWriter& w, const std::vector<uint64_t>& part_base,
                uint32_t part_bytes, uint32_t elems, uint32_t first_part, int device,
-               uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows) {
-                const Connection::GatherSpec g =
-                    gather_spec(part_base, part_bytes, elems, first_part, rows);
+               uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows,
+               const std::vector<uint32_t>& records) {
+                const Connection::GatherSpec g = gather_spec(part_base, part_bytes, elems,
+                                                             first_part, rows, nullptr, 1, records);
                 py::gil_scoped_release rel;
                 return c.write_layered(w, g, scale, device, stream);
             },
             py::arg("writer"), py::arg("part_base"), py::arg("part_bytes"), py::arg("elems"),
             py::arg("first_part"), py::arg("device") = -1, py::arg("stream") = 0,
             py::arg("scale") = 1, py::arg("rows") = std::vector<uint32_t>{},
+            py::arg("records") = std::vector<uint32_t>{},
             "layered write: stored part first_part + s of every block of the writer <- "
             "part_base[s] + offset * scale; elems > 0: fp8 parts of elems bf16 elements; rows "
-            "as for w_rdma_gather")
+            "and records as for w_rdma_gather")
         .def(
             "rw_local",
             [](Connection& c, const std::string& op, const py::object& blocks, int block_size,
@@ -1101,7 +1118,7 @@ PYBIND11_MODULE(_infinistore, m) {
            uint64_t align_or, uint64_t layer_state, uint32_t layer_parts, bool layer_claim,
            uint64_t group_flags, uint64_t group_counters, uint32_t group_seq,
            uint32_t group_parts, const std::vector<uint32_t>& rows, uint64_t piece_off,
-           uint32_t pieces) {
+           uint32_t pieces, const std::vector<uint32_t>& records) {
             if (part_base.empty() || part_base.size() > kernels::kGatherMaxParts)
                 throw std::runtime_error("kv_gather_fp8: 1 to GATHER_MAX_PARTS parts");
             if (layer_state && first_part + part_base.size() > layer_parts)
@@ -1135,6 +1152,7 @@ PYBIND11_MODULE(_infinistore, m) {
                 throw std::runtime_error("kv_gather_fp8: rows is 5 or 7 values");
             if (!rows.empty()) G.part_bytes = 2 * elems;  // bytes of the parts' bf16 view
             G.piece_off = as_ptr<const uint64_t>(piece_off);
+            G.records = parse_records(records);
             const cudaError_t e =
                 kernels::launch_kv_gather_fp8(G, elems, variant, as_ptr<CUstream_st>(stream));
             if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
@@ -1147,7 +1165,10 @@ PYBIND11_MODULE(_infinistore, m) {
         py::arg("layer_claim") = false, py::arg("group_flags") = 0, py::arg("group_counters") = 0,
         py::arg("group_seq") = 0, py::arg("group_parts") = 0,
         py::arg("rows") = std::vector<uint32_t>{}, py::arg("piece_off") = 0, py::arg("pieces") = 1,
-        "gathered fp8 blocks: descs as for kv_gather; pieces as for kv_gather; part s (elems bf16 elements at "
+        py::arg("records") = std::vector<uint32_t>{},
+        "gathered fp8 blocks: descs as for kv_gather; records = (latent, rope): every part is "
+        "elems / (latent + rope) bf16 tokens stored as fp8 token records (kv_write_fp8_records, "
+        "kv_read_fp8_records; whole parts, any variant); pieces as for kv_gather; part s (elems bf16 elements at "
         "part_base[s] + local offset) <-> fp8 page first_part + s of the block; layer_* and "
         "group_* as for kv_gather (a layered read always runs the ld/st kernel); rows as for "
         "kv_gather, in bytes of the parts' bf16 view: a read dequantises those rows of each "
@@ -1308,6 +1329,14 @@ PYBIND11_MODULE(_infinistore, m) {
     k.def("fp8_block_bytes", &kernels::fp8_block_bytes);
     k.def("fp8_gather_bytes", &kernels::fp8_gather_bytes, py::arg("nparts"), py::arg("elems"),
           "bytes of nparts fp8 pages of elems elements end to end (a gathered fp8 block)");
+    k.def(
+        "fp8_records_bytes",
+        [](uint32_t nparts, uint32_t elems, uint32_t latent, uint32_t rope) {
+            return kernels::fp8_records_bytes(nparts, elems, kernels::Fp8Records{latent, rope});
+        },
+        py::arg("nparts"), py::arg("elems"), py::arg("latent"), py::arg("rope"),
+        "bytes of a gathered block of nparts parts of elems bf16 elements stored as fp8 token "
+        "records of latent + rope elements");
     k.def(
         "kv_bcast_nvls",
         [](uint64_t descs, uint32_t n, uint32_t bytes, int max_ctas, uint64_t stream,
@@ -1879,6 +1908,54 @@ PYBIND11_MODULE(_infinistore, m) {
           py::arg("slices") = 1, py::arg("dst_slice_pitch") = 0, py::arg("align_or") = 0,
           py::arg("write") = true, py::arg("group_parts") = 0, py::arg("max_ctas") = 0,
           py::arg("sm_count") = 132, py::arg("resident") = 1, py::arg("pieces") = 1);
+    // fp8 token records (kernels/launch_plan.h): the geometry the record movers use
+    t.def(
+        "fp8_records",
+        [](uint32_t latent, uint32_t rope) {
+            const kernels::Fp8Records r{latent, rope};
+            py::dict d;
+            d["ok"] = r.ok();
+            d["token_elems"] = r.token_elems();
+            d["scale_offset"] = r.scale_offset();
+            d["rope_offset"] = r.rope_offset();
+            d["record_bytes"] = r.record_bytes();
+            return d;
+        },
+        py::arg("latent"), py::arg("rope"));
+    t.def(
+        "fp8_record_offset",
+        [](uint32_t latent, uint32_t rope, uint32_t tokens, uint32_t s, uint32_t t) {
+            return kernels::fp8_record_offset(kernels::Fp8Records{latent, rope}, tokens, s, t);
+        },
+        py::arg("latent"), py::arg("rope"), py::arg("tokens"), py::arg("part"), py::arg("token"));
+    t.def(
+        "fp8_records_bytes",
+        [](uint32_t nparts, uint32_t elems, uint32_t latent, uint32_t rope) {
+            return kernels::fp8_records_bytes(nparts, elems, kernels::Fp8Records{latent, rope});
+        },
+        py::arg("nparts"), py::arg("elems"), py::arg("latent"), py::arg("rope"));
+    t.def("plan_gather_fp8_records",
+          [plan_dict](uint32_t n, uint32_t nparts, uint32_t elems, uint32_t latent, uint32_t rope,
+                      uint64_t align_or, uint32_t group_parts, bool write, int max_ctas,
+                      int sm_count, int resident, uint32_t rows) {
+              static uint32_t flags[1];
+              kernels::GatherLaunch a;
+              a.n = n;
+              a.nparts = nparts;
+              a.write = write;
+              a.align_or = align_or;
+              a.group_flags = group_parts ? flags : nullptr;
+              a.group_parts = group_parts;
+              a.max_ctas = max_ctas;
+              a.records = kernels::Fp8Records{latent, rope};
+              a.rows.rows = rows;  // any row geometry is refused
+              return plan_dict(
+                  kernels::plan_gather_fp8_records(a, elems, sm_count, {resident, resident}));
+          },
+          py::arg("n"), py::arg("nparts"), py::arg("elems"), py::arg("latent"), py::arg("rope"),
+          py::arg("align_or") = 0, py::arg("group_parts") = 0, py::arg("write") = false,
+          py::arg("max_ctas") = 0, py::arg("sm_count") = 132, py::arg("resident") = 1,
+          py::arg("rows") = 0);
     t.def("fp8_rows_read_bytes", &fp8_rows_read_bytes, py::arg("rows"), py::arg("row_bytes"),
           py::arg("src_pitch"), py::arg("src_col") = 0,
           "bytes_read of a row-sliced read of one stored fp8 part (geometry in bf16 bytes)");

@@ -19,7 +19,8 @@ _REFERENCE_SURFACE = (
     "register_server", "purge_kv_map", "get_kvmap_len", "check_supported",
 )
 # added here: in-process server control, statistics, checkpoint / resume, row-sliced reads
-_ADDITIONS = ("stop_server", "server_stats", "dump_kv_map", "load_kv_map", "PartRows")
+_ADDITIONS = ("stop_server", "server_stats", "dump_kv_map", "load_kv_map", "PartRows",
+              "FP8Records")
 
 __all__ = [*_REFERENCE_SURFACE, *_ADDITIONS]
 globals().update({_name: getattr(_lib, _name) for _name in __all__})

@@ -21,7 +21,7 @@ from __future__ import annotations
 import asyncio
 import os
 import time
-from typing import List, Tuple
+from typing import List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -413,6 +413,71 @@ class PartRows:
         return out
 
 
+class FP8Records:
+    """fp8 token records: how a gathered fp8 call stores each part when its parts are MLA
+    latent pages (``records=`` on ``rdma_write_cache_gather_fp8``, ``read_cache_scatter_fp8``,
+    ``read_cache_scatter_layered(fp8=True)``, ``gather_writer(fp8=True)`` and
+    ``fp8_gather_block_bytes``).  A part of ``part_size`` bf16 elements is ``part_size //
+    token_dim`` tokens of ``latent_dim + rope_dim`` elements, ``[token][latent + rope]``, and
+    each token is stored as one record::
+
+        [latent_dim x e4m3][latent_dim / 128 x fp32 scale][rope_dim x bf16, verbatim]
+
+    Each 128-element run of a token's latent is one row of the fp8 row contract (one scale per
+    run, the rules of every fp8 page); the RoPE elements, which do not tolerate fp8, are copied
+    as they are, NaN payloads included.  512 + 64 gives 656-byte records, 0.57 of the bf16
+    bytes.  Only whole parts: no ``rows=``."""
+
+    __slots__ = ("latent_dim", "rope_dim")
+
+    def __init__(self, latent_dim: int = 512, rope_dim: int = 64):
+        self.latent_dim, self.rope_dim = int(latent_dim), int(rope_dim)
+
+    def __repr__(self):
+        return f"FP8Records(latent_dim={self.latent_dim}, rope_dim={self.rope_dim})"
+
+    def __eq__(self, other):
+        return (isinstance(other, FP8Records) and self.latent_dim == other.latent_dim
+                and self.rope_dim == other.rope_dim)
+
+    def __hash__(self):
+        return hash((self.latent_dim, self.rope_dim))
+
+    @property
+    def token_dim(self) -> int:
+        return self.latent_dim + self.rope_dim
+
+    @property
+    def record_bytes(self) -> int:
+        """Bytes of one token's record."""
+        return self.latent_dim + 4 * (self.latent_dim // 128) + 2 * self.rope_dim
+
+    def check(self, part_size: Optional[int] = None) -> None:
+        """Raises ``ValueError`` unless the geometry is one the record movers take
+        (``latent_dim`` a positive multiple of 128, ``rope_dim`` a multiple of 8 and a record
+        of a multiple of 16 bytes) and, when given, ``part_size`` is a positive whole number of
+        tokens."""
+        if self.latent_dim < 128 or self.latent_dim % 128 or self.rope_dim < 0 or self.rope_dim % 8:
+            raise ValueError(f"{self}: latent_dim must be a positive multiple of 128 and "
+                             f"rope_dim a multiple of 8")
+        if self.latent_dim > 1 << 20 or self.rope_dim > 1 << 20:
+            raise ValueError(f"{self}: latent_dim and rope_dim are at most 2^20")
+        if self.record_bytes % 16:
+            raise ValueError(f"{self}: a record of {self.record_bytes} bytes is not a multiple "
+                             f"of 16 bytes")
+        if part_size is not None and (int(part_size) <= 0 or int(part_size) % self.token_dim):
+            raise ValueError(f"{self}: part_size {int(part_size)} is not a whole number of "
+                             f"{self.token_dim}-element tokens")
+
+    def native(self) -> list:
+        """(latent, rope) for the connection."""
+        return [self.latent_dim, self.rope_dim]
+
+
+def _native_records(records: "FP8Records | None") -> list:
+    return records.native() if records is not None else []
+
+
 def _raise_if_fp8_pages_unaligned(cache: torch.Tensor, offsets) -> None:
     """After a refused fp8 call: ValueError when a page (``offsets`` in elements of ``cache``)
     does not start 16-byte aligned.  The fp8 kernels move bf16 in 16-byte vectors, so the
@@ -707,7 +772,8 @@ class InfinityConnection:
     # ------------------------------------------------------------------ gathered blocks
     def _gather_parts(self, parts, offsets, part_size: int, first_part: int = 0,
                       block_parts=None, fp8: bool = False, rows: "PartRows | None" = None, *,
-                      nblocks=None, stream="current", write: bool = False):
+                      nblocks=None, stream="current", write: bool = False,
+                      records: "FP8Records | None" = None):
         """Checks a gathered call before anything is enqueued: parts ``first_part ..
         first_part + len(parts) - 1`` of the blocks at ``offsets`` (elements, a list or an int64
         ndarray; ``nblocks`` of them when given), in a parts list ``[(tensor, base), ...]``, of
@@ -718,11 +784,21 @@ class InfinityConnection:
         part (``src_offset == 0`` and ``slices * width == src_pitch``).  2-D ``offsets``
         ``(n, k)`` (with ``rows``, ``k`` dividing ``rows.count``): piece i of every part of
         block b, rows ``i * count / k .. (i + 1) * count / k - 1``, is at ``offsets[b, i]``;
-        ``k == 1`` is the 1-D call.  Returns (absolute byte address of every part, device
+        ``k == 1`` is the 1-D call.  ``records`` (an :class:`FP8Records`, with ``fp8``): the
+        parts are stored as token records, ``part_size`` a whole number of tokens, no ``rows``.
+        Returns (absolute byte address of every part, device
         ordinal or -1, element size, int64 offsets, stream handle, piece table): with pieces
         the offsets are zeros and the piece table is the ``(n, k)`` offsets, else None."""
         if self._mode != "rdma":
             raise Exception("gathered blocks need a connected rdma connection")
+        if records is not None:
+            if not isinstance(records, FP8Records):
+                raise ValueError(f"records must be an FP8Records, not {type(records).__name__}")
+            if not fp8:
+                raise ValueError("records= stores fp8 token records: it needs an fp8 call")
+            if rows is not None:
+                raise ValueError("records= takes whole parts: it cannot be combined with rows=")
+            records.check(part_size)
         offs = np.ascontiguousarray(offsets, dtype=np.int64)
         table = None
         if offs.ndim == 2 and offs.shape[1] == 1:
@@ -769,7 +845,8 @@ class InfinityConnection:
             raise ValueError("part_size must be positive")
         first = parts[0][0]
         es = first.element_size()
-        pool_part = self.fp8_gather_block_bytes(1, part_size) if fp8 else part_size * es
+        pool_part = (self.fp8_gather_block_bytes(1, part_size, records=records) if fp8
+                     else part_size * es)
         nparts = first_part + len(parts) if block_parts is None else int(block_parts)
         if nparts * pool_part > _GATHER_MAX_BLOCK_BYTES:
             raise ValueError(f"{nparts} parts of {pool_part} bytes exceed the "
@@ -792,7 +869,7 @@ class InfinityConnection:
         if fp8:
             if first.dtype != torch.bfloat16:
                 raise ValueError(f"fp8 gathered blocks take bf16 tensors, not {first.dtype}")
-            if part_size % 512:
+            if records is None and part_size % 512:
                 raise ValueError(f"fp8 gathered blocks need a part_size that is a multiple of "
                                  f"512 elements, not {part_size}")
             if rows is not None and any(v % 8 for v in (
@@ -892,14 +969,24 @@ class InfinityConnection:
 
     # ------------------------------------------------------------------ gathered fp8 blocks
     @staticmethod
-    def fp8_gather_block_bytes(nparts: int, part_size: int) -> int:
+    def fp8_gather_block_bytes(nparts: int, part_size: int,
+                               records: "FP8Records | None" = None) -> int:
         """Pool bytes of a gathered fp8 block of ``nparts`` parts of ``part_size`` bf16
         elements (what to pass to ``allocate_rdma``): ``nparts`` fp8 pages end to end, each
-        ``fp8_page_bytes(part_size)``."""
-        return _infinistore.kernels.fp8_gather_bytes(int(nparts), int(part_size))
+        ``fp8_page_bytes(part_size)``.  With ``records`` (an :class:`FP8Records`; ValueError
+        unless ``part_size`` is a whole number of its tokens): ``nparts * part_size //
+        token_dim`` records of ``records.record_bytes`` bytes."""
+        if records is None:
+            return _infinistore.kernels.fp8_gather_bytes(int(nparts), int(part_size))
+        if not isinstance(records, FP8Records):
+            raise ValueError(f"records must be an FP8Records, not {type(records).__name__}")
+        records.check(part_size)
+        return _infinistore.kernels.fp8_records_bytes(int(nparts), int(part_size),
+                                                      records.latent_dim, records.rope_dim)
 
     def rdma_write_cache_gather_fp8(self, parts, offsets, part_size: int, remote_blocks,
-                                    stream="current", rows: "PartRows | None" = None):
+                                    stream="current", rows: "PartRows | None" = None,
+                                    records: "FP8Records | None" = None):
         """``rdma_write_cache_gather`` with every part quantised to e4m3 (one fp32 scale per
         128 elements) inside the write kernel: part ``s`` of a block is the fp8 page that
         ``rdma_write_cache_fp8`` would store for it, at byte
@@ -908,22 +995,30 @@ class InfinityConnection:
         elements, and part bases and offsets are 16-byte aligned.  The blocks must have been
         allocated with ``fp8_gather_block_bytes(len(parts), part_size)`` bytes.  ``rows`` as
         for ``rdma_write_cache_gather``, in multiples of 8 elements: each stored page is the
-        one the write without rows stores for the transposed page."""
+        one the write without rows stores for the transposed page.
+
+        ``records`` (an :class:`FP8Records`): part ``s`` is stored as token records instead,
+        ``part_size // records.token_dim`` of them from byte
+        ``fp8_gather_block_bytes(s, part_size, records=records)``; allocate
+        ``fp8_gather_block_bytes(len(parts), part_size, records=records)`` bytes.  No
+        ``rows``."""
         bases, dev, es, offs, s, table = self._gather_parts(parts, offsets, part_size, fp8=True,
                                                             rows=rows, nblocks=len(remote_blocks),
-                                                            stream=stream, write=True)
+                                                            stream=stream, write=True,
+                                                            records=records)
         native_rows = rows.native(es) if rows is not None else []
         if not len(offs):
             return 0
         ret = self.conn.w_rdma_gather(bases, int(part_size) * es, int(part_size), offs,
                                       remote_blocks, dev, s, es, native_rows,
-                                      **_piece_args(table))
+                                      **_piece_args(table), records=_native_records(records))
         if ret < 0:
             raise Exception(f"Failed to write to infinistore, ret = {ret}: {self.conn.last_error()}")
         return 0
 
     def read_cache_scatter_fp8(self, parts, blocks, part_size: int, first_part: int = 0,
-                               stream="current", rows: "PartRows | None" = None):
+                               stream="current", rows: "PartRows | None" = None,
+                               records: "FP8Records | None" = None):
         """Read blocks written by ``rdma_write_cache_gather_fp8``: fp8 page ``first_part + s``
         of every block is dequantised into part ``s`` (``blocks``, misses and ``first_part`` as
         for ``read_cache_scatter``).  With ``device_lookup`` a stored block shorter than
@@ -934,25 +1029,32 @@ class InfinityConnection:
         only those rows, as ``read_cache_scatter(rows=...)`` does, dequantising each with its
         128-element group's scale: the result is bit for bit the same rows of a whole-part
         read.  ``width``, ``src_pitch``, ``src_offset`` and ``dst_pitch`` must be multiples of 8
-        elements; rows need not line up with the scale groups."""
+        elements; rows need not line up with the scale groups.
+
+        ``records`` (an :class:`FP8Records`, what the writer used): the blocks hold token
+        records, each dequantised latent row bit for bit ``bf16_rne(e4m3 * scale)`` and the
+        RoPE elements copied back verbatim.  With ``device_lookup`` a stored block shorter than
+        ``fp8_gather_block_bytes(first_part + len(parts), part_size, records=records)`` is a
+        miss.  No ``rows``."""
         keys, offs = _split_blocks(blocks)
         bases, dev, es, offs, s, table = self._gather_parts(parts, offs, part_size, first_part,
                                                             fp8=True, rows=rows,
-                                                            nblocks=len(keys), stream=stream)
+                                                            nblocks=len(keys), stream=stream,
+                                                            records=records)
         native_rows = rows.native(es) if rows is not None else []
         if not len(offs):
             return
         ret = self.conn.r_rdma_scatter(bases, int(part_size) * es, int(part_size), int(first_part),
                                        (keys, offs), dev, s, es, native_rows,
-                                       **_piece_args(table))
+                                       **_piece_args(table), records=_native_records(records))
         if ret < 0:
             raise Exception(f"Failed to read to infinistore, ret = {ret}: {self.conn.last_error()}")
 
     # ------------------------------------------------------------------ layered scattered reads
     def read_cache_scatter_layered(self, parts, blocks, part_size: int, group_parts: int = 2,
                                    first_part: int = 0, fp8: bool = False,
-                                   stream="current", rows: "PartRows | None" = None
-                                   ) -> "ScatterRead":
+                                   stream="current", rows: "PartRows | None" = None,
+                                   records: "FP8Records | None" = None) -> "ScatterRead":
         """``read_cache_scatter`` (``read_cache_scatter_fp8`` with ``fp8``) in one call whose
         parts are released to consumers group by group: group ``g`` is parts
         ``g * group_parts .. g * group_parts + group_parts - 1`` of every block (with the
@@ -966,11 +1068,12 @@ class InfinityConnection:
         read's post-copy index check: when ``sync()`` reports a miss, treat the whole read as
         failed, as for any read.  A missing key on a connection without ``device_lookup``
         raises here; the exception's ``read`` attribute is the failed reader.  ``rows`` as for
-        ``read_cache_scatter[_fp8]``."""
+        ``read_cache_scatter[_fp8]``, ``records`` (with ``fp8``) as for
+        ``read_cache_scatter_fp8``."""
         keys, offs = _split_blocks(blocks)
         bases, dev, es, offs, s, table = self._gather_parts(parts, offs, part_size, first_part,
                                                             fp8=fp8, rows=rows, nblocks=len(keys),
-                                                            stream=stream)
+                                                            stream=stream, records=records)
         if dev < 0:
             raise ValueError("layered reads take CUDA tensors")
         if not self.conn.server_has_hbm():
@@ -982,7 +1085,7 @@ class InfinityConnection:
         self.conn.r_rdma_scatter(bases, int(part_size) * es, int(part_size) if fp8 else 0,
                                  int(first_part), (keys, offs), dev, s, es,
                                  rows.native(es) if rows is not None else [], native, group_parts,
-                                 **_piece_args(table))
+                                 **_piece_args(table), records=_native_records(records))
         read = ScatterRead(self, native, parts[0][0].device)
         if native.failed:
             err = Exception(f"Failed to read to infinistore: {self.conn.last_error()}")
@@ -992,7 +1095,7 @@ class InfinityConnection:
 
     # ------------------------------------------------------------------ layered gathered writes
     def gather_writer(self, remote_blocks, offsets, nparts: int, part_size: int,
-                      fp8: bool = False) -> "GatherWriter":
+                      fp8: bool = False, records: "FP8Records | None" = None) -> "GatherWriter":
         """A writer that stores the ``nparts`` parts of gathered blocks over several calls, as
         prefill produces them (``GatherWriter.write``), instead of in one call after the last
         layer.  ``remote_blocks`` were allocated with ``nparts * part_size * element_size``
@@ -1001,9 +1104,18 @@ class InfinityConnection:
         readable once all of its parts have landed; until then it is missing to reads and
         ``check_exist`` and, like any allocated key, counted by ``get_match_last_index``.
         Blocks the server marked as already existing are skipped.  A writer that never
-        completes leaves its blocks uncommitted; closing the connection releases them."""
+        completes leaves its blocks uncommitted; closing the connection releases them.
+        ``records`` (an :class:`FP8Records`, with ``fp8``): every call stores token records,
+        and the blocks were allocated with ``fp8_gather_block_bytes(nparts, part_size,
+        records=records)`` bytes."""
         if self._mode != "rdma":
             raise Exception("gathered blocks need a connected rdma connection")
+        if records is not None:
+            if not isinstance(records, FP8Records):
+                raise ValueError(f"records must be an FP8Records, not {type(records).__name__}")
+            if not fp8:
+                raise ValueError("records= stores fp8 token records: it needs fp8=True")
+            records.check(part_size)
         offs = np.ascontiguousarray(offsets, dtype=np.int64)
         if offs.ndim == 2 and offs.shape[1] == 1:
             offs = offs[:, 0]
@@ -1021,7 +1133,7 @@ class InfinityConnection:
         native = self.conn.gather_writer(
             remote_blocks, offs if table is None else np.zeros(len(offs), dtype=np.int64),
             int(nparts), **_piece_args(table))
-        return GatherWriter(self, native, offs, int(nparts), int(part_size), bool(fp8))
+        return GatherWriter(self, native, offs, int(nparts), int(part_size), bool(fp8), records)
 
     async def read_cache_async(self, cache: torch.Tensor, blocks: List[Tuple[str, int]],
                                page_size: int, stream="current"):
@@ -1257,13 +1369,14 @@ class GatherWriter:
     calls; ``sync()`` commits the blocks completed so far."""
 
     def __init__(self, conn: "InfinityConnection", native, offsets: np.ndarray, nparts: int,
-                 part_size: int, fp8: bool):
+                 part_size: int, fp8: bool, records: "FP8Records | None" = None):
         self._conn = conn
         self._w = native
         self._offs = offsets
         self.nparts = nparts
         self.part_size = part_size
         self.fp8 = fp8
+        self.records = records
         self._dev = None  # (device, dtype) of the first call
 
     @property
@@ -1301,7 +1414,7 @@ class GatherWriter:
             raise ValueError("a writer made with 2-D offsets (pieces) needs rows= on every call")
         bases, dev, es, _, s, _ = conn._gather_parts(parts, self._offs, self.part_size, first_part,
                                                      self.nparts, self.fp8, rows, stream=stream,
-                                                     write=True)
+                                                     write=True, records=self.records)
         native_rows = rows.native(es) if rows is not None else []
         first = parts[0][0]
         if self._dev is not None and self._dev != (first.device, first.dtype):
@@ -1310,7 +1423,7 @@ class GatherWriter:
         self._dev = (first.device, first.dtype)
         ret = conn.conn.w_rdma_layered(self._w, bases, self.part_size * es,
                                        self.part_size if self.fp8 else 0, first_part, dev, s, es,
-                                       native_rows)
+                                       native_rows, _native_records(self.records))
         if ret < 0:
             raise Exception(f"Failed to write to infinistore, ret = {ret}: "
                             f"{conn.conn.last_error()}")

@@ -57,6 +57,42 @@ LAYOUTS: Dict[str, KVLayout] = {
 }
 
 
+@dataclass(frozen=True)
+class MLALayout:
+    """The KV cache of a multi-head latent attention model (DeepSeek-V2/V3/R1): one latent
+    tensor per layer, each token ``latent_dim`` compressed-KV elements followed by ``rope_dim``
+    decoupled RoPE-key elements.  Every tensor-parallel rank holds the same latent, so the
+    layout has no TP degree and no KV heads."""
+
+    name: str
+    layers: int
+    latent_dim: int = 512
+    rope_dim: int = 64
+    page_tokens: int = 64
+    dtype: torch.dtype = torch.bfloat16
+
+    @property
+    def token_dim(self) -> int:
+        return self.latent_dim + self.rope_dim
+
+    @property
+    def page_elems(self) -> int:
+        """Elements of one layer's page."""
+        return self.page_tokens * self.token_dim
+
+    @property
+    def page_bytes(self) -> int:
+        return self.page_elems * torch.empty((), dtype=self.dtype).element_size()
+
+
+# MLA models (layers; 512 latent + 64 RoPE dimensions each).
+MLA_LAYOUTS: Dict[str, MLALayout] = {
+    "deepseek-v2-lite": MLALayout("deepseek-v2-lite", 27),
+    "deepseek-v2": MLALayout("deepseek-v2", 60),
+    "deepseek-v3": MLALayout("deepseek-v3", 61),
+}
+
+
 def get_layout(name: str, page_tokens: int = 128, dtype: torch.dtype = torch.bfloat16,
                tp: int = 1) -> KVLayout:
     base = LAYOUTS[name]
@@ -131,3 +167,11 @@ def chunk_key(model: str, chunk_tokens: int, tp_rank: int, chunk_hash: str) -> s
     keys of different chunk sizes, and page keys, never resolve to each other's blocks.
     ``chunk_hash`` comes from ``chain_hashes(token_ids, chunk_tokens)``."""
     return f"{model}/L{ALL_LAYERS}/KVx{int(chunk_tokens)}/tp{tp_rank}/{chunk_hash}"
+
+
+def mla_page_key(model: str, page_hash: str, fp8: bool = False) -> str:
+    """Key of one all-layer MLA page (``MLAKVCache.write_pages``): ``model/Lall/MLA/<hash>``,
+    or ``MLA8`` for fp8 token records.  It has no TP field, because every rank at every degree
+    holds the same latent and names the same block; and the stored format is part of the key,
+    so a bf16 reader never resolves an fp8 block, nor the other way round."""
+    return f"{model}/L{ALL_LAYERS}/{'MLA8' if fp8 else 'MLA'}/{page_hash}"

@@ -6,8 +6,17 @@ from typing import List, Optional, Sequence
 import numpy as np
 import torch
 
-from ..lib import _GATHER_MAX_BLOCK_BYTES, PartRows
-from .kv_layout import ALL_LAYERS, KVLayout, chunk_key, page_key, tp_sources
+from ..lib import _GATHER_MAX_BLOCK_BYTES, FP8Records, PartRows
+from .kv_layout import (ALL_LAYERS, KVLayout, MLALayout, chunk_key, mla_page_key, page_key,
+                        tp_sources)
+
+
+def _layer_range(layers: Optional[range], n: int) -> range:
+    """``layers`` (default all ``n``), checked: a non-empty step-1 range within 0..n."""
+    layers = range(n) if layers is None else layers
+    if layers.step != 1 or not len(layers) or layers.start < 0 or layers.stop > n:
+        raise ValueError(f"layers must be a non-empty step-1 range within 0..{n}")
+    return layers
 
 
 def layer_keys(layout: KVLayout, tp_rank: int, layer: int, kv: int,
@@ -118,11 +127,7 @@ class _PagedCache:
         return self._sources(pages, page_hashes, source_tp)
 
     def _check_layers(self, layers: Optional[range]) -> range:
-        layers = range(self.layout.layers) if layers is None else layers
-        if layers.step != 1 or not len(layers) or layers.start < 0 or layers.stop > self.layout.layers:
-            raise ValueError(f"layers must be a non-empty step-1 range within "
-                             f"0..{self.layout.layers}")
-        return layers
+        return _layer_range(layers, self.layout.layers)
 
     def _write_rows(self) -> Optional[PartRows]:
         """How this cache's page fills a stored token-major part on a write: the ``PartRows``
@@ -604,3 +609,152 @@ class HeadMajorKVCache(_PagedCache):
             return None
         return PartRows(tokens, dim, heads * dim, 0, dst_pitch=dim, slices=heads,
                         dst_slice_pitch=tokens * dim)
+
+
+class MLAKVCache:
+    """The KV cache of an MLA model: ``data[layer, page, token]`` is one token's latent and
+    RoPE elements (``layout.token_dim``), vLLM's per-layer MLA block shape stacked over the
+    layers.  All-layer pages are stored under one key per page (``mla_page_key``) as
+    ``layout.layers`` parts, part l being the page of layer l: in bf16 exactly ``data[l,
+    page]``, with ``fp8`` as fp8 token records (:class:`FP8Records`: e4m3 latent with one scale
+    per 128 elements, RoPE kept in bf16), about 0.57 of the bytes.
+
+    The key names no TP rank: every rank holds the same latent, so every rank, at any TP
+    degree, reads the same block, and every rank may call ``write_pages`` - the store keeps
+    the first writer's block.  The methods follow the semantics and refusals of the
+    ``PagedKVCache`` methods of the same names: step-1 layer ranges, first writer wins, a
+    failed read leaves its pages untouched and reported.  ``fp8`` must be what the writer
+    used; bf16 and fp8 pages have different keys."""
+
+    def __init__(self, layout: MLALayout, num_pages: int, device):
+        self.layout = layout
+        self.num_pages = num_pages
+        self.records = FP8Records(layout.latent_dim, layout.rope_dim)
+        self.data = torch.zeros(layout.layers, num_pages, layout.page_tokens, layout.token_dim,
+                                dtype=layout.dtype, device=device)
+        self._registered = set()
+
+    def page_keys(self, page_hashes: Sequence[str], fp8: bool = False) -> List[str]:
+        """Store keys of all-layer pages (``kv_layout.mla_page_key``)."""
+        return [mla_page_key(self.layout.name, h, fp8) for h in page_hashes]
+
+    def _ensure_registered(self, conn):
+        if id(conn) not in self._registered:
+            conn.register_mr(self.data)
+            self._registered.add(id(conn))
+
+    def _parts(self, layers: range):
+        return [(self.data, layer * self.num_pages * self.layout.page_elems) for layer in layers]
+
+    def _offsets(self, pages: Sequence[int], page_hashes: Sequence[str]) -> np.ndarray:
+        if len(pages) != len(page_hashes):
+            raise ValueError(f"{len(pages)} pages for {len(page_hashes)} page hashes")
+        return np.asarray(pages, dtype=np.int64) * self.layout.page_elems
+
+    def _format(self, conn, fp8: bool):
+        """(records or None, bytes of a block) of the format; ValueError before anything is
+        allocated for fp8 with a cache that is not bf16 on a CUDA device."""
+        n = self.layout.layers
+        if not fp8:
+            return None, n * self.layout.page_bytes
+        if self.data.dtype != torch.bfloat16 or self.data.device.type != "cuda":
+            raise ValueError("fp8 MLA pages need a bf16 cache on a CUDA device")
+        return self.records, conn.fp8_gather_block_bytes(n, self.layout.page_elems,
+                                                         records=self.records)
+
+    def write_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
+                    stream="current", fp8: bool = False) -> int:
+        """Upload every layer's latent page of each page under one key per page.  Blocks
+        whose key already exists are skipped (first writer wins).  Returns the number of
+        blocks asked for."""
+        records, nbytes = self._format(conn, fp8)
+        offs = self._offsets(pages, page_hashes)
+        self._ensure_registered(conn)
+        blocks = conn.allocate_rdma(self.page_keys(page_hashes, fp8), nbytes)
+        parts, part = self._parts(range(self.layout.layers)), self.layout.page_elems
+        if fp8:
+            conn.rdma_write_cache_gather_fp8(parts, offs, part, blocks, stream=stream,
+                                             records=records)
+        else:
+            conn.rdma_write_cache_gather(parts, offs, part, blocks, stream=stream)
+        return len(blocks)
+
+    def page_writer(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
+                    fp8: bool = False) -> "MLAPageWriter":
+        """Allocate all-layer pages (as ``write_pages``) and return a writer whose
+        ``write_layers(range(l, l + 1))`` stores layer l right after it has been produced.  A
+        page becomes readable once its last layer has landed."""
+        records, nbytes = self._format(conn, fp8)
+        offs = self._offsets(pages, page_hashes)
+        self._ensure_registered(conn)
+        blocks = conn.allocate_rdma(self.page_keys(page_hashes, fp8), nbytes)
+        return MLAPageWriter(self, conn.gather_writer(blocks, offs, self.layout.layers,
+                                                      self.layout.page_elems, fp8=fp8,
+                                                      records=records))
+
+    def read_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
+                   layers: Optional[range] = None, stream="current", fp8: bool = False) -> int:
+        """Fetch pages written by ``write_pages`` (or ``page_writer``) of any rank into pages
+        ``pages``; ``layers`` (a step-1 range, default all) reads only those layers' parts.
+        A missing page fails the read (it raises, or with ``device_lookup`` ``sync()`` reports
+        the miss) and leaves its pages untouched.  Returns the number of blocks read."""
+        records, _ = self._format(conn, fp8)
+        offs = self._offsets(pages, page_hashes)
+        layers = _layer_range(layers, self.layout.layers)
+        self._ensure_registered(conn)
+        blocks = (self.page_keys(page_hashes, fp8), offs)
+        if fp8:
+            conn.read_cache_scatter_fp8(self._parts(layers), blocks, self.layout.page_elems,
+                                        first_part=layers.start, stream=stream, records=records)
+        else:
+            conn.read_cache_scatter(self._parts(layers), blocks, self.layout.page_elems,
+                                    first_part=layers.start, stream=stream)
+        return len(offs)
+
+    def read_pages_layered(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
+                           layers: Optional[range] = None, fp8: bool = False,
+                           stream="current") -> "PageRead":
+        """``read_pages`` in one call that releases each layer as it lands: the returned
+        reader's ``wait_layer(l, stream)`` makes later work on ``stream`` wait, on the GPU, for
+        layer l.  A layer is released before the read's post-copy index check: when ``sync()``
+        reports a miss, the whole read failed."""
+        records, _ = self._format(conn, fp8)
+        offs = self._offsets(pages, page_hashes)
+        layers = _layer_range(layers, self.layout.layers)
+        self._ensure_registered(conn)
+        read = conn.read_cache_scatter_layered(
+            self._parts(layers), (self.page_keys(page_hashes, fp8), offs), self.layout.page_elems,
+            group_parts=1, first_part=layers.start, fp8=fp8, stream=stream, records=records)
+        return PageRead(read, layers)
+
+    def cached_prefix_pages(self, conn, page_hashes: Sequence[str], fp8: bool = False) -> int:
+        """How many leading pages of this prefix the store holds in this format."""
+        if not page_hashes:
+            return 0
+        try:
+            return conn.get_match_last_index(self.page_keys(page_hashes, fp8)) + 1
+        except Exception:
+            return 0
+
+    def touch_prefix(self, conn, page_hashes: Sequence[str], fp8: bool = False) -> int:
+        """Tell an evicting store (``--evict``) that these pages were just used.  Returns the
+        number of blocks refreshed."""
+        keys = self.page_keys(page_hashes, fp8)
+        return conn.touch(keys) if keys else 0
+
+
+class MLAPageWriter:
+    """Layer-by-layer upload of all-layer MLA pages (``MLAKVCache.page_writer``)."""
+
+    def __init__(self, cache: MLAKVCache, writer):
+        self.cache = cache
+        self.writer = writer
+
+    @property
+    def complete(self) -> bool:
+        return self.writer.complete
+
+    def write_layers(self, layers: range, stream="current") -> None:
+        """Store the latent pages of ``layers`` (a non-empty step-1 range) of every page."""
+        layers = _layer_range(layers, self.cache.layout.layers)
+        self.writer.write(self.cache._parts(layers), layers.start, stream=stream)

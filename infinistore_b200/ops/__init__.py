@@ -349,13 +349,20 @@ def fp8_gather_bytes(nparts: int, elems: int) -> int:
     return K.fp8_gather_bytes(nparts, elems)
 
 
+def fp8_records_bytes(nparts: int, elems: int, latent: int, rope: int) -> int:
+    """Bytes of a gathered block of ``nparts`` parts of ``elems`` bf16 elements stored as fp8
+    token records of ``latent + rope`` elements: part s starts at fp8_records_bytes(s, ...)."""
+    return K.fp8_records_bytes(nparts, elems, latent, rope)
+
+
 def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, write: bool,
                   first_part: int = 0, max_ctas: int = 0, status: Optional[torch.Tensor] = None,
                   align_or: int = 0, publish: Optional[PublishArgs] = None,
                   variant: str = "auto", layer: Optional[LayerState] = None,
                   claim: bool = False, release: Optional[GroupRelease] = None,
                   rows: Optional[Sequence[int]] = None,
-                  pieces: Optional[torch.Tensor] = None) -> None:
+                  pieces: Optional[torch.Tensor] = None,
+                  records: Optional[Sequence[int]] = None) -> None:
     """Gathered fp8 blocks (``kv_gather`` with quantisation): part s of block i is a bf16 page
     of ``elems`` elements at ``part_base[s] + local offset`` and fp8 page first_part + s of
     the block, at byte ``fp8_gather_bytes(first_part + s, elems)``.  ``descs``, ``layer`` and
@@ -372,7 +379,10 @@ def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, wri
     strided local part, as ``kv_gather``'s row write does (kv_write_fp8_rows, whatever the
     variant); the rows must fill the stored part, and ``publish`` / ``layer`` / ``claim`` work
     as without rows.  ``pieces`` as for ``kv_gather`` (kv_read_fp8_pieces,
-    kv_write_fp8_pieces)."""
+    kv_write_fp8_pieces).  ``records`` = (latent, rope): every part is ``elems // (latent +
+    rope)`` bf16 tokens stored as fp8 token records (``lib.FP8Records``; kv_write_fp8_records,
+    kv_read_fp8_records, whatever the variant), part s at byte ``fp8_records_bytes(first_part +
+    s, elems, latent, rope)`` of the block; no ``rows`` or ``pieces``."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
     bases = [int(b) for b in part_base]
     for b in bases:
@@ -384,7 +394,8 @@ def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, wri
                         max_ctas, _stream(descs.device), *pub,
                         status.data_ptr() if status is not None else 0, align_or, *lay,
                         *_release_args(release),
-                        [int(r) for r in rows] if rows is not None else [], *_piece_args(pieces))
+                        [int(r) for r in rows] if rows is not None else [], *_piece_args(pieces),
+                        [int(r) for r in records] if records is not None else [])
 
 
 def fp8_reference(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
