@@ -21,7 +21,7 @@ from __future__ import annotations
 import asyncio
 import os
 import time
-from typing import List, Optional, Tuple
+from typing import List, NamedTuple, Optional, Tuple
 
 import numpy as np
 import torch
@@ -474,8 +474,51 @@ class FP8Records:
         return [self.latent_dim, self.rope_dim]
 
 
-def _native_records(records: "FP8Records | None") -> list:
-    return records.native() if records is not None else []
+def _check_records(records: "FP8Records | None", part_size: int, fp8: bool = True,
+                   rows: "PartRows | None" = None) -> None:
+    """The checks of every ``records=`` (None: no records): an :class:`FP8Records`, of an fp8
+    call without ``rows=``, whose parts are a whole number of its tokens."""
+    if records is None:
+        return
+    if not isinstance(records, FP8Records):
+        raise ValueError(f"records must be an FP8Records, not {type(records).__name__}")
+    if not fp8:
+        raise ValueError("records= stores fp8 token records: it needs an fp8 call")
+    if rows is not None:
+        raise ValueError("records= takes whole parts: it cannot be combined with rows=")
+    records.check(part_size)
+
+
+def _block_offsets(offsets, nblocks: Optional[int] = None) -> np.ndarray:
+    """The local offsets (elements) of gathered blocks as int64: 1-D, or ``(n, k)`` with one
+    column per piece of a block, where ``(n, 1)`` is 1-D.  ValueError for another shape, for
+    other than ``nblocks`` rows (when given) and for a negative offset."""
+    offs = np.atleast_1d(np.ascontiguousarray(offsets, dtype=np.int64))
+    if offs.ndim == 2 and offs.shape[1] == 1:
+        offs = offs[:, 0]
+    elif offs.ndim > 2:
+        raise ValueError("offsets are 1-D, or 2-D with one column per piece")
+    if nblocks is not None and len(offs) != nblocks:
+        raise ValueError(f"{len(offs)} offsets for {nblocks} blocks")
+    if offs.size and int(offs.min()) < 0:
+        raise ValueError("offsets must not be negative")
+    return offs
+
+
+class _Gather(NamedTuple):
+    """A gathered call that passed ``InfinityConnection._gather_parts``: what its native entry
+    takes."""
+
+    bases: List[int]  # absolute byte address of every part
+    dev: int  # device ordinal, or -1 for CPU tensors
+    es: int  # element size
+    offsets: np.ndarray  # int64 block offsets in elements; zeros when pieces carry them
+    stream: int
+    part_bytes: int
+    elems: int  # the part size in elements for fp8, else 0
+    rows: list  # native row geometry (PartRows.native), or []
+    records: list  # native fp8 records (FP8Records.native), or []
+    pieces: dict  # piece arguments (_piece_args), or {}
 
 
 def _raise_if_fp8_pages_unaligned(cache: torch.Tensor, offsets) -> None:
@@ -786,37 +829,19 @@ class InfinityConnection:
         block b, rows ``i * count / k .. (i + 1) * count / k - 1``, is at ``offsets[b, i]``;
         ``k == 1`` is the 1-D call.  ``records`` (an :class:`FP8Records`, with ``fp8``): the
         parts are stored as token records, ``part_size`` a whole number of tokens, no ``rows``.
-        Returns (absolute byte address of every part, device
-        ordinal or -1, element size, int64 offsets, stream handle, piece table): with pieces
-        the offsets are zeros and the piece table is the ``(n, k)`` offsets, else None."""
+        Returns the native call's arguments (``_Gather``): with pieces its offsets are zeros
+        and its piece arguments carry the ``(n, k)`` offsets."""
         if self._mode != "rdma":
             raise Exception("gathered blocks need a connected rdma connection")
-        if records is not None:
-            if not isinstance(records, FP8Records):
-                raise ValueError(f"records must be an FP8Records, not {type(records).__name__}")
-            if not fp8:
-                raise ValueError("records= stores fp8 token records: it needs an fp8 call")
-            if rows is not None:
-                raise ValueError("records= takes whole parts: it cannot be combined with rows=")
-            records.check(part_size)
-        offs = np.ascontiguousarray(offsets, dtype=np.int64)
+        _check_records(records, part_size, fp8, rows)
+        offs = _block_offsets(offsets, nblocks)
         table = None
-        if offs.ndim == 2 and offs.shape[1] == 1:
-            offs = offs[:, 0]
-        elif offs.ndim == 2:
+        if offs.ndim == 2:
             if rows is None:
                 raise ValueError("2-D offsets (one per piece of a block) need rows=")
             if rows.count % offs.shape[1]:
                 raise ValueError(f"{offs.shape[1]} pieces do not divide the {rows.count} rows")
-            table = offs
-            offs = np.zeros(len(table), dtype=np.int64)
-        elif offs.ndim > 2:
-            raise ValueError("offsets are 1-D, or 2-D with one column per piece")
-        offs = offs.reshape(-1)
-        if nblocks is not None and len(offs) != nblocks:
-            raise ValueError(f"{len(offs)} offsets for {nblocks} blocks")
-        if len(offs) and int(offs.min()) < 0:
-            raise ValueError("offsets must not be negative")
+            table, offs = offs, np.zeros(len(offs), dtype=np.int64)
         first_part = int(first_part)
         if first_part < 0:
             raise ValueError("first_part must not be negative")
@@ -825,8 +850,6 @@ class InfinityConnection:
             extent = PartRows(rows.count // k, rows.width, rows.src_pitch, rows.src_offset,
                               dst_pitch=rows.dst_pitch, slices=rows.slices,
                               dst_slice_pitch=rows.dst_slice_pitch).check(int(part_size) // k)
-            if table.size and int(table.min()) < 0:
-                raise ValueError("offsets must not be negative")
         else:
             extent = rows.check(part_size) if rows is not None else int(part_size)
         if write and rows is not None and (rows.src_offset != 0
@@ -891,7 +914,66 @@ class InfinityConnection:
         if dev < 0 and self.conn.server_has_hbm():
             raise ValueError("gathered blocks of CPU tensors need a host-memory pool "
                              "(--pool-backend host)")
-        return bases, dev, es, offs, _stream_of(first, stream), table
+        return _Gather(bases, dev, es, offs, _stream_of(first, stream), part_size * es,
+                       part_size if fp8 else 0, rows.native(es) if rows is not None else [],
+                       records.native() if records is not None else [], _piece_args(table))
+
+    def _gather_write(self, parts, offsets, part_size: int, stream, rows: "PartRows | None",
+                      fp8: bool, records: "FP8Records | None", remote_blocks=None,
+                      writer: "GatherWriter | None" = None, first_part: int = 0) -> None:
+        """The gathered write, bf16 or fp8: into ``remote_blocks`` in one call
+        (``rdma_write_cache_gather[_fp8]``), or parts from ``first_part`` of the blocks of a
+        layered ``writer`` (``GatherWriter.write``)."""
+        one_call = writer is None
+        g = self._gather_parts(parts, offsets, part_size, first_part,
+                               None if one_call else writer.nparts, fp8, rows,
+                               nblocks=len(remote_blocks) if one_call else None, stream=stream,
+                               write=True, records=records)
+        if not one_call:
+            writer._claim(parts[0][0])
+            ret = self.conn.w_rdma_layered(writer._w, g.bases, g.part_bytes, g.elems, first_part,
+                                           g.dev, g.stream, g.es, g.rows, g.records)
+        elif len(g.offsets):
+            ret = self.conn.w_rdma_gather(g.bases, g.part_bytes, g.elems, g.offsets, remote_blocks,
+                                          g.dev, g.stream, g.es, g.rows, **g.pieces,
+                                          records=g.records)
+        else:
+            return
+        if ret < 0:
+            raise Exception(f"Failed to write to infinistore, ret = {ret}: {self.conn.last_error()}")
+
+    def _scatter_read(self, parts, blocks, part_size: int, first_part: int, stream,
+                      rows: "PartRows | None", fp8: bool, records: "FP8Records | None",
+                      group_parts: Optional[int] = None) -> "ScatterRead | None":
+        """The scattered read, bf16 or fp8: ``read_cache_scatter[_fp8]``, or with
+        ``group_parts`` the layered ``read_cache_scatter_layered``, which returns its reader."""
+        keys, offs = _split_blocks(blocks)
+        g = self._gather_parts(parts, offs, part_size, first_part, fp8=fp8, rows=rows,
+                               nblocks=len(keys), stream=stream, records=records)
+        args = (g.bases, g.part_bytes, g.elems, int(first_part), (keys, g.offsets), g.dev,
+                g.stream, g.es, g.rows)
+        if group_parts is None:
+            if len(g.offsets):
+                ret = self.conn.r_rdma_scatter(*args, **g.pieces, records=g.records)
+                if ret < 0:
+                    raise Exception(f"Failed to read to infinistore, ret = {ret}: "
+                                    f"{self.conn.last_error()}")
+            return None
+        if g.dev < 0:
+            raise ValueError("layered reads take CUDA tensors")
+        if not self.conn.server_has_hbm():
+            raise ValueError("layered reads need a pool in GPU memory")
+        group_parts = int(group_parts)
+        if group_parts < 1 or len(g.bases) % group_parts:
+            raise ValueError(f"group_parts {group_parts} does not divide the {len(g.bases)} parts")
+        native = _infinistore.ScatterReader()
+        self.conn.r_rdma_scatter(*args, native, group_parts, **g.pieces, records=g.records)
+        read = ScatterRead(self, native, parts[0][0].device)
+        if native.failed:
+            err = Exception(f"Failed to read to infinistore: {self.conn.last_error()}")
+            err.read = read
+            raise err
+        return read
 
     def rdma_write_cache_gather(self, parts, offsets, part_size: int, remote_blocks,
                                 stream="current", rows: "PartRows | None" = None):
@@ -921,16 +1003,7 @@ class InfinityConnection:
         rows of every stored part split into k runs, and run i of block b is taken from
         ``offsets[b, i]`` - e.g. a chunk of k engine pages stored under one key, each page where
         the block table puts it.  k must divide ``rows.count``; ``(n, 1)`` is the 1-D call."""
-        bases, dev, es, offs, s, table = self._gather_parts(parts, offsets, part_size, rows=rows,
-                                                            nblocks=len(remote_blocks),
-                                                            stream=stream, write=True)
-        native_rows = rows.native(es) if rows is not None else []
-        if not len(offs):
-            return 0
-        ret = self.conn.w_rdma_gather(bases, int(part_size) * es, 0, offs, remote_blocks, dev, s,
-                                      es, native_rows, **_piece_args(table))
-        if ret < 0:
-            raise Exception(f"Failed to write to infinistore, ret = {ret}: {self.conn.last_error()}")
+        self._gather_write(parts, offsets, part_size, stream, rows, False, None, remote_blocks)
         return 0
 
     def read_cache_scatter(self, parts, blocks, part_size: int, first_part: int = 0,
@@ -954,18 +1027,7 @@ class InfinityConnection:
         enqueued.  With ``rows``, ``(keys, offsets)`` may carry an ``(n, k)`` int64 array
         (pieces, as for ``rdma_write_cache_gather``): run i of the rows of block b lands at
         ``offsets[b, i]``."""
-        keys, offs = _split_blocks(blocks)
-        bases, dev, es, offs, s, table = self._gather_parts(parts, offs, part_size, first_part,
-                                                            rows=rows, nblocks=len(keys),
-                                                            stream=stream)
-        native_rows = rows.native(es) if rows is not None else []
-        if not len(offs):
-            return
-        ret = self.conn.r_rdma_scatter(bases, int(part_size) * es, 0, int(first_part),
-                                       (keys, offs), dev, s, es, native_rows,
-                                       **_piece_args(table))
-        if ret < 0:
-            raise Exception(f"Failed to read to infinistore, ret = {ret}: {self.conn.last_error()}")
+        self._scatter_read(parts, blocks, part_size, first_part, stream, rows, False, None)
 
     # ------------------------------------------------------------------ gathered fp8 blocks
     @staticmethod
@@ -978,9 +1040,7 @@ class InfinityConnection:
         token_dim`` records of ``records.record_bytes`` bytes."""
         if records is None:
             return _infinistore.kernels.fp8_gather_bytes(int(nparts), int(part_size))
-        if not isinstance(records, FP8Records):
-            raise ValueError(f"records must be an FP8Records, not {type(records).__name__}")
-        records.check(part_size)
+        _check_records(records, part_size)
         return _infinistore.kernels.fp8_records_bytes(int(nparts), int(part_size),
                                                       records.latent_dim, records.rope_dim)
 
@@ -1002,18 +1062,7 @@ class InfinityConnection:
         ``fp8_gather_block_bytes(s, part_size, records=records)``; allocate
         ``fp8_gather_block_bytes(len(parts), part_size, records=records)`` bytes.  No
         ``rows``."""
-        bases, dev, es, offs, s, table = self._gather_parts(parts, offsets, part_size, fp8=True,
-                                                            rows=rows, nblocks=len(remote_blocks),
-                                                            stream=stream, write=True,
-                                                            records=records)
-        native_rows = rows.native(es) if rows is not None else []
-        if not len(offs):
-            return 0
-        ret = self.conn.w_rdma_gather(bases, int(part_size) * es, int(part_size), offs,
-                                      remote_blocks, dev, s, es, native_rows,
-                                      **_piece_args(table), records=_native_records(records))
-        if ret < 0:
-            raise Exception(f"Failed to write to infinistore, ret = {ret}: {self.conn.last_error()}")
+        self._gather_write(parts, offsets, part_size, stream, rows, True, records, remote_blocks)
         return 0
 
     def read_cache_scatter_fp8(self, parts, blocks, part_size: int, first_part: int = 0,
@@ -1036,19 +1085,7 @@ class InfinityConnection:
         RoPE elements copied back verbatim.  With ``device_lookup`` a stored block shorter than
         ``fp8_gather_block_bytes(first_part + len(parts), part_size, records=records)`` is a
         miss.  No ``rows``."""
-        keys, offs = _split_blocks(blocks)
-        bases, dev, es, offs, s, table = self._gather_parts(parts, offs, part_size, first_part,
-                                                            fp8=True, rows=rows,
-                                                            nblocks=len(keys), stream=stream,
-                                                            records=records)
-        native_rows = rows.native(es) if rows is not None else []
-        if not len(offs):
-            return
-        ret = self.conn.r_rdma_scatter(bases, int(part_size) * es, int(part_size), int(first_part),
-                                       (keys, offs), dev, s, es, native_rows,
-                                       **_piece_args(table), records=_native_records(records))
-        if ret < 0:
-            raise Exception(f"Failed to read to infinistore, ret = {ret}: {self.conn.last_error()}")
+        self._scatter_read(parts, blocks, part_size, first_part, stream, rows, True, records)
 
     # ------------------------------------------------------------------ layered scattered reads
     def read_cache_scatter_layered(self, parts, blocks, part_size: int, group_parts: int = 2,
@@ -1070,28 +1107,8 @@ class InfinityConnection:
         raises here; the exception's ``read`` attribute is the failed reader.  ``rows`` as for
         ``read_cache_scatter[_fp8]``, ``records`` (with ``fp8``) as for
         ``read_cache_scatter_fp8``."""
-        keys, offs = _split_blocks(blocks)
-        bases, dev, es, offs, s, table = self._gather_parts(parts, offs, part_size, first_part,
-                                                            fp8=fp8, rows=rows, nblocks=len(keys),
-                                                            stream=stream, records=records)
-        if dev < 0:
-            raise ValueError("layered reads take CUDA tensors")
-        if not self.conn.server_has_hbm():
-            raise ValueError("layered reads need a pool in GPU memory")
-        group_parts = int(group_parts)
-        if group_parts < 1 or len(bases) % group_parts:
-            raise ValueError(f"group_parts {group_parts} does not divide the {len(bases)} parts")
-        native = _infinistore.ScatterReader()
-        self.conn.r_rdma_scatter(bases, int(part_size) * es, int(part_size) if fp8 else 0,
-                                 int(first_part), (keys, offs), dev, s, es,
-                                 rows.native(es) if rows is not None else [], native, group_parts,
-                                 **_piece_args(table), records=_native_records(records))
-        read = ScatterRead(self, native, parts[0][0].device)
-        if native.failed:
-            err = Exception(f"Failed to read to infinistore: {self.conn.last_error()}")
-            err.read = read
-            raise err
-        return read
+        return self._scatter_read(parts, blocks, part_size, first_part, stream, rows, fp8, records,
+                                  group_parts)
 
     # ------------------------------------------------------------------ layered gathered writes
     def gather_writer(self, remote_blocks, offsets, nparts: int, part_size: int,
@@ -1110,21 +1127,8 @@ class InfinityConnection:
         records=records)`` bytes."""
         if self._mode != "rdma":
             raise Exception("gathered blocks need a connected rdma connection")
-        if records is not None:
-            if not isinstance(records, FP8Records):
-                raise ValueError(f"records must be an FP8Records, not {type(records).__name__}")
-            if not fp8:
-                raise ValueError("records= stores fp8 token records: it needs fp8=True")
-            records.check(part_size)
-        offs = np.ascontiguousarray(offsets, dtype=np.int64)
-        if offs.ndim == 2 and offs.shape[1] == 1:
-            offs = offs[:, 0]
-        if offs.ndim not in (1, 2):
-            raise ValueError("offsets are 1-D, or 2-D with one column per piece")
-        if len(offs) != len(remote_blocks):
-            raise ValueError(f"{len(offs)} offsets for {len(remote_blocks)} remote blocks")
-        if offs.size and int(offs.min()) < 0:
-            raise ValueError("offsets must not be negative")
+        _check_records(records, part_size, fp8)
+        offs = _block_offsets(offsets, len(remote_blocks))
         if not 1 <= int(nparts) <= GATHER_MAX_PARTS:
             raise ValueError(f"a block holds 1 to {GATHER_MAX_PARTS} parts, not {nparts}")
         if int(part_size) <= 0:
@@ -1409,21 +1413,14 @@ class GatherWriter:
         written = self._w.written
         if any(written[first_part:first_part + len(parts)]):
             raise ValueError("the part range overlaps parts written before")
-        conn = self._conn
         if self._offs.ndim == 2 and rows is None:
             raise ValueError("a writer made with 2-D offsets (pieces) needs rows= on every call")
-        bases, dev, es, _, s, _ = conn._gather_parts(parts, self._offs, self.part_size, first_part,
-                                                     self.nparts, self.fp8, rows, stream=stream,
-                                                     write=True, records=self.records)
-        native_rows = rows.native(es) if rows is not None else []
-        first = parts[0][0]
+        self._conn._gather_write(parts, self._offs, self.part_size, stream, rows, self.fp8,
+                                 self.records, writer=self, first_part=first_part)
+
+    def _claim(self, first: torch.Tensor) -> None:
+        """The first call fixes the device and dtype; ValueError for another one later."""
         if self._dev is not None and self._dev != (first.device, first.dtype):
             raise ValueError(f"parts on {first.device} as {first.dtype}, the writer's first call "
                              f"used {self._dev[0]} as {self._dev[1]}")
         self._dev = (first.device, first.dtype)
-        ret = conn.conn.w_rdma_layered(self._w, bases, self.part_size * es,
-                                       self.part_size if self.fp8 else 0, first_part, dev, s, es,
-                                       native_rows, _native_records(self.records))
-        if ret < 0:
-            raise Exception(f"Failed to write to infinistore, ret = {ret}: "
-                            f"{conn.conn.last_error()}")

@@ -1,7 +1,7 @@
 """A paged KV cache whose pages are store blocks, with layer-wise streaming."""
 from __future__ import annotations
 
-from typing import List, Optional, Sequence
+from typing import List, NamedTuple, Optional, Sequence
 
 import numpy as np
 import torch
@@ -26,7 +26,121 @@ def layer_keys(layout: KVLayout, tp_rank: int, layer: int, kv: int,
     return [page_key(layout.name, layer, kind, tp_rank, h) for h in page_hashes]
 
 
-class _PagedCache:
+class _Plan(NamedTuple):
+    """One all-layer call: a block per key, landing at ``offsets`` (elements of a page of
+    ``data``; ``(n, k)`` for chunks of k pages, one column per page) through ``rows``
+    (``PartRows``; None: whole parts), each stored part ``part`` elements."""
+
+    keys: List[str]
+    offsets: np.ndarray
+    rows: Optional[PartRows]
+    part: int
+
+    def by_rows(self) -> bool:
+        """Whether heads move row by row: rows that are not each page whole, as one row."""
+        pages = self.offsets.shape[1] if self.offsets.ndim == 2 else 0
+        return self.rows is not None and self.rows.count != pages
+
+
+def _prefix_pages(conn, groups: List[List[str]]) -> int:
+    """Leading blocks of a prefix every group of keys holds (0 when none, or on an error)."""
+    try:
+        return min(conn.get_match_last_index(keys) + 1 for keys in groups)
+    except Exception:
+        return 0
+
+
+def _touch(conn, groups: List[List[str]]) -> int:
+    keys = [k for ks in groups for k in ks]
+    return conn.touch(keys) if keys else 0
+
+
+class _AllLayerPages:
+    """What every cache of all-layer pages shares: ``data[layer, part, page]`` with
+    ``_per_layer`` parts per layer (K and V, or MLA's one latent part), registration with each
+    connection, and the I/O of blocks that hold a page (or chunk) of every layer, each layer's
+    parts side by side.  A subclass builds the ``_Plan`` of a call; ``_store``, ``_writer``,
+    and ``_read`` (plain or layered) run it in the format ``fp8`` chooses: bf16, fp8 pages, or
+    (with ``records``) fp8 token records."""
+
+    _per_layer = 2
+    _fp8_pages = "fp8 all-layer pages"  # what the fp8 refusal names
+    records: Optional[FP8Records] = None  # how fp8 stores a part; None: as an fp8 page
+
+    def __init__(self, layout, num_pages: int, data: torch.Tensor):
+        self.layout = layout
+        self.num_pages = num_pages
+        self.data = data
+        self._registered = set()
+
+    def _ensure_registered(self, conn):
+        if id(conn) not in self._registered:
+            conn.register_mr(self.data)
+            self._registered.add(id(conn))
+
+    def _parts(self, layers: range):
+        n = self.num_pages * self.layout.page_elems
+        return [(self.data, (layer * self._per_layer + i) * n)
+                for layer in layers for i in range(self._per_layer)]
+
+    def _format(self, plan: _Plan, fp8: bool) -> Optional[FP8Records]:
+        """The records of the call's format (None: bf16 or fp8 pages).  ValueError, before
+        anything happens, for fp8 unless the cache is bf16 on a CUDA device, its records take
+        the part, and, when heads move row by row, ``head_dim`` is a multiple of 8."""
+        if not fp8:
+            return None
+        if self.data.dtype != torch.bfloat16 or self.data.device.type != "cuda":
+            raise ValueError(f"{self._fp8_pages} need a bf16 cache on a CUDA device")
+        # a read or write that regroups heads moves them in 8-element vectors; a head need not
+        # fill a 128-element scale group
+        if plan.by_rows() and self.layout.head_dim % 8:
+            raise ValueError(f"fp8 pages moved head by head (read from another TP degree, or "
+                             f"into or out of a head-major cache) need a head_dim that is a "
+                             f"multiple of 8, not {self.layout.head_dim}")
+        if self.records is not None:
+            self.records.check(plan.part)
+        return self.records
+
+    def _allocate(self, conn, plan: _Plan, fp8: bool):
+        """(blocks, records) of a write; ValueError before anything is allocated for a refused
+        format or a block over the block limit."""
+        records = self._format(plan, fp8)
+        nparts = self._per_layer * self.layout.layers
+        nbytes = (conn.fp8_gather_block_bytes(nparts, plan.part, records=records) if fp8
+                  else nparts * plan.part * self.data.element_size())
+        if nbytes > _GATHER_MAX_BLOCK_BYTES:
+            raise ValueError(f"a block of {nparts} parts of {plan.part} elements takes {nbytes} "
+                             f"bytes, over the {_GATHER_MAX_BLOCK_BYTES}-byte block limit")
+        self._ensure_registered(conn)
+        return conn.allocate_rdma(plan.keys, nbytes), records
+
+    def _store(self, conn, plan: _Plan, fp8: bool, stream) -> int:
+        blocks, records = self._allocate(conn, plan, fp8)
+        conn._gather_write(self._parts(range(self.layout.layers)), plan.offsets, plan.part,
+                           stream, plan.rows, fp8, records, blocks)
+        return len(blocks)
+
+    def _writer(self, conn, plan: _Plan, fp8: bool) -> "PageWriter":
+        blocks, records = self._allocate(conn, plan, fp8)
+        return PageWriter(self, conn.gather_writer(blocks, plan.offsets,
+                                                   self._per_layer * self.layout.layers,
+                                                   plan.part, fp8=fp8, records=records),
+                          plan.rows)
+
+    def _read(self, conn, plan: _Plan, layers: Optional[range], fp8: bool, stream,
+              layered: bool = False):
+        """Reads ``layers`` (checked, default all) of the plan's blocks: returns the number of
+        blocks, or with ``layered`` the ``PageRead``."""
+        records = self._format(plan, fp8)
+        layers = _layer_range(layers, self.layout.layers)
+        self._ensure_registered(conn)
+        read = conn._scatter_read(self._parts(layers), (plan.keys, plan.offsets), plan.part,
+                                  self._per_layer * layers.start, stream, plan.rows, fp8,
+                                  records, self._per_layer if layered else None)
+        return PageRead(read, layers) if layered else len(plan.keys)
+
+
+class _PagedCache(_AllLayerPages):
     """What the token-major :class:`PagedKVCache` and the head-major :class:`HeadMajorKVCache`
     share: ``data[layer, kv, page]`` is one page of ``layout.page_elems`` elements, per-layer
     and all-layer keys, and the writes and reads of all-layer pages (one key per page, parts
@@ -43,11 +157,8 @@ class _PagedCache:
     stretched over the chunk."""
 
     def __init__(self, layout: KVLayout, num_pages: int, tp_rank: int, data: torch.Tensor):
-        self.layout = layout
-        self.num_pages = num_pages
+        super().__init__(layout, num_pages, data)
         self.tp_rank = tp_rank
-        self.data = data
-        self._registered = set()
 
     # ------------------------------------------------------------------ geometry
     def page_offset(self, layer: int, kv: int, page: int) -> int:
@@ -57,28 +168,10 @@ class _PagedCache:
     def keys(self, layer: int, kv: int, page_hashes: Sequence[str]) -> List[str]:
         return layer_keys(self.layout, self.tp_rank, layer, kv, page_hashes)
 
-    def _ensure_registered(self, conn):
-        if id(conn) not in self._registered:
-            conn.register_mr(self.data)
-            self._registered.add(id(conn))
-
     # ------------------------------------------------------------------ all-layer pages
     def page_keys(self, page_hashes: Sequence[str]) -> List[str]:
         """Store keys of all-layer pages (``PagedKVCache.write_pages``)."""
         return [page_key(self.layout.name, ALL_LAYERS, "KV", self.tp_rank, h) for h in page_hashes]
-
-    def _parts(self, layers: range):
-        return [(self.data, self.page_offset(layer, kv, 0)) for layer in layers for kv in (0, 1)]
-
-    def _check_fp8(self, rows: bool = False):
-        if self.data.dtype != torch.bfloat16 or self.data.device.type != "cuda":
-            raise ValueError("fp8 all-layer pages need a bf16 cache on a CUDA device")
-        # a read or write that regroups heads moves them in 8-element vectors; a head need not
-        # fill a 128-element scale group
-        if rows and self.layout.head_dim % 8:
-            raise ValueError(f"fp8 pages moved head by head (read from another TP degree, or "
-                             f"into or out of a head-major cache) need a head_dim that is a "
-                             f"multiple of 8, not {self.layout.head_dim}")
 
     def _cross_tp(self, source_tp: Optional[int]) -> bool:
         """Whether a read of pages written at ``source_tp`` regroups heads."""
@@ -91,13 +184,13 @@ class _PagedCache:
         raise NotImplementedError
 
     def _sources(self, pages: Sequence[int], page_hashes: Sequence[str],
-                 source_tp: Optional[int], chunk_pages: int = 0):
-        """The blocks of a read of pages written at ``source_tp`` (None: this TP degree, by
-        this rank): one per (page, source rank), keyed by the writer rank, each landing at its
-        heads of the reader's page, and the rows every block gives (``PartRows``, or None for
-        whole parts) and the stored part size.  ``chunk_pages`` k > 0: ``pages`` is an (n, k)
-        block table of chunks, and the blocks are one per (chunk, source rank), with (blocks,
-        k) offsets and the chunk's rows (``_chunk_rows``)."""
+                 source_tp: Optional[int], chunk_pages: int = 0) -> _Plan:
+        """The plan of a read of pages written at ``source_tp`` (None: this TP degree, by this
+        rank): one block per (page, source rank), keyed by the writer rank, each landing at its
+        heads of the reader's page, with the rows every block gives (None for whole parts) and
+        the stored part size.  ``chunk_pages`` k > 0: ``pages`` is an (n, k) block table of
+        chunks, and the blocks are one per (chunk, source rank), with (blocks, k) offsets and
+        the chunk's rows (``_chunk_rows``)."""
         lay = self.layout
         wl = lay if source_tp is None else lay.with_tp(int(source_tp))
         srcs = (tp_sources(lay, lay.tp, self.tp_rank, wl.tp) if self._cross_tp(source_tp)
@@ -114,47 +207,36 @@ class _PagedCache:
                     for h in page_hashes for w, *_ in srcs]
             offs = (np.asarray(pages, dtype=np.int64)[:, None, :] * lay.page_elems
                     + dst[None, :, None])
-            return (keys, offs.reshape(-1, chunk_pages),
-                    self._chunk_rows(rows, chunk_pages, wl.page_elems),
-                    chunk_pages * wl.page_elems)
+            return _Plan(keys, offs.reshape(-1, chunk_pages),
+                         self._chunk_rows(rows, chunk_pages, wl.page_elems),
+                         chunk_pages * wl.page_elems)
         keys = [page_key(lay.name, ALL_LAYERS, "KV", w, h) for h in page_hashes for w, *_ in srcs]
         offs = np.asarray(pages, dtype=np.int64)[:, None] * lay.page_elems + dst[None, :]
-        return keys, offs.reshape(-1), rows, wl.page_elems
+        return _Plan(keys, offs.reshape(-1), rows, wl.page_elems)
 
     def _blocks(self, pages: Sequence[int], page_hashes: Sequence[str],
-                source_tp: Optional[int]):
-        """keys, offsets, rows and stored part size of a read of all-layer pages."""
+                source_tp: Optional[int]) -> _Plan:
+        """The plan of a read of all-layer pages."""
         return self._sources(pages, page_hashes, source_tp)
-
-    def _check_layers(self, layers: Optional[range]) -> range:
-        return _layer_range(layers, self.layout.layers)
 
     def _write_rows(self) -> Optional[PartRows]:
         """How this cache's page fills a stored token-major part on a write: the ``PartRows``
         (None: the page is the stored part, written whole)."""
         raise NotImplementedError
 
+    def _write_plan(self, pages: Sequence[int], page_hashes: Sequence[str]) -> _Plan:
+        elems = self.layout.page_elems
+        return _Plan(self.page_keys(page_hashes), np.asarray(pages, dtype=np.int64) * elems,
+                     self._write_rows(), elems)
+
     def write_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
                     stream="current", fp8: bool = False) -> int:
         """Upload every layer's K and V of each page under one key per page.  ``fp8``: every
-        part is stored as e4m3 with per-128 scales (``rdma_write_cache_gather_fp8``), about
+        part is stored as e4m3 with per-128 scales (the gathered fp8 write), about
         half the pool bytes; read such pages back with ``read_pages(fp8=True)``.  The stored
         pages are the same whichever cache writes them.  Blocks whose key already exists are
         skipped (first writer wins).  Returns the number of blocks written."""
-        rows = self._write_rows()
-        if fp8:
-            self._check_fp8(rows is not None)  # before any block is allocated
-        self._ensure_registered(conn)
-        layers = range(self.layout.layers)
-        keys = self.page_keys(page_hashes)
-        elems = self.layout.page_elems
-        nbytes = (conn.fp8_gather_block_bytes(2 * len(layers), elems) if fp8
-                  else 2 * len(layers) * self.layout.page_bytes)
-        blocks = conn.allocate_rdma(keys, nbytes)
-        offs = np.asarray(pages, dtype=np.int64) * elems
-        write = conn.rdma_write_cache_gather_fp8 if fp8 else conn.rdma_write_cache_gather
-        write(self._parts(layers), offs, elems, blocks, stream=stream, rows=rows)
-        return len(keys)
+        return self._store(conn, self._write_plan(pages, page_hashes), fp8, stream)
 
     def page_writer(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
                     fp8: bool = False) -> "PageWriter":
@@ -162,16 +244,7 @@ class _PagedCache:
         layer by layer: ``write_layers(range(l, l + 1))`` right after layer l has produced its
         KV, so the upload overlaps the next layer's compute and one key per page is kept.
         Read the pages back with ``read_pages(fp8=fp8)``."""
-        if fp8:
-            self._check_fp8(self._write_rows() is not None)  # before any block is allocated
-        self._ensure_registered(conn)
-        nparts = 2 * self.layout.layers
-        elems = self.layout.page_elems
-        nbytes = (conn.fp8_gather_block_bytes(nparts, elems) if fp8
-                  else nparts * self.layout.page_bytes)
-        blocks = conn.allocate_rdma(self.page_keys(page_hashes), nbytes)
-        offs = np.asarray(pages, dtype=np.int64) * elems
-        return PageWriter(self, conn.gather_writer(blocks, offs, nparts, elems, fp8=fp8))
+        return self._writer(conn, self._write_plan(pages, page_hashes), fp8)
 
     def read_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
                    layers: Optional[range] = None, stream="current", fp8: bool = False,
@@ -190,15 +263,7 @@ class _PagedCache:
         untouched, so treat every page of a failed read as not read.  With ``fp8`` the read
         kernel dequantises each source's heads out of its fp8 pages in the same way
         (``head_dim`` a multiple of 8).  Returns the number of (page, source) blocks read."""
-        keys, offs, rows, part = self._blocks(pages, page_hashes, source_tp)
-        if fp8:
-            self._check_fp8(rows is not None)
-        self._ensure_registered(conn)
-        layers = self._check_layers(layers)
-        read = conn.read_cache_scatter_fp8 if fp8 else conn.read_cache_scatter
-        read(self._parts(layers), (keys, offs), part, first_part=2 * layers.start,
-             stream=stream, rows=rows)
-        return len(keys)
+        return self._read(conn, self._blocks(pages, page_hashes, source_tp), layers, fp8, stream)
 
     def read_pages_layered(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
                            layers: Optional[range] = None, fp8: bool = False,
@@ -209,15 +274,8 @@ class _PagedCache:
         arrived, with no host synchronisation.  ``layers`` (a step-1 range, default all),
         ``fp8`` and ``source_tp`` as for ``read_pages``.  A layer is released before the
         read's post-copy index check: when ``sync()`` reports a miss, the whole read failed."""
-        keys, offs, rows, part = self._blocks(pages, page_hashes, source_tp)
-        if fp8:
-            self._check_fp8(rows is not None)
-        self._ensure_registered(conn)
-        layers = self._check_layers(layers)
-        read = conn.read_cache_scatter_layered(self._parts(layers), (keys, offs), part,
-                                               group_parts=2, first_part=2 * layers.start,
-                                               fp8=fp8, stream=stream, rows=rows)
-        return PageRead(read, layers)
+        return self._read(conn, self._blocks(pages, page_hashes, source_tp), layers, fp8, stream,
+                          layered=True)
 
     def source_page_keys(self, page_hashes: Sequence[str], source_tp: int) -> List[List[str]]:
         """All-layer page keys of every writer rank at ``source_tp`` that holds some of this
@@ -225,6 +283,22 @@ class _PagedCache:
         srcs = tp_sources(self.layout, self.layout.tp, self.tp_rank, int(source_tp))
         return [[page_key(self.layout.name, ALL_LAYERS, "KV", w, h) for h in page_hashes]
                 for w, *_ in srcs]
+
+    def _key_groups(self, page_hashes: Sequence[str], all_layer_pages: bool,
+                    source_tp: Optional[int], chunk_pages: int, layer_parts) -> List[List[str]]:
+        """The keys of a prefix, one list per source rank: of chunks of ``chunk_pages`` pages,
+        of all-layer pages (``all_layer_pages``, needed by ``source_tp``), or else this rank's
+        per-layer keys of the (layer, kv) pairs ``layer_parts``."""
+        if chunk_pages:
+            return (self.source_chunk_keys(page_hashes, chunk_pages, source_tp)
+                    if self._cross_tp(source_tp) else [self.chunk_keys(page_hashes, chunk_pages)])
+        if self._cross_tp(source_tp):
+            if not all_layer_pages:
+                raise ValueError("source_tp needs all_layer_pages")
+            return self.source_page_keys(page_hashes, source_tp)
+        if all_layer_pages:
+            return [self.page_keys(page_hashes)]
+        return [self.keys(layer, kv, page_hashes) for layer, kv in layer_parts]
 
     def cached_prefix_pages(self, conn, page_hashes: Sequence[str],
                             layer: Optional[int] = None, all_layer_pages: bool = False,
@@ -238,29 +312,9 @@ class _PagedCache:
         (``write_chunks``), and the answer counts chunks."""
         if not page_hashes:
             return 0
-        if chunk_pages:
-            groups = (self.source_chunk_keys(page_hashes, chunk_pages, source_tp)
-                      if self._cross_tp(source_tp) else [self.chunk_keys(page_hashes, chunk_pages)])
-            try:
-                return min(conn.get_match_last_index(keys) + 1 for keys in groups)
-            except Exception:
-                return 0
-        if self._cross_tp(source_tp):
-            if not all_layer_pages:
-                raise ValueError("source_tp needs all_layer_pages")
-            try:
-                return min(conn.get_match_last_index(keys) + 1
-                           for keys in self.source_page_keys(page_hashes, source_tp))
-            except Exception:
-                return 0
-        if all_layer_pages:
-            keys = self.page_keys(page_hashes)
-        else:
-            keys = self.keys(self.layout.layers - 1 if layer is None else layer, 1, page_hashes)
-        try:
-            return conn.get_match_last_index(keys) + 1
-        except Exception:
-            return 0
+        layer = self.layout.layers - 1 if layer is None else layer
+        return _prefix_pages(conn, self._key_groups(page_hashes, all_layer_pages, source_tp,
+                                                    chunk_pages, [(layer, 1)]))
 
     def touch_prefix(self, conn, page_hashes: Sequence[str], all_layer_pages: bool = False,
                      source_tp: Optional[int] = None, chunk_pages: int = 0) -> int:
@@ -270,25 +324,9 @@ class _PagedCache:
         blocks refreshed.  ``all_layer_pages``: the pages were written with ``write_pages``;
         ``source_tp`` (with it): at that TP degree, and every source rank's key is touched.
         ``chunk_pages`` k > 0: chunk hashes of chunks of k pages (``write_chunks``)."""
-        if chunk_pages:
-            keys = ([k for ks in self.source_chunk_keys(page_hashes, chunk_pages, source_tp)
-                     for k in ks] if self._cross_tp(source_tp)
-                    else self.chunk_keys(page_hashes, chunk_pages))
-            return conn.touch(keys) if keys else 0
-        if self._cross_tp(source_tp):
-            if not all_layer_pages:
-                raise ValueError("source_tp needs all_layer_pages")
-            keys = [k for ks in self.source_page_keys(page_hashes, source_tp) for k in ks]
-            return conn.touch(keys) if keys else 0
-        if all_layer_pages:
-            keys = self.page_keys(page_hashes)
-            return conn.touch(keys) if keys else 0
-        keys: List[str] = []
-        for layer in range(self.layout.layers):
-            for kv in (0, 1):
-                keys.extend(self.keys(layer, kv, page_hashes))
-        return conn.touch(keys) if keys else 0
-
+        every = [(layer, kv) for layer in range(self.layout.layers) for kv in (0, 1)]
+        return _touch(conn, self._key_groups(page_hashes, all_layer_pages, source_tp,
+                                             chunk_pages, every))
 
     # ------------------------------------------------------------------ all-layer chunks
     @staticmethod
@@ -331,28 +369,16 @@ class _PagedCache:
                              "on it")
         return table
 
-    def _chunk_block_bytes(self, conn, k: int, fp8: bool) -> int:
-        """Pool bytes of one chunk; ValueError over the block limit."""
-        nparts, elems = 2 * self.layout.layers, k * self.layout.page_elems
-        nbytes = (conn.fp8_gather_block_bytes(nparts, elems) if fp8
-                  else nparts * k * self.layout.page_bytes)
-        if nbytes > _GATHER_MAX_BLOCK_BYTES:
-            raise ValueError(f"a chunk of {k} pages takes {nbytes} bytes, over the "
-                             f"{_GATHER_MAX_BLOCK_BYTES}-byte block limit")
-        return nbytes
-
-    def _chunk_write(self, conn, block_table, chunk_hashes: Sequence[str], fp8: bool):
-        """Checks, allocates and returns (blocks, offsets, rows, stored part size) of a chunk
-        write."""
+    def _chunk_write_plan(self, block_table, chunk_hashes: Sequence[str]) -> _Plan:
         table = self._chunk_table(block_table, chunk_hashes, read=False)
         k, elems = table.shape[1], self.layout.page_elems
-        rows = self._chunk_rows(self._write_rows(), k, elems)
-        if fp8:  # heads move row by row unless each page is one row
-            self._check_fp8(rows.count != k)
-        nbytes = self._chunk_block_bytes(conn, k, fp8)
-        self._ensure_registered(conn)
-        blocks = conn.allocate_rdma(self.chunk_keys(chunk_hashes, k), nbytes)
-        return blocks, table * elems, rows, k * elems
+        return _Plan(self.chunk_keys(chunk_hashes, k), table * elems,
+                     self._chunk_rows(self._write_rows(), k, elems), k * elems)
+
+    def _chunk_read_plan(self, block_table, chunk_hashes: Sequence[str],
+                         source_tp: Optional[int]) -> _Plan:
+        table = self._chunk_table(block_table, chunk_hashes, read=True)
+        return self._sources(table, chunk_hashes, source_tp, chunk_pages=table.shape[1])
 
     def write_chunks(self, conn, block_table, chunk_hashes: Sequence[str], stream="current",
                      fp8: bool = False) -> int:
@@ -364,27 +390,13 @@ class _PagedCache:
         ``ValueError`` before any block is allocated for a table whose row count differs from
         the hashes, a page index outside the cache, a chunk over the block limit and every
         ``write_pages`` refusal.  Returns the number of blocks written."""
-        blocks, offs, rows, part = self._chunk_write(conn, block_table, chunk_hashes, fp8)
-        write = conn.rdma_write_cache_gather_fp8 if fp8 else conn.rdma_write_cache_gather
-        write(self._parts(range(self.layout.layers)), offs, part, blocks, stream=stream, rows=rows)
-        return len(blocks)
+        return self._store(conn, self._chunk_write_plan(block_table, chunk_hashes), fp8, stream)
 
     def chunk_writer(self, conn, block_table, chunk_hashes: Sequence[str],
                      fp8: bool = False) -> "PageWriter":
         """``page_writer`` for chunks (``write_chunks``): ``write_layers`` stores layers of
         every chunk as they are produced."""
-        blocks, offs, rows, part = self._chunk_write(conn, block_table, chunk_hashes, fp8)
-        writer = conn.gather_writer(blocks, offs, 2 * self.layout.layers, part, fp8=fp8)
-        return PageWriter(self, writer, rows)
-
-    def _chunk_read(self, block_table, chunk_hashes: Sequence[str], layers, fp8: bool,
-                    source_tp: Optional[int]):
-        table = self._chunk_table(block_table, chunk_hashes, read=True)
-        keys, offs, rows, part = self._sources(table, chunk_hashes, source_tp,
-                                               chunk_pages=table.shape[1])
-        if fp8:  # heads move row by row unless each page is one row
-            self._check_fp8(rows.count != table.shape[1])
-        return keys, offs, rows, part, self._check_layers(layers)
+        return self._writer(conn, self._chunk_write_plan(block_table, chunk_hashes), fp8)
 
     def read_chunks(self, conn, block_table, chunk_hashes: Sequence[str],
                     layers: Optional[range] = None, stream="current", fp8: bool = False,
@@ -393,25 +405,15 @@ class _PagedCache:
         ``source_tp``, as for ``read_pages``): page i of chunk b lands in this cache's page
         ``block_table[b, i]``.  A page that appears twice in the table raises ``ValueError``
         (two chunks would race on it).  Returns the number of (chunk, source) blocks read."""
-        keys, offs, rows, part, layers = self._chunk_read(block_table, chunk_hashes, layers, fp8,
-                                                          source_tp)
-        self._ensure_registered(conn)
-        read = conn.read_cache_scatter_fp8 if fp8 else conn.read_cache_scatter
-        read(self._parts(layers), (keys, offs), part, first_part=2 * layers.start,
-             stream=stream, rows=rows)
-        return len(keys)
+        return self._read(conn, self._chunk_read_plan(block_table, chunk_hashes, source_tp),
+                          layers, fp8, stream)
 
     def read_chunks_layered(self, conn, block_table, chunk_hashes: Sequence[str],
                             layers: Optional[range] = None, fp8: bool = False,
                             stream="current", source_tp: Optional[int] = None) -> "PageRead":
         """``read_pages_layered`` for chunks (``read_chunks``)."""
-        keys, offs, rows, part, layers = self._chunk_read(block_table, chunk_hashes, layers, fp8,
-                                                          source_tp)
-        self._ensure_registered(conn)
-        read = conn.read_cache_scatter_layered(self._parts(layers), (keys, offs), part,
-                                               group_parts=2, first_part=2 * layers.start,
-                                               fp8=fp8, stream=stream, rows=rows)
-        return PageRead(read, layers)
+        return self._read(conn, self._chunk_read_plan(block_table, chunk_hashes, source_tp),
+                          layers, fp8, stream, layered=True)
 
 
 class PagedKVCache(_PagedCache):
@@ -476,37 +478,37 @@ class PagedKVCache(_PagedCache):
         return rows, lay.head_dim
 
     def _blocks(self, pages: Sequence[int], page_hashes: Sequence[str],
-                source_tp: Optional[int]):
+                source_tp: Optional[int]) -> _Plan:
         if self._cross_tp(source_tp):
             return self._sources(pages, page_hashes, source_tp)
         # this rank's own pages land whole: the same token-major layout
-        return (self.page_keys(page_hashes),
-                np.asarray(pages, dtype=np.int64) * self.layout.page_elems, None,
-                self.layout.page_elems)
+        return _Plan(self.page_keys(page_hashes),
+                     np.asarray(pages, dtype=np.int64) * self.layout.page_elems, None,
+                     self.layout.page_elems)
 
     def _write_rows(self):
         return None  # the stored layout: whole parts
 
 
 class PageWriter:
-    """Layer-by-layer upload of all-layer pages (``page_writer`` of either cache)."""
+    """Layer-by-layer upload of all-layer pages (``page_writer`` or ``chunk_writer`` of every
+    cache)."""
 
-    def __init__(self, cache: _PagedCache, writer, rows: Optional[PartRows] = None):
+    def __init__(self, cache: _AllLayerPages, writer, rows: Optional[PartRows] = None):
         self.cache = cache
         self.writer = writer
-        self._chunk_rows = rows  # a chunk writer's rows (chunk_writer); None: the page's
+        self.rows = rows  # how the cache's pages fill each stored part (None: whole)
 
     @property
     def complete(self) -> bool:
         return self.writer.complete
 
     def write_layers(self, layers: range, stream="current") -> None:
-        """Store the K and V parts of ``layers`` (a non-empty step-1 range) of every page."""
-        n = self.cache.layout.layers
-        if layers.step != 1 or not len(layers) or layers.start < 0 or layers.stop > n:
-            raise ValueError(f"layers must be a non-empty step-1 range within 0..{n}")
-        rows = self._chunk_rows if self._chunk_rows is not None else self.cache._write_rows()
-        self.writer.write(self.cache._parts(layers), 2 * layers.start, stream=stream, rows=rows)
+        """Store the parts (K and V, or the MLA latent) of ``layers`` (a non-empty step-1
+        range) of every page."""
+        layers = _layer_range(layers, self.cache.layout.layers)
+        self.writer.write(self.cache._parts(layers), self.cache._per_layer * layers.start,
+                          stream=stream, rows=self.rows)
 
 
 class PageRead:
@@ -611,7 +613,7 @@ class HeadMajorKVCache(_PagedCache):
                         dst_slice_pitch=tokens * dim)
 
 
-class MLAKVCache:
+class MLAKVCache(_AllLayerPages):
     """The KV cache of an MLA model: ``data[layer, page, token]`` is one token's latent and
     RoPE elements (``layout.token_dim``), vLLM's per-layer MLA block shape stacked over the
     layers.  All-layer pages are stored under one key per page (``mla_page_key``) as
@@ -626,71 +628,39 @@ class MLAKVCache:
     failed read leaves its pages untouched and reported.  ``fp8`` must be what the writer
     used; bf16 and fp8 pages have different keys."""
 
+    _per_layer = 1
+    _fp8_pages = "fp8 MLA pages"
+
     def __init__(self, layout: MLALayout, num_pages: int, device):
-        self.layout = layout
-        self.num_pages = num_pages
+        super().__init__(layout, num_pages,
+                         torch.zeros(layout.layers, num_pages, layout.page_tokens,
+                                     layout.token_dim, dtype=layout.dtype, device=device))
         self.records = FP8Records(layout.latent_dim, layout.rope_dim)
-        self.data = torch.zeros(layout.layers, num_pages, layout.page_tokens, layout.token_dim,
-                                dtype=layout.dtype, device=device)
-        self._registered = set()
 
     def page_keys(self, page_hashes: Sequence[str], fp8: bool = False) -> List[str]:
         """Store keys of all-layer pages (``kv_layout.mla_page_key``)."""
         return [mla_page_key(self.layout.name, h, fp8) for h in page_hashes]
 
-    def _ensure_registered(self, conn):
-        if id(conn) not in self._registered:
-            conn.register_mr(self.data)
-            self._registered.add(id(conn))
-
-    def _parts(self, layers: range):
-        return [(self.data, layer * self.num_pages * self.layout.page_elems) for layer in layers]
-
-    def _offsets(self, pages: Sequence[int], page_hashes: Sequence[str]) -> np.ndarray:
+    def _plan(self, pages: Sequence[int], page_hashes: Sequence[str], fp8: bool) -> _Plan:
         if len(pages) != len(page_hashes):
             raise ValueError(f"{len(pages)} pages for {len(page_hashes)} page hashes")
-        return np.asarray(pages, dtype=np.int64) * self.layout.page_elems
-
-    def _format(self, conn, fp8: bool):
-        """(records or None, bytes of a block) of the format; ValueError before anything is
-        allocated for fp8 with a cache that is not bf16 on a CUDA device."""
-        n = self.layout.layers
-        if not fp8:
-            return None, n * self.layout.page_bytes
-        if self.data.dtype != torch.bfloat16 or self.data.device.type != "cuda":
-            raise ValueError("fp8 MLA pages need a bf16 cache on a CUDA device")
-        return self.records, conn.fp8_gather_block_bytes(n, self.layout.page_elems,
-                                                         records=self.records)
+        elems = self.layout.page_elems
+        return _Plan(self.page_keys(page_hashes, fp8), np.asarray(pages, dtype=np.int64) * elems,
+                     None, elems)
 
     def write_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
                     stream="current", fp8: bool = False) -> int:
         """Upload every layer's latent page of each page under one key per page.  Blocks
         whose key already exists are skipped (first writer wins).  Returns the number of
         blocks asked for."""
-        records, nbytes = self._format(conn, fp8)
-        offs = self._offsets(pages, page_hashes)
-        self._ensure_registered(conn)
-        blocks = conn.allocate_rdma(self.page_keys(page_hashes, fp8), nbytes)
-        parts, part = self._parts(range(self.layout.layers)), self.layout.page_elems
-        if fp8:
-            conn.rdma_write_cache_gather_fp8(parts, offs, part, blocks, stream=stream,
-                                             records=records)
-        else:
-            conn.rdma_write_cache_gather(parts, offs, part, blocks, stream=stream)
-        return len(blocks)
+        return self._store(conn, self._plan(pages, page_hashes, fp8), fp8, stream)
 
     def page_writer(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
-                    fp8: bool = False) -> "MLAPageWriter":
+                    fp8: bool = False) -> "PageWriter":
         """Allocate all-layer pages (as ``write_pages``) and return a writer whose
         ``write_layers(range(l, l + 1))`` stores layer l right after it has been produced.  A
         page becomes readable once its last layer has landed."""
-        records, nbytes = self._format(conn, fp8)
-        offs = self._offsets(pages, page_hashes)
-        self._ensure_registered(conn)
-        blocks = conn.allocate_rdma(self.page_keys(page_hashes, fp8), nbytes)
-        return MLAPageWriter(self, conn.gather_writer(blocks, offs, self.layout.layers,
-                                                      self.layout.page_elems, fp8=fp8,
-                                                      records=records))
+        return self._writer(conn, self._plan(pages, page_hashes, fp8), fp8)
 
     def read_pages(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
                    layers: Optional[range] = None, stream="current", fp8: bool = False) -> int:
@@ -698,18 +668,7 @@ class MLAKVCache:
         ``pages``; ``layers`` (a step-1 range, default all) reads only those layers' parts.
         A missing page fails the read (it raises, or with ``device_lookup`` ``sync()`` reports
         the miss) and leaves its pages untouched.  Returns the number of blocks read."""
-        records, _ = self._format(conn, fp8)
-        offs = self._offsets(pages, page_hashes)
-        layers = _layer_range(layers, self.layout.layers)
-        self._ensure_registered(conn)
-        blocks = (self.page_keys(page_hashes, fp8), offs)
-        if fp8:
-            conn.read_cache_scatter_fp8(self._parts(layers), blocks, self.layout.page_elems,
-                                        first_part=layers.start, stream=stream, records=records)
-        else:
-            conn.read_cache_scatter(self._parts(layers), blocks, self.layout.page_elems,
-                                    first_part=layers.start, stream=stream)
-        return len(offs)
+        return self._read(conn, self._plan(pages, page_hashes, fp8), layers, fp8, stream)
 
     def read_pages_layered(self, conn, pages: Sequence[int], page_hashes: Sequence[str],
                            layers: Optional[range] = None, fp8: bool = False,
@@ -718,43 +677,16 @@ class MLAKVCache:
         reader's ``wait_layer(l, stream)`` makes later work on ``stream`` wait, on the GPU, for
         layer l.  A layer is released before the read's post-copy index check: when ``sync()``
         reports a miss, the whole read failed."""
-        records, _ = self._format(conn, fp8)
-        offs = self._offsets(pages, page_hashes)
-        layers = _layer_range(layers, self.layout.layers)
-        self._ensure_registered(conn)
-        read = conn.read_cache_scatter_layered(
-            self._parts(layers), (self.page_keys(page_hashes, fp8), offs), self.layout.page_elems,
-            group_parts=1, first_part=layers.start, fp8=fp8, stream=stream, records=records)
-        return PageRead(read, layers)
+        return self._read(conn, self._plan(pages, page_hashes, fp8), layers, fp8, stream,
+                          layered=True)
 
     def cached_prefix_pages(self, conn, page_hashes: Sequence[str], fp8: bool = False) -> int:
         """How many leading pages of this prefix the store holds in this format."""
         if not page_hashes:
             return 0
-        try:
-            return conn.get_match_last_index(self.page_keys(page_hashes, fp8)) + 1
-        except Exception:
-            return 0
+        return _prefix_pages(conn, [self.page_keys(page_hashes, fp8)])
 
     def touch_prefix(self, conn, page_hashes: Sequence[str], fp8: bool = False) -> int:
         """Tell an evicting store (``--evict``) that these pages were just used.  Returns the
         number of blocks refreshed."""
-        keys = self.page_keys(page_hashes, fp8)
-        return conn.touch(keys) if keys else 0
-
-
-class MLAPageWriter:
-    """Layer-by-layer upload of all-layer MLA pages (``MLAKVCache.page_writer``)."""
-
-    def __init__(self, cache: MLAKVCache, writer):
-        self.cache = cache
-        self.writer = writer
-
-    @property
-    def complete(self) -> bool:
-        return self.writer.complete
-
-    def write_layers(self, layers: range, stream="current") -> None:
-        """Store the latent pages of ``layers`` (a non-empty step-1 range) of every page."""
-        layers = _layer_range(layers, self.cache.layout.layers)
-        self.writer.write(self.cache._parts(layers), layers.start, stream=stream)
+        return _touch(conn, [self.page_keys(page_hashes, fp8)])
