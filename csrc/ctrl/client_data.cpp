@@ -900,8 +900,12 @@ const char* Connection::gather_refusal(const GatherSpec& g, const uint64_t* offs
         if (g.fp8_elems % g.records.token_elems() || g.fp8_elems > uint32_t(INT32_MAX))
             return "bad part size for fp8 records: a whole number of tokens of latent + rope "
                    "elements";
-        if (g.rows.rows || g.rows.pieces != 1 || g.piece_off)
+        if (g.rows.rows || (g.rows.pieces == 1 && g.piece_off))
             return "fp8 records take whole parts: no row geometry or pieces";
+        // pieces of whole tokens (kv_fp8_records.cu), at the offsets of the piece table
+        if (g.rows.pieces > 1 && !g.piece_off) return "bad pieces: fp8 records need a piece table";
+        if (g.rows.pieces > 1 && (g.fp8_elems / g.records.token_elems()) % g.rows.pieces)
+            return "bad pieces: the piece count must divide a part's tokens";
     } else if (g.fp8_elems ? g.fp8_elems % 512 || g.fp8_elems > uint32_t(INT32_MAX)
                            : !g.part_bytes) {
         return "bad part size: raw parts of 1 byte or more, fp8 parts of a multiple of 512 "
@@ -913,7 +917,7 @@ const char* Connection::gather_refusal(const GatherSpec& g, const uint64_t* offs
     if (block_parts > uint64_t(INT32_MAX) / g.pool_part_bytes())
         return "bad parts list: a block holds at most 2^31 - 1 bytes";
     const kernels::PartRows& r = g.rows;
-    if (r.pieces == 0 || (r.pieces > 1 && (!r.rows || !g.piece_off)))
+    if (r.pieces == 0 || (r.pieces > 1 && ((!r.rows && !g.records.latent) || !g.piece_off)))
         return "bad pieces: pieces >= 1, and pieces > 1 need row geometry and a piece table";
     if (r.pieces > 1 && r.rows % r.pieces)
         return "bad pieces: the piece count must divide the rows";

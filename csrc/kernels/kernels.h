@@ -313,7 +313,12 @@ struct GatherLaunch {
     // align_or covers every piece offset.
     const uint64_t* piece_off = nullptr;
     // fp8 launches only (launch_kv_gather_fp8): records.latent != 0 stores each part as token
-    // records (Fp8Records) instead of an fp8 page.  Whole parts only (rows.rows == 0).
+    // records (Fp8Records) instead of an fp8 page.  No row geometry (rows.rows == 0); with
+    // rows.pieces = k > 1 and piece_off, each part's tokens are k runs of tokens / k tokens:
+    // token t of part s of block b is at part_base[s] + desc's local offset + piece_off[b * k +
+    // t / (tokens / k)] + (t % (tokens / k)) * 2 * token_elems, and stays at
+    // fp8_record_offset(records, tokens, first_part + s, t) in the pool block, so a chunk of k
+    // pages is stored as the records of one page of k times the tokens.
     Fp8Records records;
 };
 // The TMA pipeline for 16-byte aligned parts of at least kPipeMinBytes, the ld/st kernel

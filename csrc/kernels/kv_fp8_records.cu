@@ -5,6 +5,10 @@
 //                          straight into the (peer) pool block, then the in-band commit
 //                          (gather_items' control warp: one-shot or a layered writer's).
 //   kv_read_fp8_records  : records -> bf16 part, plain or layered (scatter_items).
+//   kv_{write,read}_fp8_records_pieces : the same with pieces (GatherLaunch::rows.pieces = k >
+//                          1): each part's tokens are k runs of tokens / k tokens, run t of
+//                          block b at its local offset + piece_off[b * k + t] - a chunk of k
+//                          engine pages stored as the records of one page of k times the tokens.
 //
 // The latent is quantised in 128-element rows of the fp8 row contract (fp8_row.cuh): a
 // half-warp owns one row per step as in kv_fp8.cu's write_fp8 (lane l: elements 8l..8l+7, one
@@ -180,6 +184,63 @@ __global__ void __launch_bounds__(kThreads)
     });
 }
 
+// With pieces: the items of the whole-part kernels (runs of `chunk` tokens, which need not line
+// up with the pieces: at 512 + 64 a run is 14 tokens) are cut where the piece t / pt changes
+// (pt = tokens / pieces), and each cut runs the whole-part body from its piece's place in the
+// caller's part: piece_off[block * pieces + t / pt] + (t % pt) tokens, one piece-offset load per
+// cut.  A record, and so a scale row, never crosses a token, so a cut never splits one.  The
+// reads' minimum of 3 CTAs per SM lets ptxas give them 80 registers; without it the layered
+// read was held to 64 and spilled.
+__global__ void __launch_bounds__(kThreads + 32)
+    kv_write_fp8_records_pieces_kernel(const CopyDesc* __restrict__ descs,
+                                       const __grid_constant__ GatherParts parts, uint32_t n,
+                                       uint32_t nparts, uint32_t tokens, uint32_t chunk,
+                                       uint32_t cpp, uint32_t first_part, Fp8Records r,
+                                       const uint64_t* __restrict__ piece_off, uint32_t pieces,
+                                       Publish pub, LayerCommit lc) {
+    gather_items(descs, n, nparts, tokens, chunk, cpp, pub, lc,
+                 [&](const CopyDesc& d, uint32_t block, uint32_t s, uint32_t t0, uint32_t nt) {
+                     const uint32_t pt = tokens / pieces, tb = 2 * r.token_elems();
+                     const uint64_t* off = piece_off + uint64_t(block) * pieces;
+                     const uint64_t src = parts.base[s] + d.src;
+                     uint8_t* rec = reinterpret_cast<uint8_t*>(
+                         d.dst + fp8_record_offset(r, tokens, first_part + s, t0));
+                     for (uint32_t t = t0; t < t0 + nt;) {
+                         const uint32_t p = t / pt, e = min(t0 + nt, (p + 1) * pt);
+                         write_records(rec + size_t(t - t0) * r.record_bytes(),
+                                       reinterpret_cast<const uint8_t*>(src + off[p]) +
+                                           size_t(t - p * pt) * tb,
+                                       e - t, r);
+                         t = e;
+                     }
+                 });
+}
+
+template <bool LAYERED>
+__global__ void __launch_bounds__(kThreads, 3)
+    kv_read_fp8_records_pieces_kernel(const CopyDesc* __restrict__ descs,
+                                      const __grid_constant__ GatherParts parts, uint32_t n,
+                                      uint32_t nparts, uint32_t tokens, uint32_t chunk,
+                                      uint32_t cpp, uint32_t first_part, Fp8Records r,
+                                      const uint64_t* __restrict__ piece_off, uint32_t pieces,
+                                      uint32_t* status, GroupRelease rel) {
+    scatter_items<LAYERED>(descs, n, nparts, cpp, status, rel, [&](const CopyDesc& d,
+                                                                  const LayeredItem& it) {
+        const uint32_t pt = tokens / pieces, tb = 2 * r.token_elems();
+        const uint32_t t0 = it.chunk * chunk, t1 = min(t0 + chunk, tokens);
+        const uint64_t* off = piece_off + uint64_t(it.block) * pieces;
+        const uint64_t dst = parts.base[it.part] + d.dst;
+        const uint8_t* rec = reinterpret_cast<const uint8_t*>(
+            d.src + fp8_record_offset(r, tokens, first_part + it.part, t0));
+        for (uint32_t t = t0; t < t1;) {
+            const uint32_t p = t / pt, e = min(t1, (p + 1) * pt);
+            read_records(reinterpret_cast<uint8_t*>(dst + off[p]) + size_t(t - p * pt) * tb,
+                         rec + size_t(t - t0) * r.record_bytes(), e - t, r);
+            t = e;
+        }
+    });
+}
+
 template <bool WRITE, bool LAYERED>
 cudaError_t launch_records(const GatherLaunch& a, uint32_t elems, cudaStream_t stream) {
     const LaunchPlan p =
@@ -205,6 +266,32 @@ cudaError_t launch_records(const GatherLaunch& a, uint32_t elems, cudaStream_t s
     return cudaGetLastError();
 }
 
+// The same plan and grid for pieces, with the residency of the pieces kernels.
+template <bool WRITE, bool LAYERED>
+cudaError_t launch_records_pieces(const GatherLaunch& a, uint32_t elems, cudaStream_t stream) {
+    const LaunchPlan p =
+        WRITE ? plan_gather_fp8_records(
+                    a, elems, sm_count(),
+                    cached_resident<kv_write_fp8_records_pieces_kernel,
+                                    kv_write_fp8_records_pieces_kernel, kThreads + 32>())
+              : plan_gather_fp8_records(
+                    a, elems, sm_count(),
+                    cached_resident<kv_read_fp8_records_pieces_kernel<LAYERED>,
+                                    kv_read_fp8_records_pieces_kernel<LAYERED>, kThreads>());
+    if (!p.valid) return cudaErrorInvalidValue;
+    const GatherParts parts = parts_of(a);
+    const uint32_t tokens = elems / a.records.token_elems();
+    if constexpr (WRITE)
+        kv_write_fp8_records_pieces_kernel<<<p.ctas, kThreads + 32, 0, stream>>>(
+            a.descs, parts, a.n, a.nparts, tokens, p.chunk, p.cpb, a.first_part, a.records,
+            a.piece_off, a.rows.pieces, publish_of(a, true), layer_of(a));
+    else
+        kv_read_fp8_records_pieces_kernel<LAYERED><<<p.ctas, kThreads, 0, stream>>>(
+            a.descs, parts, a.n, a.nparts, tokens, p.chunk, p.cpb, a.first_part, a.records,
+            a.piece_off, a.rows.pieces, a.status, release_of(a));
+    return cudaGetLastError();
+}
+
 }  // namespace
 
 cudaError_t launch_kv_gather_fp8_records(const GatherLaunch& a, uint32_t elems,
@@ -213,6 +300,12 @@ cudaError_t launch_kv_gather_fp8_records(const GatherLaunch& a, uint32_t elems,
     if (!a.part_base) return cudaErrorInvalidValue;
     const bool layered = a.group_flags != nullptr;
     if (layered && !a.group_counters) return cudaErrorInvalidValue;
+    if (a.rows.pieces > 1) {  // pieces of whole tokens, at the offsets of the piece table
+        if (!a.piece_off) return cudaErrorInvalidValue;
+        if (a.write) return launch_records_pieces<true, false>(a, elems, stream);
+        return layered ? launch_records_pieces<false, true>(a, elems, stream)
+                       : launch_records_pieces<false, false>(a, elems, stream);
+    }
     if (a.write) return launch_records<true, false>(a, elems, stream);
     return layered ? launch_records<false, true>(a, elems, stream)
                    : launch_records<false, false>(a, elems, stream);

@@ -452,8 +452,11 @@ inline uint64_t fp8_records_bytes(uint32_t nparts, uint32_t elems, const Fp8Reco
 // Reads (plain or layered) and writes of whole parts as records: always the ld/st kernels.
 // A work item is a run of `chunk` tokens of one part, about kFp8Chunk elements, or every token
 // of the part under ldst_items' rule; cpb is runs per part, and a layered read numbers items with
-// layered_item as whole parts do.  Refused: bad records (Fp8Records::ok), a part that is not a
-// whole number of tokens, row geometry, part bases or local offsets that are not 16-byte
+// layered_item as whole parts do.  Pieces (rows.pieces = k > 1, no row geometry): each
+// part's tokens are k runs of tokens / k, and the items, chunk, cpb and grid are those of whole
+// parts (the kernels cut items at piece boundaries).  Refused: bad records (Fp8Records::ok), a
+// part that is not a whole number of tokens, row geometry, pieces that do not divide the
+// tokens, part bases, local offsets or piece offsets (all in align_or) that are not 16-byte
 // aligned, and more than kMaxItems work items.  The grid is one wave of the CTAs the kernel
 // keeps resident (res.r16).
 inline LaunchPlan plan_gather_fp8_records(const GatherLaunch& a, uint32_t elems, int sms,
@@ -461,8 +464,9 @@ inline LaunchPlan plan_gather_fp8_records(const GatherLaunch& a, uint32_t elems,
     const Fp8Records& r = a.records;
     const uint64_t parts = uint64_t(a.n) * a.nparts;
     if (!r.ok() || elems == 0 || elems % r.token_elems() != 0 || a.rows.rows != 0 ||
-        a.rows.pieces != 1 || a.nparts == 0 || a.nparts > kGatherMaxParts || !groups_ok(a) ||
-        (a.align_or & 15) != 0 || parts > kMaxItems)
+        a.rows.pieces == 0 || (elems / r.token_elems()) % a.rows.pieces != 0 || a.nparts == 0 ||
+        a.nparts > kGatherMaxParts || !groups_ok(a) || (a.align_or & 15) != 0 ||
+        parts > kMaxItems)
         return invalid_plan();
     const uint32_t te = r.token_elems();
     LaunchPlan p;

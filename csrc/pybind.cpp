@@ -665,7 +665,9 @@ PYBIND11_MODULE(_infinistore, m) {
             py::arg("records") = std::vector<uint32_t>{},
             "gathered write: block i = part s at part_base[s] + offsets[i] * scale, s = 0..S-1; "
             "elems > 0: bf16 parts of elems elements, quantised into fp8 page s of block i, or "
-            "with records = (latent, rope) into elems / (latent + rope) fp8 token records; "
+            "with records = (latent, rope) into elems / (latent + rope) fp8 token records "
+            "(with pieces > 1 and no rows: run t of pieces runs of whole tokens from "
+            "part_base[s] + offset + piece_off[i * pieces + t]); "
             "rows = (rows, row_bytes, src_pitch, 0, dst_pitch[, slices, dst_slice_pitch]) filling "
             "each stored part: slice j of stored row r from part_base[s] + offset + r * "
             "dst_pitch + j * dst_slice_pitch; pieces > 1 (with rows): piece_off holds pieces "
@@ -1168,7 +1170,10 @@ PYBIND11_MODULE(_infinistore, m) {
         py::arg("records") = std::vector<uint32_t>{},
         "gathered fp8 blocks: descs as for kv_gather; records = (latent, rope): every part is "
         "elems / (latent + rope) bf16 tokens stored as fp8 token records (kv_write_fp8_records, "
-        "kv_read_fp8_records; whole parts, any variant); pieces as for kv_gather; part s (elems bf16 elements at "
+        "kv_read_fp8_records; no rows, any variant; with pieces > 1 and piece_off, run t of "
+        "the elems / (latent + rope) / pieces tokens of each part at its local offset + "
+        "piece_off[i * pieces + t]: kv_{write,read}_fp8_records_pieces); pieces as for "
+        "kv_gather; part s (elems bf16 elements at "
         "part_base[s] + local offset) <-> fp8 page first_part + s of the block; layer_* and "
         "group_* as for kv_gather (a layered read always runs the ld/st kernel); rows as for "
         "kv_gather, in bytes of the parts' bf16 view: a read dequantises those rows of each "
@@ -1937,7 +1942,7 @@ PYBIND11_MODULE(_infinistore, m) {
     t.def("plan_gather_fp8_records",
           [plan_dict](uint32_t n, uint32_t nparts, uint32_t elems, uint32_t latent, uint32_t rope,
                       uint64_t align_or, uint32_t group_parts, bool write, int max_ctas,
-                      int sm_count, int resident, uint32_t rows) {
+                      int sm_count, int resident, uint32_t rows, uint32_t pieces) {
               static uint32_t flags[1];
               kernels::GatherLaunch a;
               a.n = n;
@@ -1949,13 +1954,14 @@ PYBIND11_MODULE(_infinistore, m) {
               a.max_ctas = max_ctas;
               a.records = kernels::Fp8Records{latent, rope};
               a.rows.rows = rows;  // any row geometry is refused
+              a.rows.pieces = pieces;  // piece offsets count in align_or
               return plan_dict(
                   kernels::plan_gather_fp8_records(a, elems, sm_count, {resident, resident}));
           },
           py::arg("n"), py::arg("nparts"), py::arg("elems"), py::arg("latent"), py::arg("rope"),
           py::arg("align_or") = 0, py::arg("group_parts") = 0, py::arg("write") = false,
           py::arg("max_ctas") = 0, py::arg("sm_count") = 132, py::arg("resident") = 1,
-          py::arg("rows") = 0);
+          py::arg("rows") = 0, py::arg("pieces") = 1);
     t.def("fp8_rows_read_bytes", &fp8_rows_read_bytes, py::arg("rows"), py::arg("row_bytes"),
           py::arg("src_pitch"), py::arg("src_col") = 0,
           "bytes_read of a row-sliced read of one stored fp8 part (geometry in bf16 bytes)");

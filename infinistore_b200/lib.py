@@ -828,7 +828,9 @@ class InfinityConnection:
         ``(n, k)`` (with ``rows``, ``k`` dividing ``rows.count``): piece i of every part of
         block b, rows ``i * count / k .. (i + 1) * count / k - 1``, is at ``offsets[b, i]``;
         ``k == 1`` is the 1-D call.  ``records`` (an :class:`FP8Records`, with ``fp8``): the
-        parts are stored as token records, ``part_size`` a whole number of tokens, no ``rows``.
+        parts are stored as token records, ``part_size`` a whole number of tokens, no ``rows``;
+        its 2-D offsets need no ``rows``: piece i of every part of block b, tokens ``i * T / k
+        .. (i + 1) * T / k - 1`` of the part's ``T`` tokens, is at ``offsets[b, i]``.
         Returns the native call's arguments (``_Gather``): with pieces its offsets are zeros
         and its piece arguments carry the ``(n, k)`` offsets."""
         if self._mode != "rdma":
@@ -837,15 +839,21 @@ class InfinityConnection:
         offs = _block_offsets(offsets, nblocks)
         table = None
         if offs.ndim == 2:
-            if rows is None:
+            if records is not None:  # pieces of whole tokens
+                tokens = int(part_size) // records.token_dim
+                if tokens % offs.shape[1]:
+                    raise ValueError(f"{offs.shape[1]} pieces do not divide the {tokens} tokens")
+            elif rows is None:
                 raise ValueError("2-D offsets (one per piece of a block) need rows=")
-            if rows.count % offs.shape[1]:
+            elif rows.count % offs.shape[1]:
                 raise ValueError(f"{offs.shape[1]} pieces do not divide the {rows.count} rows")
             table, offs = offs, np.zeros(len(offs), dtype=np.int64)
         first_part = int(first_part)
         if first_part < 0:
             raise ValueError("first_part must not be negative")
-        if table is not None:  # each piece is count / k rows of part_size / k elements
+        if table is not None and records is not None:  # each piece is part_size / k elements
+            extent = int(part_size) // table.shape[1]
+        elif table is not None:  # each piece is count / k rows of part_size / k elements
             k = table.shape[1]
             extent = PartRows(rows.count // k, rows.width, rows.src_pitch, rows.src_offset,
                               dst_pitch=rows.dst_pitch, slices=rows.slices,
@@ -1061,7 +1069,11 @@ class InfinityConnection:
         ``part_size // records.token_dim`` of them from byte
         ``fp8_gather_block_bytes(s, part_size, records=records)``; allocate
         ``fp8_gather_block_bytes(len(parts), part_size, records=records)`` bytes.  No
-        ``rows``."""
+        ``rows``; ``offsets`` may be an ``(n, k)`` int64 array (pieces of whole tokens, k
+        dividing ``part_size // records.token_dim``): tokens ``i * T / k .. (i + 1) * T / k -
+        1`` of every part of block b, of its ``T`` tokens, are taken from ``offsets[b, i]`` -
+        e.g. a chunk of k MLA engine pages stored as the records of one page of k times the
+        tokens."""
         self._gather_write(parts, offsets, part_size, stream, rows, True, records, remote_blocks)
         return 0
 
@@ -1084,7 +1096,9 @@ class InfinityConnection:
         records, each dequantised latent row bit for bit ``bf16_rne(e4m3 * scale)`` and the
         RoPE elements copied back verbatim.  With ``device_lookup`` a stored block shorter than
         ``fp8_gather_block_bytes(first_part + len(parts), part_size, records=records)`` is a
-        miss.  No ``rows``."""
+        miss.  No ``rows``; ``(keys, offsets)`` may carry an ``(n, k)`` int64 array (pieces of
+        whole tokens, as for ``rdma_write_cache_gather_fp8``): run i of every part's tokens of
+        block b lands at ``offsets[b, i]``."""
         self._scatter_read(parts, blocks, part_size, first_part, stream, rows, True, records)
 
     # ------------------------------------------------------------------ layered scattered reads
@@ -1105,8 +1119,8 @@ class InfinityConnection:
         read's post-copy index check: when ``sync()`` reports a miss, treat the whole read as
         failed, as for any read.  A missing key on a connection without ``device_lookup``
         raises here; the exception's ``read`` attribute is the failed reader.  ``rows`` as for
-        ``read_cache_scatter[_fp8]``, ``records`` (with ``fp8``) as for
-        ``read_cache_scatter_fp8``."""
+        ``read_cache_scatter[_fp8]``, ``records`` (with ``fp8``, and its pieces of whole
+        tokens without ``rows``) as for ``read_cache_scatter_fp8``."""
         return self._scatter_read(parts, blocks, part_size, first_part, stream, rows, fp8, records,
                                   group_parts)
 
@@ -1124,7 +1138,9 @@ class InfinityConnection:
         completes leaves its blocks uncommitted; closing the connection releases them.
         ``records`` (an :class:`FP8Records`, with ``fp8``): every call stores token records,
         and the blocks were allocated with ``fp8_gather_block_bytes(nparts, part_size,
-        records=records)`` bytes."""
+        records=records)`` bytes.  2-D ``offsets`` ``(n, k)`` are pieces, used by every call:
+        of rows (each call passes ``rows=``), or with ``records`` of whole tokens (no
+        ``rows=``), as for ``rdma_write_cache_gather[_fp8]``."""
         if self._mode != "rdma":
             raise Exception("gathered blocks need a connected rdma connection")
         _check_records(records, part_size, fp8)
@@ -1402,7 +1418,8 @@ class GatherWriter:
         or runs past the block, another device or dtype, a complete or failed writer, and
         everything ``rdma_write_cache_gather`` (``_gather_fp8``) refuses.  ``rows`` as for
         ``rdma_write_cache_gather``; one call may take rows and another not, and every call
-        stores whole parts."""
+        stores whole parts.  A writer made with ``records`` and 2-D offsets (pieces of whole
+        tokens) takes no ``rows``."""
         if self._w.failed or self._w.complete:
             raise ValueError("the writer is complete or has failed")
         parts = list(parts)
@@ -1413,7 +1430,7 @@ class GatherWriter:
         written = self._w.written
         if any(written[first_part:first_part + len(parts)]):
             raise ValueError("the part range overlaps parts written before")
-        if self._offs.ndim == 2 and rows is None:
+        if self._offs.ndim == 2 and rows is None and self.records is None:
             raise ValueError("a writer made with 2-D offsets (pieces) needs rows= on every call")
         self._conn._gather_write(parts, self._offs, self.part_size, stream, rows, self.fp8,
                                  self.records, writer=self, first_part=first_part)

@@ -175,3 +175,13 @@ def mla_page_key(model: str, page_hash: str, fp8: bool = False) -> str:
     holds the same latent and names the same block; and the stored format is part of the key,
     so a bf16 reader never resolves an fp8 block, nor the other way round."""
     return f"{model}/L{ALL_LAYERS}/{'MLA8' if fp8 else 'MLA'}/{page_hash}"
+
+
+def mla_chunk_key(model: str, chunk_tokens: int, chunk_hash: str, fp8: bool = False) -> str:
+    """Key of one all-layer MLA chunk of ``chunk_tokens`` tokens (``MLAKVCache.write_chunks``):
+    ``model/Lall/MLAx<tokens>/<hash>``, or ``MLA8x<tokens>`` for fp8 token records.  Like
+    ``mla_page_key`` it has no TP field and names the format; like ``chunk_key`` it names the
+    token count, so MLA caches of any page size that store the same chunk size name the same
+    block, and chunks of another size, pages and K/V keys never resolve to it.  ``chunk_hash``
+    comes from ``chain_hashes(token_ids, chunk_tokens)``."""
+    return f"{model}/L{ALL_LAYERS}/{'MLA8' if fp8 else 'MLA'}x{int(chunk_tokens)}/{chunk_hash}"

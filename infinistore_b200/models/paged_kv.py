@@ -7,8 +7,8 @@ import numpy as np
 import torch
 
 from ..lib import _GATHER_MAX_BLOCK_BYTES, FP8Records, PartRows
-from .kv_layout import (ALL_LAYERS, KVLayout, MLALayout, chunk_key, mla_page_key, page_key,
-                        tp_sources)
+from .kv_layout import (ALL_LAYERS, KVLayout, MLALayout, chunk_key, mla_chunk_key, mla_page_key,
+                        page_key, tp_sources)
 
 
 def _layer_range(layers: Optional[range], n: int) -> range:
@@ -82,6 +82,33 @@ class _AllLayerPages:
         n = self.num_pages * self.layout.page_elems
         return [(self.data, (layer * self._per_layer + i) * n)
                 for layer in layers for i in range(self._per_layer)]
+
+    @staticmethod
+    def _chunk_rows(rows: Optional[PartRows], k: int, part: int) -> PartRows:
+        """The rows of a k-page chunk from one page's rows (``_source_rows``, ``_write_rows``):
+        ``k * count`` rows with the same pitches, one piece per page.  A page that is its
+        stored part of ``part`` elements, contiguously, is one row of ``part`` elements."""
+        if rows is None or (rows.slices == 1 and rows.src_offset == 0
+                            and rows.width == rows.src_pitch == rows.dst_pitch):
+            return PartRows(k, part, part, 0, dst_pitch=part)
+        return PartRows(rows.count * k, rows.width, rows.src_pitch, rows.src_offset,
+                        dst_pitch=rows.dst_pitch, slices=rows.slices,
+                        dst_slice_pitch=rows.dst_slice_pitch)
+
+    def _chunk_table(self, block_table, chunk_hashes: Sequence[str], read: bool) -> np.ndarray:
+        """The checked (n, k) block table of chunks; ValueError before anything happens."""
+        table = np.asarray(block_table, dtype=np.int64)
+        if table.ndim != 2 or table.shape[1] < 1:
+            raise ValueError("block_table is an (n, k) array of page indices, k >= 1")
+        if table.shape[0] != len(chunk_hashes):
+            raise ValueError(f"{table.shape[0]} block-table rows for {len(chunk_hashes)} chunk "
+                             f"hashes")
+        if table.size and (int(table.min()) < 0 or int(table.max()) >= self.num_pages):
+            raise ValueError(f"a page index is outside 0..{self.num_pages - 1}")
+        if read and len(np.unique(table)) != table.size:
+            raise ValueError("a page appears twice in the block table: two chunks would land "
+                             "on it")
+        return table
 
     def _format(self, plan: _Plan, fp8: bool) -> Optional[FP8Records]:
         """The records of the call's format (None: bf16 or fp8 pages).  ValueError, before
@@ -329,18 +356,6 @@ class _PagedCache(_AllLayerPages):
                                              chunk_pages, every))
 
     # ------------------------------------------------------------------ all-layer chunks
-    @staticmethod
-    def _chunk_rows(rows: Optional[PartRows], k: int, part: int) -> PartRows:
-        """The rows of a k-page chunk from one page's rows (``_source_rows``, ``_write_rows``):
-        ``k * count`` rows with the same pitches, one piece per page.  A page that is its
-        stored part of ``part`` elements, contiguously, is one row of ``part`` elements."""
-        if rows is None or (rows.slices == 1 and rows.src_offset == 0
-                            and rows.width == rows.src_pitch == rows.dst_pitch):
-            return PartRows(k, part, part, 0, dst_pitch=part)
-        return PartRows(rows.count * k, rows.width, rows.src_pitch, rows.src_offset,
-                        dst_pitch=rows.dst_pitch, slices=rows.slices,
-                        dst_slice_pitch=rows.dst_slice_pitch)
-
     def chunk_keys(self, chunk_hashes: Sequence[str], chunk_pages: int) -> List[str]:
         """Store keys of chunks of ``chunk_pages`` pages (``kv_layout.chunk_key``)."""
         tokens = int(chunk_pages) * self.layout.page_tokens
@@ -353,21 +368,6 @@ class _PagedCache(_AllLayerPages):
         srcs = tp_sources(self.layout, self.layout.tp, self.tp_rank, int(source_tp))
         return [[chunk_key(self.layout.name, tokens, w, h) for h in chunk_hashes]
                 for w, *_ in srcs]
-
-    def _chunk_table(self, block_table, chunk_hashes: Sequence[str], read: bool) -> np.ndarray:
-        """The checked (n, k) block table of chunks; ValueError before anything happens."""
-        table = np.asarray(block_table, dtype=np.int64)
-        if table.ndim != 2 or table.shape[1] < 1:
-            raise ValueError("block_table is an (n, k) array of page indices, k >= 1")
-        if table.shape[0] != len(chunk_hashes):
-            raise ValueError(f"{table.shape[0]} block-table rows for {len(chunk_hashes)} chunk "
-                             f"hashes")
-        if table.size and (int(table.min()) < 0 or int(table.max()) >= self.num_pages):
-            raise ValueError(f"a page index is outside 0..{self.num_pages - 1}")
-        if read and len(np.unique(table)) != table.size:
-            raise ValueError("a page appears twice in the block table: two chunks would land "
-                             "on it")
-        return table
 
     def _chunk_write_plan(self, block_table, chunk_hashes: Sequence[str]) -> _Plan:
         table = self._chunk_table(block_table, chunk_hashes, read=False)
@@ -626,7 +626,14 @@ class MLAKVCache(_AllLayerPages):
     the first writer's block.  The methods follow the semantics and refusals of the
     ``PagedKVCache`` methods of the same names: step-1 layer ranges, first writer wins, a
     failed read leaves its pages untouched and reported.  ``fp8`` must be what the writer
-    used; bf16 and fp8 pages have different keys."""
+    used; bf16 and fp8 pages have different keys.
+
+    Chunks (``write_chunks``, ``chunk_writer``, ``read_chunks[_layered]``) store k pages under
+    one key (``mla_chunk_key``): the stored block is the all-layer page of ``k * page_tokens``
+    tokens that an ``MLAKVCache`` of that page size stores, so caches of different page sizes
+    share chunks of one size, and page i of chunk b is this cache's page ``block_table[b, i]``.
+    The kernels land each page through the block table: bf16 as one row per page
+    (``PartRows`` pieces), fp8 as pieces of whole tokens of the record movers."""
 
     _per_layer = 1
     _fp8_pages = "fp8 MLA pages"
@@ -680,13 +687,74 @@ class MLAKVCache(_AllLayerPages):
         return self._read(conn, self._plan(pages, page_hashes, fp8), layers, fp8, stream,
                           layered=True)
 
-    def cached_prefix_pages(self, conn, page_hashes: Sequence[str], fp8: bool = False) -> int:
-        """How many leading pages of this prefix the store holds in this format."""
+    def _prefix_keys(self, page_hashes: Sequence[str], fp8: bool, chunk_pages: int) -> List[str]:
+        return (self.chunk_keys(page_hashes, chunk_pages, fp8) if chunk_pages
+                else self.page_keys(page_hashes, fp8))
+
+    def cached_prefix_pages(self, conn, page_hashes: Sequence[str], fp8: bool = False,
+                            chunk_pages: int = 0) -> int:
+        """How many leading pages of this prefix the store holds in this format.
+        ``chunk_pages`` k > 0: ``page_hashes`` are chunk hashes of chunks of k pages
+        (``write_chunks``), and the answer counts chunks."""
         if not page_hashes:
             return 0
-        return _prefix_pages(conn, [self.page_keys(page_hashes, fp8)])
+        return _prefix_pages(conn, [self._prefix_keys(page_hashes, fp8, chunk_pages)])
 
-    def touch_prefix(self, conn, page_hashes: Sequence[str], fp8: bool = False) -> int:
+    def touch_prefix(self, conn, page_hashes: Sequence[str], fp8: bool = False,
+                     chunk_pages: int = 0) -> int:
         """Tell an evicting store (``--evict``) that these pages were just used.  Returns the
-        number of blocks refreshed."""
-        return _touch(conn, [self.page_keys(page_hashes, fp8)])
+        number of blocks refreshed.  ``chunk_pages`` k > 0: chunk hashes of chunks of k pages
+        (``write_chunks``)."""
+        return _touch(conn, [self._prefix_keys(page_hashes, fp8, chunk_pages)])
+
+    # ------------------------------------------------------------------ all-layer chunks
+    def chunk_keys(self, chunk_hashes: Sequence[str], chunk_pages: int,
+                   fp8: bool = False) -> List[str]:
+        """Store keys of chunks of ``chunk_pages`` pages (``kv_layout.mla_chunk_key``)."""
+        tokens = int(chunk_pages) * self.layout.page_tokens
+        return [mla_chunk_key(self.layout.name, tokens, h, fp8) for h in chunk_hashes]
+
+    def _chunk_plan(self, block_table, chunk_hashes: Sequence[str], fp8: bool,
+                    read: bool) -> _Plan:
+        """A chunk's part is the page of ``k * page_tokens`` tokens; in bf16 each page of the
+        block table is one row of it (``_chunk_rows``), in fp8 one piece of whole tokens."""
+        table = self._chunk_table(block_table, chunk_hashes, read)
+        k, elems = table.shape[1], self.layout.page_elems
+        return _Plan(self.chunk_keys(chunk_hashes, k, fp8), table * elems,
+                     None if fp8 else self._chunk_rows(None, k, elems), k * elems)
+
+    def write_chunks(self, conn, block_table, chunk_hashes: Sequence[str], stream="current",
+                     fp8: bool = False) -> int:
+        """``write_pages`` for chunks: chunk b, pages ``block_table[b, 0..k-1]`` of this cache
+        in token order (``k * page_tokens`` tokens), is stored under ``chunk_keys`` as the
+        all-layer page an ``MLAKVCache`` with ``page_tokens = k * page_tokens`` stores for the
+        same tokens, in bf16 or (``fp8``) as token records.  ``chunk_hashes`` come from
+        ``chain_hashes(token_ids, k * page_tokens)``; only full chunks are stored.  Blocks
+        whose key already exists are skipped.  Raises ``ValueError`` before any block is
+        allocated for a table whose row count differs from the hashes, a page index outside
+        the cache, a chunk over the block limit and every ``write_pages`` refusal.  Returns
+        the number of blocks asked for."""
+        return self._store(conn, self._chunk_plan(block_table, chunk_hashes, fp8, False), fp8,
+                           stream)
+
+    def chunk_writer(self, conn, block_table, chunk_hashes: Sequence[str],
+                     fp8: bool = False) -> "PageWriter":
+        """``page_writer`` for chunks (``write_chunks``): ``write_layers`` stores layers of
+        every chunk as they are produced."""
+        return self._writer(conn, self._chunk_plan(block_table, chunk_hashes, fp8, False), fp8)
+
+    def read_chunks(self, conn, block_table, chunk_hashes: Sequence[str],
+                    layers: Optional[range] = None, stream="current", fp8: bool = False) -> int:
+        """``read_pages`` for chunks written by ``write_chunks`` / ``chunk_writer`` of a cache
+        of any page size: page i of chunk b lands in this cache's page ``block_table[b, i]``.
+        A page that appears twice in the table raises ``ValueError`` (two chunks would race
+        on it).  Returns the number of blocks read."""
+        return self._read(conn, self._chunk_plan(block_table, chunk_hashes, fp8, True), layers,
+                          fp8, stream)
+
+    def read_chunks_layered(self, conn, block_table, chunk_hashes: Sequence[str],
+                            layers: Optional[range] = None, fp8: bool = False,
+                            stream="current") -> "PageRead":
+        """``read_pages_layered`` for chunks (``read_chunks``)."""
+        return self._read(conn, self._chunk_plan(block_table, chunk_hashes, fp8, True), layers,
+                          fp8, stream, layered=True)

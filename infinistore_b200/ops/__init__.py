@@ -382,7 +382,10 @@ def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, wri
     kv_write_fp8_pieces).  ``records`` = (latent, rope): every part is ``elems // (latent +
     rope)`` bf16 tokens stored as fp8 token records (``lib.FP8Records``; kv_write_fp8_records,
     kv_read_fp8_records, whatever the variant), part s at byte ``fp8_records_bytes(first_part +
-    s, elems, latent, rope)`` of the block; no ``rows`` or ``pieces``."""
+    s, elems, latent, rope)`` of the block; no ``rows``.  ``records`` with ``pieces`` (k > 1,
+    dividing the part's tokens T): tokens ``t * T / k .. (t + 1) * T / k - 1`` of each part of
+    block i are at its local offset + ``pieces[i, t]`` (kv_write_fp8_records_pieces,
+    kv_read_fp8_records_pieces), stored where the whole-part write stores them."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
     bases = [int(b) for b in part_base]
     for b in bases:
