@@ -210,11 +210,18 @@ class Connection {
         // fp8 parts only: records.latent != 0 stores every part as fp8_elems / token_elems()
         // token records (kernels::Fp8Records) instead of an fp8 page; whole parts only
         kernels::Fp8Records records;
+        // fp8 parts only: a host array of nparts scales makes the parts e4m3 caches
+        // (kernels::GatherLaunch::part_scale): part s is fp8_elems bytes of float8_e4m3fn of
+        // scale part_scale[s], stored as an fp8 page; whole parts only
+        const float* part_scale = nullptr;
         // pool bytes of a part: part_bytes, kernels::fp8_gather_bytes(1, fp8_elems), or with
         // records kernels::fp8_records_bytes(1, fp8_elems, records)
         uint64_t pool_part_bytes() const;
-        // bytes of a part in the caller's tensors: part_bytes, or 2 * fp8_elems (bf16)
-        uint64_t view_part_bytes() const { return fp8_elems ? 2ull * fp8_elems : part_bytes; }
+        // bytes of a part in the caller's tensors: part_bytes, 2 * fp8_elems (bf16), or with
+        // part_scale fp8_elems (e4m3)
+        uint64_t view_part_bytes() const {
+            return part_scale ? fp8_elems : fp8_elems ? 2ull * fp8_elems : part_bytes;
+        }
         // bytes a stored block must hold to serve a read: parts 0 .. first_part + nparts - 1
         uint64_t need_bytes() const { return (uint64_t(first_part) + nparts) * pool_part_bytes(); }
     };
@@ -238,6 +245,7 @@ class Connection {
         uint64_t scale = 0;               // bytes per offset unit, fixed by the first call
         uint32_t fp8_elems = 0;           // fp8 elements per part (0: raw bytes), first call
         kernels::Fp8Records records;      // GatherSpec::records of the first call
+        bool e4m3 = false;                // the first call's parts were e4m3 (part_scale)
         uint32_t part_bytes = 0;          // pool bytes of a part, first call
         bool failed = false;
         void* event = nullptr;            // cudaEvent_t recorded after the last launch
@@ -254,7 +262,7 @@ class Connection {
                                                 uint32_t pieces = 1);
     // Stores parts g.first_part .. g.first_part + g.nparts - 1 of every block of `w`; offsets
     // are scaled by `scale`.  Refuses part ranges written before, a device, scale, fp8_elems,
-    // records or part size other than the first call's, a complete or failed writer, and a writer made
+    // records, e4m3 parts (part_scale) or not, or part size other than the first call's, a complete or failed writer, and a writer made
     // before the connection was last closed (its blocks and index ways were released).  A
     // refused call leaves the writer as it was.
     int write_layered(GatherWriter& w, const GatherSpec& g, uint64_t scale, int device,

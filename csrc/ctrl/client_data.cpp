@@ -6,6 +6,7 @@
 #include <algorithm>
 #include <atomic>
 #include <cerrno>
+#include <cfloat>
 #include <chrono>
 #include <cstring>
 #include <mutex>
@@ -291,6 +292,7 @@ kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n,
     G.ring_bytes = pipe_ring_;
     G.rows = g.rows;  // the caller stages the piece table beside the descriptors
     G.records = g.records;
+    G.part_scale = g.part_scale;
     return G;
 }
 
@@ -892,6 +894,18 @@ const char* Connection::gather_refusal(const GatherSpec& g, const uint64_t* offs
                                        int device, bool write, const GatherWriter* w) const {
     if (!g.part_base || g.nparts < 1 || g.nparts > kernels::kGatherMaxParts)
         return "bad parts list: 1 to GATHER_MAX_PARTS parts";
+    if (g.part_scale) {  // e4m3 caches: whole fp8 pages of e4m3 parts at one scale each
+        if (!g.fp8_elems) return "e4m3 parts (scales) need fp8 parts";
+        if (g.records.latent || g.rows.rows || g.rows.pieces != 1 || g.piece_off)
+            return "e4m3 parts (scales) take whole parts: no records, row geometry or pieces";
+        for (uint32_t s = 0; s < g.nparts; ++s)
+            if (!(g.part_scale[s] >= FLT_MIN && g.part_scale[s] <= FLT_MAX))
+                return "bad scale for e4m3 parts: every scale must be finite, positive and normal";
+        if (w && w->device != -2 && !w->e4m3)
+            return "e4m3 parts (scales) differ from the writer's first call";
+    } else if (w && w->device != -2 && w->e4m3) {
+        return "parts without scales differ from the writer's first call, whose parts were e4m3";
+    }
     if (g.records.latent) {  // token records: whole parts of whole tokens, bf16 in the tensors
         if (!g.fp8_elems) return "fp8 records need fp8 parts (bf16 elements in the tensors)";
         if (!g.records.ok())
@@ -1078,6 +1092,7 @@ int Connection::write_layered(GatherWriter& w, const GatherSpec& g, uint64_t sca
         w.scale = scale;
         w.fp8_elems = g.fp8_elems;
         w.records = g.records;
+        w.e4m3 = g.part_scale != nullptr;
         w.part_bytes = uint32_t(g.pool_part_bytes());
         w.offsets.swap(scaled);
         w.piece_off.swap(scaled_pieces);

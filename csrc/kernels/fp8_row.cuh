@@ -13,6 +13,11 @@
 // inf, which read back as a row of NaN.
 // There is no direct bf16<->e4m3 cvt on sm_90a: quantise via f32, dequantise via f16x2 (e4m3
 // -> f16 is exact).
+// e4m3 caches (kv_fp8_cache.cu) store a part's e4m3 bytes verbatim with every group scale the
+// part's scale s_c, and a read requantises a stored group (bytes q, scale s_g) to its cache's
+// scale: verbatim when s_g and s_c are the same float (bitwise), else
+//   r  = min(rn32(s_g / s_c), FLT_MAX)          (IEEE division: __fdiv_rn)
+//   q' = e4m3_satfinite_rne(rn32(e4m3(q) * r))  (requant16; NaN -> 0x7F, zeros keep the sign)
 #pragma once
 
 #include <cuda_bf16.h>
@@ -105,6 +110,26 @@ __device__ __forceinline__ uint4 dequant8(uint2 v, float sc) {
         o[2 * j + 1] = f2_to_bf16x2(f23.x * sc, f23.y * sc);
     }
     return make_uint4(o[0], o[1], o[2], o[3]);
+}
+
+// 16 e4m3 values of one group (v) requantised by the ratio r of their stored scale to the
+// reading cache's (kv_fp8_cache.cu, docs/kernels.md "e4m3 cache contract"):
+//   q' = e4m3_satfinite_rne(rn32(e4m3(q) * r))
+// e4m3 -> f16 is exact, f16 -> f32 too, and __fmul_rn keeps the product from being contracted
+// or flushed.  A NaN code comes out as 0x7F, a zero keeps its sign, finite values beyond +-448
+// (and an f32 product that overflows) saturate to +-448.
+__device__ __forceinline__ uint4 requant16(uint4 v, float r) {
+    uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const uint32_t h01 = cvt_f16x2_e4m3x2(uint16_t(w[j] & 0xffffu));
+        const uint32_t h23 = cvt_f16x2_e4m3x2(uint16_t(w[j] >> 16));
+        const float2 f01 = __half22float2(*reinterpret_cast<const __half2*>(&h01));
+        const float2 f23 = __half22float2(*reinterpret_cast<const __half2*>(&h23));
+        w[j] = uint32_t(cvt_e4m3x2(__fmul_rn(f01.y, r), __fmul_rn(f01.x, r))) |
+               (uint32_t(cvt_e4m3x2(__fmul_rn(f23.y, r), __fmul_rn(f23.x, r))) << 16);
+    }
+    return make_uint4(w[0], w[1], w[2], w[3]);
 }
 
 }  // namespace istore::kernels::fp8row

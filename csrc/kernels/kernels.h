@@ -320,6 +320,11 @@ struct GatherLaunch {
     // fp8_record_offset(records, tokens, first_part + s, t) in the pool block, so a chunk of k
     // pages is stored as the records of one page of k times the tokens.
     Fp8Records records;
+    // fp8 launches only: part_scale != nullptr (a host array of nparts floats, finite, positive
+    // and normal) makes the parts e4m3 caches (kv_fp8_cache.cu): part s is `elems` bytes of
+    // float8_e4m3fn at part_base[s] + the local offset with scale part_scale[s], stored as the
+    // fp8 page of a whole part.  No records, row geometry or pieces.
+    const float* part_scale = nullptr;
 };
 // The TMA pipeline for 16-byte aligned parts of at least kPipeMinBytes, the ld/st kernel
 // (kv_copy.cu) otherwise: the same rule launch_kv_copy applies to whole blocks.  Reads run
@@ -392,6 +397,11 @@ cudaError_t launch_kv_gather_fp8(const GatherLaunch& a, uint32_t elems, int vari
                                  cudaStream_t stream);
 cudaError_t launch_kv_gather_fp8_records(const GatherLaunch& a, uint32_t elems,
                                          cudaStream_t stream);
+// With a.part_scale the parts are e4m3 caches instead (kv_fp8_cache.cu, ld/st whatever the
+// variant): a write keeps each part's `elems` e4m3 bytes verbatim as the page payload with
+// every group scale part_scale[s]; a read requantises each stored group to part_scale[s]
+// (verbatim when the scales are equal).  The block is the one launch_kv_gather_fp8 stores.
+cudaError_t launch_kv_gather_e4m3(const GatherLaunch& a, uint32_t elems, cudaStream_t stream);
 cudaError_t launch_kv_fp8_pipe_gather(const GatherLaunch& a, uint32_t elems, cudaStream_t stream);
 
 // Device-side key lookup: hash the packed key bytes, probe the index, and either build

@@ -437,6 +437,7 @@ cudaError_t launch_kv_read_fp8(const Fp8Launch& a, cudaStream_t stream) {
 
 cudaError_t launch_kv_gather_fp8(const GatherLaunch& a, uint32_t elems, int variant,
                                  cudaStream_t stream) {
+    if (a.part_scale) return launch_kv_gather_e4m3(a, elems, stream);
     if (a.records.latent) return launch_kv_gather_fp8_records(a, elems, stream);
     if (a.n == 0) return cudaSuccess;
     if (!a.part_base) return cudaErrorInvalidValue;

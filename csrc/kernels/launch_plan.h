@@ -478,4 +478,28 @@ inline LaunchPlan plan_gather_fp8_records(const GatherLaunch& a, uint32_t elems,
     return p;
 }
 
+// ---------------------------------------------------------------- e4m3 caches
+// Reads (plain or layered) and writes of e4m3 parts (GatherLaunch::part_scale,
+// kv_fp8_cache.cu): always the ld/st kernels.  A work item is a run of kLdStChunk payload bytes
+// of one part (256 groups), or the whole part under ldst_items' rule; cpb is runs per part, and
+// a layered read numbers items with layered_item as whole parts do.  Refused: row geometry,
+// pieces, records, a part of 0 or not a multiple of 512 elements, part bases or local offsets
+// (align_or) that are not 16-byte aligned, 0 or more than kGatherMaxParts parts, groups
+// groups_ok refuses and more than kMaxItems work items.  The grid is one wave of the CTAs the
+// kernel keeps resident (res.r16).
+inline LaunchPlan plan_gather_e4m3(const GatherLaunch& a, uint32_t elems, int sms,
+                                   LdStResident res) {
+    const uint64_t parts = uint64_t(a.n) * a.nparts;
+    if (a.rows.rows != 0 || a.rows.pieces != 1 || a.records.latent != 0 || elems == 0 ||
+        elems % 512 != 0 || (a.align_or & 15) != 0 || a.nparts == 0 ||
+        a.nparts > kGatherMaxParts || !groups_ok(a) || parts > kMaxItems)
+        return invalid_plan();
+    LaunchPlan p;
+    p.kernel = Kernel::kLdStFp8;
+    ldst_items(p, parts, elems, kLdStChunk, 1u << 20, sms);
+    if (parts * p.cpb > kMaxItems) return invalid_plan();
+    p.ctas = clamp_grid(a.max_ctas > 0 ? a.max_ctas : res.r16 * sms, parts * p.cpb);
+    return p;
+}
+
 }  // namespace istore::kernels

@@ -211,15 +211,22 @@ kernels::Fp8Records parse_records(const std::vector<uint32_t>& v) {
 // A gathered call's parts: part s at part_base[s] (which must outlive the spec); elems > 0:
 // bf16 parts of elems elements stored as fp8 pages, or with records (parse_records) as token
 // records.  rows: a row-sliced read's or write's geometry (parse_rows); empty: whole parts.
-// The connection checks the values.
+// scales: one per part for e4m3 parts (GatherSpec::part_scale), or empty.  scales and
+// part_base must outlive the spec.  The connection checks the values.
 Connection::GatherSpec gather_spec(const std::vector<uint64_t>& part_base, uint32_t part_bytes,
                                    uint32_t elems, uint32_t first_part,
                                    const std::vector<uint32_t>& rows = {},
                                    const std::vector<uint64_t>* piece_off = nullptr,
                                    uint32_t pieces = 1,
-                                   const std::vector<uint32_t>& records = {}) {
+                                   const std::vector<uint32_t>& records = {},
+                                   const std::vector<float>& scales = {}) {
     Connection::GatherSpec g;
     g.records = parse_records(records);
+    if (!scales.empty()) {
+        if (scales.size() != part_base.size())
+            throw py::value_error("scales holds one scale per part");
+        g.part_scale = scales.data();
+    }
     if (pieces > 1) g.piece_off = piece_off->data();
     g.part_base = part_base.data();
     g.nparts = uint32_t(part_base.size());
@@ -645,7 +652,8 @@ PYBIND11_MODULE(_infinistore, m) {
             [](Connection& c, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
                uint32_t elems, const py::object& offsets, const py::object& remote_blocks,
                int device, uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows,
-               const py::object& piece_off, uint32_t pieces, const std::vector<uint32_t>& records) {
+               const py::object& piece_off, uint32_t pieces, const std::vector<uint32_t>& records,
+               const std::vector<float>& scales) {
                 BlockSpan rb;
                 OffsetSpan off;
                 blocks_from_py(remote_blocks, rb);
@@ -654,7 +662,8 @@ PYBIND11_MODULE(_infinistore, m) {
                 for (size_t i = 0; i < off.n; ++i) bytes[i] = off.data[i] * scale;
                 const std::vector<uint64_t> table = piece_table(piece_off, off.n, pieces, scale);
                 const Connection::GatherSpec g =
-                    gather_spec(part_base, part_bytes, elems, 0, rows, &table, pieces, records);
+                    gather_spec(part_base, part_bytes, elems, 0, rows, &table, pieces, records,
+                                scales);
                 py::gil_scoped_release rel;
                 return c.w_rdma_gather(g, bytes.data(), bytes.size(), rb.data, rb.n, device, stream);
             },
@@ -662,7 +671,7 @@ PYBIND11_MODULE(_infinistore, m) {
             py::arg("remote_blocks"), py::arg("device") = -1, py::arg("stream") = 0,
             py::arg("scale") = 1, py::arg("rows") = std::vector<uint32_t>{},
             py::arg("piece_off") = py::none(), py::arg("pieces") = 1,
-            py::arg("records") = std::vector<uint32_t>{},
+            py::arg("records") = std::vector<uint32_t>{}, py::arg("scales") = std::vector<float>{},
             "gathered write: block i = part s at part_base[s] + offsets[i] * scale, s = 0..S-1; "
             "elems > 0: bf16 parts of elems elements, quantised into fp8 page s of block i, or "
             "with records = (latent, rope) into elems / (latent + rope) fp8 token records "
@@ -672,19 +681,22 @@ PYBIND11_MODULE(_infinistore, m) {
             "each stored part: slice j of stored row r from part_base[s] + offset + r * "
             "dst_pitch + j * dst_slice_pitch; pieces > 1 (with rows): piece_off holds pieces "
             "offsets per block (times scale), and run t of rows / pieces rows comes from "
-            "part_base[s] + offset + piece_off[i * pieces + t]")
+            "part_base[s] + offset + piece_off[i * pieces + t]; scales (one per part, elems > "
+            "0, whole parts): the parts are elems bytes of e4m3 of those scales, stored verbatim "
+            "as fp8 pages whose group scales are the part's")
         .def(
             "r_rdma_scatter",
             [](Connection& c, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
                uint32_t elems, uint32_t first_part, const py::object& blocks, int device,
                uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows,
                Connection::ScatterReader* reader, uint32_t group_parts, const py::object& piece_off,
-               uint32_t pieces, const std::vector<uint32_t>& records) {
+               uint32_t pieces, const std::vector<uint32_t>& records,
+               const std::vector<float>& scales) {
                 std::vector<KeyOffset> kb;
                 blocks_list_from_py(blocks, scale, kb);
                 const std::vector<uint64_t> table = piece_table(piece_off, kb.size(), pieces, scale);
                 Connection::GatherSpec g = gather_spec(part_base, part_bytes, elems, first_part,
-                                                       rows, &table, pieces, records);
+                                                       rows, &table, pieces, records, scales);
                 g.reader = reader;
                 g.group_parts = group_parts;
                 py::gil_scoped_release rel;
@@ -695,7 +707,7 @@ PYBIND11_MODULE(_infinistore, m) {
             py::arg("scale") = 1, py::arg("rows") = std::vector<uint32_t>{},
             py::arg("reader") = py::none(), py::arg("group_parts") = 0,
             py::arg("piece_off") = py::none(), py::arg("pieces") = 1,
-            py::arg("records") = std::vector<uint32_t>{},
+            py::arg("records") = std::vector<uint32_t>{}, py::arg("scales") = std::vector<float>{},
             "scattered read: stored part first_part + s of each block -> part_base[s] + offset; "
             "elems > 0: fp8 pages (or with records, token records) dequantised into bf16 parts "
             "of elems elements; rows = (rows, "
@@ -703,7 +715,8 @@ PYBIND11_MODULE(_infinistore, m) {
             "rows of each part, slice j of row r to part_base[s] + offset + r * dst_pitch + j * "
             "dst_slice_pitch; reader: a layered read whose parts are "
             "released in groups of group_parts (check reader.failed); pieces as for "
-            "w_rdma_gather")
+            "w_rdma_gather; scales (one per part): e4m3 parts, each stored group requantised to "
+            "its part's scale (verbatim when the scales are equal)")
         .def(
             "wait_layered",
             [](Connection& c, const Connection::ScatterReader& r, uint32_t group, uint64_t stream) {
@@ -746,19 +759,19 @@ PYBIND11_MODULE(_infinistore, m) {
             [](Connection& c, Connection::GatherWriter& w, const std::vector<uint64_t>& part_base,
                uint32_t part_bytes, uint32_t elems, uint32_t first_part, int device,
                uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows,
-               const std::vector<uint32_t>& records) {
-                const Connection::GatherSpec g = gather_spec(part_base, part_bytes, elems,
-                                                             first_part, rows, nullptr, 1, records);
+               const std::vector<uint32_t>& records, const std::vector<float>& scales) {
+                const Connection::GatherSpec g = gather_spec(
+                    part_base, part_bytes, elems, first_part, rows, nullptr, 1, records, scales);
                 py::gil_scoped_release rel;
                 return c.write_layered(w, g, scale, device, stream);
             },
             py::arg("writer"), py::arg("part_base"), py::arg("part_bytes"), py::arg("elems"),
             py::arg("first_part"), py::arg("device") = -1, py::arg("stream") = 0,
             py::arg("scale") = 1, py::arg("rows") = std::vector<uint32_t>{},
-            py::arg("records") = std::vector<uint32_t>{},
+            py::arg("records") = std::vector<uint32_t>{}, py::arg("scales") = std::vector<float>{},
             "layered write: stored part first_part + s of every block of the writer <- "
-            "part_base[s] + offset * scale; elems > 0: fp8 parts of elems bf16 elements; rows "
-            "and records as for w_rdma_gather")
+            "part_base[s] + offset * scale; elems > 0: fp8 parts of elems bf16 elements; rows, "
+            "records and scales as for w_rdma_gather (every call with scales or none)")
         .def(
             "rw_local",
             [](Connection& c, const std::string& op, const py::object& blocks, int block_size,
@@ -1120,9 +1133,11 @@ PYBIND11_MODULE(_infinistore, m) {
            uint64_t align_or, uint64_t layer_state, uint32_t layer_parts, bool layer_claim,
            uint64_t group_flags, uint64_t group_counters, uint32_t group_seq,
            uint32_t group_parts, const std::vector<uint32_t>& rows, uint64_t piece_off,
-           uint32_t pieces, const std::vector<uint32_t>& records) {
+           uint32_t pieces, const std::vector<uint32_t>& records, const std::vector<float>& scales) {
             if (part_base.empty() || part_base.size() > kernels::kGatherMaxParts)
                 throw std::runtime_error("kv_gather_fp8: 1 to GATHER_MAX_PARTS parts");
+            if (!scales.empty() && scales.size() != part_base.size())
+                throw std::runtime_error("kv_gather_fp8: one scale per part");
             if (layer_state && first_part + part_base.size() > layer_parts)
                 throw std::runtime_error("kv_gather_fp8: first_part + parts > layer_parts");
             if (group_flags && (write || !group_counters || !group_parts ||
@@ -1155,6 +1170,7 @@ PYBIND11_MODULE(_infinistore, m) {
             if (!rows.empty()) G.part_bytes = 2 * elems;  // bytes of the parts' bf16 view
             G.piece_off = as_ptr<const uint64_t>(piece_off);
             G.records = parse_records(records);
+            G.part_scale = scales.empty() ? nullptr : scales.data();
             const cudaError_t e =
                 kernels::launch_kv_gather_fp8(G, elems, variant, as_ptr<CUstream_st>(stream));
             if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
@@ -1167,7 +1183,7 @@ PYBIND11_MODULE(_infinistore, m) {
         py::arg("layer_claim") = false, py::arg("group_flags") = 0, py::arg("group_counters") = 0,
         py::arg("group_seq") = 0, py::arg("group_parts") = 0,
         py::arg("rows") = std::vector<uint32_t>{}, py::arg("piece_off") = 0, py::arg("pieces") = 1,
-        py::arg("records") = std::vector<uint32_t>{},
+        py::arg("records") = std::vector<uint32_t>{}, py::arg("scales") = std::vector<float>{},
         "gathered fp8 blocks: descs as for kv_gather; records = (latent, rope): every part is "
         "elems / (latent + rope) bf16 tokens stored as fp8 token records (kv_write_fp8_records, "
         "kv_read_fp8_records; no rows, any variant; with pieces > 1 and piece_off, run t of "
@@ -1178,7 +1194,10 @@ PYBIND11_MODULE(_infinistore, m) {
         "group_* as for kv_gather (a layered read always runs the ld/st kernel); rows as for "
         "kv_gather, in bytes of the parts' bf16 view: a read dequantises those rows of each "
         "fp8 page (kv_read_fp8_rows), a write quantises stored pages whose rows it loads from "
-        "the strided parts (kv_write_fp8_rows)");
+        "the strided parts (kv_write_fp8_rows); scales (one per part): every part is elems "
+        "bytes of e4m3 of that scale (kv_write_e4m3_gather, kv_read_e4m3_scatter; whole parts, "
+        "any variant): a write keeps the bytes with every group scale the part's, a read "
+        "requantises each stored group to it");
     k.def(
         "stream_wait_value",
         [](uint64_t addr, uint32_t value, uint64_t stream) {
@@ -1962,6 +1981,28 @@ PYBIND11_MODULE(_infinistore, m) {
           py::arg("align_or") = 0, py::arg("group_parts") = 0, py::arg("write") = false,
           py::arg("max_ctas") = 0, py::arg("sm_count") = 132, py::arg("resident") = 1,
           py::arg("rows") = 0, py::arg("pieces") = 1);
+    t.def("plan_gather_e4m3",
+          [plan_dict](uint32_t n, uint32_t nparts, uint32_t elems, uint64_t align_or,
+                      uint32_t group_parts, bool write, int max_ctas, int sm_count, int resident,
+                      uint32_t rows, uint32_t pieces, bool records) {
+              static uint32_t flags[1];
+              kernels::GatherLaunch a;
+              a.n = n;
+              a.nparts = nparts;
+              a.write = write;
+              a.align_or = align_or;
+              a.group_flags = group_parts ? flags : nullptr;
+              a.group_parts = group_parts;
+              a.max_ctas = max_ctas;
+              a.rows.rows = rows;  // any row geometry is refused
+              a.rows.pieces = pieces;
+              if (records) a.records = kernels::Fp8Records{512, 64};  // records are refused
+              return plan_dict(kernels::plan_gather_e4m3(a, elems, sm_count, {resident, resident}));
+          },
+          py::arg("n"), py::arg("nparts"), py::arg("elems"), py::arg("align_or") = 0,
+          py::arg("group_parts") = 0, py::arg("write") = false, py::arg("max_ctas") = 0,
+          py::arg("sm_count") = 132, py::arg("resident") = 1, py::arg("rows") = 0,
+          py::arg("pieces") = 1, py::arg("records") = false);
     t.def("fp8_rows_read_bytes", &fp8_rows_read_bytes, py::arg("rows"), py::arg("row_bytes"),
           py::arg("src_pitch"), py::arg("src_col") = 0,
           "bytes_read of a row-sliced read of one stored fp8 part (geometry in bf16 bytes)");

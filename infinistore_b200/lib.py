@@ -489,6 +489,38 @@ def _check_records(records: "FP8Records | None", part_size: int, fp8: bool = Tru
     records.check(part_size)
 
 
+def _check_scales(scales, nparts: int, fp8: bool, rows: "PartRows | None" = None,
+                  records: "FP8Records | None" = None) -> Optional[np.ndarray]:
+    """The checks of every ``scales=`` (None: no scales): one scale per part (a sequence, an
+    ndarray or a CPU tensor), of an fp8 call of whole parts (no ``rows``, ``records`` or pieces),
+    each finite, positive and normal as a float32 (``2^-126 <= s <= FLT_MAX``).  Returns the
+    scales as a 1-D float32 array."""
+    if scales is None:
+        return None
+    if not fp8:
+        raise ValueError("scales= makes the parts e4m3 caches stored as fp8 pages: it needs an "
+                         "fp8 call")
+    if rows is not None or records is not None:
+        raise ValueError("scales= takes whole parts: it cannot be combined with rows= or "
+                         "records=")
+    if isinstance(scales, torch.Tensor):
+        if scales.device.type != "cpu":
+            raise ValueError(f"scales must be on the CPU, not {scales.device}")
+        scales = scales.detach().to(torch.float32).numpy()
+    with np.errstate(over="ignore"):
+        out = np.array(scales, dtype=np.float32)
+    if out.ndim != 1 or len(out) != int(nparts):
+        raise ValueError(f"scales holds one scale per part: {int(nparts)}, not "
+                         f"{out.size if out.ndim else 1}")
+    ok = np.isfinite(out) & (out >= np.float32(2.0 ** -126))
+    if not ok.all():
+        bad = float(out[~ok][0])
+        raise ValueError(f"scale {bad} of an e4m3 part is not finite, positive and normal "
+                         f"(2^-126 <= s <= FLT_MAX as a float32)")
+    out.setflags(write=False)
+    return out
+
+
 def _block_offsets(offsets, nblocks: Optional[int] = None) -> np.ndarray:
     """The local offsets (elements) of gathered blocks as int64: 1-D, or ``(n, k)`` with one
     column per piece of a block, where ``(n, 1)`` is 1-D.  ValueError for another shape, for
@@ -519,6 +551,7 @@ class _Gather(NamedTuple):
     rows: list  # native row geometry (PartRows.native), or []
     records: list  # native fp8 records (FP8Records.native), or []
     pieces: dict  # piece arguments (_piece_args), or {}
+    scales: list  # one float32 scale per e4m3 part (_check_scales), or []
 
 
 def _raise_if_fp8_pages_unaligned(cache: torch.Tensor, offsets) -> None:
@@ -816,7 +849,7 @@ class InfinityConnection:
     def _gather_parts(self, parts, offsets, part_size: int, first_part: int = 0,
                       block_parts=None, fp8: bool = False, rows: "PartRows | None" = None, *,
                       nblocks=None, stream="current", write: bool = False,
-                      records: "FP8Records | None" = None):
+                      records: "FP8Records | None" = None, scales=None):
         """Checks a gathered call before anything is enqueued: parts ``first_part ..
         first_part + len(parts) - 1`` of the blocks at ``offsets`` (elements, a list or an int64
         ndarray; ``nblocks`` of them when given), in a parts list ``[(tensor, base), ...]``, of
@@ -831,12 +864,16 @@ class InfinityConnection:
         parts are stored as token records, ``part_size`` a whole number of tokens, no ``rows``;
         its 2-D offsets need no ``rows``: piece i of every part of block b, tokens ``i * T / k
         .. (i + 1) * T / k - 1`` of the part's ``T`` tokens, is at ``offsets[b, i]``.
-        Returns the native call's arguments (``_Gather``): with pieces its offsets are zeros
+        ``scales`` (with ``fp8``, one per part, ``_check_scales``): the parts are
+        ``float8_e4m3fn`` CUDA tensors of those scales (e4m3 caches), whole parts only: no
+        ``rows``, ``records`` or 2-D offsets.  Returns the native call's arguments (``_Gather``): with pieces its offsets are zeros
         and its piece arguments carry the ``(n, k)`` offsets."""
         if self._mode != "rdma":
             raise Exception("gathered blocks need a connected rdma connection")
         _check_records(records, part_size, fp8, rows)
         offs = _block_offsets(offsets, nblocks)
+        if scales is not None and offs.ndim == 2:
+            raise ValueError("scales= takes whole parts: no pieces (2-D offsets)")
         table = None
         if offs.ndim == 2:
             if records is not None:  # pieces of whole tokens
@@ -871,6 +908,7 @@ class InfinityConnection:
             if not (isinstance(part, (tuple, list)) and len(part) == 2
                     and isinstance(part[0], torch.Tensor)):
                 raise ValueError(f"part {i} is not a (tensor, base) pair")
+        scales = _check_scales(scales, len(parts), fp8, rows, records)
         part_size = int(part_size)
         if part_size <= 0:
             raise ValueError("part_size must be positive")
@@ -898,7 +936,10 @@ class InfinityConnection:
                                  f"{extent} runs past the tensor's {t.numel()} elements")
             bases.append(t.data_ptr() + base * es)
         if fp8:
-            if first.dtype != torch.bfloat16:
+            if scales is not None and first.dtype != torch.float8_e4m3fn:
+                raise ValueError(f"e4m3 parts (scales=) take float8_e4m3fn tensors, not "
+                                 f"{first.dtype}")
+            if scales is None and first.dtype != torch.bfloat16:
                 raise ValueError(f"fp8 gathered blocks take bf16 tensors, not {first.dtype}")
             if records is None and part_size % 512:
                 raise ValueError(f"fp8 gathered blocks need a part_size that is a multiple of "
@@ -924,27 +965,29 @@ class InfinityConnection:
                              "(--pool-backend host)")
         return _Gather(bases, dev, es, offs, _stream_of(first, stream), part_size * es,
                        part_size if fp8 else 0, rows.native(es) if rows is not None else [],
-                       records.native() if records is not None else [], _piece_args(table))
+                       records.native() if records is not None else [], _piece_args(table),
+                       scales.tolist() if scales is not None else [])
 
     def _gather_write(self, parts, offsets, part_size: int, stream, rows: "PartRows | None",
                       fp8: bool, records: "FP8Records | None", remote_blocks=None,
-                      writer: "GatherWriter | None" = None, first_part: int = 0) -> None:
-        """The gathered write, bf16 or fp8: into ``remote_blocks`` in one call
-        (``rdma_write_cache_gather[_fp8]``), or parts from ``first_part`` of the blocks of a
-        layered ``writer`` (``GatherWriter.write``)."""
+                      writer: "GatherWriter | None" = None, first_part: int = 0,
+                      scales=None) -> None:
+        """The gathered write, bf16 or fp8 (with ``scales``, of e4m3 parts): into
+        ``remote_blocks`` in one call (``rdma_write_cache_gather[_fp8]``), or parts from
+        ``first_part`` of the blocks of a layered ``writer`` (``GatherWriter.write``)."""
         one_call = writer is None
         g = self._gather_parts(parts, offsets, part_size, first_part,
                                None if one_call else writer.nparts, fp8, rows,
                                nblocks=len(remote_blocks) if one_call else None, stream=stream,
-                               write=True, records=records)
+                               write=True, records=records, scales=scales)
         if not one_call:
             writer._claim(parts[0][0])
             ret = self.conn.w_rdma_layered(writer._w, g.bases, g.part_bytes, g.elems, first_part,
-                                           g.dev, g.stream, g.es, g.rows, g.records)
+                                           g.dev, g.stream, g.es, g.rows, g.records, g.scales)
         elif len(g.offsets):
             ret = self.conn.w_rdma_gather(g.bases, g.part_bytes, g.elems, g.offsets, remote_blocks,
                                           g.dev, g.stream, g.es, g.rows, **g.pieces,
-                                          records=g.records)
+                                          records=g.records, scales=g.scales)
         else:
             return
         if ret < 0:
@@ -952,17 +995,19 @@ class InfinityConnection:
 
     def _scatter_read(self, parts, blocks, part_size: int, first_part: int, stream,
                       rows: "PartRows | None", fp8: bool, records: "FP8Records | None",
-                      group_parts: Optional[int] = None) -> "ScatterRead | None":
-        """The scattered read, bf16 or fp8: ``read_cache_scatter[_fp8]``, or with
-        ``group_parts`` the layered ``read_cache_scatter_layered``, which returns its reader."""
+                      group_parts: Optional[int] = None, scales=None) -> "ScatterRead | None":
+        """The scattered read, bf16 or fp8 (with ``scales``, into e4m3 parts):
+        ``read_cache_scatter[_fp8]``, or with ``group_parts`` the layered
+        ``read_cache_scatter_layered``, which returns its reader."""
         keys, offs = _split_blocks(blocks)
         g = self._gather_parts(parts, offs, part_size, first_part, fp8=fp8, rows=rows,
-                               nblocks=len(keys), stream=stream, records=records)
+                               nblocks=len(keys), stream=stream, records=records, scales=scales)
         args = (g.bases, g.part_bytes, g.elems, int(first_part), (keys, g.offsets), g.dev,
                 g.stream, g.es, g.rows)
         if group_parts is None:
             if len(g.offsets):
-                ret = self.conn.r_rdma_scatter(*args, **g.pieces, records=g.records)
+                ret = self.conn.r_rdma_scatter(*args, **g.pieces, records=g.records,
+                                               scales=g.scales)
                 if ret < 0:
                     raise Exception(f"Failed to read to infinistore, ret = {ret}: "
                                     f"{self.conn.last_error()}")
@@ -975,7 +1020,8 @@ class InfinityConnection:
         if group_parts < 1 or len(g.bases) % group_parts:
             raise ValueError(f"group_parts {group_parts} does not divide the {len(g.bases)} parts")
         native = _infinistore.ScatterReader()
-        self.conn.r_rdma_scatter(*args, native, group_parts, **g.pieces, records=g.records)
+        self.conn.r_rdma_scatter(*args, native, group_parts, **g.pieces, records=g.records,
+                                 scales=g.scales)
         read = ScatterRead(self, native, parts[0][0].device)
         if native.failed:
             err = Exception(f"Failed to read to infinistore: {self.conn.last_error()}")
@@ -1054,7 +1100,7 @@ class InfinityConnection:
 
     def rdma_write_cache_gather_fp8(self, parts, offsets, part_size: int, remote_blocks,
                                     stream="current", rows: "PartRows | None" = None,
-                                    records: "FP8Records | None" = None):
+                                    records: "FP8Records | None" = None, scales=None):
         """``rdma_write_cache_gather`` with every part quantised to e4m3 (one fp32 scale per
         128 elements) inside the write kernel: part ``s`` of a block is the fp8 page that
         ``rdma_write_cache_fp8`` would store for it, at byte
@@ -1073,13 +1119,23 @@ class InfinityConnection:
         dividing ``part_size // records.token_dim``): tokens ``i * T / k .. (i + 1) * T / k -
         1`` of every part of block b, of its ``T`` tokens, are taken from ``offsets[b, i]`` -
         e.g. a chunk of k MLA engine pages stored as the records of one page of k times the
-        tokens."""
-        self._gather_write(parts, offsets, part_size, stream, rows, True, records, remote_blocks)
+        tokens.
+
+        ``scales`` (one float32 scale per part: a sequence, an ndarray or a CPU tensor) writes
+        an engine's e4m3 KV cache: the parts are ``float8_e4m3fn`` CUDA tensors (offsets and
+        ``part_size`` in elements, which are bytes; part bases and offsets 16-byte aligned),
+        value ``e4m3(q) * scales[s]``.  Part ``s`` is stored as the same fp8 page, its e4m3
+        bytes kept verbatim (NaN codes included) and every group scale ``scales[s]``: nothing
+        is lost, and every fp8 reader reads it.  Whole parts only (no ``rows``, ``records`` or
+        2-D offsets); each scale must be finite, positive and normal, or ``ValueError`` is
+        raised before anything is enqueued."""
+        self._gather_write(parts, offsets, part_size, stream, rows, True, records, remote_blocks,
+                           scales=scales)
         return 0
 
     def read_cache_scatter_fp8(self, parts, blocks, part_size: int, first_part: int = 0,
                                stream="current", rows: "PartRows | None" = None,
-                               records: "FP8Records | None" = None):
+                               records: "FP8Records | None" = None, scales=None):
         """Read blocks written by ``rdma_write_cache_gather_fp8``: fp8 page ``first_part + s``
         of every block is dequantised into part ``s`` (``blocks``, misses and ``first_part`` as
         for ``read_cache_scatter``).  With ``device_lookup`` a stored block shorter than
@@ -1098,14 +1154,23 @@ class InfinityConnection:
         ``fp8_gather_block_bytes(first_part + len(parts), part_size, records=records)`` is a
         miss.  No ``rows``; ``(keys, offsets)`` may carry an ``(n, k)`` int64 array (pieces of
         whole tokens, as for ``rdma_write_cache_gather_fp8``): run i of every part's tokens of
-        block b lands at ``offsets[b, i]``."""
-        self._scatter_read(parts, blocks, part_size, first_part, stream, rows, True, records)
+        block b lands at ``offsets[b, i]``.
+
+        ``scales`` (as for ``rdma_write_cache_gather_fp8``): the parts are e4m3 caches of those
+        scales, and each stored 128-element group (bytes ``q``, scale ``s_g``) is requantised
+        to its part's scale ``s_c`` inside the read: its bytes are copied when ``s_g`` and
+        ``s_c`` are the same float, else ``q' = e4m3_satfinite_rne(rn32(e4m3(q) * min(rn32(s_g
+        / s_c), FLT_MAX)))`` - NaN codes become 0x7F, zeros keep their sign, finite values
+        beyond +-448 saturate.  Pages written by a bf16 cache with ``fp8`` read this way too."""
+        self._scatter_read(parts, blocks, part_size, first_part, stream, rows, True, records,
+                           scales=scales)
 
     # ------------------------------------------------------------------ layered scattered reads
     def read_cache_scatter_layered(self, parts, blocks, part_size: int, group_parts: int = 2,
                                    first_part: int = 0, fp8: bool = False,
                                    stream="current", rows: "PartRows | None" = None,
-                                   records: "FP8Records | None" = None) -> "ScatterRead":
+                                   records: "FP8Records | None" = None,
+                                   scales=None) -> "ScatterRead":
         """``read_cache_scatter`` (``read_cache_scatter_fp8`` with ``fp8``) in one call whose
         parts are released to consumers group by group: group ``g`` is parts
         ``g * group_parts .. g * group_parts + group_parts - 1`` of every block (with the
@@ -1120,9 +1185,10 @@ class InfinityConnection:
         failed, as for any read.  A missing key on a connection without ``device_lookup``
         raises here; the exception's ``read`` attribute is the failed reader.  ``rows`` as for
         ``read_cache_scatter[_fp8]``, ``records`` (with ``fp8``, and its pieces of whole
-        tokens without ``rows``) as for ``read_cache_scatter_fp8``."""
+        tokens without ``rows``) and ``scales`` (with ``fp8``) as for
+        ``read_cache_scatter_fp8``."""
         return self._scatter_read(parts, blocks, part_size, first_part, stream, rows, fp8, records,
-                                  group_parts)
+                                  group_parts, scales=scales)
 
     # ------------------------------------------------------------------ layered gathered writes
     def gather_writer(self, remote_blocks, offsets, nparts: int, part_size: int,
@@ -1409,7 +1475,7 @@ class GatherWriter:
         return self._w.failed
 
     def write(self, parts, first_part: int, stream="current",
-              rows: "PartRows | None" = None) -> None:
+              rows: "PartRows | None" = None, scales=None) -> None:
         """Store parts ``first_part .. first_part + len(parts) - 1`` of every block: stored
         part ``first_part + s`` of block i is ``parts[s][0].view(-1)[parts[s][1] + offsets[i]
         : ... + part_size]``.  ``parts`` is ``[(tensor, base), ...]`` as for
@@ -1419,7 +1485,9 @@ class GatherWriter:
         everything ``rdma_write_cache_gather`` (``_gather_fp8``) refuses.  ``rows`` as for
         ``rdma_write_cache_gather``; one call may take rows and another not, and every call
         stores whole parts.  A writer made with ``records`` and 2-D offsets (pieces of whole
-        tokens) takes no ``rows``."""
+        tokens) takes no ``rows``.  ``scales`` (an fp8 writer's, one per part of this call, as
+        for ``rdma_write_cache_gather_fp8``): the parts are e4m3 caches; every call of a writer
+        passes scales, or none does."""
         if self._w.failed or self._w.complete:
             raise ValueError("the writer is complete or has failed")
         parts = list(parts)
@@ -1433,7 +1501,7 @@ class GatherWriter:
         if self._offs.ndim == 2 and rows is None and self.records is None:
             raise ValueError("a writer made with 2-D offsets (pieces) needs rows= on every call")
         self._conn._gather_write(parts, self._offs, self.part_size, stream, rows, self.fp8,
-                                 self.records, writer=self, first_part=first_part)
+                                 self.records, writer=self, first_part=first_part, scales=scales)
 
     def _claim(self, first: torch.Tensor) -> None:
         """The first call fixes the device and dtype; ValueError for another one later."""

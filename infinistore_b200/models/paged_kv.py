@@ -6,7 +6,7 @@ from typing import List, NamedTuple, Optional, Sequence
 import numpy as np
 import torch
 
-from ..lib import _GATHER_MAX_BLOCK_BYTES, FP8Records, PartRows
+from ..lib import _GATHER_MAX_BLOCK_BYTES, FP8Records, PartRows, _check_scales
 from .kv_layout import (ALL_LAYERS, KVLayout, MLALayout, chunk_key, mla_chunk_key, mla_page_key,
                         page_key, tp_sources)
 
@@ -24,6 +24,28 @@ def layer_keys(layout: KVLayout, tp_rank: int, layer: int, kv: int,
     """Store keys of one layer's K (kv = 0) or V (kv = 1) pages."""
     kind = "K" if kv == 0 else "V"
     return [page_key(layout.name, layer, kind, tp_rank, h) for h in page_hashes]
+
+
+def _e4m3_scales(layout: KVLayout, device, kv_scales) -> np.ndarray:
+    """The checked ``kv_scales`` of an e4m3 cache: a read-only float32 ``(layers, 2)`` host copy
+    of ``[k_scale, v_scale]`` per layer.  ValueError, before anything is allocated, unless the
+    layout is ``float8_e4m3fn`` on a CUDA device and every scale is finite, positive and
+    normal."""
+    if layout.dtype != torch.float8_e4m3fn:
+        raise ValueError(f"kv_scales makes an e4m3 cache: the layout's dtype must be "
+                         f"torch.float8_e4m3fn, not {layout.dtype}")
+    if torch.device(device).type != "cuda":
+        raise ValueError(f"an e4m3 cache (kv_scales=) lives on a CUDA device, not {device}")
+    if isinstance(kv_scales, torch.Tensor):
+        kv_scales = kv_scales.detach().to("cpu", torch.float32).numpy()
+    with np.errstate(over="ignore"):
+        out = np.array(kv_scales, dtype=np.float32)
+    if out.shape != (layout.layers, 2):
+        raise ValueError(f"kv_scales is a ({layout.layers}, 2) array of [k_scale, v_scale] per "
+                         f"layer, not of shape {out.shape}")
+    _check_scales(out.reshape(-1), out.size, True)
+    out.setflags(write=False)
+    return out
 
 
 class _Plan(NamedTuple):
@@ -61,11 +83,13 @@ class _AllLayerPages:
     connection, and the I/O of blocks that hold a page (or chunk) of every layer, each layer's
     parts side by side.  A subclass builds the ``_Plan`` of a call; ``_store``, ``_writer``,
     and ``_read`` (plain or layered) run it in the format ``fp8`` chooses: bf16, fp8 pages, or
-    (with ``records``) fp8 token records."""
+    (with ``records``) fp8 token records.  An e4m3 cache (``kv_scales``) stores its e4m3
+    parts as fp8 pages at the scales of their layers, and takes ``fp8=True`` only."""
 
     _per_layer = 2
     _fp8_pages = "fp8 all-layer pages"  # what the fp8 refusal names
     records: Optional[FP8Records] = None  # how fp8 stores a part; None: as an fp8 page
+    kv_scales: Optional[np.ndarray] = None  # (layers, _per_layer) float32: an e4m3 cache
 
     def __init__(self, layout, num_pages: int, data: torch.Tensor):
         self.layout = layout
@@ -82,6 +106,13 @@ class _AllLayerPages:
         n = self.num_pages * self.layout.page_elems
         return [(self.data, (layer * self._per_layer + i) * n)
                 for layer in layers for i in range(self._per_layer)]
+
+    def _scales(self, layers: range) -> Optional[np.ndarray]:
+        """The scales of the parts of ``layers``, K and V alternating (None: not an e4m3
+        cache)."""
+        if self.kv_scales is None:
+            return None
+        return self.kv_scales[layers.start:layers.stop].reshape(-1)
 
     @staticmethod
     def _chunk_rows(rows: Optional[PartRows], k: int, part: int) -> PartRows:
@@ -113,7 +144,16 @@ class _AllLayerPages:
     def _format(self, plan: _Plan, fp8: bool) -> Optional[FP8Records]:
         """The records of the call's format (None: bf16 or fp8 pages).  ValueError, before
         anything happens, for fp8 unless the cache is bf16 on a CUDA device, its records take
-        the part, and, when heads move row by row, ``head_dim`` is a multiple of 8."""
+        the part, and, when heads move row by row, ``head_dim`` is a multiple of 8.  An e4m3
+        cache takes only fp8 calls of whole pages at its own TP degree (no chunks)."""
+        if self.kv_scales is not None:
+            if not fp8:
+                raise ValueError("an e4m3 cache (kv_scales=) stores its pages as fp8 pages: it "
+                                 "needs fp8=True")
+            if plan.rows is not None or plan.offsets.ndim == 2:
+                raise ValueError("an e4m3 cache (kv_scales=) reads and writes whole pages at its "
+                                 "own TP degree: no source_tp of another degree and no chunks")
+            return None
         if not fp8:
             return None
         if self.data.dtype != torch.bfloat16 or self.data.device.type != "cuda":
@@ -143,8 +183,9 @@ class _AllLayerPages:
 
     def _store(self, conn, plan: _Plan, fp8: bool, stream) -> int:
         blocks, records = self._allocate(conn, plan, fp8)
-        conn._gather_write(self._parts(range(self.layout.layers)), plan.offsets, plan.part,
-                           stream, plan.rows, fp8, records, blocks)
+        layers = range(self.layout.layers)
+        conn._gather_write(self._parts(layers), plan.offsets, plan.part, stream, plan.rows, fp8,
+                           records, blocks, scales=self._scales(layers))
         return len(blocks)
 
     def _writer(self, conn, plan: _Plan, fp8: bool) -> "PageWriter":
@@ -163,7 +204,8 @@ class _AllLayerPages:
         self._ensure_registered(conn)
         read = conn._scatter_read(self._parts(layers), (plan.keys, plan.offsets), plan.part,
                                   self._per_layer * layers.start, stream, plan.rows, fp8,
-                                  records, self._per_layer if layered else None)
+                                  records, self._per_layer if layered else None,
+                                  scales=self._scales(layers))
         return PageRead(read, layers) if layered else len(plan.keys)
 
 
@@ -426,12 +468,27 @@ class PagedKVCache(_PagedCache):
     Layer-wise streaming (docs/source/design.rst:56-63): ``write_layer`` is called right
     after layer l's KV has been produced, on the producing stream; the page mover runs on
     the connection's own streams behind it, so the upload overlaps the next layer's compute.
+
+    ``kv_scales`` (a ``(layers, 2)`` array of ``[k_scale, v_scale]``, with a
+    ``torch.float8_e4m3fn`` layout on a CUDA device) makes an **e4m3 cache**, the cache of an
+    engine that keeps its KV in e4m3 with one scale per layer's K and V (value ``e4m3(q) *
+    scale``).  Its ``write_pages``, ``page_writer(...).write_layers``, ``read_pages`` and
+    ``read_pages_layered`` take ``fp8=True`` and use the all-layer page keys: a write stores
+    every part's e4m3 bytes verbatim as the fp8 page with every group scale its layer's, so a
+    bf16 cache's ``read_pages(fp8=True)`` reads it, and a read requantises each stored group to
+    this cache's scales (``read_cache_scatter_fp8(scales=)``), so pages a bf16 cache wrote with
+    ``fp8=True`` read into it.  ``fp8=False``, ``source_tp`` of another degree and the chunk
+    methods raise ``ValueError`` before anything is allocated.  ``kv_scales`` keeps a read-only
+    float32 host copy of the scales.
     """
 
-    def __init__(self, layout: KVLayout, num_pages: int, device, tp_rank: int = 0):
+    def __init__(self, layout: KVLayout, num_pages: int, device, tp_rank: int = 0,
+                 kv_scales=None):
+        scales = None if kv_scales is None else _e4m3_scales(layout, device, kv_scales)
         super().__init__(layout, num_pages, tp_rank,
                          torch.zeros(layout.layers, 2, num_pages, layout.page_elems,
                                      dtype=layout.dtype, device=device))
+        self.kv_scales = scales
 
     def page(self, layer: int, kv: int, page: int) -> torch.Tensor:
         return self.data[layer, kv, page]
@@ -508,7 +565,7 @@ class PageWriter:
         range) of every page."""
         layers = _layer_range(layers, self.cache.layout.layers)
         self.writer.write(self.cache._parts(layers), self.cache._per_layer * layers.start,
-                          stream=stream, rows=self.rows)
+                          stream=stream, rows=self.rows, scales=self.cache._scales(layers))
 
 
 class PageRead:

@@ -362,7 +362,8 @@ def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, wri
                   claim: bool = False, release: Optional[GroupRelease] = None,
                   rows: Optional[Sequence[int]] = None,
                   pieces: Optional[torch.Tensor] = None,
-                  records: Optional[Sequence[int]] = None) -> None:
+                  records: Optional[Sequence[int]] = None,
+                  scales: Optional[Sequence[float]] = None) -> None:
     """Gathered fp8 blocks (``kv_gather`` with quantisation): part s of block i is a bf16 page
     of ``elems`` elements at ``part_base[s] + local offset`` and fp8 page first_part + s of
     the block, at byte ``fp8_gather_bytes(first_part + s, elems)``.  ``descs``, ``layer`` and
@@ -385,7 +386,12 @@ def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, wri
     s, elems, latent, rope)`` of the block; no ``rows``.  ``records`` with ``pieces`` (k > 1,
     dividing the part's tokens T): tokens ``t * T / k .. (t + 1) * T / k - 1`` of each part of
     block i are at its local offset + ``pieces[i, t]`` (kv_write_fp8_records_pieces,
-    kv_read_fp8_records_pieces), stored where the whole-part write stores them."""
+    kv_read_fp8_records_pieces), stored where the whole-part write stores them.  ``scales``
+    (one float32 per part): every part is ``elems`` bytes of e4m3 (an e4m3 cache) of that
+    scale, whole parts only, whatever the variant.  A write (kv_write_e4m3_gather) stores the
+    bytes verbatim as the fp8 page's payload with every group scale the part's; a read
+    (kv_read_e4m3_scatter) copies a stored group whose scale is the part's and requantises any
+    other to it (docs/kernels.md, "e4m3 cache contract")."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
     bases = [int(b) for b in part_base]
     for b in bases:
@@ -398,7 +404,8 @@ def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, wri
                         status.data_ptr() if status is not None else 0, align_or, *lay,
                         *_release_args(release),
                         [int(r) for r in rows] if rows is not None else [], *_piece_args(pieces),
-                        [int(r) for r in records] if records is not None else [])
+                        [int(r) for r in records] if records is not None else [],
+                        [float(v) for v in scales] if scales is not None else [])
 
 
 def fp8_reference(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
