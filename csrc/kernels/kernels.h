@@ -85,11 +85,16 @@ inline uint32_t index_shard_of(uint64_t h2, uint32_t nshards) {
     return nshards <= 1 ? 0u : uint32_t((h2 >> 20) % nshards);
 }
 
+// kStatMiss counts a block that a read did not find once, however many work items it is cut
+// into.  A read that re-checks its entries after the copy (ReadFusedLaunch::validate,
+// launch_index_validate) also counts every stale work item in both kStatMiss and kStatStale:
+// a whole block, or each chunk of a block split over several CTAs, since the chunks are copied
+// and re-checked independently.
 enum Status : int {
     kStatMiss = 0,         // blocks skipped by a read because the key was not in the index
     kStatPublishFail = 1,  // index insertions that found the table full
     kStatMatch = 2,        // result of the last match_last_index launch (int32)
-    kStatStale = 3,        // blocks whose index entry changed while they were read (evicted)
+    kStatStale = 3,        // work items whose index entry changed while they were read (evicted)
     kStatWords = 8,
 };
 
@@ -338,7 +343,8 @@ struct GatherParts {
 struct ReadFusedLaunch;
 // A scattered read through the device index in ONE launch (kv_pipe.cu): the resolver warp of
 // kv_pipe_read feeding the gather pipeline.  CTA c owns blocks c, c + grid, ...: each key is
-// probed once, by the CTA that moves all of its parts, and re-checked after the copy.  `r`
+// probed once, by the CTA that moves all of its parts, and re-checked after the copy when
+// r.validate is set.  `r`
 // carries keys, dst_off (local byte offsets; dst_base 0), index, segments, status, grid cap
 // and ring geometry; `g` the parts (descs, recs and write are ignored).  Needs 16-byte aligned
 // parts and at least as many blocks as CTAs (fewer: lookup + launch_kv_gather + validate).
@@ -485,16 +491,18 @@ struct ReadFusedLaunch {
     static constexpr int kMaxSegs = 16;
     uint64_t seg_base[kMaxSegs] = {0};
     uint32_t nsegs = 0;
-    uint32_t* status = nullptr;          // status[kStatMiss] counts keys that were not found
+    uint32_t* status = nullptr;          // status[kStatMiss] counts blocks that were not found
     int max_ctas = 0;
-    bool validate = false;               // re-check every entry's tag after its copy (eviction)
+    // re-check every entry's tag after its copy (eviction, purge); needs `status`
+    bool validate = false;
     int variant = kCopyAuto;             // kCopyTma: resolver warp feeding the TMA pipeline
     uint32_t stage_bytes = 0;            // TMA pipeline geometry, 0 = default
     uint32_t ring_bytes = 0;
 };
 // kCopyAuto / kCopyTma run the TMA pipeline (kv_pipe.cu) when the transfer is 16-byte
-// aligned and the blocks are >= kPipeMinBytes; the ld/st kernel otherwise.  Both re-check
-// every entry after its copy.
+// aligned and the blocks are >= kPipeMinBytes; the ld/st kernel otherwise.  With a.validate
+// every fused read (these two, launch_kv_pipe_scatter_read, launch_kv_fp8_read_fused)
+// re-checks each entry after its copy; without it none does.
 cudaError_t launch_kv_read_fused(const ReadFusedLaunch& a, cudaStream_t stream);
 cudaError_t launch_kv_pipe_read(const ReadFusedLaunch& a, cudaStream_t stream);
 // The same for fp8 pages ([elems x e4m3][elems/128 x fp32 scale] in the pool, bf16 at the

@@ -316,8 +316,9 @@ cudaError_t launch_kv_fp8_pipe_gather(const GatherLaunch& a, uint32_t elems, cud
 }
 
 // read_cache_fp8 through the device index in one launch: keys -> (resolver warp) -> pool
-// blocks -> dequantised pages.  Same contract as launch_kv_read_fused (misses and entries that
-// changed under the copy are counted in status[kStatMiss] / [kStatStale]).
+// blocks -> dequantised pages.  Same contract as launch_kv_read_fused (misses, and with
+// a.validate entries that changed under the copy, are counted in status[kStatMiss] /
+// [kStatStale]).
 bool fp8_read_fused_supported(const ReadFusedLaunch& a, uint32_t elems) {
     return elems > 0 && elems % 512 == 0 && (a.align_or & 15) == 0;
 }

@@ -327,8 +327,9 @@ __global__ void __launch_bounds__(kPipeThreads)
 // CTA c owns blocks c, c + grid, ...; the resolver warp resolves them in that order, one probe
 // per key.  Loader and storer walk the CTA's local items k = 0, 1, ...: part (k / cpb) % nparts
 // (sh.cpb chunks per part) of the CTA's block k / (nparts * sh.cpb), so every part of a block
-// is moved by the CTA that resolved it.  The resolver re-checks each entry once the storer has
-// handed its queue half back (every load of those blocks has completed by then).
+// is moved by the CTA that resolved it.  With validate, the resolver re-checks each entry once
+// the storer has handed its queue half back (every load of those blocks has completed by then):
+// a stale block counts once, as a block is one resolver item here.
 __global__ void __launch_bounds__(kPipeThreads)
     kv_pipe_scatter_read_kernel(const __grid_constant__ ResolveArgs a,
                                 const __grid_constant__ GatherParts parts, const Shape sh,

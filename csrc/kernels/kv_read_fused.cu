@@ -87,7 +87,7 @@ __global__ void __launch_bounds__(kThreads)
                 src_of[p][lane] = res.src;
                 if (res.src == 0 && item % cpb == 0 && a.status) atomicAdd(a.status + kStatMiss, 1u);
                 // every chunk of a block is copied at a different time: each item re-checks
-                // the entry after its own copy
+                // the entry after its own copy (a stale block counts once per chunk)
                 if (p) {
                     slot1 = res.slot_plus1;
                     tag1 = res.tag;
@@ -137,7 +137,7 @@ cudaError_t launch_kv_read_fused(const ReadFusedLaunch& a, cudaStream_t stream) 
         ldst_resident(kv_read_fused_kernel<16>, kv_read_fused_kernel<32>, kThreads);
     const LaunchPlan p = plan_read_fused(a, sm_count(), res);
     // default: resolver warp + TMA pipeline (kv_pipe.cu); this file's ld/st kernel serves
-    // small or unaligned pages.  Both re-check every entry after its copy.
+    // small or unaligned pages.  Both re-check every entry after its copy when a.validate.
     if (p.kernel == Kernel::kTma) return launch_kv_pipe_read(a, stream);
     const auto go = [&](auto* kernel) {
         kernel<<<p.ctas, kThreads, 0, stream>>>(a, p.chunk, p.cpb);

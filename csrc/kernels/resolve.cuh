@@ -9,10 +9,12 @@
 // with no server round trip; the reference resolves keys in the server's map and answers with
 // a message (src/infinistore.cpp:424-533).
 //
-// Optimistic read: no lease is taken.  Once the storer has handed a half back - every byte of
-// its blocks has been read from the pool by then - the resolver re-loads the tags it
-// resolved.  A block that was purged or evicted meanwhile (its space may already belong to
-// another key) shows a changed tag and is reported as a miss (kStatMiss + kStatStale).
+// Optimistic read: no lease is taken.  With ReadFusedLaunch::validate (and a status array),
+// once the storer has handed a half back - every byte of its items has been read from the pool
+// by then - the resolver re-loads the tags it resolved.  An item whose block was purged or
+// evicted meanwhile (its space may already belong to another key) shows a changed tag and is
+// reported as a miss (kStatMiss + kStatStale), once per item: a block split into several
+// chunks counts once for each chunk that saw the change.
 #pragma once
 
 #include "../core/hash.h"
@@ -34,6 +36,7 @@ struct ResolveArgs {
     uint64_t seg_base[ReadFusedLaunch::kMaxSegs];
     uint32_t nsegs;
     uint32_t* status;
+    bool validate;  // re-check every resolved entry after its copy
 };
 
 inline ResolveArgs resolve_args(const ReadFusedLaunch& a) {
@@ -50,6 +53,7 @@ inline ResolveArgs resolve_args(const ReadFusedLaunch& a) {
     for (uint32_t s = 0; s < a.nsegs && s < uint32_t(ReadFusedLaunch::kMaxSegs); ++s)
         r.seg_base[s] = a.seg_base[s];
     r.status = a.status;
+    r.validate = a.validate;
     return r;
 }
 
@@ -80,7 +84,7 @@ __device__ __forceinline__ void resolver_warp(const ResolveArgs& a, ResolveQueue
     uint32_t vslot0 = 0, vtag0 = 0, vslot1 = 0, vtag1 = 0;  // scalars: no local memory
     auto recheck = [&](uint32_t p) {
         const uint32_t slot = p ? vslot1 : vslot0, tag = p ? vtag1 : vtag0;
-        if (slot && a.status &&
+        if (slot && a.validate && a.status &&
             !idx::still_valid(idx::table_of_slot(a.table, a.shards, slot), idx::slot_local(slot), tag)) {
             atomicAdd(a.status + kStatMiss, 1u);
             atomicAdd(a.status + kStatStale, 1u);

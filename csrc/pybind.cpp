@@ -432,6 +432,42 @@ T* as_ptr(uint64_t p) {
     return reinterpret_cast<T*>(p);
 }
 
+// Index shards 1, 2, ... of a launch from their native list of (table address, bucket mask);
+// the launch's own table is shard 0.  An empty list leaves the launch unsharded.  Refused
+// before any launch: more than kMaxIndexShards tables in all, a null table, and a mask that is
+// not slots / 8 - 1 of a power-of-two table whose slot ids fit under the shard bits.
+kernels::IndexShards parse_shards(const std::vector<std::pair<uint64_t, uint64_t>>& v) {
+    kernels::IndexShards s;
+    if (v.empty()) return s;
+    if (v.size() + 1 > kernels::kMaxIndexShards)
+        throw py::value_error("shards: at most " + std::to_string(kernels::kMaxIndexShards) +
+                              " index tables in all");
+    constexpr uint64_t kMaxBuckets = (1ull << kernels::kSlotShardShift) / kernels::kIndexWays;
+    for (size_t i = 0; i < v.size(); ++i) {
+        const auto [table, mask] = v[i];
+        if (!table) throw py::value_error("shards: a null index table");
+        if (mask >= kMaxBuckets || ((mask + 1) & mask) != 0)
+            throw py::value_error("shards: a bucket mask is slots / 8 - 1 of a power-of-two "
+                                  "table of at most 2^29 slots");
+        s.table[i] = as_ptr<kernels::IndexBucket>(table);
+        s.mask[i] = mask;
+    }
+    s.n = uint32_t(v.size() + 1);
+    return s;
+}
+
+// Segment bases of a launch that resolves pool addresses, refused past kMaxSegs.
+template <typename Launch>
+void set_segments(Launch& a, const std::vector<uint64_t>& seg_base) {
+    if (seg_base.size() > size_t(Launch::kMaxSegs))
+        throw py::value_error("seg_base: at most " + std::to_string(Launch::kMaxSegs) +
+                              " segment bases");
+    a.nsegs = uint32_t(seg_base.size());
+    for (uint32_t i = 0; i < a.nsegs; ++i) a.seg_base[i] = seg_base[i];
+}
+
+using ShardList = std::vector<std::pair<uint64_t, uint64_t>>;
+
 }  // namespace
 
 PYBIND11_MODULE(_infinistore, m) {
@@ -1025,8 +1061,10 @@ PYBIND11_MODULE(_infinistore, m) {
         [](uint64_t descs, uint32_t n, uint32_t bytes, int variant, int max_ctas, uint64_t stream,
            uint64_t recs, uint64_t table, uint64_t table_mask, uint64_t done, uint64_t status,
            uint64_t align_or, uint64_t trace, bool all_local, uint32_t debug,
-           uint32_t stage_bytes, uint32_t ring_bytes, const std::vector<int64_t>& fan_delta) {
+           uint32_t stage_bytes, uint32_t ring_bytes, const std::vector<int64_t>& fan_delta,
+           const ShardList& shards) {
             kernels::CopyLaunch L;
+            L.shards = parse_shards(shards);
             L.stage_bytes = stage_bytes;
             L.ring_bytes = ring_bytes;
             if (!fan_delta.empty()) {
@@ -1056,7 +1094,10 @@ PYBIND11_MODULE(_infinistore, m) {
         py::arg("table") = 0, py::arg("table_mask") = 0, py::arg("done") = 0,
         py::arg("status") = 0, py::arg("align_or") = 0, py::arg("trace") = 0,
         py::arg("all_local") = false, py::arg("debug") = 0, py::arg("stage_bytes") = 0,
-        py::arg("ring_bytes") = 0, py::arg("fan_delta") = std::vector<int64_t>());
+        py::arg("ring_bytes") = 0, py::arg("fan_delta") = std::vector<int64_t>(),
+        py::arg("shards") = ShardList(),
+        "shards: (table, bucket mask) of index shards 1, 2, ... for the publish; a key is "
+        "published in the table its fingerprint selects (index_shard_of)");
     k.attr("GATHER_MAX_PARTS") = int(kernels::kGatherMaxParts);
     k.def(
         "kv_gather",
@@ -1066,9 +1107,10 @@ PYBIND11_MODULE(_infinistore, m) {
            uint32_t stage_bytes, uint32_t ring_bytes, uint64_t layer_state, uint32_t layer_parts,
            bool layer_claim, uint64_t group_flags, uint64_t group_counters, uint32_t group_seq,
            uint32_t group_parts, const std::vector<uint32_t>& rows, uint64_t piece_off,
-           uint32_t pieces) {
+           uint32_t pieces, const ShardList& shards) {
             if (part_base.empty() || part_base.size() > kernels::kGatherMaxParts)
                 throw std::runtime_error("kv_gather: 1 to GATHER_MAX_PARTS parts");
+            const kernels::IndexShards sh = parse_shards(shards);
             if (layer_state && first_part + part_base.size() > layer_parts)
                 throw std::runtime_error("kv_gather: first_part + parts > layer_parts");
             if (group_flags && (write || !group_counters || !group_parts ||
@@ -1102,6 +1144,7 @@ PYBIND11_MODULE(_infinistore, m) {
             if (!parse_rows(rows, pieces, G.rows))
                 throw std::runtime_error("kv_gather: rows is 5 or 7 values");
             G.piece_off = as_ptr<const uint64_t>(piece_off);
+            G.shards = sh;
             const cudaError_t e = kernels::launch_kv_gather(G, as_ptr<CUstream_st>(stream));
             if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
         },
@@ -1113,7 +1156,7 @@ PYBIND11_MODULE(_infinistore, m) {
         py::arg("layer_state") = 0, py::arg("layer_parts") = 0, py::arg("layer_claim") = false,
         py::arg("group_flags") = 0, py::arg("group_counters") = 0, py::arg("group_seq") = 0,
         py::arg("group_parts") = 0, py::arg("rows") = std::vector<uint32_t>{},
-        py::arg("piece_off") = 0, py::arg("pieces") = 1,
+        py::arg("piece_off") = 0, py::arg("pieces") = 1, py::arg("shards") = ShardList(),
         "gathered blocks: descs[i] = write {local byte offset, block address} / read {block "
         "address or 0, local byte offset}; part s of block i at part_base[s] + local offset is "
         "stored part first_part + s.  layer_state (3 zeroed u32 per block, kept across the "
@@ -1124,7 +1167,7 @@ PYBIND11_MODULE(_infinistore, m) {
         "u32 per group.  rows (5 or 7 values): a row-sliced read, or a write whose rows fill "
         "each stored part.  pieces > 1 (with rows): piece_off is the device address of n * "
         "pieces byte offsets, and run t of block i's rows / pieces rows is at part_base[s] + "
-        "local offset + piece_off[i * pieces + t]");
+        "local offset + piece_off[i * pieces + t].  shards as for kv_copy");
     k.def(
         "kv_gather_fp8",
         [](uint64_t descs, uint32_t n, const std::vector<uint64_t>& part_base, uint32_t elems,
@@ -1262,8 +1305,10 @@ PYBIND11_MODULE(_infinistore, m) {
            uint64_t table_mask, const std::vector<uint64_t>& seg_base, uint64_t out_descs,
            uint64_t dst_off, uint64_t dst_base, uint32_t need_bytes, uint64_t present,
            uint64_t status, uint64_t ticket, bool want_match, uint64_t stream,
-           uint64_t found_at, bool accept_claimed) {
+           uint64_t found_at, bool accept_claimed, const ShardList& shards) {
             kernels::LookupLaunch Q;
+            Q.shards = parse_shards(shards);
+            set_segments(Q, seg_base);
             Q.accept_claimed = accept_claimed;
             Q.found_at = as_ptr<kernels::LookupLaunch::FoundAt>(found_at);
             Q.key_bytes = as_ptr<const uint8_t>(key_bytes);
@@ -1272,8 +1317,6 @@ PYBIND11_MODULE(_infinistore, m) {
             Q.n = n;
             Q.table = as_ptr<const kernels::IndexBucket>(table);
             Q.table_mask = table_mask;
-            Q.nsegs = uint32_t(std::min<size_t>(seg_base.size(), kernels::LookupLaunch::kMaxSegs));
-            for (uint32_t i = 0; i < Q.nsegs; ++i) Q.seg_base[i] = seg_base[i];
             Q.out_descs = as_ptr<kernels::CopyDesc>(out_descs);
             Q.dst_off = as_ptr<const uint64_t>(dst_off);
             Q.dst_base = dst_base;
@@ -1290,11 +1333,15 @@ PYBIND11_MODULE(_infinistore, m) {
         py::arg("out_descs") = 0, py::arg("dst_off") = 0, py::arg("dst_base") = 0,
         py::arg("need_bytes") = 0, py::arg("present") = 0, py::arg("status") = 0,
         py::arg("ticket") = 0, py::arg("want_match") = false, py::arg("stream") = 0,
-        py::arg("found_at") = 0, py::arg("accept_claimed") = false);
+        py::arg("found_at") = 0, py::arg("accept_claimed") = false,
+        py::arg("shards") = ShardList(),
+        "shards as for kv_copy: found_at slot ids carry the shard in their top 3 bits");
     k.def(
         "index_validate",
-        [](uint64_t found_at, uint32_t n, uint64_t table, uint64_t status, uint64_t stream) {
+        [](uint64_t found_at, uint32_t n, uint64_t table, uint64_t status, uint64_t stream,
+           const ShardList& shards) {
             kernels::ValidateLaunch V;
+            V.shards = parse_shards(shards);
             V.found_at = as_ptr<const kernels::LookupLaunch::FoundAt>(found_at);
             V.n = n;
             V.table = as_ptr<const kernels::IndexBucket>(table);
@@ -1303,7 +1350,87 @@ PYBIND11_MODULE(_infinistore, m) {
             if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
         },
         py::arg("found_at"), py::arg("n"), py::arg("table"), py::arg("status"),
-        py::arg("stream") = 0);
+        py::arg("stream") = 0, py::arg("shards") = ShardList(),
+        "shards: the tables index_lookup resolved found_at in (as for kv_copy)");
+    k.def(
+        "read_fused",
+        [](uint64_t key_bytes, uint64_t key_off, uint64_t key_len, uint32_t n, uint64_t table,
+           uint64_t table_mask, const std::vector<uint64_t>& seg_base, uint64_t dst_base,
+           uint64_t dst_off, uint32_t bytes, uint64_t align_or, uint64_t status, int max_ctas,
+           bool validate, int variant, uint32_t stage_bytes, uint32_t ring_bytes, uint64_t stream,
+           const ShardList& shards, uint32_t elems, const std::vector<uint64_t>& part_base,
+           uint32_t part_bytes, uint32_t first_part) {
+            kernels::ReadFusedLaunch R;
+            R.shards = parse_shards(shards);
+            set_segments(R, seg_base);
+            if (validate && !status)
+                throw py::value_error("read_fused: validate counts into a status array");
+            if (elems && !part_base.empty())
+                throw py::value_error("read_fused: fp8 pages or gathered parts, not both");
+            R.key_bytes = as_ptr<const uint8_t>(key_bytes);
+            R.key_off = as_ptr<const uint32_t>(key_off);
+            R.key_len = as_ptr<const uint32_t>(key_len);
+            R.n = n;
+            R.table = as_ptr<const kernels::IndexBucket>(table);
+            R.table_mask = table_mask;
+            R.dst_base = dst_base;
+            R.dst_off = as_ptr<const uint64_t>(dst_off);
+            R.bytes = bytes;
+            R.align_or = align_or;
+            R.status = as_ptr<uint32_t>(status);
+            R.max_ctas = max_ctas;
+            R.validate = validate;
+            R.variant = variant;
+            R.stage_bytes = stage_bytes;
+            R.ring_bytes = ring_bytes;
+            const auto s = as_ptr<CUstream_st>(stream);
+            cudaError_t e;
+            if (!part_base.empty()) {
+                kernels::GatherLaunch G;
+                G.n = n;
+                G.write = false;
+                G.part_base = part_base.data();
+                G.nparts = uint32_t(part_base.size());
+                G.part_bytes = part_bytes;
+                G.first_part = first_part;
+                G.align_or = align_or;
+                for (const uint64_t b : part_base) G.align_or |= b;
+                G.status = R.status;
+                G.max_ctas = max_ctas;
+                if (part_base.size() > kernels::kGatherMaxParts ||
+                    !kernels::scatter_read_fused_supported(R, G) ||
+                    (uint64_t(first_part) + G.nparts) * part_bytes > 0xffffffffull ||
+                    uint64_t(n) * G.nparts > 0x7fffffffull)
+                    throw py::value_error(
+                        "read_fused: gathered parts need 1 to GATHER_MAX_PARTS 16-byte aligned "
+                        "parts of a nonzero multiple of 16 bytes, blocks within 2^32 bytes, and at "
+                        "least as many blocks as CTAs");
+                e = kernels::launch_kv_pipe_scatter_read(R, G, s);
+            } else if (elems) {
+                if (!kernels::fp8_read_fused_supported(R, elems))
+                    throw py::value_error("read_fused: fp8 pages need a multiple of 512 "
+                                          "elements and 16-byte aligned destinations");
+                e = kernels::launch_kv_fp8_read_fused(R, elems, s);
+            } else {
+                e = kernels::launch_kv_read_fused(R, s);
+            }
+            if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
+        },
+        py::arg("key_bytes"), py::arg("key_off"), py::arg("key_len"), py::arg("n"),
+        py::arg("table"), py::arg("table_mask"), py::arg("seg_base"), py::arg("dst_base"),
+        py::arg("dst_off"), py::arg("bytes"), py::arg("align_or") = 0, py::arg("status") = 0,
+        py::arg("max_ctas") = 0, py::arg("validate") = true, py::arg("variant") = 0,
+        py::arg("stage_bytes") = 0, py::arg("ring_bytes") = 0, py::arg("stream") = 0,
+        py::arg("shards") = ShardList(), py::arg("elems") = 0,
+        py::arg("part_base") = std::vector<uint64_t>(), py::arg("part_bytes") = 0,
+        py::arg("first_part") = 0,
+        "read_cache through the device index in one launch: key i (packed as for index_lookup) "
+        "is resolved and its pool page of `bytes` lands at dst_base + dst_off[i] "
+        "(kv_read_fused, or kv_pipe_read by variant and alignment).  elems > 0: fp8 pages "
+        "dequantised to bf16 (kv_fp8_pipe).  part_base: gathered blocks, stored part "
+        "first_part + s of part_bytes landing at part_base[s] + dst_off[i] "
+        "(kv_pipe_scatter_read).  A miss is counted once per block in status[STAT_MISS]; "
+        "validate re-checks every entry after its copy.  shards as for kv_copy");
     k.def(
         "index_erase",
         [](uint64_t recs, uint32_t n, uint64_t table, uint64_t table_mask, uint64_t stream) {

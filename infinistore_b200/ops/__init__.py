@@ -58,7 +58,8 @@ def kv_copy(descs: torch.Tensor, nbytes: int, variant: str = "auto", max_ctas: i
                   publish.mask if publish else 0,
                   publish.done.data_ptr() if publish else 0,
                   status.data_ptr() if status is not None else 0, align_or, 0, all_local, debug,
-                  stage_bytes, ring_bytes, [int(d) for d in fan_deltas] if fan_deltas else [])
+                  stage_bytes, ring_bytes, [int(d) for d in fan_deltas] if fan_deltas else [],
+                  publish.shard_args if publish else [])
 
 
 class LayerState:
@@ -156,7 +157,8 @@ def kv_gather(descs: torch.Tensor, part_base: Sequence[int], part_bytes: int, wr
                     max_ctas, _stream(descs.device), *pub,
                     status.data_ptr() if status is not None else 0, align_or, stage_bytes,
                     ring_bytes, *lay, *_release_args(release),
-                    [int(r) for r in rows] if rows is not None else [], *_piece_args(pieces))
+                    [int(r) for r in rows] if rows is not None else [], *_piece_args(pieces),
+                    publish.shard_args if publish else [])
 
 
 def kv_copy_multicast(descs: torch.Tensor, nbytes: int, dst_deltas: Sequence[int],
@@ -191,11 +193,19 @@ def kv_read_swizzle_hnd(descs: torch.Tensor, dst: torch.Tensor, tokens: int, hea
                       status.data_ptr() if status is not None else 0, stage_bytes, ring_bytes)
 
 
+def _shard_args(shards: Optional[Sequence[torch.Tensor]]) -> List[Tuple[int, int]]:
+    """(address, bucket mask) of index shards 1, 2, ... for the native launchers."""
+    return [(t.data_ptr(), index_bucket_mask(t)) for t in shards] if shards else []
+
+
 class PublishArgs:
-    """Index records to publish with a write: one 32-byte entry per block."""
+    """Index records to publish with a write: one 32-byte entry per block.  ``shards``: the
+    tables of index shards 1, 2, ... (``table`` is shard 0); each key is published in the
+    table its fingerprint selects (``testing.index_shard_of``).  Only ``kv_copy`` and
+    ``kv_gather`` publish into shards."""
 
     def __init__(self, table: torch.Tensor, keys: Sequence[bytes], addrs: Sequence[int],
-                 gens: Sequence[int], size: int):
+                 gens: Sequence[int], size: int, shards: Optional[Sequence[torch.Tensor]] = None):
         dev = table.device
         rec = np.zeros((len(keys), 4), dtype=np.uint64)
         for i, k in enumerate(keys):
@@ -208,6 +218,8 @@ class PublishArgs:
         self.addrs = list(addrs)
         self.keys = list(keys)
         self.done = torch.zeros(3 * len(keys), dtype=torch.int32, device=dev)  # done | slot | tag
+        self.shards = list(shards) if shards else []
+        self.shard_args = _shard_args(self.shards)
 
 
 def new_index_table(slots: int, device) -> torch.Tensor:
@@ -234,12 +246,13 @@ def pack_keys(keys: Sequence[bytes], device) -> Tuple[torch.Tensor, torch.Tensor
 def index_lookup(table: torch.Tensor, keys: Sequence[bytes], seg_base: Sequence[int] = (),
                  dst_base: int = 0, dst_off: Optional[Sequence[int]] = None, need_bytes: int = 0,
                  want_match: bool = False, found_at: Optional[torch.Tensor] = None,
-                 accept_claimed: bool = False):
+                 accept_claimed: bool = False, shards: Optional[Sequence[torch.Tensor]] = None):
     """Probe `table` for `keys`.  Returns (descs | None, present bitmap, match index | None).
     `accept_claimed`: ways claimed by a writer that has not committed yet count as present
     (the reference's rule for get_match_last_index; never for reads).
     `found_at` ((n, 2) int32, optional) receives (slot + 1, tag) of every hit for
-    :func:`index_validate`."""
+    :func:`index_validate`; the slot id carries the key's shard in its top 3 bits.
+    `shards`: the tables of index shards 1, 2, ... as for :class:`PublishArgs`."""
     dev = table.device
     kb, ko, kl = pack_keys(keys, dev)
     n = len(keys)
@@ -256,7 +269,7 @@ def index_lookup(table: torch.Tensor, keys: Sequence[bytes], seg_base: Sequence[
                        doff.data_ptr() if doff is not None else 0, dst_base, need_bytes,
                        present.data_ptr(), status.data_ptr(), ticket.data_ptr(), want_match,
                        _stream(dev), found_at.data_ptr() if found_at is not None else 0,
-                       accept_claimed)
+                       accept_claimed, _shard_args(shards))
     match = None
     if want_match:
         torch.cuda.synchronize(dev)
@@ -279,15 +292,54 @@ def index_erase(table: torch.Tensor, keys: Sequence[bytes], addrs: Sequence[int]
     torch.cuda.synchronize(dev)  # recs must outlive the kernel
 
 
-def index_validate(table: torch.Tensor, found_at: torch.Tensor) -> int:
-    """Number of entries that changed since the lookup that filled `found_at`."""
+def index_validate(table: torch.Tensor, found_at: torch.Tensor,
+                   shards: Optional[Sequence[torch.Tensor]] = None) -> int:
+    """Number of entries that changed since the lookup that filled `found_at` (with the same
+    `shards`)."""
     dev = table.device
     status = torch.zeros(K.STAT_WORDS, dtype=torch.int32, device=dev)
     with torch.cuda.device(dev):
         K.index_validate(found_at.data_ptr(), found_at.shape[0], table.data_ptr(),
-                         status.data_ptr(), _stream(dev))
+                         status.data_ptr(), _stream(dev), _shard_args(shards))
     torch.cuda.synchronize(dev)
     return int(status[K.STAT_STALE].item())
+
+
+def read_fused(table: torch.Tensor, keys: Sequence[bytes], dst_base: int,
+               dst_off: Sequence[int], nbytes: int, seg_base: Sequence[int],
+               status: torch.Tensor, shards: Optional[Sequence[torch.Tensor]] = None,
+               variant: str = "auto", max_ctas: int = 0, validate: bool = True,
+               align_or: int = 0, stage_bytes: int = 0, ring_bytes: int = 0, elems: int = 0,
+               part_base: Optional[Sequence[int]] = None, part_bytes: int = 0,
+               first_part: int = 0) -> None:
+    """read_cache through the device index in one launch: `keys[i]` is resolved in `table`
+    (and `shards`) and its pool page of `nbytes` lands at ``dst_base + dst_off[i]``; the page
+    is at ``seg_base[seg] + offset`` of its entry's address ``(seg + 1) << 44 | offset``, and an
+    entry smaller than the read is a miss.  Misses count once per block in
+    ``status[STAT_MISS]``; `validate` re-checks every entry after its copy (``STAT_STALE``).
+    `variant` and the alignment of the destinations choose kv_read_fused (byte, 16- or 32-byte
+    vectors) or kv_pipe_read (csrc/kernels/launch_plan.h: plan_read_fused); `align_or` is ORed
+    with every destination address here.  `elems` > 0: fp8 pages of `elems` e4m3 values and
+    their scales, dequantised to bf16 (kv_fp8_pipe; `nbytes` is not read).  `part_base`:
+    gathered blocks, stored part ``first_part + s`` of `part_bytes` landing at ``part_base[s] +
+    dst_off[i]`` (kv_pipe_scatter_read; needs at least as many blocks as CTAs).  Geometries the
+    kernels do not support are refused with ValueError before anything is launched."""
+    dev = table.device
+    kb, ko, kl = pack_keys(keys, dev)
+    offs = [int(o) for o in dst_off]
+    doff = torch.tensor(offs, dtype=torch.int64, device=dev)
+    align_or |= int(dst_base)
+    for o in offs:
+        align_or |= o
+    bases = [int(b) for b in part_base] if part_base is not None else []
+    for b in bases:
+        align_or |= b
+    with torch.cuda.device(dev):
+        K.read_fused(kb.data_ptr(), ko.data_ptr(), kl.data_ptr(), len(keys), table.data_ptr(),
+                     index_bucket_mask(table), [int(b) for b in seg_base], int(dst_base),
+                     doff.data_ptr(), nbytes, align_or, status.data_ptr(), max_ctas, validate,
+                     VARIANTS[variant], stage_bytes, ring_bytes, _stream(dev),
+                     _shard_args(shards), elems, bases, part_bytes, first_part)
 
 
 def presence_bits(present: torch.Tensor, n: int) -> List[bool]:
@@ -322,6 +374,7 @@ def kv_write_fp8(descs: torch.Tensor, elems: int, max_ctas: int = 0,
     TMA-pipelined kernel (kv_fp8_pipe.cu) when elems % 512 == 0, else / "ldst": kv_fp8.cu;
     "pipe4": the pipeline with 4 compute warps.  ``align_or``: the OR of every page address;
     pages that are not 16-byte aligned are refused (RuntimeError), never launched."""
+    assert not (publish and publish.shards), "kv_write_fp8 publishes into one table"
     with torch.cuda.device(descs.device):
         K.kv_write_fp8(descs.data_ptr(), descs.shape[0], elems, 128, max_ctas,
                        _stream(descs.device),
@@ -393,6 +446,7 @@ def kv_gather_fp8(descs: torch.Tensor, part_base: Sequence[int], elems: int, wri
     (kv_read_e4m3_scatter) copies a stored group whose scale is the part's and requantises any
     other to it (docs/kernels.md, "e4m3 cache contract")."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
+    assert not (publish and publish.shards), "kv_gather_fp8 publishes into one table"
     bases = [int(b) for b in part_base]
     for b in bases:
         align_or |= b
