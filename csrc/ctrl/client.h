@@ -214,6 +214,10 @@ class Connection {
         // (kernels::GatherLaunch::part_scale): part s is fp8_elems bytes of float8_e4m3fn of
         // scale part_scale[s], stored as an fp8 page; whole parts only
         const float* part_scale = nullptr;
+        // bf16 parts only: a RoPE shift applied to the rotary dimensions of the parts as they
+        // move (kernels::GatherLaunch::rope; must outlive the call); CUDA tensors, whole parts
+        // of whole heads, no fp8, records, scales, rows or pieces
+        const kernels::RopeShift* rope = nullptr;
         // pool bytes of a part: part_bytes, kernels::fp8_gather_bytes(1, fp8_elems), or with
         // records kernels::fp8_records_bytes(1, fp8_elems, records)
         uint64_t pool_part_bytes() const;
@@ -246,6 +250,7 @@ class Connection {
         uint32_t fp8_elems = 0;           // fp8 elements per part (0: raw bytes), first call
         kernels::Fp8Records records;      // GatherSpec::records of the first call
         bool e4m3 = false;                // the first call's parts were e4m3 (part_scale)
+        bool rope = false;                // the first call shifted RoPE (GatherSpec::rope)
         uint32_t part_bytes = 0;          // pool bytes of a part, first call
         bool failed = false;
         void* event = nullptr;            // cudaEvent_t recorded after the last launch
@@ -262,7 +267,7 @@ class Connection {
                                                 uint32_t pieces = 1);
     // Stores parts g.first_part .. g.first_part + g.nparts - 1 of every block of `w`; offsets
     // are scaled by `scale`.  Refuses part ranges written before, a device, scale, fp8_elems,
-    // records, e4m3 parts (part_scale) or not, or part size other than the first call's, a complete or failed writer, and a writer made
+    // records, e4m3 parts (part_scale) or not, a RoPE shift or not, or part size other than the first call's, a complete or failed writer, and a writer made
     // before the connection was last closed (its blocks and index ways were released).  A
     // refused call leaves the writer as it was.
     int write_layered(GatherWriter& w, const GatherSpec& g, uint64_t scale, int device,

@@ -293,6 +293,7 @@ kernels::GatherLaunch Connection::gather_launch(const GatherSpec& g, uint32_t n,
     G.rows = g.rows;  // the caller stages the piece table beside the descriptors
     G.records = g.records;
     G.part_scale = g.part_scale;
+    G.rope = g.rope;
     return G;
 }
 
@@ -906,6 +907,27 @@ const char* Connection::gather_refusal(const GatherSpec& g, const uint64_t* offs
     } else if (w && w->device != -2 && w->e4m3) {
         return "parts without scales differ from the writer's first call, whose parts were e4m3";
     }
+    if (g.rope) {  // RoPE-shifted segments: bf16 whole parts of whole heads on the GPU
+        if (g.fp8_elems || g.records.latent || g.part_scale)
+            return "a RoPE shift takes bf16 parts: no fp8, records or scales";
+        if (g.rows.rows || g.rows.pieces != 1 || g.piece_off)
+            return "a RoPE shift takes whole parts: no row geometry or pieces";
+        if (!g.rope->ok())
+            return "bad RoPE geometry: head_elems, rot_offset and rot_dim multiples of 8 (neox: "
+                   "rot_dim of 16), 1 to 128 pairs, rot_offset + rot_dim <= head_elems";
+        if (!g.part_bytes || g.part_bytes % (2ull * g.rope->head_elems))
+            return "bad part size for a RoPE shift: a whole number of bf16 heads";
+        if (!g.rope->finite()) return "bad RoPE table: every cos and sin must be finite";
+        if (device < 0) return "a RoPE shift needs CUDA tensors";
+        uint64_t align_or = 0;
+        for (uint32_t s = 0; s < g.nparts; ++s) align_or |= g.part_base[s];
+        for (size_t i = 0; i < n; ++i) align_or |= offs[i];
+        if (align_or & 15) return "a RoPE shift needs 16-byte aligned part bases and offsets";
+        if (w && w->device != -2 && !w->rope)
+            return "a RoPE shift differs from the writer's first call, which had none";
+    } else if (w && w->device != -2 && w->rope) {
+        return "parts without a RoPE shift differ from the writer's first call, which had one";
+    }
     if (g.records.latent) {  // token records: whole parts of whole tokens, bf16 in the tensors
         if (!g.fp8_elems) return "fp8 records need fp8 parts (bf16 elements in the tensors)";
         if (!g.records.ok())
@@ -994,8 +1016,8 @@ int Connection::r_rdma_scatter(const GatherSpec& g, const std::vector<KeyOffset>
         r->group_parts = g.group_parts;
         r->groups = g.group_parts && g.nparts % g.group_parts == 0 ? g.nparts / g.group_parts : 0;
     }
-    std::vector<uint64_t> offs;  // only the fp8 alignment check reads them
-    if (g.fp8_elems) {
+    std::vector<uint64_t> offs;  // only the fp8 and RoPE alignment checks read them
+    if (g.fp8_elems || g.rope) {
         offs.resize(blocks.size());
         for (size_t i = 0; i < blocks.size(); ++i) offs[i] = blocks[i].offset;
     }
@@ -1093,6 +1115,7 @@ int Connection::write_layered(GatherWriter& w, const GatherSpec& g, uint64_t sca
         w.fp8_elems = g.fp8_elems;
         w.records = g.records;
         w.e4m3 = g.part_scale != nullptr;
+        w.rope = g.rope != nullptr;
         w.part_bytes = uint32_t(g.pool_part_bytes());
         w.offsets.swap(scaled);
         w.piece_off.swap(scaled_pieces);

@@ -269,6 +269,48 @@ struct Fp8Records {
     }
 };
 
+// Position-free KV segments (GatherLaunch::rope, kv_rope.cu): a RoPE shift applied to the
+// rotary dimensions of the stored bf16 parts as they move, so a page is stored at position 0
+// and read at any position.  Every part is a run of heads of head_elems bf16 elements; pairs
+// lie in elements [rot_offset, rot_offset + rot_dim) of each head, (i, i + rot_dim / 2)
+// (neox) or (2i, 2i + 1) (interleaved), and pair i turns by the angle whose cos and sin are
+// (c[i], s[i]) (the host builds the table; no trig runs on the GPU):
+//   a' = bf16_rne(rn32(rn32(a * c) - rn32(b * s))),  b' = bf16_rne(rn32(rn32(a * s) + rn32(b * c)))
+// Every other element is copied verbatim, and so is every part that does not rotate: with
+// even_parts only stored parts first_part + s of even index rotate (K of K/V pairs).  A table
+// whose every pair is (1, 0) (shift 0) copies the whole call verbatim.
+constexpr uint32_t kRopeMaxPairs = 128;
+struct RopeShift {
+    uint32_t head_elems = 0;   // bf16 elements of a head (a token, for an MLA latent part)
+    uint32_t rot_offset = 0;   // first rotary element of a head
+    uint32_t rot_dim = 0;      // rotary elements of a head: rot_dim / 2 pairs
+    uint32_t interleaved = 0;  // 1: pairs (2i, 2i + 1); 0: neox pairs (i, i + rot_dim / 2)
+    uint32_t even_parts = 0;   // 1: only stored parts of even index rotate; 0: every part
+    float c[kRopeMaxPairs];    // cos of pair i's angle
+    float s[kRopeMaxPairs];    // sin of pair i's angle
+
+    // 16-byte vectors of whole pairs: head_elems, rot_offset and rot_dim multiples of 8 (neox:
+    // rot_dim of 16, so both halves are whole vectors), 1 to kRopeMaxPairs pairs, inside a head
+    bool ok() const {
+        return head_elems != 0 && head_elems % 8 == 0 && rot_offset % 8 == 0 && rot_dim != 0 &&
+               rot_dim % (interleaved ? 8 : 16) == 0 && rot_dim / 2 <= kRopeMaxPairs &&
+               uint64_t(rot_offset) + rot_dim <= head_elems && interleaved <= 1 &&
+               even_parts <= 1;
+    }
+    bool finite() const {
+        for (uint32_t i = 0; i < rot_dim / 2 && i < kRopeMaxPairs; ++i)
+            if (!(c[i] >= -3.40282347e38f && c[i] <= 3.40282347e38f) ||
+                !(s[i] >= -3.40282347e38f && s[i] <= 3.40282347e38f))
+                return false;
+        return true;
+    }
+    bool identity() const {
+        for (uint32_t i = 0; i < rot_dim / 2 && i < kRopeMaxPairs; ++i)
+            if (c[i] != 1.0f || s[i] != 0.0f) return false;
+        return true;
+    }
+};
+
 struct GatherLaunch {
     // per block, device-addressable: write {local byte offset, pool address},
     // read {pool address or 0 = miss, local byte offset}
@@ -330,12 +372,21 @@ struct GatherLaunch {
     // float8_e4m3fn at part_base[s] + the local offset with scale part_scale[s], stored as the
     // fp8 page of a whole part.  No records, row geometry or pieces.
     const float* part_scale = nullptr;
+    // bf16 launches only (launch_kv_gather): rope != nullptr (a host pointer) shifts the
+    // rotary dimensions of the parts as they move (RopeShift, kv_rope.cu).  Whole parts of
+    // whole heads, 16-byte aligned: no row geometry, pieces, records or scales
+    // (plan_gather_rope).
+    const RopeShift* rope = nullptr;
 };
 // The TMA pipeline for 16-byte aligned parts of at least kPipeMinBytes, the ld/st kernel
 // (kv_copy.cu) otherwise: the same rule launch_kv_copy applies to whole blocks.  Reads run
 // kv_scatter_ldst and writes kv_gather_ldst, with one body per part shape (whole parts, rows,
-// slices, pieces) around the item walks of gather_items.cuh.
+// slices, pieces) around the item walks of gather_items.cuh.  With a.rope the launch runs
+// kv_rope.cu's movers (launch_kv_gather_rope), or, for an identity table, the plain movers.
 cudaError_t launch_kv_gather(const GatherLaunch& a, cudaStream_t stream);
+// kv_write_rope_gather / kv_read_rope_scatter<LAYERED>: the ld/st movers of launch_kv_gather
+// with a.rope applied inside the copy (plain or layered reads, one-shot or layered writes).
+cudaError_t launch_kv_gather_rope(const GatherLaunch& a, cudaStream_t stream);
 cudaError_t launch_kv_pipe_gather(const GatherLaunch& a, cudaStream_t stream);
 struct GatherParts {
     uint64_t base[kGatherMaxParts];
@@ -347,7 +398,8 @@ struct ReadFusedLaunch;
 // r.validate is set.  `r`
 // carries keys, dst_off (local byte offsets; dst_base 0), index, segments, status, grid cap
 // and ring geometry; `g` the parts (descs, recs and write are ignored).  Needs 16-byte aligned
-// parts and at least as many blocks as CTAs (fewer: lookup + launch_kv_gather + validate).
+// parts, no RoPE shift (g.rope) and at least as many blocks as CTAs (fewer: lookup +
+// launch_kv_gather + validate).
 bool scatter_read_fused_supported(const ReadFusedLaunch& r, const GatherLaunch& g);
 cudaError_t launch_kv_pipe_scatter_read(const ReadFusedLaunch& r, const GatherLaunch& g,
                                         cudaStream_t stream);

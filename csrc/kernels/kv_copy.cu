@@ -302,6 +302,12 @@ cudaError_t launch_kv_gather(const GatherLaunch& a, cudaStream_t stream) {
     if (uint64_t(a.nparts) * a.part_bytes > 0xffffffffull) return cudaErrorInvalidValue;
     const bool layered = a.group_flags != nullptr;
     if (layered && !a.group_counters) return cudaErrorInvalidValue;
+    // RoPE shifts: the geometry is checked even when the table turns nothing, which the plain
+    // movers below then copy verbatim
+    if (a.rope) {
+        if (!plan_gather_rope(a, 1, {}).valid || !a.rope->finite()) return cudaErrorInvalidValue;
+        if (!a.rope->identity()) return launch_kv_gather_rope(a, stream);
+    }
     // pieces split rows, at the offsets of the piece table
     if (a.rows.pieces != 1 && (!a.rows.rows || !a.piece_off)) return cudaErrorInvalidValue;
     const GatherParts parts = parts_of(a);

@@ -4,7 +4,8 @@
 // resident (occupancy API), so the choice is unit-tested on the CPU
 // (_infinistore.testing.plan_copy / plan_gather / plan_read_fused / plan_fp8 /
 // plan_gather_fp8 / plan_gather_rows / plan_gather_fp8_rows / plan_gather_rows_write /
-// plan_gather_fp8_rows_write; plan_gather_layered is plan_gather of a layered read).  The
+// plan_gather_fp8_rows_write / plan_gather_e4m3 / plan_gather_rope; plan_gather_layered is
+// plan_gather of a layered read).  The
 // gathered ld/st kernels these plans choose walk their items in gather_items.cuh.
 #pragma once
 
@@ -497,6 +498,35 @@ inline LaunchPlan plan_gather_e4m3(const GatherLaunch& a, uint32_t elems, int sm
     LaunchPlan p;
     p.kernel = Kernel::kLdStFp8;
     ldst_items(p, parts, elems, kLdStChunk, 1u << 20, sms);
+    if (parts * p.cpb > kMaxItems) return invalid_plan();
+    p.ctas = clamp_grid(a.max_ctas > 0 ? a.max_ctas : res.r16 * sms, parts * p.cpb);
+    return p;
+}
+
+// ---------------------------------------------------------------- RoPE-shifted parts
+// Reads (plain or layered) and writes of bf16 whole parts with a RoPE shift
+// (GatherLaunch::rope, kv_rope.cu): always the ld/st kernels.  A work item is a run of whole
+// heads of one part, about kLdStChunk bytes (at least one head), or the whole part under
+// ldst_items' rule; chunk is in bytes, cpb is runs per part, and a layered read numbers items
+// with layered_item as whole parts do.  Refused: no rope or a RopeShift that is not ok(), row
+// geometry, pieces, records, scales, a part that is not a whole number of heads, part bases or
+// local offsets (align_or) that are not 16-byte aligned, 0 or more than kGatherMaxParts parts,
+// groups groups_ok refuses and more than kMaxItems work items.  The grid is one wave of the
+// CTAs the kernel keeps resident (res.r16).
+inline LaunchPlan plan_gather_rope(const GatherLaunch& a, int sms, LdStResident res) {
+    const RopeShift* r = a.rope;
+    const uint64_t parts = uint64_t(a.n) * a.nparts;
+    if (!r || !r->ok() || a.rows.rows != 0 || a.rows.pieces != 1 || a.records.latent != 0 ||
+        a.part_scale || a.part_bytes == 0 || a.part_bytes % (2 * r->head_elems) != 0 ||
+        (a.align_or & 15) != 0 || a.nparts == 0 || a.nparts > kGatherMaxParts ||
+        !groups_ok(a) || parts > kMaxItems)
+        return invalid_plan();
+    const uint32_t head_bytes = 2 * r->head_elems;
+    LaunchPlan p;
+    p.kernel = Kernel::kLdSt16;
+    ldst_items(p, parts, a.part_bytes / head_bytes, std::max(1u, kLdStChunk / head_bytes),
+               std::max(1u, (1u << 20) / head_bytes), sms);
+    p.chunk *= head_bytes;  // heads -> bytes: at most part_bytes
     if (parts * p.cpb > kMaxItems) return invalid_plan();
     p.ctas = clamp_grid(a.max_ctas > 0 ? a.max_ctas : res.r16 * sms, parts * p.cpb);
     return p;

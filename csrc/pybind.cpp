@@ -208,6 +208,32 @@ kernels::Fp8Records parse_records(const std::vector<uint32_t>& v) {
     return kernels::Fp8Records{v[0], v[1]};
 }
 
+// A RoPE shift from its native form: None (no shift, false) or (head_elems, rot_offset,
+// rot_dim, interleaved, even_parts, cos, sin) with rot_dim / 2 cosines and sines.  The
+// connection and the launcher check the geometry and the values.
+bool parse_rope(const py::object& o, kernels::RopeShift& r) {
+    if (o.is_none()) return false;
+    const auto t = o.cast<py::tuple>();
+    if (t.size() != 7)
+        throw py::value_error("rope is (head_elems, rot_offset, rot_dim, interleaved, "
+                              "even_parts, cos, sin)");
+    r = kernels::RopeShift{};
+    r.head_elems = t[0].cast<uint32_t>();
+    r.rot_offset = t[1].cast<uint32_t>();
+    r.rot_dim = t[2].cast<uint32_t>();
+    r.interleaved = t[3].cast<bool>() ? 1 : 0;
+    r.even_parts = t[4].cast<bool>() ? 1 : 0;
+    const auto c = t[5].cast<std::vector<float>>(), s = t[6].cast<std::vector<float>>();
+    if (r.rot_dim % 2 || c.size() != r.rot_dim / 2 || s.size() != c.size() ||
+        c.size() > kernels::kRopeMaxPairs)
+        throw py::value_error("rope: rot_dim / 2 (at most 128) cosines and as many sines");
+    for (size_t i = 0; i < c.size(); ++i) {
+        r.c[i] = c[i];
+        r.s[i] = s[i];
+    }
+    return true;
+}
+
 // A gathered call's parts: part s at part_base[s] (which must outlive the spec); elems > 0:
 // bf16 parts of elems elements stored as fp8 pages, or with records (parse_records) as token
 // records.  rows: a row-sliced read's or write's geometry (parse_rows); empty: whole parts.
@@ -689,7 +715,7 @@ PYBIND11_MODULE(_infinistore, m) {
                uint32_t elems, const py::object& offsets, const py::object& remote_blocks,
                int device, uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows,
                const py::object& piece_off, uint32_t pieces, const std::vector<uint32_t>& records,
-               const std::vector<float>& scales) {
+               const std::vector<float>& scales, const py::object& rope) {
                 BlockSpan rb;
                 OffsetSpan off;
                 blocks_from_py(remote_blocks, rb);
@@ -697,9 +723,11 @@ PYBIND11_MODULE(_infinistore, m) {
                 std::vector<uint64_t> bytes(off.n);
                 for (size_t i = 0; i < off.n; ++i) bytes[i] = off.data[i] * scale;
                 const std::vector<uint64_t> table = piece_table(piece_off, off.n, pieces, scale);
-                const Connection::GatherSpec g =
+                Connection::GatherSpec g =
                     gather_spec(part_base, part_bytes, elems, 0, rows, &table, pieces, records,
                                 scales);
+                kernels::RopeShift rs;
+                if (parse_rope(rope, rs)) g.rope = &rs;
                 py::gil_scoped_release rel;
                 return c.w_rdma_gather(g, bytes.data(), bytes.size(), rb.data, rb.n, device, stream);
             },
@@ -708,6 +736,7 @@ PYBIND11_MODULE(_infinistore, m) {
             py::arg("scale") = 1, py::arg("rows") = std::vector<uint32_t>{},
             py::arg("piece_off") = py::none(), py::arg("pieces") = 1,
             py::arg("records") = std::vector<uint32_t>{}, py::arg("scales") = std::vector<float>{},
+            py::arg("rope") = py::none(),
             "gathered write: block i = part s at part_base[s] + offsets[i] * scale, s = 0..S-1; "
             "elems > 0: bf16 parts of elems elements, quantised into fp8 page s of block i, or "
             "with records = (latent, rope) into elems / (latent + rope) fp8 token records "
@@ -719,7 +748,9 @@ PYBIND11_MODULE(_infinistore, m) {
             "offsets per block (times scale), and run t of rows / pieces rows comes from "
             "part_base[s] + offset + piece_off[i * pieces + t]; scales (one per part, elems > "
             "0, whole parts): the parts are elems bytes of e4m3 of those scales, stored verbatim "
-            "as fp8 pages whose group scales are the part's")
+            "as fp8 pages whose group scales are the part's; rope = (head_elems, rot_offset, "
+            "rot_dim, interleaved, even_parts, cos, sin) (bf16 whole parts): the rotary pairs of "
+            "every head of the rotating parts are turned by the table as they are stored")
         .def(
             "r_rdma_scatter",
             [](Connection& c, const std::vector<uint64_t>& part_base, uint32_t part_bytes,
@@ -727,12 +758,14 @@ PYBIND11_MODULE(_infinistore, m) {
                uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows,
                Connection::ScatterReader* reader, uint32_t group_parts, const py::object& piece_off,
                uint32_t pieces, const std::vector<uint32_t>& records,
-               const std::vector<float>& scales) {
+               const std::vector<float>& scales, const py::object& rope) {
                 std::vector<KeyOffset> kb;
                 blocks_list_from_py(blocks, scale, kb);
                 const std::vector<uint64_t> table = piece_table(piece_off, kb.size(), pieces, scale);
                 Connection::GatherSpec g = gather_spec(part_base, part_bytes, elems, first_part,
                                                        rows, &table, pieces, records, scales);
+                kernels::RopeShift rs;
+                if (parse_rope(rope, rs)) g.rope = &rs;
                 g.reader = reader;
                 g.group_parts = group_parts;
                 py::gil_scoped_release rel;
@@ -744,6 +777,7 @@ PYBIND11_MODULE(_infinistore, m) {
             py::arg("reader") = py::none(), py::arg("group_parts") = 0,
             py::arg("piece_off") = py::none(), py::arg("pieces") = 1,
             py::arg("records") = std::vector<uint32_t>{}, py::arg("scales") = std::vector<float>{},
+            py::arg("rope") = py::none(),
             "scattered read: stored part first_part + s of each block -> part_base[s] + offset; "
             "elems > 0: fp8 pages (or with records, token records) dequantised into bf16 parts "
             "of elems elements; rows = (rows, "
@@ -752,7 +786,8 @@ PYBIND11_MODULE(_infinistore, m) {
             "dst_slice_pitch; reader: a layered read whose parts are "
             "released in groups of group_parts (check reader.failed); pieces as for "
             "w_rdma_gather; scales (one per part): e4m3 parts, each stored group requantised to "
-            "its part's scale (verbatim when the scales are equal)")
+            "its part's scale (verbatim when the scales are equal); rope as for w_rdma_gather, "
+            "turning the pairs as they land")
         .def(
             "wait_layered",
             [](Connection& c, const Connection::ScatterReader& r, uint32_t group, uint64_t stream) {
@@ -795,9 +830,12 @@ PYBIND11_MODULE(_infinistore, m) {
             [](Connection& c, Connection::GatherWriter& w, const std::vector<uint64_t>& part_base,
                uint32_t part_bytes, uint32_t elems, uint32_t first_part, int device,
                uint64_t stream, uint64_t scale, const std::vector<uint32_t>& rows,
-               const std::vector<uint32_t>& records, const std::vector<float>& scales) {
-                const Connection::GatherSpec g = gather_spec(
+               const std::vector<uint32_t>& records, const std::vector<float>& scales,
+               const py::object& rope) {
+                Connection::GatherSpec g = gather_spec(
                     part_base, part_bytes, elems, first_part, rows, nullptr, 1, records, scales);
+                kernels::RopeShift rs;
+                if (parse_rope(rope, rs)) g.rope = &rs;
                 py::gil_scoped_release rel;
                 return c.write_layered(w, g, scale, device, stream);
             },
@@ -805,9 +843,11 @@ PYBIND11_MODULE(_infinistore, m) {
             py::arg("first_part"), py::arg("device") = -1, py::arg("stream") = 0,
             py::arg("scale") = 1, py::arg("rows") = std::vector<uint32_t>{},
             py::arg("records") = std::vector<uint32_t>{}, py::arg("scales") = std::vector<float>{},
+            py::arg("rope") = py::none(),
             "layered write: stored part first_part + s of every block of the writer <- "
             "part_base[s] + offset * scale; elems > 0: fp8 parts of elems bf16 elements; rows, "
-            "records and scales as for w_rdma_gather (every call with scales or none)")
+            "records, scales and rope as for w_rdma_gather (every call with scales or none, and "
+            "with rope or none)")
         .def(
             "rw_local",
             [](Connection& c, const std::string& op, const py::object& blocks, int block_size,
@@ -1107,9 +1147,11 @@ PYBIND11_MODULE(_infinistore, m) {
            uint32_t stage_bytes, uint32_t ring_bytes, uint64_t layer_state, uint32_t layer_parts,
            bool layer_claim, uint64_t group_flags, uint64_t group_counters, uint32_t group_seq,
            uint32_t group_parts, const std::vector<uint32_t>& rows, uint64_t piece_off,
-           uint32_t pieces, const ShardList& shards) {
+           uint32_t pieces, const ShardList& shards, const py::object& rope) {
             if (part_base.empty() || part_base.size() > kernels::kGatherMaxParts)
                 throw std::runtime_error("kv_gather: 1 to GATHER_MAX_PARTS parts");
+            kernels::RopeShift rs;
+            const bool has_rope = parse_rope(rope, rs);
             const kernels::IndexShards sh = parse_shards(shards);
             if (layer_state && first_part + part_base.size() > layer_parts)
                 throw std::runtime_error("kv_gather: first_part + parts > layer_parts");
@@ -1145,6 +1187,7 @@ PYBIND11_MODULE(_infinistore, m) {
                 throw std::runtime_error("kv_gather: rows is 5 or 7 values");
             G.piece_off = as_ptr<const uint64_t>(piece_off);
             G.shards = sh;
+            G.rope = has_rope ? &rs : nullptr;
             const cudaError_t e = kernels::launch_kv_gather(G, as_ptr<CUstream_st>(stream));
             if (e != cudaSuccess) throw std::runtime_error(cudaGetErrorString(e));
         },
@@ -1157,6 +1200,7 @@ PYBIND11_MODULE(_infinistore, m) {
         py::arg("group_flags") = 0, py::arg("group_counters") = 0, py::arg("group_seq") = 0,
         py::arg("group_parts") = 0, py::arg("rows") = std::vector<uint32_t>{},
         py::arg("piece_off") = 0, py::arg("pieces") = 1, py::arg("shards") = ShardList(),
+        py::arg("rope") = py::none(),
         "gathered blocks: descs[i] = write {local byte offset, block address} / read {block "
         "address or 0, local byte offset}; part s of block i at part_base[s] + local offset is "
         "stored part first_part + s.  layer_state (3 zeroed u32 per block, kept across the "
@@ -1167,7 +1211,10 @@ PYBIND11_MODULE(_infinistore, m) {
         "u32 per group.  rows (5 or 7 values): a row-sliced read, or a write whose rows fill "
         "each stored part.  pieces > 1 (with rows): piece_off is the device address of n * "
         "pieces byte offsets, and run t of block i's rows / pieces rows is at part_base[s] + "
-        "local offset + piece_off[i * pieces + t].  shards as for kv_copy");
+        "local offset + piece_off[i * pieces + t].  shards as for kv_copy.  rope = (head_elems, "
+        "rot_offset, rot_dim, interleaved, even_parts, cos, sin): whole bf16 parts whose rotary "
+        "pairs are turned as they move (kv_write_rope_gather, kv_read_rope_scatter; a table of "
+        "(1, 0) pairs copies verbatim)");
     k.def(
         "kv_gather_fp8",
         [](uint64_t descs, uint32_t n, const std::vector<uint64_t>& part_base, uint32_t elems,
@@ -2130,6 +2177,42 @@ PYBIND11_MODULE(_infinistore, m) {
           py::arg("group_parts") = 0, py::arg("write") = false, py::arg("max_ctas") = 0,
           py::arg("sm_count") = 132, py::arg("resident") = 1, py::arg("rows") = 0,
           py::arg("pieces") = 1, py::arg("records") = false);
+    t.def("plan_gather_rope",
+          [plan_dict](uint32_t n, uint32_t nparts, uint32_t part_bytes, uint32_t head_elems,
+                      uint32_t rot_offset, uint32_t rot_dim, bool interleaved, uint64_t align_or,
+                      uint32_t group_parts, bool write, int max_ctas, int sm_count, int resident,
+                      uint32_t rows, uint32_t pieces, bool records, bool scales, bool rope) {
+              static uint32_t flags[1];
+              static const float scale[kernels::kGatherMaxParts] = {};
+              kernels::RopeShift rs;
+              rs.head_elems = head_elems;
+              rs.rot_offset = rot_offset;
+              rs.rot_dim = rot_dim;
+              rs.interleaved = interleaved ? 1 : 0;
+              kernels::GatherLaunch a;
+              a.n = n;
+              a.nparts = nparts;
+              a.part_bytes = part_bytes;
+              a.write = write;
+              a.align_or = align_or;
+              a.group_flags = group_parts ? flags : nullptr;
+              a.group_parts = group_parts;
+              a.max_ctas = max_ctas;
+              a.rows.rows = rows;  // any row geometry is refused
+              a.rows.pieces = pieces;
+              if (records) a.records = kernels::Fp8Records{512, 64};  // records are refused
+              if (scales) a.part_scale = scale;                       // scales are refused
+              a.rope = rope ? &rs : nullptr;
+              return plan_dict(kernels::plan_gather_rope(a, sm_count, {resident, resident}));
+          },
+          py::arg("n"), py::arg("nparts"), py::arg("part_bytes"), py::arg("head_elems"),
+          py::arg("rot_offset") = 0, py::arg("rot_dim") = 0, py::arg("interleaved") = false,
+          py::arg("align_or") = 0, py::arg("group_parts") = 0, py::arg("write") = false,
+          py::arg("max_ctas") = 0, py::arg("sm_count") = 132, py::arg("resident") = 1,
+          py::arg("rows") = 0, py::arg("pieces") = 1, py::arg("records") = false,
+          py::arg("scales") = false, py::arg("rope") = true,
+          "plan_gather_rope of a launch of n blocks of nparts bf16 parts of part_bytes, heads of "
+          "head_elems with rot_dim rotary elements from rot_offset (rope=False: no RopeShift)");
     t.def("fp8_rows_read_bytes", &fp8_rows_read_bytes, py::arg("rows"), py::arg("row_bytes"),
           py::arg("src_pitch"), py::arg("src_col") = 0,
           "bytes_read of a row-sliced read of one stored fp8 part (geometry in bf16 bytes)");

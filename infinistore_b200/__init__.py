@@ -20,7 +20,7 @@ _REFERENCE_SURFACE = (
 )
 # added here: in-process server control, statistics, checkpoint / resume, row-sliced reads
 _ADDITIONS = ("stop_server", "server_stats", "dump_kv_map", "load_kv_map", "PartRows",
-              "FP8Records")
+              "FP8Records", "RotaryConfig", "RopeShift", "rope_inv_freq", "rope_table")
 
 __all__ = [*_REFERENCE_SURFACE, *_ADDITIONS]
 globals().update({_name: getattr(_lib, _name) for _name in __all__})

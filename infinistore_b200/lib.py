@@ -521,6 +521,116 @@ def _check_scales(scales, nparts: int, fp8: bool, rows: "PartRows | None" = None
     return out
 
 
+class RotaryConfig:
+    """An engine's rotary embedding: ``rot_dim`` rotary elements per head (``rot_dim / 2``
+    pairs, at most 128) turned by ``position * inv_freq[i]``.  ``inv_freq`` holds the
+    engine's own ``rot_dim / 2`` frequencies, so scaled schedules (Llama-3.1, YaRN) need
+    nothing here; ``rope_inv_freq`` gives the standard one.  Pairs are ``(i, i + rot_dim / 2)``
+    (neox, the default) or ``(2i, 2i + 1)`` (``interleaved``)."""
+
+    def __init__(self, rot_dim: int, inv_freq, interleaved: bool = False):
+        rot_dim = int(rot_dim)
+        if rot_dim <= 0 or rot_dim % 2 or rot_dim // 2 > 128:
+            raise ValueError(f"rot_dim is a positive even number of at most 256, not {rot_dim}")
+        freq = np.array(inv_freq, dtype=np.float64).reshape(-1)
+        if len(freq) != rot_dim // 2:
+            raise ValueError(f"inv_freq holds rot_dim / 2 = {rot_dim // 2} values, not "
+                             f"{len(freq)}")
+        if not np.isfinite(freq).all():
+            raise ValueError("inv_freq must be finite")
+        freq.setflags(write=False)
+        self.rot_dim = rot_dim
+        self.inv_freq = freq
+        self.interleaved = bool(interleaved)
+
+    def __repr__(self):
+        return (f"RotaryConfig(rot_dim={self.rot_dim}, interleaved={self.interleaved}, "
+                f"inv_freq=[{self.inv_freq[0]:g}, ..., {self.inv_freq[-1]:g}])")
+
+    def __eq__(self, other):
+        return (isinstance(other, RotaryConfig) and self.rot_dim == other.rot_dim
+                and self.interleaved == other.interleaved
+                and np.array_equal(self.inv_freq, other.inv_freq))
+
+
+def rope_inv_freq(rot_dim: int, base: float = 10000.0) -> np.ndarray:
+    """The standard RoPE schedule: ``inv_freq[i] = base ** (-2i / rot_dim)``, float64."""
+    return 1.0 / np.float64(base) ** (np.arange(0, int(rot_dim), 2, dtype=np.float64)
+                                      / int(rot_dim))
+
+
+def rope_table(rotary: RotaryConfig, shift: int) -> Tuple[np.ndarray, np.ndarray]:
+    """The (cos, sin) table of a shift of ``shift`` positions: float32 arrays of ``rot_dim /
+    2`` values, ``c_i = f32(cos(f64(shift) * inv_freq_i))`` and ``s_i = f32(sin(...))``.  The
+    same table goes to the kernels (``RopeShift``), so no trig runs on the GPU."""
+    ang = np.float64(int(shift)) * rotary.inv_freq
+    return np.cos(ang).astype(np.float32), np.sin(ang).astype(np.float32)
+
+
+class RopeShift:
+    """``rope=`` of the gathered bf16 calls: turn the rotary pairs of every head of the parts
+    by ``shift`` positions as they move (docs/kernels.md, "RoPE shift contract").  Each part is
+    a run of heads of ``head_elems`` elements whose rotary elements are ``[rot_offset,
+    rot_offset + rotary.rot_dim)``; with ``even_parts`` only the stored parts of even index
+    turn (K of K/V pairs: the V parts move verbatim).  A shift of 0 copies verbatim."""
+
+    def __init__(self, rotary: RotaryConfig, shift: int, head_elems: int, rot_offset: int = 0,
+                 even_parts: bool = False):
+        if not isinstance(rotary, RotaryConfig):
+            raise ValueError(f"rotary must be a RotaryConfig, not {type(rotary).__name__}")
+        self.rotary = rotary
+        self.shift = int(shift)
+        self.head_elems = int(head_elems)
+        self.rot_offset = int(rot_offset)
+        self.even_parts = bool(even_parts)
+        self.check()
+
+    def __repr__(self):
+        return (f"RopeShift(shift={self.shift}, head_elems={self.head_elems}, "
+                f"rot_offset={self.rot_offset}, even_parts={self.even_parts}, {self.rotary})")
+
+    def check(self, part_size: Optional[int] = None) -> None:
+        """ValueError unless every pair lies in whole 16-byte vectors of a head: head_elems,
+        rot_offset and rot_dim multiples of 8 (neox: rot_dim of 16), rot_offset + rot_dim <=
+        head_elems, and (with ``part_size``) a part of whole heads."""
+        d, e, o = self.rotary.rot_dim, self.head_elems, self.rot_offset
+        if e <= 0 or e % 8 or o < 0 or o % 8 or d % (8 if self.rotary.interleaved else 16):
+            raise ValueError(f"{self}: head_elems, rot_offset and rot_dim must be multiples of 8 "
+                             f"elements (neox pairs: rot_dim a multiple of 16)")
+        if o + d > e:
+            raise ValueError(f"{self}: rot_offset + rot_dim = {o + d} runs past the "
+                             f"{e}-element head")
+        if part_size is not None and int(part_size) % e:
+            raise ValueError(f"{self}: a part of {int(part_size)} elements is not a whole "
+                             f"number of {e}-element heads")
+
+    def native(self) -> tuple:
+        """The connection's form: (head_elems, rot_offset, rot_dim, interleaved, even_parts,
+        cos, sin)."""
+        c, s = rope_table(self.rotary, self.shift)
+        return (self.head_elems, self.rot_offset, self.rotary.rot_dim, self.rotary.interleaved,
+                self.even_parts, c.tolist(), s.tolist())
+
+
+def _check_rope(rope: "RopeShift | None", part_size: int, fp8: bool, rows, records,
+                scales, pieces: bool) -> Optional[tuple]:
+    """The checks of every ``rope=`` that need no tensor (None: no shift): a
+    :class:`RopeShift` of a bf16 call of whole parts (no fp8, ``rows``, ``records``,
+    ``scales`` or pieces) of whole heads.  Returns its native form."""
+    if rope is None:
+        return None
+    if not isinstance(rope, RopeShift):
+        raise ValueError(f"rope must be a RopeShift, not {type(rope).__name__}")
+    if fp8 or records is not None or scales is not None:
+        raise ValueError("rope= shifts bf16 parts: it cannot be combined with fp8, records= or "
+                         "scales=")
+    if rows is not None or pieces:
+        raise ValueError("rope= takes whole parts: it cannot be combined with rows= or 2-D "
+                         "offsets (pieces)")
+    rope.check(part_size)
+    return rope.native()
+
+
 def _block_offsets(offsets, nblocks: Optional[int] = None) -> np.ndarray:
     """The local offsets (elements) of gathered blocks as int64: 1-D, or ``(n, k)`` with one
     column per piece of a block, where ``(n, 1)`` is 1-D.  ValueError for another shape, for
@@ -552,6 +662,7 @@ class _Gather(NamedTuple):
     records: list  # native fp8 records (FP8Records.native), or []
     pieces: dict  # piece arguments (_piece_args), or {}
     scales: list  # one float32 scale per e4m3 part (_check_scales), or []
+    rope: Optional[tuple]  # native RoPE shift (RopeShift.native), or None
 
 
 def _raise_if_fp8_pages_unaligned(cache: torch.Tensor, offsets) -> None:
@@ -849,7 +960,8 @@ class InfinityConnection:
     def _gather_parts(self, parts, offsets, part_size: int, first_part: int = 0,
                       block_parts=None, fp8: bool = False, rows: "PartRows | None" = None, *,
                       nblocks=None, stream="current", write: bool = False,
-                      records: "FP8Records | None" = None, scales=None):
+                      records: "FP8Records | None" = None, scales=None,
+                      rope: "RopeShift | None" = None):
         """Checks a gathered call before anything is enqueued: parts ``first_part ..
         first_part + len(parts) - 1`` of the blocks at ``offsets`` (elements, a list or an int64
         ndarray; ``nblocks`` of them when given), in a parts list ``[(tensor, base), ...]``, of
@@ -866,12 +978,15 @@ class InfinityConnection:
         .. (i + 1) * T / k - 1`` of the part's ``T`` tokens, is at ``offsets[b, i]``.
         ``scales`` (with ``fp8``, one per part, ``_check_scales``): the parts are
         ``float8_e4m3fn`` CUDA tensors of those scales (e4m3 caches), whole parts only: no
-        ``rows``, ``records`` or 2-D offsets.  Returns the native call's arguments (``_Gather``): with pieces its offsets are zeros
+        ``rows``, ``records`` or 2-D offsets.  ``rope`` (a :class:`RopeShift`, ``_check_rope``):
+        bf16 CUDA parts of whole heads, 16-byte aligned part bases and offsets, no fp8,
+        ``rows``, ``records``, ``scales`` or 2-D offsets.  Returns the native call's arguments (``_Gather``): with pieces its offsets are zeros
         and its piece arguments carry the ``(n, k)`` offsets."""
         if self._mode != "rdma":
             raise Exception("gathered blocks need a connected rdma connection")
         _check_records(records, part_size, fp8, rows)
         offs = _block_offsets(offsets, nblocks)
+        rope_native = _check_rope(rope, part_size, fp8, rows, records, scales, offs.ndim == 2)
         if scales is not None and offs.ndim == 2:
             raise ValueError("scales= takes whole parts: no pieces (2-D offsets)")
         table = None
@@ -959,6 +1074,17 @@ class InfinityConnection:
                 raise ValueError("fp8 gathered blocks need 16-byte aligned part bases and offsets")
             if first.device.type != "cuda":
                 raise ValueError("fp8 gathered blocks take CUDA tensors")
+        if rope is not None:
+            if first.dtype != torch.bfloat16 or first.device.type != "cuda":
+                raise ValueError(f"rope= shifts bf16 CUDA parts, not {first.dtype} on "
+                                 f"{first.device}")
+            align = 0
+            for b in bases:
+                align |= b
+            if local.size:
+                align |= int(np.bitwise_or.reduce(local.reshape(-1) * es))
+            if align & 15:
+                raise ValueError("rope= needs 16-byte aligned part bases and offsets")
         dev = _device_of(first)
         if dev < 0 and self.conn.server_has_hbm():
             raise ValueError("gathered blocks of CPU tensors need a host-memory pool "
@@ -966,12 +1092,12 @@ class InfinityConnection:
         return _Gather(bases, dev, es, offs, _stream_of(first, stream), part_size * es,
                        part_size if fp8 else 0, rows.native(es) if rows is not None else [],
                        records.native() if records is not None else [], _piece_args(table),
-                       scales.tolist() if scales is not None else [])
+                       scales.tolist() if scales is not None else [], rope_native)
 
     def _gather_write(self, parts, offsets, part_size: int, stream, rows: "PartRows | None",
                       fp8: bool, records: "FP8Records | None", remote_blocks=None,
                       writer: "GatherWriter | None" = None, first_part: int = 0,
-                      scales=None) -> None:
+                      scales=None, rope: "RopeShift | None" = None) -> None:
         """The gathered write, bf16 or fp8 (with ``scales``, of e4m3 parts): into
         ``remote_blocks`` in one call (``rdma_write_cache_gather[_fp8]``), or parts from
         ``first_part`` of the blocks of a layered ``writer`` (``GatherWriter.write``)."""
@@ -979,15 +1105,16 @@ class InfinityConnection:
         g = self._gather_parts(parts, offsets, part_size, first_part,
                                None if one_call else writer.nparts, fp8, rows,
                                nblocks=len(remote_blocks) if one_call else None, stream=stream,
-                               write=True, records=records, scales=scales)
+                               write=True, records=records, scales=scales, rope=rope)
         if not one_call:
             writer._claim(parts[0][0])
             ret = self.conn.w_rdma_layered(writer._w, g.bases, g.part_bytes, g.elems, first_part,
-                                           g.dev, g.stream, g.es, g.rows, g.records, g.scales)
+                                           g.dev, g.stream, g.es, g.rows, g.records, g.scales,
+                                           g.rope)
         elif len(g.offsets):
             ret = self.conn.w_rdma_gather(g.bases, g.part_bytes, g.elems, g.offsets, remote_blocks,
                                           g.dev, g.stream, g.es, g.rows, **g.pieces,
-                                          records=g.records, scales=g.scales)
+                                          records=g.records, scales=g.scales, rope=g.rope)
         else:
             return
         if ret < 0:
@@ -995,19 +1122,21 @@ class InfinityConnection:
 
     def _scatter_read(self, parts, blocks, part_size: int, first_part: int, stream,
                       rows: "PartRows | None", fp8: bool, records: "FP8Records | None",
-                      group_parts: Optional[int] = None, scales=None) -> "ScatterRead | None":
+                      group_parts: Optional[int] = None, scales=None,
+                      rope: "RopeShift | None" = None) -> "ScatterRead | None":
         """The scattered read, bf16 or fp8 (with ``scales``, into e4m3 parts):
         ``read_cache_scatter[_fp8]``, or with ``group_parts`` the layered
         ``read_cache_scatter_layered``, which returns its reader."""
         keys, offs = _split_blocks(blocks)
         g = self._gather_parts(parts, offs, part_size, first_part, fp8=fp8, rows=rows,
-                               nblocks=len(keys), stream=stream, records=records, scales=scales)
+                               nblocks=len(keys), stream=stream, records=records, scales=scales,
+                               rope=rope)
         args = (g.bases, g.part_bytes, g.elems, int(first_part), (keys, g.offsets), g.dev,
                 g.stream, g.es, g.rows)
         if group_parts is None:
             if len(g.offsets):
                 ret = self.conn.r_rdma_scatter(*args, **g.pieces, records=g.records,
-                                               scales=g.scales)
+                                               scales=g.scales, rope=g.rope)
                 if ret < 0:
                     raise Exception(f"Failed to read to infinistore, ret = {ret}: "
                                     f"{self.conn.last_error()}")
@@ -1021,7 +1150,7 @@ class InfinityConnection:
             raise ValueError(f"group_parts {group_parts} does not divide the {len(g.bases)} parts")
         native = _infinistore.ScatterReader()
         self.conn.r_rdma_scatter(*args, native, group_parts, **g.pieces, records=g.records,
-                                 scales=g.scales)
+                                 scales=g.scales, rope=g.rope)
         read = ScatterRead(self, native, parts[0][0].device)
         if native.failed:
             err = Exception(f"Failed to read to infinistore: {self.conn.last_error()}")
@@ -1030,7 +1159,8 @@ class InfinityConnection:
         return read
 
     def rdma_write_cache_gather(self, parts, offsets, part_size: int, remote_blocks,
-                                stream="current", rows: "PartRows | None" = None):
+                                stream="current", rows: "PartRows | None" = None,
+                                rope: "RopeShift | None" = None):
         """Write block ``i`` as the concatenation over ``s`` of
         ``parts[s][0].view(-1)[parts[s][1] + offsets[i] : ... + part_size]``.
 
@@ -1056,12 +1186,21 @@ class InfinityConnection:
         With ``rows``, ``offsets`` may be an ``(n, k)`` int64 array (pieces): the ``rows.count``
         rows of every stored part split into k runs, and run i of block b is taken from
         ``offsets[b, i]`` - e.g. a chunk of k engine pages stored under one key, each page where
-        the block table puts it.  k must divide ``rows.count``; ``(n, 1)`` is the 1-D call."""
-        self._gather_write(parts, offsets, part_size, stream, rows, False, None, remote_blocks)
+        the block table puts it.  k must divide ``rows.count``; ``(n, 1)`` is the 1-D call.
+
+        ``rope`` (a :class:`RopeShift`) turns the rotary pairs of every head of the rotating
+        parts by ``rope.shift`` positions inside the write kernel (a segment written at
+        position ``p0`` passes ``-p0``, so the stored page is the segment at position 0).  The
+        parts are bf16 CUDA tensors of whole heads, 16-byte aligned, whole parts only (no
+        ``rows`` or 2-D offsets); anything else raises ``ValueError`` before anything is
+        enqueued."""
+        self._gather_write(parts, offsets, part_size, stream, rows, False, None, remote_blocks,
+                           rope=rope)
         return 0
 
     def read_cache_scatter(self, parts, blocks, part_size: int, first_part: int = 0,
-                           stream="current", rows: "PartRows | None" = None):
+                           stream="current", rows: "PartRows | None" = None,
+                           rope: "RopeShift | None" = None):
         """Scatter parts ``first_part .. first_part + len(parts) - 1`` of every stored block
         into the parts list (see ``rdma_write_cache_gather``): stored part ``first_part + s``
         of block ``(key, offset)`` lands at ``parts[s][1] + offset`` of ``parts[s][0]``.
@@ -1080,8 +1219,13 @@ class InfinityConnection:
         tensor-parallel degree.  Bad geometry raises ``ValueError`` before anything is
         enqueued.  With ``rows``, ``(keys, offsets)`` may carry an ``(n, k)`` int64 array
         (pieces, as for ``rdma_write_cache_gather``): run i of the rows of block b lands at
-        ``offsets[b, i]``."""
-        self._scatter_read(parts, blocks, part_size, first_part, stream, rows, False, None)
+        ``offsets[b, i]``.
+
+        ``rope`` (a :class:`RopeShift`, as for ``rdma_write_cache_gather``) turns the rotary
+        pairs as they land: a segment stored at position 0 read at position ``p1`` passes
+        ``p1``.  ``rope.even_parts`` counts stored parts, from ``first_part``."""
+        self._scatter_read(parts, blocks, part_size, first_part, stream, rows, False, None,
+                           rope=rope)
 
     # ------------------------------------------------------------------ gathered fp8 blocks
     @staticmethod
@@ -1170,7 +1314,7 @@ class InfinityConnection:
                                    first_part: int = 0, fp8: bool = False,
                                    stream="current", rows: "PartRows | None" = None,
                                    records: "FP8Records | None" = None,
-                                   scales=None) -> "ScatterRead":
+                                   scales=None, rope: "RopeShift | None" = None) -> "ScatterRead":
         """``read_cache_scatter`` (``read_cache_scatter_fp8`` with ``fp8``) in one call whose
         parts are released to consumers group by group: group ``g`` is parts
         ``g * group_parts .. g * group_parts + group_parts - 1`` of every block (with the
@@ -1186,9 +1330,9 @@ class InfinityConnection:
         raises here; the exception's ``read`` attribute is the failed reader.  ``rows`` as for
         ``read_cache_scatter[_fp8]``, ``records`` (with ``fp8``, and its pieces of whole
         tokens without ``rows``) and ``scales`` (with ``fp8``) as for
-        ``read_cache_scatter_fp8``."""
+        ``read_cache_scatter_fp8``; ``rope`` (without ``fp8``) as for ``read_cache_scatter``."""
         return self._scatter_read(parts, blocks, part_size, first_part, stream, rows, fp8, records,
-                                  group_parts, scales=scales)
+                                  group_parts, scales=scales, rope=rope)
 
     # ------------------------------------------------------------------ layered gathered writes
     def gather_writer(self, remote_blocks, offsets, nparts: int, part_size: int,
@@ -1475,7 +1619,8 @@ class GatherWriter:
         return self._w.failed
 
     def write(self, parts, first_part: int, stream="current",
-              rows: "PartRows | None" = None, scales=None) -> None:
+              rows: "PartRows | None" = None, scales=None,
+              rope: "RopeShift | None" = None) -> None:
         """Store parts ``first_part .. first_part + len(parts) - 1`` of every block: stored
         part ``first_part + s`` of block i is ``parts[s][0].view(-1)[parts[s][1] + offsets[i]
         : ... + part_size]``.  ``parts`` is ``[(tensor, base), ...]`` as for
@@ -1487,7 +1632,9 @@ class GatherWriter:
         stores whole parts.  A writer made with ``records`` and 2-D offsets (pieces of whole
         tokens) takes no ``rows``.  ``scales`` (an fp8 writer's, one per part of this call, as
         for ``rdma_write_cache_gather_fp8``): the parts are e4m3 caches; every call of a writer
-        passes scales, or none does."""
+        passes scales, or none does.  ``rope`` (a bf16 writer's, as for
+        ``rdma_write_cache_gather``; ``even_parts`` counts stored parts): every call of a writer
+        passes a shift, or none does."""
         if self._w.failed or self._w.complete:
             raise ValueError("the writer is complete or has failed")
         parts = list(parts)
@@ -1501,7 +1648,8 @@ class GatherWriter:
         if self._offs.ndim == 2 and rows is None and self.records is None:
             raise ValueError("a writer made with 2-D offsets (pieces) needs rows= on every call")
         self._conn._gather_write(parts, self._offs, self.part_size, stream, rows, self.fp8,
-                                 self.records, writer=self, first_part=first_part, scales=scales)
+                                 self.records, writer=self, first_part=first_part, scales=scales,
+                                 rope=rope)
 
     def _claim(self, first: torch.Tensor) -> None:
         """The first call fixes the device and dtype; ValueError for another one later."""

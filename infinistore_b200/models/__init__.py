@@ -10,9 +10,9 @@ kernels serve directly: a head-major decode cache filled by the layout-swizzling
 (``HeadMajorKVCache``) and several caches of one GPU filled by one fetch (``read_layer_multi``).
 """
 from .kv_layout import (KVLayout, LAYOUTS, MLA_LAYOUTS, MLALayout, get_layout, chain_hashes,
-                        mla_chunk_key, mla_page_key, page_key)
+                        mla_chunk_key, mla_page_key, mla_segment_key, page_key, segment_key)
 from .paged_kv import HeadMajorKVCache, MLAKVCache, PagedKVCache, layer_keys, read_layer_multi
 
 __all__ = ["KVLayout", "LAYOUTS", "get_layout", "chain_hashes", "page_key", "PagedKVCache",
            "HeadMajorKVCache", "layer_keys", "read_layer_multi", "MLALayout", "MLA_LAYOUTS",
-           "mla_page_key", "mla_chunk_key", "MLAKVCache"]
+           "mla_page_key", "mla_chunk_key", "MLAKVCache", "segment_key", "mla_segment_key"]

@@ -185,3 +185,20 @@ def mla_chunk_key(model: str, chunk_tokens: int, chunk_hash: str, fp8: bool = Fa
     block, and chunks of another size, pages and K/V keys never resolve to it.  ``chunk_hash``
     comes from ``chain_hashes(token_ids, chunk_tokens)``."""
     return f"{model}/L{ALL_LAYERS}/{'MLA8' if fp8 else 'MLA'}x{int(chunk_tokens)}/{chunk_hash}"
+
+
+def segment_key(model: str, page_tokens: int, tp_rank: int, segment_hash: str) -> str:
+    """Key of one position-free all-layer page of a KV segment (``PagedKVCache.write_segment``):
+    ``model/Lall/KVseg<page_tokens>/tp<rank>/<hash>``.  The page is stored at position 0 (its
+    keys' RoPE turned back by the segment's position), so the key names no position, and its
+    kind field differs from every page and chunk key's, so neither ever resolves to the other's
+    block.  ``segment_hash`` comes from ``chain_hashes(segment_tokens, page_tokens)`` over the
+    segment's own tokens."""
+    return f"{model}/L{ALL_LAYERS}/KVseg{int(page_tokens)}/tp{tp_rank}/{segment_hash}"
+
+
+def mla_segment_key(model: str, page_tokens: int, segment_hash: str) -> str:
+    """Key of one position-free all-layer MLA page of a segment (``MLAKVCache.write_segment``):
+    ``model/Lall/MLAseg<page_tokens>/<hash>``, with no TP field (every rank holds the same
+    latent), distinct from every MLA page and chunk key."""
+    return f"{model}/L{ALL_LAYERS}/MLAseg{int(page_tokens)}/{segment_hash}"

@@ -6,9 +6,10 @@ from typing import List, NamedTuple, Optional, Sequence
 import numpy as np
 import torch
 
-from ..lib import _GATHER_MAX_BLOCK_BYTES, FP8Records, PartRows, _check_scales
+from ..lib import (_GATHER_MAX_BLOCK_BYTES, FP8Records, PartRows, RopeShift, RotaryConfig,
+                   _check_scales)
 from .kv_layout import (ALL_LAYERS, KVLayout, MLALayout, chunk_key, mla_chunk_key, mla_page_key,
-                        page_key, tp_sources)
+                        mla_segment_key, page_key, segment_key, tp_sources)
 
 
 def _layer_range(layers: Optional[range], n: int) -> range:
@@ -181,22 +182,24 @@ class _AllLayerPages:
         self._ensure_registered(conn)
         return conn.allocate_rdma(plan.keys, nbytes), records
 
-    def _store(self, conn, plan: _Plan, fp8: bool, stream) -> int:
+    def _store(self, conn, plan: _Plan, fp8: bool, stream,
+               rope: Optional[RopeShift] = None) -> int:
         blocks, records = self._allocate(conn, plan, fp8)
         layers = range(self.layout.layers)
         conn._gather_write(self._parts(layers), plan.offsets, plan.part, stream, plan.rows, fp8,
-                           records, blocks, scales=self._scales(layers))
+                           records, blocks, scales=self._scales(layers), rope=rope)
         return len(blocks)
 
-    def _writer(self, conn, plan: _Plan, fp8: bool) -> "PageWriter":
+    def _writer(self, conn, plan: _Plan, fp8: bool,
+                rope: Optional[RopeShift] = None) -> "PageWriter":
         blocks, records = self._allocate(conn, plan, fp8)
         return PageWriter(self, conn.gather_writer(blocks, plan.offsets,
                                                    self._per_layer * self.layout.layers,
                                                    plan.part, fp8=fp8, records=records),
-                          plan.rows)
+                          plan.rows, rope)
 
     def _read(self, conn, plan: _Plan, layers: Optional[range], fp8: bool, stream,
-              layered: bool = False):
+              layered: bool = False, rope: Optional[RopeShift] = None):
         """Reads ``layers`` (checked, default all) of the plan's blocks: returns the number of
         blocks, or with ``layered`` the ``PageRead``."""
         records = self._format(plan, fp8)
@@ -205,8 +208,118 @@ class _AllLayerPages:
         read = conn._scatter_read(self._parts(layers), (plan.keys, plan.offsets), plan.part,
                                   self._per_layer * layers.start, stream, plan.rows, fp8,
                                   records, self._per_layer if layered else None,
-                                  scales=self._scales(layers))
+                                  scales=self._scales(layers), rope=rope)
         return PageRead(read, layers) if layered else len(plan.keys)
+
+
+class _Segments:
+    """Position-free KV segments of an all-layer page cache with a ``rotary`` config
+    (:class:`PagedKVCache`, :class:`MLAKVCache`): a run of pages whose first token sits at
+    ``position`` of this request is stored as the segment at position 0 - the write kernel
+    turns the keys' RoPE back by ``position`` - under keys of the segment's own tokens
+    (``segment_keys``), and read at any position, turned forward inside the read kernel.  So
+    content that comes back behind another preamble (a retrieved document, a tool schema, a
+    chat history whose oldest turns were cut) is read instead of recomputed.
+
+    Only the keys' rotary dimensions move: V, the MLA latent and the non-rotary dimensions are
+    byte for byte what the engine holds, and a shift of 0 moves every byte verbatim.  The
+    tokens of a reused segment did not attend to the new preamble; whether that approximation
+    is acceptable, and whether to recompute some of its tokens, is the engine's decision.
+
+    The segment calls run through the page calls' one plan / store / writer / read path, in
+    bf16 only (no ``fp8``, ``source_tp`` or chunks).  They raise ``ValueError`` before anything
+    is allocated on a cache without ``rotary``, on an e4m3 cache, for a ``position`` that is
+    negative or not a multiple of ``page_tokens`` (whole pages land), and for a rotary config
+    that does not fit the layout."""
+
+    rotary: Optional[RotaryConfig] = None
+
+    def _segment_geometry(self):
+        """(head_elems, rot_offset, even_parts) of the rotary pairs in a stored part."""
+        raise NotImplementedError
+
+    def _segment_plan(self, pages: Sequence[int], segment_hashes: Sequence[str]) -> _Plan:
+        if len(pages) != len(segment_hashes):
+            raise ValueError(f"{len(pages)} pages for {len(segment_hashes)} segment hashes")
+        elems = self.layout.page_elems
+        return _Plan(self.segment_keys(segment_hashes),
+                     np.asarray(pages, dtype=np.int64) * elems, None, elems)
+
+    def _shift(self, position, sign: int) -> RopeShift:
+        """The checked RoPE shift of a segment at ``position``: ``-position`` for a write,
+        ``+position`` for a read."""
+        if self.rotary is None:
+            raise ValueError("segments need a cache made with rotary= (its RotaryConfig)")
+        if self.kv_scales is not None:
+            raise ValueError("an e4m3 cache (kv_scales=) stores no segments: they are bf16")
+        if self.data.dtype != torch.bfloat16 or self.data.device.type != "cuda":
+            raise ValueError("segments need a bf16 cache on a CUDA device")
+        if isinstance(position, bool) or not isinstance(position, (int, np.integer)):
+            raise ValueError(f"position is an int, not {type(position).__name__}")
+        position, tokens = int(position), self.layout.page_tokens
+        if position < 0 or position % tokens:
+            raise ValueError(f"position {position} must be a non-negative multiple of "
+                             f"page_tokens = {tokens}: a segment lands as whole pages")
+        head_elems, rot_offset, even_parts = self._segment_geometry()
+        return RopeShift(self.rotary, sign * position, head_elems, rot_offset, even_parts)
+
+    def segment_keys(self, segment_hashes: Sequence[str]) -> List[str]:
+        raise NotImplementedError
+
+    def write_segment(self, conn, pages: Sequence[int], segment_hashes: Sequence[str],
+                      position: int, stream="current") -> int:
+        """Store pages ``pages``, whose first token sits at ``position`` of this request, as
+        the segment at position 0 under ``segment_keys(segment_hashes)``, every layer's parts
+        of a page under one key.  ``segment_hashes`` come from ``chain_hashes(segment_tokens,
+        page_tokens)`` over the segment's own tokens.  Blocks whose key already exists are
+        skipped (first writer wins).  Returns the number of blocks asked for."""
+        rope = self._shift(position, -1)
+        return self._store(conn, self._segment_plan(pages, segment_hashes), False, stream, rope)
+
+    def segment_writer(self, conn, pages: Sequence[int], segment_hashes: Sequence[str],
+                       position: int) -> "PageWriter":
+        """``write_segment`` layer by layer: the writer's ``write_layers(range(l, l + 1))``
+        stores layer l right after it has been produced; a page becomes readable once its last
+        layer has landed."""
+        rope = self._shift(position, -1)
+        return self._writer(conn, self._segment_plan(pages, segment_hashes), False, rope)
+
+    def read_segment(self, conn, pages: Sequence[int], segment_hashes: Sequence[str],
+                     position: int, layers: Optional[range] = None, stream="current") -> int:
+        """Fetch a stored segment into pages ``pages``, its first token at ``position`` of this
+        request: the keys' RoPE is turned forward by ``position`` inside the read.  ``layers``
+        (a step-1 range, default all) reads only those layers.  A missing page fails the read
+        (it raises, or with ``device_lookup`` ``sync()`` reports the miss) and leaves its pages
+        untouched.  Returns the number of blocks read."""
+        rope = self._shift(position, 1)
+        return self._read(conn, self._segment_plan(pages, segment_hashes), layers, False, stream,
+                          rope=rope)
+
+    def read_segment_layered(self, conn, pages: Sequence[int], segment_hashes: Sequence[str],
+                             position: int, layers: Optional[range] = None,
+                             stream="current") -> "PageRead":
+        """``read_segment`` in one call that releases each layer as it lands
+        (``wait_layer(l, stream)``, as for ``read_pages_layered``)."""
+        rope = self._shift(position, 1)
+        return self._read(conn, self._segment_plan(pages, segment_hashes), layers, False, stream,
+                          layered=True, rope=rope)
+
+    def cached_segment_pages(self, conn, segment_hashes: Sequence[str]) -> int:
+        """How many leading pages of this segment the store holds."""
+        if not segment_hashes:
+            return 0
+        return _prefix_pages(conn, [self.segment_keys(segment_hashes)])
+
+    def touch_segment(self, conn, segment_hashes: Sequence[str]) -> int:
+        """Tell an evicting store that these segment pages were just used.  Returns the number
+        of blocks refreshed."""
+        return _touch(conn, [self.segment_keys(segment_hashes)])
+
+
+def _check_rotary(rotary) -> Optional[RotaryConfig]:
+    if rotary is not None and not isinstance(rotary, RotaryConfig):
+        raise ValueError(f"rotary must be a RotaryConfig, not {type(rotary).__name__}")
+    return rotary
 
 
 class _PagedCache(_AllLayerPages):
@@ -458,7 +571,7 @@ class _PagedCache(_AllLayerPages):
                           layers, fp8, stream, layered=True)
 
 
-class PagedKVCache(_PagedCache):
+class PagedKVCache(_Segments, _PagedCache):
     """``cache[layer, kv, page]`` is one contiguous page of ``layout.page_elems`` elements.
 
     The whole cache is one tensor, registered once with the connection (``register_mr``) and
@@ -480,15 +593,22 @@ class PagedKVCache(_PagedCache):
     ``fp8=True`` read into it.  ``fp8=False``, ``source_tp`` of another degree and the chunk
     methods raise ``ValueError`` before anything is allocated.  ``kv_scales`` keeps a read-only
     float32 host copy of the scales.
+
+    ``rotary`` (a :class:`RotaryConfig`) makes the cache store position-free segments
+    (``write_segment``, ``segment_writer``, ``read_segment[_layered]``; see ``_Segments``):
+    the pairs lie in the leading ``rotary.rot_dim`` dimensions of every KV head (vLLM's partial
+    rotary), and only the K parts turn.
     """
 
     def __init__(self, layout: KVLayout, num_pages: int, device, tp_rank: int = 0,
-                 kv_scales=None):
+                 kv_scales=None, rotary: Optional[RotaryConfig] = None):
         scales = None if kv_scales is None else _e4m3_scales(layout, device, kv_scales)
+        rotary = _check_rotary(rotary)
         super().__init__(layout, num_pages, tp_rank,
                          torch.zeros(layout.layers, 2, num_pages, layout.page_elems,
                                      dtype=layout.dtype, device=device))
         self.kv_scales = scales
+        self.rotary = rotary
 
     def page(self, layer: int, kv: int, page: int) -> torch.Tensor:
         return self.data[layer, kv, page]
@@ -546,15 +666,26 @@ class PagedKVCache(_PagedCache):
     def _write_rows(self):
         return None  # the stored layout: whole parts
 
+    # ------------------------------------------------------------------ segments
+    def segment_keys(self, segment_hashes: Sequence[str]) -> List[str]:
+        """Store keys of segment pages (``kv_layout.segment_key``)."""
+        return [segment_key(self.layout.name, self.layout.page_tokens, self.tp_rank, h)
+                for h in segment_hashes]
+
+    def _segment_geometry(self):
+        return self.layout.head_dim, 0, True  # every KV head's leading dims; K parts only
+
 
 class PageWriter:
     """Layer-by-layer upload of all-layer pages (``page_writer`` or ``chunk_writer`` of every
     cache)."""
 
-    def __init__(self, cache: _AllLayerPages, writer, rows: Optional[PartRows] = None):
+    def __init__(self, cache: _AllLayerPages, writer, rows: Optional[PartRows] = None,
+                 rope: Optional[RopeShift] = None):
         self.cache = cache
         self.writer = writer
         self.rows = rows  # how the cache's pages fill each stored part (None: whole)
+        self.rope = rope  # a segment writer's RoPE shift (None: pages)
 
     @property
     def complete(self) -> bool:
@@ -565,7 +696,8 @@ class PageWriter:
         range) of every page."""
         layers = _layer_range(layers, self.cache.layout.layers)
         self.writer.write(self.cache._parts(layers), self.cache._per_layer * layers.start,
-                          stream=stream, rows=self.rows, scales=self.cache._scales(layers))
+                          stream=stream, rows=self.rows, scales=self.cache._scales(layers),
+                          rope=self.rope)
 
 
 class PageRead:
@@ -670,7 +802,7 @@ class HeadMajorKVCache(_PagedCache):
                         dst_slice_pitch=tokens * dim)
 
 
-class MLAKVCache(_AllLayerPages):
+class MLAKVCache(_Segments, _AllLayerPages):
     """The KV cache of an MLA model: ``data[layer, page, token]`` is one token's latent and
     RoPE elements (``layout.token_dim``), vLLM's per-layer MLA block shape stacked over the
     layers.  All-layer pages are stored under one key per page (``mla_page_key``) as
@@ -690,16 +822,35 @@ class MLAKVCache(_AllLayerPages):
     tokens that an ``MLAKVCache`` of that page size stores, so caches of different page sizes
     share chunks of one size, and page i of chunk b is this cache's page ``block_table[b, i]``.
     The kernels land each page through the block table: bf16 as one row per page
-    (``PartRows`` pieces), fp8 as pieces of whole tokens of the record movers."""
+    (``PartRows`` pieces), fp8 as pieces of whole tokens of the record movers.
+
+    ``rotary`` (a :class:`RotaryConfig` of ``rot_dim == rope_dim``) makes the cache store
+    position-free segments (``write_segment``, ``segment_writer``, ``read_segment[_layered]``;
+    see ``_Segments``): each token's trailing ``rope_dim`` elements turn, its latent moves
+    verbatim."""
 
     _per_layer = 1
     _fp8_pages = "fp8 MLA pages"
 
-    def __init__(self, layout: MLALayout, num_pages: int, device):
+    def __init__(self, layout: MLALayout, num_pages: int, device,
+                 rotary: Optional[RotaryConfig] = None):
+        rotary = _check_rotary(rotary)
         super().__init__(layout, num_pages,
                          torch.zeros(layout.layers, num_pages, layout.page_tokens,
                                      layout.token_dim, dtype=layout.dtype, device=device))
         self.records = FP8Records(layout.latent_dim, layout.rope_dim)
+        self.rotary = rotary
+
+    def segment_keys(self, segment_hashes: Sequence[str]) -> List[str]:
+        """Store keys of segment pages (``kv_layout.mla_segment_key``)."""
+        return [mla_segment_key(self.layout.name, self.layout.page_tokens, h)
+                for h in segment_hashes]
+
+    def _segment_geometry(self):
+        if self.rotary is not None and self.rotary.rot_dim != self.layout.rope_dim:
+            raise ValueError(f"an MLA cache's rotary config turns its {self.layout.rope_dim} "
+                             f"RoPE elements: rot_dim {self.rotary.rot_dim} does not fit")
+        return self.layout.token_dim, self.layout.latent_dim, False  # one "head" per token
 
     def page_keys(self, page_hashes: Sequence[str], fp8: bool = False) -> List[str]:
         """Store keys of all-layer pages (``kv_layout.mla_page_key``)."""

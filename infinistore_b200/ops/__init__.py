@@ -124,7 +124,8 @@ def kv_gather(descs: torch.Tensor, part_base: Sequence[int], part_bytes: int, wr
               align_or: int = 0, stage_bytes: int = 0, ring_bytes: int = 0,
               publish: Optional["PublishArgs"] = None, layer: Optional[LayerState] = None,
               claim: bool = False, release: Optional[GroupRelease] = None,
-              rows: Optional[Sequence[int]] = None, pieces: Optional[torch.Tensor] = None) -> None:
+              rows: Optional[Sequence[int]] = None, pieces: Optional[torch.Tensor] = None,
+              rope=None) -> None:
     """Gathered blocks (csrc/kernels/kernels.h ``GatherLaunch``): block i is len(part_base)
     parts of ``part_bytes``, part s at ``part_base[s] + local offset``.  ``descs`` is (n, 2)
     int64: write {local byte offset, block address}, read {block address or 0 = miss, local
@@ -146,8 +147,12 @@ def kv_gather(descs: torch.Tensor, part_base: Sequence[int], part_bytes: int, wr
     ``publish`` / ``layer`` / ``claim`` work as without rows.  ``pieces`` (with ``rows``), an
     (n, k) int64 CUDA tensor of local byte offsets: block i's rows are k runs of rows / k
     rows, run t at part s's local address + ``pieces[i, t]`` (kv_scatter_pieces,
-    kv_gather_pieces_write); ``align_or`` must include them."""
+    kv_gather_pieces_write); ``align_or`` must include them.  ``rope`` (a ``RopeShift``, or its
+    native tuple): whole bf16 parts whose rotary pairs are turned by its table as they move
+    (kv_write_rope_gather, kv_read_rope_scatter; docs/kernels.md, "RoPE shift contract")."""
     assert descs.is_cuda and descs.dtype == torch.int64 and descs.is_contiguous()
+    if rope is not None and not isinstance(rope, tuple):
+        rope = rope.native()
     bases = [int(b) for b in part_base]
     for b in bases:
         align_or |= b
@@ -158,7 +163,7 @@ def kv_gather(descs: torch.Tensor, part_base: Sequence[int], part_bytes: int, wr
                     status.data_ptr() if status is not None else 0, align_or, stage_bytes,
                     ring_bytes, *lay, *_release_args(release),
                     [int(r) for r in rows] if rows is not None else [], *_piece_args(pieces),
-                    publish.shard_args if publish else [])
+                    publish.shard_args if publish else [], rope)
 
 
 def kv_copy_multicast(descs: torch.Tensor, nbytes: int, dst_deltas: Sequence[int],

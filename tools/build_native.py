@@ -50,6 +50,7 @@ CUDA_SOURCES = [
     "kernels/kv_fp8.cu",
     "kernels/kv_fp8_records.cu",
     "kernels/kv_fp8_cache.cu",
+    "kernels/kv_rope.cu",
     "kernels/kv_fp8_pipe.cu",
     "kernels/kv_doorbell.cu",
     "kernels/kv_bcast_nvls.cu",
